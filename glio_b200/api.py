@@ -100,6 +100,7 @@ class Context:
             msg = self._lib.glio_last_error(None)
             raise GlioError(f"glio_create failed ({rc}): {msg.decode() if msg else ''}")
         self._keep = []
+        self.device = device
 
     def close(self):
         if getattr(self, "_h", None):
@@ -404,6 +405,72 @@ def _extract_features(self, cloud_xyzi, scan_start, scan_end, ds_rate=1, edge_th
 
 
 Context.extract_features = _extract_features
+
+
+class ImuState(C.Structure):
+    """glio_imu_state: idx_imu, current_time_imu, gyr_0, first_imu of Preprocessing (GLIO/src/Preprocessing.cpp:33-39).
+    A fresh (zero) state has seen no IMU sample yet."""
+    _fields_ = [("idx_imu", C.c_int64), ("current_time_imu", C.c_double), ("gyr_0", C.c_double * 3), ("first_imu", C.c_int32),
+                ("reserved", C.c_int32)]
+
+
+def imu_sweep_rotation(state, stamps, gyro, t_scan_next):
+    """The sweep's IMU rotation qIMU (w, x, y, z): processIMU + solveRotation (Preprocessing.cpp:202-259) over the IMU buffer
+    received so far (stamps[n] seconds, gyro[n, 3] rad/s) up to t_scan_next.  `state` (ImuState) carries over between sweeps."""
+    st = np.ascontiguousarray(stamps, np.float64).ravel(); g = np.ascontiguousarray(gyro, np.float64).reshape(-1, 3)
+    if len(g) != len(st):
+        raise ValueError("stamps and gyro must have the same number of samples")
+    q = np.zeros(4)
+    L = lib()
+    rc = L.glio_imu_sweep_rotation(C.byref(state), _ptr(st), _ptr(g), C.c_int64(len(st)), C.c_double(t_scan_next), _ptr(q))
+    if rc != 0:
+        msg = L.glio_last_error(None)
+        raise GlioError(f"glio_imu_sweep_rotation failed ({rc}): {msg.decode() if msg else ''}")
+    return q
+
+
+def _prepare_scan(self, raw, n_scans, q_imu=None, q_lb=None, out="host"):
+    """Preprocessing::cloudHandler's sweep preparation (GLIO/src/Preprocessing.cpp:387-526) on the device: NaN / 3 m filters, ring
+    assignment, relative time and IMU de-skew, rings concatenated.  raw: (n, stride) float32 numpy array or CUDA tensor with x, y, z
+    in columns 0..2 (pcl::PointXYZI: stride 8).  q_imu: the sweep's rotation (imu_sweep_rotation), None = identity; q_lb: the
+    extrinsic, default synth.Q_LB.  Returns (cloud (m, 4) x,y,z,intensity, scan_start, scan_end); with out="device" the cloud
+    is a CUDA tensor that extract_features takes as it is."""
+    if out not in ("host", "device"):
+        raise ValueError("out must be 'host' or 'device'")
+    if q_lb is None:
+        from . import synth
+        q_lb = synth.Q_LB
+    keep, p, n, stride, mem = _points_arg(raw)
+    qi = None if q_imu is None else np.ascontiguousarray(q_imu, np.float64)
+    ql = np.ascontiguousarray(q_lb, np.float64)
+    ss = np.empty(n_scans, np.int32); se = np.empty(n_scans, np.int32)
+    m = C.c_int64(0)
+    if out == "device":
+        import torch
+        dev = torch.device("cuda", self.device)           # the context's GPU: the library rejects memory of any other
+        buf = torch.empty((max(n, 1), 4), dtype=torch.float32, device=dev)
+        # the buffer comes from torch's caching allocator on torch's stream, the library writes it on the context's stream:
+        # let torch's pending work on that memory finish first (the library call itself returns only when its writes are done)
+        torch.cuda.current_stream(dev).synchronize()
+        optr, omem = C.c_void_p(buf.data_ptr()), DEVICE
+    else:
+        buf = np.empty((n, 4), np.float32)
+        optr, omem = _ptr(buf), HOST
+    self._chk(self._lib.glio_prepare_scan(self._h, p, C.c_int64(n), C.c_int(stride), C.c_int(mem), C.c_int(n_scans), _ptr(qi), _ptr(ql),
+                                          optr, C.c_int(omem), C.c_int64(n), C.byref(m), _ptr(ss), _ptr(se)))
+    return buf[:m.value], ss, se
+
+
+def _scanprep_guard_hits(self, reset=False):
+    """glio_scanprep_stats: atanf / atan2f evaluations of prepare_scan decided in double-double since the last reset."""
+    h = C.c_int64(0)
+    self._chk(self._lib.glio_scanprep_stats(self._h, C.byref(h), C.c_int(1 if reset else 0)))
+    return int(h.value)
+
+
+Context.prepare_scan = _prepare_scan
+Context.KERNELS = ["k_sp_bounds", "k_sp_consts", "k_sp_classify", "k_sp_ranges", "k_sp_emit"] + Context.KERNELS
+Context.scanprep_guard_hits = _scanprep_guard_hits
 
 
 HOST_MARG_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_double))

@@ -137,6 +137,9 @@ struct glio_ctx {
   DevBuf<int32_t> d_keep;
   // front-end feature extraction work space
   DevBuf<float> f_cloud, f_curv; DevBuf<int8_t> f_label, f_picked; DevBuf<int32_t> f_scan, f_ring, f_lf, f_counts, f_out; DevBuf<float4> f_ds, f_outds;
+  // front-end sweep preparation work space
+  DevBuf<float> sp_raw, sp_ori; DevBuf<int8_t> sp_ring; DevBuf<int32_t> sp_hist, sp_hscan, sp_small; DevBuf<int> sp_scan_tmp;
+  DevBuf<SweepConsts> sp_consts; DevBuf<float4> sp_out; DevBuf<unsigned long long> sp_hits;
   // K2e scratch (kept in the context: no cudaMalloc / cudaFree per call, nothing to leak when a call throws)
   DevBuf<EdgeItem> e_items; DevBuf<int> e_start; DevBuf<double> e_part, e_out, e_poses;
 
@@ -474,6 +477,8 @@ void glio_destroy(glio_ctx* c) {
   c->d_partials.release(); c->d_out.release(); c->d_poses.release(); c->d_r.release(); c->d_J.release(); c->h_out.release();
   c->h_poses.release(); c->h_flag.release(); c->d_ticket.release(); c->w_knn_idx.release(); c->w_knn_sqd.release(); c->d_stats.release(); c->w_deferred.release();
   c->f_cloud.release(); c->f_curv.release(); c->f_label.release(); c->f_picked.release(); c->f_scan.release(); c->f_ring.release(); c->f_lf.release(); c->f_counts.release(); c->f_out.release(); c->f_ds.release(); c->f_outds.release();
+  c->sp_raw.release(); c->sp_ori.release(); c->sp_ring.release(); c->sp_hist.release(); c->sp_hscan.release(); c->sp_small.release();
+  c->sp_scan_tmp.release(); c->sp_consts.release(); c->sp_out.release(); c->sp_hits.release();
   c->e_items.release(); c->e_start.release(); c->e_part.release(); c->e_out.release(); c->e_poses.release();
   for (auto& r : c->lc.recs) { cudaEventDestroy(r.a); cudaEventDestroy(r.b); }
   for (auto& e : c->lc.pool) cudaEventDestroy(e);
@@ -1052,6 +1057,96 @@ int glio_extract_features(glio_ctx* c, const float* cloud_xyzi, int64_t n, int s
     if (less_flat && cnt[3]) GLIO_CUDA_TRY(cudaMemcpyAsync(less_flat, a.out_less_flat, cnt[3] * sizeof(int32_t), cudaMemcpyDeviceToHost, c->st));
     if (less_flat_ds && cnt[4]) GLIO_CUDA_TRY(cudaMemcpyAsync(less_flat_ds, a.out_ds, cnt[4] * sizeof(float4), cudaMemcpyDeviceToHost, c->st));
     GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
+  });
+}
+
+// ---- front-end sweep preparation (SURVEY 8 f-5): Preprocessing::cloudHandler, GLIO/src/Preprocessing.cpp:387-526
+int glio_prepare_scan(glio_ctx* c, const float* raw, int64_t n, int stride, int mem, int n_scans, const double q_imu[4],
+                      const double q_lb[4], float* out_xyzi, int out_mem, int64_t out_capacity, int64_t* n_out,
+                      int32_t* scan_start, int32_t* scan_end) {
+  if (!c) return GLIO_ERR_ARG;
+  return guarded(c, [&] {
+    GLIO_REQUIRE(raw && n > 0 && n < ((int64_t)1 << 30), GLIO_ERR_ARG, "glio_prepare_scan: bad sweep");
+    GLIO_REQUIRE(stride >= 3 && stride <= 64, GLIO_ERR_ARG, "glio_prepare_scan: stride_floats must be in [3,64]");
+    GLIO_REQUIRE(n_scans == 16 || n_scans == 32 || n_scans == 64, GLIO_ERR_ARG, "glio_prepare_scan: n_scans must be 16, 32 or 64 (wrong scan number)");
+    GLIO_REQUIRE(n_out && out_capacity >= 0 && (out_xyzi || out_capacity == 0), GLIO_ERR_ARG, "glio_prepare_scan: bad output arguments");
+    // a GLIO_DEVICE pointer must be memory of the context's GPU that the kernels can address: a host pointer, another GPU's
+    // memory or a misaligned output is an argument error, never a fault
+    auto on_device = [c](const void* p) {
+      cudaPointerAttributes at{};
+      if (cudaPointerGetAttributes(&at, p) != cudaSuccess) { cudaGetLastError(); return false; }
+      return (at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged) && at.device == c->device;
+    };
+    GLIO_REQUIRE(mem != GLIO_DEVICE || on_device(raw), GLIO_ERR_ARG, "glio_prepare_scan: mem = GLIO_DEVICE but raw is not device memory of the context's GPU");
+    GLIO_REQUIRE(((uintptr_t)raw & 3) == 0, GLIO_ERR_ARG, "glio_prepare_scan: raw must be 4-byte aligned");
+    GLIO_REQUIRE(out_mem != GLIO_DEVICE || !out_xyzi || on_device(out_xyzi), GLIO_ERR_ARG, "glio_prepare_scan: out_mem = GLIO_DEVICE but out_xyzi is not device memory of the context's GPU");
+    GLIO_REQUIRE(out_mem != GLIO_DEVICE || ((uintptr_t)out_xyzi & 15) == 0, GLIO_ERR_ARG, "glio_prepare_scan: a device out_xyzi must be 16-byte aligned (float4 stores)");
+    ScanPrepArgs a{};
+    // per-sweep rotation constants (:186-191): qIMU (NaN -> identity, :415-417), q_lb, q_lb.inverse(), Identity.dot(qIMU)
+    const double ident[4] = {1.0, 0.0, 0.0, 0.0};
+    const double* qi = q_imu ? q_imu : ident;
+    if (std::isnan(qi[0]) || std::isnan(qi[1]) || std::isnan(qi[2]) || std::isnan(qi[3])) qi = ident;
+    const double* ql = q_lb ? q_lb : ident;
+    for (int d = 0; d < 4; ++d) { a.q_imu[d] = qi[d]; a.q_lb[d] = ql[d]; }
+    const double n2 = ((ql[1] * ql[1] + ql[2] * ql[2]) + ql[3] * ql[3]) + ql[0] * ql[0];       // coeffs() = x, y, z, w
+    if (n2 > 0.0) { a.q_lb_inv[0] = ql[0] / n2; a.q_lb_inv[1] = -ql[1] / n2; a.q_lb_inv[2] = -ql[2] / n2; a.q_lb_inv[3] = -ql[3] / n2; }
+    a.dot = ((0.0 * qi[1] + 0.0 * qi[2]) + 0.0 * qi[3]) + 1.0 * qi[0];
+    const double absd = std::fabs(a.dot);
+    a.slerp_linear = absd >= 1.0 - std::numeric_limits<double>::epsilon();
+    a.theta = std::acos(absd); a.sin_theta = std::sin(a.theta);
+
+    a.raw = raw;
+    if (mem != GLIO_DEVICE) {
+      c->sp_raw.reserve((size_t)n * stride);
+      GLIO_CUDA_TRY(cudaMemcpyAsync(c->sp_raw.p, raw, (size_t)n * stride * sizeof(float), cudaMemcpyHostToDevice, c->st));
+      a.raw = c->sp_raw.p;
+    }
+    a.stride = stride; a.n = n; a.n_scans = n_scans; a.nb = (int)((n + 255) / 256);
+    c->sp_ring.reserve(n); c->sp_ori.reserve(n);
+    c->sp_hist.reserve((size_t)n_scans * a.nb); c->sp_hscan.reserve((size_t)n_scans * a.nb);
+    c->sp_small.reserve(5 + 2 * 64); c->sp_consts.reserve(1);
+    if (!c->sp_hits.p) { c->sp_hits.reserve(1); GLIO_CUDA_TRY(cudaMemsetAsync(c->sp_hits.p, 0, sizeof(unsigned long long), c->st)); }
+    a.consts = c->sp_consts.p; a.small = c->sp_small.p; a.ring = c->sp_ring.p; a.ori = c->sp_ori.p;
+    a.hist = c->sp_hist.p; a.hscan = c->sp_hscan.p; a.scan_tmp = &c->sp_scan_tmp; a.guard_hits = c->sp_hits.p;
+    if (out_mem == GLIO_DEVICE) { a.out = reinterpret_cast<float4*>(out_xyzi); a.out_capacity = out_capacity; }
+    else { c->sp_out.reserve(n); a.out = c->sp_out.p; a.out_capacity = n; }
+    scanprep_run(a, c->st, c->lc);
+    std::vector<int32_t> small((size_t)5 + 2 * n_scans);
+    GLIO_CUDA_TRY(cudaMemcpyAsync(small.data(), a.small, small.size() * sizeof(int32_t), cudaMemcpyDeviceToHost, c->st));
+    GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
+    GLIO_REQUIRE(small[3] != 0, GLIO_ERR_ARG, "glio_prepare_scan: no point of the sweep is finite and at least 3 m from the sensor");
+    const int64_t m = small[4];
+    *n_out = m;
+    if (scan_start) std::memcpy(scan_start, small.data() + 5, n_scans * sizeof(int32_t));
+    if (scan_end) std::memcpy(scan_end, small.data() + 5 + n_scans, n_scans * sizeof(int32_t));
+    GLIO_REQUIRE(m <= out_capacity, GLIO_ERR_ARG, "glio_prepare_scan: out_capacity is smaller than the number of kept points");
+    if (out_mem != GLIO_DEVICE && m > 0) {
+      GLIO_CUDA_TRY(cudaMemcpyAsync(out_xyzi, a.out, (size_t)m * sizeof(float4), cudaMemcpyDeviceToHost, c->st));
+      GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
+    }
+  });
+}
+
+int glio_scanprep_stats(glio_ctx* c, int64_t* guard_hits, int reset) {
+  if (!c) return GLIO_ERR_ARG;
+  return guarded(c, [&] {
+    unsigned long long h = 0;
+    if (c->sp_hits.p) {
+      GLIO_CUDA_TRY(cudaMemcpyAsync(&h, c->sp_hits.p, sizeof(h), cudaMemcpyDeviceToHost, c->st));
+      GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
+      if (reset) GLIO_CUDA_TRY(cudaMemsetAsync(c->sp_hits.p, 0, sizeof(h), c->st));
+    }
+    if (guard_hits) *guard_hits = (int64_t)h;
+  });
+}
+
+int glio_imu_sweep_rotation(glio_imu_state* st, const double* stamps, const double* gyro_xyz, int64_t n_buf, double t_scan_next,
+                            double q_wxyz[4]) {
+  return guarded(nullptr, [&] {
+    GLIO_REQUIRE(st && q_wxyz && n_buf >= 0 && (n_buf == 0 || (stamps && gyro_xyz)), GLIO_ERR_ARG, "glio_imu_sweep_rotation: bad arguments");
+    GLIO_REQUIRE(st->idx_imu >= 0 && st->idx_imu <= n_buf, GLIO_ERR_ARG, "glio_imu_sweep_rotation: idx_imu is past the end of the buffer");
+    GLIO_REQUIRE(n_buf > 0 || !st->first_imu, GLIO_ERR_ARG, "glio_imu_sweep_rotation: empty IMU buffer after the first sample");
+    imu_sweep_rotation(st, stamps, gyro_xyz, n_buf, t_scan_next, q_wxyz);
   });
 }
 

@@ -273,4 +273,27 @@ struct FeatArgs {
 
 void features_run(FeatArgs& a, cudaStream_t st, LaunchCounter& lc);
 
+// ---- front-end sweep preparation (scanprep.cu; Preprocessing.cpp:387-526)
+struct SweepConsts {
+  int ok;                              // 0: no point survives the NaN / 3 m filters
+  float start_ori, end_ori;            // :401-410
+  double c_first_lo, c_first_hi;       // startOri - M_PI/2, startOri + M_PI*3/2   (:491-494)
+  double c_second_lo, c_second_hi;     // endOri - M_PI*3/2, endOri + M_PI/2       (:501-504)
+};
+struct ScanPrepArgs {
+  const float* raw; int stride; int64_t n; int n_scans; int nb;    // nb: blocks of 256 raw points
+  // per-sweep rotation constants, computed once on the host
+  double q_imu[4], q_lb[4], q_lb_inv[4];                           // w, x, y, z
+  double dot, theta, sin_theta; int slerp_linear;                  // Eigen slerp: d, acos|d|, sin(theta), |d| >= 1 - eps
+  SweepConsts* consts;
+  int32_t* small;                      // [0] first kept-by-filter index, [1] last, [2] halfPassed index, [3] ok, [4] count, [5..] ranges
+  int8_t* ring; float* ori;            // [n] ring id (-1 skipped), raw azimuth -atan2f(y, x)
+  int32_t* hist; int32_t* hscan;       // [n_scans][nb] per-block ring counts and their ring-major exclusive scan
+  DevBuf<int>* scan_tmp;
+  unsigned long long* guard_hits;      // correctly rounded atanf / atan2f: evaluations decided in double-double
+  float4* out; int64_t out_capacity;
+};
+void scanprep_run(ScanPrepArgs& a, cudaStream_t st, LaunchCounter& lc);
+void imu_sweep_rotation(glio_imu_state* st, const double* stamps, const double* gyro, int64_t n, double t_cur, double q[4]);
+
 }  // namespace glio

@@ -175,6 +175,70 @@ def batch_problem(K=200, Q=100_000, seed=SEED0 + 3, search_range=6, rng_range=50
     return dict(scans=scans, poses_true=truth, poses_init=init, K=K, Q=Q, search_range=search_range, seed=seed)
 
 
+def raw_elevations(n_rings):
+    """Elevation table (degrees) of a raw sweep for the ring rules of Preprocessing.cpp:441-483: every line sits inside its ring's
+    interval, plus lines each rule treats specially.  16: VLP-16's -15..15 step 2, one line at -16.5 that int() truncates toward
+    zero into ring 0, one at +17 (ring 16, skipped).  32: the centres of int((angle + 92/3) * 3/4), one line truncated into ring 0,
+    one above (ring 32) and one below (ring -1), both skipped.  64: 33 lines on the upper branch 2 - (k + 0.1)/3 (rings 0..32),
+    31 on the lower branch -8.83 - (j + 0.1)/2 (rings 33..63: 51..63 and angle < -24.33 are rejected), and one line above +2
+    (int() gives ring 0, rejected by angle > 2)."""
+    if n_rings == 16:
+        return np.concatenate([np.arange(-15.0, 16.0, 2.0), [-16.5, 17.0]])
+    if n_rings == 32:
+        return np.concatenate([-92.0 / 3.0 + 4.0 / 3.0 * (np.arange(32) + 0.5), [-92.0 / 3.0 - 0.5, 12.5, -33.0]])
+    if n_rings == 64:
+        return np.concatenate([2.0 - (np.arange(33) + 0.1) / 3.0, -8.83 - (np.arange(1, 32) + 0.1) / 2.0, [2.3]])
+    raise ValueError("n_rings must be 16, 32 or 64")
+
+
+def raw_sweep(n_rings=32, n_az=1875, start_az=0.3, coverage=2 * np.pi - 0.02, yaw_rate=0.0, seed=SEED0 + 12, t0=100.0,
+              sweep_time=0.1, imu_rate=400.0, noise=0.01, nan_frac=0.01, near_frac=0.005, n_zaxis=4):
+    """A raw spinning-LiDAR sweep as the driver delivers it (the input of Preprocessing::cloudHandler, GLIO/src/Preprocessing.cpp:387):
+    firing after firing (azimuth-major), the lines of a firing interleaved, x,y,z,intensity float32 (intensity = a reflectivity the
+    reference ignores).  The head turns clockwise from azimuth start_az through `coverage` radians (slightly less or more than
+    2 pi reaches the endOri corrections of :406-410) in sweep_time seconds while the sensor yaws at yaw_rate rad/s; rays are cast
+    against the street-canyon scene in the sensor's pose at the firing's time.  Misses and a fraction nan_frac of the returns are
+    NaN, a fraction near_frac are returns closer than 3 m, and n_zaxis points lie on the z axis (x = y = 0).
+    Returns dict(raw (n, 4) float32, stamps, gyro (m, 3): IMU samples at imu_rate covering the sweep, t_scan_next = end of sweep,
+    elev_deg: the line table)."""
+    rng = np.random.default_rng(seed)
+    sc = Scene(-60.0, 60.0, rng)
+    origin = np.array([0.3, -0.4, 0.2])
+    elev = np.deg2rad(raw_elevations(n_rings))
+    L = len(elev)
+    order = (np.arange(L) * 11) % L                          # interleaved firing order of the lines
+    k = np.repeat(np.arange(n_az), L)
+    line = np.tile(order, n_az)
+    az = start_az - coverage * k / n_az
+    psi = yaw_rate * sweep_time * k / n_az                   # sensor yaw at the firing's time
+    e = elev[line]
+    d = np.stack([np.cos(e) * np.cos(az), np.cos(e) * np.sin(az), np.sin(e)], 1)          # sensor frame
+    dw = np.stack([np.cos(psi) * d[:, 0] - np.sin(psi) * d[:, 1], np.sin(psi) * d[:, 0] + np.cos(psi) * d[:, 1], d[:, 2]], 1)
+    best = np.full(len(d), np.inf)
+    for o, u, v, nrm in zip(sc.o, sc.u, sc.v, sc.n):
+        den = dw @ nrm
+        with np.errstate(divide="ignore", invalid="ignore"):
+            t = ((o - origin) @ nrm) / den
+            hit = origin + t[:, None] * dw - o
+            a = (hit @ u) / (u @ u); b = (hit @ v) / (v @ v)
+        ok = (np.abs(den) > 1e-9) & (t > 0.5) & (a >= 0) & (a <= 1) & (b >= 0) & (b <= 1)
+        best = np.where(ok & (t < best), t, best)
+    rg = best + rng.normal(0.0, noise, len(best))
+    near = rng.random(len(rg)) < near_frac
+    rg[near] = rng.uniform(0.5, 2.9, int(near.sum()))
+    rg[~np.isfinite(best) | (best > 80.0) | (rng.random(len(rg)) < nan_frac)] = np.nan
+    raw = np.empty((len(d), 4), np.float32)
+    raw[:, :3] = rg[:, None] * d
+    raw[:, 3] = rng.uniform(0.0, 100.0, len(d))
+    if n_zaxis:
+        at = rng.choice(len(raw), n_zaxis, replace=False)
+        raw[at, 0] = 0.0; raw[at, 1] = 0.0
+        raw[at, 2] = rng.choice([-1.0, 1.0], n_zaxis) * rng.uniform(3.5, 20.0, n_zaxis)
+    stamps = t0 - 0.05 + np.arange(int((sweep_time + 0.1) * imu_rate) + 1) / imu_rate
+    gyro = np.zeros((len(stamps), 3)); gyro[:, 2] = yaw_rate
+    return dict(raw=raw, stamps=stamps, gyro=gyro, t_scan_next=t0 + sweep_time, elev_deg=np.rad2deg(elev))
+
+
 def ring_scan(n_rings=32, n_az=1500, seed=SEED0 + 11, fov=(-25.0, 15.0), noise=0.01, drop=0.02):
     """A spinning-LiDAR sweep of the street-canyon scene, ring by ring, for the front end's feature extraction (SURVEY 8 f-4):
     rays are cast from the sensor against the scene's rectangles (nearest hit), range noise N(0, noise), a fraction `drop` of the

@@ -83,7 +83,8 @@ int64_t glio_launch_count(const glio_ctx* ctx);
  * | k_knn_tile + k_defer_scatter + k_knn_tile2 + k_knn_team [4] | k_knn_box_start + k_knn_grow [5] | k_knn_box_far + k_knn_far [6]
  * | k_knn_box_cells [7], k_plane_fit, k_plane_fit_pair, k_flags, k_compact;
  * K2 k_eval_unary, k_eval_unary_cost, k_eval_binary, k_eval_binary_cost, k_bin_assemble; local map k_lm_transform, k_vox_*;
- * front end k_feat_curvature, k_feat_select, k_feat_voxel, k_feat_offsets, k_feat_gather). */
+ * front end k_feat_curvature, k_feat_select, k_feat_voxel, k_feat_offsets, k_feat_gather; sweep preparation k_sp_bounds,
+ * k_sp_consts, k_sp_classify, k_sp_ranges, k_sp_emit). */
 int glio_profile_enable(glio_ctx* ctx, int on);
 int glio_profile_get(glio_ctx* ctx, const char* kernel_name, double* ms_total, int64_t* launches);
 /* statistics: number of queries a first search pass handed to its second pass (GLIO_KNN_MODE 0 and 4; 0 in the default mode) */
@@ -272,6 +273,42 @@ int glio_extract_features(glio_ctx* ctx, const float* cloud_xyzi, int64_t n, int
                           const int32_t* scan_end, int ds_rate, double edge_thres, double surf_thres, float ds_v, float* curvature, int8_t* label,
                           int32_t* sharp, int64_t* n_sharp, int32_t* less_sharp, int64_t* n_less_sharp, int32_t* flat, int64_t* n_flat,
                           int32_t* less_flat, int64_t* n_less_flat, float* less_flat_ds, int64_t* n_less_flat_ds);
+
+/* ---- front-end sweep preparation (SURVEY 8 f-5): Preprocessing::cloudHandler, GLIO/src/Preprocessing.cpp:387-526.
+ * raw = the sweep as received, x,y,z at floats 0..2 of stride_floats (pcl::PointXYZI: stride 8; the input intensity is not used).
+ * Points with a non-finite coordinate or closer than 3 m are dropped (:396-397), every other point gets its ring id from its
+ * elevation for n_scans 16 / 32 / 64 (:438-483; out-of-range rings are skipped), its relative time from the azimuth state machine
+ * (:489-507), intensity = ring + 0.1 relTime, and is de-skewed by Identity.slerp(relTime, q_imu) conjugated by q_lb
+ * (undistortion, :176-200).  out_xyzi receives `laserCloud`: the kept points ring after ring in input order as packed float4
+ * x,y,z,intensity (the stride 4, offset 3 layout of glio_extract_features), scan_start / scan_end[n_scans] =
+ * scanStartInd / scanEndInd (:521-526; an empty ring has start = end + 11).  q_imu / q_lb are w,x,y,z; NULL means identity,
+ * and a q_imu with a NaN component is replaced by identity (:415-417).  *n_out is always the true count; if it exceeds
+ * out_capacity the call fails with GLIO_ERR_ARG and nothing is written past out_capacity.  out_mem = GLIO_DEVICE writes
+ * straight into device memory, ready for glio_extract_features(..., 4, 3, GLIO_DEVICE, ...); that out_xyzi must be
+ * 16-byte aligned (it is written as float4), raw must be 4-byte aligned, and GLIO_DEVICE pointers must belong to the
+ * context's GPU (otherwise GLIO_ERR_ARG before anything runs).  The call returns when its work is complete.  A sweep in which no point
+ * survives the NaN / 3 m filters fails with GLIO_ERR_ARG (the reference would read point 0 of an empty cloud).
+ * atanf / atan2f are correctly rounded (DESIGN 2); glio_scanprep_stats counts the evaluations that needed the double-double
+ * decision (reset != 0 zeroes the counter). */
+int glio_prepare_scan(glio_ctx* ctx, const float* raw, int64_t n, int stride_floats, int mem, int n_scans, const double q_imu[4],
+                      const double q_lb[4], float* out_xyzi, int out_mem, int64_t out_capacity, int64_t* n_out,
+                      int32_t* scan_start, int32_t* scan_end);
+int glio_scanprep_stats(glio_ctx* ctx, int64_t* guard_hits, int reset);
+
+/* The sweep's IMU rotation qIMU: Preprocessing::processIMU + solveRotation (:202-207, :222-259, deltaQ of
+ * GLIO/include/utils/math_tools.h:126-138), integrating the gyro samples of the buffer up to t_scan_next from identity.
+ * stamps[n_buf] (seconds) and gyro_xyz[3*n_buf] (rad/s) are the whole IMU buffer received so far (imu_buf); the state carries
+ * idx_imu / current_time_imu / gyr_0 from sweep to sweep.  Zero-initialise it: the first call with samples performs
+ * imuHandler's first-sample initialisation (:281-293).  With no sample yet q = identity.  Host code, no context. */
+typedef struct {
+  int64_t idx_imu;
+  double current_time_imu;
+  double gyr_0[3];
+  int32_t first_imu;
+  int32_t reserved;
+} glio_imu_state;
+int glio_imu_sweep_rotation(glio_imu_state* st, const double* stamps, const double* gyro_xyz, int64_t n_buf, double t_scan_next,
+                            double q_wxyz[4]);
 
 /* ---- K3: marginalisation of the oldest keyframe (MarginalizationInfo, GLIO/src/MarginalizationFactor.cpp:82-202; call site
  * Estimator.cpp:2462-2608).  The reference re-evaluates EVERY LiDAR factor of the window (:2538-2576, one virtual Evaluate per
