@@ -719,3 +719,114 @@ Context.batch_select = _batch_select
 Context.batch_pair_list = _batch_pair_list
 Context.batch_clear = _batch_clear
 Context.eval_binary = _eval_binary
+
+
+# ---------------------------------------------------------------------------------------------------
+# front-end LiDAR odometry (LidarOdometry::run, GLIO/src/LidarOdometry.cpp:661-695)
+# ---------------------------------------------------------------------------------------------------
+class OdomOptions(C.Structure):
+    _fields_ = [("max_num_iter", C.c_int32), ("scan_match_cnt", C.c_int32), ("deskew", C.c_int32), ("reserved", C.c_int32),
+                ("max_solver_time_s", C.c_double)]
+
+
+ODOM_MAX_ROUNDS = 8
+
+
+class OdomReport(C.Structure):
+    _fields_ = [("pose", C.c_double * 7), ("rel_pose", C.c_double * 7), ("initialised", C.c_int32), ("keyframe", C.c_int32),
+                ("skipped", C.c_int32), ("n_rounds", C.c_int32), ("n_map", C.c_int64), ("n_scan", C.c_int64),
+                ("round_n_match", C.c_int64 * ODOM_MAX_ROUNDS), ("round_iterations", C.c_int32 * ODOM_MAX_ROUNDS),
+                ("round_successful", C.c_int32 * ODOM_MAX_ROUNDS), ("round_termination", C.c_int32 * ODOM_MAX_ROUNDS),
+                ("reserved", C.c_int32), ("round_pose", (C.c_double * 7) * ODOM_MAX_ROUNDS), ("summary", SolverSummary)]
+
+
+def default_odom_options(**kw):
+    o = OdomOptions()
+    lib().glio_odom_default_options(C.byref(o))
+    for k, v in kw.items():
+        setattr(o, k, v)
+    return o
+
+
+def _cloud4_arg(a):
+    """(n, 4) float32 x,y,z,intensity: numpy array (host) or contiguous CUDA tensor (device)."""
+    if a is None:
+        return None, None, 0, HOST
+    if isinstance(a, np.ndarray):
+        h = np.ascontiguousarray(a, dtype=np.float32).reshape(-1, 4)
+        return h, _ptr(h), h.shape[0], HOST
+    if hasattr(a, "data_ptr"):
+        if not (a.is_cuda and a.is_contiguous() and a.dtype.itemsize == 4 and a.dim() == 2 and a.shape[1] == 4):
+            raise ValueError("a device cloud must be a contiguous (n, 4) float32 CUDA tensor")
+        return a, C.c_void_p(a.data_ptr()), a.shape[0], DEVICE
+    raise TypeError("clouds must be numpy arrays or CUDA torch tensors")
+
+
+class Odometry:
+    """The front end's LidarOdometry node on the device: one step() per sweep with its surf features (extract_features'
+    less_flat_ds) and optionally its full cloud (prepare_scan's output), both (n, 4) x,y,z,intensity, numpy or CUDA tensors.
+    Runs on the context's GPU and stream; its state is its own (see glio_odom_step in include/glio_b200.h)."""
+
+    def __init__(self, ctx, **options):
+        self.ctx = ctx
+        self._lib = ctx._lib
+        self.options = default_odom_options(**options)
+        self._h = C.c_void_p()
+        ctx._chk(self._lib.glio_odom_create(ctx._h, C.byref(self.options), C.byref(self._h)))
+
+    def close(self):
+        if getattr(self, "_h", None) and self.ctx._h:      # a closed context has already freed its odometries
+            self._lib.glio_odom_destroy(self._h)
+        self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def reset(self):
+        self.ctx._chk(self._lib.glio_odom_reset(self._h))
+
+    def step(self, surf, full=None, out="host"):
+        """Returns dict(pose (7,) t,q; rel_pose (7,) t,q; initialised, keyframe, skipped: bool; n_map, n_scan; rounds: list of
+        dict(n_match, iterations, successful, termination, pose); summary: the last round's SolverSummary; surf / full: the
+        published clouds (None when this sweep publishes nothing or the input was not given)."""
+        if out not in ("host", "device"):
+            raise ValueError("out must be 'host' or 'device'")
+        ks, ps, ns, ms = _cloud4_arg(surf)
+        kf, pf, nf, mf = _cloud4_arg(full)
+        if out == "device":
+            import torch
+            dev = torch.device("cuda", self.ctx.device)
+            so = torch.empty((max(ns, 1), 4), dtype=torch.float32, device=dev)
+            fo = torch.empty((max(nf, 1), 4), dtype=torch.float32, device=dev) if full is not None else None
+            # torch's allocator hands the memory out on torch's stream, the library writes it on the context's: let torch finish first
+            torch.cuda.current_stream(dev).synchronize()
+            pso, pfo, om = C.c_void_p(so.data_ptr()), (C.c_void_p(fo.data_ptr()) if fo is not None else None), DEVICE
+        else:
+            so = np.empty((ns, 4), np.float32)
+            fo = np.empty((nf, 4), np.float32) if full is not None else None
+            pso, pfo, om = _ptr(so), _ptr(fo), HOST
+        rep = OdomReport()
+        self.ctx._chk(self._lib.glio_odom_step(self._h, ps, C.c_int64(ns), C.c_int(ms), pf, C.c_int64(nf), C.c_int(mf), pso, pfo,
+                                               C.c_int(om), C.byref(rep)))
+        published = bool(rep.initialised or rep.keyframe)
+        rounds = [dict(n_match=int(rep.round_n_match[r]), iterations=int(rep.round_iterations[r]), successful=int(rep.round_successful[r]),
+                       termination=int(rep.round_termination[r]), pose=np.array(rep.round_pose[r][:])) for r in range(rep.n_rounds)]
+        return dict(pose=np.array(rep.pose[:]), rel_pose=np.array(rep.rel_pose[:]), initialised=bool(rep.initialised),
+                    keyframe=bool(rep.keyframe), skipped=bool(rep.skipped), n_map=int(rep.n_map), n_scan=int(rep.n_scan), rounds=rounds,
+                    summary=rep.summary, surf=so[:ns] if published else None,
+                    full=(fo[:nf] if published and fo is not None else None))
+
+    def clouds(self):
+        """The last step's filtered map and filtered scan, (n, 3) float32 each (debug copy-out)."""
+        nm = C.c_int64(0); nsc = C.c_int64(0)
+        self.ctx._chk(self._lib.glio_odom_get_clouds(self._h, C.c_int64(0), None, C.byref(nm), C.c_int64(0), None, C.byref(nsc)))
+        m = np.empty((nm.value, 3), np.float32); s = np.empty((nsc.value, 3), np.float32)
+        self.ctx._chk(self._lib.glio_odom_get_clouds(self._h, C.c_int64(nm.value), _ptr(m), C.byref(nm), C.c_int64(nsc.value), _ptr(s),
+                                                     C.byref(nsc)))
+        return m, s
+
+
+Context.KERNELS = Context.KERNELS + ["k_odom_publish"]

@@ -149,10 +149,10 @@ struct glio_ctx {
   DevBuf<double> d_partials, d_out, d_poses, d_r, d_J;
   PinnedBuf<double> h_out, h_poses;
   // local map maintenance (SURVEY 8 f-1): world-frame keyframe clouds in deque order, concatenation, voxel filter work space
-  struct LmFrame { DevBuf<float4> pts; int64_t n = 0; };
-  std::deque<std::unique_ptr<LmFrame>> lm_frames;
-  std::vector<std::unique_ptr<LmFrame>> lm_spare;      // buffers of popped frames, reused by the next push (no cudaFree / cudaMalloc per keyframe)
-  DevBuf<float> lm_stage; DevBuf<float4> lm_cat; VoxelWork lm_vox; int64_t map_n = 0;
+  LocalMap lm;
+  DevBuf<float> lm_stage; int64_t map_n = 0;
+  // front-end odometries created on this context (glio_odom_create); glio_destroy frees those still attached
+  std::vector<glio_odom*> odoms;
   cudaStream_t st_copy = nullptr;       // window scans travel on their own stream so the upload of the next window can overlap a running solve
   cudaEvent_t ev_scans = nullptr, ev_main = nullptr;
   bool scans_pending = false;
@@ -199,6 +199,13 @@ int guarded(glio_ctx* ctx, F&& f) {
   }
 }
 
+// true when p is memory of the context's GPU that its kernels can address
+bool on_ctx_device(const glio_ctx* c, const void* p) {
+  cudaPointerAttributes at{};
+  if (cudaPointerGetAttributes(&at, p) != cudaSuccess) { cudaGetLastError(); return false; }
+  return (at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged) && at.device == c->device;
+}
+
 // bring `n` points (stride floats each) to the device; returns the device pointer to read from
 const float* stage_points(glio_ctx* c, DevBuf<float>& buf, const float* xyz, int64_t n, int stride, int mem) {
   GLIO_REQUIRE(xyz != nullptr && n > 0, GLIO_ERR_ARG, "null or empty point array");
@@ -209,38 +216,39 @@ const float* stage_points(glio_ctx* c, DevBuf<float>& buf, const float* xyz, int
   return buf.p;
 }
 
-void ensure_work(glio_ctx* c, int64_t Qt, bool pair) {
+void ensure_work(glio_ctx* c, int64_t Qt, bool pair, bool keep_debug) {
   c->w_pm.reserve((size_t)Qt); c->w_pmq.reserve((size_t)Qt); c->w_seg.reserve((size_t)Qt);
   c->w_status.reserve((size_t)Qt); c->w_weight.reserve((size_t)Qt);
   c->w_flags.reserve((size_t)Qt + 1); c->w_pos.reserve((size_t)Qt + 1);
   c->w_knn_idx.reserve((size_t)Qt * 5); c->w_knn_sqd.reserve((size_t)Qt * 5); c->w_deferred.reserve((size_t)2 * Qt);
   if (!c->d_stats.p) { c->d_stats.reserve(4); GLIO_CUDA_TRY(cudaMemsetAsync(c->d_stats.p, 0, 4 * sizeof(unsigned long long), c->st)); }
   if (pair) c->w_nc.reserve((size_t)Qt * 6); else c->w_nsd.reserve((size_t)Qt);
-  if (c->prm.keep_debug) { c->w_idx5.reserve((size_t)Qt * 5); c->w_sqd5.reserve((size_t)Qt * 5); c->w_plane.reserve((size_t)Qt * 4); }
+  if (keep_debug) { c->w_idx5.reserve((size_t)Qt * 5); c->w_sqd5.reserve((size_t)Qt * 5); c->w_plane.reserve((size_t)Qt * 4); }
 }
 
-AssocWork make_work(glio_ctx* c, int64_t Qt, bool pair) {
+AssocWork make_work(glio_ctx* c, int64_t Qt, bool pair, bool keep_debug) {
   AssocWork w{};
   w.Qt = Qt; w.pm = c->w_pm.p; w.pmq = c->w_pmq.p; w.seg = c->w_seg.p; w.status = c->w_status.p;
   w.knn_idx = c->w_knn_idx.p; w.knn_sqd = c->w_knn_sqd.p; w.n_fallback = c->d_stats.p;
   w.knn_mode = c->knn_mode; w.tile_rings = c->tile_rings; w.grow_mode = c->grow_mode; w.deferred = c->w_deferred.p; w.n_deferred = reinterpret_cast<unsigned int*>(c->d_stats.p + 2);
   w.nsd = pair ? nullptr : c->w_nsd.p; w.weight = c->w_weight.p; w.normal_cent = pair ? c->w_nc.p : nullptr;
-  if (c->prm.keep_debug) { w.idx5 = c->w_idx5.p; w.sqd5 = c->w_sqd5.p; w.plane = c->w_plane.p; }
+  if (keep_debug) { w.idx5 = c->w_idx5.p; w.sqd5 = c->w_sqd5.p; w.plane = c->w_plane.p; }
   return w;
 }
 
-// run scan-to-map association for the given slots (one launch), compact, fetch counts
-void associate_slots(glio_ctx* c, const std::vector<int>& ids, const std::vector<std::array<double, 7>>& lidar_poses,
-                     int64_t* n_match) {
-  GLIO_REQUIRE(c->has_map, GLIO_ERR_STATE, "glio_set_map must be called before association");
+// run scan-to-map association of the given slots against `grid` with `gates` (one launch), compact, fetch counts.  The
+// context's association workspace is scratch; the map, gates and slots are the caller's (the window path passes the
+// context's own, the odometry its own).
+void associate_slots(glio_ctx* c, const GridBuild& grid, const AssocGates& gates, bool keep_debug, const std::vector<Slot*>& slots,
+                     const std::vector<std::array<double, 7>>& lidar_poses, int64_t* n_match) {
   if (c->scans_pending) { GLIO_CUDA_TRY(cudaStreamWaitEvent(c->st, c->ev_scans, 0)); c->scans_pending = false; }
   Trace tr(c->st, "associate");
-  const int nseg = (int)ids.size();
+  const int nseg = (int)slots.size();
   std::vector<SegDesc> segs(nseg);
   std::vector<CompactDst> dst(nseg);
   int64_t Qt = 0;
   for (int s = 0; s < nseg; ++s) {
-    Slot& sl = c->slot(ids[s]);
+    Slot& sl = *slots[s];
     GLIO_REQUIRE(sl.Q > 0 && sl.scan_ptr, GLIO_ERR_STATE, "slot has no scan");
     segs[s].src = sl.scan_ptr; segs[s].stride = sl.stride; segs[s].count = sl.Q; segs[s].offset = Qt;
     for (int k = 0; k < 3; ++k) segs[s].t[k] = lidar_poses[s][k];
@@ -250,21 +258,20 @@ void associate_slots(glio_ctx* c, const std::vector<int>& ids, const std::vector
     sl.n_sel = -1;
     Qt += sl.Q;
   }
-  ensure_work(c, Qt, false);
+  ensure_work(c, Qt, false, keep_debug);
   c->d_segs.reserve(nseg); c->d_dst.reserve(nseg); c->d_counts.reserve(nseg); c->h_counts.reserve(nseg);
   GLIO_CUDA_TRY(cudaMemcpyAsync(c->d_segs.p, segs.data(), nseg * sizeof(SegDesc), cudaMemcpyHostToDevice, c->st));
   GLIO_CUDA_TRY(cudaMemcpyAsync(c->d_dst.p, dst.data(), nseg * sizeof(CompactDst), cudaMemcpyHostToDevice, c->st));
-  AssocWork w = make_work(c, Qt, false);
-  AssocGates gates{c->prm.kd_max_radius, c->prm.surf_dist_thres, c->prm.weight_min};
+  AssocWork w = make_work(c, Qt, false, keep_debug);
   tr.mark("setup+h2d");
-  assoc_run(c->map, c->d_segs.p, nseg, w, gates, nullptr, 0, c->cell_count, c->cell_pos, c->scan_tmp, c->st, c->lc);
+  assoc_run(grid, c->d_segs.p, nseg, w, gates, nullptr, 0, c->cell_count, c->cell_pos, c->scan_tmp, c->st, c->lc);
   tr.mark("assoc_run");
   compact_run(w, c->d_segs.p, nseg, c->w_flags.p, c->w_pos.p, c->scan_tmp, c->d_dst.p, c->d_counts.p, c->st, c->lc);
   tr.mark("compact");
   GLIO_CUDA_TRY(cudaMemcpyAsync(c->h_counts.p, c->d_counts.p, nseg * sizeof(int), cudaMemcpyDeviceToHost, c->st));
-  if (c->prm.keep_debug) {
+  if (keep_debug) {
     for (int s = 0; s < nseg; ++s) {
-      Slot& sl = c->slot(ids[s]);
+      Slot& sl = *slots[s];
       const int64_t o = segs[s].offset, q = sl.Q;
       sl.dbg_status.reserve(q); sl.dbg_idx5.reserve(5 * q); sl.dbg_sqd5.reserve(5 * q); sl.dbg_pm.reserve(q); sl.dbg_plane.reserve(4 * q);
       GLIO_CUDA_TRY(cudaMemcpyAsync(sl.dbg_status.p, w.status + o, q, cudaMemcpyDeviceToDevice, c->st));
@@ -277,28 +284,38 @@ void associate_slots(glio_ctx* c, const std::vector<int>& ids, const std::vector
   }
   GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
   for (int s = 0; s < nseg; ++s) {
-    Slot& sl = c->slot(ids[s]);
+    Slot& sl = *slots[s];
     sl.n_match = c->h_counts.p[s];
     if (n_match) n_match[s] = sl.n_match;
   }
-  c->items_dirty = true;
   tr.mark("done");
 }
 
-void build_items(glio_ctx* c, int W) {
-  if (!c->items_dirty && c->items_W == W) return;
+// the context's own window association: its map, its gates, slots 0..
+void associate_ctx_slots(glio_ctx* c, const std::vector<int>& ids, const std::vector<std::array<double, 7>>& lidar_poses, int64_t* n_match) {
+  GLIO_REQUIRE(c->has_map, GLIO_ERR_STATE, "glio_set_map must be called before association");
+  std::vector<Slot*> sl;
+  for (int id : ids) sl.push_back(&c->slot(id));
+  const AssocGates gates{c->prm.kd_max_radius, c->prm.surf_dist_thres, c->prm.weight_min};
+  associate_slots(c, c->map, gates, c->prm.keep_debug != 0, sl, lidar_poses, n_match);
+  c->items_dirty = true;
+}
+
+// evaluation work items of the given slots (slot k = keyframe k, nullptr = none): start[k] = first item of keyframe k
+std::vector<EvalItem> plan_items(const std::vector<const Slot*>& slots, int eval_slots, std::vector<int>& start) {
+  const int W = (int)slots.size();
   std::vector<EvalItem> items;
-  std::vector<int> start(W + 1, 0);
+  start.assign(W + 1, 0);
   // item size: the whole launch should be about one wave of 2 resident blocks per SM (less per-item reduction
   // overhead, no wave-quantisation tail), but never below GLIO_ITEM_MAX residuals per item
   int64_t n_total = 0;
-  for (int k = 0; k < W && (size_t)k < c->slots.size(); ++k) if (c->slots[k]) n_total += c->slots[k]->n_sel >= 0 ? c->slots[k]->n_sel : c->slots[k]->n_match;
-  int64_t item_size = (n_total + c->eval_slots - 1) / std::max(c->eval_slots, 1);
+  for (int k = 0; k < W; ++k) if (slots[k]) n_total += slots[k]->n_sel >= 0 ? slots[k]->n_sel : slots[k]->n_match;
+  int64_t item_size = (n_total + eval_slots - 1) / std::max(eval_slots, 1);
   item_size = std::max<int64_t>(GLIO_ITEM_MAX, ((item_size + 255) / 256) * 256);
   for (int k = 0; k < W; ++k) {
     start[k] = (int)items.size();
-    if ((size_t)k >= c->slots.size() || !c->slots[k]) continue;
-    Slot& sl = *c->slots[k];
+    if (!slots[k]) continue;
+    const Slot& sl = *slots[k];
     const bool sel = sl.n_sel >= 0;
     const int64_t n = sel ? sl.n_sel : sl.n_match;
     const float4* cpw = sel ? sl.s_cpw.p : sl.m_cpw.p;
@@ -311,16 +328,37 @@ void build_items(glio_ctx* c, int W) {
     }
   }
   start[W] = (int)items.size();
-  c->n_items = (int)items.size();
-  c->d_items.reserve(items.size() + 1); c->d_kf_item_start.reserve(W + 1);
-  c->d_partials.reserve((items.size() + 1) * GLIO_NACC);
+  return items;
+}
+
+// The work items of one evaluation target in device memory, and the constants its residuals are evaluated with.
+struct EvalTarget {
+  const EvalItem* d_items; int n_items; const int* d_kf_item_start; double* d_partials;
+  EvalParams ep;
+};
+
+// uploads planned items into the given device buffers; reserves the context's per-evaluation buffers for W keyframes
+void upload_items(glio_ctx* c, int W, const std::vector<EvalItem>& items, const std::vector<int>& start, DevBuf<EvalItem>& d_items,
+                  DevBuf<int>& d_start, DevBuf<double>& d_partials) {
+  d_items.reserve(items.size() + 1); d_start.reserve(W + 1);
+  d_partials.reserve((items.size() + 1) * GLIO_NACC);
   c->d_out.reserve((size_t)W * GLIO_NACC); c->h_out.reserve((size_t)W * GLIO_NACC);
   c->d_poses.reserve((size_t)W * 7); c->h_poses.reserve((size_t)W * 7);
   if (!c->d_ticket.p) { c->d_ticket.reserve(1); GLIO_CUDA_TRY(cudaMemsetAsync(c->d_ticket.p, 0, sizeof(unsigned int), c->st)); }
   if (!items.empty())
-    GLIO_CUDA_TRY(cudaMemcpyAsync(c->d_items.p, items.data(), items.size() * sizeof(EvalItem), cudaMemcpyHostToDevice, c->st));
-  GLIO_CUDA_TRY(cudaMemcpyAsync(c->d_kf_item_start.p, start.data(), (W + 1) * sizeof(int), cudaMemcpyHostToDevice, c->st));
+    GLIO_CUDA_TRY(cudaMemcpyAsync(d_items.p, items.data(), items.size() * sizeof(EvalItem), cudaMemcpyHostToDevice, c->st));
+  GLIO_CUDA_TRY(cudaMemcpyAsync(d_start.p, start.data(), (W + 1) * sizeof(int), cudaMemcpyHostToDevice, c->st));
   GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));   // items/start are stack vectors
+}
+
+void build_items(glio_ctx* c, int W) {
+  if (!c->items_dirty && c->items_W == W) return;
+  std::vector<const Slot*> sl(W, nullptr);
+  for (int k = 0; k < W && (size_t)k < c->slots.size(); ++k) sl[k] = c->slots[k].get();
+  std::vector<int> start;
+  const std::vector<EvalItem> items = plan_items(sl, c->eval_slots, start);
+  c->n_items = (int)items.size();
+  upload_items(c, W, items, start, c->d_items, c->d_kf_item_start, c->d_partials);
   c->items_dirty = false;
   c->items_W = W;
 }
@@ -357,8 +395,9 @@ void fill_summary(const SolverSummary& S, int n, glio_solver_summary* summary, g
 }
 
 // device evaluation of all active unary residuals -> c->h_out (W x 28: 21 upper-tri H, 6 g, 1 cost), synchronised
-// launch half: returns the epoch to wait for (0: nothing was launched, h_out already holds zeros)
-unsigned int eval_unary_launch(glio_ctx* c, int W, const double* poses_body, int jac_kind, bool want_jac) {
+// launch half: returns the epoch to wait for (0: nothing was launched, h_out already holds zeros).  tgt = nullptr evaluates the
+// context's own slots with its glio_params; otherwise the target's items and constants (the odometry's).
+unsigned int eval_unary_launch(glio_ctx* c, int W, const double* poses_body, int jac_kind, bool want_jac, const EvalTarget* tgt = nullptr) {
   if (c->marg_pending) {            // an asynchronous marginalisation still owns the result buffer until its worker has copied it
     while (!c->marg_pending->copied.load(std::memory_order_acquire)) {
 #if defined(__x86_64__)
@@ -366,12 +405,17 @@ unsigned int eval_unary_launch(glio_ctx* c, int W, const double* poses_body, int
 #endif
     }
   }
-  build_items(c, W);
+  EvalTarget own{};
+  if (!tgt) {
+    build_items(c, W);
+    own = EvalTarget{c->d_items.p, c->n_items, c->d_kf_item_start.p, c->d_partials.p, eval_params(c)};
+    tgt = &own;
+  }
   // Zero-copy round trip: the W poses travel in the kernel parameters, the last block writes the W x 28 result into
   // pinned host memory and raises an epoch flag the host spins on.  This replaces H2D copy + launch + D2H copy +
   // stream synchronise on the per-iteration path, and lets the caller evaluate its host factors while the kernel runs.
   memcpy(c->h_poses.p, poses_body, (size_t)W * 7 * sizeof(double));
-  if (c->n_items <= 0) {
+  if (tgt->n_items <= 0) {
     GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
     memset(c->h_out.p, 0, (size_t)W * GLIO_NACC * sizeof(double));
     return 0u;
@@ -379,8 +423,8 @@ unsigned int eval_unary_launch(glio_ctx* c, int W, const double* poses_body, int
   if (!c->h_flag.p) { c->h_flag.reserve(4); memset(c->h_flag.p, 0, 4 * sizeof(unsigned int)); }
   const unsigned int epoch = ++c->eval_epoch;
   if (W > EV_MAXW) GLIO_CUDA_TRY(cudaMemcpyAsync(c->d_poses.p, c->h_poses.p, (size_t)W * 7 * sizeof(double), cudaMemcpyHostToDevice, c->st));
-  eval_unary_run(c->d_items.p, c->n_items, W, c->d_poses.p, eval_params(c), jac_kind, want_jac, c->d_partials.p, c->h_out.p,
-                 c->d_kf_item_start.p, c->d_ticket.p, c->st, c->lc, c->h_flag.p, epoch, c->h_poses.p);
+  eval_unary_run(tgt->d_items, tgt->n_items, W, c->d_poses.p, tgt->ep, jac_kind, want_jac, tgt->d_partials, c->h_out.p,
+                 tgt->d_kf_item_start, c->d_ticket.p, c->st, c->lc, c->h_flag.p, epoch, c->h_poses.p);
   (void)cudaStreamQuery(c->st);            // pushes the launch to the device now (otherwise it may sit in the driver's queue until the next API call)
   return epoch;
 }
@@ -453,6 +497,7 @@ int glio_create(int device, const glio_params* params, glio_ctx** out) {
 void glio_destroy(glio_ctx* c) {
   if (!c) return;
   cudaSetDevice(c->device);
+  while (!c->odoms.empty()) glio_odom_destroy(c->odoms.back());   // an odometry still attached (it detaches itself)
   if (c->marg_thread.joinable()) {
     if (c->marg_pending) { glio_marg_prior* dropped = nullptr; glio_marg_job_wait(c->marg_pending, &dropped); if (dropped) glio_marg_prior_destroy(dropped); }
     { std::lock_guard<std::mutex> lk(c->marg_mu); c->marg_quit = true; }
@@ -462,9 +507,7 @@ void glio_destroy(glio_ctx* c) {
   if (c->st_copy) cudaStreamSynchronize(c->st_copy);
   if (c->st) cudaStreamSynchronize(c->st);
   c->map.release(); c->map_stage.release(); c->map_stage2.release(); if (c->ev_map) cudaEventDestroy(c->ev_map);
-  for (auto& f : c->lm_frames) f->pts.release();
-  for (auto& f : c->lm_spare) f->pts.release();
-  c->lm_frames.clear(); c->lm_spare.clear(); c->lm_stage.release(); c->lm_cat.release(); c->lm_vox.release();
+  c->lm.release(); c->lm_stage.release();
   for (auto& f : c->frames) { f.second->scan.release(); f.second->grid.release(); }
   for (auto& p : c->pairs) { p->m_cpw.release(); p->m_nc.release(); p->m_src.release(); p->s_cpw.release(); p->s_nc.release(); }
   c->d_bin_items.release(); c->d_pair_item_start.release(); c->d_kf_inc_start.release(); c->d_inc.release(); c->d_bin_partials.release();
@@ -619,10 +662,7 @@ int glio_localmap_clear(glio_ctx* c) {
   if (!c) return GLIO_ERR_ARG;
   return guarded(c, [&] {
     GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
-    for (auto& f : c->lm_frames) f->pts.release();
-    c->lm_frames.clear();
-    for (auto& f : c->lm_spare) f->pts.release();
-    c->lm_spare.clear();
+    c->lm.clear();
   });
 }
 
@@ -631,56 +671,37 @@ int glio_localmap_push(glio_ctx* c, int at_front, const float* cloud_xyz, int64_
   return guarded(c, [&] {
     GLIO_REQUIRE(t && q, GLIO_ERR_ARG, "null pose");
     const float* d = stage_points(c, c->lm_stage, cloud_xyz, n, stride, mem);
-    std::unique_ptr<glio_ctx::LmFrame> f;
-    if (!c->lm_spare.empty()) { f = std::move(c->lm_spare.back()); c->lm_spare.pop_back(); }
-    else f = std::make_unique<glio_ctx::LmFrame>();
-    f->pts.reserve((size_t)n); f->n = n;
-    localmap_transform(d, stride, n, t, q, f->pts.p, c->st, c->lc);        // transformCloud: float(q*double(p)+t)
+    c->lm.push(at_front != 0, d, stride, n, t, q, c->st, c->lc);           // transformCloud: float(q*double(p)+t)
     if (mem != GLIO_DEVICE) GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));    // the staging buffer is reused by the next push
-    if (at_front) c->lm_frames.push_front(std::move(f)); else c->lm_frames.push_back(std::move(f));
   });
 }
 
 int glio_localmap_pop_front(glio_ctx* c) {
   if (!c) return GLIO_ERR_ARG;
   return guarded(c, [&] {
-    GLIO_REQUIRE(!c->lm_frames.empty(), GLIO_ERR_STATE, "local map holds no keyframe cloud");
-    // the stream is ordered: anything still reading the popped buffer was enqueued before whatever reuses it
-    c->lm_spare.push_back(std::move(c->lm_frames.front()));
-    c->lm_frames.pop_front();
+    GLIO_REQUIRE(!c->lm.frames.empty(), GLIO_ERR_STATE, "local map holds no keyframe cloud");
+    c->lm.pop_front();
   });
 }
 
 int glio_localmap_size(glio_ctx* c, int* n_frames, int64_t* n_points) {
   if (!c) return GLIO_ERR_ARG;
-  int64_t np = 0;
-  for (auto& f : c->lm_frames) np += f->n;
-  if (n_frames) *n_frames = (int)c->lm_frames.size();
-  if (n_points) *n_points = np;
+  if (n_frames) *n_frames = (int)c->lm.frames.size();
+  if (n_points) *n_points = c->lm.n_points();
   return GLIO_OK;
 }
 
 int glio_localmap_build(glio_ctx* c, float leaf, int64_t* n_map) {
   if (!c) return GLIO_ERR_ARG;
   return guarded(c, [&] {
-    int64_t N = 0;
-    for (auto& f : c->lm_frames) N += f->n;
-    GLIO_REQUIRE(N >= 5, GLIO_ERR_STATE, "local map needs at least 5 points");
-    c->lm_cat.reserve((size_t)N);
-    int64_t o = 0;
-    for (auto& f : c->lm_frames) {                                          // *surf_local_map += *recent_surf_keyframes[i]
-      GLIO_CUDA_TRY(cudaMemcpyAsync(c->lm_cat.p + o, f->pts.p, (size_t)f->n * sizeof(float4), cudaMemcpyDeviceToDevice, c->st));
-      o += f->n;
-    }
-    const int64_t m = leaf > 0.f ? voxel_filter_run(c->lm_vox, c->lm_cat.p, N, leaf, c->st, c->lc) : -1;   // ds_filter_surf_map.filter
-    if (m >= 0) {
-      GLIO_REQUIRE(m >= 5, GLIO_ERR_STATE, "down-sampled local map has fewer than 5 points");
-      grid_build(c->map, c->lm_vox.out_xyz.p, 3, m, nullptr, nullptr, c->prm.cell_size, c->pts_per_cell, c->st, c->lc);   // kd_tree_surf_local_map->setInputCloud
-      c->map_n = m;
-    } else {                                                                // leaf <= 0, or PCL's pass-through when the voxel grid would overflow
-      grid_build(c->map, reinterpret_cast<const float*>(c->lm_cat.p), 4, N, nullptr, nullptr, c->prm.cell_size, c->pts_per_cell, c->st, c->lc);
-      c->map_n = N;
-    }
+    GLIO_REQUIRE(c->lm.n_points() >= 5, GLIO_ERR_STATE, "local map needs at least 5 points");
+    // *surf_local_map += *recent_surf_keyframes[i] (:3605-3608), ds_filter_surf_map.filter (:3617-3618); leaf <= 0, or PCL's
+    // pass-through when the voxel grid would overflow, leaves the concatenation as it is
+    const float* pts = nullptr; int stride = 0; bool filtered = false;
+    const int64_t m = c->lm.build(leaf, &pts, &stride, &filtered, c->st, c->lc);
+    GLIO_REQUIRE(!filtered || m >= 5, GLIO_ERR_STATE, "down-sampled local map has fewer than 5 points");
+    grid_build(c->map, pts, stride, m, nullptr, nullptr, c->prm.cell_size, c->pts_per_cell, c->st, c->lc);   // kd_tree_surf_local_map->setInputCloud
+    c->map_n = m;
     c->has_map = true;
     if (n_map) *n_map = c->map_n;
   });
@@ -711,7 +732,7 @@ int glio_assoc_scan_to_map(glio_ctx* c, int slot, const float* scan_xyz, int64_t
     std::vector<std::array<double, 7>> lp(1);
     for (int k = 0; k < 3; ++k) lp[0][k] = t[k];
     for (int k = 0; k < 4; ++k) lp[0][3 + k] = q[k];
-    associate_slots(c, std::vector<int>{slot}, lp, n_match);
+    associate_ctx_slots(c, std::vector<int>{slot}, lp, n_match);
   });
 }
 
@@ -789,7 +810,7 @@ int glio_window_associate(glio_ctx* c, int W, const double* poses_body, int64_t*
       ids[k] = k;
       lidar_pose_in_map(c->prm.q_lb, c->prm.t_lb, poses_body + 7 * k, &lp[k][0], &lp[k][3]);   // Estimator.cpp:2216-2217
     }
-    associate_slots(c, ids, lp, n_match);
+    associate_ctx_slots(c, ids, lp, n_match);
   });
 }
 
@@ -1072,11 +1093,7 @@ int glio_prepare_scan(glio_ctx* c, const float* raw, int64_t n, int stride, int 
     GLIO_REQUIRE(n_out && out_capacity >= 0 && (out_xyzi || out_capacity == 0), GLIO_ERR_ARG, "glio_prepare_scan: bad output arguments");
     // a GLIO_DEVICE pointer must be memory of the context's GPU that the kernels can address: a host pointer, another GPU's
     // memory or a misaligned output is an argument error, never a fault
-    auto on_device = [c](const void* p) {
-      cudaPointerAttributes at{};
-      if (cudaPointerGetAttributes(&at, p) != cudaSuccess) { cudaGetLastError(); return false; }
-      return (at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged) && at.device == c->device;
-    };
+    auto on_device = [c](const void* p) { return on_ctx_device(c, p); };
     GLIO_REQUIRE(mem != GLIO_DEVICE || on_device(raw), GLIO_ERR_ARG, "glio_prepare_scan: mem = GLIO_DEVICE but raw is not device memory of the context's GPU");
     GLIO_REQUIRE(((uintptr_t)raw & 3) == 0, GLIO_ERR_ARG, "glio_prepare_scan: raw must be 4-byte aligned");
     GLIO_REQUIRE(out_mem != GLIO_DEVICE || !out_xyzi || on_device(out_xyzi), GLIO_ERR_ARG, "glio_prepare_scan: out_mem = GLIO_DEVICE but out_xyzi is not device memory of the context's GPU");
@@ -1160,14 +1177,25 @@ void glio_default_solver_options(glio_solver_options* o) {
   o->fuse_candidate_jacobian = 1;
 }
 
-static int window_solve_impl(glio_ctx* c, int W, double* poses, double* speed_bias, glio_host_factors_fn host_factors,
-                             glio_host_factors_band_fn host_band, int hb_hint, void* user,
-                             const glio_solver_options* options, glio_solver_summary* summary, glio_iteration* iter_log, int iter_cap,
-                             double* step_log, int64_t step_cap) {
-  if (!c) return GLIO_ERR_ARG;
-  return guarded(c, [&] {
-    GLIO_REQUIRE(W > 0 && W <= 4096 && poses, GLIO_ERR_ARG, "bad arguments");
-    glio_solver_options o; if (options) o = *options; else glio_default_solver_options(&o);
+static SolverOptions solver_options_from(const glio_solver_options& o) {
+  SolverOptions so;
+  so.max_num_iterations = o.max_num_iterations; so.dogleg_type = o.dogleg_type; so.use_nonmonotonic_steps = o.use_nonmonotonic_steps != 0;
+  so.max_consecutive_nonmonotonic_steps = o.max_consecutive_nonmonotonic_steps;
+  so.initial_trust_region_radius = o.initial_trust_region_radius; so.max_trust_region_radius = o.max_trust_region_radius;
+  so.min_trust_region_radius = o.min_trust_region_radius; so.min_relative_decrease = o.min_relative_decrease;
+  so.min_lm_diagonal = o.min_lm_diagonal; so.max_lm_diagonal = o.max_lm_diagonal;
+  so.max_num_consecutive_invalid_steps = o.max_num_consecutive_invalid_steps; so.jacobi_scaling = o.jacobi_scaling != 0;
+  so.function_tolerance = o.function_tolerance; so.gradient_tolerance = o.gradient_tolerance; so.parameter_tolerance = o.parameter_tolerance;
+  so.fuse_candidate_jacobian = o.fuse_candidate_jacobian != 0;
+  GLIO_REQUIRE(o.trust_region_strategy == 0 || o.trust_region_strategy == 1, GLIO_ERR_ARG, "trust_region_strategy must be 0 (DOGLEG) or 1 (LEVENBERG_MARQUARDT)");
+  so.trust_region_strategy = o.trust_region_strategy;
+  return so;
+}
+
+// The minimizer over W poses (and speed-bias states) with the LiDAR blocks of `tgt` (nullptr: the context's slots and glio_params)
+// plus the host factors.  Throws on error; poses / speed_bias are in/out.
+static void solve_core(glio_ctx* c, int W, double* poses, double* speed_bias, glio_host_factors_fn host_factors, glio_host_factors_band_fn host_band,
+                       int hb_hint, void* user, const SolverOptions& so, const EvalTarget* tgt, SolverSummary& S) {
     const bool sb = speed_bias != nullptr;
     const int nt = sb ? 15 : 6, na = sb ? 16 : 7, n = W * nt;
     std::vector<ParamBlock> blocks;
@@ -1176,17 +1204,6 @@ static int window_solve_impl(glio_ctx* c, int W, double* poses, double* speed_bi
       blocks.push_back(ParamBlock{na * k + 3, 4, nt * k + 3, 3, true, nullptr});
       if (sb) blocks.push_back(ParamBlock{na * k + 7, 9, nt * k + 6, 9, false, nullptr});
     }
-    SolverOptions so;
-    so.max_num_iterations = o.max_num_iterations; so.dogleg_type = o.dogleg_type; so.use_nonmonotonic_steps = o.use_nonmonotonic_steps != 0;
-    so.max_consecutive_nonmonotonic_steps = o.max_consecutive_nonmonotonic_steps;
-    so.initial_trust_region_radius = o.initial_trust_region_radius; so.max_trust_region_radius = o.max_trust_region_radius;
-    so.min_trust_region_radius = o.min_trust_region_radius; so.min_relative_decrease = o.min_relative_decrease;
-    so.min_lm_diagonal = o.min_lm_diagonal; so.max_lm_diagonal = o.max_lm_diagonal;
-    so.max_num_consecutive_invalid_steps = o.max_num_consecutive_invalid_steps; so.jacobi_scaling = o.jacobi_scaling != 0;
-    so.function_tolerance = o.function_tolerance; so.gradient_tolerance = o.gradient_tolerance; so.parameter_tolerance = o.parameter_tolerance;
-    so.fuse_candidate_jacobian = o.fuse_candidate_jacobian != 0;
-    GLIO_REQUIRE(o.trust_region_strategy == 0 || o.trust_region_strategy == 1, GLIO_ERR_ARG, "trust_region_strategy must be 0 (DOGLEG) or 1 (LEVENBERG_MARQUARDT)");
-    so.trust_region_strategy = o.trust_region_strategy;
     TrustRegionDogleg solver(blocks, so);
     std::vector<double> x((size_t)W * na), pz((size_t)W * 7), sz((size_t)W * 9);
     for (int k = 0; k < W; ++k) {
@@ -1201,7 +1218,7 @@ static int window_solve_impl(glio_ctx* c, int W, double* poses, double* speed_bi
         if (sb) for (int i = 0; i < 9; ++i) sz[9 * k + i] = xa[(size_t)na * k + 7 + i];
       }
       // the device evaluates the LiDAR residuals while the host evaluates its own factors
-      const unsigned int epoch = eval_unary_launch(c, W, pz.data(), 0, want_jac);
+      const unsigned int epoch = eval_unary_launch(c, W, pz.data(), 0, want_jac, tgt);
       double ct = 0;
       if (want_jac) std::fill(g, g + n, 0.0);
       auto add_device = [&]() {
@@ -1250,13 +1267,25 @@ static int window_solve_impl(glio_ctx* c, int W, double* poses, double* speed_bi
       *cost = ct;
       return std::isfinite(ct);
     };
-    SolverSummary S;
     solver.solve(x.data(), eval, &S);
     for (int k = 0; k < W; ++k) {
       for (int i = 0; i < 7; ++i) poses[7 * k + i] = x[(size_t)na * k + i];
       if (sb) for (int i = 0; i < 9; ++i) speed_bias[9 * k + i] = x[(size_t)na * k + 7 + i];
     }
-    fill_summary(S, n, summary, iter_log, iter_cap, step_log, step_cap);
+}
+
+static int window_solve_impl(glio_ctx* c, int W, double* poses, double* speed_bias, glio_host_factors_fn host_factors,
+                             glio_host_factors_band_fn host_band, int hb_hint, void* user,
+                             const glio_solver_options* options, glio_solver_summary* summary, glio_iteration* iter_log, int iter_cap,
+                             double* step_log, int64_t step_cap) {
+  if (!c) return GLIO_ERR_ARG;
+  return guarded(c, [&] {
+    GLIO_REQUIRE(W > 0 && W <= 4096 && poses, GLIO_ERR_ARG, "bad arguments");
+    glio_solver_options o; if (options) o = *options; else glio_default_solver_options(&o);
+    const SolverOptions so = solver_options_from(o);
+    SolverSummary S;
+    solve_core(c, W, poses, speed_bias, host_factors, host_band, hb_hint, user, so, nullptr, S);
+    fill_summary(S, W * (speed_bias ? 15 : 6), summary, iter_log, iter_cap, step_log, step_cap);
   });
 }
 
@@ -1359,10 +1388,10 @@ int glio_batch_associate_pairs(glio_ctx* c, const int32_t* pairs_cur, const int3
         for (int k = 0; k < 4; ++k) segs[s].q[k] = fc.pose[3 + k];
         Qt += fc.Q;
       }
-      ensure_work(c, Qt, true);
+      ensure_work(c, Qt, true, c->prm.keep_debug != 0);
       c->d_segs.reserve(nseg); c->d_dst.reserve(nseg); c->d_counts.reserve(nseg); c->h_counts.reserve(nseg);
       GLIO_CUDA_TRY(cudaMemcpyAsync(c->d_segs.p, segs.data(), nseg * sizeof(SegDesc), cudaMemcpyHostToDevice, c->st));
-      AssocWork w = make_work(c, Qt, true);
+      AssocWork w = make_work(c, Qt, true, c->prm.keep_debug != 0);
       assoc_run(fo.grid, c->d_segs.p, nseg, w, gates, fo.scan_ptr, fo.stride, c->cell_count, c->cell_pos, c->scan_tmp, c->st, c->lc);
       compact_count(w, c->d_segs.p, nseg, c->w_flags.p, c->w_pos.p, c->scan_tmp, c->d_counts.p, c->st, c->lc);
       GLIO_CUDA_TRY(cudaMemcpyAsync(c->h_counts.p, c->d_counts.p, nseg * sizeof(int), cudaMemcpyDeviceToHost, c->st));
@@ -1732,6 +1761,278 @@ int glio_eval_edge(glio_ctx* c, int W, const double* poses_body, double* H, doub
       if (g) for (int p = 0; p < 6; ++p) g[6 * k + p] = o[21 + p];
       if (cost) cost[k] = o[27];
     }
+  });
+}
+
+}  // extern "C"
+
+// ------------------------------------------------------------------------------------------------------------
+// front-end LiDAR odometry (SURVEY 8 f-6): LidarOdometry::run, GLIO/src/LidarOdometry.cpp:661-695
+// ------------------------------------------------------------------------------------------------------------
+struct glio_odom {
+  glio_ctx* ctx = nullptr;
+  glio_odom_options opt{};
+  // the node's state; poses in its own layout q(w,x,y,z), t(x,y,z)
+  bool initialized = false;             // system_initialized
+  double abs_pose[7], rel_pose[7];
+  int64_t n_poses = 0;                  // pose_cloud_frame->points.size()
+  double last_pose[7];                  // pose_info_cloud_frame->points.back()
+  bool kf = true;
+  int64_t kf_num = 0, latest_frame_idx = 0;
+  double trans_last_kf[3], quat_last_kf[4];
+  // device state
+  LocalMap lm;                          // recent_surf_frames, surf_from_map and down_size_filter_surf_map
+  VoxelWork scan_vox;                   // down_size_filter_surf
+  DevBuf<float> last_ds; int last_ds_stride = 3; int64_t last_ds_n = 0;   // surf_frames.back(): the previous sweep's surf_last_ds
+  DevBuf<float4> in_surf, in_full, out_surf, out_full;                    // owned copy of the surf input, staging of host clouds
+  const float* map_pts = nullptr; int map_stride = 3; int64_t map_n = 0;  // surf_from_map_ds of the last step
+  GridBuild grid;                       // kd_tree_surf_last
+  Slot slot;                            // surf_current_pts / surf_normal
+  DevBuf<EvalItem> d_items; DevBuf<int> d_start; DevBuf<double> d_partials;
+
+  void reset_state() {
+    initialized = false;
+    for (int k = 0; k < 7; ++k) { abs_pose[k] = k == 0 ? 1.0 : 0.0; rel_pose[k] = abs_pose[k]; last_pose[k] = abs_pose[k]; }
+    n_poses = 0; kf = true; kf_num = 0; latest_frame_idx = 0;
+    trans_last_kf[0] = trans_last_kf[1] = trans_last_kf[2] = 0.0;
+    quat_last_kf[0] = 1.0; quat_last_kf[1] = quat_last_kf[2] = quat_last_kf[3] = 0.0;
+    while (!lm.frames.empty()) lm.pop_front();   // buffers kept for the next run
+    last_ds_n = 0; map_pts = nullptr; map_n = 0;
+  }
+  void release() {
+    lm.release(); scan_vox.release(); last_ds.release(); in_surf.release(); in_full.release(); out_surf.release(); out_full.release();
+    grid.release(); slot.release(); d_items.release(); d_start.release(); d_partials.release();
+  }
+};
+
+namespace {
+
+// VoxelGrid(0.2) of n device points (float4); *pts / *stride receive the filtered cloud, or the input when PCL passes it through
+int64_t odom_voxel(glio_ctx* c, VoxelWork& w, const float4* in, int64_t n, const float** pts, int* stride) {
+  if (n <= 0) { *pts = nullptr; *stride = 3; return 0; }
+  const int64_t m = voxel_filter_run(w, in, n, 0.2f, c->st, c->lc);
+  if (m >= 0) { *pts = w.out_xyz.p; *stride = 3; return m; }
+  *pts = reinterpret_cast<const float*>(in); *stride = 4;
+  return n;
+}
+
+void odom_step(glio_odom* o, const float4* surf, int64_t n_surf, const float4* full, int64_t n_full, float* surf_out, float* full_out,
+               int out_mem, glio_odom_report* rep) {
+  glio_ctx* c = o->ctx;
+  glio_odom_report R;
+  memset(&R, 0, sizeof(R));
+  // outputs of this sweep, written only when the node publishes
+  float4* so = nullptr; float4* fo = nullptr;
+  if (out_mem == GLIO_DEVICE) { so = reinterpret_cast<float4*>(surf_out); fo = reinterpret_cast<float4*>(full_out); }
+  else {
+    if (surf_out && n_surf) { o->out_surf.reserve((size_t)n_surf); so = o->out_surf.p; }
+    if (full_out && n_full) { o->out_full.reserve((size_t)n_full); fo = o->out_full.p; }
+  }
+  bool publish = false;
+  double trans[3] = {0.0, 0.0, 0.0};
+  int deskew = 0;
+  if (!o->initialized) {
+    // savePoses with abs_pose = identity and an empty surf_last_ds, then checkInitialization: the clouds pass through unchanged
+    o->n_poses += 1;
+    for (int k = 0; k < 7; ++k) o->last_pose[k] = o->abs_pose[k];
+    o->last_ds_n = 0; o->map_n = 0;
+    o->initialized = true;
+    R.initialised = 1;
+    publish = true;
+  } else {
+    odom_predict(o->abs_pose, o->rel_pose);                                    // poseInitialization
+    // buildLocalMap (:267-288)
+    const float* src = nullptr; int64_t src_n = 0;                              // float4 points, scan or world frame
+    if (o->n_poses <= 1) { src = reinterpret_cast<const float*>(surf); src_n = n_surf; }   // the sweep's own surf cloud, scan frame
+    else {
+      const double t[3] = {o->last_pose[4], o->last_pose[5], o->last_pose[6]};
+      const double q[4] = {o->last_pose[0], o->last_pose[1], o->last_pose[2], o->last_pose[3]};
+      if (o->lm.frames.size() < 20) o->lm.push(false, o->last_ds.p, o->last_ds_stride, o->last_ds_n, t, q, c->st, c->lc);
+      else if (o->latest_frame_idx != o->n_poses - 1) {
+        o->lm.pop_front();
+        o->latest_frame_idx = o->n_poses - 1;
+        o->lm.push(false, o->last_ds.p, o->last_ds_stride, o->last_ds_n, t, q, c->st, c->lc);
+      }
+      bool filtered = false; int cat_stride = 4;
+      src_n = o->lm.build(0.f, &src, &cat_stride, &filtered, c->st, c->lc);      // concatenation only (float4): the filter follows
+    }
+    // downSampleCloud (:305-313)
+    o->map_n = odom_voxel(c, o->lm.vox, reinterpret_cast<const float4*>(src), src_n, &o->map_pts, &o->map_stride);
+    const float* scan = nullptr; int scan_stride = 3;
+    const int64_t scan_n = odom_voxel(c, o->scan_vox, surf, n_surf, &scan, &scan_stride);
+    R.n_map = o->map_n; R.n_scan = scan_n;
+    // updateTransformationWithCeres (:474-579)
+    if (o->map_n < 10) R.skipped = 1;                                           // "Not enough feature points from the map"
+    else {
+      grid_build(o->grid, o->map_pts, o->map_stride, o->map_n, nullptr, nullptr, 0.f, c->pts_per_cell, c->st, c->lc);
+      const int rounds = o->n_poses < 2 ? 8 : o->opt.scan_match_cnt;
+      const AssocGates gates{1.0, 0.06, 0.4};
+      EvalParams ep{};
+      ep.q_lb[0] = 1.0; ep.lidar_const = 1.0; ep.huber_delta = 0.1; ep.unit_score = 1;       // LidarPlaneNormIncreFactor, HuberLoss(0.1)
+      glio_solver_options go; glio_default_solver_options(&go);
+      go.trust_region_strategy = 1; go.max_num_iterations = o->opt.max_num_iter;             // Ceres defaults: LEVENBERG_MARQUARDT
+      SolverOptions sopt = solver_options_from(go);
+      sopt.max_solver_time_in_seconds = o->opt.max_solver_time_s;
+      o->slot.scan_ptr = scan; o->slot.stride = scan_stride; o->slot.Q = scan_n;
+      SolverSummary S;
+      for (int r = 0; r < rounds; ++r) {
+        double x[7] = {o->abs_pose[4], o->abs_pose[5], o->abs_pose[6], o->abs_pose[0], o->abs_pose[1], o->abs_pose[2], o->abs_pose[3]};
+        int64_t nm = 0;
+        if (scan_n > 0) {
+          const std::array<double, 7> lp = {x[0], x[1], x[2], x[3], x[4], x[5], x[6]};
+          associate_slots(c, o->grid, gates, false, std::vector<Slot*>{&o->slot}, std::vector<std::array<double, 7>>{lp}, &nm);
+        }
+        if (nm > 0) {
+          std::vector<int> start;
+          const std::vector<EvalItem> items = plan_items(std::vector<const Slot*>{&o->slot}, c->eval_slots, start);
+          upload_items(c, 1, items, start, o->d_items, o->d_start, o->d_partials);
+          const EvalTarget tgt{o->d_items.p, (int)items.size(), o->d_start.p, o->d_partials.p, ep};
+          solve_core(c, 1, x, nullptr, nullptr, nullptr, -1, nullptr, sopt, &tgt, S);
+        } else {
+          // no residual uses the pose: Ceres drops the parameter blocks and Minimize returns at once (solver.cc:410-418)
+          S = SolverSummary();
+          S.termination = TERM_CONVERGENCE;
+          S.message = "Function tolerance reached. No non-constant parameter blocks found.";
+        }
+        o->abs_pose[4] = x[0]; o->abs_pose[5] = x[1]; o->abs_pose[6] = x[2];
+        o->abs_pose[0] = x[3]; o->abs_pose[1] = x[4]; o->abs_pose[2] = x[5]; o->abs_pose[3] = x[6];
+        if (o->abs_pose[0] < 0) for (int k = 0; k < 4; ++k) o->abs_pose[k] = -o->abs_pose[k];      // unifyQuaternion (:532-542)
+        R.round_n_match[r] = nm;
+        R.round_iterations[r] = (int)S.iterations.size();
+        R.round_successful[r] = S.num_successful_steps;
+        R.round_termination[r] = S.termination;
+        for (int k = 0; k < 3; ++k) R.round_pose[r][k] = o->abs_pose[4 + k];
+        for (int k = 0; k < 4; ++k) R.round_pose[r][3 + k] = o->abs_pose[k];
+      }
+      R.n_rounds = rounds;
+      fill_summary(S, 6, &R.summary, nullptr, 0, nullptr, 0);
+      if (odom_keyframe_rule(o->abs_pose + 4, o->abs_pose, o->trans_last_kf, o->quat_last_kf, o->n_poses, o->kf_num)) {
+        o->kf = true;
+        for (int k = 0; k < 3; ++k) o->trans_last_kf[k] = o->abs_pose[4 + k];
+        for (int k = 0; k < 4; ++k) o->quat_last_kf[k] = o->abs_pose[k];
+      } else o->kf = false;
+    }
+    // savePoses: the pose and surf_last_ds of this sweep
+    double prev[7];
+    for (int k = 0; k < 7; ++k) { prev[k] = o->last_pose[k]; o->last_pose[k] = o->abs_pose[k]; }
+    o->n_poses += 1;
+    o->last_ds_stride = scan_stride; o->last_ds_n = scan_n;
+    if (scan_n > 0) {
+      o->last_ds.reserve((size_t)scan_n * scan_stride);
+      GLIO_CUDA_TRY(cudaMemcpyAsync(o->last_ds.p, scan, (size_t)scan_n * scan_stride * sizeof(float), cudaMemcpyDeviceToDevice, c->st));
+    }
+    odom_relative(prev, o->abs_pose, o->rel_pose);                              // computeRelative
+    if (o->kf) {
+      o->kf_num = o->n_poses;
+      publish = true;
+      deskew = o->opt.deskew != 0;
+      trans[0] = o->rel_pose[4]; trans[1] = o->rel_pose[5]; trans[2] = o->rel_pose[6];
+    }
+    R.keyframe = o->kf ? 1 : 0;
+  }
+  if (publish) {
+    odom_publish_run(surf, so ? n_surf : 0, full, fo ? n_full : 0, so, fo, trans, deskew, c->st, c->lc);
+    if (out_mem != GLIO_DEVICE) {
+      if (so) GLIO_CUDA_TRY(cudaMemcpyAsync(surf_out, so, (size_t)n_surf * sizeof(float4), cudaMemcpyDeviceToHost, c->st));
+      if (fo) GLIO_CUDA_TRY(cudaMemcpyAsync(full_out, fo, (size_t)n_full * sizeof(float4), cudaMemcpyDeviceToHost, c->st));
+    }
+  }
+  GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
+  for (int k = 0; k < 3; ++k) { R.pose[k] = o->abs_pose[4 + k]; R.rel_pose[k] = o->rel_pose[4 + k]; }
+  for (int k = 0; k < 4; ++k) { R.pose[3 + k] = o->abs_pose[k]; R.rel_pose[3 + k] = o->rel_pose[k]; }
+  if (rep) *rep = R;
+}
+
+}  // namespace
+
+extern "C" {
+
+void glio_odom_default_options(glio_odom_options* o) {
+  if (!o) return;
+  memset(o, 0, sizeof(*o));
+  o->max_num_iter = 12; o->scan_match_cnt = 1; o->deskew = 0; o->max_solver_time_s = 0.015;   // GLIO/config/config_urban_hk.yaml:19-21
+}
+
+int glio_odom_create(glio_ctx* c, const glio_odom_options* options, glio_odom** out) {
+  if (!c || !out) return GLIO_ERR_ARG;
+  *out = nullptr;
+  return guarded(c, [&] {
+    glio_odom_options opt; if (options) opt = *options; else glio_odom_default_options(&opt);
+    GLIO_REQUIRE(opt.max_num_iter >= 0 && opt.scan_match_cnt >= 1 && opt.scan_match_cnt <= GLIO_ODOM_MAX_ROUNDS && opt.max_solver_time_s >= 0.0,
+                 GLIO_ERR_ARG, "glio_odom_create: need max_num_iter >= 0, 1 <= scan_match_cnt <= 8, max_solver_time_s >= 0");
+    std::unique_ptr<glio_odom> o(new glio_odom());
+    o->ctx = c; o->opt = opt;
+    o->grid.build_pairs = false;
+    o->reset_state();
+    c->odoms.push_back(o.get());
+    *out = o.release();
+  });
+}
+
+void glio_odom_destroy(glio_odom* o) {
+  if (!o) return;
+  glio_ctx* c = o->ctx;
+  cudaSetDevice(c->device);
+  cudaStreamSynchronize(c->st);
+  o->release();
+  c->odoms.erase(std::remove(c->odoms.begin(), c->odoms.end(), o), c->odoms.end());
+  delete o;
+}
+
+int glio_odom_reset(glio_odom* o) {
+  if (!o) return GLIO_ERR_ARG;
+  return guarded(o->ctx, [&] { GLIO_CUDA_TRY(cudaStreamSynchronize(o->ctx->st)); o->reset_state(); });
+}
+
+int glio_odom_step(glio_odom* o, const float* surf, int64_t n_surf, int surf_mem, const float* full, int64_t n_full, int full_mem,
+                   float* surf_out, float* full_out, int out_mem, glio_odom_report* rep) {
+  if (!o) return GLIO_ERR_ARG;
+  glio_ctx* c = o->ctx;
+  return guarded(c, [&] {
+    // every argument is checked before anything is enqueued or any state changes
+    const int64_t kMax = (int64_t)1 << 30;
+    GLIO_REQUIRE(n_surf >= 0 && n_surf < kMax && (surf || n_surf == 0), GLIO_ERR_ARG, "glio_odom_step: bad surf cloud");
+    GLIO_REQUIRE(n_full >= 0 && n_full < kMax && (full || n_full == 0), GLIO_ERR_ARG, "glio_odom_step: bad full cloud");
+    GLIO_REQUIRE((surf_mem == GLIO_HOST || surf_mem == GLIO_DEVICE) && (full_mem == GLIO_HOST || full_mem == GLIO_DEVICE) &&
+                 (out_mem == GLIO_HOST || out_mem == GLIO_DEVICE), GLIO_ERR_ARG, "glio_odom_step: mem must be GLIO_HOST or GLIO_DEVICE");
+    auto dev_ok = [c](const void* p) { return on_ctx_device(c, p) && ((uintptr_t)p & 15) == 0; };
+    GLIO_REQUIRE(surf_mem != GLIO_DEVICE || n_surf == 0 || dev_ok(surf), GLIO_ERR_ARG,
+                 "glio_odom_step: a GLIO_DEVICE surf cloud must be 16-byte aligned memory of the context's GPU");
+    GLIO_REQUIRE(full_mem != GLIO_DEVICE || n_full == 0 || dev_ok(full), GLIO_ERR_ARG,
+                 "glio_odom_step: a GLIO_DEVICE full cloud must be 16-byte aligned memory of the context's GPU");
+    GLIO_REQUIRE(out_mem != GLIO_DEVICE || ((!surf_out || n_surf == 0 || dev_ok(surf_out)) && (!full_out || n_full == 0 || dev_ok(full_out))),
+                 GLIO_ERR_ARG, "glio_odom_step: device outputs must be 16-byte aligned memory of the context's GPU (float4 stores)");
+    // the surf cloud is kept for the whole step (map of sweep 2, scan filter, pass-through): always an owned device copy
+    o->in_surf.reserve((size_t)std::max<int64_t>(n_surf, 1));
+    if (n_surf) GLIO_CUDA_TRY(cudaMemcpyAsync(o->in_surf.p, surf, (size_t)n_surf * sizeof(float4),
+                                              surf_mem == GLIO_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, c->st));
+    const float4* d_full = reinterpret_cast<const float4*>(full);
+    if (n_full && full_mem != GLIO_DEVICE) {
+      o->in_full.reserve((size_t)n_full);
+      GLIO_CUDA_TRY(cudaMemcpyAsync(o->in_full.p, full, (size_t)n_full * sizeof(float4), cudaMemcpyHostToDevice, c->st));
+      d_full = o->in_full.p;
+    }
+    odom_step(o, o->in_surf.p, n_surf, d_full, n_full, surf_out, full_out, out_mem, rep);
+  });
+}
+
+int glio_odom_get_clouds(glio_odom* o, int64_t map_capacity, float* map_xyz, int64_t* n_map, int64_t scan_capacity, float* scan_xyz, int64_t* n_scan) {
+  if (!o) return GLIO_ERR_ARG;
+  glio_ctx* c = o->ctx;
+  return guarded(c, [&] {
+    const int64_t nm = o->map_pts ? o->map_n : 0, ns = o->last_ds_n;
+    if (n_map) *n_map = nm;
+    if (n_scan) *n_scan = ns;
+    GLIO_REQUIRE((!map_xyz || map_capacity >= nm) && (!scan_xyz || scan_capacity >= ns), GLIO_ERR_ARG, "glio_odom_get_clouds: capacity too small");
+    auto fetch = [&](const float* d, int stride, int64_t n, float* xyz) {
+      if (!xyz || n <= 0) return;
+      std::vector<float> h((size_t)n * stride);
+      GLIO_CUDA_TRY(cudaMemcpyAsync(h.data(), d, h.size() * sizeof(float), cudaMemcpyDeviceToHost, c->st));
+      GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
+      for (int64_t i = 0; i < n; ++i) for (int k = 0; k < 3; ++k) xyz[3 * i + k] = h[(size_t)i * stride + k];
+    };
+    fetch(o->map_pts, o->map_stride, nm, map_xyz);
+    fetch(o->last_ds.p, o->last_ds_stride, ns, scan_xyz);
   });
 }
 

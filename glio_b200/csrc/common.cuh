@@ -7,6 +7,8 @@
 #include <algorithm>
 #include <cmath>
 #include <cstring>
+#include <deque>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -198,6 +200,25 @@ void localmap_transform(const float* d_xyz, int stride, int64_t n, const double*
 // returns the number of filtered points (in w.out_xyz / w.out_vox), or -1 when PCL would pass the input through unchanged
 int64_t voxel_filter_run(VoxelWork& w, const float4* d_in, int64_t n, float leaf, cudaStream_t st, LaunchCounter& lc);
 
+// A deque of world-frame clouds, their concatenation and its voxel filter: the context's local map (glio_localmap_*,
+// Estimator.cpp:3529-3618) and the odometry's (LidarOdometry.cpp:267-288, :305-313) are both one of these.
+struct LocalMap {
+  struct Frame { DevBuf<float4> pts; int64_t n = 0; };
+  std::deque<std::unique_ptr<Frame>> frames;
+  std::vector<std::unique_ptr<Frame>> spare;   // buffers of popped frames, reused by the next push (no cudaFree / cudaMalloc per frame)
+  DevBuf<float4> cat;
+  VoxelWork vox;
+  // transformCloud(cloud, {t, q}) = float(q*double(p)+t) on the device, then push_front / push_back
+  void push(bool at_front, const float* d_xyz, int stride, int64_t n, const double* t, const double* q, cudaStream_t st, LaunchCounter& lc);
+  void pop_front();            // the stream is ordered: anything still reading the popped buffer was enqueued before whatever reuses it
+  void clear();                // frees every frame buffer
+  int64_t n_points() const;
+  // concatenate (oldest first) and VoxelGrid(leaf) when leaf > 0; *pts / *stride receive the device cloud.  Returns its size and
+  // sets *filtered = false when leaf <= 0 or PCL's overflow rule passed the concatenation through unchanged.
+  int64_t build(float leaf, const float** pts, int* stride, bool* filtered, cudaStream_t st, LaunchCounter& lc);
+  void release() { clear(); cat.release(); vox.release(); }
+};
+
 // ---- K1 / K1b (assoc.cu)
 void assoc_run(const GridBuild& gb, const SegDesc* d_segs, int nseg, const AssocWork& w, const AssocGates& gates,
                const float* oth_local, int oth_stride, DevBuf<int>& cell_count, DevBuf<int>& cell_pos,
@@ -295,5 +316,18 @@ struct ScanPrepArgs {
 };
 void scanprep_run(ScanPrepArgs& a, cudaStream_t st, LaunchCounter& lc);
 void imu_sweep_rotation(glio_imu_state* st, const double* stamps, const double* gyro, int64_t n, double t_cur, double q[4]);
+
+// ---- front-end odometry (odometry.cu; LidarOdometry.cpp).  Poses here are the reference's abs_pose / rel_pose layout:
+// q(w,x,y,z) then t(x,y,z).  Host arithmetic is scalar double in Eigen's operation order, built without FMA contraction.
+void odom_predict(double abs_pose[7], const double rel_pose[7]);                                   // poseInitialization, :406-433
+void odom_relative(const double prev[7], const double cur[7], double rel_pose[7]);                 // computeRelative, :435-471
+// the keyframe test of updateTransformationWithCeres (:566-578); size = pose count before this sweep's savePoses
+bool odom_keyframe_rule(const double t_cur[3], const double q_cur[4], const double t_last_kf[3], const double q_last_kf[4],
+                        int64_t size, int64_t kf_num);
+void odom_quat_inverse(const double q[4], double o[4]);                                              // Eigen inverse(): conj / squaredNorm
+// publishCloudLast's undistortion (:176-200, :619-632) of surf and full in one launch: trans = rel_pose translation;
+// deskew = 0 copies the clouds (checkInitialization, or if_to_deskew = false)
+void odom_publish_run(const float4* surf, int64_t n_surf, const float4* full, int64_t n_full, float4* surf_out, float4* full_out,
+                      const double trans[3], int deskew, cudaStream_t st, LaunchCounter& lc);
 
 }  // namespace glio

@@ -445,5 +445,47 @@ int64_t voxel_filter_run(VoxelWork& w, const float4* d_in, int64_t n, float leaf
   return (int64_t)m;
 }
 
+void LocalMap::push(bool at_front, const float* d_xyz, int stride, int64_t n, const double* t, const double* q, cudaStream_t st, LaunchCounter& lc) {
+  std::unique_ptr<Frame> f;
+  if (!spare.empty()) { f = std::move(spare.back()); spare.pop_back(); }
+  else f = std::make_unique<Frame>();
+  f->pts.reserve((size_t)n); f->n = n;
+  if (n > 0) localmap_transform(d_xyz, stride, n, t, q, f->pts.p, st, lc);
+  if (at_front) frames.push_front(std::move(f)); else frames.push_back(std::move(f));
+}
+
+void LocalMap::pop_front() {
+  spare.push_back(std::move(frames.front()));
+  frames.pop_front();
+}
+
+void LocalMap::clear() {
+  for (auto& f : frames) f->pts.release();
+  frames.clear();
+  for (auto& f : spare) f->pts.release();
+  spare.clear();
+}
+
+int64_t LocalMap::n_points() const {
+  int64_t np = 0;
+  for (auto& f : frames) np += f->n;
+  return np;
+}
+
+int64_t LocalMap::build(float leaf, const float** pts, int* stride, bool* filtered, cudaStream_t st, LaunchCounter& lc) {
+  const int64_t N = n_points();
+  cat.reserve((size_t)N);
+  int64_t o = 0;
+  for (auto& f : frames) {
+    if (f->n) GLIO_CUDA_TRY(cudaMemcpyAsync(cat.p + o, f->pts.p, (size_t)f->n * sizeof(float4), cudaMemcpyDeviceToDevice, st));
+    o += f->n;
+  }
+  const int64_t m = (leaf > 0.f && N > 0) ? voxel_filter_run(vox, cat.p, N, leaf, st, lc) : -1;
+  *filtered = m >= 0;
+  if (m >= 0) { *pts = vox.out_xyz.p; *stride = 3; return m; }
+  *pts = reinterpret_cast<const float*>(cat.p); *stride = 4;
+  return N;
+}
+
 
 }  // namespace glio

@@ -191,6 +191,41 @@ def raw_elevations(n_rings):
     raise ValueError("n_rings must be 16, 32 or 64")
 
 
+def _nearest_hit(sc, origin, dw, rects=None):
+    """Distance along each world-frame ray dw[i] from origin (one point, or one per ray) to the nearest rectangle of the scene hit
+    further than 0.5 m; inf for a miss.  rects: indices of the rectangles to test (default: all)."""
+    best = np.full(len(dw), np.inf)
+    for i in (range(len(sc.o)) if rects is None else rects):
+        o, u, v, nrm = sc.o[i], sc.u[i], sc.v[i], sc.n[i]
+        den = dw @ nrm
+        with np.errstate(divide="ignore", invalid="ignore"):
+            t = ((o - origin) @ nrm) / den
+            hit = origin + t[:, None] * dw - o
+            a = (hit @ u) / (u @ u); b = (hit @ v) / (v @ v)
+        ok = (np.abs(den) > 1e-9) & (t > 0.5) & (a >= 0) & (a <= 1) & (b >= 0) & (b <= 1)
+        best = np.where(ok & (t < best), t, best)
+    return best
+
+
+def _cast_firings(sc, origin, e, az, psi, rng, noise, near_frac, nan_frac, n_zaxis, rects=None):
+    """Raw returns (n, 4) float32 in the sensor frame for rays of elevation e and azimuth az from a sensor yawed by psi at origin."""
+    d = np.stack([np.cos(e) * np.cos(az), np.cos(e) * np.sin(az), np.sin(e)], 1)          # sensor frame
+    dw = np.stack([np.cos(psi) * d[:, 0] - np.sin(psi) * d[:, 1], np.sin(psi) * d[:, 0] + np.cos(psi) * d[:, 1], d[:, 2]], 1)
+    best = _nearest_hit(sc, origin, dw, rects)
+    rg = best + rng.normal(0.0, noise, len(best))
+    near = rng.random(len(rg)) < near_frac
+    rg[near] = rng.uniform(0.5, 2.9, int(near.sum()))
+    rg[~np.isfinite(best) | (best > 80.0) | (rng.random(len(rg)) < nan_frac)] = np.nan
+    raw = np.empty((len(d), 4), np.float32)
+    raw[:, :3] = rg[:, None] * d
+    raw[:, 3] = rng.uniform(0.0, 100.0, len(d))
+    if n_zaxis:
+        at = rng.choice(len(raw), n_zaxis, replace=False)
+        raw[at, 0] = 0.0; raw[at, 1] = 0.0
+        raw[at, 2] = rng.choice([-1.0, 1.0], n_zaxis) * rng.uniform(3.5, 20.0, n_zaxis)
+    return raw
+
+
 def raw_sweep(n_rings=32, n_az=1875, start_az=0.3, coverage=2 * np.pi - 0.02, yaw_rate=0.0, seed=SEED0 + 12, t0=100.0,
               sweep_time=0.1, imu_rate=400.0, noise=0.01, nan_frac=0.01, near_frac=0.005, n_zaxis=4):
     """A raw spinning-LiDAR sweep as the driver delivers it (the input of Preprocessing::cloudHandler, GLIO/src/Preprocessing.cpp:387):
@@ -211,32 +246,56 @@ def raw_sweep(n_rings=32, n_az=1875, start_az=0.3, coverage=2 * np.pi - 0.02, ya
     line = np.tile(order, n_az)
     az = start_az - coverage * k / n_az
     psi = yaw_rate * sweep_time * k / n_az                   # sensor yaw at the firing's time
-    e = elev[line]
-    d = np.stack([np.cos(e) * np.cos(az), np.cos(e) * np.sin(az), np.sin(e)], 1)          # sensor frame
-    dw = np.stack([np.cos(psi) * d[:, 0] - np.sin(psi) * d[:, 1], np.sin(psi) * d[:, 0] + np.cos(psi) * d[:, 1], d[:, 2]], 1)
-    best = np.full(len(d), np.inf)
-    for o, u, v, nrm in zip(sc.o, sc.u, sc.v, sc.n):
-        den = dw @ nrm
-        with np.errstate(divide="ignore", invalid="ignore"):
-            t = ((o - origin) @ nrm) / den
-            hit = origin + t[:, None] * dw - o
-            a = (hit @ u) / (u @ u); b = (hit @ v) / (v @ v)
-        ok = (np.abs(den) > 1e-9) & (t > 0.5) & (a >= 0) & (a <= 1) & (b >= 0) & (b <= 1)
-        best = np.where(ok & (t < best), t, best)
-    rg = best + rng.normal(0.0, noise, len(best))
-    near = rng.random(len(rg)) < near_frac
-    rg[near] = rng.uniform(0.5, 2.9, int(near.sum()))
-    rg[~np.isfinite(best) | (best > 80.0) | (rng.random(len(rg)) < nan_frac)] = np.nan
-    raw = np.empty((len(d), 4), np.float32)
-    raw[:, :3] = rg[:, None] * d
-    raw[:, 3] = rng.uniform(0.0, 100.0, len(d))
-    if n_zaxis:
-        at = rng.choice(len(raw), n_zaxis, replace=False)
-        raw[at, 0] = 0.0; raw[at, 1] = 0.0
-        raw[at, 2] = rng.choice([-1.0, 1.0], n_zaxis) * rng.uniform(3.5, 20.0, n_zaxis)
+    raw = _cast_firings(sc, origin, elev[line], az, psi, rng, noise, near_frac, nan_frac, n_zaxis)
     stamps = t0 - 0.05 + np.arange(int((sweep_time + 0.1) * imu_rate) + 1) / imu_rate
     gyro = np.zeros((len(stamps), 3)); gyro[:, 2] = yaw_rate
     return dict(raw=raw, stamps=stamps, gyro=gyro, t_scan_next=t0 + sweep_time, elev_deg=np.rad2deg(elev))
+
+
+def raw_drive(K, n_rings=32, speed=5.0, yaw_rate=0.1, seed=SEED0 + 13, n_az=1875, sweep_time=0.1, t0=100.0, imu_rate=400.0,
+              noise=0.01, nan_frac=0.01, weave_period=8.0):
+    """K consecutive raw sweeps (raw_sweep's format) of a sensor driving through ONE street-canyon scene at `speed` m/s, its yaw rate
+    weaving as yaw_rate * cos(2 pi t / weave_period) rad/s; every firing is cast from the sensor's pose at its own time, so each sweep
+    carries the motion that happens during it.  Returns dict(sweeps: list of (n, 4) float32, poses (K, 7): t(x,y,z), q(w,x,y,z) of
+    the sensor at the start of each sweep in the frame of the first, stamps / gyro (m, 3): IMU samples at imu_rate over the whole
+    drive, t_scan_next (K,): end time of each sweep, t0)."""
+    rng = np.random.default_rng(seed)
+    path = speed * K * sweep_time
+    sc = Scene(-60.0, path + 60.0, rng, n_boxes=int(round(30 * (path + 120.0) / 140.0)))
+    origin0 = np.array([0.3, -0.4, 0.2])
+    # yaw and position on a 1 ms grid (trapezoidal integration), interpolated at the firing times
+    dt = 1e-3
+    tg = np.arange(0.0, K * sweep_time + 2 * dt, dt)
+    w = 2 * np.pi / weave_period
+    yawg = yaw_rate * np.sin(w * tg) / w
+    vx, vy = speed * np.cos(yawg), speed * np.sin(yawg)
+    xg = np.concatenate([[0.0], np.cumsum(0.5 * (vx[1:] + vx[:-1]) * dt)])
+    yg = np.concatenate([[0.0], np.cumsum(0.5 * (vy[1:] + vy[:-1]) * dt)])
+
+    def state(t):
+        return np.interp(t, tg, xg), np.interp(t, tg, yg), yaw_rate * np.sin(w * t) / w
+
+    elev = np.deg2rad(raw_elevations(n_rings))
+    L = len(elev)
+    order = (np.arange(L) * 11) % L
+    # rectangles that can give a return within 80 m of some point of the sweep (the others cannot change the nearest hit)
+    x_lo_r = np.minimum(sc.o[:, 0], sc.o[:, 0] + sc.u[:, 0] + sc.v[:, 0]); x_hi_r = np.maximum(sc.o[:, 0], sc.o[:, 0] + sc.u[:, 0] + sc.v[:, 0])
+    sweeps, poses = [], np.zeros((K, 7))
+    for k in range(K):
+        kk = np.repeat(np.arange(n_az), L)
+        tf = (k + kk / n_az) * sweep_time
+        x, y, psi = state(tf)
+        origin = np.stack([origin0[0] + x, origin0[1] + y, np.full(len(x), origin0[2])], 1)
+        az = 0.3 - (2 * np.pi - 0.02) * kk / n_az
+        xs, _, _ = state(np.array([k * sweep_time, (k + 1) * sweep_time]))
+        rects = np.nonzero((x_hi_r > xs.min() + origin0[0] - 81.0) & (x_lo_r < xs.max() + origin0[0] + 81.0))[0]
+        sweeps.append(_cast_firings(sc, origin, elev[np.tile(order, n_az)], az, psi, rng, noise, 0.0, nan_frac, 0, rects))
+        xk, yk, pk = state(k * sweep_time)
+        poses[k, :3] = [xk, yk, 0.0]
+        poses[k, 3:] = [np.cos(pk / 2), 0.0, 0.0, np.sin(pk / 2)]
+    stamps = t0 - 0.05 + np.arange(int((K * sweep_time + 0.1) * imu_rate) + 1) / imu_rate
+    gyro = np.zeros((len(stamps), 3)); gyro[:, 2] = yaw_rate * np.cos(w * (stamps - t0))
+    return dict(sweeps=sweeps, poses=poses, stamps=stamps, gyro=gyro, t_scan_next=t0 + (np.arange(K) + 1) * sweep_time, t0=t0)
 
 
 def ring_scan(n_rings=32, n_az=1500, seed=SEED0 + 11, fov=(-25.0, 15.0), noise=0.01, drop=0.02):

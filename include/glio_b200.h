@@ -84,7 +84,7 @@ int64_t glio_launch_count(const glio_ctx* ctx);
  * | k_knn_box_cells [7], k_plane_fit, k_plane_fit_pair, k_flags, k_compact;
  * K2 k_eval_unary, k_eval_unary_cost, k_eval_binary, k_eval_binary_cost, k_bin_assemble; local map k_lm_transform, k_vox_*;
  * front end k_feat_curvature, k_feat_select, k_feat_voxel, k_feat_offsets, k_feat_gather; sweep preparation k_sp_bounds,
- * k_sp_consts, k_sp_classify, k_sp_ranges, k_sp_emit). */
+ * k_sp_consts, k_sp_classify, k_sp_ranges, k_sp_emit; odometry k_odom_publish). */
 int glio_profile_enable(glio_ctx* ctx, int on);
 int glio_profile_get(glio_ctx* ctx, const char* kernel_name, double* ms_total, int64_t* launches);
 /* statistics: number of queries a first search pass handed to its second pass (GLIO_KNN_MODE 0 and 4; 0 in the default mode) */
@@ -310,6 +310,65 @@ typedef struct {
 int glio_imu_sweep_rotation(glio_imu_state* st, const double* stamps, const double* gyro_xyz, int64_t n_buf, double t_scan_next,
                             double q_wxyz[4]);
 
+/* ---- front-end LiDAR odometry (SURVEY 8 f-6): the LidarOdometry node, GLIO/src/LidarOdometry.cpp:661-695 (run) and what it calls.
+ * One glio_odom_step per sweep takes that sweep's surf features (`/surf_features`, the less_flat_ds of glio_extract_features) and
+ * optionally its full cloud (`/lidar_cloud_cutted`, the output of glio_prepare_scan), both packed float4 x,y,z,intensity, and runs
+ *   sweep 1      savePoses of the identity pose and an EMPTY scan frame, clouds published unchanged, no odometry (checkInitialization);
+ *   later sweeps poseInitialization (:406-433); the local map (:267-288): on sweep 2 the sweep's own surf cloud, afterwards the last
+ *                20 sweeps' VoxelGrid(0.2)-filtered surf clouds moved to the world frame by their final poses, concatenated oldest
+ *                first; VoxelGrid(0.2) of the map and of the surf cloud (:305-313; PCL's pass-through on voxel-index overflow
+ *                included); fewer than 10 map points: stop here, the pose stays the prediction and the keyframe flag keeps its
+ *                previous value (:477-480); otherwise scan_match_cnt rounds (8 on sweep 2) of association (findCorrespondingSurfFeatures,
+ *                :343-404: squared radius 1.0, plane 0.06, weight 0.4) + a fresh Levenberg-Marquardt solve (HuberLoss(0.1),
+ *                LidarPlaneNormIncreFactor; a round without matches leaves the pose as it is, like Ceres with no residual) +
+ *                unifyQuaternion; the keyframe rule (:566-578); savePoses; computeRelative (:435-471); on a keyframe the
+ *                clouds are published, translation de-skewed by the relative pose when deskew != 0 (publishCloudLast, :619-659).
+ * The odometry runs on its context's device, stream, launch counter and profiler but owns all its state: it never reads or
+ * changes the context's glio_params, map, local map, window slots or batch frames, so one context can run
+ * prepare -> extract -> odometry and the window path side by side.  glio_destroy frees odometries still attached to the context. */
+typedef struct {
+  int32_t max_num_iter;       /* lidar_odometry/max_num_iter: 12 (GLIO/config/config_urban_hk.yaml:19; code default 15) */
+  int32_t scan_match_cnt;     /* 1 (:20); the second sweep always runs 8 rounds (LidarOdometry.cpp:493-496); at most 8 */
+  int32_t deskew;             /* if_to_deskew: 0 (:21; code default 1) */
+  int32_t reserved;
+  double max_solver_time_s;   /* max_solver_time_in_seconds 0.015 (LidarOdometry.cpp:524): wall clock, checked after every iteration */
+} glio_odom_options;
+void glio_odom_default_options(glio_odom_options* o);   /* the shipped configuration above */
+
+enum { GLIO_ODOM_MAX_ROUNDS = 8 };
+typedef struct {
+  double pose[7];             /* /odom: t(x,y,z), q(w,x,y,z) - the reference's abs_pose is q(w,x,y,z), t(x,y,z) */
+  double rel_pose[7];         /* /each_odom, the pose relative to the previous sweep, t then q (reference rel_pose: q then t) */
+  int32_t initialised;        /* 1 on the first sweep after creation / reset: clouds passed through, no odometry */
+  int32_t keyframe;           /* kf: the clouds were published (always 0 on the first sweep) */
+  int32_t skipped;            /* the filtered map had fewer than 10 points: no round ran */
+  int32_t n_rounds;
+  int64_t n_map, n_scan;      /* points of the filtered map and of the filtered scan */
+  int64_t round_n_match[GLIO_ODOM_MAX_ROUNDS];
+  int32_t round_iterations[GLIO_ODOM_MAX_ROUNDS];    /* LM iteration records (iteration 0 included); 0 for a round without matches */
+  int32_t round_successful[GLIO_ODOM_MAX_ROUNDS];    /* successful steps */
+  int32_t round_termination[GLIO_ODOM_MAX_ROUNDS];   /* glio_solver_summary.termination */
+  int32_t reserved;
+  double round_pose[GLIO_ODOM_MAX_ROUNDS][7];        /* pose after each round (t, q), after unifyQuaternion */
+  glio_solver_summary summary;                       /* the last round's solve */
+} glio_odom_report;
+
+typedef struct glio_odom glio_odom;
+int glio_odom_create(glio_ctx* ctx, const glio_odom_options* options /* NULL: defaults */, glio_odom** out);
+void glio_odom_destroy(glio_odom* od);
+int glio_odom_reset(glio_odom* od);   /* back to the state before the first sweep (buffers are kept) */
+/* surf_xyzi[n_surf] / full_xyzi[n_full] (full may be NULL with n_full = 0) are host or device memory as surf_mem / full_mem say;
+ * surf_out / full_out (each as large as its input, either may be NULL) are written only when the node publishes: on the first
+ * sweep and on keyframes.  Device pointers must be 16-byte aligned memory of the context's GPU (the clouds are read and written
+ * as float4); a bad argument is GLIO_ERR_ARG before anything runs.  An empty surf cloud is allowed (nothing matches).
+ * The call returns when its work is complete. */
+int glio_odom_step(glio_odom* od, const float* surf_xyzi, int64_t n_surf, int surf_mem, const float* full_xyzi, int64_t n_full, int full_mem,
+                   float* surf_out, float* full_out, int out_mem, glio_odom_report* rep);
+/* debug copy-out of the last step's filtered map (surf_from_map_ds, x,y,z in the filter's output order) and filtered scan
+ * (surf_last_ds); either pointer may be NULL; the counts are always written.  Fails with GLIO_ERR_ARG if a capacity is too small. */
+int glio_odom_get_clouds(glio_odom* od, int64_t map_capacity, float* map_xyz, int64_t* n_map, int64_t scan_capacity, float* scan_xyz,
+                         int64_t* n_scan);
+
 /* ---- K3: marginalisation of the oldest keyframe (MarginalizationInfo, GLIO/src/MarginalizationFactor.cpp:82-202; call site
  * Estimator.cpp:2462-2608).  The reference re-evaluates EVERY LiDAR factor of the window (:2538-2576, one virtual Evaluate per
  * residual) plus the IMU factor KF0->KF1 and the previous prior, accumulates the dense A = J^T J, b = J^T r with the ambient
@@ -328,7 +387,7 @@ int glio_window_marginalize(glio_ctx* ctx, int W, const double* poses, const dou
  * association to the GPU meanwhile (the reference does these strictly one after the other, Estimator.cpp:2462-2608 then the next
  * processImage).  One job at a time per context.  glio_marg_job_wait joins the job, frees it and returns the prior (identical to
  * glio_window_marginalize's); call it before the next solve needs the prior.  glio_destroy joins AND frees an abandoned job: a job
- * handle must not be used after its context is gone.  A context is otherwise single-threaded: calls on one context must not
+ * handle must not be used after its context is gone (the same holds for a glio_odom, which glio_destroy also frees).  A context is otherwise single-threaded: calls on one context must not
  * overlap, the worker is the library's own. */
 typedef struct glio_marg_job glio_marg_job;
 int glio_window_marginalize_async(glio_ctx* ctx, int W, const double* poses, const double* speed_bias, glio_host_marg_fn host_marg,
