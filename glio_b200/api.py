@@ -830,3 +830,179 @@ class Odometry:
 
 
 Context.KERNELS = Context.KERNELS + ["k_odom_publish"]
+
+
+# ---------------------------------------------------------------------------------------------------------------------------
+# loop-closure registration (detectLoopClosure / performLoopClosure, GLIO/src/Estimator.cpp:5101-5273, without the GTSAM half)
+# ---------------------------------------------------------------------------------------------------------------------------
+ICP_NOT_CONVERGED, ICP_ITERATIONS, ICP_TRANSFORM, ICP_ABS_MSE, ICP_REL_MSE, ICP_NO_CORRESPONDENCES = range(6)
+
+
+class IcpOptions(C.Structure):
+    _fields_ = [("max_iterations", C.c_int32), ("reserved", C.c_int32), ("max_correspondence_distance", C.c_double),
+                ("transformation_epsilon", C.c_double), ("euclidean_fitness_epsilon", C.c_double)]
+
+
+class IcpIteration(C.Structure):
+    _fields_ = [("transformation", C.c_float * 16), ("n_corr", C.c_int64), ("mse", C.c_double)]
+
+
+class IcpResult(C.Structure):
+    _fields_ = [("converged", C.c_int32), ("state", C.c_int32), ("iterations", C.c_int32), ("host_syncs", C.c_int32),
+                ("n_source", C.c_int64), ("n_target", C.c_int64), ("n_corr", C.c_int64), ("launches", C.c_int64),
+                ("final_transformation", C.c_float * 16), ("fitness", C.c_double)]
+
+
+class LoopOptions(C.Structure):
+    _fields_ = [("lc_search_radius", C.c_double), ("lc_time_thres", C.c_double), ("lc_map_width", C.c_int32), ("lc_icp_thres", C.c_float),
+                ("slide_window_width", C.c_int32), ("leaf", C.c_float), ("q_lb", C.c_double * 4), ("t_lb", C.c_double * 3),
+                ("icp", IcpOptions)]
+
+
+class LoopReport(C.Structure):
+    _fields_ = [("detected", C.c_int32), ("closest_his_idx", C.c_int32), ("latest_frame_idx", C.c_int32), ("accepted", C.c_int32),
+                ("n_latest", C.c_int64), ("n_latest_ds", C.c_int64), ("n_his", C.c_int64), ("n_his_ds", C.c_int64),
+                ("n_candidates", C.c_int64), ("icp", IcpResult), ("pose_from", C.c_double * 7), ("pose_to", C.c_double * 7),
+                ("noise_score", C.c_double), ("time_last_loop", C.c_double)]
+
+
+_ICP_KEYS = ("max_iterations", "max_correspondence_distance", "transformation_epsilon", "euclidean_fitness_epsilon")
+
+
+def default_icp_options(**kw):
+    o = IcpOptions()
+    lib().glio_icp_default_options(C.byref(o))
+    for k, v in kw.items():
+        setattr(o, k, v)
+    return o
+
+
+def default_loop_options(**kw):
+    """glio_loop_default_options (the shipped configuration); the ICP settings may be given by name as well."""
+    o = LoopOptions()
+    lib().glio_loop_default_options(C.byref(o))
+    for k, v in kw.items():
+        if k in ("q_lb", "t_lb"):
+            arr = getattr(o, k)
+            for i, x in enumerate(v):
+                arr[i] = float(x)
+        elif k in _ICP_KEYS:
+            setattr(o.icp, k, v)
+        else:
+            setattr(o, k, v)
+    return o
+
+
+def _icp_dict(r):
+    return dict(converged=bool(r.converged), state=int(r.state), iterations=int(r.iterations), host_syncs=int(r.host_syncs),
+                n_source=int(r.n_source), n_target=int(r.n_target), n_corr=int(r.n_corr), launches=int(r.launches),
+                final=np.array(r.final_transformation[:], np.float32).reshape(4, 4), fitness=float(r.fitness))
+
+
+def _icp_align(self, src, tgt, iter_log=True, correspondences=False, aligned=True, **options):
+    """pcl::IterativeClosestPoint::align (identity guess) + getFitnessScore on the device.  src / tgt: (n, stride) float32 numpy arrays or
+    CUDA tensors with x, y, z in columns 0..2.  options: the glio_icp_options fields (default: the Estimator's settings).  Returns
+    the result dict (converged, state, iterations, host_syncs, n_corr, launches, final (4x4), fitness) plus aligned (n, 3), log (list of
+    (transformation, n_corr, mse)) and corr ((query, match, dist) of the last correspondence estimation) when asked for."""
+    opt = default_icp_options(**options)
+    ks, ps, ns, ss, ms = _points_arg(src) if _npts(src) else (None, None, 0, 3, HOST)
+    kt, pt, nt, st, mt = _points_arg(tgt) if _npts(tgt) else (None, None, 0, 3, HOST)
+    al = np.empty((ns, 3), np.float32) if aligned else None
+    cap = opt.max_iterations if iter_log else 0
+    log = (IcpIteration * max(cap, 1))()
+    cq = cm = cd = None
+    if correspondences:
+        cq = np.empty(max(ns, 1), np.int32); cm = np.empty(max(ns, 1), np.int32); cd = np.empty(max(ns, 1), np.float32)
+    res = IcpResult()
+    self._chk(self._lib.glio_icp_align(self._h, ps, C.c_int64(ns), C.c_int(ss), C.c_int(ms), pt, C.c_int64(nt), C.c_int(st), C.c_int(mt),
+                                       C.byref(opt), _ptr(al), C.byref(res), log if cap else None, C.c_int(cap), _ptr(cq), _ptr(cm), _ptr(cd),
+                                       C.c_int64(ns if correspondences else 0)))
+    out = _icp_dict(res)
+    if aligned:
+        out["aligned"] = al
+    if iter_log:
+        k = min(res.iterations, cap)
+        out["log"] = [(np.array(log[i].transformation[:], np.float32).reshape(4, 4), int(log[i].n_corr), float(log[i].mse)) for i in range(k)]
+    if correspondences:
+        nc = int(res.n_corr)
+        out["corr"] = (cq[:nc].copy(), cm[:nc].copy(), cd[:nc].copy())
+    return out
+
+
+def _npts(a):
+    return a is not None and (a.shape[0] if hasattr(a, "shape") else len(a)) > 0
+
+
+Context.icp_align = _icp_align
+
+
+class LoopClosure:
+    """The Estimator's loop-closure keyframe store and its detection + registration step on the device (see glio_loop_step in
+    include/glio_b200.h).  Keyframe clouds stay resident on the context's GPU; the state is the object's own."""
+
+    def __init__(self, ctx, **options):
+        self.ctx = ctx
+        self._lib = ctx._lib
+        self.options = default_loop_options(**options)
+        self._h = C.c_void_p()
+        ctx._chk(self._lib.glio_loop_create(ctx._h, C.byref(self.options), C.byref(self._h)))
+
+    def close(self):
+        if getattr(self, "_h", None) and self.ctx._h:      # a closed context has already freed its loop objects
+            self._lib.glio_loop_destroy(self._h)
+        self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def reset(self):
+        self.ctx._chk(self._lib.glio_loop_reset(self._h))
+
+    def __len__(self):
+        n = C.c_int(0)
+        self.ctx._chk(self._lib.glio_loop_size(self._h, C.byref(n)))
+        return int(n.value)
+
+    def add_keyframe(self, cloud, pose, time):
+        """cloud: (n, stride) float32 numpy array or CUDA tensor, lidar frame (surf_last_ds); pose: body pose t, q; returns its index."""
+        if _npts(cloud):
+            keep, p, n, stride, mem = _points_arg(cloud)
+        else:
+            p, n, stride, mem = None, 0, 3, HOST
+        ps = np.ascontiguousarray(pose, np.float64)
+        idx = C.c_int32(0)
+        self.ctx._chk(self._lib.glio_loop_add_keyframe(self._h, p, C.c_int64(n), C.c_int(stride), C.c_int(mem), _ptr(ps), C.c_double(time),
+                                                       C.byref(idx)))
+        return int(idx.value)
+
+    def set_poses(self, first, poses):
+        ps = np.ascontiguousarray(poses, np.float64).reshape(-1, 7)
+        self.ctx._chk(self._lib.glio_loop_set_poses(self._h, C.c_int(first), C.c_int(len(ps)), _ptr(ps)))
+
+    def step(self, select_xyz, time_new_odom):
+        """Returns dict(detected, closest_his_idx, latest_frame_idx, accepted, n_latest, n_latest_ds, n_his, n_his_ds, n_candidates,
+        icp (result dict, None when nothing ran), pose_from / pose_to (t, q; None unless accepted), noise_score, time_last_loop)."""
+        s = np.ascontiguousarray(select_xyz, np.float32)
+        rep = LoopReport()
+        self.ctx._chk(self._lib.glio_loop_step(self._h, _ptr(s), C.c_double(time_new_odom), C.byref(rep)))
+        acc = bool(rep.accepted)
+        return dict(detected=bool(rep.detected), closest_his_idx=int(rep.closest_his_idx), latest_frame_idx=int(rep.latest_frame_idx),
+                    accepted=acc, n_latest=int(rep.n_latest), n_latest_ds=int(rep.n_latest_ds), n_his=int(rep.n_his), n_his_ds=int(rep.n_his_ds),
+                    n_candidates=int(rep.n_candidates), icp=_icp_dict(rep.icp) if rep.detected else None,
+                    pose_from=np.array(rep.pose_from[:]) if acc else None, pose_to=np.array(rep.pose_to[:]) if acc else None,
+                    noise_score=float(rep.noise_score) if acc else None, time_last_loop=float(rep.time_last_loop))
+
+    def clouds(self):
+        """The last registration's filtered latest and history clouds, (n, 3) float32 each (debug copy-out)."""
+        nl = C.c_int64(0); nh = C.c_int64(0)
+        self.ctx._chk(self._lib.glio_loop_get_clouds(self._h, C.c_int64(0), None, C.byref(nl), C.c_int64(0), None, C.byref(nh)))
+        a = np.empty((nl.value, 3), np.float32); b = np.empty((nh.value, 3), np.float32)
+        self.ctx._chk(self._lib.glio_loop_get_clouds(self._h, C.c_int64(nl.value), _ptr(a), C.byref(nl), C.c_int64(nh.value), _ptr(b), C.byref(nh)))
+        return a, b
+
+
+Context.KERNELS = Context.KERNELS + ["k_lc_load", "k_lc_qhist", "k_lc_qscatter", "k_lc_init", "k_lc_nn", "k_lc_compact", "k_lc_sum0",
+                                     "k_lc_sum1", "k_lc_means", "k_lc_solve", "k_lc_transform", "k_lc_final", "k_lc_fitness"]

@@ -1,6 +1,7 @@
 // capi.cu — the extern "C" boundary (include/glio_b200.h) and the context that owns device state.
 // No CPU fallback: without a CUDA device glio_create fails.
 #include <array>
+#include <cfloat>
 #include <atomic>
 #include <condition_variable>
 #include <mutex>
@@ -153,7 +154,10 @@ struct glio_ctx {
   DevBuf<float> lm_stage; int64_t map_n = 0;
   // front-end odometries created on this context (glio_odom_create); glio_destroy frees those still attached
   std::vector<glio_odom*> odoms;
-  cudaStream_t st_copy = nullptr;       // window scans travel on their own stream so the upload of the next window can overlap a running solve
+  // loop-closure registration: glio_icp_align's work space and staging, and the loop objects created on this context
+  IcpWork icp; DevBuf<float> icp_src, icp_tgt;
+  std::vector<glio_loop*> loops;
+  cudaStream_t st_copy = nullptr;      // window scans travel on their own stream so the upload of the next window can overlap a running solve
   cudaEvent_t ev_scans = nullptr, ev_main = nullptr;
   bool scans_pending = false;
   PinnedBuf<unsigned int> h_flag;      // completion epoch written by the last block of k_eval_unary
@@ -498,6 +502,7 @@ void glio_destroy(glio_ctx* c) {
   if (!c) return;
   cudaSetDevice(c->device);
   while (!c->odoms.empty()) glio_odom_destroy(c->odoms.back());   // an odometry still attached (it detaches itself)
+  while (!c->loops.empty()) glio_loop_destroy(c->loops.back());   // likewise a loop object
   if (c->marg_thread.joinable()) {
     if (c->marg_pending) { glio_marg_prior* dropped = nullptr; glio_marg_job_wait(c->marg_pending, &dropped); if (dropped) glio_marg_prior_destroy(dropped); }
     { std::lock_guard<std::mutex> lk(c->marg_mu); c->marg_quit = true; }
@@ -523,6 +528,7 @@ void glio_destroy(glio_ctx* c) {
   c->sp_raw.release(); c->sp_ori.release(); c->sp_ring.release(); c->sp_hist.release(); c->sp_hscan.release(); c->sp_small.release();
   c->sp_scan_tmp.release(); c->sp_consts.release(); c->sp_out.release(); c->sp_hits.release();
   c->e_items.release(); c->e_start.release(); c->e_part.release(); c->e_out.release(); c->e_poses.release();
+  c->icp.release(); c->icp_src.release(); c->icp_tgt.release();
   for (auto& r : c->lc.recs) { cudaEventDestroy(r.a); cudaEventDestroy(r.b); }
   for (auto& e : c->lc.pool) cudaEventDestroy(e);
   c->lc.recs.clear(); c->lc.pool.clear();
@@ -2033,6 +2039,303 @@ int glio_odom_get_clouds(glio_odom* o, int64_t map_capacity, float* map_xyz, int
     };
     fetch(o->map_pts, o->map_stride, nm, map_xyz);
     fetch(o->last_ds.p, o->last_ds_stride, ns, scan_xyz);
+  });
+}
+
+}  // extern "C"
+
+// ------------------------------------------------------------------------------------------------------------
+// loop-closure registration (SURVEY 8 f-7): detectLoopClosure / performLoopClosure, GLIO/src/Estimator.cpp:5101-5273
+// ------------------------------------------------------------------------------------------------------------
+struct glio_loop {
+  glio_ctx* ctx = nullptr;
+  glio_loop_options opt{};
+  double q_bl[4], t_bl[3];
+  struct Keyframe {
+    DevBuf<float> xyz;                  // surf_frames[k], packed x,y,z (lidar frame)
+    int64_t n = 0;
+    double pose[7];                     // pose_info_keyframe[k]: t, q
+    double time = 0.0;
+    float pos[3];                       // pose_keyframe[k]
+  };
+  std::vector<std::unique_ptr<Keyframe>> kfs;
+  double time_last_loop = 0.0;
+  LocalMap latest, his;                 // latest_key_frames / his_key_frames and ds_filter_his_frames
+  const float* lat_pts = nullptr; int lat_stride = 3; int64_t lat_n = 0;
+  const float* his_pts = nullptr; int his_stride = 3; int64_t his_n = 0;
+  IcpWork icp;
+  void release() {
+    for (auto& k : kfs) k->xyz.release();
+    kfs.clear(); latest.release(); his.release(); icp.release();
+  }
+};
+
+namespace {
+
+// the concatenation of the given keyframes moved to the world frame, filtered: returns the filtered size, *n_raw the concatenated one
+int64_t loop_cloud(glio_loop* L, LocalMap& lm, const std::vector<int>& ids, int64_t* n_raw, const float** pts, int* stride) {
+  glio_ctx* c = L->ctx;
+  while (!lm.frames.empty()) lm.pop_front();
+  for (int k : ids) {
+    const glio_loop::Keyframe& kf = *L->kfs[k];
+    double t[3], q[4];
+    loop_world_of_cloud(kf.pose, L->q_bl, L->t_bl, t, q);
+    lm.push(false, kf.xyz.p, 3, kf.n, t, q, c->st, c->lc);               // *cloud += *transformCloud(surf_frames[k], q_tmp, t_tmp)
+  }
+  *n_raw = lm.n_points();
+  bool filtered = false;
+  return lm.build(L->opt.leaf, pts, stride, &filtered, c->st, c->lc);     // ds_filter_his_frames.filter
+}
+
+void fill_icp_result(const IcpState& h, int64_t n_src, int64_t n_tgt, int syncs, int64_t launches, glio_icp_result* r) {
+  memset(r, 0, sizeof(*r));
+  r->converged = h.converged; r->state = h.state; r->iterations = h.nr_iter; r->host_syncs = syncs;
+  r->n_source = n_src; r->n_target = n_tgt; r->n_corr = h.n_corr; r->launches = launches;
+  for (int k = 0; k < 16; ++k) r->final_transformation[k] = h.final_T[k];
+  r->fitness = h.fitness;
+}
+
+void loop_step(glio_loop* L, const float sel[3], double time_new_odom, glio_loop_report* rep) {
+  glio_ctx* c = L->ctx;
+  glio_loop_report R;
+  memset(&R, 0, sizeof(R));
+  R.closest_his_idx = -1; R.latest_frame_idx = -1;
+  R.icp.fitness = DBL_MAX;
+  const int K = (int)L->kfs.size();
+  if (K > 0) {                                                               // performLoopClosure: pose_keyframe->points.empty()
+    // kd_tree_his_key_poses->radiusSearch(select_pose, lc_search_radius, ...): FLANN's float L2_Simple distance, kept when below
+    // float(radius^2), sorted by (distance, index)
+    const float r2 = (float)(L->opt.lc_search_radius * L->opt.lc_search_radius);
+    std::vector<std::pair<float, int>> hits;
+    for (int k = 0; k < K; ++k) {
+      const float* p = L->kfs[k]->pos;
+      const float d0 = sel[0] - p[0], d1 = sel[1] - p[1], d2 = sel[2] - p[2];
+      float d = 0.f; d = d + d0 * d0; d = d + d1 * d1; d = d + d2 * d2;
+      if (d < r2) hits.emplace_back(d, k);
+    }
+    std::sort(hits.begin(), hits.end());
+    R.n_candidates = (int64_t)hits.size();
+    for (auto& h : hits)
+      if (std::abs(L->kfs[h.second]->time - time_new_odom) > L->opt.lc_time_thres) { R.closest_his_idx = h.second; break; }
+    if (R.closest_his_idx >= 0 && !(std::abs(L->time_last_loop - time_new_odom) < 0.2)) {
+      R.detected = 1;
+      const int latest = K - L->opt.slide_window_width;
+      R.latest_frame_idx = latest;
+      std::vector<int> ids;
+      for (int j = 0; j < 6; ++j) if (latest - j >= 0) ids.push_back(latest - j);
+      L->lat_n = loop_cloud(L, L->latest, ids, &R.n_latest, &L->lat_pts, &L->lat_stride);
+      ids.clear();
+      for (int j = -L->opt.lc_map_width; j <= L->opt.lc_map_width; ++j) {
+        const int k = R.closest_his_idx + j;
+        if (k < 0 || k > latest) continue;
+        ids.push_back(k);
+      }
+      L->his_n = loop_cloud(L, L->his, ids, &R.n_his, &L->his_pts, &L->his_stride);
+      R.n_latest_ds = L->lat_n; R.n_his_ds = L->his_n;
+      // pcl::IterativeClosestPoint: source latest_key_frames_ds, target his_key_frames_ds, identity guess; then getFitnessScore
+      const int64_t l0 = c->lc.n;
+      IcpState h; int syncs = 0;
+      icp_run(L->icp, L->lat_pts, L->lat_stride, L->lat_n, L->his_pts, L->his_stride, L->his_n, L->opt.icp, 0, c->pts_per_cell, c->st, c->lc, &h, &syncs);
+      fill_icp_result(h, L->lat_n, L->his_n, syncs, c->lc.n - l0, &R.icp);
+      if (h.converged && !(h.fitness > (double)L->opt.lc_icp_thres)) {
+        R.accepted = 1;
+        loop_pose_from(h.final_T, L->kfs[latest]->pose, R.pose_from);
+        for (int k = 0; k < 7; ++k) R.pose_to[k] = L->kfs[R.closest_his_idx]->pose[k];
+        R.noise_score = h.fitness;
+        L->time_last_loop = L->kfs[latest]->time;
+      }
+    }
+  }
+  R.time_last_loop = L->time_last_loop;
+  if (rep) *rep = R;
+}
+
+bool dev_ptr_ok(const glio_ctx* c, const void* p, uintptr_t align) { return on_ctx_device(c, p) && ((uintptr_t)p & (align - 1)) == 0; }
+
+}  // namespace
+
+extern "C" {
+
+void glio_icp_default_options(glio_icp_options* o) {
+  if (!o) return;
+  memset(o, 0, sizeof(*o));
+  o->max_iterations = 100; o->max_correspondence_distance = 30.0; o->transformation_epsilon = 1e-6; o->euclidean_fitness_epsilon = 1e-6;
+}
+
+static void check_icp_options(const glio_icp_options& o) {
+  GLIO_REQUIRE(o.max_iterations >= 1 && o.max_iterations <= 100000 && o.max_correspondence_distance > 0.0 &&
+               std::isfinite(o.max_correspondence_distance) && o.transformation_epsilon >= 0.0 && o.euclidean_fitness_epsilon >= 0.0,
+               GLIO_ERR_ARG, "icp options: need 1 <= max_iterations <= 100000, a finite positive correspondence distance, epsilons >= 0");
+}
+
+int glio_icp_align(glio_ctx* c, const float* src, int64_t n_src, int src_stride, int src_mem, const float* tgt, int64_t n_tgt, int tgt_stride,
+                   int tgt_mem, const glio_icp_options* options, float* aligned_xyz, glio_icp_result* res, glio_icp_iteration* iter_log,
+                   int iter_cap, int32_t* corr_query, int32_t* corr_match, float* corr_dist, int64_t corr_cap) {
+  if (!c) return GLIO_ERR_ARG;
+  return guarded(c, [&] {
+    glio_icp_options o; if (options) o = *options; else glio_icp_default_options(&o);
+    check_icp_options(o);
+    const int64_t kMax = (int64_t)1 << 30;
+    GLIO_REQUIRE(n_src >= 0 && n_src < kMax && (src || n_src == 0) && n_tgt >= 0 && n_tgt < kMax && (tgt || n_tgt == 0), GLIO_ERR_ARG,
+                 "glio_icp_align: bad cloud pointer or size");
+    GLIO_REQUIRE(src_stride >= 3 && src_stride <= 64 && tgt_stride >= 3 && tgt_stride <= 64, GLIO_ERR_ARG, "glio_icp_align: stride_floats must be in [3,64]");
+    GLIO_REQUIRE((src_mem == GLIO_HOST || src_mem == GLIO_DEVICE) && (tgt_mem == GLIO_HOST || tgt_mem == GLIO_DEVICE), GLIO_ERR_ARG,
+                 "glio_icp_align: mem must be GLIO_HOST or GLIO_DEVICE");
+    GLIO_REQUIRE((src_mem != GLIO_DEVICE || n_src == 0 || dev_ptr_ok(c, src, 4)) && (tgt_mem != GLIO_DEVICE || n_tgt == 0 || dev_ptr_ok(c, tgt, 4)),
+                 GLIO_ERR_ARG, "glio_icp_align: a GLIO_DEVICE cloud must be 4-byte aligned memory of the context's GPU");
+    GLIO_REQUIRE(iter_cap >= 0 && (iter_log || iter_cap == 0) && corr_cap >= 0, GLIO_ERR_ARG, "glio_icp_align: bad log capacities");
+    const float* ds = src; const float* dt = tgt;
+    if (n_src && src_mem != GLIO_DEVICE) ds = stage_points(c, c->icp_src, src, n_src, src_stride, src_mem);
+    if (n_tgt && tgt_mem != GLIO_DEVICE) dt = stage_points(c, c->icp_tgt, tgt, n_tgt, tgt_stride, tgt_mem);
+    const int64_t l0 = c->lc.n;
+    IcpState h; int syncs = 0;
+    icp_run(c->icp, ds, src_stride, n_src, dt, tgt_stride, n_tgt, o, iter_cap, c->pts_per_cell, c->st, c->lc, &h, &syncs);
+    if (res) fill_icp_result(h, n_src, n_tgt, syncs, c->lc.n - l0, res);
+    if (aligned_xyz && n_src > 0) {
+      std::vector<float4> a((size_t)n_src);
+      GLIO_CUDA_TRY(cudaMemcpyAsync(a.data(), c->icp.fit.p, (size_t)n_src * sizeof(float4), cudaMemcpyDeviceToHost, c->st));
+      GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
+      for (int64_t i = 0; i < n_src; ++i) { aligned_xyz[3 * i] = a[i].x; aligned_xyz[3 * i + 1] = a[i].y; aligned_xyz[3 * i + 2] = a[i].z; }
+    }
+    const int nlog = std::min(iter_cap, h.nr_iter);
+    if (iter_log && nlog > 0) {
+      GLIO_CUDA_TRY(cudaMemcpyAsync(iter_log, c->icp.log.p, (size_t)nlog * sizeof(glio_icp_iteration), cudaMemcpyDeviceToHost, c->st));
+      GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
+    }
+    const int64_t nc = std::min<int64_t>(corr_cap, h.n_corr);
+    if (nc > 0 && n_src > 0 && n_tgt > 0) {
+      if (corr_query) GLIO_CUDA_TRY(cudaMemcpyAsync(corr_query, c->icp.cq.p, (size_t)nc * sizeof(int32_t), cudaMemcpyDeviceToHost, c->st));
+      if (corr_match) GLIO_CUDA_TRY(cudaMemcpyAsync(corr_match, c->icp.cm.p, (size_t)nc * sizeof(int32_t), cudaMemcpyDeviceToHost, c->st));
+      if (corr_dist) GLIO_CUDA_TRY(cudaMemcpyAsync(corr_dist, c->icp.cd.p, (size_t)nc * sizeof(float), cudaMemcpyDeviceToHost, c->st));
+      GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
+    }
+  });
+}
+
+void glio_loop_default_options(glio_loop_options* o) {
+  if (!o) return;
+  memset(o, 0, sizeof(*o));
+  o->lc_search_radius = 25.0; o->lc_time_thres = 30.0; o->lc_map_width = 25; o->lc_icp_thres = 0.2f;   // config_urban_hk.yaml:80-83
+  o->slide_window_width = 5; o->leaf = 0.4f;
+  o->q_lb[0] = 1.0; o->t_lb[2] = 0.28;                                                                  // :90-97
+  glio_icp_default_options(&o->icp);
+}
+
+int glio_loop_create(glio_ctx* c, const glio_loop_options* options, glio_loop** out) {
+  if (!c || !out) return GLIO_ERR_ARG;
+  *out = nullptr;
+  return guarded(c, [&] {
+    glio_loop_options opt; if (options) opt = *options; else glio_loop_default_options(&opt);
+    check_icp_options(opt.icp);
+    GLIO_REQUIRE(opt.lc_search_radius > 0.0 && std::isfinite(opt.lc_search_radius) && opt.lc_time_thres >= 0.0 && opt.lc_map_width >= 0 &&
+                 opt.lc_map_width <= 100000 && opt.slide_window_width >= 1 && opt.leaf > 0.f && std::isfinite(opt.lc_icp_thres),
+                 GLIO_ERR_ARG, "glio_loop_create: need lc_search_radius > 0, lc_time_thres >= 0, lc_map_width >= 0, slide_window_width >= 1, leaf > 0");
+    const double n2 = opt.q_lb[0] * opt.q_lb[0] + opt.q_lb[1] * opt.q_lb[1] + opt.q_lb[2] * opt.q_lb[2] + opt.q_lb[3] * opt.q_lb[3];
+    GLIO_REQUIRE(n2 > 0.0 && std::isfinite(n2), GLIO_ERR_ARG, "glio_loop_create: q_lb must be a non-zero finite quaternion");
+    std::unique_ptr<glio_loop> L(new glio_loop());
+    L->ctx = c; L->opt = opt;
+    loop_extrinsic_bl(opt.q_lb, opt.t_lb, L->q_bl, L->t_bl);
+    c->loops.push_back(L.get());
+    *out = L.release();
+  });
+}
+
+void glio_loop_destroy(glio_loop* L) {
+  if (!L) return;
+  glio_ctx* c = L->ctx;
+  cudaSetDevice(c->device);
+  cudaStreamSynchronize(c->st);
+  L->release();
+  c->loops.erase(std::remove(c->loops.begin(), c->loops.end(), L), c->loops.end());
+  delete L;
+}
+
+int glio_loop_reset(glio_loop* L) {
+  if (!L) return GLIO_ERR_ARG;
+  return guarded(L->ctx, [&] {
+    GLIO_CUDA_TRY(cudaStreamSynchronize(L->ctx->st));
+    for (auto& k : L->kfs) k->xyz.release();
+    L->kfs.clear();
+    L->time_last_loop = 0.0;
+    L->lat_pts = L->his_pts = nullptr; L->lat_n = L->his_n = 0;
+  });
+}
+
+int glio_loop_add_keyframe(glio_loop* L, const float* cloud, int64_t n, int stride, int mem, const double pose[7], double time, int32_t* index) {
+  if (!L) return GLIO_ERR_ARG;
+  glio_ctx* c = L->ctx;
+  return guarded(c, [&] {
+    GLIO_REQUIRE(n >= 0 && n < ((int64_t)1 << 30) && (cloud || n == 0), GLIO_ERR_ARG, "glio_loop_add_keyframe: bad cloud pointer or size");
+    GLIO_REQUIRE(stride >= 3 && stride <= 64, GLIO_ERR_ARG, "glio_loop_add_keyframe: stride_floats must be in [3,64]");
+    GLIO_REQUIRE(mem == GLIO_HOST || mem == GLIO_DEVICE, GLIO_ERR_ARG, "glio_loop_add_keyframe: mem must be GLIO_HOST or GLIO_DEVICE");
+    GLIO_REQUIRE(mem != GLIO_DEVICE || n == 0 || dev_ptr_ok(c, cloud, 4), GLIO_ERR_ARG,
+                 "glio_loop_add_keyframe: a GLIO_DEVICE cloud must be 4-byte aligned memory of the context's GPU");
+    GLIO_REQUIRE(pose != nullptr && std::isfinite(time), GLIO_ERR_ARG, "glio_loop_add_keyframe: null pose or non-finite time");
+    for (int k = 0; k < 7; ++k) GLIO_REQUIRE(std::isfinite(pose[k]), GLIO_ERR_ARG, "glio_loop_add_keyframe: non-finite pose");
+    GLIO_REQUIRE(L->kfs.size() < (size_t)0x7fffffff, GLIO_ERR_ARG, "glio_loop_add_keyframe: too many keyframes");
+    std::unique_ptr<glio_loop::Keyframe> kf(new glio_loop::Keyframe());
+    kf->n = n;
+    if (n > 0) {
+      kf->xyz.reserve((size_t)n * 3);
+      // x,y,z of every point packed on the way in (one pitched copy, host or device source)
+      GLIO_CUDA_TRY(cudaMemcpy2DAsync(kf->xyz.p, 3 * sizeof(float), cloud, (size_t)stride * sizeof(float), 3 * sizeof(float), (size_t)n,
+                                      mem == GLIO_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, c->st));
+      if (mem != GLIO_DEVICE) GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));    // the caller may reuse its host buffer on return
+    }
+    for (int k = 0; k < 7; ++k) kf->pose[k] = pose[k];
+    kf->time = time;
+    for (int k = 0; k < 3; ++k) kf->pos[k] = (float)pose[k];
+    L->kfs.push_back(std::move(kf));
+    if (index) *index = (int32_t)(L->kfs.size() - 1);
+  });
+}
+
+int glio_loop_set_poses(glio_loop* L, int first, int count, const double* poses) {
+  if (!L) return GLIO_ERR_ARG;
+  return guarded(L->ctx, [&] {
+    GLIO_REQUIRE(first >= 0 && count >= 0 && (int64_t)first + count <= (int64_t)L->kfs.size() && (poses || count == 0), GLIO_ERR_ARG,
+                 "glio_loop_set_poses: keyframe range out of bounds");
+    for (int64_t i = 0; i < 7 * (int64_t)count; ++i) GLIO_REQUIRE(std::isfinite(poses[i]), GLIO_ERR_ARG, "glio_loop_set_poses: non-finite pose");
+    for (int i = 0; i < count; ++i) {
+      glio_loop::Keyframe& kf = *L->kfs[first + i];
+      for (int k = 0; k < 7; ++k) kf.pose[k] = poses[7 * i + k];
+      for (int k = 0; k < 3; ++k) kf.pos[k] = (float)kf.pose[k];
+    }
+  });
+}
+
+int glio_loop_size(glio_loop* L, int* n_keyframes) {
+  if (!L) return GLIO_ERR_ARG;
+  if (n_keyframes) *n_keyframes = (int)L->kfs.size();
+  return GLIO_OK;
+}
+
+int glio_loop_step(glio_loop* L, const float select_xyz[3], double time_new_odom, glio_loop_report* rep) {
+  if (!L) return GLIO_ERR_ARG;
+  return guarded(L->ctx, [&] {
+    GLIO_REQUIRE(select_xyz != nullptr && std::isfinite(select_xyz[0]) && std::isfinite(select_xyz[1]) && std::isfinite(select_xyz[2]) &&
+                 std::isfinite(time_new_odom), GLIO_ERR_ARG, "glio_loop_step: select_xyz and time_new_odom must be finite");
+    loop_step(L, select_xyz, time_new_odom, rep);
+  });
+}
+
+int glio_loop_get_clouds(glio_loop* L, int64_t lat_cap, float* lat_xyz, int64_t* n_lat, int64_t his_cap, float* his_xyz, int64_t* n_his) {
+  if (!L) return GLIO_ERR_ARG;
+  glio_ctx* c = L->ctx;
+  return guarded(c, [&] {
+    const int64_t nl = L->lat_pts ? L->lat_n : 0, nh = L->his_pts ? L->his_n : 0;
+    if (n_lat) *n_lat = nl;
+    if (n_his) *n_his = nh;
+    GLIO_REQUIRE((!lat_xyz || lat_cap >= nl) && (!his_xyz || his_cap >= nh), GLIO_ERR_ARG, "glio_loop_get_clouds: capacity too small");
+    auto fetch = [&](const float* d, int stride, int64_t n, float* xyz) {
+      if (!xyz || n <= 0) return;
+      std::vector<float> h((size_t)n * stride);
+      GLIO_CUDA_TRY(cudaMemcpyAsync(h.data(), d, h.size() * sizeof(float), cudaMemcpyDeviceToHost, c->st));
+      GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
+      for (int64_t i = 0; i < n; ++i) for (int k = 0; k < 3; ++k) xyz[3 * i + k] = h[(size_t)i * stride + k];
+    };
+    fetch(L->lat_pts, L->lat_stride, nl, lat_xyz);
+    fetch(L->his_pts, L->his_stride, nh, his_xyz);
   });
 }
 

@@ -330,4 +330,47 @@ void odom_quat_inverse(const double q[4], double o[4]);                         
 void odom_publish_run(const float4* surf, int64_t n_surf, const float4* full, int64_t n_full, float4* surf_out, float4* full_out,
                       const double trans[3], int deskew, cudaStream_t st, LaunchCounter& lc);
 
+// ---- loop-closure registration (loop.cu; pcl::IterativeClosestPoint as Estimator.cpp:5183-5273 configures it)
+// The registration state, resident on the device and read back once per iteration batch.  Matrices are row-major 4x4 floats.
+struct IcpState {
+  int32_t done;            // set by the one-thread kernels: every later kernel of the registration returns at once
+  int32_t converged, state, nr_iter;
+  int32_t n_corr;          // correspondences of the last correspondence estimation
+  int32_t nr_fit, pad0, pad1;
+  float transformation[16], final_T[16];
+  float smean[3], tmean[3];
+  double prev_mse, mse, fitness;
+};
+struct IcpConvergence {    // DefaultConvergenceCriteria as IterativeClosestPoint::computeTransformation sets it
+  int32_t max_iterations, log_cap;
+  double translation_threshold, rotation_threshold, mse_threshold_relative, mse_threshold_absolute;
+};
+struct IcpWork {
+  GridBuild grid;                                     // the target (fixed over the iterations)
+  DevBuf<float4> src0, cur, fit;                      // input, input_transformed (updated in place), input * final
+  DevBuf<int> qcount, qstart, perm, scan_tmp;         // cell order of the source
+  DevBuf<int> nn_idx, flags, pos, cq, cm;
+  DevBuf<float> nn_d, cd;
+  DevBuf<float> pf0, pf1; DevBuf<double> pd0, pd1;    // partial sums, levels 0 and 1
+  DevBuf<glio_icp_iteration> log;
+  DevBuf<IcpState> state;
+  IcpState last{};
+  int64_t n_src = 0, n_tgt = 0;
+  void release() {
+    grid.release(); src0.release(); cur.release(); fit.release(); qcount.release(); qstart.release(); perm.release(); scan_tmp.release();
+    nn_idx.release(); flags.release(); pos.release(); cq.release(); cm.release(); nn_d.release(); cd.release();
+    pf0.release(); pf1.release(); pd0.release(); pd1.release(); log.release(); state.release();
+  }
+};
+// one registration of d_src (n_src points, src_stride floats apart) onto d_tgt; *out receives the final state (fitness included).
+// w.fit holds the aligned cloud (float4), w.cq / w.cm / w.cd the last correspondence list, w.log the first min(log_cap, iterations)
+// iteration records.
+void icp_run(IcpWork& w, const float* d_src, int src_stride, int64_t n_src, const float* d_tgt, int tgt_stride, int64_t n_tgt,
+             const glio_icp_options& o, int log_cap, float pts_per_cell, cudaStream_t st, LaunchCounter& lc, IcpState* out, int* host_syncs);
+// host pose arithmetic of performLoopClosure / detectLoopClosure (poses t, q; scalar double in Eigen's order)
+void loop_quat_from_R(const double R[9], double q[4]);
+void loop_extrinsic_bl(const double q_lb[4], const double t_lb[3], double q_bl[4], double t_bl[3]);
+void loop_world_of_cloud(const double pose[7], const double q_bl[4], const double t_bl[3], double t[3], double q[4]);
+void loop_pose_from(const float final_T[16], const double latest[7], double out[7]);
+
 }  // namespace glio

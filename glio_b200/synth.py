@@ -330,3 +330,32 @@ def ring_scan(n_rings=32, n_az=1500, seed=SEED0 + 11, fov=(-25.0, 15.0), noise=0
         clouds.append(cl)
         start.append(total + 5); total += len(cl); end.append(total - 6)
     return np.concatenate(clouds), np.asarray(start, np.int32), np.asarray(end, np.int32)
+
+
+def loop_drive(K=240, n_points=2500, dt=0.5, speed=2.0, lane=3.0, drift_t=0.01, drift_yaw_deg=0.01, rng_range=40.0, seed=SEED0 + 14,
+               t0=1000.0):
+    """Keyframe surf clouds of one street-canyon scene along a closed path, for the loop closure (GLIO/src/Estimator.cpp:5090-5273).
+
+    The sensor drives out along the lane y = -lane for K/2 keyframes, turns round and drives back along y = +lane to where it
+    started: keyframe k and keyframe K-1-k see the same stretch of street, (K-1-2k)*dt seconds apart, so the path revisits its
+    beginning after more than lc_time_thres seconds once K*dt is large enough.  clouds[k] is n_points points of the scene within
+    rng_range of the sensor in the lidar frame of the TRUE pose (float32, packed x,y,z); poses[k] (t, q) carries a drift that grows
+    with k: a yaw of drift_yaw_deg*k degrees about the origin and a shift of (drift_t*k, drift_t*k/2, 0) metres, so a registration
+    of the returning keyframes against the outbound ones has a real correction to find.  times[k] = t0 + k*dt."""
+    rng = np.random.default_rng(seed)
+    half = K // 2
+    x_max = speed * dt * max(half - 1, 1)
+    scene = Scene(-rng_range - 10.0, x_max + rng_range + 10.0, rng)
+    truth = np.zeros((K, 7)); poses = np.zeros((K, 7))
+    for k in range(K):
+        out = k < half
+        x = speed * dt * (k if out else K - 1 - k)
+        truth[k, :3] = [x, -lane if out else lane, 0.0]
+        truth[k, 3:] = quat_from_rpy(0.0, 0.0, 0.0 if out else np.pi)
+        psi = np.deg2rad(drift_yaw_deg * k)
+        qd = quat_from_rpy(0.0, 0.0, psi)
+        poses[k, :3] = quat_to_R(qd) @ truth[k, :3] + [drift_t * k, 0.5 * drift_t * k, 0.0]
+        q = quat_mul(qd, truth[k, 3:])
+        poses[k, 3:] = q / np.linalg.norm(q)
+    clouds = [scan_in_lidar_frame(scene, truth[k], n_points, rng, rng_range) for k in range(K)]
+    return dict(clouds=clouds, poses=poses, poses_true=truth, times=t0 + dt * np.arange(K), K=K, dt=dt, seed=seed)

@@ -84,7 +84,9 @@ int64_t glio_launch_count(const glio_ctx* ctx);
  * | k_knn_box_cells [7], k_plane_fit, k_plane_fit_pair, k_flags, k_compact;
  * K2 k_eval_unary, k_eval_unary_cost, k_eval_binary, k_eval_binary_cost, k_bin_assemble; local map k_lm_transform, k_vox_*;
  * front end k_feat_curvature, k_feat_select, k_feat_voxel, k_feat_offsets, k_feat_gather; sweep preparation k_sp_bounds,
- * k_sp_consts, k_sp_classify, k_sp_ranges, k_sp_emit; odometry k_odom_publish). */
+ * k_sp_consts, k_sp_classify, k_sp_ranges, k_sp_emit; odometry k_odom_publish; loop-closure registration k_lc_load, k_lc_qhist,
+ * k_lc_qscatter, k_lc_init, k_lc_nn, k_lc_compact, k_lc_sum0, k_lc_sum1, k_lc_means, k_lc_solve, k_lc_transform, k_lc_final,
+ * k_lc_fitness). */
 int glio_profile_enable(glio_ctx* ctx, int on);
 int glio_profile_get(glio_ctx* ctx, const char* kernel_name, double* ms_total, int64_t* launches);
 /* statistics: number of queries a first search pass handed to its second pass (GLIO_KNN_MODE 0 and 4; 0 in the default mode) */
@@ -368,6 +370,121 @@ int glio_odom_step(glio_odom* od, const float* surf_xyzi, int64_t n_surf, int su
  * (surf_last_ds); either pointer may be NULL; the counts are always written.  Fails with GLIO_ERR_ARG if a capacity is too small. */
 int glio_odom_get_clouds(glio_odom* od, int64_t map_capacity, float* map_xyz, int64_t* n_map, int64_t scan_capacity, float* scan_xyz,
                          int64_t* n_scan);
+
+/* ---- loop-closure registration (SURVEY 8 f-7): the registration half of the Estimator's loop closure, detectLoopClosure and
+ * performLoopClosure (GLIO/src/Estimator.cpp:5101-5273) up to the GTSAM BetweenFactor, which stays with the caller.
+ *
+ * glio_icp_align = pcl::IterativeClosestPoint<PointXYZI, PointXYZI>::align with an identity guess (:5204-5214), restated from PCL 1.8
+ * (registration/impl/icp.hpp, transformation_estimation_svd.hpp = pcl::umeyama without scaling, correspondence_estimation.hpp,
+ * default_convergence_criteria.hpp) and getFitnessScore (registration.hpp).  Per iteration: exact 1-NN of every source point in the
+ * target (FLANN L2_Simple<float> distances, ties by index), kept when the float squared distance is <= max_correspondence_distance^2,
+ * in source order; fewer than 3: NO_CORRESPONDENCES, not converged; else umeyama in float (Eigen 3.3 JacobiSVD<Matrix3f>), the
+ * source transformed IN PLACE by that transformation in float ((t0 x + t1 y) + t2 z) + t3, final = transformation * final, and
+ * DefaultConvergenceCriteria (max iterations: converged; cos = 0.5 (float trace - 1) >= 1 - eps and float |t|^2 <= eps; absolute
+ * MSE change < 1e-12; relative MSE change < euclidean_fitness_epsilon).  The aligned cloud is the input transformed by final; the
+ * fitness is the double mean of the 1-NN squared distances of that cloud over every point (DBL_MAX when no point counts).  Sums run
+ * in the fixed order documented in glio_b200/csrc/loop.cu (DESIGN 2).  Kernel names for glio_profile_get: k_lc_load, k_lc_qhist,
+ * k_lc_qscatter, k_lc_init, k_lc_nn, k_lc_compact, k_lc_sum0, k_lc_sum1, k_lc_means, k_lc_solve, k_lc_transform, k_lc_final,
+ * k_lc_fitness (and the K0 grid kernels). */
+enum { GLIO_ICP_NOT_CONVERGED = 0, GLIO_ICP_ITERATIONS = 1, GLIO_ICP_TRANSFORM = 2, GLIO_ICP_ABS_MSE = 3, GLIO_ICP_REL_MSE = 4,
+       GLIO_ICP_NO_CORRESPONDENCES = 5 };   /* pcl::registration::DefaultConvergenceCriteria::ConvergenceState */
+typedef struct {
+  int32_t max_iterations;              /* setMaximumIterations(100)              (Estimator.cpp:5198) */
+  int32_t reserved;
+  double max_correspondence_distance;  /* setMaxCorrespondenceDistance(30)       (:5197) */
+  double transformation_epsilon;       /* setTransformationEpsilon(1e-6)         (:5199) */
+  double euclidean_fitness_epsilon;    /* setEuclideanFitnessEpsilon(1e-6)       (:5200); setRANSACIterations(5) has no effect on plain ICP */
+} glio_icp_options;
+void glio_icp_default_options(glio_icp_options* o);   /* the settings above */
+
+typedef struct {
+  float transformation[16];            /* this iteration's transformation_, row-major 4x4 */
+  int64_t n_corr;                      /* correspondences it was estimated from */
+  double mse;                          /* double mean of their squared distances (calculateMSE) */
+} glio_icp_iteration;
+
+typedef struct {
+  int32_t converged;                   /* hasConverged() */
+  int32_t state;                       /* GLIO_ICP_* */
+  int32_t iterations;                  /* nr_iterations_ */
+  int32_t host_syncs;                  /* host synchronisations the registration cost */
+  int64_t n_source, n_target;
+  int64_t n_corr;                      /* correspondences of the last correspondence estimation */
+  int64_t launches;                    /* kernels launched */
+  float final_transformation[16];      /* getFinalTransformation(), row-major 4x4 */
+  double fitness;                      /* getFitnessScore() */
+} glio_icp_result;
+
+/* src[n_src] / tgt[n_tgt]: x,y,z at floats 0..2 of stride_floats (3..64), host or device memory as src_mem / tgt_mem say (device
+ * pointers: 4-byte aligned memory of the context's GPU).  options NULL = glio_icp_default_options.  aligned_xyz[3 n_src] (host, may
+ * be NULL): the aligned cloud.  iter_log[iter_cap] (may be NULL): the first iter_cap iterations.  corr_query / corr_match / corr_dist
+ * (host, each may be NULL, room for corr_cap entries): the last correspondence estimation, (source index, target index, float squared
+ * distance) in source order; res->n_corr is its true length.  Does not touch the context's map, local map, window slots or batch
+ * frames.  Returns when its work is complete. */
+int glio_icp_align(glio_ctx* ctx, const float* src, int64_t n_src, int src_stride, int src_mem, const float* tgt, int64_t n_tgt,
+                   int tgt_stride, int tgt_mem, const glio_icp_options* options, float* aligned_xyz, glio_icp_result* res,
+                   glio_icp_iteration* iter_log, int iter_cap, int32_t* corr_query, int32_t* corr_match, float* corr_dist, int64_t corr_cap);
+
+/* The loop object: the Estimator's keyframe store for the loop closure and its detection / registration step.
+ *   keyframe k: surf_frames[k] (its surf_last_ds, lidar frame, :4150-4153), pose_info_keyframe[k] (body pose t, q and time,
+ *   :4253-4264) and pose_keyframe[k] (the same position as float x,y,z, the cloud of the radius search).  Keyframe clouds stay
+ *   resident on the device: each crosses PCIe once, in glio_loop_add_keyframe.  glio_loop_set_poses overwrites poses after
+ *   insertion (updatePose, :3435-3450; correctPoses); the times stay.
+ *   glio_loop_step(select_xyz, time_new_odom) = performLoopClosure (:5183-5273) without the GTSAM half:
+ *     detection (:5101-5181): radius search of pose_keyframe around select_xyz (float squared distance < float(r^2), sorted by
+ *       distance, ties by index), closest_his_idx = the first result with |time - time_new_odom| > lc_time_thres; no candidate when
+ *       none passes or |time_last_loop - time_new_odom| < 0.2; latest_frame_idx_loop = size - slide_window_width;
+ *     the latest cloud: keyframes latest - j, j = 0..5, newest first, negative indices skipped; the history cloud: closest + j,
+ *       j = -lc_map_width..lc_map_width, oldest first, outside [0, latest] skipped; each moved by q_po*q_bl, q_po*t_bl + t_po
+ *       (transformCloud, :1517-1545; q_bl = q_lb^-1, t_bl = -(q_bl t_lb), :873-877), concatenated, VoxelGrid(leaf) (:855);
+ *     glio_icp_align(latest_ds onto his_ds) with the options' ICP settings; accepted when converged and fitness <= lc_icp_thres;
+ *     then pose_from = (qIncre * q_latest, qIncre * t_latest + t) with qIncre Eigen's quaternion of final's rotation, pose_to = the
+ *       history keyframe's pose, noise score = fitness, time_last_loop = time[latest] (the caller adds
+ *       BetweenFactor(poseFrom.between(poseTo)) to its own pose graph).
+ *   With no candidate the step launches nothing.  The loop object runs on its context's device, stream, launch counter and profiler
+ *   but owns its state: it never reads or changes the context's glio_params, map, local map, window slots, batch frames or
+ *   odometries.  glio_destroy frees loop objects still attached to the context. */
+typedef struct {
+  double lc_search_radius;             /* 25 (GLIO/config/config_urban_hk.yaml:80; code default 7.0, Estimator.cpp:667-670) */
+  double lc_time_thres;                /* 30 (:83; code default 30, Estimator.cpp:637-640) */
+  int32_t lc_map_width;                /* 25 (:81; code default 25) */
+  float lc_icp_thres;                  /* 0.2 (:82; code default 0.3); a float in the reference (Estimator.cpp:230) */
+  int32_t slide_window_width;          /* 5 (:66) */
+  float leaf;                          /* ds_filter_his_frames.setLeafSize(0.4) (Estimator.cpp:855) */
+  double q_lb[4];                      /* extrinsic, w,x,y,z (config_urban_hk.yaml:90-93) */
+  double t_lb[3];                      /* (:94-97) */
+  glio_icp_options icp;
+} glio_loop_options;
+void glio_loop_default_options(glio_loop_options* o);   /* the shipped configuration above */
+
+typedef struct {
+  int32_t detected;                    /* detectLoopClosure() returned true: the registration ran */
+  int32_t closest_his_idx;             /* -1: no keyframe passed the radius and time tests */
+  int32_t latest_frame_idx;            /* latest_frame_idx_loop (valid when detected) */
+  int32_t accepted;                    /* converged and fitness <= lc_icp_thres */
+  int64_t n_latest, n_latest_ds, n_his, n_his_ds;   /* cloud sizes before / after the voxel filter */
+  int64_t n_candidates;                /* keyframes inside the search radius */
+  glio_icp_result icp;
+  double pose_from[7], pose_to[7];     /* t then q (the reference builds gtsam poses from q and t) */
+  double noise_score;                  /* the fitness, the variance of the loop factor's diagonal noise model */
+  double time_last_loop;               /* after this step */
+} glio_loop_report;
+
+typedef struct glio_loop glio_loop;
+int glio_loop_create(glio_ctx* ctx, const glio_loop_options* options /* NULL: defaults */, glio_loop** out);
+void glio_loop_destroy(glio_loop* lp);
+int glio_loop_reset(glio_loop* lp);    /* no keyframe, time_last_loop = 0 (device buffers are kept) */
+/* cloud[n] (n >= 0) with stride_floats in [3,64], host or device memory (device: 4-byte aligned memory of the context's GPU);
+ * pose[7] = body pose t, q; returns the keyframe's index in *index (may be NULL). */
+int glio_loop_add_keyframe(glio_loop* lp, const float* cloud, int64_t n, int stride_floats, int mem, const double pose[7], double time,
+                           int32_t* index);
+int glio_loop_set_poses(glio_loop* lp, int first, int count, const double* poses /* count x 7 */);
+int glio_loop_size(glio_loop* lp, int* n_keyframes);
+int glio_loop_step(glio_loop* lp, const float select_xyz[3], double time_new_odom, glio_loop_report* rep);
+/* debug copy-out of the last registration's filtered clouds (latest_key_frames_ds, his_key_frames_ds; x,y,z in the filter's output
+ * order); either pointer may be NULL, the counts are always written; GLIO_ERR_ARG if a capacity is too small. */
+int glio_loop_get_clouds(glio_loop* lp, int64_t latest_capacity, float* latest_xyz, int64_t* n_latest, int64_t his_capacity, float* his_xyz,
+                         int64_t* n_his);
 
 /* ---- K3: marginalisation of the oldest keyframe (MarginalizationInfo, GLIO/src/MarginalizationFactor.cpp:82-202; call site
  * Estimator.cpp:2462-2608).  The reference re-evaluates EVERY LiDAR factor of the window (:2538-2576, one virtual Evaluate per
