@@ -135,7 +135,7 @@ class Context:
         self._lib.glio_lidar_pose(C.byref(self.params), _ptr(pb), _ptr(t2), _ptr(q2))
         return t2, q2
 
-    KERNELS = ["k_feat_curvature", "k_feat_select", "k_feat_voxel", "k_feat_offsets", "k_feat_gather", "k_knn_tile", "k_knn_tile2", "k_defer_scatter", "k_knn_box_start", "k_knn_grow", "k_knn_box_far", "k_knn_far", "k_knn_box_cells", "k_knn_team", "k_make_pairs", "k_knn_search", "k_knn_deferred", "k_knn_thread", "k_knn_box", "k_plane_fit", "k_plane_fit_pair", "k_eval_unary", "k_eval_unary_cost", "k_transform_hist", "k_order_scatter",
+    KERNELS = ["k_feat_curvature", "k_feat_select", "k_feat_voxel", "k_feat_offsets", "k_feat_gather", "k_knn_box", "k_plane_fit", "k_plane_fit_pair", "k_eval_unary", "k_eval_unary_cost", "k_transform_hist", "k_order_scatter",
                "k_compact", "k_flags", "k_cell_hist", "k_cell_scatter", "k_load_bounds", "k_scan_block", "k_scan_add",
                "k_eval_binary", "k_eval_binary_cost", "k_bin_assemble",
                "k_lm_transform", "k_vox_hist", "k_vox_scatter", "k_vox_sort", "k_vox_flags", "k_vox_centroid", "k_init_bounds"]
@@ -153,6 +153,7 @@ class Context:
         return out
 
     def knn_fallback_queries(self, reset=False):
+        """Queries the kNN search handed to a second pass: always 0, the box search has none (glio_get_stats)."""
         n = C.c_int64(0)
         self._chk(self._lib.glio_get_stats(self._h, C.byref(n), C.c_int(1 if reset else 0)))
         return int(n.value)

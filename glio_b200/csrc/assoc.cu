@@ -4,8 +4,7 @@
 // findGlobalCorrespondingSurfFeatures[Add]_Batch (Estimator.cpp:3710-3892):
 //   transform -> exact 5-NN (FLANN L2_Simple<float> distances, ties by index) -> gate on the squared 5th
 //   distance -> 5x3 column-pivoted Householder LS plane fit (double) -> validity -> weight -> outputs.
-// Exactness of the kNN: a box of grid cells around the query is searched and grown (face by face in the default
-// k_knn_box, ring by ring in k_knn_thread / the warp-cooperative k_knn_search kept for comparison, GLIO_KNN_MODE) until
+// Exactness of the kNN: a box of grid cells around the query is searched and grown face by face (k_knn_box) until
 // the 5th best distance is provably inside the searched box, or the box already covers the gate radius (then anything
 // unseen fails the gate anyway).
 //
@@ -59,169 +58,15 @@ __global__ void __launch_bounds__(256) k_order_scatter(GridDesc grid, int64_t Qt
 }
 
 // ---------------------------------------------------------------------------------------------------
-// K1a (warp-cooperative variant, GLIO_KNN_MODE=0; not the default - see DESIGN.md section 4 for the measurements).
-// Queries arrive sorted by grid cell, so the 32 queries of a warp sit in a short run of x-adjacent cells of one
-// (y,z) row.  The warp stages the rows around that run — each row is ONE contiguous range of the counting-sorted
-// map (x is the fastest cell coordinate) — through shared memory with coalesced 16-byte loads, and every lane scans
-// the same candidate list (broadcast LDS, uniform trip count: no divergence).  The scanned box grows ring by ring
-// (shell cells only, nothing is visited twice) until every lane's 5th distance is provably inside the box, or the
-// box covers the gate radius (anything unseen then fails the radius gate anyway).
-// Intermediate results are written in sorted order, structure-of-arrays: coalesced here and in K1b.
+// K1a (box growth): one query per thread; each (y,z) row of cells is one contiguous range of the sorted map, and the
+// queries arrive cell-sorted, so the loads of neighbouring threads hit the same lines.  The searched box of a query
+// grows one FACE at a time instead of one ring at a time.  After the start box (3x3x3 cells around the query) a face
+// is pushed out by one cell layer only if something nearer than the current 5th distance could still hide behind it:
+// the face is not at the grid border, not farther than the gate radius, and closer to the query than the 5th distance.
+// A query near one cell wall with a 5th neighbour a little beyond it scans one extra slab of 9 cells instead of the 98
+// cells of a full second ring; the top-5 is exact (every unscanned point lies beyond some face, all faces are at least
+// the 5th distance away), faces are re-tested with the freshest 5th distance.
 // ---------------------------------------------------------------------------------------------------
-constexpr int KNN_WARPS = 4;
-constexpr int KNN_SPAN_MAX = 12;
-
-__global__ void __launch_bounds__(32 * KNN_WARPS) k_knn_search(SearchArgs a) {
-  __shared__ __align__(16) float sx[KNN_WARPS][32], sy[KNN_WARPS][32], sz[KNN_WARPS][32];
-  __shared__ __align__(16) int si[KNN_WARPS][32];
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  const int64_t p = ((int64_t)blockIdx.x * KNN_WARPS + wid) * 32 + lane;
-  const bool active = p < a.Qt;
-  const GridDesc& G = a.grid;
-  const float INF = __int_as_float(0x7f800000);
-  float qx = 0.f, qy = 0.f, qz = 0.f;
-  if (active) { const float4 q4 = a.pmq[p]; qx = q4.x; qy = q4.y; qz = q4.z; }
-  const int cx = cell_coord(qx, G.ox, G.inv_cell), cy = cell_coord(qy, G.oy, G.inv_cell), cz = cell_coord(qz, G.oz, G.inv_cell);
-  Top5 t;
-  top5_init(t);
-  const f32x2_t qx2 = pack2(qx, qx), qy2 = pack2(qy, qy), qz2 = pack2(qz, qz);
-  const int rmax = (int)ceilf((sqrtf(a.gate_sq) + 2e-3f) * G.inv_cell) + 1;
-  // far outside the grid: nothing within the gate radius
-  const bool far_out = cx < -rmax || cy < -rmax || cz < -rmax || cx >= G.nx + rmax || cy >= G.ny + rmax || cz >= G.nz + rmax;
-  bool done = !active || far_out;
-  const int* __restrict__ cs = G.cell_start;
-  unsigned long long extra_rings = 0;
-  for (;;) {
-    const unsigned pending = __ballot_sync(0xffffffffu, !done);
-    if (!pending) break;
-    const int leader = __ffs(pending) - 1;
-    const int lcx = __shfl_sync(0xffffffffu, cx, leader), lcy = __shfl_sync(0xffffffffu, cy, leader), lcz = __shfl_sync(0xffffffffu, cz, leader);
-    const bool part = !done && cy == lcy && cz == lcz && cx >= lcx && cx < lcx + KNN_SPAN_MAX;
-    const int hix = __reduce_max_sync(0xffffffffu, part ? cx : lcx);
-    bool unproven = part;
-    bool defer = false;
-    const int rlim = min(rmax, a.tile_rings);
-    for (int r = 1; r <= rlim; ++r) {
-      const int xa = lcx - r, xb = hix + r;                 // scanned cell range in x after this ring
-      const int x0 = max(xa, 0), x1 = min(xb, G.nx - 1);
-      const int z0 = max(lcz - r, 0), z1 = min(lcz + r, G.nz - 1);
-      const int y0 = max(lcy - r, 0), y1 = min(lcy + r, G.ny - 1);
-      const int nzr = z1 - z0 + 1, nyr = y1 - y0 + 1;
-      for (int ri = 0; ri < nzr * nyr; ++ri) {
-        {
-          // visit order: for the first ring the query's own row first, then the rest (the 5th distance shrinks early
-          // and the pre-filter rejects more); later rings in plain row order
-          int zz = z0 + ri / nyr, yy = y0 + ri % nyr;
-          if (r == 1 && lcz >= z0 && lcz <= z1 && lcy >= y0 && lcy <= y1) {
-            const int own = (lcz - z0) * nyr + (lcy - y0);
-            const int rj = ri == 0 ? own : (ri <= own ? ri - 1 : ri);
-            zz = z0 + rj / nyr; yy = y0 + rj % nyr;
-          }
-          const int z = zz, y = yy;
-          const bool zshell = (z == lcz - r) || (z == lcz + r);
-          const int row = (z * G.ny + y) * G.nx;
-          const bool shell = r == 1 || zshell || (y == lcy - r) || (y == lcy + r);
-          // shell rows are new: whole x-range; inner rows were scanned up to [xa+1, xb-1]: only the two end cells
-          for (int part_i = 0; part_i < 2; ++part_i) {
-            int s, e;
-            if (shell) { if (part_i == 1 || x0 > x1) break; s = __ldg(&cs[row + x0]); e = __ldg(&cs[row + x1 + 1]); }
-            else {
-              const int xc = part_i == 0 ? xa : xb;
-              if (xc < 0 || xc >= G.nx) continue;
-              s = __ldg(&cs[row + xc]); e = __ldg(&cs[row + xc + 1]);
-            }
-            for (int base = s; base < e; base += 32) {
-              const int k = base + lane;
-              float4 pt = make_float4(1.0e18f, 1.0e18f, 1.0e18f, 0.f);       // filler for the odd lane of the last pair (never pushed)
-              if (k < e) pt = __ldg(&G.pts[k]);
-              sx[wid][lane] = pt.x; sy[wid][lane] = pt.y; sz[wid][lane] = pt.z; si[wid][lane] = __float_as_int(pt.w);
-              __syncwarp();
-              const int cnt = min(32, e - base);
-              if (unproven) {
-                const f32x2_t* px2 = reinterpret_cast<const f32x2_t*>(sx[wid]);
-                const f32x2_t* py2 = reinterpret_cast<const f32x2_t*>(sy[wid]);
-                const f32x2_t* pz2 = reinterpret_cast<const f32x2_t*>(sz[wid]);
-                for (int j = 0; j < cnt; j += 2) {
-                  const f32x2_t dx = sub2(qx2, px2[j >> 1]), dy = sub2(qy2, py2[j >> 1]), dz = sub2(qz2, pz2[j >> 1]);
-                  const f32x2_t a2 = fma2(dz, dz, fma2(dy, dy, mul2(dx, dx)));
-                  float a0, a1; unpack2(a2, a0, a1);
-                  const float thr = key_dist(t.k4) * 1.000001f;             // +inf until five candidates were seen
-                  if (a0 <= thr) top5_push(t, l2_simple(qx, qy, qz, sx[wid][j], sy[wid][j], sz[wid][j]), si[wid][j]);
-                  if (j + 1 < cnt && a1 <= key_dist(t.k4) * 1.000001f) top5_push(t, l2_simple(qx, qy, qz, sx[wid][j + 1], sy[wid][j + 1], sz[wid][j + 1]), si[wid][j + 1]);
-                }
-              }
-              __syncwarp();
-            }
-          }
-        }
-      }
-      if (unproven) {
-        // distance to the faces of the scanned box; faces clipped by the grid are infinitely far (nothing lives outside)
-        float b = INF;
-        if (xa > 0)               b = fminf(b, qx - (G.ox + (float)xa * G.cell));
-        if (xb < G.nx - 1)        b = fminf(b, (G.ox + (float)(xb + 1) * G.cell) - qx);
-        if (lcy - r > 0)          b = fminf(b, qy - (G.oy + (float)(lcy - r) * G.cell));
-        if (lcy + r < G.ny - 1)   b = fminf(b, (G.oy + (float)(lcy + r + 1) * G.cell) - qy);
-        if (lcz - r > 0)          b = fminf(b, qz - (G.oz + (float)(lcz - r) * G.cell));
-        if (lcz + r < G.nz - 1)   b = fminf(b, (G.oz + (float)(lcz + r + 1) * G.cell) - qz);
-        const float bs = b * 0.999f - 2e-3f;   // safety: float rounding of cell assignment / face positions
-        if ((b == INF) || (bs > 0.f && key_dist(t.k4) <= bs * bs)) unproven = false;
-        else if (r == rlim && rlim < rmax) defer = true;      // not provable inside the tile: single-query pass
-      }
-      if (!__ballot_sync(0xffffffffu, unproven)) break;
-    }
-    if (part) done = true;
-    // warp-aggregated append of the deferred queries
-    const unsigned dm = __ballot_sync(0xffffffffu, defer);
-    if (dm) {
-      unsigned int base = 0;
-      if (lane == 0) { base = atomicAdd(a.n_deferred, (unsigned int)__popc(dm)); extra_rings += __popc(dm); }
-      base = __shfl_sync(0xffffffffu, base, 0);
-      if (defer) a.deferred[base + __popc(dm & ((1u << lane) - 1u))] = (uint32_t)p;
-    }
-  }
-  if (a.n_fallback && lane == 0 && extra_rings) atomicAdd(a.n_fallback, extra_rings);
-  if (active) {
-    a.knn_idx[0 * a.Qt + p] = key_idx(t.k0); a.knn_idx[1 * a.Qt + p] = key_idx(t.k1); a.knn_idx[2 * a.Qt + p] = key_idx(t.k2);
-    a.knn_idx[3 * a.Qt + p] = key_idx(t.k3); a.knn_idx[4 * a.Qt + p] = key_idx(t.k4);
-    a.knn_sqd[0 * a.Qt + p] = key_dist(t.k0); a.knn_sqd[1 * a.Qt + p] = key_dist(t.k1); a.knn_sqd[2 * a.Qt + p] = key_dist(t.k2);
-    a.knn_sqd[3 * a.Qt + p] = key_dist(t.k3); a.knn_sqd[4 * a.Qt + p] = key_dist(t.k4);
-  }
-}
-
-// ---------------------------------------------------------------------------------------------------
-// K1a (per-thread variants, GLIO_KNN_MODE=1..3): one query per thread, rings of cells around the query's own cell, each (y,z) row of a
-// ring is one contiguous range of the sorted map.  Fewer candidate evaluations per query than the tile pass (the
-// searched box is exactly the query's own), at the price of divergent trip counts.  Queries arrive cell-sorted, so
-// the loads of neighbouring threads hit the same lines.
-// ---------------------------------------------------------------------------------------------------
-// K1a (ring growth, knn_mode 1): one query per thread, whole rings until the 5th distance is provably inside the box.
-__global__ void __launch_bounds__(128, 7) k_knn_thread(SearchArgs a) {
-  __shared__ int sbnd[18 * 128];                     // [row bound][thread]: conflict-free columns
-  const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (p >= a.Qt) return;
-  const GridDesc& g = a.grid;
-  const float4 q4 = a.pmq[p];
-  const float qx = q4.x, qy = q4.y, qz = q4.z;
-  Top5 t; top5_init(t);
-  const int cx = cell_coord(qx, g.ox, g.inv_cell), cy = cell_coord(qy, g.oy, g.inv_cell), cz = cell_coord(qz, g.oz, g.inv_cell);
-  const int rmax = (int)ceilf((sqrtf(a.gate_sq) + 2e-3f) * g.inv_cell) + 1;
-  const bool far_out = cx < -rmax || cy < -rmax || cz < -rmax || cx >= g.nx + rmax || cy >= g.ny + rmax || cz >= g.nz + rmax;
-  float d4f = __int_as_float(0x7f800000);
-  if (!far_out) thread_rings(g, qx, qy, qz, cx, cy, cz, 1, rmax, rmax, t, d4f, sbnd + threadIdx.x);
-  store_top5(a, p, t);
-}
-
-// ---------------------------------------------------------------------------------------------------
-// K1a (box growth): the searched box of a query grows one FACE at a time instead of one ring at a time.  After the
-// start box (3x3x3 cells around the query, or only its own cell when start_own) a face is pushed out by one cell
-// layer only if something nearer than the current 5th distance could still hide behind it: the face is not at the
-// grid border, not farther than the gate radius, and closer to the query than the 5th distance.  A query near one
-// cell wall with a 5th neighbour a little beyond it scans one extra slab of 9 cells instead of the 98 cells of a
-// full second ring; the top-5 is exact under the same proof as the ring search (every unscanned point lies beyond
-// some face, all faces are at least the 5th distance away), faces are re-tested with the freshest 5th distance.
-// ---------------------------------------------------------------------------------------------------
-template <bool START_OWN>
 __global__ void __launch_bounds__(128, 6) k_knn_box(SearchArgs a) {
   __shared__ int sbnd[18 * 128];
   const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -236,98 +81,10 @@ __global__ void __launch_bounds__(128, 6) k_knn_box(SearchArgs a) {
   const bool far_out = cx < -rmax || cy < -rmax || cz < -rmax || cx >= g.nx + rmax || cy >= g.ny + rmax || cz >= g.nz + rmax;
   float d4f = __int_as_float(0x7f800000);
   if (!far_out) {
-    int lx, hx, ly, hy, lz, hz;
-    if (START_OWN) {
-      lx = hx = cx; ly = hy = cy; lz = hz = cz;
-      scan_rows(g, cx, cx, cy, cy, cz, cz, qx, qy, qz, t, d4f);
-    } else {
-      lx = cx - 1; hx = cx + 1; ly = cy - 1; hy = cy + 1; lz = cz - 1; hz = cz + 1;
-      thread_rings(g, qx, qy, qz, cx, cy, cz, 1, 1, rmax, t, d4f, sbnd + threadIdx.x);
-    }
-    box_grow(g, qx, qy, qz, gate_r, rmax, lx, hx, ly, hy, lz, hz, t, d4f, a.grow_mode ? sbnd + threadIdx.x : nullptr);
+    scan_start_box(g, qx, qy, qz, cx, cy, cz, t, d4f, sbnd + threadIdx.x);
+    box_grow(g, qx, qy, qz, gate_r, rmax, cx - 1, cx + 1, cy - 1, cy + 1, cz - 1, cz + 1, t, d4f, sbnd + threadIdx.x);
   }
   store_top5(a, p, t);
-}
-
-// ---------------------------------------------------------------------------------------------------
-// K1a': single-query pass for the few queries the tile pass could not prove within its first ring (their 5th
-// neighbour is farther than one cell: sparse map, or a query displaced from the surface by the pose error).
-// One warp per query: the 32 lanes each test one candidate of a batch; the replicated top-5 is updated with the
-// survivors in lane order (uniform control flow).  Rings are scanned from scratch, segment bounds of a whole ring
-// are fetched by the lanes in parallel (one latency per ring instead of one per row), empty segments are skipped.
-// ---------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(128) k_knn_deferred(SearchArgs a) {
-  const int lane = threadIdx.x & 31;
-  const unsigned int nwarps = gridDim.x * (blockDim.x >> 5);
-  const unsigned int nd = *a.n_deferred;
-  const GridDesc& G = a.grid;
-  const float INF = __int_as_float(0x7f800000);
-  const int* __restrict__ cs = G.cell_start;
-  const int rmax = (int)ceilf((sqrtf(a.gate_sq) + 2e-3f) * G.inv_cell) + 1;
-  for (unsigned int it = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); it < nd; it += nwarps) {
-    const int64_t p = a.deferred[it];
-    const float4 q4 = a.pmq[p];
-    const float qx = q4.x, qy = q4.y, qz = q4.z;
-    const int cx = cell_coord(qx, G.ox, G.inv_cell), cy = cell_coord(qy, G.oy, G.inv_cell), cz = cell_coord(qz, G.oz, G.inv_cell);
-    Top5 t; top5_init(t);
-    for (int r = 1; r <= rmax; ++r) {
-      // segments of ring r: every row (dy,dz) of the (2r+1)^2 square; shell rows span [cx-r, cx+r], inner rows only the
-      // two end cells.  Segment index = row * 2 + part.
-      const int side = 2 * r + 1, nseg = side * side * 2;
-      for (int sb = 0; sb < nseg; sb += 32) {
-        const int sidx = sb + lane;
-        int s = 0, e = 0;
-        if (sidx < nseg) {
-          const int rowi = sidx >> 1, part = sidx & 1;
-          const int dz = rowi / side - r, dy = rowi % side - r;
-          const int z = cz + dz, y = cy + dy;
-          if (z >= 0 && z < G.nz && y >= 0 && y < G.ny) {
-            const bool shell = r == 1 || dz == -r || dz == r || dy == -r || dy == r;
-            const int row = (z * G.ny + y) * G.nx;
-            if (shell) {
-              const int x0 = max(cx - r, 0), x1 = min(cx + r, G.nx - 1);
-              if (part == 0 && x0 <= x1) { s = __ldg(&cs[row + x0]); e = __ldg(&cs[row + x1 + 1]); }
-            } else {
-              const int xc = part == 0 ? cx - r : cx + r;
-              if (xc >= 0 && xc < G.nx) { s = __ldg(&cs[row + xc]); e = __ldg(&cs[row + xc + 1]); }
-            }
-          }
-        }
-        unsigned m = __ballot_sync(0xffffffffu, e > s);
-        while (m) {
-          const int j = __ffs(m) - 1; m &= m - 1;
-          const int ss = __shfl_sync(0xffffffffu, s, j), ee = __shfl_sync(0xffffffffu, e, j);
-          for (int base = ss; base < ee; base += 32) {
-            const int k = base + lane;
-            unsigned long long key = KEY_EMPTY;
-            if (k < ee) { const float4 pt = __ldg(&G.pts[k]); key = make_key(l2_simple(qx, qy, qz, pt.x, pt.y, pt.z), __float_as_int(pt.w)); }
-            unsigned c = __ballot_sync(0xffffffffu, key < t.k4);
-            while (c) {
-              const int l = __ffs(c) - 1; c &= c - 1;
-              const unsigned long long kl = __shfl_sync(0xffffffffu, key, l);
-              if (kl < t.k4) { t.k4 = kl; GLIO_KSWAP(t.k3, t.k4) GLIO_KSWAP(t.k2, t.k3) GLIO_KSWAP(t.k1, t.k2) GLIO_KSWAP(t.k0, t.k1) }
-            }
-          }
-        }
-      }
-      float b = INF;
-      if (cx - r > 0)        b = fminf(b, qx - (G.ox + (float)(cx - r) * G.cell));
-      if (cx + r < G.nx - 1) b = fminf(b, (G.ox + (float)(cx + r + 1) * G.cell) - qx);
-      if (cy - r > 0)        b = fminf(b, qy - (G.oy + (float)(cy - r) * G.cell));
-      if (cy + r < G.ny - 1) b = fminf(b, (G.oy + (float)(cy + r + 1) * G.cell) - qy);
-      if (cz - r > 0)        b = fminf(b, qz - (G.oz + (float)(cz - r) * G.cell));
-      if (cz + r < G.nz - 1) b = fminf(b, (G.oz + (float)(cz + r + 1) * G.cell) - qz);
-      if (b == INF) break;
-      const float bs = b * 0.999f - 2e-3f;
-      if (bs > 0.f && key_dist(t.k4) <= bs * bs) break;
-    }
-    if (lane == 0) {
-      a.knn_idx[0 * a.Qt + p] = key_idx(t.k0); a.knn_idx[1 * a.Qt + p] = key_idx(t.k1); a.knn_idx[2 * a.Qt + p] = key_idx(t.k2);
-      a.knn_idx[3 * a.Qt + p] = key_idx(t.k3); a.knn_idx[4 * a.Qt + p] = key_idx(t.k4);
-      a.knn_sqd[0 * a.Qt + p] = key_dist(t.k0); a.knn_sqd[1 * a.Qt + p] = key_dist(t.k1); a.knn_sqd[2 * a.Qt + p] = key_dist(t.k2);
-      a.knn_sqd[3 * a.Qt + p] = key_dist(t.k3); a.knn_sqd[4 * a.Qt + p] = key_dist(t.k4);
-    }
-  }
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -354,14 +111,8 @@ struct FitArgs {
   double* plane;
 };
 
-#ifndef GLIO_FIT_REGATHER
-#define GLIO_FIT_REGATHER 1
-#endif
-#ifndef GLIO_FIT_MINBLOCKS
-#define GLIO_FIT_MINBLOCKS (GLIO_FIT_REGATHER ? 5 : 4)
-#endif
 template <bool PAIR>
-__global__ void __launch_bounds__(128, GLIO_FIT_MINBLOCKS) k_plane_fit(FitArgs a) {
+__global__ void __launch_bounds__(128, 5) k_plane_fit(FitArgs a) {
   const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= a.Qt) return;
   const float4 q4 = a.pmq[p];
@@ -375,7 +126,6 @@ __global__ void __launch_bounds__(128, GLIO_FIT_MINBLOCKS) k_plane_fit(FitArgs a
   double n[3] = {0, 0, 0}, d = 0;
   double nl[3] = {0, 0, 0}, cl[3] = {0, 0, 0};
   if (id[4] != 0x7fffffff && (double)d4 < a.gates.max_radius) {           // Estimator.cpp:3651 / :3751
-#if GLIO_FIT_REGATHER
     // the five neighbours are gathered twice (for the fit, and again for the validity test: L1/L2 hits) so that the 15 doubles
     // are not live across the QR: ~30 registers less, one more resident block per SM
     int pos[5];
@@ -397,28 +147,6 @@ __global__ void __launch_bounds__(128, GLIO_FIT_MINBLOCKS) k_plane_fit(FitArgs a
       const double v = dadd(dadd(dadd(dmul(n[0], (double)m.x), dmul(n[1], (double)m.y)), dmul(n[2], (double)m.z)), d);
       if (fabs(v) > a.gates.dist_thres) ok = false;
     }
-#else
-    double A[3][5];
-#pragma unroll
-    for (int j = 0; j < 5; ++j) {
-      const float4 m = __ldg(&a.pts_sorted[__ldg(&a.sorted_pos[id[j]])]);
-      A[0][j] = (double)m.x; A[1][j] = (double)m.y; A[2][j] = (double)m.z;
-    }
-    double Aw[3][5];
-#pragma unroll
-    for (int c = 0; c < 3; ++c)
-#pragma unroll
-      for (int j = 0; j < 5; ++j) Aw[c][j] = A[c][j];
-    double x[3];
-    plane_solve5(Aw, x);                                                    // :3661
-    plane_from_solution(x, n, d);                                           // :3662-3663
-    bool ok = true;
-#pragma unroll
-    for (int j = 0; j < 5; ++j) {                                           // :3667-3674
-      const double v = dadd(dadd(dadd(dmul(n[0], A[0][j]), dmul(n[1], A[1][j])), dmul(n[2], A[2][j])), d);
-      if (fabs(v) > a.gates.dist_thres) ok = false;
-    }
-#endif
     if (ok) {
       w = weight_of(n, d, q4.x, q4.y, q4.z);                                // :3678-3679
       st = ((double)w > a.gates.weight_min) ? GLIO_MATCH_VALID : GLIO_MATCH_FAIL_WEIGHT;  // :3681
@@ -484,29 +212,8 @@ void assoc_run(const GridBuild& gb, const SegDesc* d_segs, int nseg, const Assoc
   lc.begin("k_order_scatter", st); k_order_scatter<<<nb, 256, 0, st>>>(grid, Qt, w.pm, cell_pos.p, cell_count.p, w.pmq); lc.end(st);
   SearchArgs sa;
   sa.grid = grid; sa.Qt = Qt; sa.pm = w.pm; sa.pmq = w.pmq; sa.gate_sq = (float)gates.max_radius;
-  sa.knn_idx = w.knn_idx; sa.knn_sqd = w.knn_sqd; sa.n_fallback = w.n_fallback; sa.store_all_sqd = w.idx5 != nullptr;
-  sa.tile_rings = w.tile_rings; sa.grow_mode = w.grow_mode; sa.deferred = w.deferred; sa.n_deferred = w.n_deferred;
-  GLIO_CUDA_TRY(cudaMemsetAsync(w.n_deferred, 0, sizeof(unsigned int), st));
-  const unsigned ns = (unsigned)((Qt + 32 * KNN_WARPS - 1) / (32 * KNN_WARPS));
-  if (w.knn_mode == 7) {
-    knn_box_cells_run(sa, st, lc);
-  } else if (w.knn_mode == 6) {
-    knn_box_far_run(sa, st, lc);
-  } else if (w.knn_mode == 5) {
-    knn_box2_run(sa, cell_count, scan_tmp, st, lc);
-  } else if (w.knn_mode == 4) {
-    knn_tile_run(sa, gb.pairs.p, cell_count, scan_tmp, st, lc);      // cell_count is free again after the query scatter
-  } else if (w.knn_mode == 2 || w.knn_mode == 3) {
-    lc.begin("k_knn_box", st);
-    if (w.knn_mode == 3) k_knn_box<true><<<(unsigned)((Qt + 127) / 128), 128, 0, st>>>(sa);
-    else k_knn_box<false><<<(unsigned)((Qt + 127) / 128), 128, 0, st>>>(sa);
-    lc.end(st);
-  } else if (w.knn_mode == 1) {
-    lc.begin("k_knn_thread", st); k_knn_thread<<<(unsigned)((Qt + 127) / 128), 128, 0, st>>>(sa); lc.end(st);
-  } else {
-    lc.begin("k_knn_search", st); k_knn_search<<<ns, 32 * KNN_WARPS, 0, st>>>(sa); lc.end(st);
-    if (w.tile_rings < 32) { lc.begin("k_knn_deferred", st); k_knn_deferred<<<kNumSMs * 8, 128, 0, st>>>(sa); lc.end(st); }
-  }
+  sa.knn_idx = w.knn_idx; sa.knn_sqd = w.knn_sqd; sa.store_all_sqd = w.idx5 != nullptr;
+  lc.begin("k_knn_box", st); k_knn_box<<<(unsigned)((Qt + 127) / 128), 128, 0, st>>>(sa); lc.end(st);
   FitArgs fa;
   fa.Qt = Qt; fa.pm = w.pm; fa.pmq = w.pmq; fa.knn_idx = w.knn_idx; fa.knn_sqd = w.knn_sqd; fa.gates = gates;
   fa.pts_sorted = gb.pts.p; fa.sorted_pos = gb.sorted_pos.p; fa.oth_local = oth_local; fa.oth_stride = oth_stride;

@@ -123,12 +123,7 @@ struct glio_ctx {
   DevBuf<int32_t> w_idx5;
   DevBuf<float> w_sqd5;
   DevBuf<int32_t> w_knn_idx;
-  DevBuf<uint32_t> w_deferred;
-  int tile_rings = 64;         // tuning hook: env GLIO_TILE_RINGS (>= 32: the tile pass scans all rings itself)
-  int grow_mode = 1;           // growth slabs of the box search: 1 = batched row bounds + row culling, 0 = row after row (env GLIO_KNN_GROW)
-  int knn_mode = 2;            // 2: per-thread box growth (default, fastest measured); 3: same from the own cell; 1: per-thread ring growth; 0: warp-cooperative tile pass; 4-7: the measured alternatives of knn_tile.cu (env GLIO_KNN_MODE)
   DevBuf<float> w_knn_sqd;
-  DevBuf<unsigned long long> d_stats;
   DevBuf<int> w_flags, w_pos, cell_count, cell_pos, scan_tmp;
   DevBuf<SegDesc> d_segs;
   DevBuf<CompactDst> d_dst;
@@ -224,8 +219,7 @@ void ensure_work(glio_ctx* c, int64_t Qt, bool pair, bool keep_debug) {
   c->w_pm.reserve((size_t)Qt); c->w_pmq.reserve((size_t)Qt); c->w_seg.reserve((size_t)Qt);
   c->w_status.reserve((size_t)Qt); c->w_weight.reserve((size_t)Qt);
   c->w_flags.reserve((size_t)Qt + 1); c->w_pos.reserve((size_t)Qt + 1);
-  c->w_knn_idx.reserve((size_t)Qt * 5); c->w_knn_sqd.reserve((size_t)Qt * 5); c->w_deferred.reserve((size_t)2 * Qt);
-  if (!c->d_stats.p) { c->d_stats.reserve(4); GLIO_CUDA_TRY(cudaMemsetAsync(c->d_stats.p, 0, 4 * sizeof(unsigned long long), c->st)); }
+  c->w_knn_idx.reserve((size_t)Qt * 5); c->w_knn_sqd.reserve((size_t)Qt * 5);
   if (pair) c->w_nc.reserve((size_t)Qt * 6); else c->w_nsd.reserve((size_t)Qt);
   if (keep_debug) { c->w_idx5.reserve((size_t)Qt * 5); c->w_sqd5.reserve((size_t)Qt * 5); c->w_plane.reserve((size_t)Qt * 4); }
 }
@@ -233,8 +227,7 @@ void ensure_work(glio_ctx* c, int64_t Qt, bool pair, bool keep_debug) {
 AssocWork make_work(glio_ctx* c, int64_t Qt, bool pair, bool keep_debug) {
   AssocWork w{};
   w.Qt = Qt; w.pm = c->w_pm.p; w.pmq = c->w_pmq.p; w.seg = c->w_seg.p; w.status = c->w_status.p;
-  w.knn_idx = c->w_knn_idx.p; w.knn_sqd = c->w_knn_sqd.p; w.n_fallback = c->d_stats.p;
-  w.knn_mode = c->knn_mode; w.tile_rings = c->tile_rings; w.grow_mode = c->grow_mode; w.deferred = c->w_deferred.p; w.n_deferred = reinterpret_cast<unsigned int*>(c->d_stats.p + 2);
+  w.knn_idx = c->w_knn_idx.p; w.knn_sqd = c->w_knn_sqd.p;
   w.nsd = pair ? nullptr : c->w_nsd.p; w.weight = c->w_weight.p; w.normal_cent = pair ? c->w_nc.p : nullptr;
   if (keep_debug) { w.idx5 = c->w_idx5.p; w.sqd5 = c->w_sqd5.p; w.plane = c->w_plane.p; }
   return w;
@@ -482,11 +475,7 @@ int glio_create(int device, const glio_params* params, glio_ctx** out) {
     c = new glio_ctx();
     c->device = device;
     if (params) c->prm = *params; else glio_default_params(&c->prm);
-    if (const char* e = getenv("GLIO_KNN_MODE")) { const int v = atoi(e); if (v >= 0 && v <= 7) c->knn_mode = v; }
-    if (const char* e = getenv("GLIO_KNN_GROW")) { const int v = atoi(e); if (v >= 0 && v <= 1) c->grow_mode = v; }
-    if (const char* e = getenv("GLIO_TILE_RINGS")) { const int v = atoi(e); if (v >= 1 && v < 64) c->tile_rings = v; }
     if (const char* e = getenv("GLIO_PTS_PER_CELL")) { const float v = (float)atof(e); if (v > 0.1f && v < 1000.f) c->pts_per_cell = v; }
-    c->map.build_pairs = c->knn_mode == 4;
     GLIO_CUDA_TRY(cudaStreamCreateWithFlags(&c->st, cudaStreamNonBlocking));
     GLIO_CUDA_TRY(cudaStreamCreateWithFlags(&c->st_copy, cudaStreamNonBlocking));
     GLIO_CUDA_TRY(cudaEventCreateWithFlags(&c->ev_scans, cudaEventDisableTiming));
@@ -523,7 +512,7 @@ void glio_destroy(glio_ctx* c) {
   c->cell_count.release(); c->cell_pos.release(); c->scan_tmp.release(); c->d_segs.release(); c->d_dst.release(); c->d_counts.release();
   c->h_counts.release(); c->d_bad.release(); c->d_keep.release(); c->d_items.release(); c->d_kf_item_start.release();
   c->d_partials.release(); c->d_out.release(); c->d_poses.release(); c->d_r.release(); c->d_J.release(); c->h_out.release();
-  c->h_poses.release(); c->h_flag.release(); c->d_ticket.release(); c->w_knn_idx.release(); c->w_knn_sqd.release(); c->d_stats.release(); c->w_deferred.release();
+  c->h_poses.release(); c->h_flag.release(); c->d_ticket.release(); c->w_knn_idx.release(); c->w_knn_sqd.release();
   c->f_cloud.release(); c->f_curv.release(); c->f_label.release(); c->f_picked.release(); c->f_scan.release(); c->f_ring.release(); c->f_lf.release(); c->f_counts.release(); c->f_out.release(); c->f_ds.release(); c->f_outds.release();
   c->sp_raw.release(); c->sp_ori.release(); c->sp_ring.release(); c->sp_hist.release(); c->sp_hscan.release(); c->sp_small.release();
   c->sp_scan_tmp.release(); c->sp_consts.release(); c->sp_out.release(); c->sp_hits.release();
@@ -575,17 +564,10 @@ int glio_profile_get(glio_ctx* c, const char* kernel_name, double* ms_total, int
   });
 }
 
-int glio_get_stats(glio_ctx* c, int64_t* knn_fallback_queries, int reset) {
+int glio_get_stats(glio_ctx* c, int64_t* knn_fallback_queries, int /*reset*/) {
   if (!c) return GLIO_ERR_ARG;
-  return guarded(c, [&] {
-    unsigned long long h[4] = {0, 0, 0, 0};
-    if (c->d_stats.p) {
-      GLIO_CUDA_TRY(cudaMemcpyAsync(h, c->d_stats.p, sizeof(h), cudaMemcpyDeviceToHost, c->st));
-      GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
-      if (reset) GLIO_CUDA_TRY(cudaMemsetAsync(c->d_stats.p, 0, sizeof(h), c->st));
-    }
-    if (knn_fallback_queries) *knn_fallback_queries = (int64_t)h[0];
-  });
+  if (knn_fallback_queries) *knn_fallback_queries = 0;    // the box search has no second pass
+  return GLIO_OK;
 }
 
 int glio_get_params(const glio_ctx* c, glio_params* out) {
@@ -1380,7 +1362,6 @@ int glio_batch_associate_pairs(glio_ctx* c, const int32_t* pairs_cur, const int3
       glio_ctx::Frame& fo = *c->frames[grp.first];
       if (!fo.grid_valid) {
         // world cloud of the searched frame (body pose applied directly to the stored points, quirk Q7) + its grid
-        fo.grid.build_pairs = c->knn_mode == 4;
         grid_build(fo.grid, fo.scan_ptr, fo.stride, fo.Q, fo.pose, fo.pose + 3, c->prm.cell_size, c->pts_per_cell, c->st, c->lc);
         fo.grid_valid = true;
       }
@@ -1968,7 +1949,6 @@ int glio_odom_create(glio_ctx* c, const glio_odom_options* options, glio_odom** 
                  GLIO_ERR_ARG, "glio_odom_create: need max_num_iter >= 0, 1 <= scan_match_cnt <= 8, max_solver_time_s >= 0");
     std::unique_ptr<glio_odom> o(new glio_odom());
     o->ctx = c; o->opt = opt;
-    o->grid.build_pairs = false;
     o->reset_state();
     c->odoms.push_back(o.get());
     *out = o.release();

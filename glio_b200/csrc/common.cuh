@@ -80,12 +80,6 @@ struct PinnedBuf {
 // fastest-varying cell coordinate, so the three x-adjacent cells of a (y,z) row are ONE contiguous range.
 // pts[k] = (x, y, z, bitcast(original index)).
 // ----------------------------------------------------------------------------------------------
-// Pair layout of the cell-sorted map for the staged tile search (knn_tile.cu): record k holds sorted points 2k and 2k+1
-// as (x0,x1,y0,y1 | z0,z1 | idx0,idx1) so that one 16-byte + one 8-byte shared-memory load feed the paired fp32
-// distance of two candidates; a row of cells is a contiguous, 32-byte aligned run of records (bulk-copy friendly).
-struct __align__(32) PairRec { float x0, x1, y0, y1, z0, z1; int i0, i1; };
-constexpr float PAIR_FAR = 1.0e18f;      // coordinate of a filler half-record: its squared distance (1e36) is finite and huge
-
 struct GridDesc {
   float ox, oy, oz;     // origin (min corner of cell (0,0,0))
   float cell, inv_cell;
@@ -119,12 +113,6 @@ struct AssocWork {
   uint16_t* seg;        // segment id of the query
   int32_t* knn_idx;     // [5][Qt] neighbour indices, sorted order (K1a -> K1b)
   float* knn_sqd;       // [5][Qt] squared distances, sorted order
-  unsigned long long* n_fallback;  // statistics: queries deferred from the tile pass to the single-query pass
-  int tile_rings;       // rings scanned by the tile pass before deferring (>= 32: never defer)
-  int grow_mode;        // box growth slabs: see SearchArgs::grow_mode
-  int knn_mode;         // 0: warp-cooperative tile pass, 1: per-thread ring growth, 2: per-thread box growth from 3x3x3, 3: box growth from the own cell, 4: staged tile search + team pass, 5: start box / growth in two launches, 6: far queries in a warp pass, 7: cell-by-cell start box (knn_tile.cu)
-  uint32_t* deferred;   // [Qt] sorted positions of deferred queries
-  unsigned int* n_deferred;
   uint8_t* status;
   float4* nsd;          // weight*n, weight*d   (scan-to-map)
   float* weight;
@@ -177,13 +165,11 @@ struct GridBuild {
   DevBuf<float4> pts;
   DevBuf<float4> tmp4;     // unsorted (transformed) points, original order: (x,y,z,idx)
   DevBuf<int> sorted_pos;  // original index -> position in pts (cell-sorted)
-  DevBuf<PairRec> pairs;   // pair layout of pts (built when build_pairs; knn_mode 4)
-  bool build_pairs = false;
   DevBuf<int> fill;        // scatter cursors
   DevBuf<int> scan_tmp;
   DevBuf<int> bounds;      // 6 order-preserving ints on device
   GridDesc desc{};
-  void release() { cell_start.release(); pts.release(); tmp4.release(); pairs.release(); sorted_pos.release(); fill.release(); scan_tmp.release(); bounds.release(); }
+  void release() { cell_start.release(); pts.release(); tmp4.release(); sorted_pos.release(); fill.release(); scan_tmp.release(); bounds.release(); }
 };
 void grid_build(GridBuild& gb, const float* d_xyz, int stride, int64_t n, const double* t, const double* q,
                 float cell_size_hint, float pts_per_cell, cudaStream_t st, LaunchCounter& lc);

@@ -190,19 +190,6 @@ __global__ void __launch_bounds__(256) k_cell_scatter(const float4* __restrict__
   }
 }
 
-// pair layout of the sorted map (see PairRec); the odd tail half-record is a far-away filler
-__global__ void __launch_bounds__(256) k_make_pairs(const float4* __restrict__ sorted, int64_t n, PairRec* __restrict__ pairs) {
-  const int64_t np = (n + 1) >> 1;
-  for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < np; k += (int64_t)gridDim.x * blockDim.x) {
-    const float4 a = sorted[2 * k];
-    float4 b = make_float4(PAIR_FAR, 0.f, 0.f, __int_as_float(0x7fffffff));
-    if (2 * k + 1 < n) b = sorted[2 * k + 1];
-    PairRec r;
-    r.x0 = a.x; r.x1 = b.x; r.y0 = a.y; r.y1 = b.y; r.z0 = a.z; r.z1 = b.z; r.i0 = __float_as_int(a.w); r.i1 = __float_as_int(b.w);
-    pairs[k] = r;
-  }
-}
-
 void grid_build(GridBuild& gb, const float* d_xyz, int stride, int64_t n, const double* t, const double* q,
                 float cell_size_hint, float pts_per_cell, cudaStream_t st, LaunchCounter& lc) {
   GLIO_REQUIRE(n > 0 && n < (int64_t)1 << 31, GLIO_ERR_ARG, "grid_build: point count out of range");
@@ -255,10 +242,6 @@ void grid_build(GridBuild& gb, const float* d_xyz, int stride, int64_t n, const 
   exclusive_scan_i32(gb.fill.p, gb.cell_start.p, ncell + 1, gb.scan_tmp, st, lc);
   GLIO_CUDA_TRY(cudaMemsetAsync(gb.fill.p, 0, (size_t)(ncell + 1) * sizeof(int), st));
   lc.begin("k_cell_scatter", st); k_cell_scatter<<<nb, 256, 0, st>>>(gb.tmp4.p, n, g, gb.cell_start.p, gb.fill.p, gb.pts.p, gb.sorted_pos.p); lc.end(st);
-  if (gb.build_pairs) {
-    gb.pairs.reserve((size_t)((n + 1) / 2 + 1));
-    lc.begin("k_make_pairs", st); k_make_pairs<<<nb, 256, 0, st>>>(gb.pts.p, n, gb.pairs.p); lc.end(st);
-  }
   GLIO_CUDA_TRY(cudaGetLastError());
   g.cell_start = gb.cell_start.p;
   g.pts = gb.pts.p;

@@ -1,5 +1,5 @@
-// knn_common.cuh — pieces shared by the K1a search kernels (assoc.cu, knn_tile.cu): the top-5 register list, the search
-// arguments and the paired fp32 helpers.
+// knn_common.cuh — the pieces of the K1a box search (assoc.cu k_knn_box): the top-5 register list, the search arguments
+// and the per-thread scanning helpers.  loop.cu shares the (distance, index) key.
 #pragma once
 #include "common.cuh"
 #include "devmath.cuh"
@@ -37,28 +37,6 @@ __device__ __forceinline__ void top5_push(Top5& t, float d, int id) {
   }
 }
 
-// ---- fp32 pairs for candidate PRE-FILTERS only.
-// Two points' coordinates travel as one 64-bit register pair (one 8-byte shared-memory load per pair); sm_90 has no
-// packed fp32 arithmetic, so each helper issues the two scalar instructions.  fma2 is a fused FFMA, so its results may
-// differ from the reference's unfused ((dx*dx)+dy*dy)+dz*dz by a few ulps.  They are therefore used only to reject
-// candidates that are clearly farther than a threshold (with a 1e-6 relative margin); every candidate that might
-// matter is re-evaluated with the exact scalar l2_simple() before it can enter a top-5.
-typedef unsigned long long f32x2_t;
-__device__ __forceinline__ f32x2_t pack2(float a, float b) { f32x2_t r; asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a), "f"(b)); return r; }
-__device__ __forceinline__ void unpack2(f32x2_t v, float& a, float& b) { asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v)); }
-__device__ __forceinline__ f32x2_t sub2(f32x2_t a, f32x2_t b) {
-  float a0, a1, b0, b1; unpack2(a, a0, a1); unpack2(b, b0, b1);
-  return pack2(__fsub_rn(a0, b0), __fsub_rn(a1, b1));
-}
-__device__ __forceinline__ f32x2_t mul2(f32x2_t a, f32x2_t b) {
-  float a0, a1, b0, b1; unpack2(a, a0, a1); unpack2(b, b0, b1);
-  return pack2(__fmul_rn(a0, b0), __fmul_rn(a1, b1));
-}
-__device__ __forceinline__ f32x2_t fma2(f32x2_t a, f32x2_t b, f32x2_t c) {
-  float a0, a1, b0, b1, c0, c1; unpack2(a, a0, a1); unpack2(b, b0, b1); unpack2(c, c0, c1);
-  return pack2(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
-}
-
 struct SearchArgs {
   GridDesc grid;
   int64_t Qt;
@@ -68,11 +46,6 @@ struct SearchArgs {
   int32_t* knn_idx;     // [5][Qt] sorted order
   float* knn_sqd;       // [5][Qt] sorted order; rows 0..3 are written only when store_all_sqd (the gate needs the 5th only)
   bool store_all_sqd;
-  int grow_mode;        // box growth slabs: 0 = row after row, 1 = row bounds fetched nine at a time + rows beyond the 5th distance skipped (GLIO_KNN_GROW)
-  unsigned long long* n_fallback;   // statistics: queries deferred to the second pass
-  int tile_rings;                   // (mode 0) rings the tile pass may scan before it defers a query
-  uint32_t* deferred;               // sorted positions of deferred queries
-  unsigned int* n_deferred;
 };
 
 __device__ __forceinline__ void store_top5(const SearchArgs& a, int64_t p, const Top5& t) {
@@ -86,7 +59,7 @@ __device__ __forceinline__ void store_top5(const SearchArgs& a, int64_t p, const
 }
 
 
-// ---- per-thread scanning helpers shared by the box-growth kernels (assoc.cu k_knn_box, knn_tile.cu k_knn_box_start / k_knn_grow)
+// ---- per-thread scanning helpers of the box search
 __device__ __forceinline__ void scan_range_keys(const float4* __restrict__ pts, int s, int e, float qx, float qy, float qz, Top5& t, float& d4f) {
   for (int k = s; k < e; ++k) {
     const float4 p = __ldg(&pts[k]);
@@ -98,75 +71,28 @@ __device__ __forceinline__ void scan_range_keys(const float4* __restrict__ pts, 
   }
 }
 
-// rings [r_lo, r_hi] of one query's search box; returns true when the top-5 is final (proven inside the scanned box,
-// the box covers the grid, or it covers the gate radius) and false when more rings are needed
-__device__ __forceinline__ bool thread_rings(const GridDesc& g, float qx, float qy, float qz, int cx, int cy, int cz, int r_lo, int r_hi, int rmax,
-                                             Top5& t, float& d4f, int* __restrict__ sb = nullptr) {
-  const float INF = __int_as_float(0x7f800000);
+// the 3x3x3 start box around the query's cell (cx, cy, cz): fetch the bounds of all nine rows up front (18 independent
+// loads in flight instead of nine dependent load -> scan steps), park them in this thread's shared-memory column, then
+// scan the query's own row first so the 5th distance tightens early
+__device__ __forceinline__ void scan_start_box(const GridDesc& g, float qx, float qy, float qz, int cx, int cy, int cz, Top5& t, float& d4f,
+                                               int* __restrict__ sb) {
   const int* __restrict__ cs = g.cell_start;
-  for (int r = r_lo; r <= r_hi; ++r) {
-    const int xa = cx - r, xb = cx + r;
-    const int x0 = max(xa, 0), x1 = min(xb, g.nx - 1);
-    if (r == 1 && sb) {
-      // first ring: fetch the bounds of all nine rows up front (18 independent loads in flight instead of nine
-      // dependent load -> scan steps), park them in this thread's shared-memory column, then scan the query's own
-      // row first so the 5th distance tightens early
+  const int x0 = max(cx - 1, 0), x1 = min(cx + 1, g.nx - 1);
 #pragma unroll
-      for (int i = 0; i < 9; ++i) {
-        const int z = cz + i / 3 - 1, y = cy + i % 3 - 1;
-        int s = 0, e = 0;
-        if (z >= 0 && z < g.nz && y >= 0 && y < g.ny && x0 <= x1) { const int row = (z * g.ny + y) * g.nx; s = __ldg(&cs[row + x0]); e = __ldg(&cs[row + x1 + 1]); }
-        sb[(2 * i) * 128] = s; sb[(2 * i + 1) * 128] = e;
-      }
-#pragma unroll 1
-      for (int i = 0; i < 9; ++i) {
-        const int o = (int)((0x862053714ull >> (4 * i)) & 15ull);     // 4,1,7,3,5,0,2,6,8
-        scan_range_keys(g.pts, sb[(2 * o) * 128], sb[(2 * o + 1) * 128], qx, qy, qz, t, d4f);
-      }
-    } else {
-      const int z0 = max(cz - r, 0), z1 = min(cz + r, g.nz - 1);
-      const int y0 = max(cy - r, 0), y1 = min(cy + r, g.ny - 1);
-      for (int z = z0; z <= z1; ++z) {
-        const bool zshell = (z == cz - r) || (z == cz + r);
-        for (int y = y0; y <= y1; ++y) {
-          const int row = (z * g.ny + y) * g.nx;
-          const bool shell = r == 1 || zshell || (y == cy - r) || (y == cy + r);
-          if (shell) {
-            if (x0 <= x1) scan_range_keys(g.pts, __ldg(&cs[row + x0]), __ldg(&cs[row + x1 + 1]), qx, qy, qz, t, d4f);
-          } else {
-            if (xa >= 0 && xa < g.nx) scan_range_keys(g.pts, __ldg(&cs[row + xa]), __ldg(&cs[row + xa + 1]), qx, qy, qz, t, d4f);
-            if (xb >= 0 && xb < g.nx) scan_range_keys(g.pts, __ldg(&cs[row + xb]), __ldg(&cs[row + xb + 1]), qx, qy, qz, t, d4f);
-          }
-        }
-      }
-    }
-    float b = INF;
-    if (cx - r > 0)        b = fminf(b, qx - (g.ox + (float)(cx - r) * g.cell));
-    if (cx + r < g.nx - 1) b = fminf(b, (g.ox + (float)(cx + r + 1) * g.cell) - qx);
-    if (cy - r > 0)        b = fminf(b, qy - (g.oy + (float)(cy - r) * g.cell));
-    if (cy + r < g.ny - 1) b = fminf(b, (g.oy + (float)(cy + r + 1) * g.cell) - qy);
-    if (cz - r > 0)        b = fminf(b, qz - (g.oz + (float)(cz - r) * g.cell));
-    if (cz + r < g.nz - 1) b = fminf(b, (g.oz + (float)(cz + r + 1) * g.cell) - qz);
-    if (b == INF) return true;
-    const float bs = b * 0.999f - 2e-3f;
-    if (bs > 0.f && key_dist(t.k4) <= bs * bs) return true;
+  for (int i = 0; i < 9; ++i) {
+    const int z = cz + i / 3 - 1, y = cy + i % 3 - 1;
+    int s = 0, e = 0;
+    if (z >= 0 && z < g.nz && y >= 0 && y < g.ny && x0 <= x1) { const int row = (z * g.ny + y) * g.nx; s = __ldg(&cs[row + x0]); e = __ldg(&cs[row + x1 + 1]); }
+    sb[(2 * i) * 128] = s; sb[(2 * i + 1) * 128] = e;
   }
-  return r_hi >= rmax;
+#pragma unroll 1
+  for (int i = 0; i < 9; ++i) {
+    const int o = (int)((0x862053714ull >> (4 * i)) & 15ull);     // 4,1,7,3,5,0,2,6,8
+    scan_range_keys(g.pts, sb[(2 * o) * 128], sb[(2 * o + 1) * 128], qx, qy, qz, t, d4f);
+  }
 }
 
-__device__ __forceinline__ void scan_rows(const GridDesc& g, int x0, int x1, int y0, int y1, int z0, int z1, float qx, float qy, float qz, Top5& t, float& d4f) {
-  x0 = max(x0, 0); x1 = min(x1, g.nx - 1); y0 = max(y0, 0); y1 = min(y1, g.ny - 1); z0 = max(z0, 0); z1 = min(z1, g.nz - 1);
-  if (x0 > x1) return;
-  const int* __restrict__ cs = g.cell_start;
-  for (int z = z0; z <= z1; ++z)
-    for (int y = y0; y <= y1; ++y) {
-      const int row = (z * g.ny + y) * g.nx;
-      scan_range_keys(g.pts, __ldg(&cs[row + x0]), __ldg(&cs[row + x1 + 1]), qx, qy, qz, t, d4f);
-    }
-}
-
-
-// The same slab scan for the growth phase, restructured for the queries that have to look far (sparse map around them, most
+// The slab scan of the growth phase, built for the queries that have to look far (sparse map around them, most
 // rows empty): (1) a row whose cells are provably farther than the current 5th distance is skipped without touching memory -
 // the same margins as the face test, strict inequality, so nothing that could enter the top-5 (ties included) is skipped;
 // (2) the bounds of up to eight surviving rows are fetched together (18 independent loads in flight) and parked in the thread's
@@ -228,7 +154,7 @@ __device__ __forceinline__ bool box_face_open(const GridDesc& g, int f, float qx
 }
 // face-by-face growth of the searched box [lx,hx] x [ly,hy] x [lz,hz] until no face is open (see k_knn_box)
 __device__ __forceinline__ void box_grow(const GridDesc& g, float qx, float qy, float qz, float gate_r, int rmax, int lx, int hx, int ly, int hy, int lz, int hz,
-                                         Top5& t, float& d4f, int* __restrict__ sb = nullptr) {
+                                         Top5& t, float& d4f, int* __restrict__ sb) {
   for (int round = 0; round < rmax + 3; ++round) {
     bool any = false;
 #pragma unroll 1
@@ -242,19 +168,11 @@ __device__ __forceinline__ void box_grow(const GridDesc& g, float qx, float qy, 
       if (ax == 0) { bx0 = bx1 = nc; if (up) hx = nc; else lx = nc; }
       else if (ax == 1) { by0 = by1 = nc; if (up) hy = nc; else ly = nc; }
       else { bz0 = bz1 = nc; if (up) hz = nc; else lz = nc; }
-      if (sb) scan_rows_batched(g, bx0, bx1, by0, by1, bz0, bz1, qx, qy, qz, t, d4f, sb);
-      else scan_rows(g, bx0, bx1, by0, by1, bz0, bz1, qx, qy, qz, t, d4f);
+      scan_rows_batched(g, bx0, bx1, by0, by1, bz0, bz1, qx, qy, qz, t, d4f, sb);
       any = true;
     }
     if (!any) break;
   }
 }
-
-// K1a, staged tile search + team pass (knn_tile.cu, GLIO_KNN_MODE=4)
-void knn_tile_run(const SearchArgs& sa, const PairRec* d_pairs, DevBuf<int>& work, DevBuf<int>& scan_tmp, cudaStream_t st, LaunchCounter& lc);
-// K1a, box search split in two launches (GLIO_KNN_MODE=5): start box for everyone, face growth for the compacted rest
-void knn_box_far_run(const SearchArgs& sa, cudaStream_t st, LaunchCounter& lc);      // GLIO_KNN_MODE=6
-void knn_box_cells_run(const SearchArgs& sa, cudaStream_t st, LaunchCounter& lc);    // GLIO_KNN_MODE=7
-void knn_box2_run(const SearchArgs& sa, DevBuf<int>& work, DevBuf<int>& scan_tmp, cudaStream_t st, LaunchCounter& lc);
 
 }  // namespace glio

@@ -78,10 +78,8 @@ int64_t glio_launch_count(const glio_ctx* ctx);
 
 /* per-kernel device time: when enabled every launch is bracketed by CUDA events on the context's stream;
  * glio_profile_get sums the elapsed time of all launches of the named kernel since profiling was enabled
- * (names: K0 k_init_bounds, k_load_bounds, k_cell_hist, k_cell_scatter, k_make_pairs, k_scan_block, k_scan_add;
- * K1 k_transform_hist, k_order_scatter, k_knn_box [GLIO_KNN_MODE 2, default] | k_knn_thread [1] | k_knn_search + k_knn_deferred [0]
- * | k_knn_tile + k_defer_scatter + k_knn_tile2 + k_knn_team [4] | k_knn_box_start + k_knn_grow [5] | k_knn_box_far + k_knn_far [6]
- * | k_knn_box_cells [7], k_plane_fit, k_plane_fit_pair, k_flags, k_compact;
+ * (names: K0 k_init_bounds, k_load_bounds, k_cell_hist, k_cell_scatter, k_scan_block, k_scan_add;
+ * K1 k_transform_hist, k_order_scatter, k_knn_box, k_plane_fit, k_plane_fit_pair, k_flags, k_compact;
  * K2 k_eval_unary, k_eval_unary_cost, k_eval_binary, k_eval_binary_cost, k_bin_assemble; local map k_lm_transform, k_vox_*;
  * front end k_feat_curvature, k_feat_select, k_feat_voxel, k_feat_offsets, k_feat_gather; sweep preparation k_sp_bounds,
  * k_sp_consts, k_sp_classify, k_sp_ranges, k_sp_emit; odometry k_odom_publish; loop-closure registration k_lc_load, k_lc_qhist,
@@ -89,7 +87,8 @@ int64_t glio_launch_count(const glio_ctx* ctx);
  * k_lc_fitness). */
 int glio_profile_enable(glio_ctx* ctx, int on);
 int glio_profile_get(glio_ctx* ctx, const char* kernel_name, double* ms_total, int64_t* launches);
-/* statistics: number of queries a first search pass handed to its second pass (GLIO_KNN_MODE 0 and 4; 0 in the default mode) */
+/* statistics: number of queries a first kNN search pass handed to a second pass.  The box search has no second pass, so
+ * this always reports 0 and `reset` is ignored; the entry point is kept for existing callers. */
 int glio_get_stats(glio_ctx* ctx, int64_t* knn_fallback_queries, int reset);
 /* vec_surf_res_cnt for slots 0..W-1 (all matches) and the number currently active (after glio_select) */
 int glio_get_match_counts(glio_ctx* ctx, int W, int64_t* n_match, int64_t* n_active);

@@ -9,7 +9,3 @@ $B --steps 20 --warmup 3 > gpurun_out/bench_line.json 2> gpurun_out/bench_line.e
 ncu --metrics gpu__time_duration.sum --clock-control none -s 300 -c 400 --csv --log-file gpurun_out/launches.csv $B --steps 4 --warmup 3 > gpurun_out/b_under_ncu.log 2>&1
 # (3) the dominant kernels, --set full (default search: k_knn_box)
 ncu --set full --clock-control none --import-source on -k regex:"k_knn_box|k_plane_fit|k_eval_unary" -s 18 -c 6 -o gpurun_out/prof_top $B --steps 2 --warmup 3 > gpurun_out/ncu_top.log 2>&1
-# (4) the staged tile search (GLIO_KNN_MODE=4): the north_star design, kept behind the switch
-GLIO_KNN_MODE=4 ncu --set full --clock-control none --import-source on -k regex:"k_knn_tile|k_knn_tile2|k_knn_team" -s 9 -c 3 -o gpurun_out/prof_tile $B --steps 2 --warmup 3 > gpurun_out/ncu_tile.log 2>&1
-SWEEP="8:2,8:4,12:4" python scripts/sweep_knn.py > gpurun_out/sweep_modes.log 2>&1
-tail -2 gpurun_out/ncu_top.log gpurun_out/ncu_tile.log; cat gpurun_out/sweep_modes.log

@@ -1,5 +1,5 @@
 """K1a tuning sweep at BASELINE cfg 2 sizes: per-kernel times (library launch-event profiler) for several
-(points-per-cell, GLIO_KNN_MODE[, GLIO_KNN_GROW]) settings given as SWEEP="ppc:mode[:grow],...", each checked bit-for-bit against the first.
+points-per-cell settings given as SWEEP="ppc,...", each checked bit-for-bit against the first.
 Not a bench value."""
 import sys, os, hashlib
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -9,21 +9,17 @@ from glio_b200 import api, synth
 W, Q, M = int(os.environ.get("W", 20)), int(os.environ.get("Q", 100000)), int(os.environ.get("M", 1000000))
 P = synth.window_problem(W=W, Q=Q, M=M)
 dmap = torch.from_numpy(P["map_xyz"]).cuda(); dscans = [torch.from_numpy(s).cuda() for s in P["scans"]]
-cfgs = [c.split(":") for c in os.environ.get("SWEEP", "8:1,8:2,8:3,6:2,12:2").split(",")]
 ref = None
-for cfg in cfgs:
-    ppc, mode = cfg[0], cfg[1]; grow = cfg[2] if len(cfg) > 2 else "1"
-    os.environ["GLIO_PTS_PER_CELL"] = ppc; os.environ["GLIO_KNN_MODE"] = mode; os.environ["GLIO_KNN_GROW"] = grow
+for ppc in os.environ.get("SWEEP", "8,6,12").split(","):
+    os.environ["GLIO_PTS_PER_CELL"] = ppc
     ctx = api.Context(0)
     ctx.set_map(dmap); ctx.window_set_scans(dscans)
     nm = ctx.window_associate(P["poses_init"])          # warm-up
-    ctx.knn_fallback_queries(reset=True)
     ctx.lib_profile(True)
     for _ in range(4):
         nm = ctx.window_associate(P["poses_init"])
     ctx.synchronize()
     prof = ctx.lib_profile_read(); ctx.lib_profile(False)
-    nfb = ctx.knn_fallback_queries() // 4
     h = hashlib.sha256()
     for s in (0, W // 2, W - 1):
         m = ctx.get_matches(s, int(nm[s]))
@@ -34,5 +30,5 @@ for cfg in cfgs:
     same = dig == ref[0] and np.array_equal(nm, ref[1])
     line = " ".join("%s=%.3f" % (k.replace("k_", ""), v[0] / v[1]) for k, v in prof.items() if k.startswith("k_knn") or k.startswith("k_plane") or k in ("k_transform_hist", "k_order_scatter"))
     knn = sum(v[0] / v[1] for k, v in prof.items() if k.startswith("k_knn"))
-    print("mode=%s grow=%s ppc=%s knn_total=%.3f ms exact=%s deferred=%d | %s" % (mode, grow, ppc, knn, same, nfb, line), flush=True)
+    print("ppc=%s knn_total=%.3f ms exact=%s | %s" % (ppc, knn, same, line), flush=True)
     ctx.close()

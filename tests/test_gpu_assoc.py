@@ -100,13 +100,10 @@ def test_map_prefetch_equals_inline_upload(ctx, oracle):
         assert np.array_equal(d0[k], d1[k]) and np.array_equal(d0[k], d2[k])
 
 
-@pytest.mark.parametrize("mode,grow", [(0, 1), (1, 1), (2, 0), (2, 1), (3, 1), (4, 1), (5, 1), (6, 1), (7, 1)])
-def test_every_search_variant_is_bit_exact(oracle, mode, grow, monkeypatch):
-    """every K1a variant kept behind GLIO_KNN_MODE / GLIO_KNN_GROW (the default box search, ring growth, the warp-cooperative and
-    the bulk-copy staged tile searches, the split / far-query / cell-by-cell variants) gives the oracle's association bit for bit;
-    the pose error is large enough that the growth and second-pass paths of each variant run"""
+def test_displaced_keyframe_search_is_bit_exact(oracle):
+    """the K1a box search gives the oracle's association bit for bit when one keyframe is displaced: the pose error is large
+    enough that many queries grow their box beyond the 3x3x3 start box"""
     from glio_b200 import api
-    monkeypatch.setenv("GLIO_KNN_MODE", str(mode)); monkeypatch.setenv("GLIO_KNN_GROW", str(grow))
     P = synth.window_problem(W=3, Q=6000, M=120000, seed=91)
     poses = P["poses_init"].copy()
     poses[1, :3] += [0.35, -0.2, 0.15]                      # displaced keyframe: many queries leave their start box
