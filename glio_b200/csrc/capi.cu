@@ -1029,6 +1029,23 @@ int glio_extract_features(glio_ctx* c, const float* cloud_xyzi, int64_t n, int s
     GLIO_REQUIRE(stride >= 4 && stride <= 64 && intensity_offset >= 3 && intensity_offset < stride, GLIO_ERR_ARG, "glio_extract_features: stride_floats must be >= 4 and 3 <= intensity_offset < stride");
     GLIO_REQUIRE(n_scans > 0 && n_scans <= 1024 && scan_start && scan_end && ds_rate >= 1 && ds_v > 0.f, GLIO_ERR_ARG, "glio_extract_features: bad ring table");
     for (int r = 0; r < n_scans; ++r) GLIO_REQUIRE(scan_start[r] >= 5 && scan_end[r] < n - 5 && scan_end[r] - scan_start[r] < n, GLIO_ERR_ARG, "glio_extract_features: ring range outside [5, n-6]");
+    {
+      // the processed rings run concurrently (one CTA each): a ring's neighbour suppression marks points up to 5 past its
+      // range, so ordered by start the next processed ring must begin at least 5 points after the previous one ends
+      std::vector<std::pair<int32_t, int>> used;
+      for (int r = 0; r < n_scans; r += ds_rate)
+        if (scan_end[r] - scan_start[r] >= 6) used.push_back({scan_start[r], r});
+      std::sort(used.begin(), used.end());
+      for (size_t k = 1; k < used.size(); ++k) {
+        const int p = used[k - 1].second, q = used[k].second;
+        if (scan_start[q] < scan_end[p] + 5) {
+          char b[256];
+          snprintf(b, sizeof(b), "glio_extract_features: rings %d [%d, %d] and %d [%d, %d] %s (processed rings need scan_start >= previous scan_end + 5)",
+                   p, scan_start[p], scan_end[p], q, scan_start[q], scan_end[q], scan_start[q] < scan_end[p] ? "overlap" : "are closer than 5 points");
+          throw Error{GLIO_ERR_ARG, b};
+        }
+      }
+    }
     FeatArgs a{};
     const float* d_cloud = cloud_xyzi;
     if (mem != GLIO_DEVICE) { c->f_cloud.reserve((size_t)n * stride); GLIO_CUDA_TRY(cudaMemcpyAsync(c->f_cloud.p, cloud_xyzi, (size_t)n * stride * sizeof(float), cudaMemcpyHostToDevice, c->st)); d_cloud = c->f_cloud.p; }

@@ -4,9 +4,12 @@
 //   k_feat_curvature  LOAM curvature of every point: |sum of the ten ring neighbours - 10 p|^2, float, the reference's
 //                     left-to-right order (:537-546)
 //   k_feat_select     one CTA per ring; the six sectors of a ring in order (their neighbour suppression reaches up to five
-//                     points into the next sector, so sectors of a ring are sequential; rings are independent: an 11-point
-//                     gap separates their processed ranges): bitonic sort of the sector by (curvature, index) in shared
-//                     memory, then the greedy pick of <= 2 sharp + <= 8 more less-sharp edge points from the top and <= 4
+//                     points into the next sector, so sectors of a ring are sequential; rings run concurrently, which is
+//                     the reference's sequential order only while no ring reads what another writes: a ring marks
+//                     picked[] from scan_start - 5 to scan_end + 4 and reads and compacts within [scan_start, scan_end), so
+//                     glio_extract_features refuses processed rings whose ranges, ordered by start, are less than 5 points
+//                     apart (scan_start[next] < scan_end[prev] + 5); the reference's layout leaves 11): bitonic sort of
+//                     the sector by (curvature, index) in shared memory, then the greedy pick of <= 2 sharp + <= 8 more less-sharp edge points from the top and <= 4
 //                     flat points from the bottom with the +-5 suppression (:549-643), then the ordered compaction of the
 //                     remaining label <= 0 points as "less flat" (:645-650)
 //   k_feat_voxel      one CTA per ring: pcl::VoxelGrid (leaf ds_v) of the ring's less-flat points, all in shared memory:

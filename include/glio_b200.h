@@ -266,8 +266,10 @@ int glio_hf_evaluate(void* user, int W, const double* poses, const double* speed
  * cloud_xyzi = `laserCloud` of the reference: the scan lines concatenated ring after ring, x,y,z,intensity at stride_floats
  * (>= 4) with the intensity at float intensity_offset (packed x,y,z,i: stride 4, offset 3; pcl::PointXYZI: stride 8, offset 4),
  * scan_start / scan_end = scanStartInd / scanEndInd per ring (:529-534; every range inside
- * [5, n-6]).  Outputs, any may be NULL: cloudCurvature[n], cloudLabel[n] (2 sharp, 1 less sharp, -1 flat, 0 other), and the
- * four feature sets in the reference's push_back order as indices into the cloud (cornerPointsSharp, cornerPointsLessSharp,
+ * [5, n-6]).  The processed rings (scan_end - scan_start >= 6 and ring % ds_rate == 0) run concurrently, so ordered by
+ * scan_start each must begin at least 5 points after the previous one's scan_end (the reference's layout leaves 11); a table
+ * with processed rings closer than that, or overlapping, is refused with GLIO_ERR_ARG naming the two rings.
+ * Outputs, any may be NULL: cloudCurvature[n], cloudLabel[n] (2 sharp, 1 less sharp, -1 flat, 0 other), and the four feature sets in the reference's push_back order as indices into the cloud (cornerPointsSharp, cornerPointsLessSharp,
  * surfPointsFlat, the less-flat points BEFORE the voxel filter) plus surfPointsLessFlat itself (x,y,z,intensity after the
  * per-ring pcl::VoxelGrid of leaf ds_v).  Equal curvatures are ordered by index (std::sort leaves it open). */
 int glio_extract_features(glio_ctx* ctx, const float* cloud_xyzi, int64_t n, int stride_floats, int intensity_offset, int mem, int n_scans, const int32_t* scan_start,
