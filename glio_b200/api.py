@@ -264,6 +264,15 @@ class Context:
         self._chk(self._lib.glio_select(self._h, C.c_int(slot), _ptr(k), C.c_int64(len(k))))
 
     # ---- K2
+    def set_matches(self, slot, cp, nsd, weight):
+        """glio_set_matches: upload a slot's plane correspondences as they are (cp (n, 3), nsd (n, 4) = (n, d), weight (n,),
+        all float32) instead of associating them; score = lidar_const * weight."""
+        cp = np.ascontiguousarray(cp, np.float32).reshape(-1, 3); nsd = np.ascontiguousarray(nsd, np.float32).reshape(-1, 4)
+        w = np.ascontiguousarray(weight, np.float32).ravel()
+        if not (len(cp) == len(nsd) == len(w)):
+            raise ValueError("cp, nsd and weight must have the same length")
+        self._chk(self._lib.glio_set_matches(self._h, C.c_int(slot), _ptr(cp), _ptr(nsd), _ptr(w), C.c_int64(len(w))))
+
     def eval_unary(self, poses_body, jac_kind=0, want_jac=True):
         pb = np.ascontiguousarray(poses_body, np.float64).reshape(-1, 7)
         W = len(pb)

@@ -394,14 +394,19 @@ void fill_summary(const SolverSummary& S, int n, glio_solver_summary* summary, g
 // device evaluation of all active unary residuals -> c->h_out (W x 28: 21 upper-tri H, 6 g, 1 cost), synchronised
 // launch half: returns the epoch to wait for (0: nothing was launched, h_out already holds zeros).  tgt = nullptr evaluates the
 // context's own slots with its glio_params; otherwise the target's items and constants (the odometry's).
-unsigned int eval_unary_launch(glio_ctx* c, int W, const double* poses_body, int jac_kind, bool want_jac, const EvalTarget* tgt = nullptr) {
-  if (c->marg_pending) {            // an asynchronous marginalisation still owns the result buffer until its worker has copied it
-    while (!c->marg_pending->copied.load(std::memory_order_acquire)) {
+// An asynchronous marginalisation owns the pinned pose and result buffers (h_poses, h_out) until its worker has copied the
+// device result: its kernel (and, above EV_MAXW keyframes, its pose upload) may still be queued.  Wait for that copy.
+void wait_marg_copied(glio_ctx* c) {
+  if (!c->marg_pending) return;
+  while (!c->marg_pending->copied.load(std::memory_order_acquire)) {
 #if defined(__x86_64__)
-      __builtin_ia32_pause();
+    __builtin_ia32_pause();
 #endif
-    }
   }
+}
+
+unsigned int eval_unary_launch(glio_ctx* c, int W, const double* poses_body, int jac_kind, bool want_jac, const EvalTarget* tgt = nullptr) {
+  wait_marg_copied(c);
   EvalTarget own{};
   if (!tgt) {
     build_items(c, W);
@@ -1315,6 +1320,7 @@ int glio_eval_unary_residuals(glio_ctx* c, int slot, const double pose_body[7], 
     if (n_out) *n_out = n;
     GLIO_REQUIRE(capacity >= n, GLIO_ERR_ARG, "capacity smaller than the residual count");
     if (n == 0) return;
+    wait_marg_copied(c);               // h_poses may still feed a pending marginalisation's upload
     c->d_r.reserve(n); c->d_J.reserve(6 * n); c->d_poses.reserve(7); c->h_poses.reserve(7);
     memcpy(c->h_poses.p, pose_body, 7 * sizeof(double));
     GLIO_CUDA_TRY(cudaMemcpyAsync(c->d_poses.p, c->h_poses.p, 7 * sizeof(double), cudaMemcpyHostToDevice, c->st));
@@ -1496,7 +1502,7 @@ void build_bin_items(glio_ctx* c, int K) {
   std::vector<std::vector<BinIncidence>> inc(K);
   for (int p = 0; p < P; ++p) {
     glio_ctx::Pair& pr = *c->pairs[p];
-    GLIO_REQUIRE(pr.cur < K && pr.oth < K, GLIO_ERR_ARG, "pair references a keyframe >= K");
+    GLIO_REQUIRE(pr.cur >= 0 && pr.oth >= 0 && pr.cur < K && pr.oth < K, GLIO_ERR_ARG, "pair references a keyframe outside [0, K)");
     pstart[p] = (int)items.size();
     const bool sel = pr.n_sel >= 0;
     const int64_t n = sel ? pr.n_sel : pr.n_match;
@@ -1584,6 +1590,11 @@ int glio_set_allreduce(glio_ctx* c, glio_allreduce_fn fn, void* user) {
 int glio_batch_declare_pairs(glio_ctx* c, const int32_t* pairs_cur, const int32_t* pairs_oth, int64_t n_pairs) {
   if (!c) return GLIO_ERR_ARG;
   return guarded(c, [&] {
+    // validate the whole list first: a refused call leaves the pair list as it was
+    GLIO_REQUIRE(n_pairs >= 0 && (n_pairs == 0 || (pairs_cur && pairs_oth)), GLIO_ERR_ARG, "glio_batch_declare_pairs: null pair arrays");
+    for (int64_t i = 0; i < n_pairs; ++i)
+      GLIO_REQUIRE(pairs_cur[i] >= 0 && pairs_oth[i] >= 0 && pairs_cur[i] != pairs_oth[i], GLIO_ERR_ARG,
+                   "glio_batch_declare_pairs: pair indices must be >= 0 and distinct");
     for (int64_t i = 0; i < n_pairs; ++i) {
       const std::pair<int, int> key(pairs_cur[i], pairs_oth[i]);
       if (c->pair_index.count(key)) continue;

@@ -549,7 +549,9 @@ int glio_batch_clear(glio_ctx* ctx);
 
 /* Creates (empty) pair entries in the given order without associating them: on a keyframe-sharded multi-GPU run
  * every rank declares the SAME global pair list and then associates only the pairs it owns, so the block
- * buffers have one layout everywhere. */
+ * buffers have one layout everywhere.  Every pair needs cur >= 0, oth >= 0 and cur != oth (the rule of
+ * glio_batch_set_pair_matches), and n_pairs > 0 needs both arrays; otherwise the call returns GLIO_ERR_ARG and
+ * leaves the pair list unchanged.  Pairs already declared are kept in place. */
 int glio_batch_declare_pairs(glio_ctx* ctx, const int32_t* pairs_cur, const int32_t* pairs_oth, int64_t n_pairs);
 
 /* Upload the matches of pair (cur, oth) instead of associating them (creates the pair when it does not exist yet) - the
