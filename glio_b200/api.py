@@ -205,6 +205,23 @@ class Context:
         self._chk(self._lib.glio_get_map(self._h, C.c_int64(len(out)), _ptr(out), C.byref(n)))
         return out
 
+    def voxel_filter(self, xyz, leaf, out="host"):
+        """pcl::VoxelGrid(leaf) of any cloud on the device (glio_voxel_filter; downSampleCloud's ds_filter_surf, Estimator.cpp:3628-3630).
+        xyz: (n, stride) float32 numpy array or CUDA tensor with x, y, z in columns 0..2.  Returns (points (m, 3) float32, filtered):
+        filtered is False when PCL's leaf-size check passed the input through.  With out="device" the points are a CUDA tensor that
+        window_set_scan and LoopClosure.add_keyframe take as they are."""
+        if out not in ("host", "device"):
+            raise ValueError("out must be 'host' or 'device'")
+        if _npts(xyz):
+            keep, p, n, stride, mem = _points_arg(xyz)
+        else:
+            p, n, stride, mem = None, 0, 3, HOST
+        buf, optr, omem = _vs_output(self, n, out)
+        m = C.c_int64(0); f = C.c_int32(0)
+        self._chk(self._lib.glio_voxel_filter(self._h, p, C.c_int64(n), C.c_int(stride), C.c_int(mem), C.c_float(leaf), C.c_int64(n), optr,
+                                              C.c_int(omem), C.byref(m), C.byref(f)))
+        return buf[:m.value], bool(f.value)
+
     def assoc_scan_to_map(self, slot, scan_xyz, t, q):
         keep, p, n, stride, mem = _points_arg(scan_xyz)
         self._keep.append(keep); self._keep = self._keep[-64:]
@@ -943,6 +960,19 @@ def _npts(a):
     return a is not None and (a.shape[0] if hasattr(a, "shape") else len(a)) > 0
 
 
+def _vs_output(ctx, n, out):
+    """room for n packed x,y,z points: a numpy array, or a CUDA tensor on the context's GPU"""
+    if out == "device":
+        import torch
+        dev = torch.device("cuda", ctx.device)
+        buf = torch.empty((max(n, 1), 3), dtype=torch.float32, device=dev)
+        # torch's allocator hands the memory out on torch's stream, the library writes it on the context's: let torch finish first
+        torch.cuda.current_stream(dev).synchronize()
+        return buf, C.c_void_p(buf.data_ptr()), DEVICE
+    buf = np.empty((n, 3), np.float32)
+    return buf, _ptr(buf), HOST
+
+
 Context.icp_align = _icp_align
 
 
@@ -955,6 +985,7 @@ class LoopClosure:
         self._lib = ctx._lib
         self.options = default_loop_options(**options)
         self._h = C.c_void_p()
+        self._sizes = []                                   # keyframe cloud sizes: the global map's capacity
         ctx._chk(self._lib.glio_loop_create(ctx._h, C.byref(self.options), C.byref(self._h)))
 
     def close(self):
@@ -970,6 +1001,7 @@ class LoopClosure:
 
     def reset(self):
         self.ctx._chk(self._lib.glio_loop_reset(self._h))
+        self._sizes = []
 
     def __len__(self):
         n = C.c_int(0)
@@ -986,7 +1018,21 @@ class LoopClosure:
         idx = C.c_int32(0)
         self.ctx._chk(self._lib.glio_loop_add_keyframe(self._h, p, C.c_int64(n), C.c_int(stride), C.c_int(mem), _ptr(ps), C.c_double(time),
                                                        C.byref(idx)))
+        self._sizes.append(int(n))
         return int(idx.value)
+
+    def global_map(self, interval=3, leaf=0.2, out="host"):
+        """save_pcd's global map (glio_loop_global_map, Estimator.cpp:5324-5349): keyframes 0, interval, ... moved by Tbl then by their
+        current pose, concatenated, VoxelGrid(leaf).  Returns (points (m, 3) float32, filtered, n_raw): filtered is False when PCL's
+        leaf-size check passed the concatenation (n_raw points) through.  out="device" returns a CUDA tensor."""
+        if out not in ("host", "device"):
+            raise ValueError("out must be 'host' or 'device'")
+        cap = sum(self._sizes[::interval]) if interval >= 1 else 0
+        buf, optr, omem = _vs_output(self.ctx, cap, out)
+        m = C.c_int64(0); raw = C.c_int64(0); f = C.c_int32(0)
+        self.ctx._chk(self._lib.glio_loop_global_map(self._h, C.c_int(interval), C.c_float(leaf), C.c_int64(cap), optr, C.c_int(omem), C.byref(m),
+                                                     C.byref(raw), C.byref(f)))
+        return buf[:m.value], bool(f.value), int(raw.value)
 
     def set_poses(self, first, poses):
         ps = np.ascontiguousarray(poses, np.float64).reshape(-1, 7)
@@ -1016,3 +1062,4 @@ class LoopClosure:
 
 Context.KERNELS = Context.KERNELS + ["k_lc_load", "k_lc_qhist", "k_lc_qscatter", "k_lc_init", "k_lc_nn", "k_lc_compact", "k_lc_sum0",
                                      "k_lc_sum1", "k_lc_means", "k_lc_solve", "k_lc_transform", "k_lc_final", "k_lc_fitness"]
+Context.KERNELS = Context.KERNELS + ["k_vs_key", "k_vs_hist", "k_vs_scatter", "k_vs_heads", "k_vs_centroid", "k_vs_pack", "k_gm_transform"]

@@ -152,6 +152,9 @@ struct glio_ctx {
   // loop-closure registration: glio_icp_align's work space and staging, and the loop objects created on this context
   IcpWork icp; DevBuf<float> icp_src, icp_tgt;
   std::vector<glio_loop*> loops;
+  // sort-based VoxelGrid of glio_voxel_filter and glio_loop_global_map: its own work space, host-input staging, the global map's
+  // concatenation and segment table
+  VoxelSortWork vsort; DevBuf<float> vs_stage; DevBuf<float4> gm_cat; DevBuf<GlobalMapSeg> gm_segs;
   cudaStream_t st_copy = nullptr;      // window scans travel on their own stream so the upload of the next window can overlap a running solve
   cudaEvent_t ev_scans = nullptr, ev_main = nullptr;
   bool scans_pending = false;
@@ -523,6 +526,7 @@ void glio_destroy(glio_ctx* c) {
   c->sp_scan_tmp.release(); c->sp_consts.release(); c->sp_out.release(); c->sp_hits.release();
   c->e_items.release(); c->e_start.release(); c->e_part.release(); c->e_out.release(); c->e_poses.release();
   c->icp.release(); c->icp_src.release(); c->icp_tgt.release();
+  c->vsort.release(); c->vs_stage.release(); c->gm_cat.release(); c->gm_segs.release();
   for (auto& r : c->lc.recs) { cudaEventDestroy(r.a); cudaEventDestroy(r.b); }
   for (auto& e : c->lc.pool) cudaEventDestroy(e);
   c->lc.recs.clear(); c->lc.pool.clear();
@@ -2344,6 +2348,91 @@ int glio_loop_get_clouds(glio_loop* L, int64_t lat_cap, float* lat_xyz, int64_t*
     };
     fetch(L->lat_pts, L->lat_stride, nl, lat_xyz);
     fetch(L->his_pts, L->his_stride, nh, his_xyz);
+  });
+}
+
+}  // extern "C"
+
+// ------------------------------------------------------------------------------------------------------------
+// pcl::VoxelGrid of any cloud and save_pcd's global map (SURVEY 8 f-8): downSampleCloud's ds_filter_surf (Estimator.cpp:3628-3630)
+// and the export at :5324-5349, on the sort-based filter of grid.cu
+// ------------------------------------------------------------------------------------------------------------
+namespace {
+
+void check_vs_output(glio_ctx* c, const char* who, int64_t capacity, const float* xyz, int out_mem, const int64_t* n_out) {
+  GLIO_REQUIRE(n_out != nullptr && capacity >= 0 && (xyz || capacity == 0), GLIO_ERR_ARG, std::string(who) + ": bad output arguments");
+  GLIO_REQUIRE(out_mem == GLIO_HOST || out_mem == GLIO_DEVICE, GLIO_ERR_ARG, std::string(who) + ": out_mem must be GLIO_HOST or GLIO_DEVICE");
+  GLIO_REQUIRE(out_mem != GLIO_DEVICE || capacity == 0 || dev_ptr_ok(c, xyz, 4), GLIO_ERR_ARG,
+               std::string(who) + ": a GLIO_DEVICE output must be 4-byte aligned memory of the context's GPU");
+}
+
+// the filter's result (c->vsort.out_xyz, m points) to the caller; nothing is written when it does not fit
+void deliver_vs_output(glio_ctx* c, const char* who, int64_t m, bool filtered, int64_t capacity, float* xyz, int out_mem, int64_t* n_out,
+                       int32_t* filt) {
+  *n_out = m;
+  if (filt) *filt = filtered ? 1 : 0;
+  GLIO_REQUIRE(m <= capacity, GLIO_ERR_ARG, std::string(who) + ": capacity is smaller than the number of output points");
+  if (m == 0) return;
+  GLIO_CUDA_TRY(cudaMemcpyAsync(xyz, c->vsort.out_xyz.p, (size_t)m * 3 * sizeof(float),
+                                out_mem == GLIO_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, c->st));
+  GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
+}
+
+}  // namespace
+
+extern "C" {
+
+int glio_voxel_filter(glio_ctx* c, const float* xyz, int64_t n, int stride, int in_mem, float leaf, int64_t capacity, float* out_xyz,
+                      int out_mem, int64_t* n_out, int32_t* filtered) {
+  if (!c) return GLIO_ERR_ARG;
+  return guarded(c, [&] {
+    const char* who = "glio_voxel_filter";
+    GLIO_REQUIRE(n >= 0 && n < ((int64_t)1 << 31) && (xyz || n == 0), GLIO_ERR_ARG, "glio_voxel_filter: bad cloud pointer or size");
+    GLIO_REQUIRE(stride >= 3 && stride <= 64, GLIO_ERR_ARG, "glio_voxel_filter: stride_floats must be in [3,64]");
+    GLIO_REQUIRE(in_mem == GLIO_HOST || in_mem == GLIO_DEVICE, GLIO_ERR_ARG, "glio_voxel_filter: in_mem must be GLIO_HOST or GLIO_DEVICE");
+    GLIO_REQUIRE(in_mem != GLIO_DEVICE || n == 0 || dev_ptr_ok(c, xyz, 4), GLIO_ERR_ARG,
+                 "glio_voxel_filter: a GLIO_DEVICE cloud must be 4-byte aligned memory of the context's GPU");
+    GLIO_REQUIRE(leaf > 0.f && std::isfinite(leaf), GLIO_ERR_ARG, "glio_voxel_filter: leaf must be positive and finite");
+    check_vs_output(c, who, capacity, out_xyz, out_mem, n_out);
+    if (n == 0) { deliver_vs_output(c, who, 0, true, capacity, out_xyz, out_mem, n_out, filtered); return; }
+    const float* d = in_mem == GLIO_DEVICE ? xyz : stage_points(c, c->vs_stage, xyz, n, stride, in_mem);
+    bool f = false;
+    const int64_t m = voxel_sort_run(c->vsort, d, stride, n, leaf, &f, c->st, c->lc);
+    deliver_vs_output(c, who, m, f, capacity, out_xyz, out_mem, n_out, filtered);
+  });
+}
+
+int glio_loop_global_map(glio_loop* L, int interval, float leaf, int64_t capacity, float* xyz, int out_mem, int64_t* n_map, int64_t* n_raw,
+                         int32_t* filtered) {
+  if (!L) return GLIO_ERR_ARG;
+  glio_ctx* c = L->ctx;
+  return guarded(c, [&] {
+    const char* who = "glio_loop_global_map";
+    GLIO_REQUIRE(interval >= 1, GLIO_ERR_ARG, "glio_loop_global_map: interval must be >= 1");
+    GLIO_REQUIRE(leaf > 0.f && std::isfinite(leaf), GLIO_ERR_ARG, "glio_loop_global_map: leaf must be positive and finite");
+    check_vs_output(c, who, capacity, xyz, out_mem, n_map);
+    // keyframes 0, interval, 2 interval, ... (:5339), in that order, each after the previous one in the concatenation
+    std::vector<GlobalMapSeg> segs;
+    int64_t N = 0, n_max = 0;
+    for (size_t i = 0; i < L->kfs.size(); i += (size_t)interval) {
+      const glio_loop::Keyframe& kf = *L->kfs[i];
+      if (kf.n == 0) continue;
+      GlobalMapSeg g;
+      g.xyz = kf.xyz.p; g.n = kf.n; g.off = N;
+      for (int k = 0; k < 3; ++k) g.t[k] = kf.pose[k];
+      for (int k = 0; k < 4; ++k) g.q[k] = kf.pose[3 + k];
+      segs.push_back(g);
+      N += kf.n; n_max = std::max(n_max, kf.n);
+    }
+    if (n_raw) *n_raw = N;
+    if (N == 0) { deliver_vs_output(c, who, 0, true, capacity, xyz, out_mem, n_map, filtered); return; }
+    GLIO_REQUIRE(N < ((int64_t)1 << 31), GLIO_ERR_ARG, "glio_loop_global_map: the concatenated map has 2^31 points or more");
+    c->gm_segs.reserve(segs.size()); c->gm_cat.reserve((size_t)N);
+    GLIO_CUDA_TRY(cudaMemcpyAsync(c->gm_segs.p, segs.data(), segs.size() * sizeof(GlobalMapSeg), cudaMemcpyHostToDevice, c->st));
+    loop_global_map_cloud(c->gm_segs.p, (int)segs.size(), n_max, L->t_bl, L->q_bl, c->gm_cat.p, c->st, c->lc);
+    bool f = false;
+    const int64_t m = voxel_sort_run(c->vsort, reinterpret_cast<const float*>(c->gm_cat.p), 4, N, leaf, &f, c->st, c->lc);   // ds_filter_global_map
+    deliver_vs_output(c, who, m, f, capacity, xyz, out_mem, n_map, filtered);
   });
 }
 

@@ -186,6 +186,22 @@ void localmap_transform(const float* d_xyz, int stride, int64_t n, const double*
 // returns the number of filtered points (in w.out_xyz / w.out_vox), or -1 when PCL would pass the input through unchanged
 int64_t voxel_filter_run(VoxelWork& w, const float4* d_in, int64_t n, float leaf, cudaStream_t st, LaunchCounter& lc);
 
+// ---- sort-based pcl::VoxelGrid (grid.cu): same output as voxel_filter_run, cost in the number of points, any bounding box
+struct VoxelSortWork {
+  DevBuf<float4> tmp4;                  // the input as (x, y, z, index)
+  DevBuf<unsigned> key0, key1;          // radix sort ping-pong: voxel keys
+  DevBuf<int> val0, val1;               //                       point indices
+  DevBuf<int> bounds, bad, hist, flags, pos, scan_tmp;
+  DevBuf<float> out_xyz;                // result, 3 floats per point
+  void release() {
+    tmp4.release(); key0.release(); key1.release(); val0.release(); val1.release(); bounds.release(); bad.release(); hist.release();
+    flags.release(); pos.release(); scan_tmp.release(); out_xyz.release();
+  }
+};
+// n (> 0, < 2^31) points stride floats apart on the device -> w.out_xyz; returns its size.  *filtered = false: PCL's leaf-size check
+// passed the input through (w.out_xyz holds the input x,y,z).  Non-finite coordinates are GLIO_ERR_ARG.
+int64_t voxel_sort_run(VoxelSortWork& w, const float* d_xyz, int stride, int64_t n, float leaf, bool* filtered, cudaStream_t st, LaunchCounter& lc);
+
 // A deque of world-frame clouds, their concatenation and its voxel filter: the context's local map (glio_localmap_*,
 // Estimator.cpp:3529-3618) and the odometry's (LidarOdometry.cpp:267-288, :305-313) are both one of these.
 struct LocalMap {
@@ -358,5 +374,10 @@ void loop_quat_from_R(const double R[9], double q[4]);
 void loop_extrinsic_bl(const double q_lb[4], const double t_lb[3], double q_bl[4], double t_bl[3]);
 void loop_world_of_cloud(const double pose[7], const double q_bl[4], const double t_bl[3], double t[3], double q[4]);
 void loop_pose_from(const float final_T[16], const double latest[7], double out[7]);
+// save_pcd's concatenation (Estimator.cpp:5338-5341): segment s (n points, packed x,y,z) moved by first, then by its own pose, each
+// transformCloud rounding to float; written to out + off as float4
+struct GlobalMapSeg { const float* xyz; int64_t n, off; double t[3], q[4]; };
+void loop_global_map_cloud(const GlobalMapSeg* d_segs, int nseg, int64_t n_max, const double t_first[3], const double q_first[4], float4* out,
+                           cudaStream_t st, LaunchCounter& lc);
 
 }  // namespace glio

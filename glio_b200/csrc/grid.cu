@@ -386,27 +386,43 @@ __global__ void __launch_bounds__(256) k_vox_centroid(const float4* __restrict__
   if (out_vox) out_vox[o] = (int)c;
 }
 
+// Set-up shared by the dense and the sort-based filter: the points (stride floats apart) copied as float4 (x, y, z, index) into
+// tmp4 while their float min / max is reduced (getMinMax3D), read back to the host (one synchronisation).
+static void voxel_bounds(const float* d_xyz, int stride, int64_t n, float4* tmp4, int* d_bounds, float mn[3], float mx[3], cudaStream_t st,
+                         LaunchCounter& lc) {
+  lc.begin("k_init_bounds", st); k_init_bounds<<<1, 32, 0, st>>>(d_bounds); lc.end(st);
+  const int nb = (int)std::min<int64_t>((n + 255) / 256, kNumSMs * 8);
+  PoseD none{};
+  lc.begin("k_load_bounds", st); k_load_bounds<<<nb, 256, 0, st>>>(d_xyz, stride, n, none, 0, tmp4, d_bounds); lc.end(st);
+  int hb[6];
+  GLIO_CUDA_TRY(cudaMemcpyAsync(hb, d_bounds, sizeof(hb), cudaMemcpyDeviceToHost, st));
+  GLIO_CUDA_TRY(cudaStreamSynchronize(st));
+  for (int d = 0; d < 3; ++d) { mn[d] = ordered_to_float_h(hb[d]); mx[d] = ordered_to_float_h(hb[3 + d]); }
+  for (int d = 0; d < 3; ++d) GLIO_REQUIRE(std::isfinite(mn[d]) && std::isfinite(mx[d]), GLIO_ERR_ARG, "voxel_filter: non-finite point coordinates");
+}
+
+// PCL's leaf-size check and voxel layout (VoxelGrid::applyFilter): false when PCL passes the input through unchanged.  div01 is
+// div0 * div1 wrapped to 32 bits, as PCL's int arithmetic leaves it.
+static bool voxel_layout(const float mn[3], const float mx[3], float leaf, VoxelDesc& v, int div[3]) {
+  const float inv = 1.0f / leaf;                               // setLeafSize: Array4f::Ones() / leaf
+  const int64_t dx = (int64_t)((mx[0] - mn[0]) * inv) + 1, dy = (int64_t)((mx[1] - mn[1]) * inv) + 1, dz = (int64_t)((mx[2] - mn[2]) * inv) + 1;
+  if (dx * dy * dz > (int64_t)0x7fffffff) return false;        // PCL: "leaf size too small", input passed through
+  v.inv = inv;
+  for (int d = 0; d < 3; ++d) { v.min_b[d] = (int)std::floor(mn[d] * inv); div[d] = (int)std::floor(mx[d] * inv) - v.min_b[d] + 1; }
+  v.div0 = div[0]; v.div01 = (int)((uint32_t)div[0] * (uint32_t)div[1]);
+  return true;
+}
+
 int64_t voxel_filter_run(VoxelWork& w, const float4* d_in, int64_t n, float leaf, cudaStream_t st, LaunchCounter& lc) {
   GLIO_REQUIRE(n > 0 && n < ((int64_t)1 << 31), GLIO_ERR_ARG, "voxel_filter: bad point count");
   GLIO_REQUIRE(leaf > 0.f, GLIO_ERR_ARG, "voxel_filter: leaf size must be positive");
   w.tmp4.reserve((size_t)n); w.bounds.reserve(8);
-  lc.begin("k_init_bounds", st); k_init_bounds<<<1, 32, 0, st>>>(w.bounds.p); lc.end(st);
   const int nb = (int)std::min<int64_t>((n + 255) / 256, kNumSMs * 8);
-  PoseD none{};
-  lc.begin("k_load_bounds", st); k_load_bounds<<<nb, 256, 0, st>>>(reinterpret_cast<const float*>(d_in), 4, n, none, 0, w.tmp4.p, w.bounds.p); lc.end(st);
-  int hb[6];
-  GLIO_CUDA_TRY(cudaMemcpyAsync(hb, w.bounds.p, sizeof(hb), cudaMemcpyDeviceToHost, st));
-  GLIO_CUDA_TRY(cudaStreamSynchronize(st));
   float mn[3], mx[3];
-  for (int d = 0; d < 3; ++d) { mn[d] = ordered_to_float_h(hb[d]); mx[d] = ordered_to_float_h(hb[3 + d]); }
-  for (int d = 0; d < 3; ++d) GLIO_REQUIRE(std::isfinite(mn[d]) && std::isfinite(mx[d]), GLIO_ERR_ARG, "voxel_filter: non-finite point coordinates");
-  const float inv = 1.0f / leaf;                               // setLeafSize: Array4f::Ones() / leaf
-  const int64_t dx = (int64_t)((mx[0] - mn[0]) * inv) + 1, dy = (int64_t)((mx[1] - mn[1]) * inv) + 1, dz = (int64_t)((mx[2] - mn[2]) * inv) + 1;
-  if (dx * dy * dz > (int64_t)0x7fffffff) return -1;           // PCL: "leaf size too small", input passed through
-  VoxelDesc v; v.inv = inv;
+  voxel_bounds(reinterpret_cast<const float*>(d_in), 4, n, w.tmp4.p, w.bounds.p, mn, mx, st, lc);
+  VoxelDesc v;
   int div[3];
-  for (int d = 0; d < 3; ++d) { v.min_b[d] = (int)std::floor(mn[d] * inv); div[d] = (int)std::floor(mx[d] * inv) - v.min_b[d] + 1; }
-  v.div0 = div[0]; v.div01 = div[0] * div[1];
+  if (!voxel_layout(mn, mx, leaf, v, div)) return -1;
   const int64_t nvox = (int64_t)div[0] * div[1] * div[2];
   GLIO_REQUIRE(nvox <= (int64_t)256 * 1024 * 1024, GLIO_ERR_ARG, "voxel_filter: more than 2^28 voxels in the bounding box (dense voxel table)");
   w.count.reserve((size_t)nvox + 2); w.start.reserve((size_t)nvox + 2); w.opos.reserve((size_t)nvox + 2);
@@ -425,6 +441,185 @@ int64_t voxel_filter_run(VoxelWork& w, const float4* d_in, int64_t n, float leaf
   GLIO_CUDA_TRY(cudaMemcpyAsync(&m, w.opos.p + nvox, sizeof(int), cudaMemcpyDeviceToHost, st));
   GLIO_CUDA_TRY(cudaStreamSynchronize(st));
   GLIO_CUDA_TRY(cudaGetLastError());
+  return (int64_t)m;
+}
+
+// =====================================================================================================================
+// Sort-based pcl::VoxelGrid (glio_voxel_filter, glio_loop_global_map): the same keys, order and sums as the dense filter above,
+// but its cost follows the number of points instead of the bounding box.  One 32-bit key per point (PCL's voxel index, int
+// arithmetic wrapped to 32 bits and compared unsigned, as PCL's cloud_point_index_idx does), a stable LSD radix sort of
+// (key, point index) over the key bits the box needs, segment heads, their exclusive scan, one centroid per segment summed in
+// input order.  Kernels: k_vs_key, per pass k_vs_hist + k_scan_block / k_scan_add + k_vs_scatter, then k_vs_heads,
+// k_scan_block / k_scan_add, k_vs_centroid; k_vs_pack instead of all of these when PCL passes the input through.
+// =====================================================================================================================
+constexpr int VS_T = 256;                 // threads of the radix kernels
+constexpr int VS_R = 8;                   // rounds of VS_T keys per block: a block sorts a tile of 2048 consecutive keys
+constexpr int VS_TILE = VS_T * VS_R;
+constexpr int VS_DIGIT = 8;               // key bits per pass
+
+__device__ __forceinline__ unsigned voxel_key(const VoxelDesc& v, float x, float y, float z) {
+  const int i0 = (int)__fsub_rn(floorf(__fmul_rn(x, v.inv)), (float)v.min_b[0]);
+  const int i1 = (int)__fsub_rn(floorf(__fmul_rn(y, v.inv)), (float)v.min_b[1]);
+  const int i2 = (int)__fsub_rn(floorf(__fmul_rn(z, v.inv)), (float)v.min_b[2]);
+  return (unsigned)i0 + (unsigned)i1 * (unsigned)v.div0 + (unsigned)i2 * (unsigned)v.div01;
+}
+
+__global__ void __launch_bounds__(256) k_vs_key(const float4* __restrict__ pts, int64_t n, VoxelDesc v, unsigned* __restrict__ keys,
+                                                int* __restrict__ vals, int* __restrict__ bad) {
+  bool finite = true;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const float4 p = pts[i];
+    finite = finite && isfinite(p.x) && isfinite(p.y) && isfinite(p.z);
+    keys[i] = voxel_key(v, p.x, p.y, p.z);
+    vals[i] = (int)i;
+  }
+  if (!finite) atomicOr(bad, 1);
+}
+
+// digit counts of one block's tile, stored digit-major (hist[d * gridDim.x + block]) so that one exclusive scan gives every
+// (digit, block) its first output position
+__global__ void __launch_bounds__(VS_T) k_vs_hist(const unsigned* __restrict__ keys, int64_t n, int shift, int nbits, int* __restrict__ hist) {
+  __shared__ int h[1 << VS_DIGIT];
+  const unsigned mask = (1u << nbits) - 1u;
+  h[threadIdx.x] = 0;
+  __syncthreads();
+  const int64_t base = (int64_t)blockIdx.x * VS_TILE;
+#pragma unroll
+  for (int r = 0; r < VS_R; ++r) {
+    const int64_t i = base + r * VS_T + threadIdx.x;
+    if (i < n) atomicAdd(&h[(keys[i] >> shift) & mask], 1);
+  }
+  __syncthreads();
+  if (threadIdx.x <= mask) hist[(int64_t)threadIdx.x * gridDim.x + blockIdx.x] = h[threadIdx.x];
+}
+
+// Stable scatter of one block's tile: the tile is taken VS_T keys at a time in input order; inside a warp the lanes with the same
+// digit rank themselves by lane (match_any), the warps of a round follow each other in warp order, and the rounds in tile order.
+__global__ void __launch_bounds__(VS_T) k_vs_scatter(const unsigned* __restrict__ kin, const int* __restrict__ vin, int64_t n, int shift,
+                                                     int nbits, const int* __restrict__ offs, unsigned* __restrict__ kout,
+                                                     int* __restrict__ vout) {
+  constexpr int NW = VS_T / 32;
+  __shared__ int run[1 << VS_DIGIT];          // next output position of each digit
+  __shared__ int wc[NW][1 << VS_DIGIT];       // this round's per-warp digit counts, then each warp's first position
+  const unsigned mask = (1u << nbits) - 1u;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const unsigned lt = (1u << lane) - 1u;
+  run[threadIdx.x] = threadIdx.x <= mask ? offs[(int64_t)threadIdx.x * gridDim.x + blockIdx.x] : 0;
+  const int64_t base = (int64_t)blockIdx.x * VS_TILE;
+  for (int r = 0; r < VS_R; ++r) {
+#pragma unroll
+    for (int w = 0; w < NW; ++w) wc[w][threadIdx.x] = 0;
+    __syncthreads();
+    const int64_t i = base + r * VS_T + threadIdx.x;
+    const bool valid = i < n;
+    const unsigned key = valid ? kin[i] : 0u;
+    const int val = valid ? vin[i] : 0;
+    const unsigned d = valid ? (key >> shift) & mask : 0xffffffffu;      // invalid lanes never match a digit
+    const unsigned peers = __match_any_sync(0xffffffffu, d);
+    const int rank = __popc(peers & lt);
+    if (valid && rank == 0) wc[warp][d] = __popc(peers);
+    __syncthreads();
+    if (threadIdx.x <= mask) {
+      int s = run[threadIdx.x];
+#pragma unroll
+      for (int w = 0; w < NW; ++w) { const int c = wc[w][threadIdx.x]; wc[w][threadIdx.x] = s; s += c; }
+      run[threadIdx.x] = s;
+    }
+    __syncthreads();
+    if (valid) {
+      const int o = wc[warp][d] + rank;
+      kout[o] = key; vout[o] = val;
+    }
+    __syncthreads();
+  }
+}
+
+__global__ void __launch_bounds__(256) k_vs_heads(const unsigned* __restrict__ keys, int64_t n, int* __restrict__ flags) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i <= n; i += (int64_t)gridDim.x * blockDim.x)
+    flags[i] = (i < n && (i == 0 || keys[i] != keys[i - 1])) ? 1 : 0;
+}
+
+// one thread per segment (its head): float sums in input order (the sort is stable), divided by the float count
+__global__ void __launch_bounds__(256) k_vs_centroid(const float4* __restrict__ pts, const unsigned* __restrict__ keys, const int* __restrict__ vals,
+                                                     const int* __restrict__ flags, const int* __restrict__ pos, int64_t n, float* __restrict__ out_xyz) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    if (!flags[i]) continue;
+    const unsigned k = keys[i];
+    float sx = 0.f, sy = 0.f, sz = 0.f;
+    int64_t j = i;
+    do {
+      const float4 p = pts[vals[j]];
+      sx = __fadd_rn(sx, p.x); sy = __fadd_rn(sy, p.y); sz = __fadd_rn(sz, p.z);
+      ++j;
+    } while (j < n && keys[j] == k);
+    const float cnt = (float)(j - i);
+    const size_t o = 3 * (size_t)pos[i];
+    out_xyz[o] = __fdiv_rn(sx, cnt); out_xyz[o + 1] = __fdiv_rn(sy, cnt); out_xyz[o + 2] = __fdiv_rn(sz, cnt);
+  }
+}
+
+// PCL's pass-through: the input x,y,z as they are
+__global__ void __launch_bounds__(256) k_vs_pack(const float4* __restrict__ pts, int64_t n, float* __restrict__ out_xyz, int* __restrict__ bad) {
+  bool finite = true;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const float4 p = pts[i];
+    finite = finite && isfinite(p.x) && isfinite(p.y) && isfinite(p.z);
+    out_xyz[3 * i] = p.x; out_xyz[3 * i + 1] = p.y; out_xyz[3 * i + 2] = p.z;
+  }
+  if (!finite) atomicOr(bad, 1);
+}
+
+static int voxel_key_bits(const int div[3]) {
+  const int64_t nvox = (int64_t)div[0] * div[1] * div[2];
+  if (nvox > ((int64_t)1 << 32)) return 32;                    // the keys wrap: every bit can differ
+  int b = 0;
+  for (int64_t m = nvox - 1; m > 0; m >>= 1) ++b;              // keys are in [0, nvox)
+  return b;
+}
+
+int64_t voxel_sort_run(VoxelSortWork& w, const float* d_xyz, int stride, int64_t n, float leaf, bool* filtered, cudaStream_t st, LaunchCounter& lc) {
+  GLIO_REQUIRE(n > 0 && n < ((int64_t)1 << 31), GLIO_ERR_ARG, "voxel_filter: bad point count");
+  GLIO_REQUIRE(leaf > 0.f && std::isfinite(leaf), GLIO_ERR_ARG, "voxel_filter: leaf size must be positive and finite");
+  w.tmp4.reserve((size_t)n); w.bounds.reserve(8); w.bad.reserve(1); w.out_xyz.reserve((size_t)n * 3);
+  float mn[3], mx[3];
+  voxel_bounds(d_xyz, stride, n, w.tmp4.p, w.bounds.p, mn, mx, st, lc);
+  // every point NaN: fminf / fmaxf skipped them all and the bounds are still the initial ones
+  GLIO_REQUIRE(mn[0] <= mx[0] && mn[1] <= mx[1] && mn[2] <= mx[2], GLIO_ERR_ARG, "voxel_filter: non-finite point coordinates");
+  GLIO_CUDA_TRY(cudaMemsetAsync(w.bad.p, 0, sizeof(int), st));
+  const int nb = (int)std::min<int64_t>((n + 255) / 256, kNumSMs * 8);
+  VoxelDesc v;
+  int div[3];
+  int m = 0;
+  *filtered = voxel_layout(mn, mx, leaf, v, div);
+  if (!*filtered) {
+    lc.begin("k_vs_pack", st); k_vs_pack<<<nb, 256, 0, st>>>(w.tmp4.p, n, w.out_xyz.p, w.bad.p); lc.end(st);
+    m = (int)n;
+  } else {
+    w.key0.reserve((size_t)n); w.key1.reserve((size_t)n); w.val0.reserve((size_t)n); w.val1.reserve((size_t)n);
+    w.flags.reserve((size_t)n + 1); w.pos.reserve((size_t)n + 1);
+    lc.begin("k_vs_key", st); k_vs_key<<<nb, 256, 0, st>>>(w.tmp4.p, n, v, w.key0.p, w.val0.p, w.bad.p); lc.end(st);
+    const int bits = voxel_key_bits(div);
+    const int64_t tiles = (n + VS_TILE - 1) / VS_TILE;
+    w.hist.reserve((size_t)tiles << VS_DIGIT);
+    unsigned *ka = w.key0.p, *kb = w.key1.p;
+    int *va = w.val0.p, *vb = w.val1.p;
+    for (int shift = 0; shift < bits; shift += VS_DIGIT) {
+      const int nbits = std::min(VS_DIGIT, bits - shift);
+      lc.begin("k_vs_hist", st); k_vs_hist<<<(unsigned)tiles, VS_T, 0, st>>>(ka, n, shift, nbits, w.hist.p); lc.end(st);
+      exclusive_scan_i32(w.hist.p, w.hist.p, tiles << nbits, w.scan_tmp, st, lc);     // in place: every thread reads its items first
+      lc.begin("k_vs_scatter", st); k_vs_scatter<<<(unsigned)tiles, VS_T, 0, st>>>(ka, va, n, shift, nbits, w.hist.p, kb, vb); lc.end(st);
+      std::swap(ka, kb); std::swap(va, vb);
+    }
+    lc.begin("k_vs_heads", st); k_vs_heads<<<nb, 256, 0, st>>>(ka, n, w.flags.p); lc.end(st);
+    exclusive_scan_i32(w.flags.p, w.pos.p, n + 1, w.scan_tmp, st, lc);
+    lc.begin("k_vs_centroid", st); k_vs_centroid<<<nb, 256, 0, st>>>(w.tmp4.p, ka, va, w.flags.p, w.pos.p, n, w.out_xyz.p); lc.end(st);
+    GLIO_CUDA_TRY(cudaMemcpyAsync(&m, w.pos.p + n, sizeof(int), cudaMemcpyDeviceToHost, st));
+  }
+  int bad = 0;
+  GLIO_CUDA_TRY(cudaMemcpyAsync(&bad, w.bad.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+  GLIO_CUDA_TRY(cudaStreamSynchronize(st));
+  GLIO_CUDA_TRY(cudaGetLastError());
+  GLIO_REQUIRE(!bad, GLIO_ERR_ARG, "voxel_filter: non-finite point coordinates");
   return (int64_t)m;
 }
 

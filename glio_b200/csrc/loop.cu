@@ -562,6 +562,36 @@ void icp_run(IcpWork& w, const float* d_src, int src_stride, int64_t n_src, cons
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
+// save_pcd's global map (Estimator.cpp:5324-5349): transformCloud(transformCloud(surf_frames[i], &Tbl), &pose_info_keyframe[i]), two
+// float roundings per point; one launch over every segment (blockIdx.y strides the segments)
+// ---------------------------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) k_gm_transform(const GlobalMapSeg* __restrict__ segs, int nseg, PoseD first, float4* __restrict__ out) {
+  for (int s = blockIdx.y; s < nseg; s += gridDim.y) {
+    const GlobalMapSeg g = segs[s];
+    PoseD pose;
+    for (int k = 0; k < 3; ++k) pose.t[k] = g.t[k];
+    for (int k = 0; k < 4; ++k) pose.q[k] = g.q[k];
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < g.n; i += (int64_t)gridDim.x * blockDim.x) {
+      float p[3] = {g.xyz[3 * i], g.xyz[3 * i + 1], g.xyz[3 * i + 2]};
+      transform_point_f(first, p, p);
+      transform_point_f(pose, p, p);
+      out[g.off + i] = make_float4(p[0], p[1], p[2], 0.f);
+    }
+  }
+}
+
+void loop_global_map_cloud(const GlobalMapSeg* d_segs, int nseg, int64_t n_max, const double t_first[3], const double q_first[4], float4* out,
+                           cudaStream_t st, LaunchCounter& lc) {
+  if (nseg <= 0 || n_max <= 0) return;
+  PoseD first;
+  for (int k = 0; k < 3; ++k) first.t[k] = t_first[k];
+  for (int k = 0; k < 4; ++k) first.q[k] = q_first[k];
+  const dim3 grid((unsigned)std::min<int64_t>((n_max + 255) / 256, 64), (unsigned)std::min(nseg, 65535));
+  lc.begin("k_gm_transform", st); k_gm_transform<<<grid, 256, 0, st>>>(d_segs, nseg, first, out); lc.end(st);
+  GLIO_CUDA_TRY(cudaGetLastError());
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
 // host pose arithmetic of performLoopClosure (scalar double, Eigen's operation order, no FMA: this unit is -fmad=false and
 // the host compiler targets baseline x86-64)
 // ---------------------------------------------------------------------------------------------------------------------

@@ -126,6 +126,24 @@ int glio_localmap_size(glio_ctx* ctx, int* n_frames, int64_t* n_points);
 int glio_localmap_build(glio_ctx* ctx, float leaf, int64_t* n_map);
 int glio_get_map(glio_ctx* ctx, int64_t capacity, float* xyz, int64_t* n_map);
 
+/* ---- pcl::VoxelGrid of any cloud (SURVEY 8 f-8): downSampleCloud's scan filter ds_filter_surf.filter (Estimator.cpp:3628-3630,
+ * leaf surfDSRange set at :852), whose output surf_last_ds becomes the keyframe cloud surf_frames[k] (:4150-4153).
+ * xyz[n] (0 <= n < 2^31): x,y,z at floats 0..2 of a stride in [3,64] (8 = pcl::PointXYZI), host or device memory (device: 4-byte
+ * aligned memory of the context's GPU).  PCL's applyFilter: inv = 1/leaf, float min / max; when (int64)((max - min) inv) + 1
+ * multiplied over the axes exceeds INT32_MAX the input x,y,z come back in input order with *filtered = 0; otherwise voxel index
+ * ijk0 + ijk1 div0 + ijk2 div0 div1 (int arithmetic, wrapped to 32 bits, ordered unsigned), one point per occupied voxel in
+ * ascending index, its float sums in input order divided by the float count (*filtered = 1).  PCL sums a voxel in the order
+ * std::sort leaves it; input order is the deterministic member of that family, the one glio_localmap_build produces too.  Only
+ * x,y,z are carried: PCL also averages intensity, which GLIO sets to scanID + 0.1 relTime (Preprocessing.cpp:509), not a
+ * measurement.  Output: packed x,y,z in out_xyz (host or device memory per out_mem; device: 4-byte aligned memory of the context's
+ * GPU).  *n_out always receives the true count; when it exceeds capacity the call fails with GLIO_ERR_ARG and writes nothing to
+ * out_xyz.  n = 0 gives 0 points and launches nothing.  Non-finite coordinates, leaf <= 0 or non-finite, a stride out of range,
+ * null or misaligned pointers are GLIO_ERR_ARG.  filtered may be NULL.  The cost follows n, not the bounding box (a stable radix
+ * sort of the voxel keys); no box size is refused.  Uses its own work space: the context's parameters, map, local map, window
+ * slots, batch frames, odometries and loop objects are untouched.  Returns when its work is complete. */
+int glio_voxel_filter(glio_ctx* ctx, const float* xyz, int64_t n, int stride_floats, int in_mem, float leaf, int64_t capacity, float* out_xyz,
+                      int out_mem, int64_t* n_out, int32_t* filtered);
+
 /* ---- K1: scan-to-map surf association for ONE keyframe slot.
  * Replaces Estimator::findCorrespondingSurfFeatures(idx, q, t)  (Estimator.cpp:3633-3708):
  * q,t is the lidar->map pose (Q2,T2 of Estimator.cpp:2216-2217).  The scan stays resident in the slot.
@@ -486,6 +504,16 @@ int glio_loop_step(glio_loop* lp, const float select_xyz[3], double time_new_odo
  * order); either pointer may be NULL, the counts are always written; GLIO_ERR_ARG if a capacity is too small. */
 int glio_loop_get_clouds(glio_loop* lp, int64_t latest_capacity, float* latest_xyz, int64_t* n_latest, int64_t his_capacity, float* his_xyz,
                          int64_t* n_his);
+/* save_pcd's global map from the keyframe store (Estimator.cpp:5324-5349; mapping_interval 3 in config_urban_hk.yaml:87,
+ * ds_filter_global_map leaf 0.2 at :856): keyframes 0, interval, 2 interval, ... < size, in that order, each point moved by
+ * transformCloud(transformCloud(surf_frames[i], &Tbl), &pose_info_keyframe[i]) (:5340) with Tbl = (q_bl, t_bl) and the keyframe's
+ * current pose (glio_loop_set_poses), each transform Eigen's double rotation rounded to float (two roundings, not the one combined
+ * pose of the loop clouds); the concatenation (*n_raw points, n_raw may be NULL) filtered as glio_voxel_filter(leaf) does, PCL's
+ * pass-through included.  Only x,y,z (the store holds no intensity).  Output conventions as glio_voxel_filter.  interval < 1 or
+ * leaf <= 0 is GLIO_ERR_ARG; an empty store gives 0 points.  Writing the PCD file stays with the caller.  Neither the loop object's
+ * state nor the context's changes. */
+int glio_loop_global_map(glio_loop* lp, int interval, float leaf, int64_t capacity, float* xyz, int out_mem, int64_t* n_map, int64_t* n_raw,
+                         int32_t* filtered);
 
 /* ---- K3: marginalisation of the oldest keyframe (MarginalizationInfo, GLIO/src/MarginalizationFactor.cpp:82-202; call site
  * Estimator.cpp:2462-2608).  The reference re-evaluates EVERY LiDAR factor of the window (:2538-2576, one virtual Evaluate per
