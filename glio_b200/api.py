@@ -137,7 +137,7 @@ class Context:
 
     KERNELS = ["k_feat_curvature", "k_feat_select", "k_feat_voxel", "k_feat_offsets", "k_feat_gather", "k_knn_box", "k_plane_fit", "k_plane_fit_pair", "k_eval_unary", "k_eval_unary_cost", "k_transform_hist", "k_order_scatter",
                "k_compact", "k_flags", "k_cell_hist", "k_cell_scatter", "k_load_bounds", "k_scan_block", "k_scan_add",
-               "k_eval_binary", "k_eval_binary_cost", "k_bin_assemble",
+               "k_eval_binary", "k_eval_binary_cost", "k_bin_assemble", "k_gather_sel", "k_sel_sample",
                "k_lm_transform", "k_vox_hist", "k_vox_scatter", "k_vox_sort", "k_vox_flags", "k_vox_centroid", "k_init_bounds"]
 
     def lib_profile(self, on):
@@ -735,6 +735,72 @@ def _batch_set_pair_matches(self, cur, oth, cp, normal_cent, weight):
 
 
 Context.batch_set_pair_matches = _batch_set_pair_matches
+
+
+# ---------------------------------------------------------------------------------------------------
+# feature selection on the device (featureSelection / globalFeatureSelection[Add]_Batch, Estimator.cpp:3894-4116, seeded)
+# ---------------------------------------------------------------------------------------------------
+class SelectOptions(C.Structure):
+    _fields_ = [("feature_res_num", C.c_int32), ("rand_set_num", C.c_int32), ("batch_feature_res_num", C.c_int32),
+                ("batch_rand_set_num", C.c_int32), ("random_select", C.c_int32), ("reserved", C.c_int32), ("seed", C.c_uint64),
+                ("nonce", C.c_uint64)]
+
+
+def select_default_options(**kw):
+    """glio_select_default_options (the shipped configuration: F 100, R 300, B 25, BR 400, random_select, seed 0, nonce 0)."""
+    o = SelectOptions()
+    lib().glio_select_default_options(C.byref(o))
+    for k, v in kw.items():
+        if not hasattr(o, k):
+            raise AttributeError(k)
+        setattr(o, k, int(v))
+    return o
+
+
+def _select_random(self, stream_ids, options=None, **kw):
+    """glio_select_random for slots 0..len(stream_ids)-1 (stream id = the slot's keyframe index); returns the active counts."""
+    ids = np.ascontiguousarray(stream_ids, np.int64)
+    opt = options if options is not None else select_default_options(**kw)
+    na = np.zeros(len(ids), np.int64)
+    self._chk(self._lib.glio_select_random(self._h, C.c_int(len(ids)), _ptr(ids), C.byref(opt), _ptr(na)))
+    return na
+
+
+def _batch_select_random(self, cur, oth, mode, options=None, **kw):
+    """glio_batch_select_random over pairs (cur[i], oth[i]) grouped by cur; mode 0 start/end, 1 incremental; returns the active counts."""
+    cur = np.ascontiguousarray(cur, np.int32); oth = np.ascontiguousarray(oth, np.int32)
+    if len(cur) != len(oth):
+        raise ValueError("cur and oth must have the same length")
+    opt = options if options is not None else select_default_options(**kw)
+    na = np.zeros(len(cur), np.int64)
+    self._chk(self._lib.glio_batch_select_random(self._h, _ptr(cur), _ptr(oth), C.c_int64(len(cur)), C.c_int(mode), C.byref(opt), _ptr(na)))
+    return na
+
+
+def _selection_out(call):
+    n = C.c_int64(0)
+    call(C.c_int64(0), None, C.byref(n))
+    if n.value < 0:
+        return None
+    keep = np.empty(n.value, np.int32)
+    call(C.c_int64(n.value), _ptr(keep), C.byref(n))
+    return keep
+
+
+def _get_selection(self, slot):
+    """The active match indices of a slot (int32 array), or None when all its matches are active."""
+    return _selection_out(lambda cap, p, n: self._chk(self._lib.glio_get_selection(self._h, C.c_int(slot), cap, p, n)))
+
+
+def _batch_get_selection(self, cur, oth):
+    """The active match indices of pair (cur, oth), or None when all its matches are active."""
+    return _selection_out(lambda cap, p, n: self._chk(self._lib.glio_batch_get_selection(self._h, C.c_int(cur), C.c_int(oth), cap, p, n)))
+
+
+Context.select_random = _select_random
+Context.batch_select_random = _batch_select_random
+Context.get_selection = _get_selection
+Context.batch_get_selection = _batch_get_selection
 Context.batch_declare_pairs = _batch_declare_pairs
 Context.batch_solve = _batch_solve
 Context.set_allreduce = _set_allreduce

@@ -13,6 +13,7 @@
 #include <chrono>
 #include <deque>
 #include <map>
+#include <set>
 #include <memory>
 
 #include "common.cuh"
@@ -33,6 +34,7 @@ struct Slot {
   DevBuf<int32_t> m_src;
   int64_t n_match = 0;
   DevBuf<float4> s_cpw, s_nsd;   // selected subset
+  DevBuf<int32_t> s_keep;        // its match indices (glio_select's list or the sampler's draws, glio_get_selection)
   int64_t n_sel = -1;            // -1: no selection -> all matches are active
   DevBuf<float4> e_cps, e_pa, e_pb;  // edge correspondences (caller-provided)
   int64_t n_edge = 0;
@@ -44,7 +46,7 @@ struct Slot {
   DevBuf<double> dbg_plane;
   int64_t dbg_Q = 0;
   void release() {
-    scan.release(); m_cpw.release(); m_nsd.release(); m_src.release(); s_cpw.release(); s_nsd.release(); e_cps.release(); e_pa.release(); e_pb.release();
+    scan.release(); m_cpw.release(); m_nsd.release(); m_src.release(); s_cpw.release(); s_nsd.release(); s_keep.release(); e_cps.release(); e_pa.release(); e_pb.release();
     dbg_status.release(); dbg_idx5.release(); dbg_sqd5.release(); dbg_pm.release(); dbg_plane.release();
   }
 };
@@ -103,7 +105,8 @@ struct glio_ctx {
   struct Pair {
     int cur = 0, oth = 0;
     DevBuf<float4> m_cpw; DevBuf<double> m_nc; DevBuf<int32_t> m_src; int64_t n_match = 0;
-    DevBuf<float4> s_cpw; DevBuf<double> s_nc; int64_t n_sel = -1;
+    DevBuf<float4> s_cpw; DevBuf<double> s_nc; DevBuf<int32_t> s_keep; int64_t n_sel = -1;
+    void release() { m_cpw.release(); m_nc.release(); m_src.release(); s_cpw.release(); s_nc.release(); s_keep.release(); }
   };
   std::map<int, std::unique_ptr<Frame>> frames;
   std::vector<std::unique_ptr<Pair>> pairs;
@@ -130,7 +133,8 @@ struct glio_ctx {
   DevBuf<int> d_counts;
   PinnedBuf<int> h_counts;
   DevBuf<int> d_bad;
-  DevBuf<int32_t> d_keep;
+  // seeded feature selection: the segment table of one k_sel_sample launch, staged in pinned memory; ev_sel marks its upload
+  DevBuf<SelSeg> d_sel_segs; PinnedBuf<SelSeg> h_sel_segs; cudaEvent_t ev_sel = nullptr;
   // front-end feature extraction work space
   DevBuf<float> f_cloud, f_curv; DevBuf<int8_t> f_label, f_picked; DevBuf<int32_t> f_scan, f_ring, f_lf, f_counts, f_out; DevBuf<float4> f_ds, f_outds;
   // front-end sweep preparation work space
@@ -511,14 +515,14 @@ void glio_destroy(glio_ctx* c) {
   c->map.release(); c->map_stage.release(); c->map_stage2.release(); if (c->ev_map) cudaEventDestroy(c->ev_map);
   c->lm.release(); c->lm_stage.release();
   for (auto& f : c->frames) { f.second->scan.release(); f.second->grid.release(); }
-  for (auto& p : c->pairs) { p->m_cpw.release(); p->m_nc.release(); p->m_src.release(); p->s_cpw.release(); p->s_nc.release(); }
+  for (auto& p : c->pairs) p->release();
   c->d_bin_items.release(); c->d_pair_item_start.release(); c->d_kf_inc_start.release(); c->d_inc.release(); c->d_bin_partials.release();
   c->d_pair_sums.release(); c->d_bin_diag.release(); c->d_bin_off.release(); c->d_bin_poses.release(); c->h_bin_diag.release(); c->h_bin_off.release(); c->h_bin_poses.release();
   for (auto& s : c->slots) if (s) s->release();
   c->w_pm.release(); c->w_pmq.release(); c->w_nsd.release(); c->w_seg.release(); c->w_status.release(); c->w_weight.release();
   c->w_nc.release(); c->w_plane.release(); c->w_idx5.release(); c->w_sqd5.release(); c->w_flags.release(); c->w_pos.release();
   c->cell_count.release(); c->cell_pos.release(); c->scan_tmp.release(); c->d_segs.release(); c->d_dst.release(); c->d_counts.release();
-  c->h_counts.release(); c->d_bad.release(); c->d_keep.release(); c->d_items.release(); c->d_kf_item_start.release();
+  c->h_counts.release(); c->d_bad.release(); c->d_items.release(); c->d_kf_item_start.release();
   c->d_partials.release(); c->d_out.release(); c->d_poses.release(); c->d_r.release(); c->d_J.release(); c->h_out.release();
   c->h_poses.release(); c->h_flag.release(); c->d_ticket.release(); c->w_knn_idx.release(); c->w_knn_sqd.release();
   c->f_cloud.release(); c->f_curv.release(); c->f_label.release(); c->f_picked.release(); c->f_scan.release(); c->f_ring.release(); c->f_lf.release(); c->f_counts.release(); c->f_out.release(); c->f_ds.release(); c->f_outds.release();
@@ -527,6 +531,7 @@ void glio_destroy(glio_ctx* c) {
   c->e_items.release(); c->e_start.release(); c->e_part.release(); c->e_out.release(); c->e_poses.release();
   c->icp.release(); c->icp_src.release(); c->icp_tgt.release();
   c->vsort.release(); c->vs_stage.release(); c->gm_cat.release(); c->gm_segs.release();
+  c->d_sel_segs.release(); c->h_sel_segs.release(); if (c->ev_sel) cudaEventDestroy(c->ev_sel);
   for (auto& r : c->lc.recs) { cudaEventDestroy(r.a); cudaEventDestroy(r.b); }
   for (auto& e : c->lc.pool) cudaEventDestroy(e);
   c->lc.recs.clear(); c->lc.pool.clear();
@@ -865,11 +870,11 @@ int glio_select(glio_ctx* c, int slot, const int32_t* keep, int64_t n) {
     GLIO_REQUIRE(n == 0 || keep, GLIO_ERR_ARG, "null selection list");
     sl.n_sel = n;
     if (n == 0) return;
-    c->d_keep.reserve(n); c->d_bad.reserve(1);
+    sl.s_keep.reserve(n); c->d_bad.reserve(1);
     sl.s_cpw.reserve(n); sl.s_nsd.reserve(n);
-    GLIO_CUDA_TRY(cudaMemcpyAsync(c->d_keep.p, keep, n * sizeof(int32_t), cudaMemcpyHostToDevice, c->st));
+    GLIO_CUDA_TRY(cudaMemcpyAsync(sl.s_keep.p, keep, n * sizeof(int32_t), cudaMemcpyHostToDevice, c->st));
     GLIO_CUDA_TRY(cudaMemsetAsync(c->d_bad.p, 0, sizeof(int), c->st));
-    gather_selection(c->d_keep.p, n, sl.n_match, sl.m_cpw.p, sl.m_nsd.p, nullptr, sl.s_cpw.p, sl.s_nsd.p, nullptr, c->d_bad.p, c->st, c->lc);
+    gather_selection(sl.s_keep.p, n, sl.n_match, sl.m_cpw.p, sl.m_nsd.p, nullptr, sl.s_cpw.p, sl.s_nsd.p, nullptr, c->d_bad.p, c->st, c->lc);
     int bad = 0;
     GLIO_CUDA_TRY(cudaMemcpyAsync(&bad, c->d_bad.p, sizeof(int), cudaMemcpyDeviceToHost, c->st));
     GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
@@ -1345,7 +1350,7 @@ int glio_batch_clear(glio_ctx* c) {
   return guarded(c, [&] {
     GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
     for (auto& f : c->frames) { f.second->scan.release(); f.second->grid.release(); }
-    for (auto& p : c->pairs) { p->m_cpw.release(); p->m_nc.release(); p->m_src.release(); p->s_cpw.release(); p->s_nc.release(); }
+    for (auto& p : c->pairs) p->release();
     c->frames.clear(); c->pairs.clear(); c->pair_index.clear(); c->bin_dirty = true;
   });
 }
@@ -1482,14 +1487,175 @@ int glio_batch_select(glio_ctx* c, int cur, int oth, const int32_t* keep, int64_
     GLIO_REQUIRE(n == 0 || keep, GLIO_ERR_ARG, "null selection list");
     pr.n_sel = n;
     if (n == 0) return;
-    c->d_keep.reserve(n); c->d_bad.reserve(1); pr.s_cpw.reserve(n); pr.s_nc.reserve(6 * n);
-    GLIO_CUDA_TRY(cudaMemcpyAsync(c->d_keep.p, keep, n * sizeof(int32_t), cudaMemcpyHostToDevice, c->st));
+    pr.s_keep.reserve(n); c->d_bad.reserve(1); pr.s_cpw.reserve(n); pr.s_nc.reserve(6 * n);
+    GLIO_CUDA_TRY(cudaMemcpyAsync(pr.s_keep.p, keep, n * sizeof(int32_t), cudaMemcpyHostToDevice, c->st));
     GLIO_CUDA_TRY(cudaMemsetAsync(c->d_bad.p, 0, sizeof(int), c->st));
-    gather_selection(c->d_keep.p, n, pr.n_match, pr.m_cpw.p, nullptr, pr.m_nc.p, pr.s_cpw.p, nullptr, pr.s_nc.p, c->d_bad.p, c->st, c->lc);
+    gather_selection(pr.s_keep.p, n, pr.n_match, pr.m_cpw.p, nullptr, pr.m_nc.p, pr.s_cpw.p, nullptr, pr.s_nc.p, c->d_bad.p, c->st, c->lc);
     int bad = 0;
     GLIO_CUDA_TRY(cudaMemcpyAsync(&bad, c->d_bad.p, sizeof(int), cudaMemcpyDeviceToHost, c->st));
     GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
     if (bad) { pr.n_sel = -1; throw Error{GLIO_ERR_ARG, "selection index out of range"}; }
+  });
+}
+
+}  // extern "C"
+
+namespace {
+
+enum { SEL_DOMAIN_WINDOW = 0, SEL_DOMAIN_STARTEND = 1, SEL_DOMAIN_ADD = 2 };
+
+void check_select_options(const glio_select_options* o) {
+  GLIO_REQUIRE(o != nullptr, GLIO_ERR_ARG, "null selection options");
+  GLIO_REQUIRE(o->feature_res_num >= 1 && o->feature_res_num <= GLIO_SEL_MAX, GLIO_ERR_ARG, "feature_res_num must be in [1, 4096]");
+  GLIO_REQUIRE(o->rand_set_num >= 1, GLIO_ERR_ARG, "rand_set_num must be >= 1");
+  GLIO_REQUIRE(o->batch_feature_res_num >= 1 && o->batch_feature_res_num <= GLIO_SEL_MAX, GLIO_ERR_ARG, "batch_feature_res_num must be in [1, 4096]");
+  GLIO_REQUIRE(o->batch_rand_set_num >= o->batch_feature_res_num, GLIO_ERR_ARG, "batch_rand_set_num must be >= batch_feature_res_num");
+}
+
+// one k_sel_sample launch over the planned segments: the table goes up in one copy from pinned memory, nothing waits for the
+// stream.  The staging buffer is only rewritten once the previous call's copy has run (an event, not a stream synchronisation).
+void select_launch(glio_ctx* c, const std::vector<SelSeg>& segs, int k_max, uint64_t domain, uint64_t seed, uint64_t nonce) {
+  if (segs.empty()) return;
+  if (!c->ev_sel) GLIO_CUDA_TRY(cudaEventCreateWithFlags(&c->ev_sel, cudaEventDisableTiming));
+  else GLIO_CUDA_TRY(cudaEventSynchronize(c->ev_sel));
+  c->h_sel_segs.reserve(segs.size()); c->d_sel_segs.reserve(segs.size());
+  memcpy(c->h_sel_segs.p, segs.data(), segs.size() * sizeof(SelSeg));
+  GLIO_CUDA_TRY(cudaMemcpyAsync(c->d_sel_segs.p, c->h_sel_segs.p, segs.size() * sizeof(SelSeg), cudaMemcpyHostToDevice, c->st));
+  GLIO_CUDA_TRY(cudaEventRecord(c->ev_sel, c->st));
+  select_sample_run(c->d_sel_segs.p, (int)segs.size(), k_max, seed, domain, nonce, c->st, c->lc);
+}
+
+}  // namespace
+
+extern "C" {
+
+void glio_select_default_options(glio_select_options* o) {
+  if (!o) return;
+  memset(o, 0, sizeof(*o));
+  o->feature_res_num = 100; o->rand_set_num = 300; o->batch_feature_res_num = 25; o->batch_rand_set_num = 400;
+  o->random_select = 1; o->seed = 0; o->nonce = 0;
+}
+
+// featureSelection (Estimator.cpp:3894-3992) for slots 0..W-1.  The outcome of every slot follows from its match count alone, so
+// the host decides it here and only the sampled slots go to the device.
+int glio_select_random(glio_ctx* c, int W, const int64_t* stream_ids, const glio_select_options* opt, int64_t* n_active) {
+  if (!c) return GLIO_ERR_ARG;
+  return guarded(c, [&] {
+    GLIO_REQUIRE(W > 0 && W <= 4096 && stream_ids, GLIO_ERR_ARG, "glio_select_random: bad window arguments");
+    check_select_options(opt);
+    const int F = opt->feature_res_num;
+    std::vector<int64_t> n_sel(W);
+    for (int k = 0; k < W; ++k) {
+      const int64_t n = (size_t)k < c->slots.size() && c->slots[k] ? c->slots[k]->n_match : 0;
+      n_sel[k] = (n < 1 || n - 1 < F) ? -1 : opt->random_select ? F : 0;    // return / sample F / the loop never runs
+    }
+    std::vector<SelSeg> segs;
+    for (int k = 0; k < W; ++k) {
+      Slot& sl = c->slot(k);
+      if (n_sel[k] > 0) {
+        sl.s_cpw.reserve(F); sl.s_nsd.reserve(F); sl.s_keep.reserve(F);
+        SelSeg g{};
+        g.cpw = sl.m_cpw.p; g.nsd = sl.m_nsd.p; g.nc = nullptr; g.o_cpw = sl.s_cpw.p; g.o_nsd = sl.s_nsd.p; g.o_nc = nullptr;
+        g.keep = sl.s_keep.p; g.n = sl.n_match; g.stream = (uint64_t)stream_ids[k]; g.k = F;
+        segs.push_back(g);
+      }
+    }
+    select_launch(c, segs, F, SEL_DOMAIN_WINDOW, opt->seed, opt->nonce);
+    for (int k = 0; k < W; ++k) {
+      Slot& sl = c->slot(k);
+      sl.n_sel = n_sel[k];
+      if (n_active) n_active[k] = n_sel[k] >= 0 ? n_sel[k] : sl.n_match;
+    }
+    c->items_dirty = true;
+  });
+}
+
+// globalFeatureSelection_Batch (mode 0, Estimator.cpp:3994-4055) / globalFeatureSelectionAdd_Batch (mode 1, :4057-4116) for the
+// listed pairs, visited in list order; a start/end pair that fails the size test ends the run of its cur (the reference's
+// `return`), an incremental one only skips itself (`continue`).
+int glio_batch_select_random(glio_ctx* c, const int32_t* cur, const int32_t* oth, int64_t n_pairs, int mode, const glio_select_options* opt,
+                             int64_t* n_active) {
+  if (!c) return GLIO_ERR_ARG;
+  return guarded(c, [&] {
+    GLIO_REQUIRE(n_pairs >= 0 && (n_pairs == 0 || (cur && oth)), GLIO_ERR_ARG, "glio_batch_select_random: null pair arrays");
+    GLIO_REQUIRE(mode == 0 || mode == 1, GLIO_ERR_ARG, "glio_batch_select_random: mode must be 0 (start/end) or 1 (incremental)");
+    check_select_options(opt);
+    const int Bn = opt->batch_feature_res_num;
+    std::vector<int> pidx((size_t)n_pairs);
+    std::vector<char> listed(c->pairs.size(), 0);
+    std::set<int> runs_seen;
+    for (int64_t i = 0; i < n_pairs; ++i) {
+      GLIO_REQUIRE(cur[i] != oth[i], GLIO_ERR_ARG, "glio_batch_select_random: cur == oth");
+      auto it = c->pair_index.find(std::make_pair((int)cur[i], (int)oth[i]));
+      GLIO_REQUIRE(it != c->pair_index.end(), GLIO_ERR_ARG, "glio_batch_select_random: pair was not associated");
+      GLIO_REQUIRE(!listed[it->second], GLIO_ERR_ARG, "glio_batch_select_random: pair listed twice");
+      listed[it->second] = 1; pidx[i] = it->second;
+      if (i == 0 || cur[i] != cur[i - 1])
+        GLIO_REQUIRE(runs_seen.insert(cur[i]).second, GLIO_ERR_ARG, "glio_batch_select_random: pair list is not grouped by cur");
+    }
+    std::vector<int64_t> n_sel((size_t)n_pairs);
+    bool stopped = false;
+    for (int64_t i = 0; i < n_pairs; ++i) {
+      const int64_t n = c->pairs[pidx[i]]->n_match;
+      if (i == 0 || cur[i] != cur[i - 1]) stopped = false;
+      if (mode == 0) {
+        if (!stopped && (n - 1 < Bn || n < 50)) stopped = true;
+        n_sel[i] = stopped ? -1 : Bn;
+      } else {
+        n_sel[i] = n <= Bn ? -1 : Bn;
+      }
+    }
+    std::vector<SelSeg> segs;
+    for (int64_t i = 0; i < n_pairs; ++i) {
+      if (n_sel[i] <= 0) continue;
+      glio_ctx::Pair& pr = *c->pairs[pidx[i]];
+      pr.s_cpw.reserve(Bn); pr.s_nc.reserve(6 * (size_t)Bn); pr.s_keep.reserve(Bn);
+      SelSeg g{};
+      g.cpw = pr.m_cpw.p; g.nsd = nullptr; g.nc = pr.m_nc.p; g.o_cpw = pr.s_cpw.p; g.o_nsd = nullptr; g.o_nc = pr.s_nc.p;
+      g.keep = pr.s_keep.p; g.n = pr.n_match; g.stream = ((uint64_t)(uint32_t)cur[i] << 32) | (uint32_t)oth[i]; g.k = Bn;
+      segs.push_back(g);
+    }
+    select_launch(c, segs, Bn, mode == 0 ? SEL_DOMAIN_STARTEND : SEL_DOMAIN_ADD, opt->seed, opt->nonce);
+    for (int64_t i = 0; i < n_pairs; ++i) {
+      glio_ctx::Pair& pr = *c->pairs[pidx[i]];
+      pr.n_sel = n_sel[i];
+      if (n_active) n_active[i] = n_sel[i] >= 0 ? n_sel[i] : pr.n_match;
+    }
+    c->bin_dirty = true;
+  });
+}
+
+}  // extern "C"
+
+namespace {
+
+void copy_selection(glio_ctx* c, int64_t n_sel, const DevBuf<int32_t>& keep, int64_t cap, int32_t* out, int64_t* n) {
+  if (n) *n = n_sel;
+  if (n_sel <= 0 || !out) return;
+  GLIO_REQUIRE(cap >= n_sel, GLIO_ERR_ARG, "capacity smaller than the selection");
+  GLIO_CUDA_TRY(cudaMemcpyAsync(out, keep.p, n_sel * sizeof(int32_t), cudaMemcpyDeviceToHost, c->st));
+  GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
+}
+
+}  // namespace
+
+extern "C" {
+
+int glio_get_selection(glio_ctx* c, int slot, int64_t capacity, int32_t* keep, int64_t* n) {
+  if (!c) return GLIO_ERR_ARG;
+  return guarded(c, [&] {
+    Slot& sl = c->slot(slot);
+    copy_selection(c, sl.n_sel, sl.s_keep, capacity, keep, n);
+  });
+}
+
+int glio_batch_get_selection(glio_ctx* c, int cur, int oth, int64_t capacity, int32_t* keep, int64_t* n) {
+  if (!c) return GLIO_ERR_ARG;
+  return guarded(c, [&] {
+    auto it = c->pair_index.find(std::make_pair(cur, oth));
+    GLIO_REQUIRE(it != c->pair_index.end(), GLIO_ERR_ARG, "pair was not associated");
+    glio_ctx::Pair& pr = *c->pairs[it->second];
+    copy_selection(c, pr.n_sel, pr.s_keep, capacity, keep, n);
   });
 }
 

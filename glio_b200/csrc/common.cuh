@@ -234,6 +234,21 @@ void compact_run(const AssocWork& w, const SegDesc* d_segs, int nseg, int* d_fla
 void gather_selection(const int32_t* d_keep, int64_t n, int64_t n_match, const float4* cpw, const float4* nsd, const double* nc,
                       float4* o_cpw, float4* o_nsd, double* o_nc, int* d_bad, cudaStream_t st, LaunchCounter& lc);
 
+// ---- feature selection (select.cu): one segment = one slot's or one pair's seeded sample of k of its n matches
+struct SelSeg {
+  const float4* cpw;    // the segment's matches (cp.xyz, weight)
+  const float4* nsd;    // (n_s.xyz, d_s), window slots; nullptr for pairs
+  const double* nc;     // 6 per match, pairs; nullptr for slots
+  float4* o_cpw; float4* o_nsd; double* o_nc;   // the selection buffers (same layout as gather_selection writes)
+  int32_t* keep;        // [k] the selected match indices in draw order
+  int64_t n;            // matches; the draws come from 0 .. n-2
+  uint64_t stream;
+  int32_t k, pad;
+};
+constexpr int GLIO_SEL_MAX = 4096;   // largest k (F or B) a segment may draw
+void select_sample_run(const SelSeg* d_segs, int nseg, int k_max, uint64_t seed, uint64_t domain, uint64_t nonce, cudaStream_t st,
+                       LaunchCounter& lc);
+
 // ---- K2 / K2b / K2e (eval.cu)
 struct EvalParams {
   double q_lb[4], t_lb[3];

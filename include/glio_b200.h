@@ -186,6 +186,38 @@ int glio_get_assoc_debug(glio_ctx* ctx, int slot, int64_t Q, uint8_t* status, in
  * keep[n] are indices into the slot's match list; n < 0 clears the selection (all matches active). */
 int glio_select(glio_ctx* ctx, int slot, const int32_t* keep, int64_t n);
 
+/* ---- feature selection on the device, with the reference's rules (Estimator.cpp:3894-4116) and a seeded sampler in place of its
+ * std::random_device draws (DESIGN 2).  Every selection is an ordered uniform sample without replacement of F (window) or B
+ * (batch) positions out of 0 .. n-2 of a list of n matches (the last match is never chosen, as in the reference).  Draw j:
+ *   u_j = word j % 4 of Philox4x64-10 at counter (j/4 + 1, stream, nonce, 0) with key (seed, domain) -- the words of
+ *         numpy.random.Philox(key=[seed, domain], counter=[0, stream, nonce, 0]).random_raw();
+ *   r_j = mulhi64(u_j, n-1-j), no rejection: uniform on [0, n-1-j) up to a bias below 2^-33 for n < 2^31;
+ *   index = the r_j-th (0-based) position of 0 .. n-2 not chosen yet, ascending.
+ * domain: 0 window, 1 batch start/end, 2 batch incremental.  stream: the caller's id per window slot (the keyframe index, so a
+ * keyframe's sample does not depend on its slot), (uint64)cur << 32 | oth per pair (so a sharded run selects what one context
+ * selects).  nonce: per call, for the reference's fresh draws per solve or batch round (e.g. activation * 4 + iterCount).
+ * One k_sel_sample launch per call covers every sampled slot or pair; its table goes up in one copy and the call does not
+ * synchronise the stream (only a call whose predecessor's table upload has not run yet waits for that copy).  The host decides
+ * each outcome from the match counts it already holds.  The selected records land where glio_select puts them. */
+typedef struct {
+  int32_t feature_res_num;        /* F = 100 (config_urban_hk.yaml:100), in [1, 4096] */
+  int32_t rand_set_num;           /* R = 300 (:101), >= 1; decides only which sizes the reference leaves undefined */
+  int32_t batch_feature_res_num;  /* B = 25 (:102), in [1, 4096] */
+  int32_t batch_rand_set_num;     /* BR = 400 (:103), >= B */
+  int32_t random_select;          /* 1 (:104) */
+  int32_t reserved;
+  uint64_t seed;                  /* 0 */
+  uint64_t nonce;                 /* 0 */
+} glio_select_options;
+void glio_select_default_options(glio_select_options* o);   /* the shipped configuration above */
+/* featureSelection for slots 0..W-1 after their association; stream_ids[W].  A slot of n matches keeps all of them when n < 1 or
+ * n - 1 < F, keeps none when random_select is 0 (the reference's loop never runs), else the F sampled matches in draw order.
+ * n_active[W] (may be NULL) receives the active counts. */
+int glio_select_random(glio_ctx* ctx, int W, const int64_t* stream_ids, const glio_select_options* options, int64_t* n_active);
+/* The active index list of a slot (glio_select's list or the sampled one): *n = -1 when all matches are active, else the count;
+ * keep[capacity] receives it (NULL: only *n is written; a capacity below the count is GLIO_ERR_ARG). */
+int glio_get_selection(glio_ctx* ctx, int slot, int64_t capacity, int32_t* keep, int64_t* n);
+
 /* ---- K2: evaluate all active unary plane residuals at the given body poses.
  * Replaces ceres::ResidualBlock::Evaluate over LidarPlaneNormFactor (LidarKeyframeFactor.h:73-122) + HuberLoss +
  * QuaternionParameterization and the J^T J / J^T r accumulation for those blocks.
@@ -572,6 +604,15 @@ int glio_batch_get_matches(glio_ctx* ctx, int cur, int oth, int64_t capacity, fl
                            double* normal_cent, int32_t* src, int64_t* n_match);
 /* globalFeatureSelection_Batch (Estimator.cpp:3994-4116) as an input index list; n < 0 clears */
 int glio_batch_select(glio_ctx* ctx, int cur, int oth, const int32_t* keep, int64_t n);
+/* globalFeatureSelection_Batch (mode 0) / globalFeatureSelectionAdd_Batch (mode 1) over cur[n_pairs], oth[n_pairs], grouped by cur
+ * and visited in list order (the reference visits ascending oth).  Mode 0: the first pair of a run with n - 1 < B or n < 50 and
+ * every later pair of that run keep all their matches (the reference returns); mode 1: a pair with n <= B keeps all its matches
+ * (continue).  Any other pair keeps its B sampled matches.  n_active[n_pairs] may be NULL.  GLIO_ERR_ARG, with nothing changed,
+ * when a list is not grouped by cur, lists a pair twice, has cur == oth or a pair that was never associated, mode is not 0 / 1, or
+ * an option is out of range. */
+int glio_batch_select_random(glio_ctx* ctx, const int32_t* cur, const int32_t* oth, int64_t n_pairs, int mode,
+                             const glio_select_options* options, int64_t* n_active);
+int glio_batch_get_selection(glio_ctx* ctx, int cur, int oth, int64_t capacity, int32_t* keep, int64_t* n);
 int glio_batch_pair_list(glio_ctx* ctx, int64_t capacity, int32_t* cur, int32_t* oth, int64_t* n_pairs);
 int glio_batch_clear(glio_ctx* ctx);
 
