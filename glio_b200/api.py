@@ -138,7 +138,8 @@ class Context:
     KERNELS = ["k_feat_curvature", "k_feat_select", "k_feat_voxel", "k_feat_offsets", "k_feat_gather", "k_knn_box", "k_plane_fit", "k_plane_fit_pair", "k_eval_unary", "k_eval_unary_cost", "k_transform_hist", "k_order_scatter",
                "k_compact", "k_flags", "k_cell_hist", "k_cell_scatter", "k_load_bounds", "k_scan_block", "k_scan_add",
                "k_eval_binary", "k_eval_binary_cost", "k_bin_assemble", "k_gather_sel", "k_sel_sample",
-               "k_lm_transform", "k_vox_hist", "k_vox_scatter", "k_vox_sort", "k_vox_flags", "k_vox_centroid", "k_init_bounds"]
+               "k_lm_transform", "k_vox_hist", "k_vox_scatter", "k_vox_sort", "k_vox_flags", "k_vox_centroid", "k_init_bounds",
+               "k_line_fit", "k_compact_edge", "k_seg_counts"]
 
     def lib_profile(self, on):
         self._chk(self._lib.glio_profile_enable(self._h, C.c_int(1 if on else 0)))
@@ -727,6 +728,120 @@ def _eval_edge(self, poses_body, want_jac=True):
 
 Context.set_edges = _set_edges
 Context.eval_edge = _eval_edge
+
+EDGE_VALID, EDGE_FAIL_RADIUS, EDGE_FAIL_LINE = 0, 1, 2
+
+
+class EdgeOptions(C.Structure):
+    _fields_ = [("max_sqdist", C.c_double), ("min_ratio", C.c_double), ("half_length", C.c_double), ("score", C.c_double)]
+
+
+def edge_default_options(**kw):
+    """glio_edge_default_options (max_sqdist 1.0, min_ratio 3.0, half_length 0.1, score 1.0), fields overridden by keyword."""
+    o = EdgeOptions()
+    lib().glio_edge_default_options(C.byref(o))
+    for k, v in kw.items():
+        if not hasattr(o, k):
+            raise AttributeError(k)
+        setattr(o, k, float(v))
+    return o
+
+
+def _set_edge_map(self, xyz):
+    """glio_set_edge_map: the corner map (its own grid; the surf map is untouched)."""
+    keep, p, n, stride, mem = _points_arg(xyz)
+    self._edge_map_keep = keep
+    self._chk(self._lib.glio_set_edge_map(self._h, p, C.c_int64(n), C.c_int(stride), C.c_int(mem)))
+
+
+def _edge_localmap_clear(self):
+    self._chk(self._lib.glio_edge_localmap_clear(self._h))
+
+
+def _edge_localmap_push(self, cloud_xyz, t, q, at_front=False):
+    keep, p, n, stride, mem = _points_arg(cloud_xyz)
+    t = np.ascontiguousarray(t, np.float64); q = np.ascontiguousarray(q, np.float64)
+    self._chk(self._lib.glio_edge_localmap_push(self._h, C.c_int(1 if at_front else 0), p, C.c_int64(n), C.c_int(stride), C.c_int(mem),
+                                                _ptr(t), _ptr(q)))
+
+
+def _edge_localmap_pop_front(self):
+    self._chk(self._lib.glio_edge_localmap_pop_front(self._h))
+
+
+def _edge_localmap_build(self, leaf=0.2):
+    """Concatenate the corner local map, VoxelGrid(leaf) (leaf <= 0: none) and make it the corner map; returns its size."""
+    n = C.c_int64(0)
+    self._chk(self._lib.glio_edge_localmap_build(self._h, C.c_float(leaf), C.byref(n)))
+    return int(n.value)
+
+
+def _window_set_edge_scan(self, slot, xyz):
+    """glio_window_set_edge_scan: one keyframe's corner points (host buffers stay referenced until the next association)."""
+    keep, p, n, stride, mem = _points_arg(xyz)
+    if not hasattr(self, "_edge_slot_keep"):
+        self._edge_slot_keep = {}
+    self._edge_slot_keep[slot] = keep
+    self._chk(self._lib.glio_window_set_edge_scan(self._h, C.c_int(slot), p, C.c_int64(n), C.c_int(stride), C.c_int(mem)))
+
+
+def _window_associate_edges(self, poses_body, options=None, **kw):
+    """Edge association of slots 0..W-1 against the corner map; returns the edge count per slot."""
+    pb = np.ascontiguousarray(poses_body, np.float64).reshape(-1, 7)
+    W = len(pb)
+    opt = options if options is not None else edge_default_options(**kw)
+    ne = np.zeros(W, np.int64)
+    self._chk(self._lib.glio_window_associate_edges(self._h, C.c_int(W), _ptr(pb), C.byref(opt), _ptr(ne)))
+    return ne
+
+
+def _get_edges(self, slot):
+    """A slot's edge list: cp, pa, pb (n, 3) float32, s (n,) float64, src (n,) int32 (-1 for uploaded edges), n."""
+    n = C.c_int64(0)
+    self._chk(self._lib.glio_get_edges(self._h, C.c_int(slot), C.c_int64(0), None, None, None, None, None, C.byref(n)))
+    m = int(n.value)
+    out = dict(cp=np.empty((m, 3), np.float32), pa=np.empty((m, 3), np.float32), pb=np.empty((m, 3), np.float32), s=np.empty(m),
+               src=np.empty(m, np.int32))
+    self._chk(self._lib.glio_get_edges(self._h, C.c_int(slot), C.c_int64(m), _ptr(out["cp"]), _ptr(out["pa"]), _ptr(out["pb"]),
+                                       _ptr(out["s"]), _ptr(out["src"]), C.byref(n)))
+    out["n"] = m
+    return out
+
+
+def _get_edge_debug(self, slot, Q):
+    """Per-query view of the slot's last edge association (keep_debug): status, idx5, sqd5, pm, eig (ascending)."""
+    out = dict(status=np.empty(Q, np.uint8), idx5=np.empty((Q, 5), np.int32), sqd5=np.empty((Q, 5), np.float32),
+               pm=np.empty((Q, 3), np.float32), eig=np.empty((Q, 3), np.float64))
+    self._chk(self._lib.glio_get_edge_debug(self._h, C.c_int(slot), C.c_int64(Q), _ptr(out["status"]), _ptr(out["idx5"]),
+                                            _ptr(out["sqd5"]), _ptr(out["pm"]), _ptr(out["eig"])))
+    return out
+
+
+def _eval_edge_kind(self, poses_body, jac_kind=0, want_jac=True):
+    """glio_eval_edge_kind: the edge blocks with tangent (0, = eval_edge) or ambient x,y,z quaternion columns (1, marginalisation)."""
+    pb = np.ascontiguousarray(poses_body, np.float64).reshape(-1, 7); W = len(pb)
+    H = np.zeros((W, 6, 6)) if want_jac else None; g = np.zeros((W, 6)) if want_jac else None; cost = np.zeros(W)
+    self._chk(self._lib.glio_eval_edge_kind(self._h, C.c_int(W), _ptr(pb), C.c_int(jac_kind), _ptr(H), _ptr(g), _ptr(cost)))
+    return dict(H=H, g=g, cost=cost)
+
+
+def _window_use_edges(self, on):
+    """glio_window_use_edges: window solves and marginalisations add the slots' edge blocks (default off)."""
+    self._chk(self._lib.glio_window_use_edges(self._h, C.c_int(1 if on else 0)))
+
+
+Context.eval_edge_kind = _eval_edge_kind
+Context.window_use_edges = _window_use_edges
+Context.set_edge_map = _set_edge_map
+Context.edge_localmap_clear = _edge_localmap_clear
+Context.edge_localmap_push = _edge_localmap_push
+Context.edge_localmap_pop_front = _edge_localmap_pop_front
+Context.edge_localmap_build = _edge_localmap_build
+Context.window_set_edge_scan = _window_set_edge_scan
+Context.window_associate_edges = _window_associate_edges
+Context.get_edges = _get_edges
+Context.get_edge_debug = _get_edge_debug
+
 def _batch_set_pair_matches(self, cur, oth, cp, normal_cent, weight):
     """Upload the matches of pair (cur, oth) instead of associating them (score = batch_score * weight)."""
     cp = np.ascontiguousarray(cp, np.float32).reshape(-1, 3); nc = np.ascontiguousarray(normal_cent, np.float64).reshape(-1, 6)

@@ -193,12 +193,12 @@ __global__ void __launch_bounds__(128, 5) k_plane_fit(FitArgs a) {
   }
 }
 
-void assoc_run(const GridBuild& gb, const SegDesc* d_segs, int nseg, const AssocWork& w, const AssocGates& gates,
-               const float* oth_local, int oth_stride, DevBuf<int>& cell_count, DevBuf<int>& cell_pos,
-               DevBuf<int>& scan_tmp, cudaStream_t st, LaunchCounter& lc) {
+// K1 front half, shared by the surf fit (assoc_run) and the line fit (edge_assoc_run): transform the queries, put them in cell
+// order and find their exact 5 nearest neighbours within sqrt(gate_sq) of the grid's cloud.  Qt > 0.
+static void assoc_search(const GridBuild& gb, const SegDesc* d_segs, int nseg, const AssocWork& w, float gate_sq, DevBuf<int>& cell_count,
+                         DevBuf<int>& cell_pos, DevBuf<int>& scan_tmp, cudaStream_t st, LaunchCounter& lc) {
   const GridDesc& grid = gb.desc;
   const int64_t Qt = w.Qt;
-  if (Qt <= 0) return;
   GLIO_REQUIRE(Qt < ((int64_t)1 << 31), GLIO_ERR_ARG, "assoc_run: too many queries in one launch");
   GLIO_REQUIRE(nseg > 0 && nseg < 65536, GLIO_ERR_ARG, "assoc_run: bad segment count");
   const int64_t ncell = (int64_t)grid.nx * grid.ny * grid.nz;
@@ -211,9 +211,17 @@ void assoc_run(const GridBuild& gb, const SegDesc* d_segs, int nseg, const Assoc
   GLIO_CUDA_TRY(cudaMemsetAsync(cell_count.p, 0, (size_t)(ncell + 1) * sizeof(int), st));
   lc.begin("k_order_scatter", st); k_order_scatter<<<nb, 256, 0, st>>>(grid, Qt, w.pm, cell_pos.p, cell_count.p, w.pmq); lc.end(st);
   SearchArgs sa;
-  sa.grid = grid; sa.Qt = Qt; sa.pm = w.pm; sa.pmq = w.pmq; sa.gate_sq = (float)gates.max_radius;
+  sa.grid = grid; sa.Qt = Qt; sa.pm = w.pm; sa.pmq = w.pmq; sa.gate_sq = gate_sq;
   sa.knn_idx = w.knn_idx; sa.knn_sqd = w.knn_sqd; sa.store_all_sqd = w.idx5 != nullptr;
   lc.begin("k_knn_box", st); k_knn_box<<<(unsigned)((Qt + 127) / 128), 128, 0, st>>>(sa); lc.end(st);
+}
+
+void assoc_run(const GridBuild& gb, const SegDesc* d_segs, int nseg, const AssocWork& w, const AssocGates& gates,
+               const float* oth_local, int oth_stride, DevBuf<int>& cell_count, DevBuf<int>& cell_pos,
+               DevBuf<int>& scan_tmp, cudaStream_t st, LaunchCounter& lc) {
+  const int64_t Qt = w.Qt;
+  if (Qt <= 0) return;
+  assoc_search(gb, d_segs, nseg, w, (float)gates.max_radius, cell_count, cell_pos, scan_tmp, st, lc);
   FitArgs fa;
   fa.Qt = Qt; fa.pm = w.pm; fa.pmq = w.pmq; fa.knn_idx = w.knn_idx; fa.knn_sqd = w.knn_sqd; fa.gates = gates;
   fa.pts_sorted = gb.pts.p; fa.sorted_pos = gb.sorted_pos.p; fa.oth_local = oth_local; fa.oth_stride = oth_stride;
@@ -283,6 +291,187 @@ void compact_run(const AssocWork& w, const SegDesc* d_segs, int nseg, int* d_fla
                  const void* d_dst /*CompactDst[nseg]*/, int* d_counts, cudaStream_t st, LaunchCounter& lc) {
   compact_count(w, d_segs, nseg, d_flags, d_pos, scan_tmp, d_counts, st, lc);
   compact_scatter(w, d_segs, nseg, d_pos, d_dst, st, lc);
+}
+
+// ---------------------------------------------------------------------------------------------------
+// K1e: scan-to-map EDGE association (glio_window_associate_edges).  The reference has no edge association; the line form
+// (curr_point, last_point_a, last_point_b, s) of LidarEdgeFactor is built here by the arithmetic include/glio_b200.h specifies,
+// and tests/edge_reference.py restates it in Python doubles.  Every operation is an explicit round-to-nearest intrinsic and the
+// file is compiled -fmad=false, so both agree bit for bit.  Queries, neighbours and the gate on the 5th squared distance come from
+// the same K1 front half (assoc_search) as the surf path.
+// ---------------------------------------------------------------------------------------------------
+constexpr int EDGE_JACOBI_MAX_SWEEPS = 32;
+
+__device__ __forceinline__ double ddiv_rn(double a, double b) { return __ddiv_rn(a, b); }
+
+// One rotation of the cyclic Jacobi method zeroing a[p][q] of the symmetric 3x3 matrix a (both triangles kept), accumulated
+// into the columns of v.  An off-diagonal element that no longer changes either diagonal element in double (|a_ii| + 100|a_pq|
+// == |a_ii| for i = p and q) is set to zero without a rotation.
+//   theta = (a_qq - a_pp) / (2 a_pq),  t = sgn(theta) / (|theta| + sqrt(theta^2 + 1))  (sgn(0) = +1),
+//   c = 1 / sqrt(t^2 + 1),  s = t c,  a_pp -= t a_pq,  a_qq += t a_pq,  a_pq = 0,
+//   r != p, q:  a_rp = c a_rp - s a_rq,  a_rq = s a_rp + c a_rq;   rows i of v:  v_ip = c v_ip - s v_iq,  v_iq = s v_ip + c v_iq
+__device__ __forceinline__ void jacobi_rotate(double (&a)[3][3], double (&v)[3][3], const int p, const int q) {
+  const double apq = a[p][q];
+  if (apq == 0.0) return;
+  const double g = dmul(100.0, fabs(apq));
+  if (dadd(fabs(a[p][p]), g) == fabs(a[p][p]) && dadd(fabs(a[q][q]), g) == fabs(a[q][q])) { a[p][q] = 0.0; a[q][p] = 0.0; return; }
+  const double theta = ddiv_rn(dsub(a[q][q], a[p][p]), dmul(2.0, apq));
+  double t = ddiv_rn(1.0, dadd(fabs(theta), __dsqrt_rn(dadd(dmul(theta, theta), 1.0))));
+  if (theta < 0.0) t = -t;
+  const double c = ddiv_rn(1.0, __dsqrt_rn(dadd(dmul(t, t), 1.0)));
+  const double s = dmul(t, c);
+  const double tapq = dmul(t, apq);
+  a[p][p] = dsub(a[p][p], tapq);
+  a[q][q] = dadd(a[q][q], tapq);
+  a[p][q] = 0.0; a[q][p] = 0.0;
+  const int r = 3 - p - q;
+  const double arp = a[r][p], arq = a[r][q];
+  a[r][p] = a[p][r] = dsub(dmul(c, arp), dmul(s, arq));
+  a[r][q] = a[q][r] = dadd(dmul(s, arp), dmul(c, arq));
+#pragma unroll
+  for (int i = 0; i < 3; ++i) {
+    const double vip = v[i][p], viq = v[i][q];
+    v[i][p] = dsub(dmul(c, vip), dmul(s, viq));
+    v[i][q] = dadd(dmul(s, vip), dmul(c, viq));
+  }
+}
+
+// Eigen-decomposition of the symmetric 3x3 a: sweeps of the rotations (0,1), (0,2), (1,2) until all three off-diagonal
+// elements are zero, at most EDGE_JACOBI_MAX_SWEEPS sweeps.  lam[0..2]: the diagonal sorted ascending, ties by index (a stable
+// sort); dir: the column of v belonging to lam[2], signed so that its largest-magnitude component (lowest index on ties) is positive.
+__device__ __forceinline__ void jacobi_eig3(double (&a)[3][3], double lam[3], double dir[3]) {
+  double v[3][3] = {{1.0, 0.0, 0.0}, {0.0, 1.0, 0.0}, {0.0, 0.0, 1.0}};
+#pragma unroll 1
+  for (int sweep = 0; sweep < EDGE_JACOBI_MAX_SWEEPS; ++sweep) {
+    if (a[0][1] == 0.0 && a[0][2] == 0.0 && a[1][2] == 0.0) break;
+    jacobi_rotate(a, v, 0, 1);
+    jacobi_rotate(a, v, 0, 2);
+    jacobi_rotate(a, v, 1, 2);
+  }
+  // three compare-exchanges of adjacent (value, index) pairs, strict: a stable ascending sort (kept in registers)
+  double l0 = a[0][0], l1 = a[1][1], l2 = a[2][2];
+  int o0 = 0, o1 = 1, o2 = 2;
+  if (l0 > l1) { const double t = l0; l0 = l1; l1 = t; const int i = o0; o0 = o1; o1 = i; }
+  if (l1 > l2) { const double t = l1; l1 = l2; l2 = t; const int i = o1; o1 = o2; o2 = i; }
+  if (l0 > l1) { const double t = l0; l0 = l1; l1 = t; const int i = o0; o0 = o1; o1 = i; }
+  lam[0] = l0; lam[1] = l1; lam[2] = l2;
+  dir[0] = o2 == 0 ? v[0][0] : (o2 == 1 ? v[0][1] : v[0][2]);
+  dir[1] = o2 == 0 ? v[1][0] : (o2 == 1 ? v[1][1] : v[1][2]);
+  dir[2] = o2 == 0 ? v[2][0] : (o2 == 1 ? v[2][1] : v[2][2]);
+  double big = dir[0];
+  if (fabs(dir[1]) > fabs(big)) big = dir[1];
+  if (fabs(dir[2]) > fabs(big)) big = dir[2];
+  if (big < 0.0) { dir[0] = -dir[0]; dir[1] = -dir[1]; dir[2] = -dir[2]; }
+}
+
+struct LineFitArgs {
+  int64_t Qt;
+  const float4* pmq;          // queries in cell-sorted order, .w = scan index
+  const int32_t* knn_idx;
+  const float* knn_sqd;
+  const float4* pts_sorted;   // the corner map, cell-sorted (x,y,z,idx)
+  const int* sorted_pos;      // original index -> position in pts_sorted
+  double max_sqdist, min_ratio, half_length;
+  uint8_t* status;
+  float4* pa;                 // per query (scan order): float(c + h v), float(c - h v)
+  float4* pb;
+  // debug (nullable)
+  int32_t* idx5;
+  float* sqd5;
+  double* eig;                // 3 per query, ascending
+};
+
+// One thread per query, in sorted order.  Gate on the squared 5th distance -> centroid -> scatter matrix -> Jacobi -> line gate.
+__global__ void __launch_bounds__(128) k_line_fit(LineFitArgs a) {
+  const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= a.Qt) return;
+  const int64_t g = __float_as_int(a.pmq[p].w);
+  int id[5];
+#pragma unroll
+  for (int j = 0; j < 5; ++j) id[j] = a.knn_idx[(int64_t)j * a.Qt + p];
+  const float d4 = a.knn_sqd[4 * a.Qt + p];
+  uint8_t st = GLIO_EDGE_FAIL_RADIUS;
+  double lam[3] = {0.0, 0.0, 0.0};
+  float4 oa = make_float4(0.f, 0.f, 0.f, 0.f), ob = oa;
+  if (id[4] != 0x7fffffff && (double)d4 < a.max_sqdist) {
+    double x[3][5];
+#pragma unroll
+    for (int j = 0; j < 5; ++j) {
+      const float4 m = __ldg(&a.pts_sorted[__ldg(&a.sorted_pos[id[j]])]);
+      x[0][j] = (double)m.x; x[1][j] = (double)m.y; x[2][j] = (double)m.z;
+    }
+    double c[3];
+#pragma unroll
+    for (int i = 0; i < 3; ++i) c[i] = ddiv_rn(dadd(dadd(dadd(dadd(x[i][0], x[i][1]), x[i][2]), x[i][3]), x[i][4]), 5.0);
+    double A[3][3] = {{0.0, 0.0, 0.0}, {0.0, 0.0, 0.0}, {0.0, 0.0, 0.0}};
+#pragma unroll
+    for (int j = 0; j < 5; ++j) {
+      const double dx = dsub(x[0][j], c[0]), dy = dsub(x[1][j], c[1]), dz = dsub(x[2][j], c[2]);
+      A[0][0] = dadd(A[0][0], dmul(dx, dx)); A[0][1] = dadd(A[0][1], dmul(dx, dy)); A[0][2] = dadd(A[0][2], dmul(dx, dz));
+      A[1][1] = dadd(A[1][1], dmul(dy, dy)); A[1][2] = dadd(A[1][2], dmul(dy, dz)); A[2][2] = dadd(A[2][2], dmul(dz, dz));
+    }
+    A[1][0] = A[0][1]; A[2][0] = A[0][2]; A[2][1] = A[1][2];
+    double v[3];
+    jacobi_eig3(A, lam, v);
+    if (lam[2] > dmul(a.min_ratio, lam[1])) {
+      st = GLIO_EDGE_VALID;
+      const double h = a.half_length;
+      oa = make_float4((float)dadd(c[0], dmul(h, v[0])), (float)dadd(c[1], dmul(h, v[1])), (float)dadd(c[2], dmul(h, v[2])), 0.f);
+      ob = make_float4((float)dsub(c[0], dmul(h, v[0])), (float)dsub(c[1], dmul(h, v[1])), (float)dsub(c[2], dmul(h, v[2])), 0.f);
+    } else st = GLIO_EDGE_FAIL_LINE;
+  }
+  a.status[g] = st;
+  a.pa[g] = oa; a.pb[g] = ob;
+  if (a.idx5) {
+#pragma unroll
+    for (int j = 0; j < 5; ++j) {
+      a.idx5[5 * g + j] = (id[j] == 0x7fffffff) ? -1 : id[j];
+      a.sqd5[5 * g + j] = a.knn_sqd[(int64_t)j * a.Qt + p];
+    }
+    a.eig[3 * g] = lam[0]; a.eig[3 * g + 1] = lam[1]; a.eig[3 * g + 2] = lam[2];
+  }
+}
+
+void edge_assoc_run(const GridBuild& gb, const SegDesc* d_segs, int nseg, const AssocWork& w, const EdgeFitParams& ep, float4* pa, float4* pb,
+                    double* eig, DevBuf<int>& cell_count, DevBuf<int>& cell_pos, DevBuf<int>& scan_tmp, cudaStream_t st, LaunchCounter& lc) {
+  const int64_t Qt = w.Qt;
+  if (Qt <= 0) return;
+  assoc_search(gb, d_segs, nseg, w, (float)ep.max_sqdist, cell_count, cell_pos, scan_tmp, st, lc);
+  LineFitArgs la;
+  la.Qt = Qt; la.pmq = w.pmq; la.knn_idx = w.knn_idx; la.knn_sqd = w.knn_sqd;
+  la.pts_sorted = gb.pts.p; la.sorted_pos = gb.sorted_pos.p;
+  la.max_sqdist = ep.max_sqdist; la.min_ratio = ep.min_ratio; la.half_length = ep.half_length;
+  la.status = w.status; la.pa = pa; la.pb = pb; la.idx5 = w.idx5; la.sqd5 = w.sqd5; la.eig = eig;
+  lc.begin("k_line_fit", st); k_line_fit<<<(unsigned)((Qt + 127) / 128), 128, 0, st>>>(la); lc.end(st);
+  GLIO_CUDA_TRY(cudaGetLastError());
+}
+
+// the valid edge records of every segment into its slot's buffers, in scan order (positions from compact_count)
+__global__ void __launch_bounds__(256) k_compact_edge(const SegDesc* __restrict__ segs, int64_t Qt, const uint16_t* __restrict__ segid,
+                                                      const uint8_t* __restrict__ status, const int* __restrict__ pos,
+                                                      const float4* __restrict__ pa, const float4* __restrict__ pb, float score,
+                                                      const EdgeDst* __restrict__ dst) {
+  const int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= Qt) return;
+  if (status[g] != GLIO_EDGE_VALID) return;
+  const int s = segid[g];
+  const SegDesc& sd = segs[s];
+  const int lp = pos[g] - pos[sd.offset];
+  const int64_t li = g - sd.offset;
+  const float* src = sd.src + li * sd.stride;
+  const EdgeDst d = dst[s];
+  d.cps[lp] = make_float4(src[0], src[1], src[2], score);
+  d.pa[lp] = pa[g];
+  d.pb[lp] = pb[g];
+  d.src[lp] = (int32_t)li;
+}
+
+void compact_edge_scatter(const AssocWork& w, const SegDesc* d_segs, const int* d_pos, const float4* pa, const float4* pb, float score,
+                          const EdgeDst* d_dst, cudaStream_t st, LaunchCounter& lc) {
+  const int64_t Qt = w.Qt;
+  const unsigned nb = (unsigned)((Qt + 255) / 256);
+  lc.begin("k_compact_edge", st); k_compact_edge<<<nb, 256, 0, st>>>(d_segs, Qt, w.seg, w.status, d_pos, pa, pb, score, d_dst); lc.end(st);
+  GLIO_CUDA_TRY(cudaGetLastError());
 }
 
 // gather (feature selection as an input index list)

@@ -36,8 +36,15 @@ struct Slot {
   DevBuf<float4> s_cpw, s_nsd;   // selected subset
   DevBuf<int32_t> s_keep;        // its match indices (glio_select's list or the sampler's draws, glio_get_selection)
   int64_t n_sel = -1;            // -1: no selection -> all matches are active
-  DevBuf<float4> e_cps, e_pa, e_pb;  // edge correspondences (caller-provided)
+  DevBuf<float4> e_cps, e_pa, e_pb;  // edge correspondences (glio_set_edges or glio_window_associate_edges)
   int64_t n_edge = 0;
+  DevBuf<int32_t> e_src;             // scan index of each edge, when they come from glio_window_associate_edges
+  bool e_has_src = false;
+  // corner scan (glio_window_set_edge_scan): same layout and ownership rules as scan / scan_ptr
+  int64_t eQ = 0;
+  int estride = 3;
+  DevBuf<float> escan;
+  const float* escan_ptr = nullptr;
   // debug (keep_debug)
   DevBuf<uint8_t> dbg_status;
   DevBuf<int32_t> dbg_idx5;
@@ -45,9 +52,16 @@ struct Slot {
   DevBuf<float4> dbg_pm;
   DevBuf<double> dbg_plane;
   int64_t dbg_Q = 0;
+  DevBuf<uint8_t> edbg_status;       // the same for the last edge association, eigenvalues in place of the plane
+  DevBuf<int32_t> edbg_idx5;
+  DevBuf<float> edbg_sqd5;
+  DevBuf<float4> edbg_pm;
+  DevBuf<double> edbg_eig;
+  int64_t edbg_Q = 0;
   void release() {
     scan.release(); m_cpw.release(); m_nsd.release(); m_src.release(); s_cpw.release(); s_nsd.release(); s_keep.release(); e_cps.release(); e_pa.release(); e_pb.release();
     dbg_status.release(); dbg_idx5.release(); dbg_sqd5.release(); dbg_pm.release(); dbg_plane.release();
+    e_src.release(); escan.release(); edbg_status.release(); edbg_idx5.release(); edbg_sqd5.release(); edbg_pm.release(); edbg_eig.release();
   }
 };
 
@@ -151,6 +165,16 @@ struct glio_ctx {
   // local map maintenance (SURVEY 8 f-1): world-frame keyframe clouds in deque order, concatenation, voxel filter work space
   LocalMap lm;
   DevBuf<float> lm_stage; int64_t map_n = 0;
+  // edge association (K1e): the corner map, the corner local map, and the per-query line-fit outputs (scan order)
+  GridBuild edge_map; bool has_edge_map = false; DevBuf<float> edge_map_stage;
+  LocalMap elm; DevBuf<float> elm_stage;
+  DevBuf<float4> w_pa, w_pb; DevBuf<double> w_eig; DevBuf<EdgeDst> d_edst;
+  // edge blocks inside the window solve and marginalisation (glio_window_use_edges): the K2e work-item plan of slots 0..W-1, rebuilt
+  // only when an edge list or W changes; K2e runs on the main stream before K2 and its W x 28 result is copied into pinned h_eout
+  // there, so K2's completion flag covers it.  edge_epoch: the evaluation epoch whose result must add h_eout.
+  bool use_edges = false, edge_items_dirty = true; int edge_items_W = -1, n_edge_items = 0;
+  DevBuf<EdgeItem> se_items; DevBuf<int> se_start; DevBuf<double> se_part, se_out, se_poses; PinnedBuf<double> h_eout;
+  unsigned int edge_epoch = 0; int edge_W = 0;
   // front-end odometries created on this context (glio_odom_create); glio_destroy frees those still attached
   std::vector<glio_odom*> odoms;
   // loop-closure registration: glio_icp_align's work space and staging, and the loop objects created on this context
@@ -412,8 +436,55 @@ void wait_marg_copied(glio_ctx* c) {
   }
 }
 
-unsigned int eval_unary_launch(glio_ctx* c, int W, const double* poses_body, int jac_kind, bool want_jac, const EvalTarget* tgt = nullptr) {
+// K2e work items of slots 0..W-1 (GLIO_ITEM_MAX residuals each, keyframe order); start[k] = first item of keyframe k
+std::vector<EdgeItem> plan_edge_items(const glio_ctx* c, int W, std::vector<int>& start) {
+  std::vector<EdgeItem> items;
+  start.assign(W + 1, 0);
+  for (int k = 0; k < W; ++k) {
+    start[k] = (int)items.size();
+    if ((size_t)k >= c->slots.size() || !c->slots[k]) continue;
+    const Slot& sl = *c->slots[k];
+    for (int64_t o = 0; o < sl.n_edge; o += GLIO_ITEM_MAX) {
+      EdgeItem it; it.cps = sl.e_cps.p + o; it.pa = sl.e_pa.p + o; it.pb = sl.e_pb.p + o;
+      it.count = (int32_t)std::min<int64_t>(GLIO_ITEM_MAX, sl.n_edge - o); it.kf = k; items.push_back(it);
+    }
+  }
+  start[W] = (int)items.size();
+  return items;
+}
+
+// Queues the edge blocks of one solve / marginalisation evaluation (poses already in c->h_poses): the pose upload, K2e and the copy
+// of its result into c->h_eout, all on the main stream ahead of K2.  Returns false when slots 0..W-1 hold no edge.
+bool edge_blocks_launch(glio_ctx* c, int W, int jac_kind, bool want_jac) {
+  if (c->edge_items_dirty || c->edge_items_W != W) {
+    std::vector<int> start;
+    const std::vector<EdgeItem> items = plan_edge_items(c, W, start);
+    c->se_items.reserve(items.size() + 1); c->se_start.reserve(W + 1); c->se_part.reserve((items.size() + 1) * GLIO_NACC);
+    if (!items.empty()) GLIO_CUDA_TRY(cudaMemcpyAsync(c->se_items.p, items.data(), items.size() * sizeof(EdgeItem), cudaMemcpyHostToDevice, c->st));
+    GLIO_CUDA_TRY(cudaMemcpyAsync(c->se_start.p, start.data(), (W + 1) * sizeof(int), cudaMemcpyHostToDevice, c->st));
+    GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));   // items / start are stack vectors
+    c->n_edge_items = (int)items.size(); c->edge_items_W = W; c->edge_items_dirty = false;
+  }
+  if (c->n_edge_items == 0) return false;
+  c->se_out.reserve((size_t)W * GLIO_NACC); c->se_poses.reserve((size_t)W * 7); c->h_eout.reserve((size_t)W * GLIO_NACC);
+  if (!c->d_ticket.p) { c->d_ticket.reserve(1); GLIO_CUDA_TRY(cudaMemsetAsync(c->d_ticket.p, 0, sizeof(unsigned int), c->st)); }
+  GLIO_CUDA_TRY(cudaMemcpyAsync(c->se_poses.p, c->h_poses.p, (size_t)W * 7 * sizeof(double), cudaMemcpyHostToDevice, c->st));
+  eval_edge_run(c->se_items.p, c->n_edge_items, W, c->se_poses.p, eval_params(c), jac_kind, want_jac, c->se_part.p, c->se_out.p, c->se_start.p,
+                c->d_ticket.p, c->st, c->lc);
+  GLIO_CUDA_TRY(cudaMemcpyAsync(c->h_eout.p, c->se_out.p, (size_t)W * GLIO_NACC * sizeof(double), cudaMemcpyDeviceToHost, c->st));
+  return true;
+}
+
+void add_edge_blocks(glio_ctx* c, int W) {
+  for (size_t i = 0; i < (size_t)W * GLIO_NACC; ++i) c->h_out.p[i] += c->h_eout.p[i];
+}
+
+// with_edges: a solve or marginalisation evaluation of the context's own slots, which adds their edge blocks when
+// glio_window_use_edges is on
+unsigned int eval_unary_launch(glio_ctx* c, int W, const double* poses_body, int jac_kind, bool want_jac, const EvalTarget* tgt = nullptr,
+                               bool with_edges = false) {
   wait_marg_copied(c);
+  const bool own_slots = tgt == nullptr;
   EvalTarget own{};
   if (!tgt) {
     build_items(c, W);
@@ -424,13 +495,16 @@ unsigned int eval_unary_launch(glio_ctx* c, int W, const double* poses_body, int
   // pinned host memory and raises an epoch flag the host spins on.  This replaces H2D copy + launch + D2H copy +
   // stream synchronise on the per-iteration path, and lets the caller evaluate its host factors while the kernel runs.
   memcpy(c->h_poses.p, poses_body, (size_t)W * 7 * sizeof(double));
+  const bool edges = with_edges && own_slots && c->use_edges && edge_blocks_launch(c, W, jac_kind, want_jac);
   if (tgt->n_items <= 0) {
     GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
     memset(c->h_out.p, 0, (size_t)W * GLIO_NACC * sizeof(double));
+    if (edges) add_edge_blocks(c, W);
     return 0u;
   }
   if (!c->h_flag.p) { c->h_flag.reserve(4); memset(c->h_flag.p, 0, 4 * sizeof(unsigned int)); }
   const unsigned int epoch = ++c->eval_epoch;
+  if (edges) { c->edge_epoch = epoch; c->edge_W = W; }
   if (W > EV_MAXW) GLIO_CUDA_TRY(cudaMemcpyAsync(c->d_poses.p, c->h_poses.p, (size_t)W * 7 * sizeof(double), cudaMemcpyHostToDevice, c->st));
   eval_unary_run(tgt->d_items, tgt->n_items, W, c->d_poses.p, tgt->ep, jac_kind, want_jac, tgt->d_partials, c->h_out.p,
                  tgt->d_kf_item_start, c->d_ticket.p, c->st, c->lc, c->h_flag.p, epoch, c->h_poses.p);
@@ -454,6 +528,7 @@ void eval_unary_wait(glio_ctx* c, unsigned int epoch) {
     }
   }
   std::atomic_thread_fence(std::memory_order_acquire);
+  if (epoch == c->edge_epoch) add_edge_blocks(c, c->edge_W);   // K2e and its copy ran before K2 on the same stream
 }
 
 // device evaluation of all active unary residuals -> c->h_out (W x 28: 21 upper-tri H, 6 g, 1 cost), synchronised
@@ -514,6 +589,9 @@ void glio_destroy(glio_ctx* c) {
   if (c->st) cudaStreamSynchronize(c->st);
   c->map.release(); c->map_stage.release(); c->map_stage2.release(); if (c->ev_map) cudaEventDestroy(c->ev_map);
   c->lm.release(); c->lm_stage.release();
+  c->edge_map.release(); c->edge_map_stage.release(); c->elm.release(); c->elm_stage.release();
+  c->w_pa.release(); c->w_pb.release(); c->w_eig.release(); c->d_edst.release();
+  c->se_items.release(); c->se_start.release(); c->se_part.release(); c->se_out.release(); c->se_poses.release(); c->h_eout.release();
   for (auto& f : c->frames) { f.second->scan.release(); f.second->grid.release(); }
   for (auto& p : c->pairs) p->release();
   c->d_bin_items.release(); c->d_pair_item_start.release(); c->d_kf_inc_start.release(); c->d_inc.release(); c->d_bin_partials.release();
@@ -659,31 +737,52 @@ int glio_map_prefetch(glio_ctx* c, const float* xyz, int64_t M, int stride) {
   });
 }
 
-// ---- local map maintenance on the device (Estimator.cpp:3529-3631 buildLocalMapWithLandMark, :3615-3618 downSampleCloud) ----
-int glio_localmap_clear(glio_ctx* c) {
+}  // extern "C"
+
+// the context's two local maps (surf: lm, corner: elm) share these
+static int localmap_clear(glio_ctx* c, LocalMap& lm) {
   if (!c) return GLIO_ERR_ARG;
   return guarded(c, [&] {
     GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
-    c->lm.clear();
+    lm.clear();
   });
 }
 
-int glio_localmap_push(glio_ctx* c, int at_front, const float* cloud_xyz, int64_t n, int stride, int mem, const double t[3], const double q[4]) {
+static int localmap_push(glio_ctx* c, LocalMap& lm, DevBuf<float>& stage, int at_front, const float* cloud_xyz, int64_t n, int stride, int mem,
+                         const double t[3], const double q[4]) {
   if (!c) return GLIO_ERR_ARG;
   return guarded(c, [&] {
     GLIO_REQUIRE(t && q, GLIO_ERR_ARG, "null pose");
-    const float* d = stage_points(c, c->lm_stage, cloud_xyz, n, stride, mem);
-    c->lm.push(at_front != 0, d, stride, n, t, q, c->st, c->lc);           // transformCloud: float(q*double(p)+t)
+    const float* d = stage_points(c, stage, cloud_xyz, n, stride, mem);
+    lm.push(at_front != 0, d, stride, n, t, q, c->st, c->lc);                // transformCloud: float(q*double(p)+t)
     if (mem != GLIO_DEVICE) GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));    // the staging buffer is reused by the next push
   });
 }
 
-int glio_localmap_pop_front(glio_ctx* c) {
+static int localmap_pop_front(glio_ctx* c, LocalMap& lm) {
   if (!c) return GLIO_ERR_ARG;
   return guarded(c, [&] {
-    GLIO_REQUIRE(!c->lm.frames.empty(), GLIO_ERR_STATE, "local map holds no keyframe cloud");
-    c->lm.pop_front();
+    GLIO_REQUIRE(!lm.frames.empty(), GLIO_ERR_STATE, "local map holds no keyframe cloud");
+    lm.pop_front();
   });
+}
+
+extern "C" {
+
+// ---- local map maintenance on the device (Estimator.cpp:3529-3631 buildLocalMapWithLandMark, :3615-3618 downSampleCloud) ----
+int glio_localmap_clear(glio_ctx* c) {
+  if (!c) return GLIO_ERR_ARG;
+  return localmap_clear(c, c->lm);
+}
+
+int glio_localmap_push(glio_ctx* c, int at_front, const float* cloud_xyz, int64_t n, int stride, int mem, const double t[3], const double q[4]) {
+  if (!c) return GLIO_ERR_ARG;
+  return localmap_push(c, c->lm, c->lm_stage, at_front, cloud_xyz, n, stride, mem, t, q);
+}
+
+int glio_localmap_pop_front(glio_ctx* c) {
+  if (!c) return GLIO_ERR_ARG;
+  return localmap_pop_front(c, c->lm);
 }
 
 int glio_localmap_size(glio_ctx* c, int* n_frames, int64_t* n_points) {
@@ -787,7 +886,8 @@ int glio_window_set_scan(glio_ctx* c, int slot, const float* scan, int64_t Q, in
 }
 
 // slideWindow (GLIO/src/Estimator.cpp: the oldest keyframe leaves, every other one moves down one slot): O(1) per slot, no
-// copies; the matches of the slots move with them.  The new keyframe's scan then goes into slot W-1 with glio_window_set_scan.
+// copies; the matches, corner scans and edges of the slots move with them.  The new keyframe's scan then goes into slot W-1 with
+// glio_window_set_scan (and its corner scan with glio_window_set_edge_scan).
 int glio_window_slide(glio_ctx* c, int W) {
   if (!c) return GLIO_ERR_ARG;
   return guarded(c, [&] {
@@ -797,8 +897,185 @@ int glio_window_slide(glio_ctx* c, int W) {
     std::unique_ptr<Slot> first = std::move(c->slots[0]);
     for (int k = 0; k + 1 < W; ++k) c->slots[k] = std::move(c->slots[k + 1]);
     c->slots[W - 1] = std::move(first);                       // its buffers are reused by the next upload
-    if (c->slots[W - 1]) { c->slots[W - 1]->Q = 0; c->slots[W - 1]->scan_ptr = nullptr; c->slots[W - 1]->n_match = 0; c->slots[W - 1]->n_sel = -1; }
-    c->items_dirty = true;
+    if (c->slots[W - 1]) {
+      Slot& s = *c->slots[W - 1];
+      s.Q = 0; s.scan_ptr = nullptr; s.n_match = 0; s.n_sel = -1;
+      s.eQ = 0; s.escan_ptr = nullptr; s.n_edge = 0; s.e_has_src = false;   // the dropped keyframe's corners and edges leave with it
+      s.dbg_Q = 0; s.edbg_Q = 0;                                              // and its debug views
+    }
+    c->items_dirty = true; c->edge_items_dirty = true;
+  });
+}
+
+// The corner scan of one keyframe, with the upload rules of glio_window_set_scan.
+int glio_window_set_edge_scan(glio_ctx* c, int slot, const float* xyz, int64_t Q, int stride, int mem) {
+  if (!c) return GLIO_ERR_ARG;
+  return guarded(c, [&] {
+    GLIO_REQUIRE(xyz != nullptr && Q > 0, GLIO_ERR_ARG, "null or empty point array");
+    GLIO_REQUIRE(stride >= 3 && stride <= 64, GLIO_ERR_ARG, "stride_floats must be in [3,64]");
+    Slot& sl = c->slot(slot);
+    if (mem == GLIO_DEVICE) sl.escan_ptr = xyz;
+    else {
+      GLIO_CUDA_TRY(cudaEventRecord(c->ev_main, c->st));
+      GLIO_CUDA_TRY(cudaStreamWaitEvent(c->st_copy, c->ev_main, 0));
+      sl.escan.reserve((size_t)Q * stride);
+      GLIO_CUDA_TRY(cudaMemcpyAsync(sl.escan.p, xyz, (size_t)Q * stride * sizeof(float), cudaMemcpyHostToDevice, c->st_copy));
+      sl.escan_ptr = sl.escan.p;
+      GLIO_CUDA_TRY(cudaEventRecord(c->ev_scans, c->st_copy)); c->scans_pending = true;
+    }
+    sl.eQ = Q; sl.estride = stride;
+  });
+}
+
+void glio_edge_default_options(glio_edge_options* o) {
+  if (!o) return;
+  o->max_sqdist = 1.0; o->min_ratio = 3.0; o->half_length = 0.1; o->score = 1.0;
+}
+
+int glio_set_edge_map(glio_ctx* c, const float* xyz, int64_t M, int stride, int mem) {
+  if (!c) return GLIO_ERR_ARG;
+  return guarded(c, [&] {
+    GLIO_REQUIRE(M >= 5, GLIO_ERR_ARG, "corner map needs at least 5 points");
+    const float* d = stage_points(c, c->edge_map_stage, xyz, M, stride, mem);
+    grid_build(c->edge_map, d, stride, M, nullptr, nullptr, c->prm.cell_size, c->pts_per_cell, c->st, c->lc);
+    c->has_edge_map = true;
+  });
+}
+
+int glio_edge_localmap_clear(glio_ctx* c) {
+  if (!c) return GLIO_ERR_ARG;
+  return localmap_clear(c, c->elm);
+}
+
+int glio_edge_localmap_push(glio_ctx* c, int at_front, const float* cloud_xyz, int64_t n, int stride, int mem, const double t[3], const double q[4]) {
+  if (!c) return GLIO_ERR_ARG;
+  return localmap_push(c, c->elm, c->elm_stage, at_front, cloud_xyz, n, stride, mem, t, q);
+}
+
+int glio_edge_localmap_pop_front(glio_ctx* c) {
+  if (!c) return GLIO_ERR_ARG;
+  return localmap_pop_front(c, c->elm);
+}
+
+int glio_edge_localmap_build(glio_ctx* c, float leaf, int64_t* n_map) {
+  if (!c) return GLIO_ERR_ARG;
+  return guarded(c, [&] {
+    GLIO_REQUIRE(c->elm.n_points() >= 5, GLIO_ERR_STATE, "corner local map needs at least 5 points");
+    const float* pts = nullptr; int stride = 0; bool filtered = false;
+    const int64_t m = c->elm.build(leaf, &pts, &stride, &filtered, c->st, c->lc);
+    GLIO_REQUIRE(!filtered || m >= 5, GLIO_ERR_STATE, "down-sampled corner local map has fewer than 5 points");
+    grid_build(c->edge_map, pts, stride, m, nullptr, nullptr, c->prm.cell_size, c->pts_per_cell, c->st, c->lc);
+    c->has_edge_map = true;
+    if (n_map) *n_map = m;
+  });
+}
+
+int glio_window_associate_edges(glio_ctx* c, int W, const double* poses_body, const glio_edge_options* options, int64_t* n_edge) {
+  if (!c) return GLIO_ERR_ARG;
+  return guarded(c, [&] {
+    GLIO_REQUIRE(W > 0 && W <= 4096 && poses_body, GLIO_ERR_ARG, "bad window arguments");
+    glio_edge_options o; if (options) o = *options; else glio_edge_default_options(&o);
+    GLIO_REQUIRE(std::isfinite(o.max_sqdist) && o.max_sqdist > 0.0 && std::isfinite(o.min_ratio) && o.min_ratio >= 0.0 &&
+                 std::isfinite(o.half_length) && o.half_length > 0.0 && std::isfinite(o.score), GLIO_ERR_ARG,
+                 "glio_edge_options: need max_sqdist > 0, min_ratio >= 0, half_length > 0 and a finite score");
+    GLIO_REQUIRE(c->has_edge_map, GLIO_ERR_STATE, "glio_set_edge_map must be called before edge association");
+    for (int k = 0; k < W; ++k)
+      GLIO_REQUIRE((size_t)k < c->slots.size() && c->slots[k] && c->slots[k]->eQ > 0 && c->slots[k]->escan_ptr, GLIO_ERR_STATE, "slot has no corner scan");
+    if (c->scans_pending) { GLIO_CUDA_TRY(cudaStreamWaitEvent(c->st, c->ev_scans, 0)); c->scans_pending = false; }
+    const bool keep_debug = c->prm.keep_debug != 0;
+    std::vector<SegDesc> segs(W);
+    std::vector<EdgeDst> dst(W);
+    int64_t Qt = 0;
+    for (int k = 0; k < W; ++k) {
+      Slot& sl = *c->slots[k];
+      segs[k].src = sl.escan_ptr; segs[k].stride = sl.estride; segs[k].count = sl.eQ; segs[k].offset = Qt;
+      lidar_pose_in_map(c->prm.q_lb, c->prm.t_lb, poses_body + 7 * k, segs[k].t, segs[k].q);   // Estimator.cpp:2216-2217
+      Qt += sl.eQ;
+    }
+    GLIO_REQUIRE(Qt < ((int64_t)1 << 31), GLIO_ERR_ARG, "glio_window_associate_edges: too many corner points in one window");
+    ensure_work(c, Qt, false, keep_debug);
+    c->w_pa.reserve((size_t)Qt); c->w_pb.reserve((size_t)Qt);
+    if (keep_debug) c->w_eig.reserve((size_t)Qt * 3);
+    c->d_segs.reserve(W); c->d_edst.reserve(W); c->d_counts.reserve(W); c->h_counts.reserve(W);
+    // the slots' edge lists are replaced from here on: a reserve may drop their old contents, so they count as empty until the
+    // counts arrive (an error below leaves them empty, never pointing at memory that does not hold them)
+    c->edge_items_dirty = true;
+    for (int k = 0; k < W; ++k) {
+      Slot& sl = *c->slots[k];
+      sl.n_edge = 0; sl.e_has_src = false;
+      sl.e_cps.reserve((size_t)sl.eQ); sl.e_pa.reserve((size_t)sl.eQ); sl.e_pb.reserve((size_t)sl.eQ); sl.e_src.reserve((size_t)sl.eQ);
+      dst[k].cps = sl.e_cps.p; dst[k].pa = sl.e_pa.p; dst[k].pb = sl.e_pb.p; dst[k].src = sl.e_src.p;
+    }
+    GLIO_CUDA_TRY(cudaMemcpyAsync(c->d_segs.p, segs.data(), W * sizeof(SegDesc), cudaMemcpyHostToDevice, c->st));
+    GLIO_CUDA_TRY(cudaMemcpyAsync(c->d_edst.p, dst.data(), W * sizeof(EdgeDst), cudaMemcpyHostToDevice, c->st));
+    AssocWork w = make_work(c, Qt, false, keep_debug);
+    const EdgeFitParams ep{o.max_sqdist, o.min_ratio, o.half_length};
+    edge_assoc_run(c->edge_map, c->d_segs.p, W, w, ep, c->w_pa.p, c->w_pb.p, keep_debug ? c->w_eig.p : nullptr, c->cell_count, c->cell_pos,
+                   c->scan_tmp, c->st, c->lc);
+    compact_count(w, c->d_segs.p, W, c->w_flags.p, c->w_pos.p, c->scan_tmp, c->d_counts.p, c->st, c->lc);
+    compact_edge_scatter(w, c->d_segs.p, c->w_pos.p, c->w_pa.p, c->w_pb.p, (float)o.score, c->d_edst.p, c->st, c->lc);
+    GLIO_CUDA_TRY(cudaMemcpyAsync(c->h_counts.p, c->d_counts.p, W * sizeof(int), cudaMemcpyDeviceToHost, c->st));
+    if (keep_debug) {
+      for (int k = 0; k < W; ++k) {
+        Slot& sl = *c->slots[k];
+        const int64_t off = segs[k].offset, q = sl.eQ;
+        sl.edbg_status.reserve(q); sl.edbg_idx5.reserve(5 * q); sl.edbg_sqd5.reserve(5 * q); sl.edbg_pm.reserve(q); sl.edbg_eig.reserve(3 * q);
+        GLIO_CUDA_TRY(cudaMemcpyAsync(sl.edbg_status.p, w.status + off, q, cudaMemcpyDeviceToDevice, c->st));
+        GLIO_CUDA_TRY(cudaMemcpyAsync(sl.edbg_idx5.p, w.idx5 + 5 * off, 5 * q * sizeof(int32_t), cudaMemcpyDeviceToDevice, c->st));
+        GLIO_CUDA_TRY(cudaMemcpyAsync(sl.edbg_sqd5.p, w.sqd5 + 5 * off, 5 * q * sizeof(float), cudaMemcpyDeviceToDevice, c->st));
+        GLIO_CUDA_TRY(cudaMemcpyAsync(sl.edbg_pm.p, w.pm + off, q * sizeof(float4), cudaMemcpyDeviceToDevice, c->st));
+        GLIO_CUDA_TRY(cudaMemcpyAsync(sl.edbg_eig.p, c->w_eig.p + 3 * off, 3 * q * sizeof(double), cudaMemcpyDeviceToDevice, c->st));
+        sl.edbg_Q = q;
+      }
+    }
+    GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
+    for (int k = 0; k < W; ++k) {
+      Slot& sl = *c->slots[k];
+      sl.n_edge = c->h_counts.p[k]; sl.e_has_src = true;
+      if (n_edge) n_edge[k] = sl.n_edge;
+    }
+  });
+}
+
+int glio_get_edges(glio_ctx* c, int slot, int64_t capacity, float* cp, float* pa, float* pb, double* s, int32_t* src, int64_t* n_out) {
+  if (!c) return GLIO_ERR_ARG;
+  return guarded(c, [&] {
+    Slot& sl = c->slot(slot);
+    const int64_t n = sl.n_edge;
+    if (n_out) *n_out = n;
+    if (!cp && !pa && !pb && !s && !src) return;             // a count query
+    GLIO_REQUIRE(capacity >= n, GLIO_ERR_ARG, "capacity smaller than the edge count");
+    if (n == 0) return;
+    std::vector<float4> h0(n), h1(n), h2(n);
+    GLIO_CUDA_TRY(cudaMemcpyAsync(h0.data(), sl.e_cps.p, n * sizeof(float4), cudaMemcpyDeviceToHost, c->st));
+    GLIO_CUDA_TRY(cudaMemcpyAsync(h1.data(), sl.e_pa.p, n * sizeof(float4), cudaMemcpyDeviceToHost, c->st));
+    GLIO_CUDA_TRY(cudaMemcpyAsync(h2.data(), sl.e_pb.p, n * sizeof(float4), cudaMemcpyDeviceToHost, c->st));
+    if (src && sl.e_has_src) GLIO_CUDA_TRY(cudaMemcpyAsync(src, sl.e_src.p, n * sizeof(int32_t), cudaMemcpyDeviceToHost, c->st));
+    GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
+    for (int64_t i = 0; i < n; ++i) {
+      if (cp) { cp[3 * i] = h0[i].x; cp[3 * i + 1] = h0[i].y; cp[3 * i + 2] = h0[i].z; }
+      if (pa) { pa[3 * i] = h1[i].x; pa[3 * i + 1] = h1[i].y; pa[3 * i + 2] = h1[i].z; }
+      if (pb) { pb[3 * i] = h2[i].x; pb[3 * i + 1] = h2[i].y; pb[3 * i + 2] = h2[i].z; }
+      if (s) s[i] = (double)h0[i].w;
+      if (src && !sl.e_has_src) src[i] = -1;
+    }
+  });
+}
+
+int glio_get_edge_debug(glio_ctx* c, int slot, int64_t Q, uint8_t* status, int32_t* idx5, float* sqd5, float* pm, double* eig) {
+  if (!c) return GLIO_ERR_ARG;
+  return guarded(c, [&] {
+    GLIO_REQUIRE(c->prm.keep_debug, GLIO_ERR_STATE, "context was created without keep_debug");
+    Slot& sl = c->slot(slot);
+    GLIO_REQUIRE(sl.edbg_Q == Q && Q > 0, GLIO_ERR_ARG, "Q does not match the slot's last edge association");
+    if (status) GLIO_CUDA_TRY(cudaMemcpyAsync(status, sl.edbg_status.p, Q, cudaMemcpyDeviceToHost, c->st));
+    if (idx5) GLIO_CUDA_TRY(cudaMemcpyAsync(idx5, sl.edbg_idx5.p, 5 * Q * sizeof(int32_t), cudaMemcpyDeviceToHost, c->st));
+    if (sqd5) GLIO_CUDA_TRY(cudaMemcpyAsync(sqd5, sl.edbg_sqd5.p, 5 * Q * sizeof(float), cudaMemcpyDeviceToHost, c->st));
+    if (eig) GLIO_CUDA_TRY(cudaMemcpyAsync(eig, sl.edbg_eig.p, 3 * Q * sizeof(double), cudaMemcpyDeviceToHost, c->st));
+    std::vector<float4> h;
+    if (pm) { h.resize(Q); GLIO_CUDA_TRY(cudaMemcpyAsync(h.data(), sl.edbg_pm.p, Q * sizeof(float4), cudaMemcpyDeviceToHost, c->st)); }
+    GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
+    if (pm) for (int64_t i = 0; i < Q; ++i) { pm[3 * i] = h[i].x; pm[3 * i + 1] = h[i].y; pm[3 * i + 2] = h[i].z; }
   });
 }
 
@@ -926,7 +1203,7 @@ glio_marg_prior* marg_finish_host(int W, double eps, std::vector<double>& A, std
 unsigned int marg_begin(glio_ctx* c, int W, const double* poses, const double* speed_bias, glio_host_marg_fn host_marg, void* user,
                         std::vector<double>& A, std::vector<double>& b) {
   const int N = 6 * W + 18;
-  const unsigned int epoch = eval_unary_launch(c, W, poses, 1, true);
+  const unsigned int epoch = eval_unary_launch(c, W, poses, 1, true, nullptr, true);
   A.assign((size_t)N * N, 0.0); b.assign(N, 0.0);
   if (host_marg) GLIO_REQUIRE(host_marg(user, W, poses, speed_bias, A.data(), b.data()) == 0, GLIO_ERR_STATE, "host_marg callback failed");
   return epoch;
@@ -1237,7 +1514,7 @@ static void solve_core(glio_ctx* c, int W, double* poses, double* speed_bias, gl
         if (sb) for (int i = 0; i < 9; ++i) sz[9 * k + i] = xa[(size_t)na * k + 7 + i];
       }
       // the device evaluates the LiDAR residuals while the host evaluates its own factors
-      const unsigned int epoch = eval_unary_launch(c, W, pz.data(), 0, want_jac, tgt);
+      const unsigned int epoch = eval_unary_launch(c, W, pz.data(), 0, want_jac, tgt, true);
       double ct = 0;
       if (want_jac) std::fill(g, g + n, 0.0);
       auto add_device = [&]() {
@@ -1896,7 +2173,7 @@ int glio_set_edges(glio_ctx* c, int slot, const float* cp, const float* pa, cons
   if (!c) return GLIO_ERR_ARG;
   return guarded(c, [&] {
     Slot& sl = c->slot(slot);
-    sl.n_edge = 0;
+    sl.n_edge = 0; sl.e_has_src = false; c->edge_items_dirty = true;
     if (n <= 0) return;
     GLIO_REQUIRE(cp && pa && pb && s, GLIO_ERR_ARG, "null edge arrays");
     std::vector<float4> h0(n), h1(n), h2(n);
@@ -1914,21 +2191,15 @@ int glio_set_edges(glio_ctx* c, int slot, const float* cp, const float* pa, cons
   });
 }
 
-int glio_eval_edge(glio_ctx* c, int W, const double* poses_body, double* H, double* g, double* cost) {
+}  // extern "C"
+
+static int eval_edge_impl(glio_ctx* c, int W, const double* poses_body, int jac_kind, double* H, double* g, double* cost) {
   if (!c) return GLIO_ERR_ARG;
   return guarded(c, [&] {
     GLIO_REQUIRE(W > 0 && W <= 4096 && poses_body, GLIO_ERR_ARG, "bad arguments");
-    std::vector<EdgeItem> items; std::vector<int> start(W + 1, 0);
-    for (int k = 0; k < W; ++k) {
-      start[k] = (int)items.size();
-      if ((size_t)k >= c->slots.size() || !c->slots[k]) continue;
-      Slot& sl = *c->slots[k];
-      for (int64_t o = 0; o < sl.n_edge; o += GLIO_ITEM_MAX) {
-        EdgeItem it; it.cps = sl.e_cps.p + o; it.pa = sl.e_pa.p + o; it.pb = sl.e_pb.p + o;
-        it.count = (int32_t)std::min<int64_t>(GLIO_ITEM_MAX, sl.n_edge - o); it.kf = k; items.push_back(it);
-      }
-    }
-    start[W] = (int)items.size();
+    GLIO_REQUIRE(jac_kind == 0 || jac_kind == 1, GLIO_ERR_ARG, "jac_kind must be 0 or 1");
+    std::vector<int> start;
+    const std::vector<EdgeItem> items = plan_edge_items(c, W, start);
     DevBuf<EdgeItem>& d_items = c->e_items; DevBuf<int>& d_start = c->e_start; DevBuf<double>& d_part = c->e_part; DevBuf<double>& d_out = c->e_out; DevBuf<double>& d_poses = c->e_poses;
     d_items.reserve(items.size() + 1); d_start.reserve(W + 1); d_part.reserve((items.size() + 1) * GLIO_NACC); d_out.reserve((size_t)W * GLIO_NACC); d_poses.reserve((size_t)W * 7);
     if (!c->d_ticket.p) { c->d_ticket.reserve(1); GLIO_CUDA_TRY(cudaMemsetAsync(c->d_ticket.p, 0, sizeof(unsigned int), c->st)); }
@@ -1936,7 +2207,7 @@ int glio_eval_edge(glio_ctx* c, int W, const double* poses_body, double* H, doub
     GLIO_CUDA_TRY(cudaMemcpyAsync(d_start.p, start.data(), (W + 1) * sizeof(int), cudaMemcpyHostToDevice, c->st));
     GLIO_CUDA_TRY(cudaMemcpyAsync(d_poses.p, poses_body, (size_t)W * 7 * sizeof(double), cudaMemcpyHostToDevice, c->st));
     const bool want_jac = H || g;
-    eval_edge_run(d_items.p, (int)items.size(), W, d_poses.p, eval_params(c), want_jac, d_part.p, d_out.p, d_start.p, c->d_ticket.p, c->st, c->lc);
+    eval_edge_run(d_items.p, (int)items.size(), W, d_poses.p, eval_params(c), jac_kind, want_jac, d_part.p, d_out.p, d_start.p, c->d_ticket.p, c->st, c->lc);
     std::vector<double> ho((size_t)W * GLIO_NACC);
     GLIO_CUDA_TRY(cudaMemcpyAsync(ho.data(), d_out.p, ho.size() * sizeof(double), cudaMemcpyDeviceToHost, c->st));
     GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
@@ -1946,6 +2217,24 @@ int glio_eval_edge(glio_ctx* c, int W, const double* poses_body, double* H, doub
       if (g) for (int p = 0; p < 6; ++p) g[6 * k + p] = o[21 + p];
       if (cost) cost[k] = o[27];
     }
+  });
+}
+
+extern "C" {
+
+int glio_eval_edge(glio_ctx* c, int W, const double* poses_body, double* H, double* g, double* cost) {
+  return eval_edge_impl(c, W, poses_body, 0, H, g, cost);
+}
+
+int glio_eval_edge_kind(glio_ctx* c, int W, const double* poses_body, int jac_kind, double* H, double* g, double* cost) {
+  return eval_edge_impl(c, W, poses_body, jac_kind, H, g, cost);
+}
+
+int glio_window_use_edges(glio_ctx* c, int on) {
+  if (!c) return GLIO_ERR_ARG;
+  return guarded(c, [&] {
+    wait_marg_copied(c);
+    c->use_edges = on != 0; c->edge_items_dirty = true;
   });
 }
 

@@ -234,6 +234,24 @@ void compact_run(const AssocWork& w, const SegDesc* d_segs, int nseg, int* d_fla
 void gather_selection(const int32_t* d_keep, int64_t n, int64_t n_match, const float4* cpw, const float4* nsd, const double* nc,
                       float4* o_cpw, float4* o_nsd, double* o_nc, int* d_bad, cudaStream_t st, LaunchCounter& lc);
 
+// ---- K1e (assoc.cu): scan-to-map edge association (glio_window_associate_edges)
+struct EdgeFitParams {
+  double max_sqdist, min_ratio, half_length;
+};
+// destination of one segment's compacted edge records (the slot's K2e inputs)
+struct EdgeDst {
+  float4* cps;    // (cp.xyz, s)
+  float4* pa;
+  float4* pb;
+  int32_t* src;
+};
+// search + line fit: w.status (GLIO_EDGE_*), pa / pb per query in scan order; w.idx5 / w.sqd5 / eig (3 per query) when w.idx5 is set
+void edge_assoc_run(const GridBuild& gb, const SegDesc* d_segs, int nseg, const AssocWork& w, const EdgeFitParams& ep, float4* pa, float4* pb,
+                    double* eig, DevBuf<int>& cell_count, DevBuf<int>& cell_pos, DevBuf<int>& scan_tmp, cudaStream_t st, LaunchCounter& lc);
+// after compact_count on w.status: the valid records of every segment into dst[segment]
+void compact_edge_scatter(const AssocWork& w, const SegDesc* d_segs, const int* d_pos, const float4* pa, const float4* pb, float score,
+                          const EdgeDst* d_dst, cudaStream_t st, LaunchCounter& lc);
+
 // ---- feature selection (select.cu): one segment = one slot's or one pair's seeded sample of k of its n matches
 struct SelSeg {
   const float4* cpw;    // the segment's matches (cp.xyz, weight)
@@ -275,7 +293,8 @@ struct EdgeItem {
   int32_t count;
   int32_t kf;
 };
-void eval_edge_run(const EdgeItem* d_items, int nitems, int W, const double* d_poses, const EvalParams& ep, bool want_jac,
+// jac_kind 0: tangent rotation columns; 1: ambient x,y,z quaternion columns (marginalisation)
+void eval_edge_run(const EdgeItem* d_items, int nitems, int W, const double* d_poses, const EvalParams& ep, int jac_kind, bool want_jac,
                    double* d_partials, double* d_out, const int* d_kf_item_start, unsigned int* d_ticket, cudaStream_t st, LaunchCounter& lc);
 
 // ---- K2b (eval.cu): binary plane factors

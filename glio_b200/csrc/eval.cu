@@ -299,7 +299,9 @@ void eval_unary_residuals_run(const float4* cpw, const float4* nsd, int64_t n, c
 // closed form (SURVEY 8 a-6):  e = (lp-a) x (lp-b), gv = s/|a-b| ((a-b) x e/|e|), dr/dt = gv, dr/ddelta = 2 (R p_b x gv).
 // Inputs per residual: cp, a, b (float3 each) + s -> 3 x 16 B loads (s rides in cp.w).
 // ---------------------------------------------------------------------------------------------------------------
-template <bool WANT_JAC>
+// JAC_KIND 0: Ceres' tangent rotation columns (solve path); 1: the ambient x,y,z quaternion columns of MarginalizationFactor.cpp:9-17
+// (marginalisation path), the K2 rule with gv in place of the plane's s n:  2w (p_b x gv) + 2((u.p_b) gv + (gv.u) p_b - 2 (gv.p_b) u)
+template <bool WANT_JAC, int JAC_KIND>
 __global__ void __launch_bounds__(EV_T) k_eval_edge(const EdgeItem* __restrict__ items, int nitems, int W, const double* __restrict__ poses,
                                                     EvalParams ep, double* __restrict__ partials, double* __restrict__ out,
                                                     const int* __restrict__ kf_item_start, unsigned int* __restrict__ ticket) {
@@ -316,6 +318,7 @@ __global__ void __launch_bounds__(EV_T) k_eval_edge(const EdgeItem* __restrict__
     quat_to_mat(qi, F.Rlbi);
     mat_mul3(R, F.Rlbi, F.M);
     F.t[0] = P[0]; F.t[1] = P[1]; F.t[2] = P[2];
+    if (JAC_KIND == 1) { F.q[0] = qn[0]; F.q[1] = qn[1]; F.q[2] = qn[2]; F.q[3] = qn[3]; }
   }
   __syncthreads();
   double acc[NACC];
@@ -342,6 +345,16 @@ __global__ void __launch_bounds__(EV_T) k_eval_edge(const EdgeItem* __restrict__
       const double k = s / dn * scale / en;
       const double gv[3] = {k * (de[1] * e[2] - de[2] * e[1]), k * (de[2] * e[0] - de[0] * e[2]), k * (de[0] * e[1] - de[1] * e[0])};
       double J[6] = {gv[0], gv[1], gv[2], 2.0 * (a1[1] * gv[2] - a1[2] * gv[1]), 2.0 * (a1[2] * gv[0] - a1[0] * gv[2]), 2.0 * (a1[0] * gv[1] - a1[1] * gv[0])};
+      if (JAC_KIND == 1) {
+        double pb[3]; mat_vec3(F.Rlbi, dx, dy, dz, pb);
+        const double w = F.q[0], ux = F.q[1], uy = F.q[2], uz = F.q[3];
+        const double udp = ux * pb[0] + uy * pb[1] + uz * pb[2];
+        const double gdu = gv[0] * ux + gv[1] * uy + gv[2] * uz;
+        const double gdp = gv[0] * pb[0] + gv[1] * pb[1] + gv[2] * pb[2];
+        J[3] = 2.0 * w * (pb[1] * gv[2] - pb[2] * gv[1]) + 2.0 * (udp * gv[0] + gdu * pb[0] - 2.0 * gdp * ux);
+        J[4] = 2.0 * w * (pb[2] * gv[0] - pb[0] * gv[2]) + 2.0 * (udp * gv[1] + gdu * pb[1] - 2.0 * gdp * uy);
+        J[5] = 2.0 * w * (pb[0] * gv[1] - pb[1] * gv[0]) + 2.0 * (udp * gv[2] + gdu * pb[2] - 2.0 * gdp * uz);
+      }
       r *= scale;
       int kk = 0;
 #pragma unroll
@@ -396,12 +409,13 @@ __global__ void __launch_bounds__(EV_T) k_eval_edge(const EdgeItem* __restrict__
   }
 }
 
-void eval_edge_run(const EdgeItem* d_items, int nitems, int W, const double* d_poses, const EvalParams& ep, bool want_jac,
+void eval_edge_run(const EdgeItem* d_items, int nitems, int W, const double* d_poses, const EvalParams& ep, int jac_kind, bool want_jac,
                    double* d_partials, double* d_out, const int* d_kf_item_start, unsigned int* d_ticket, cudaStream_t st, LaunchCounter& lc) {
   if (nitems <= 0) { GLIO_CUDA_TRY(cudaMemsetAsync(d_out, 0, (size_t)W * NACC * sizeof(double), st)); return; }
   lc.begin(want_jac ? "k_eval_edge" : "k_eval_edge_cost", st);
-  if (want_jac) k_eval_edge<true><<<nitems, EV_T, 0, st>>>(d_items, nitems, W, d_poses, ep, d_partials, d_out, d_kf_item_start, d_ticket);
-  else k_eval_edge<false><<<nitems, EV_T, 0, st>>>(d_items, nitems, W, d_poses, ep, d_partials, d_out, d_kf_item_start, d_ticket);
+  if (!want_jac) k_eval_edge<false, 0><<<nitems, EV_T, 0, st>>>(d_items, nitems, W, d_poses, ep, d_partials, d_out, d_kf_item_start, d_ticket);
+  else if (jac_kind == 0) k_eval_edge<true, 0><<<nitems, EV_T, 0, st>>>(d_items, nitems, W, d_poses, ep, d_partials, d_out, d_kf_item_start, d_ticket);
+  else k_eval_edge<true, 1><<<nitems, EV_T, 0, st>>>(d_items, nitems, W, d_poses, ep, d_partials, d_out, d_kf_item_start, d_ticket);
   lc.end(st);
   GLIO_CUDA_TRY(cudaGetLastError());
 }

@@ -162,6 +162,47 @@ def window_problem(W=20, Q=100_000, M=1_000_000, seed=SEED0 + 2, n_boxes=30):
                 t_lb=T_LB.copy(), W=W, Q=Q, M=M, seed=seed)
 
 
+def corner_sample(scene, n, rng, x_lo=None, x_hi=None, noise=0.02, jitter=1e-3):
+    """n corner points of the scene: uniform by length on the edges of its rectangles (the wall-ground lines, the cross walls'
+    and the boxes' edges), restricted to x in [x_lo, x_hi], + N(0, noise) per axis + U(-jitter, jitter) (kills kNN ties)."""
+    a = np.concatenate([scene.o, scene.o, scene.o + scene.u, scene.o + scene.v])
+    d = np.concatenate([scene.u, scene.v, scene.v, scene.u])
+    s0 = np.zeros(len(a)); s1 = np.ones(len(a))
+    if x_lo is not None:
+        along = d[:, 0] != 0
+        dx = np.where(along, d[:, 0], 1.0)
+        e0 = (x_lo - a[:, 0]) / dx; e1 = (x_hi - a[:, 0]) / dx
+        s0 = np.where(along, np.maximum(0.0, np.minimum(e0, e1)), 0.0)
+        s1 = np.where(along, np.minimum(1.0, np.maximum(e0, e1)), 1.0)
+        inside = (a[:, 0] >= x_lo) & (a[:, 0] <= x_hi)
+        s1 = np.where(along | inside, s1, 0.0)
+    length = np.linalg.norm(d, axis=1) * np.maximum(s1 - s0, 0.0)
+    idx = rng.choice(len(a), size=n, p=length / length.sum())
+    s = s0[idx] + rng.random(n) * (s1[idx] - s0[idx])
+    pts = a[idx] + s[:, None] * d[idx]
+    pts += rng.normal(0.0, noise, (n, 3))
+    pts += rng.uniform(-jitter, jitter, (n, 3))
+    return pts
+
+
+def window_edge_problem(W=20, Q=10_000, M=200_000, seed=SEED0 + 15, n_boxes=30, noise=0.02):
+    """The corner counterpart of window_problem: a corner map of M points and W corner scans of Q points each (lidar frame of
+    the true poses, range 50 m), e.g. for glio_window_associate_edges."""
+    rng = np.random.default_rng(seed)
+    scene = Scene(-60.0, W + 60.0, rng, n_boxes=n_boxes)
+    truth = trajectory(W, rng)
+    init = perturb(truth, rng)
+    map_xyz = corner_sample(scene, M, rng, -55.0, W + 55.0, noise=noise).astype(np.float32)
+    scans = []
+    for k in range(W):
+        t, q = truth[k, :3], truth[k, 3:]
+        pw = corner_sample(scene, Q, rng, t[0] - 50.0, t[0] + 50.0, noise=noise)
+        pb = (pw - t) @ quat_to_R(q)
+        scans.append((pb @ quat_to_R(Q_LB).T + T_LB).astype(np.float32))
+    return dict(map_xyz=map_xyz, scans=scans, poses_true=truth, poses_init=init, q_lb=Q_LB.copy(), t_lb=T_LB.copy(), W=W, Q=Q, M=M,
+                seed=seed)
+
+
 def batch_problem(K=200, Q=100_000, seed=SEED0 + 3, search_range=6, rng_range=50.0, frames=None):
     """cfg 3 / cfg 4 style batch problem: K keyframes, scans in the body frame.  Every scan has its own RNG stream
     (seed, k), so a rank of a sharded run can generate only the frames it holds (`frames`) and still agree with the

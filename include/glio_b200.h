@@ -43,6 +43,8 @@ enum { GLIO_HOST = 0, GLIO_DEVICE = 1 };
 
 /* per-query association status (mirrors the reference's three failure counters, Estimator.cpp:3641-3643) */
 enum { GLIO_MATCH_VALID = 0, GLIO_MATCH_FAIL_RADIUS = 1, GLIO_MATCH_FAIL_PLANE = 2, GLIO_MATCH_FAIL_WEIGHT = 3 };
+/* per-query edge association status (glio_window_associate_edges) */
+enum { GLIO_EDGE_VALID = 0, GLIO_EDGE_FAIL_RADIUS = 1, GLIO_EDGE_FAIL_LINE = 2 };
 
 /* All tunables of the path in one POD (SURVEY.md §5 "Config / flags"). */
 typedef struct {
@@ -646,6 +648,69 @@ int glio_marginalize(const double* A, const double* b, int n_total, int m, doubl
  * glio_eval_edge returns the same per-keyframe 6x6 / 6 / cost blocks as glio_eval_unary (add them to the plane blocks). */
 int glio_set_edges(glio_ctx* ctx, int slot, const float* cp, const float* pa, const float* pb, const double* s, int64_t n);
 int glio_eval_edge(glio_ctx* ctx, int W, const double* poses_body, double* H, double* g, double* cost);
+/* The same blocks with jac_kind 0 (Ceres tangent rotation columns: identical to glio_eval_edge) or 1 (the ambient x,y,z quaternion
+ * columns of MarginalizationFactor.cpp:9-17 with ResidualBlockInfo::Evaluate's Huber corrector: what the marginalisation uses). */
+int glio_eval_edge_kind(glio_ctx* ctx, int W, const double* poses_body, int jac_kind, double* H, double* g, double* cost);
+/* on != 0: every evaluation inside glio_window_solve, glio_window_solve_band, glio_window_marginalize and
+ * glio_window_marginalize_async (Jacobian and cost-only alike) adds the edge blocks of slots 0..W-1 (glio_set_edges or
+ * glio_window_associate_edges) to their plane blocks: tangent columns in the solve, ambient columns in the marginalisation.
+ * Default off: those calls then ignore edges entirely.  The K2e work-item plan is rebuilt only when an edge list, the window or
+ * this switch changes.  K2e is launched on the context's stream before K2, and its result is copied to pinned host memory
+ * before K2 starts, so the host reads it after K2's completion flag and never earlier; the asynchronous marginalisation adds
+ * it in the same place, so its prior stays bit-identical to the synchronous pass. */
+int glio_window_use_edges(glio_ctx* ctx, int on);
+
+/* ---- K1e: scan-to-map EDGE association on the device, producing K2e's inputs.  The reference defines LidarEdgeFactor but has
+ * no association for it, so this library defines one (the LOAM-family line form); nothing in the reference pins it.  For each
+ * corner point p of slot k, with the lidar->map pose (Q2, T2) of Estimator.cpp:2216-2217 formed from poses_body[k]:
+ *   1. p_m = float(Q2 double(p) + T2), the transform and rounding of K1;
+ *   2. the exact 5 nearest neighbours a_0..a_4 of p_m in the CORNER map (squared float distances ascending, ties by index: the
+ *      K0 grid and K1's box search);
+ *   3. status GLIO_EDGE_FAIL_RADIUS unless (double)sqd[4] < max_sqdist;
+ *   4. centroid c = (a_0 + a_1 + a_2 + a_3 + a_4) / 5.0 in double, summed nearest first;
+ *   5. scatter matrix C = sum_j (a_j - c)(a_j - c)^T in double, same order, not divided;
+ *   6. eigen-decomposition of C by cyclic Jacobi: rotations (0,1), (0,2), (1,2) per sweep; rotation theta = (c_qq - c_pp) /
+ *      (2 c_pq), t = sgn(theta) / (|theta| + sqrt(theta^2 + 1)) with sgn(0) = +1, c = 1 / sqrt(t^2 + 1), s = t c; an element with
+ *      |c_ii| + 100 |c_pq| == |c_ii| for both i = p, q is zeroed without rotating; sweeps stop when all three off-diagonal elements
+ *      are zero, at most 32 sweeps.  Eigenvalues lambda_0 <= lambda_1 <= lambda_2 (stable: ties by index); v = the eigenvector of
+ *      lambda_2 with its largest-magnitude component (lowest index on ties) positive.  Only + - * / sqrt, round-to-nearest, no FMA;
+ *   7. status GLIO_EDGE_FAIL_LINE unless lambda_2 > min_ratio * lambda_1 (five identical points fail, exactly collinear ones pass);
+ *   8. otherwise GLIO_EDGE_VALID and, in scan order, cp = p (scan frame), pa = float(c + h v), pb = float(c - h v),
+ *      s = (float)score, src = the index of p in the scan, h = half_length.
+ * Eigen's SelfAdjointEigenSolver would give eigenvalues a few ulps away, so a ratio within a few ulps of min_ratio may decide the
+ * other way there. */
+typedef struct {
+  double max_sqdist;    /* 1.0: gate on the squared 5th distance (m^2), > 0 */
+  double min_ratio;     /* 3.0: line gate lambda_2 > min_ratio lambda_1, >= 0 */
+  double half_length;   /* 0.1: pa, pb lie half_length (m) either side of the centroid, > 0 */
+  double score;         /* 1.0: s of every edge residual */
+} glio_edge_options;
+void glio_edge_default_options(glio_edge_options* o);
+/* The corner map: its own K0 grid, M >= 5 points (stride in [3,64], host or device memory as glio_set_map).  The surf map and its
+ * grid are untouched. */
+int glio_set_edge_map(glio_ctx* ctx, const float* xyz, int64_t M, int stride_floats, int mem);
+/* The corner local map: a second local map of the context (the corner counterpart of glio_localmap_*, same semantics);
+ * glio_edge_localmap_build makes it the corner map. */
+int glio_edge_localmap_clear(glio_ctx* ctx);
+int glio_edge_localmap_push(glio_ctx* ctx, int at_front, const float* cloud_xyz, int64_t n, int stride_floats, int mem,
+                            const double t[3], const double q[4]);
+int glio_edge_localmap_pop_front(glio_ctx* ctx);
+int glio_edge_localmap_build(glio_ctx* ctx, float leaf, int64_t* n_map);
+/* One keyframe's corner scan (e.g. glio_extract_features' less-sharp points) into one slot: host buffers travel on the copy
+ * stream as with glio_window_set_scan.  glio_window_slide moves the corner scans and edges with their slots and leaves the
+ * recycled last slot with neither. */
+int glio_window_set_edge_scan(glio_ctx* ctx, int slot, const float* xyz, int64_t Q, int stride_floats, int mem);
+/* Edge association of slots 0..W-1 against the corner map in one pass (launch count independent of W); each slot's edge list
+ * (what glio_set_edges would upload, src included) is replaced, n_edge[W] (may be NULL) receives the counts.  options NULL = the
+ * defaults.  One host synchronisation, for the counts.  Bad options are GLIO_ERR_ARG; no corner map, or a slot without a corner
+ * scan, is GLIO_ERR_STATE; both change nothing. */
+int glio_window_associate_edges(glio_ctx* ctx, int W, const double* poses_body, const glio_edge_options* options, int64_t* n_edge);
+/* copy-out of a slot's edge list (any pointer may be NULL): cp/pa/pb[3n] float, s[n] double, src[n] int32 (-1 for edges uploaded
+ * with glio_set_edges).  *n receives the count; all arrays NULL only counts, otherwise a capacity below the count is GLIO_ERR_ARG. */
+int glio_get_edges(glio_ctx* ctx, int slot, int64_t capacity, float* cp, float* pa, float* pb, double* s, int32_t* src, int64_t* n);
+/* per-query view of the slot's last edge association (needs params.keep_debug): status[Q] u8 (GLIO_EDGE_*), idx5[5Q] (-1: none),
+ * sqd5[5Q], pm[3Q], eig[3Q] double (lambda ascending; 0 for GLIO_EDGE_FAIL_RADIUS). */
+int glio_get_edge_debug(glio_ctx* ctx, int slot, int64_t Q, uint8_t* status, int32_t* idx5, float* sqd5, float* pm, double* eig);
 
 /* ---- batch minimizer (replaces ceres::Solve of optimizeBatchWithLandMark, Estimator.cpp:3275-3284: SUBSPACE_DOGLEG,
  * nonmonotonic steps, max_num_iter iterations; options == NULL selects exactly those).  The normal equations are
