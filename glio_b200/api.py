@@ -139,7 +139,8 @@ class Context:
                "k_compact", "k_flags", "k_cell_hist", "k_cell_scatter", "k_load_bounds", "k_scan_block", "k_scan_add",
                "k_eval_binary", "k_eval_binary_cost", "k_bin_assemble", "k_gather_sel", "k_sel_sample",
                "k_lm_transform", "k_vox_hist", "k_vox_scatter", "k_vox_sort", "k_vox_flags", "k_vox_centroid", "k_init_bounds",
-               "k_line_fit", "k_compact_edge", "k_seg_counts"]
+               "k_line_fit", "k_compact_edge", "k_seg_counts", "k_line_fit_pair", "k_eval_binary_edge", "k_eval_binary_edge_cost",
+               "k_bin_pair_add"]
 
     def lib_profile(self, on):
         self._chk(self._lib.glio_profile_enable(self._h, C.c_int(1 if on else 0)))
@@ -850,6 +851,79 @@ def _batch_set_pair_matches(self, cur, oth, cp, normal_cent, weight):
 
 
 Context.batch_set_pair_matches = _batch_set_pair_matches
+
+
+# ---------------------------------------------------------------------------------------------------
+# batch edges: scan-to-multiscan edge association (K1be) and binary point-to-edge factors (K2be)
+# ---------------------------------------------------------------------------------------------------
+def _batch_set_edge_frame(self, frame, xyz):
+    """glio_batch_set_edge_frame: the corner scan (body frame, 0 points allowed) of a frame set with batch_set_frame."""
+    if isinstance(xyz, np.ndarray) and xyz.size == 0:
+        stride = xyz.shape[1] if xyz.ndim == 2 else 3
+        keep, p, n, mem = None, None, 0, HOST
+    else:
+        keep, p, n, stride, mem = _points_arg(xyz)
+    if not hasattr(self, "_edge_frame_keep"):
+        self._edge_frame_keep = {}
+    self._edge_frame_keep[frame] = keep
+    self._chk(self._lib.glio_batch_set_edge_frame(self._h, C.c_int(frame), p, C.c_int64(n), C.c_int(stride), C.c_int(mem)))
+
+
+def _batch_associate_edges_pairs(self, cur, oth, options=None, **kw):
+    """K1be over pairs (cur[i], oth[i]); returns the edge count per pair."""
+    cur = np.ascontiguousarray(cur, np.int32); oth = np.ascontiguousarray(oth, np.int32)
+    if len(cur) != len(oth):
+        raise ValueError("cur and oth must have the same length")
+    opt = options if options is not None else edge_default_options(**kw)
+    ne = np.zeros(len(cur), np.int64)
+    self._chk(self._lib.glio_batch_associate_edges_pairs(self._h, _ptr(cur), _ptr(oth), C.c_int64(len(cur)), C.byref(opt), _ptr(ne)))
+    return ne
+
+
+def _batch_get_edges(self, cur, oth):
+    """The edge list of pair (cur, oth): cp (cur's frame), pa, pb (oth's frame) (n, 3) float32, s (n,), src (n,) int32, n."""
+    n = C.c_int64(0)
+    self._chk(self._lib.glio_batch_get_edges(self._h, C.c_int(cur), C.c_int(oth), C.c_int64(0), None, None, None, None, None, C.byref(n)))
+    m = int(n.value)
+    out = dict(cp=np.empty((m, 3), np.float32), pa=np.empty((m, 3), np.float32), pb=np.empty((m, 3), np.float32), s=np.empty(m),
+               src=np.empty(m, np.int32))
+    self._chk(self._lib.glio_batch_get_edges(self._h, C.c_int(cur), C.c_int(oth), C.c_int64(m), _ptr(out["cp"]), _ptr(out["pa"]),
+                                             _ptr(out["pb"]), _ptr(out["s"]), _ptr(out["src"]), C.byref(n)))
+    out["n"] = m
+    return out
+
+
+def _batch_set_pair_edges(self, cur, oth, cp, pa, pb, s):
+    """Upload the edge list of pair (cur, oth) instead of associating it (src reads back as -1)."""
+    cp = np.ascontiguousarray(cp, np.float32).reshape(-1, 3); pa = np.ascontiguousarray(pa, np.float32).reshape(-1, 3)
+    pb = np.ascontiguousarray(pb, np.float32).reshape(-1, 3); s = np.ascontiguousarray(s, np.float64)
+    self._chk(self._lib.glio_batch_set_pair_edges(self._h, C.c_int(cur), C.c_int(oth), _ptr(cp), _ptr(pa), _ptr(pb), _ptr(s),
+                                                  C.c_int64(len(s))))
+
+
+def _eval_binary_edge(self, poses, want_jac=True):
+    """glio_eval_binary_edge: the binary edge blocks alone, in eval_binary's layout and pair order."""
+    pb = np.ascontiguousarray(poses, np.float64).reshape(-1, 7); K = len(pb)
+    n = C.c_int64(0)
+    self._chk(self._lib.glio_batch_pair_list(self._h, C.c_int64(0), None, None, C.byref(n)))
+    P = int(n.value)
+    Hd = np.zeros((K, 6, 6)) if want_jac else None; Ho = np.zeros((P, 6, 6)) if want_jac else None
+    g = np.zeros((K, 6)) if want_jac else None; cost = np.zeros(1)
+    self._chk(self._lib.glio_eval_binary_edge(self._h, C.c_int(K), _ptr(pb), _ptr(Hd), _ptr(Ho), _ptr(g), _ptr(cost)))
+    return dict(Hdiag=Hd, Hoff=Ho, g=g, cost=float(cost[0]))
+
+
+def _batch_use_edges(self, on):
+    """glio_batch_use_edges: batch solves add the pairs' edge blocks (default off)."""
+    self._chk(self._lib.glio_batch_use_edges(self._h, C.c_int(1 if on else 0)))
+
+
+Context.batch_set_edge_frame = _batch_set_edge_frame
+Context.batch_associate_edges_pairs = _batch_associate_edges_pairs
+Context.batch_get_edges = _batch_get_edges
+Context.batch_set_pair_edges = _batch_set_pair_edges
+Context.eval_binary_edge = _eval_binary_edge
+Context.batch_use_edges = _batch_use_edges
 
 
 # ---------------------------------------------------------------------------------------------------

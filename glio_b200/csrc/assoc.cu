@@ -364,6 +364,25 @@ __device__ __forceinline__ void jacobi_eig3(double (&a)[3][3], double lam[3], do
   if (big < 0.0) { dir[0] = -dir[0]; dir[1] = -dir[1]; dir[2] = -dir[2]; }
 }
 
+// steps 4-5 of the line fit: centroid c (summed nearest first, / 5.0) and the undivided scatter matrix A (both triangles) of the
+// five points x[coordinate][neighbour].  The same operations in the same order as k_line_fit's inline copy, which is kept as it
+// is so that its generated code does not change.
+__device__ __forceinline__ void centroid_scatter5(const double (&x)[3][5], double c[3], double (&A)[3][3]) {
+#pragma unroll
+  for (int i = 0; i < 3; ++i) c[i] = ddiv_rn(dadd(dadd(dadd(dadd(x[i][0], x[i][1]), x[i][2]), x[i][3]), x[i][4]), 5.0);
+#pragma unroll
+  for (int i = 0; i < 3; ++i)
+#pragma unroll
+    for (int k = 0; k < 3; ++k) A[i][k] = 0.0;
+#pragma unroll
+  for (int j = 0; j < 5; ++j) {
+    const double dx = dsub(x[0][j], c[0]), dy = dsub(x[1][j], c[1]), dz = dsub(x[2][j], c[2]);
+    A[0][0] = dadd(A[0][0], dmul(dx, dx)); A[0][1] = dadd(A[0][1], dmul(dx, dy)); A[0][2] = dadd(A[0][2], dmul(dx, dz));
+    A[1][1] = dadd(A[1][1], dmul(dy, dy)); A[1][2] = dadd(A[1][2], dmul(dy, dz)); A[2][2] = dadd(A[2][2], dmul(dz, dz));
+  }
+  A[1][0] = A[0][1]; A[2][0] = A[0][2]; A[2][1] = A[1][2];
+}
+
 struct LineFitArgs {
   int64_t Qt;
   const float4* pmq;          // queries in cell-sorted order, .w = scan index
@@ -432,8 +451,50 @@ __global__ void __launch_bounds__(128) k_line_fit(LineFitArgs a) {
   }
 }
 
+// K1be, pair mode (glio_batch_associate_edges_pairs): the same gates on the world cloud of the searched frame; a valid query's line
+// is then refitted (steps 4-6 again) on the same five indices in the searched frame's local coordinates as stored, as the pair plane
+// fit refits its plane (Estimator.cpp:3752-3772), and pa / pb are that local line.  Debug views are not written.
+__global__ void __launch_bounds__(128) k_line_fit_pair(LineFitArgs a, const float* __restrict__ oth_local, int oth_stride) {
+  const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= a.Qt) return;
+  const int64_t g = __float_as_int(a.pmq[p].w);
+  int id[5];
+#pragma unroll
+  for (int j = 0; j < 5; ++j) id[j] = a.knn_idx[(int64_t)j * a.Qt + p];
+  const float d4 = a.knn_sqd[4 * a.Qt + p];
+  uint8_t st = GLIO_EDGE_FAIL_RADIUS;
+  float4 oa = make_float4(0.f, 0.f, 0.f, 0.f), ob = oa;
+  if (id[4] != 0x7fffffff && (double)d4 < a.max_sqdist) {
+    double x[3][5];
+#pragma unroll
+    for (int j = 0; j < 5; ++j) {
+      const float4 m = __ldg(&a.pts_sorted[__ldg(&a.sorted_pos[id[j]])]);
+      x[0][j] = (double)m.x; x[1][j] = (double)m.y; x[2][j] = (double)m.z;
+    }
+    double c[3], A[3][3], lam[3], v[3];
+    centroid_scatter5(x, c, A);
+    jacobi_eig3(A, lam, v);
+    if (lam[2] > dmul(a.min_ratio, lam[1])) {
+      st = GLIO_EDGE_VALID;
+#pragma unroll
+      for (int j = 0; j < 5; ++j) {
+        const float* lp = oth_local + (int64_t)id[j] * oth_stride;
+        x[0][j] = (double)lp[0]; x[1][j] = (double)lp[1]; x[2][j] = (double)lp[2];
+      }
+      centroid_scatter5(x, c, A);
+      jacobi_eig3(A, lam, v);
+      const double h = a.half_length;
+      oa = make_float4((float)dadd(c[0], dmul(h, v[0])), (float)dadd(c[1], dmul(h, v[1])), (float)dadd(c[2], dmul(h, v[2])), 0.f);
+      ob = make_float4((float)dsub(c[0], dmul(h, v[0])), (float)dsub(c[1], dmul(h, v[1])), (float)dsub(c[2], dmul(h, v[2])), 0.f);
+    } else st = GLIO_EDGE_FAIL_LINE;
+  }
+  a.status[g] = st;
+  a.pa[g] = oa; a.pb[g] = ob;
+}
+
 void edge_assoc_run(const GridBuild& gb, const SegDesc* d_segs, int nseg, const AssocWork& w, const EdgeFitParams& ep, float4* pa, float4* pb,
-                    double* eig, DevBuf<int>& cell_count, DevBuf<int>& cell_pos, DevBuf<int>& scan_tmp, cudaStream_t st, LaunchCounter& lc) {
+                    double* eig, const float* oth_local, int oth_stride, DevBuf<int>& cell_count, DevBuf<int>& cell_pos,
+                    DevBuf<int>& scan_tmp, cudaStream_t st, LaunchCounter& lc) {
   const int64_t Qt = w.Qt;
   if (Qt <= 0) return;
   assoc_search(gb, d_segs, nseg, w, (float)ep.max_sqdist, cell_count, cell_pos, scan_tmp, st, lc);
@@ -442,7 +503,9 @@ void edge_assoc_run(const GridBuild& gb, const SegDesc* d_segs, int nseg, const 
   la.pts_sorted = gb.pts.p; la.sorted_pos = gb.sorted_pos.p;
   la.max_sqdist = ep.max_sqdist; la.min_ratio = ep.min_ratio; la.half_length = ep.half_length;
   la.status = w.status; la.pa = pa; la.pb = pb; la.idx5 = w.idx5; la.sqd5 = w.sqd5; la.eig = eig;
-  lc.begin("k_line_fit", st); k_line_fit<<<(unsigned)((Qt + 127) / 128), 128, 0, st>>>(la); lc.end(st);
+  const unsigned nk = (unsigned)((Qt + 127) / 128);
+  if (oth_local) { lc.begin("k_line_fit_pair", st); k_line_fit_pair<<<nk, 128, 0, st>>>(la, oth_local, oth_stride); lc.end(st); }
+  else { lc.begin("k_line_fit", st); k_line_fit<<<nk, 128, 0, st>>>(la); lc.end(st); }
   GLIO_CUDA_TRY(cudaGetLastError());
 }
 

@@ -115,12 +115,23 @@ struct glio_ctx {
     DevBuf<float> scan; const float* scan_ptr = nullptr;
     double pose[7] = {0, 0, 0, 1, 0, 0, 0};
     GridBuild grid; bool grid_valid = false;
+    // corner scan (glio_batch_set_edge_frame): same layout and ownership rules as scan / scan_ptr, 0 points allowed; its world
+    // cloud's grid is built when a pair first searches it and dropped with the pose
+    bool has_edge = false; int64_t eQ = 0; int estride = 3;
+    DevBuf<float> escan; const float* escan_ptr = nullptr;
+    GridBuild egrid; bool egrid_valid = false;
+    void release() { scan.release(); grid.release(); escan.release(); egrid.release(); }
   };
   struct Pair {
     int cur = 0, oth = 0;
     DevBuf<float4> m_cpw; DevBuf<double> m_nc; DevBuf<int32_t> m_src; int64_t n_match = 0;
     DevBuf<float4> s_cpw; DevBuf<double> s_nc; DevBuf<int32_t> s_keep; int64_t n_sel = -1;
-    void release() { m_cpw.release(); m_nc.release(); m_src.release(); s_cpw.release(); s_nc.release(); s_keep.release(); }
+    // edge list (glio_batch_associate_edges_pairs or glio_batch_set_pair_edges): cp in cur's frame with s in .w, pa / pb in oth's
+    DevBuf<float4> e_cps, e_pa, e_pb; DevBuf<int32_t> e_src; int64_t n_edge = 0; bool e_has_src = false;
+    void release() {
+      m_cpw.release(); m_nc.release(); m_src.release(); s_cpw.release(); s_nc.release(); s_keep.release();
+      e_cps.release(); e_pa.release(); e_pb.release(); e_src.release();
+    }
   };
   std::map<int, std::unique_ptr<Frame>> frames;
   std::vector<std::unique_ptr<Pair>> pairs;
@@ -130,6 +141,10 @@ struct glio_ctx {
   DevBuf<BinItem> d_bin_items; DevBuf<int> d_pair_item_start, d_kf_inc_start; DevBuf<BinIncidence> d_inc;
   DevBuf<double> d_bin_partials, d_pair_sums, d_bin_diag, d_bin_off, d_bin_poses;
   PinnedBuf<double> h_bin_diag, h_bin_off, h_bin_poses;
+  // binary edge blocks (glio_batch_use_edges, glio_eval_binary_edge): the K2be work-item plan, rebuilt only when an edge list, K,
+  // the pair count or the switch changes; its per-pair sums are added to the plane sums before the one block assembly
+  bool batch_use_edges = false, bedge_dirty = true; int bedge_K = -1, bedge_P = -1, n_bedge_items = 0;
+  DevBuf<BinEdgeItem> d_bedge_items; DevBuf<int> d_bedge_pstart; DevBuf<double> d_bedge_partials, d_bedge_sums;
 
   // association workspace
   DevBuf<float4> w_pm, w_pmq, w_nsd;
@@ -592,8 +607,9 @@ void glio_destroy(glio_ctx* c) {
   c->edge_map.release(); c->edge_map_stage.release(); c->elm.release(); c->elm_stage.release();
   c->w_pa.release(); c->w_pb.release(); c->w_eig.release(); c->d_edst.release();
   c->se_items.release(); c->se_start.release(); c->se_part.release(); c->se_out.release(); c->se_poses.release(); c->h_eout.release();
-  for (auto& f : c->frames) { f.second->scan.release(); f.second->grid.release(); }
+  for (auto& f : c->frames) f.second->release();
   for (auto& p : c->pairs) p->release();
+  c->d_bedge_items.release(); c->d_bedge_pstart.release(); c->d_bedge_partials.release(); c->d_bedge_sums.release();
   c->d_bin_items.release(); c->d_pair_item_start.release(); c->d_kf_inc_start.release(); c->d_inc.release(); c->d_bin_partials.release();
   c->d_pair_sums.release(); c->d_bin_diag.release(); c->d_bin_off.release(); c->d_bin_poses.release(); c->h_bin_diag.release(); c->h_bin_off.release(); c->h_bin_poses.release();
   for (auto& s : c->slots) if (s) s->release();
@@ -932,6 +948,23 @@ void glio_edge_default_options(glio_edge_options* o) {
   o->max_sqdist = 1.0; o->min_ratio = 3.0; o->half_length = 0.1; o->score = 1.0;
 }
 
+}  // extern "C"
+
+namespace {
+
+// the options of an edge association call (NULL: the defaults), validated
+glio_edge_options edge_options_or_default(const glio_edge_options* options) {
+  glio_edge_options o; if (options) o = *options; else glio_edge_default_options(&o);
+  GLIO_REQUIRE(std::isfinite(o.max_sqdist) && o.max_sqdist > 0.0 && std::isfinite(o.min_ratio) && o.min_ratio >= 0.0 &&
+               std::isfinite(o.half_length) && o.half_length > 0.0 && std::isfinite(o.score), GLIO_ERR_ARG,
+               "glio_edge_options: need max_sqdist > 0, min_ratio >= 0, half_length > 0 and a finite score");
+  return o;
+}
+
+}  // namespace
+
+extern "C" {
+
 int glio_set_edge_map(glio_ctx* c, const float* xyz, int64_t M, int stride, int mem) {
   if (!c) return GLIO_ERR_ARG;
   return guarded(c, [&] {
@@ -974,10 +1007,7 @@ int glio_window_associate_edges(glio_ctx* c, int W, const double* poses_body, co
   if (!c) return GLIO_ERR_ARG;
   return guarded(c, [&] {
     GLIO_REQUIRE(W > 0 && W <= 4096 && poses_body, GLIO_ERR_ARG, "bad window arguments");
-    glio_edge_options o; if (options) o = *options; else glio_edge_default_options(&o);
-    GLIO_REQUIRE(std::isfinite(o.max_sqdist) && o.max_sqdist > 0.0 && std::isfinite(o.min_ratio) && o.min_ratio >= 0.0 &&
-                 std::isfinite(o.half_length) && o.half_length > 0.0 && std::isfinite(o.score), GLIO_ERR_ARG,
-                 "glio_edge_options: need max_sqdist > 0, min_ratio >= 0, half_length > 0 and a finite score");
+    const glio_edge_options o = edge_options_or_default(options);
     GLIO_REQUIRE(c->has_edge_map, GLIO_ERR_STATE, "glio_set_edge_map must be called before edge association");
     for (int k = 0; k < W; ++k)
       GLIO_REQUIRE((size_t)k < c->slots.size() && c->slots[k] && c->slots[k]->eQ > 0 && c->slots[k]->escan_ptr, GLIO_ERR_STATE, "slot has no corner scan");
@@ -1010,8 +1040,8 @@ int glio_window_associate_edges(glio_ctx* c, int W, const double* poses_body, co
     GLIO_CUDA_TRY(cudaMemcpyAsync(c->d_edst.p, dst.data(), W * sizeof(EdgeDst), cudaMemcpyHostToDevice, c->st));
     AssocWork w = make_work(c, Qt, false, keep_debug);
     const EdgeFitParams ep{o.max_sqdist, o.min_ratio, o.half_length};
-    edge_assoc_run(c->edge_map, c->d_segs.p, W, w, ep, c->w_pa.p, c->w_pb.p, keep_debug ? c->w_eig.p : nullptr, c->cell_count, c->cell_pos,
-                   c->scan_tmp, c->st, c->lc);
+    edge_assoc_run(c->edge_map, c->d_segs.p, W, w, ep, c->w_pa.p, c->w_pb.p, keep_debug ? c->w_eig.p : nullptr, nullptr, 0, c->cell_count,
+                   c->cell_pos, c->scan_tmp, c->st, c->lc);
     compact_count(w, c->d_segs.p, W, c->w_flags.p, c->w_pos.p, c->scan_tmp, c->d_counts.p, c->st, c->lc);
     compact_edge_scatter(w, c->d_segs.p, c->w_pos.p, c->w_pa.p, c->w_pb.p, (float)o.score, c->d_edst.p, c->st, c->lc);
     GLIO_CUDA_TRY(cudaMemcpyAsync(c->h_counts.p, c->d_counts.p, W * sizeof(int), cudaMemcpyDeviceToHost, c->st));
@@ -1037,28 +1067,58 @@ int glio_window_associate_edges(glio_ctx* c, int W, const double* poses_body, co
   });
 }
 
+}  // extern "C"
+
+namespace {
+
+// copy-out of an edge list (glio_get_edges / glio_batch_get_edges): all arrays NULL only counts
+void copy_edges_out(glio_ctx* c, int64_t n, const float4* d_cps, const float4* d_pa, const float4* d_pb, const int32_t* d_src, bool has_src,
+                    int64_t capacity, float* cp, float* pa, float* pb, double* s, int32_t* src, int64_t* n_out) {
+  if (n_out) *n_out = n;
+  if (!cp && !pa && !pb && !s && !src) return;             // a count query
+  GLIO_REQUIRE(capacity >= n, GLIO_ERR_ARG, "capacity smaller than the edge count");
+  if (n == 0) return;
+  std::vector<float4> h0(n), h1(n), h2(n);
+  GLIO_CUDA_TRY(cudaMemcpyAsync(h0.data(), d_cps, n * sizeof(float4), cudaMemcpyDeviceToHost, c->st));
+  GLIO_CUDA_TRY(cudaMemcpyAsync(h1.data(), d_pa, n * sizeof(float4), cudaMemcpyDeviceToHost, c->st));
+  GLIO_CUDA_TRY(cudaMemcpyAsync(h2.data(), d_pb, n * sizeof(float4), cudaMemcpyDeviceToHost, c->st));
+  if (src && has_src) GLIO_CUDA_TRY(cudaMemcpyAsync(src, d_src, n * sizeof(int32_t), cudaMemcpyDeviceToHost, c->st));
+  GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
+  for (int64_t i = 0; i < n; ++i) {
+    if (cp) { cp[3 * i] = h0[i].x; cp[3 * i + 1] = h0[i].y; cp[3 * i + 2] = h0[i].z; }
+    if (pa) { pa[3 * i] = h1[i].x; pa[3 * i + 1] = h1[i].y; pa[3 * i + 2] = h1[i].z; }
+    if (pb) { pb[3 * i] = h2[i].x; pb[3 * i + 1] = h2[i].y; pb[3 * i + 2] = h2[i].z; }
+    if (s) s[i] = (double)h0[i].w;
+    if (src && !has_src) src[i] = -1;
+  }
+}
+
+// upload of an edge list (glio_set_edges / glio_batch_set_pair_edges): (cp, s) / pa / pb as float4, n > 0
+void upload_edges(glio_ctx* c, int64_t n, const float* cp, const float* pa, const float* pb, const double* s, DevBuf<float4>& d_cps,
+                  DevBuf<float4>& d_pa, DevBuf<float4>& d_pb) {
+  GLIO_REQUIRE(cp && pa && pb && s, GLIO_ERR_ARG, "null edge arrays");
+  std::vector<float4> h0(n), h1(n), h2(n);
+  for (int64_t i = 0; i < n; ++i) {
+    h0[i] = make_float4(cp[3 * i], cp[3 * i + 1], cp[3 * i + 2], (float)s[i]);
+    h1[i] = make_float4(pa[3 * i], pa[3 * i + 1], pa[3 * i + 2], 0.f);
+    h2[i] = make_float4(pb[3 * i], pb[3 * i + 1], pb[3 * i + 2], 0.f);
+  }
+  d_cps.reserve(n); d_pa.reserve(n); d_pb.reserve(n);
+  GLIO_CUDA_TRY(cudaMemcpyAsync(d_cps.p, h0.data(), n * sizeof(float4), cudaMemcpyHostToDevice, c->st));
+  GLIO_CUDA_TRY(cudaMemcpyAsync(d_pa.p, h1.data(), n * sizeof(float4), cudaMemcpyHostToDevice, c->st));
+  GLIO_CUDA_TRY(cudaMemcpyAsync(d_pb.p, h2.data(), n * sizeof(float4), cudaMemcpyHostToDevice, c->st));
+  GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
+}
+
+}  // namespace
+
+extern "C" {
+
 int glio_get_edges(glio_ctx* c, int slot, int64_t capacity, float* cp, float* pa, float* pb, double* s, int32_t* src, int64_t* n_out) {
   if (!c) return GLIO_ERR_ARG;
   return guarded(c, [&] {
     Slot& sl = c->slot(slot);
-    const int64_t n = sl.n_edge;
-    if (n_out) *n_out = n;
-    if (!cp && !pa && !pb && !s && !src) return;             // a count query
-    GLIO_REQUIRE(capacity >= n, GLIO_ERR_ARG, "capacity smaller than the edge count");
-    if (n == 0) return;
-    std::vector<float4> h0(n), h1(n), h2(n);
-    GLIO_CUDA_TRY(cudaMemcpyAsync(h0.data(), sl.e_cps.p, n * sizeof(float4), cudaMemcpyDeviceToHost, c->st));
-    GLIO_CUDA_TRY(cudaMemcpyAsync(h1.data(), sl.e_pa.p, n * sizeof(float4), cudaMemcpyDeviceToHost, c->st));
-    GLIO_CUDA_TRY(cudaMemcpyAsync(h2.data(), sl.e_pb.p, n * sizeof(float4), cudaMemcpyDeviceToHost, c->st));
-    if (src && sl.e_has_src) GLIO_CUDA_TRY(cudaMemcpyAsync(src, sl.e_src.p, n * sizeof(int32_t), cudaMemcpyDeviceToHost, c->st));
-    GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
-    for (int64_t i = 0; i < n; ++i) {
-      if (cp) { cp[3 * i] = h0[i].x; cp[3 * i + 1] = h0[i].y; cp[3 * i + 2] = h0[i].z; }
-      if (pa) { pa[3 * i] = h1[i].x; pa[3 * i + 1] = h1[i].y; pa[3 * i + 2] = h1[i].z; }
-      if (pb) { pb[3 * i] = h2[i].x; pb[3 * i + 1] = h2[i].y; pb[3 * i + 2] = h2[i].z; }
-      if (s) s[i] = (double)h0[i].w;
-      if (src && !sl.e_has_src) src[i] = -1;
-    }
+    copy_edges_out(c, sl.n_edge, sl.e_cps.p, sl.e_pa.p, sl.e_pb.p, sl.e_src.p, sl.e_has_src, capacity, cp, pa, pb, s, src, n_out);
   });
 }
 
@@ -1626,9 +1686,9 @@ int glio_batch_clear(glio_ctx* c) {
   if (!c) return GLIO_ERR_ARG;
   return guarded(c, [&] {
     GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
-    for (auto& f : c->frames) { f.second->scan.release(); f.second->grid.release(); }
+    for (auto& f : c->frames) f.second->release();
     for (auto& p : c->pairs) p->release();
-    c->frames.clear(); c->pairs.clear(); c->pair_index.clear(); c->bin_dirty = true;
+    c->frames.clear(); c->pairs.clear(); c->pair_index.clear(); c->bin_dirty = true; c->bedge_dirty = true;
   });
 }
 
@@ -1640,7 +1700,7 @@ int glio_batch_set_frame(glio_ctx* c, int frame, const float* scan_xyz, int64_t 
     if (!fp) fp.reset(new glio_ctx::Frame());
     glio_ctx::Frame& f = *fp;
     f.scan_ptr = stage_points(c, f.scan, scan_xyz, Q, stride, mem);
-    f.Q = Q; f.stride = stride; f.grid_valid = false;
+    f.Q = Q; f.stride = stride; f.grid_valid = false; f.egrid_valid = false;
     for (int i = 0; i < 7; ++i) f.pose[i] = pose[i];
   });
 }
@@ -1652,7 +1712,7 @@ int glio_batch_set_pose(glio_ctx* c, int frame, const double pose[7]) {
     auto it = c->frames.find(frame);
     GLIO_REQUIRE(it != c->frames.end() && pose, GLIO_ERR_ARG, "unknown frame");
     for (int i = 0; i < 7; ++i) it->second->pose[i] = pose[i];
-    it->second->grid_valid = false;
+    it->second->grid_valid = false; it->second->egrid_valid = false;
   });
 }
 
@@ -1772,6 +1832,137 @@ int glio_batch_select(glio_ctx* c, int cur, int oth, const int32_t* keep, int64_
     GLIO_CUDA_TRY(cudaMemcpyAsync(&bad, c->d_bad.p, sizeof(int), cudaMemcpyDeviceToHost, c->st));
     GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
     if (bad) { pr.n_sel = -1; throw Error{GLIO_ERR_ARG, "selection index out of range"}; }
+  });
+}
+
+}  // extern "C"
+
+namespace {
+
+// the pair (cur, oth) of the pair list, appended with no matches and no edges when it is not there yet
+glio_ctx::Pair& pair_entry(glio_ctx* c, int cur, int oth) {
+  const std::pair<int, int> key(cur, oth);
+  auto it = c->pair_index.find(key);
+  if (it != c->pair_index.end()) return *c->pairs[it->second];
+  c->pair_index[key] = (int)c->pairs.size();
+  c->pairs.emplace_back(new glio_ctx::Pair());
+  c->pairs.back()->cur = cur; c->pairs.back()->oth = oth;
+  c->bin_dirty = true;
+  return *c->pairs.back();
+}
+
+}  // namespace
+
+extern "C" {
+
+// ---- K1be / K2be: scan-to-multiscan edge association and binary point-to-edge factors
+int glio_batch_set_edge_frame(glio_ctx* c, int frame, const float* xyz, int64_t Q, int stride, int mem) {
+  if (!c) return GLIO_ERR_ARG;
+  return guarded(c, [&] {
+    auto it = c->frames.find(frame);
+    GLIO_REQUIRE(it != c->frames.end(), GLIO_ERR_STATE, "glio_batch_set_edge_frame: frame was not set with glio_batch_set_frame");
+    GLIO_REQUIRE(Q >= 0 && stride >= 3 && stride <= 64, GLIO_ERR_ARG, "glio_batch_set_edge_frame: need Q >= 0 and stride_floats in [3,64]");
+    glio_ctx::Frame& f = *it->second;
+    const float* p = Q > 0 ? stage_points(c, f.escan, xyz, Q, stride, mem) : nullptr;
+    f.escan_ptr = p; f.eQ = Q; f.estride = stride; f.has_edge = true; f.egrid_valid = false;
+  });
+}
+
+// K1be over the listed pairs, one group per searched frame: its corner grid (built once, reused by every pair that searches it),
+// one search + line-fit launch for all the group's queries, compaction straight into the pairs' edge lists, one host
+// synchronisation for the counts.
+int glio_batch_associate_edges_pairs(glio_ctx* c, const int32_t* pairs_cur, const int32_t* pairs_oth, int64_t n_pairs,
+                                     const glio_edge_options* options, int64_t* n_edge) {
+  if (!c) return GLIO_ERR_ARG;
+  return guarded(c, [&] {
+    GLIO_REQUIRE(n_pairs > 0 && pairs_cur && pairs_oth, GLIO_ERR_ARG, "bad pair list");
+    const glio_edge_options o = edge_options_or_default(options);
+    std::map<int, std::vector<int64_t>> by_oth;
+    for (int64_t i = 0; i < n_pairs; ++i) {
+      GLIO_REQUIRE(c->frames.count(pairs_cur[i]) && c->frames.count(pairs_oth[i]) && pairs_cur[i] != pairs_oth[i], GLIO_ERR_ARG,
+                   "pair references an unknown frame");
+      by_oth[pairs_oth[i]].push_back(i);
+    }
+    for (int64_t i = 0; i < n_pairs; ++i)
+      GLIO_REQUIRE(c->frames[pairs_cur[i]]->has_edge && c->frames[pairs_oth[i]]->has_edge, GLIO_ERR_STATE,
+                   "pair frame has no corner scan (glio_batch_set_edge_frame)");
+    const EdgeFitParams ep{o.max_sqdist, o.min_ratio, o.half_length};
+    c->bedge_dirty = true;
+    for (auto& grp : by_oth) {
+      glio_ctx::Frame& fo = *c->frames[grp.first];
+      // the group's pairs; their edge lists count as empty until the counts arrive (a reserve may drop the old contents)
+      std::vector<glio_ctx::Pair*> prs;
+      for (int64_t i : grp.second) {
+        glio_ctx::Pair& pr = pair_entry(c, pairs_cur[i], pairs_oth[i]);
+        pr.n_edge = 0; pr.e_has_src = false;
+        prs.push_back(&pr);
+        if (n_edge) n_edge[i] = 0;
+      }
+      if (fo.eQ == 0) continue;                 // nothing to search: every query fails the radius gate
+      std::vector<SegDesc> segs;
+      std::vector<EdgeDst> dst;
+      std::vector<int64_t> seg_item;
+      int64_t Qt = 0;
+      for (size_t s = 0; s < grp.second.size(); ++s) {
+        const glio_ctx::Frame& fc = *c->frames[pairs_cur[grp.second[s]]];
+        if (fc.eQ == 0) continue;
+        SegDesc sd;
+        sd.src = fc.escan_ptr; sd.stride = fc.estride; sd.count = fc.eQ; sd.offset = Qt;
+        for (int k = 0; k < 3; ++k) sd.t[k] = fc.pose[k];          // body pose applied directly to the stored points (quirk Q7)
+        for (int k = 0; k < 4; ++k) sd.q[k] = fc.pose[3 + k];
+        glio_ctx::Pair& pr = *prs[s];
+        pr.e_cps.reserve((size_t)fc.eQ); pr.e_pa.reserve((size_t)fc.eQ); pr.e_pb.reserve((size_t)fc.eQ); pr.e_src.reserve((size_t)fc.eQ);
+        dst.push_back(EdgeDst{pr.e_cps.p, pr.e_pa.p, pr.e_pb.p, pr.e_src.p});
+        segs.push_back(sd); seg_item.push_back((int64_t)s);
+        Qt += fc.eQ;
+      }
+      if (segs.empty()) continue;
+      GLIO_REQUIRE(Qt < ((int64_t)1 << 31), GLIO_ERR_ARG, "glio_batch_associate_edges_pairs: too many corner points searching one frame");
+      if (!fo.egrid_valid) {
+        grid_build(fo.egrid, fo.escan_ptr, fo.estride, fo.eQ, fo.pose, fo.pose + 3, c->prm.cell_size, c->pts_per_cell, c->st, c->lc);
+        fo.egrid_valid = true;
+      }
+      const int nseg = (int)segs.size();
+      ensure_work(c, Qt, false, false);
+      c->w_pa.reserve((size_t)Qt); c->w_pb.reserve((size_t)Qt);
+      c->d_segs.reserve(nseg); c->d_edst.reserve(nseg); c->d_counts.reserve(nseg); c->h_counts.reserve(nseg);
+      GLIO_CUDA_TRY(cudaMemcpyAsync(c->d_segs.p, segs.data(), nseg * sizeof(SegDesc), cudaMemcpyHostToDevice, c->st));
+      GLIO_CUDA_TRY(cudaMemcpyAsync(c->d_edst.p, dst.data(), nseg * sizeof(EdgeDst), cudaMemcpyHostToDevice, c->st));
+      AssocWork w = make_work(c, Qt, false, false);
+      edge_assoc_run(fo.egrid, c->d_segs.p, nseg, w, ep, c->w_pa.p, c->w_pb.p, nullptr, fo.escan_ptr, fo.estride, c->cell_count, c->cell_pos,
+                     c->scan_tmp, c->st, c->lc);
+      compact_count(w, c->d_segs.p, nseg, c->w_flags.p, c->w_pos.p, c->scan_tmp, c->d_counts.p, c->st, c->lc);
+      compact_edge_scatter(w, c->d_segs.p, c->w_pos.p, c->w_pa.p, c->w_pb.p, (float)o.score, c->d_edst.p, c->st, c->lc);
+      GLIO_CUDA_TRY(cudaMemcpyAsync(c->h_counts.p, c->d_counts.p, nseg * sizeof(int), cudaMemcpyDeviceToHost, c->st));
+      GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
+      for (int s = 0; s < nseg; ++s) {
+        glio_ctx::Pair& pr = *prs[seg_item[s]];
+        pr.n_edge = c->h_counts.p[s]; pr.e_has_src = true;
+        if (n_edge) n_edge[grp.second[seg_item[s]]] = pr.n_edge;
+      }
+    }
+  });
+}
+
+int glio_batch_get_edges(glio_ctx* c, int cur, int oth, int64_t capacity, float* cp, float* pa, float* pb, double* s, int32_t* src, int64_t* n) {
+  if (!c) return GLIO_ERR_ARG;
+  return guarded(c, [&] {
+    auto it = c->pair_index.find(std::make_pair(cur, oth));
+    GLIO_REQUIRE(it != c->pair_index.end(), GLIO_ERR_ARG, "pair is not on the pair list");
+    glio_ctx::Pair& pr = *c->pairs[it->second];
+    copy_edges_out(c, pr.n_edge, pr.e_cps.p, pr.e_pa.p, pr.e_pb.p, pr.e_src.p, pr.e_has_src, capacity, cp, pa, pb, s, src, n);
+  });
+}
+
+int glio_batch_set_pair_edges(glio_ctx* c, int cur, int oth, const float* cp, const float* pa, const float* pb, const double* s, int64_t n) {
+  if (!c) return GLIO_ERR_ARG;
+  return guarded(c, [&] {
+    GLIO_REQUIRE(cur >= 0 && oth >= 0 && cur != oth, GLIO_ERR_ARG, "bad pair");
+    GLIO_REQUIRE(n >= 0 && (n == 0 || (cp && pa && pb && s)), GLIO_ERR_ARG, "null edge arrays");
+    glio_ctx::Pair& pr = pair_entry(c, cur, oth);
+    pr.n_edge = 0; pr.e_has_src = false; c->bedge_dirty = true;
+    if (n > 0) upload_edges(c, n, cp, pa, pb, s, pr.e_cps, pr.e_pa, pr.e_pb);
+    pr.n_edge = n;
   });
 }
 
@@ -1980,15 +2171,55 @@ void build_bin_items(glio_ctx* c, int K) {
   c->bin_dirty = false; c->bin_K = K;
 }
 
+// work items of the binary edge evaluation: each pair's edge list in runs of GLIO_ITEM_MAX, pairs in pair-list order (rebuilt when
+// an edge list, K or the pair count changes, or the switch is turned; build_bin_items runs first and checks the pairs against K)
+void build_bedge_items(glio_ctx* c, int K) {
+  const int P = (int)c->pairs.size();
+  if (!c->bedge_dirty && c->bedge_K == K && c->bedge_P == P) return;
+  std::vector<BinEdgeItem> items;
+  std::vector<int> pstart(P + 1, 0);
+  for (int p = 0; p < P; ++p) {
+    glio_ctx::Pair& pr = *c->pairs[p];
+    pstart[p] = (int)items.size();
+    for (int64_t o = 0; o < pr.n_edge; o += GLIO_ITEM_MAX) {
+      BinEdgeItem it; it.cps = pr.e_cps.p + o; it.pa = pr.e_pa.p + o; it.pb = pr.e_pb.p + o;
+      it.count = (int32_t)std::min<int64_t>(GLIO_ITEM_MAX, pr.n_edge - o); it.kf_c = pr.cur; it.kf_o = pr.oth;
+      items.push_back(it);
+    }
+  }
+  pstart[P] = (int)items.size();
+  c->n_bedge_items = (int)items.size();
+  c->d_bedge_items.reserve(items.size() + 1); c->d_bedge_pstart.reserve(P + 1);
+  c->d_bedge_partials.reserve((items.size() + 1) * GLIO_NACC_BIN); c->d_bedge_sums.reserve((size_t)(P + 1) * GLIO_NACC_BIN);
+  if (!items.empty()) GLIO_CUDA_TRY(cudaMemcpyAsync(c->d_bedge_items.p, items.data(), items.size() * sizeof(BinEdgeItem), cudaMemcpyHostToDevice, c->st));
+  GLIO_CUDA_TRY(cudaMemcpyAsync(c->d_bedge_pstart.p, pstart.data(), (P + 1) * sizeof(int), cudaMemcpyHostToDevice, c->st));
+  GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
+  c->bedge_dirty = false; c->bedge_K = K; c->bedge_P = P;
+}
+
+// what a binary evaluation returns: the plane blocks (glio_eval_binary), plane + edge blocks (glio_batch_solve with
+// glio_batch_use_edges on), or the edge blocks alone (glio_eval_binary_edge)
+enum BinBlocks { BIN_PLANES = 0, BIN_PLANES_EDGES = 1, BIN_EDGES = 2 };
+
 // device evaluation of all active binary residuals -> c->h_bin_diag (K x 28), c->h_bin_off (P x 36): everything is queued
-// (kernels, the all-reduce of a sharded run, the copies to pinned host memory); eval_binary_wait makes the result visible
-void eval_binary_launch(glio_ctx* c, int K, const double* poses, bool want_jac, double huber) {
+// (kernels, the all-reduce of a sharded run, the copies to pinned host memory); eval_binary_wait makes the result visible.
+// With edges, each pair's sums are S_plane + S_edge before the one block assembly, so the all-reduce is the same as without.
+void eval_binary_launch(glio_ctx* c, int K, const double* poses, bool want_jac, double huber, BinBlocks what = BIN_PLANES) {
   build_bin_items(c, K);
+  if (what != BIN_PLANES) build_bedge_items(c, K);
+  const bool add_edges = what == BIN_PLANES_EDGES && c->n_bedge_items > 0;   // no edges: exactly the plane launches
   const int P = (int)c->pairs.size();
   memcpy(c->h_bin_poses.p, poses, (size_t)K * 7 * sizeof(double));
   GLIO_CUDA_TRY(cudaMemcpyAsync(c->d_bin_poses.p, c->h_bin_poses.p, (size_t)K * 7 * sizeof(double), cudaMemcpyHostToDevice, c->st));
-  eval_binary_run(c->d_bin_items.p, c->n_bin_items, c->d_pair_item_start.p, P, K, c->d_bin_poses.p, c->prm.batch_score, huber, want_jac,
-                  c->d_bin_partials.p, c->d_pair_sums.p, c->d_kf_inc_start.p, c->d_inc.p, c->d_bin_diag.p, c->d_bin_off.p, nullptr, c->st, c->lc);
+  if (what == BIN_EDGES || add_edges)
+    eval_binary_edge_run(c->d_bedge_items.p, c->n_bedge_items, c->d_bedge_pstart.p, P, c->d_bin_poses.p, want_jac, c->d_bedge_partials.p,
+                         c->d_bedge_sums.p, c->st, c->lc);
+  if (what == BIN_EDGES)
+    bin_assemble_run(c->d_bedge_sums.p, K, P, c->d_kf_inc_start.p, c->d_inc.p, want_jac, c->d_bin_diag.p, c->d_bin_off.p, c->st, c->lc);
+  else
+    eval_binary_run(c->d_bin_items.p, c->n_bin_items, c->d_pair_item_start.p, P, K, c->d_bin_poses.p, c->prm.batch_score, huber, want_jac,
+                    c->d_bin_partials.p, c->d_pair_sums.p, c->d_kf_inc_start.p, c->d_inc.p, c->d_bin_diag.p, c->d_bin_off.p, nullptr, c->st,
+                    c->lc, add_edges ? c->d_bedge_sums.p : nullptr);
   if (c->allreduce) {
     // keyframe-sharded evaluation: every rank holds the same pair list but only its own pairs carry residuals;
     // one sum over ranks of the pose-block buffers per evaluation (SURVEY 8e "pose-block allreduce")
@@ -2000,21 +2231,18 @@ void eval_binary_launch(glio_ctx* c, int K, const double* poses, bool want_jac, 
   if (want_jac && P > 0) GLIO_CUDA_TRY(cudaMemcpyAsync(c->h_bin_off.p, c->d_bin_off.p, (size_t)P * 36 * sizeof(double), cudaMemcpyDeviceToHost, c->st));
 }
 void eval_binary_wait(glio_ctx* c) { GLIO_CUDA_TRY(cudaStreamSynchronize(c->st)); }
-void eval_binary_blocks(glio_ctx* c, int K, const double* poses, bool want_jac, double huber) {
-  eval_binary_launch(c, K, poses, want_jac, huber);
+void eval_binary_blocks(glio_ctx* c, int K, const double* poses, bool want_jac, double huber, BinBlocks what = BIN_PLANES) {
+  eval_binary_launch(c, K, poses, want_jac, huber, what);
   eval_binary_wait(c);
 }
 
-}  // namespace
-
-extern "C" {
-
-int glio_eval_binary(glio_ctx* c, int K, const double* poses, double* Hdiag, double* Hoff, double* g, double* cost) {
+// glio_eval_binary / glio_eval_binary_edge: the blocks as 6x6 / 6 / total cost on the host
+int eval_binary_out(glio_ctx* c, int K, const double* poses, BinBlocks what, double* Hdiag, double* Hoff, double* g, double* cost) {
   if (!c) return GLIO_ERR_ARG;
   return guarded(c, [&] {
     GLIO_REQUIRE(K > 0 && poses, GLIO_ERR_ARG, "bad arguments");
     const bool want_jac = Hdiag || Hoff || g;
-    eval_binary_blocks(c, K, poses, want_jac, /*no loss on batch LiDAR factors, Estimator.cpp:2768*/ 0.0);
+    eval_binary_blocks(c, K, poses, want_jac, /*no loss on batch LiDAR factors, Estimator.cpp:2768*/ 0.0, what);
     double ct = 0;
     for (int k = 0; k < K; ++k) {
       const double* o = c->h_bin_diag.p + (size_t)k * GLIO_NACC;
@@ -2025,6 +2253,24 @@ int glio_eval_binary(glio_ctx* c, int K, const double* poses, double* Hdiag, dou
     if (Hoff) memcpy(Hoff, c->h_bin_off.p, c->pairs.size() * 36 * sizeof(double));
     if (cost) *cost = ct;
   });
+}
+
+}  // namespace
+
+extern "C" {
+
+int glio_eval_binary(glio_ctx* c, int K, const double* poses, double* Hdiag, double* Hoff, double* g, double* cost) {
+  return eval_binary_out(c, K, poses, BIN_PLANES, Hdiag, Hoff, g, cost);
+}
+
+int glio_eval_binary_edge(glio_ctx* c, int K, const double* poses, double* Hdiag, double* Hoff, double* g, double* cost) {
+  return eval_binary_out(c, K, poses, BIN_EDGES, Hdiag, Hoff, g, cost);
+}
+
+int glio_batch_use_edges(glio_ctx* c, int on) {
+  if (!c) return GLIO_ERR_ARG;
+  c->batch_use_edges = on != 0; c->bedge_dirty = true;
+  return GLIO_OK;
 }
 
 
@@ -2125,7 +2371,7 @@ int glio_batch_solve(glio_ctx* c, int K, double* poses, double* speed_bias, glio
       }
       // the device evaluates the LiDAR pairs (and a sharded run sums them over the ranks) while the host evaluates its own
       // factors into the freshly reset band; the device blocks are added when they have arrived
-      eval_binary_launch(c, K, pz.data(), want_jac, 0.0);
+      eval_binary_launch(c, K, pz.data(), want_jac, 0.0, c->batch_use_edges ? BIN_PLANES_EDGES : BIN_PLANES);
       double ct = 0;
       int hrc = 0;
       if (want_jac) { H->reset(n, hb); std::fill(g, g + n, 0.0); }
@@ -2175,18 +2421,7 @@ int glio_set_edges(glio_ctx* c, int slot, const float* cp, const float* pa, cons
     Slot& sl = c->slot(slot);
     sl.n_edge = 0; sl.e_has_src = false; c->edge_items_dirty = true;
     if (n <= 0) return;
-    GLIO_REQUIRE(cp && pa && pb && s, GLIO_ERR_ARG, "null edge arrays");
-    std::vector<float4> h0(n), h1(n), h2(n);
-    for (int64_t i = 0; i < n; ++i) {
-      h0[i] = make_float4(cp[3 * i], cp[3 * i + 1], cp[3 * i + 2], (float)s[i]);
-      h1[i] = make_float4(pa[3 * i], pa[3 * i + 1], pa[3 * i + 2], 0.f);
-      h2[i] = make_float4(pb[3 * i], pb[3 * i + 1], pb[3 * i + 2], 0.f);
-    }
-    sl.e_cps.reserve(n); sl.e_pa.reserve(n); sl.e_pb.reserve(n);
-    GLIO_CUDA_TRY(cudaMemcpyAsync(sl.e_cps.p, h0.data(), n * sizeof(float4), cudaMemcpyHostToDevice, c->st));
-    GLIO_CUDA_TRY(cudaMemcpyAsync(sl.e_pa.p, h1.data(), n * sizeof(float4), cudaMemcpyHostToDevice, c->st));
-    GLIO_CUDA_TRY(cudaMemcpyAsync(sl.e_pb.p, h2.data(), n * sizeof(float4), cudaMemcpyHostToDevice, c->st));
-    GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
+    upload_edges(c, n, cp, pa, pb, s, sl.e_cps, sl.e_pa, sl.e_pb);
     sl.n_edge = n;
   });
 }

@@ -245,9 +245,12 @@ struct EdgeDst {
   float4* pb;
   int32_t* src;
 };
-// search + line fit: w.status (GLIO_EDGE_*), pa / pb per query in scan order; w.idx5 / w.sqd5 / eig (3 per query) when w.idx5 is set
+// search + line fit: w.status (GLIO_EDGE_*), pa / pb per query in scan order; w.idx5 / w.sqd5 / eig (3 per query) when w.idx5 is set.
+// oth_local != nullptr: pair mode (K1be), the line of a valid query refitted in the searched frame's stored coordinates (oth_stride
+// floats apart, original order); no debug views.
 void edge_assoc_run(const GridBuild& gb, const SegDesc* d_segs, int nseg, const AssocWork& w, const EdgeFitParams& ep, float4* pa, float4* pb,
-                    double* eig, DevBuf<int>& cell_count, DevBuf<int>& cell_pos, DevBuf<int>& scan_tmp, cudaStream_t st, LaunchCounter& lc);
+                    double* eig, const float* oth_local, int oth_stride, DevBuf<int>& cell_count, DevBuf<int>& cell_pos,
+                    DevBuf<int>& scan_tmp, cudaStream_t st, LaunchCounter& lc);
 // after compact_count on w.status: the valid records of every segment into dst[segment]
 void compact_edge_scatter(const AssocWork& w, const SegDesc* d_segs, const int* d_pos, const float4* pa, const float4* pb, float score,
                           const EdgeDst* d_dst, cudaStream_t st, LaunchCounter& lc);
@@ -307,10 +310,26 @@ struct BinItem {
 constexpr int GLIO_NACC_BIN = 55;   // uu(6) uv(9) vv(6) uz(9) vz(9) zz(6) | r*u(3) r*v(3) r*z(3) | cost
 // incidence list of a keyframe for the deterministic block assembly: (pair index, role 0 = cur / 1 = oth)
 struct BinIncidence { int32_t pair; int32_t role; };
+// d_pair_sums_edge (nullable): per-pair K2be sums added to the plane sums (S = S_plane + S_edge) before the block assembly
 void eval_binary_run(const BinItem* d_items, int nitems, const int* d_pair_item_start, int n_pairs, int K, const double* d_poses,
                      double score_scale, double huber_delta, bool want_jac, double* d_partials, double* d_pair_sums,
                      const int* d_kf_inc_start, const BinIncidence* d_inc, double* d_diag /*K*28*/, double* d_off /*n_pairs*36*/,
-                     double* d_cost, cudaStream_t st, LaunchCounter& lc);
+                     double* d_cost, cudaStream_t st, LaunchCounter& lc, const double* d_pair_sums_edge = nullptr);
+// k_bin_assemble alone: per-pair sums S -> d_diag (K x 28) and, with want_jac, d_off (n_pairs x 36)
+void bin_assemble_run(const double* d_pair_sums, int K, int n_pairs, const int* d_kf_inc_start, const BinIncidence* d_inc, bool want_jac,
+                      double* d_diag, double* d_off, cudaStream_t st, LaunchCounter& lc);
+
+// ---- K2be (eval.cu): binary point-to-edge factors, the edge counterpart of BinaryLidarPlaneNormFactor
+struct BinEdgeItem {
+  const float4* cps;          // (cp.xyz in cur's body frame, s)
+  const float4* pa;           // line point a in oth's body frame
+  const float4* pb;           // line point b in oth's body frame
+  int32_t count;
+  int32_t kf_c, kf_o;
+};
+// per-item partials (GLIO_NACC_BIN layout of K2b) and their per-pair sums in item order -> d_pair_sums (n_pairs x 55)
+void eval_binary_edge_run(const BinEdgeItem* d_items, int nitems, const int* d_pair_item_start, int n_pairs, const double* d_poses,
+                          bool want_jac, double* d_partials, double* d_pair_sums, cudaStream_t st, LaunchCounter& lc);
 
 // ---- front-end feature extraction (features.cu; Preprocessing.cpp:529-655)
 constexpr int FEAT_MAX_SHARP = 12, FEAT_MAX_LESS_SHARP = 60, FEAT_MAX_FLAT = 24;   // per ring: 6 sectors x (2, 10, 4)

@@ -516,6 +516,108 @@ __global__ void __launch_bounds__(BIN_T) k_eval_binary(const BinItem* __restrict
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// K2be: binary point-to-edge factors (glio_batch_use_edges, glio_eval_binary_edge), the conventions of
+// BinaryLidarPlaneNormFactor (no extrinsic, the line moves with oth, no loss):
+//   p_w = R(q_c) cp + t_c ;  A = R(q_o) a_l + t_o ;  B = R(q_o) b_l + t_o ;  e = (p_w - A) x (p_w - B) ;  r = s |e| / |A - B|
+// tangent Jacobians:  J_c = [g | 2 (R(q_c)cp x g)],  J_o = [-g | 2 (g x (p_w - t_o))]  with  g = s/|A-B| ((A-B) x e/|e|),
+// i.e. K2b's u, v, z with g in place of s N: the same 55 sums, so k_bin_pair_sums and k_bin_assemble take them unchanged.
+// Differences are formed relative to t_o (p_w - t_o and R(q_o) a_l), so kilometre offsets cancel before the cross product.
+// A point exactly on its line (|e| = 0) behaves as in K2e: r = 0 and a non-finite g.
+// HBM traffic per residual: 3 x 16 B (cp with s in .w, a_l, b_l).
+// ---------------------------------------------------------------------------------------------------------------
+template <bool WANT_JAC>
+__global__ void __launch_bounds__(BIN_T) k_eval_binary_edge(const BinEdgeItem* __restrict__ items, const double* __restrict__ poses,
+                                                            double* __restrict__ partials) {
+  __shared__ PairFrame F;
+  __shared__ double red[BIN_T / 32][NB];
+  const BinEdgeItem it = items[blockIdx.x];
+  if (threadIdx.x == 0) {
+    const double* P1 = poses + 7 * it.kf_c; const double* P2 = poses + 7 * it.kf_o;
+    double q1[4] = {P1[3], P1[4], P1[5], P1[6]}, q2[4] = {P2[3], P2[4], P2[5], P2[6]};
+    quat_to_mat(q1, F.R1); quat_to_mat(q2, F.R2);
+    F.t1[0] = P1[0]; F.t1[1] = P1[1]; F.t1[2] = P1[2]; F.t2[0] = P2[0]; F.t2[1] = P2[1]; F.t2[2] = P2[2];
+  }
+  __syncthreads();
+  double acc[NB];
+#pragma unroll
+  for (int k = 0; k < NB; ++k) acc[k] = 0.0;
+  for (int i = threadIdx.x; i < it.count; i += BIN_T) {
+    const float4 c4 = __ldg(&it.cps[i]);
+    const float4 a4 = __ldg(&it.pa[i]);
+    const float4 b4 = __ldg(&it.pb[i]);
+    const double s = (double)c4.w;
+    double a1[3]; mat_vec3(F.R1, (double)c4.x, (double)c4.y, (double)c4.z, a1);
+    const double pm[3] = {a1[0] + F.t1[0] - F.t2[0], a1[1] + F.t1[1] - F.t2[1], a1[2] + F.t1[2] - F.t2[2]};   // p_w - t_o
+    double ra[3]; mat_vec3(F.R2, (double)a4.x, (double)a4.y, (double)a4.z, ra);                             // A - t_o
+    double rb[3]; mat_vec3(F.R2, (double)b4.x, (double)b4.y, (double)b4.z, rb);                             // B - t_o
+    const double u[3] = {pm[0] - ra[0], pm[1] - ra[1], pm[2] - ra[2]};
+    const double w[3] = {pm[0] - rb[0], pm[1] - rb[1], pm[2] - rb[2]};
+    const double e[3] = {u[1] * w[2] - u[2] * w[1], u[2] * w[0] - u[0] * w[2], u[0] * w[1] - u[1] * w[0]};
+    const double de[3] = {ra[0] - rb[0], ra[1] - rb[1], ra[2] - rb[2]};
+    const double en = sqrt(e[0] * e[0] + e[1] * e[1] + e[2] * e[2]);
+    const double dn = sqrt(de[0] * de[0] + de[1] * de[1] + de[2] * de[2]);
+    const double r = en / dn * s;
+    acc[54] += 0.5 * (r * r);
+    if (WANT_JAC) {
+      const double k = s / dn / en;
+      const double gv[3] = {k * (de[1] * e[2] - de[2] * e[1]), k * (de[2] * e[0] - de[0] * e[2]), k * (de[0] * e[1] - de[1] * e[0])};
+      const double v[3] = {2.0 * (a1[1] * gv[2] - a1[2] * gv[1]), 2.0 * (a1[2] * gv[0] - a1[0] * gv[2]), 2.0 * (a1[0] * gv[1] - a1[1] * gv[0])};
+      const double z[3] = {2.0 * (gv[1] * pm[2] - gv[2] * pm[1]), 2.0 * (gv[2] * pm[0] - gv[0] * pm[2]), 2.0 * (gv[0] * pm[1] - gv[1] * pm[0])};
+      int kk = 0;
+#pragma unroll
+      for (int a = 0; a < 3; ++a)
+#pragma unroll
+        for (int b = a; b < 3; ++b) acc[kk++] += gv[a] * gv[b];       // uu  [0,6)
+#pragma unroll
+      for (int a = 0; a < 3; ++a)
+#pragma unroll
+        for (int b = 0; b < 3; ++b) acc[kk++] += gv[a] * v[b];        // uv  [6,15)
+#pragma unroll
+      for (int a = 0; a < 3; ++a)
+#pragma unroll
+        for (int b = a; b < 3; ++b) acc[kk++] += v[a] * v[b];         // vv  [15,21)
+#pragma unroll
+      for (int a = 0; a < 3; ++a)
+#pragma unroll
+        for (int b = 0; b < 3; ++b) acc[kk++] += gv[a] * z[b];        // uz  [21,30)
+#pragma unroll
+      for (int a = 0; a < 3; ++a)
+#pragma unroll
+        for (int b = 0; b < 3; ++b) acc[kk++] += v[a] * z[b];         // vz  [30,39)
+#pragma unroll
+      for (int a = 0; a < 3; ++a)
+#pragma unroll
+        for (int b = a; b < 3; ++b) acc[kk++] += z[a] * z[b];         // zz  [39,45)
+#pragma unroll
+      for (int a = 0; a < 3; ++a) { acc[45 + a] += r * gv[a]; acc[48 + a] += r * v[a]; acc[51 + a] += r * z[a]; }
+    }
+  }
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+#pragma unroll
+  for (int k = WANT_JAC ? 0 : 54; k < NB; ++k) {
+    double v = acc[k];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    if (lane == 0) red[wid][k] = v;
+  }
+  __syncthreads();
+  if (threadIdx.x < NB) {
+    double v = 0.0;
+    if (WANT_JAC || threadIdx.x == 54) {
+#pragma unroll
+      for (int w4 = 0; w4 < BIN_T / 32; ++w4) v += red[w4][threadIdx.x];
+    }
+    partials[(size_t)blockIdx.x * NB + threadIdx.x] = v;
+  }
+}
+
+// S += S_edge over n_pairs x NB sums (the binary plane and edge factors of a pair share one block assembly)
+__global__ void __launch_bounds__(256) k_bin_pair_add(double* __restrict__ S, const double* __restrict__ S_edge, int n) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) S[i] += S_edge[i];
+}
+
 // per pair: sum of its items' partials, in item order (deterministic)
 __global__ void __launch_bounds__(64) k_bin_pair_sums(const double* __restrict__ partials, const int* __restrict__ pair_item_start,
                                                       double* __restrict__ pair_sums) {
@@ -571,7 +673,7 @@ __global__ void __launch_bounds__(64) k_bin_assemble(const double* __restrict__ 
 void eval_binary_run(const BinItem* d_items, int nitems, const int* d_pair_item_start, int n_pairs, int K, const double* d_poses,
                      double score_scale, double huber_delta, bool want_jac, double* d_partials, double* d_pair_sums,
                      const int* d_kf_inc_start, const BinIncidence* d_inc, double* d_diag, double* d_off, double* d_cost,
-                     cudaStream_t st, LaunchCounter& lc) {
+                     cudaStream_t st, LaunchCounter& lc, const double* d_pair_sums_edge) {
   (void)d_cost;
   if (nitems > 0) {
     lc.begin(want_jac ? "k_eval_binary" : "k_eval_binary_cost", st);
@@ -581,10 +683,33 @@ void eval_binary_run(const BinItem* d_items, int nitems, const int* d_pair_item_
   }
   if (n_pairs > 0) {
     lc.begin("k_bin_pair_sums", st); k_bin_pair_sums<<<n_pairs, 64, 0, st>>>(d_partials, d_pair_item_start, d_pair_sums); lc.end(st);
+    if (d_pair_sums_edge) {
+      const int n = n_pairs * NB;
+      lc.begin("k_bin_pair_add", st); k_bin_pair_add<<<(n + 255) / 256, 256, 0, st>>>(d_pair_sums, d_pair_sums_edge, n); lc.end(st);
+    }
   }
+  bin_assemble_run(d_pair_sums, K, n_pairs, d_kf_inc_start, d_inc, want_jac, d_diag, d_off, st, lc);
+}
+
+void bin_assemble_run(const double* d_pair_sums, int K, int n_pairs, const int* d_kf_inc_start, const BinIncidence* d_inc, bool want_jac,
+                      double* d_diag, double* d_off, cudaStream_t st, LaunchCounter& lc) {
   lc.begin("k_bin_assemble", st);
   k_bin_assemble<<<K + (want_jac ? n_pairs : 0), 64, 0, st>>>(d_pair_sums, K, n_pairs, d_kf_inc_start, d_inc, nullptr, d_diag, d_off);
   lc.end(st);
+  GLIO_CUDA_TRY(cudaGetLastError());
+}
+
+void eval_binary_edge_run(const BinEdgeItem* d_items, int nitems, const int* d_pair_item_start, int n_pairs, const double* d_poses,
+                          bool want_jac, double* d_partials, double* d_pair_sums, cudaStream_t st, LaunchCounter& lc) {
+  if (nitems > 0) {
+    lc.begin(want_jac ? "k_eval_binary_edge" : "k_eval_binary_edge_cost", st);
+    if (want_jac) k_eval_binary_edge<true><<<nitems, BIN_T, 0, st>>>(d_items, d_poses, d_partials);
+    else k_eval_binary_edge<false><<<nitems, BIN_T, 0, st>>>(d_items, d_poses, d_partials);
+    lc.end(st);
+  }
+  if (n_pairs > 0) {
+    lc.begin("k_bin_pair_sums", st); k_bin_pair_sums<<<n_pairs, 64, 0, st>>>(d_partials, d_pair_item_start, d_pair_sums); lc.end(st);
+  }
   GLIO_CUDA_TRY(cudaGetLastError());
 }
 

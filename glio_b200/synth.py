@@ -216,6 +216,27 @@ def batch_problem(K=200, Q=100_000, seed=SEED0 + 3, search_range=6, rng_range=50
     return dict(scans=scans, poses_true=truth, poses_init=init, K=K, Q=Q, search_range=search_range, seed=seed)
 
 
+def batch_edge_problem(K=200, Q=10_000, seed=SEED0 + 3, search_range=6, frames=None, rng_range=50.0, noise=0.02):
+    """The corner counterpart of batch_problem: the same scene and poses for the same (K, seed), and corner scans of Q points in the
+    body frame (corner_sample within rng_range of the true pose), e.g. for glio_batch_set_edge_frame.  Every corner scan has its own
+    RNG stream (seed, k, 1), so a rank generates only its frames (`frames`; dist.frames_needed gives the halo); corner_scans[k] is
+    None for frames not requested."""
+    rng = np.random.default_rng(seed)
+    scene = Scene(-60.0, K + 60.0, rng)
+    truth = trajectory(K, rng)
+    init = perturb(truth, rng, sig_t=0.03, sig_r_deg=0.2)
+    want = set(range(K)) if frames is None else set(int(f) for f in frames)
+    scans = []
+    for k in range(K):
+        if k not in want:
+            scans.append(None)
+            continue
+        t, q = truth[k, :3], truth[k, 3:]
+        pw = corner_sample(scene, Q, np.random.default_rng([seed, k, 1]), t[0] - rng_range, t[0] + rng_range, noise=noise)
+        scans.append(((pw - t) @ quat_to_R(q)).astype(np.float32))
+    return dict(corner_scans=scans, poses_true=truth, poses_init=init, K=K, Q=Q, search_range=search_range, seed=seed)
+
+
 def raw_elevations(n_rings):
     """Elevation table (degrees) of a raw sweep for the ring rules of Preprocessing.cpp:441-483: every line sits inside its ring's
     interval, plus lines each rule treats specially.  16: VLP-16's -15..15 step 2, one line at -16.5 that int() truncates toward

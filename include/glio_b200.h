@@ -712,6 +712,53 @@ int glio_get_edges(glio_ctx* ctx, int slot, int64_t capacity, float* cp, float* 
  * sqd5[5Q], pm[3Q], eig[3Q] double (lambda ascending; 0 for GLIO_EDGE_FAIL_RADIUS). */
 int glio_get_edge_debug(glio_ctx* ctx, int slot, int64_t Q, uint8_t* status, int32_t* idx5, float* sqd5, float* pm, double* eig);
 
+/* ---- K1be / K2be: scan-to-multiscan EDGE association and binary point-to-edge factors in the batch solve.  The reference has
+ * neither; this is the batch counterpart of K1e / K2e, written the way K1b / K2b extend K1 / K2.
+ *
+ * The corner scan of a batch frame already registered with glio_batch_set_frame (unknown frame: GLIO_ERR_STATE, nothing changes):
+ * Q >= 0 points (0 to 4 are accepted: no pair that searches the frame gets an edge), stride in [3,64], host or device memory as
+ * glio_batch_set_frame; stored as received, in the body frame (quirk Q7).  The frame's pose is the one of glio_batch_set_frame /
+ * glio_batch_set_pose; both drop the corner grid as they drop the surf grid, and glio_batch_clear releases it. */
+int glio_batch_set_edge_frame(glio_ctx* ctx, int frame, const float* xyz, int64_t Q, int stride_floats, int mem);
+/* K1be: edge association of the pairs (cur[i], oth[i]).  For every corner point p of frame cur, with (t_c, q_c) cur's pose:
+ *   1. p_w = float(R(q_c) double(p) + t_c): K1b's transform, the body pose applied directly;
+ *   2. the exact 5 nearest neighbours of p_w in oth's corner cloud moved by oth's pose (the same transform), on its own K0 grid,
+ *      built once and reused by every pair that searches oth until oth's pose or corner scan changes;
+ *   3.-7. steps 3-7 of K1e on those five world points: the gate (double)sqd[4] < max_sqdist, the centroid, the scatter matrix, the
+ *      cyclic Jacobi and the line gate lambda_2 > min_ratio lambda_1 (status GLIO_EDGE_FAIL_RADIUS / GLIO_EDGE_FAIL_LINE);
+ *   8. for a valid query, steps 4-6 again on the same five indices in oth's LOCAL coordinates as stored (no gate on that fit; the
+ *      pair plane fit refits its plane the same way, Estimator.cpp:3752-3772), giving c_l and v_l; then, in scan order,
+ *      cp = p, pa = float(c_l + h v_l), pb = float(c_l - h v_l) (oth's frame), s = (float)score, src = the index of p in cur's scan.
+ * The arithmetic rules of K1e hold (only + - * / sqrt, round-to-nearest, no FMA).  Each pair's edge list is replaced; a pair not on
+ * the pair list yet is appended, with no plane matches (as glio_batch_set_pair_matches appends one).  Pairs are grouped by oth: one
+ * search launch and one host synchronisation (for the counts) per group, besides the grid build's own when oth's grid is built.
+ * n_edge[n_pairs] (may be NULL) receives the counts.  options NULL = the defaults.  An unknown frame, cur == oth or bad options is
+ * GLIO_ERR_ARG, a cur or oth without a corner scan is GLIO_ERR_STATE; both change nothing.  Feature selection
+ * (glio_batch_select*) leaves edge lists alone: all edges of a pair are evaluated. */
+int glio_batch_associate_edges_pairs(glio_ctx* ctx, const int32_t* cur, const int32_t* oth, int64_t n_pairs, const glio_edge_options* options,
+                                     int64_t* n_edge);
+/* copy-out of the edge list of pair (cur, oth), the conventions of glio_get_edges (pa / pb in oth's frame); a pair not on the pair
+ * list is GLIO_ERR_ARG */
+int glio_batch_get_edges(glio_ctx* ctx, int cur, int oth, int64_t capacity, float* cp, float* pa, float* pb, double* s, int32_t* src,
+                         int64_t* n);
+/* upload of the edge list of pair (cur, oth) (appended to the pair list if needed), as glio_set_edges: cp[3n] in cur's frame,
+ * pa/pb[3n] in oth's frame, s[n] (stored as float); src reads back as -1 */
+int glio_batch_set_pair_edges(glio_ctx* ctx, int cur, int oth, const float* cp, const float* pa, const float* pb, const double* s, int64_t n);
+/* K2be, the binary point-to-edge factor, with the conventions of BinaryLidarPlaneNormFactor (no extrinsic, the line moves with oth,
+ * no loss, Estimator.cpp:2768):
+ *   p_w = R(q_c) cp + t_c,  A = R(q_o) pa + t_o,  B = R(q_o) pb + t_o,  e = (p_w - A) x (p_w - B),  r = s |e| / |A - B|;
+ *   g = s / |A - B| ((A - B) x e / |e|),  J_c = [g | 2 (R(q_c) cp x g)],  J_o = [-g | 2 (g x (p_w - t_o))]  (tangent columns).
+ * A point exactly on its line (|e| = 0) is treated as by K2e: r = 0 and non-finite Jacobian entries.
+ * glio_eval_binary_edge returns the edge blocks alone in glio_eval_binary's layout and pair order (with the all-reduce hook, if set,
+ * as glio_eval_binary). */
+int glio_eval_binary_edge(glio_ctx* ctx, int K, const double* poses, double* Hdiag, double* Hoff, double* g, double* cost);
+/* on != 0: every evaluation inside glio_batch_solve (Jacobian and cost-only alike) adds the pairs' edge blocks: each pair's sums are
+ * S_plane + S_edge, each summed in item order, before the one block assembly, so a sharded run makes the same all-reduce calls as
+ * without edges.  Default off: glio_batch_solve then launches what it launches without edges; so it does when no pair has an edge.
+ * glio_eval_binary never includes edges.  The edge work-item plan is rebuilt only when an edge list, K, the pair count or this
+ * switch changes. */
+int glio_batch_use_edges(glio_ctx* ctx, int on);
+
 /* ---- batch minimizer (replaces ceres::Solve of optimizeBatchWithLandMark, Estimator.cpp:3275-3284: SUBSPACE_DOGLEG,
  * nonmonotonic steps, max_num_iter iterations; options == NULL selects exactly those).  The normal equations are
  * block-banded (half bandwidth (max|cur-oth|+1)*nt - 1) and stored/factored in band form.  Host factors (IMU chain,
