@@ -25,44 +25,60 @@ using namespace glio;
 
 namespace {
 
-struct Slot {
-  int64_t Q = 0;
+// n points, stride floats apart, on the device: uploaded into `own`, or a caller-owned device pointer (GLIO_DEVICE input)
+struct PointSet {
+  int64_t n = 0;
   int stride = 3;
-  DevBuf<float> scan;            // device copy of the scan (stride floats per point)
-  const float* scan_ptr = nullptr;  // == scan.p, or a caller-owned device pointer (GLIO_DEVICE input)
+  DevBuf<float> own;
+  const float* ptr = nullptr;    // == own.p, or the caller's pointer
+  void clear() { n = 0; ptr = nullptr; }
+};
+
+// the per-query views of one association (keep_debug): fit holds 4 doubles per query (the plane) or 3 (the line's eigenvalues)
+struct AssocDebug {
+  DevBuf<uint8_t> status;
+  DevBuf<int32_t> idx5;
+  DevBuf<float> sqd5;
+  DevBuf<float4> pm;
+  DevBuf<double> fit;
+  int64_t Q = 0;
+};
+
+// edge correspondences: cp with s in .w, line points pa / pb; src = scan index of each edge when an association produced them
+struct EdgeList {
+  DevBuf<float4> cps, pa, pb;
+  DevBuf<int32_t> src;
+  int64_t n = 0;
+  bool has_src = false;
+  void clear() { n = 0; has_src = false; }
+  // room for q edges; a reserve may drop the old contents, so the list must count as empty until it is refilled
+  EdgeDst reserve(int64_t q) {
+    cps.reserve((size_t)q); pa.reserve((size_t)q); pb.reserve((size_t)q); src.reserve((size_t)q);
+    return EdgeDst{cps.p, pa.p, pb.p, src.p};
+  }
+};
+
+struct Slot {
+  PointSet scan;                 // surf scan
   DevBuf<float4> m_cpw, m_nsd;   // compacted matches, scan order
   DevBuf<int32_t> m_src;
   int64_t n_match = 0;
   DevBuf<float4> s_cpw, s_nsd;   // selected subset
   DevBuf<int32_t> s_keep;        // its match indices (glio_select's list or the sampler's draws, glio_get_selection)
   int64_t n_sel = -1;            // -1: no selection -> all matches are active
-  DevBuf<float4> e_cps, e_pa, e_pb;  // edge correspondences (glio_set_edges or glio_window_associate_edges)
-  int64_t n_edge = 0;
-  DevBuf<int32_t> e_src;             // scan index of each edge, when they come from glio_window_associate_edges
-  bool e_has_src = false;
-  // corner scan (glio_window_set_edge_scan): same layout and ownership rules as scan / scan_ptr
-  int64_t eQ = 0;
-  int estride = 3;
-  DevBuf<float> escan;
-  const float* escan_ptr = nullptr;
-  // debug (keep_debug)
-  DevBuf<uint8_t> dbg_status;
-  DevBuf<int32_t> dbg_idx5;
-  DevBuf<float> dbg_sqd5;
-  DevBuf<float4> dbg_pm;
-  DevBuf<double> dbg_plane;
-  int64_t dbg_Q = 0;
-  DevBuf<uint8_t> edbg_status;       // the same for the last edge association, eigenvalues in place of the plane
-  DevBuf<int32_t> edbg_idx5;
-  DevBuf<float> edbg_sqd5;
-  DevBuf<float4> edbg_pm;
-  DevBuf<double> edbg_eig;
-  int64_t edbg_Q = 0;
-  void release() {
-    scan.release(); m_cpw.release(); m_nsd.release(); m_src.release(); s_cpw.release(); s_nsd.release(); s_keep.release(); e_cps.release(); e_pa.release(); e_pb.release();
-    dbg_status.release(); dbg_idx5.release(); dbg_sqd5.release(); dbg_pm.release(); dbg_plane.release();
-    e_src.release(); escan.release(); edbg_status.release(); edbg_idx5.release(); edbg_sqd5.release(); edbg_pm.release(); edbg_eig.release();
-  }
+  EdgeList edges;                // glio_set_edges or glio_window_associate_edges
+  PointSet corners;              // corner scan (glio_window_set_edge_scan)
+  AssocDebug dbg, edge_dbg;      // keep_debug: the last plane and the last edge association
+};
+
+// a map the window associates against (surf or corner points): its grid, and the local map that can build it
+struct FeatureMap {
+  GridBuild grid;
+  bool valid = false;
+  int64_t n = 0;
+  DevBuf<float> stage;           // host-input staging
+  LocalMap lm;
+  DevBuf<float> lm_stage;
 };
 
 }  // namespace
@@ -101,37 +117,30 @@ struct glio_ctx {
 
   int eval_slots = 296;        // resident evaluation blocks: 2 per SM (set from the device at creation)
   float pts_per_cell = 8.0f;   // target points per occupied grid cell (tuning hook: env GLIO_PTS_PER_CELL)
-  GridBuild map;
-  bool has_map = false;
-  DevBuf<float> map_stage;
+  FeatureMap map, edge_map;    // surf and corner
   // map prefetch (glio_map_prefetch): the next window's local map travels on the copy stream while the current window is marginalised
   DevBuf<float> map_stage2; const float* pf_ptr = nullptr; int64_t pf_M = 0; int pf_stride = 0; cudaEvent_t ev_map = nullptr;
 
   std::vector<std::unique_ptr<Slot>> slots;
 
   // ---- batch (scan-to-multiscan) state
+  // a frame's cloud and the grid of its world copy, built when a pair first searches it and dropped with the pose
+  struct FrameCloud { PointSet pts; GridBuild grid; bool grid_valid = false; };
   struct Frame {
-    int64_t Q = 0; int stride = 3;
-    DevBuf<float> scan; const float* scan_ptr = nullptr;
     double pose[7] = {0, 0, 0, 1, 0, 0, 0};
-    GridBuild grid; bool grid_valid = false;
-    // corner scan (glio_batch_set_edge_frame): same layout and ownership rules as scan / scan_ptr, 0 points allowed; its world
-    // cloud's grid is built when a pair first searches it and dropped with the pose
-    bool has_edge = false; int64_t eQ = 0; int estride = 3;
-    DevBuf<float> escan; const float* escan_ptr = nullptr;
-    GridBuild egrid; bool egrid_valid = false;
-    void release() { scan.release(); grid.release(); escan.release(); egrid.release(); }
+    FrameCloud surf;
+    FrameCloud corners;          // glio_batch_set_edge_frame, 0 points allowed
+    bool has_edge = false;
+    void set_pose(const double p[7]) {
+      for (int i = 0; i < 7; ++i) pose[i] = p[i];
+      surf.grid_valid = false; corners.grid_valid = false;
+    }
   };
   struct Pair {
     int cur = 0, oth = 0;
     DevBuf<float4> m_cpw; DevBuf<double> m_nc; DevBuf<int32_t> m_src; int64_t n_match = 0;
     DevBuf<float4> s_cpw; DevBuf<double> s_nc; DevBuf<int32_t> s_keep; int64_t n_sel = -1;
-    // edge list (glio_batch_associate_edges_pairs or glio_batch_set_pair_edges): cp in cur's frame with s in .w, pa / pb in oth's
-    DevBuf<float4> e_cps, e_pa, e_pb; DevBuf<int32_t> e_src; int64_t n_edge = 0; bool e_has_src = false;
-    void release() {
-      m_cpw.release(); m_nc.release(); m_src.release(); s_cpw.release(); s_nc.release(); s_keep.release();
-      e_cps.release(); e_pa.release(); e_pb.release(); e_src.release();
-    }
+    EdgeList edges;              // glio_batch_associate_edges_pairs or glio_batch_set_pair_edges: cp in cur's frame, pa / pb in oth's
   };
   std::map<int, std::unique_ptr<Frame>> frames;
   std::vector<std::unique_ptr<Pair>> pairs;
@@ -177,12 +186,7 @@ struct glio_ctx {
   DevBuf<int> d_kf_item_start;
   DevBuf<double> d_partials, d_out, d_poses, d_r, d_J;
   PinnedBuf<double> h_out, h_poses;
-  // local map maintenance (SURVEY 8 f-1): world-frame keyframe clouds in deque order, concatenation, voxel filter work space
-  LocalMap lm;
-  DevBuf<float> lm_stage; int64_t map_n = 0;
-  // edge association (K1e): the corner map, the corner local map, and the per-query line-fit outputs (scan order)
-  GridBuild edge_map; bool has_edge_map = false; DevBuf<float> edge_map_stage;
-  LocalMap elm; DevBuf<float> elm_stage;
+  // edge association (K1e): the per-query line-fit outputs (scan order)
   DevBuf<float4> w_pa, w_pb; DevBuf<double> w_eig; DevBuf<EdgeDst> d_edst;
   // edge blocks inside the window solve and marginalisation (glio_window_use_edges): the K2e work-item plan of slots 0..W-1, rebuilt
   // only when an edge list or W changes; K2e runs on the main stream before K2 and its W x 28 result is copied into pinned h_eout
@@ -261,6 +265,61 @@ const float* stage_points(glio_ctx* c, DevBuf<float>& buf, const float* xyz, int
   return buf.p;
 }
 
+// the same into a point set (main stream)
+void stage_points(glio_ctx* c, PointSet& ps, const float* xyz, int64_t n, int stride, int mem) {
+  ps.ptr = stage_points(c, ps.own, xyz, n, stride, mem);
+  ps.n = n; ps.stride = stride;
+}
+
+// Host clouds travel on the copy stream, so the next window's upload can overlap a running solve; device clouds are borrowed.
+// Per call the copy stream waits once for the main stream (nothing queued there may still read the buffers) and one event,
+// which the next association waits for, marks the end of all the uploads.
+void upload_points_async(glio_ctx* c, const std::vector<PointSet*>& sets, const float* const* xyz, const int64_t* n, int stride, int mem) {
+  if (mem != GLIO_DEVICE) {
+    GLIO_CUDA_TRY(cudaEventRecord(c->ev_main, c->st));
+    GLIO_CUDA_TRY(cudaStreamWaitEvent(c->st_copy, c->ev_main, 0));
+  }
+  for (size_t i = 0; i < sets.size(); ++i) {
+    PointSet& ps = *sets[i];
+    if (mem == GLIO_DEVICE) ps.ptr = xyz[i];
+    else {
+      ps.own.reserve((size_t)n[i] * stride);
+      GLIO_CUDA_TRY(cudaMemcpyAsync(ps.own.p, xyz[i], (size_t)n[i] * stride * sizeof(float), cudaMemcpyHostToDevice, c->st_copy));
+      ps.ptr = ps.own.p;
+    }
+    ps.n = n[i]; ps.stride = stride;
+  }
+  if (mem != GLIO_DEVICE) { GLIO_CUDA_TRY(cudaEventRecord(c->ev_scans, c->st_copy)); c->scans_pending = true; }
+}
+
+// one association segment: the points of ps from global query index off on, moved by pose = (t, q)
+SegDesc make_seg(const PointSet& ps, int64_t off, const double* pose) {
+  SegDesc sd;
+  sd.src = ps.ptr; sd.stride = ps.stride; sd.count = ps.n; sd.offset = off;
+  for (int k = 0; k < 3; ++k) sd.t[k] = pose[k];
+  for (int k = 0; k < 4; ++k) sd.q[k] = pose[3 + k];
+  return sd;
+}
+
+// the x, y, z of n float4 into xyz (3 floats each) and, when w is set, their w
+void unpack_float4(const float4* h, int64_t n, float* xyz, float* w = nullptr) {
+  for (int64_t i = 0; i < n; ++i) {
+    if (xyz) { xyz[3 * i] = h[i].x; xyz[3 * i + 1] = h[i].y; xyz[3 * i + 2] = h[i].z; }
+    if (w) w[i] = h[i].w;
+  }
+}
+
+// queues the copy of the association's per-query views [off, off + q) from the work space into d (fit: nfit doubles per query)
+void capture_debug(glio_ctx* c, AssocDebug& d, const AssocWork& w, const double* fit, int nfit, int64_t off, int64_t q) {
+  d.status.reserve(q); d.idx5.reserve(5 * q); d.sqd5.reserve(5 * q); d.pm.reserve(q); d.fit.reserve(nfit * q);
+  GLIO_CUDA_TRY(cudaMemcpyAsync(d.status.p, w.status + off, q, cudaMemcpyDeviceToDevice, c->st));
+  GLIO_CUDA_TRY(cudaMemcpyAsync(d.idx5.p, w.idx5 + 5 * off, 5 * q * sizeof(int32_t), cudaMemcpyDeviceToDevice, c->st));
+  GLIO_CUDA_TRY(cudaMemcpyAsync(d.sqd5.p, w.sqd5 + 5 * off, 5 * q * sizeof(float), cudaMemcpyDeviceToDevice, c->st));
+  GLIO_CUDA_TRY(cudaMemcpyAsync(d.pm.p, w.pm + off, q * sizeof(float4), cudaMemcpyDeviceToDevice, c->st));
+  GLIO_CUDA_TRY(cudaMemcpyAsync(d.fit.p, fit + nfit * off, nfit * q * sizeof(double), cudaMemcpyDeviceToDevice, c->st));
+  d.Q = q;
+}
+
 void ensure_work(glio_ctx* c, int64_t Qt, bool pair, bool keep_debug) {
   c->w_pm.reserve((size_t)Qt); c->w_pmq.reserve((size_t)Qt); c->w_seg.reserve((size_t)Qt);
   c->w_status.reserve((size_t)Qt); c->w_weight.reserve((size_t)Qt);
@@ -292,14 +351,12 @@ void associate_slots(glio_ctx* c, const GridBuild& grid, const AssocGates& gates
   int64_t Qt = 0;
   for (int s = 0; s < nseg; ++s) {
     Slot& sl = *slots[s];
-    GLIO_REQUIRE(sl.Q > 0 && sl.scan_ptr, GLIO_ERR_STATE, "slot has no scan");
-    segs[s].src = sl.scan_ptr; segs[s].stride = sl.stride; segs[s].count = sl.Q; segs[s].offset = Qt;
-    for (int k = 0; k < 3; ++k) segs[s].t[k] = lidar_poses[s][k];
-    for (int k = 0; k < 4; ++k) segs[s].q[k] = lidar_poses[s][3 + k];
-    sl.m_cpw.reserve((size_t)sl.Q); sl.m_nsd.reserve((size_t)sl.Q); sl.m_src.reserve((size_t)sl.Q);
+    GLIO_REQUIRE(sl.scan.n > 0 && sl.scan.ptr, GLIO_ERR_STATE, "slot has no scan");
+    segs[s] = make_seg(sl.scan, Qt, lidar_poses[s].data());
+    sl.m_cpw.reserve((size_t)sl.scan.n); sl.m_nsd.reserve((size_t)sl.scan.n); sl.m_src.reserve((size_t)sl.scan.n);
     dst[s].cpw = sl.m_cpw.p; dst[s].nsd = sl.m_nsd.p; dst[s].nc = nullptr; dst[s].src = sl.m_src.p;
     sl.n_sel = -1;
-    Qt += sl.Q;
+    Qt += sl.scan.n;
   }
   ensure_work(c, Qt, false, keep_debug);
   c->d_segs.reserve(nseg); c->d_dst.reserve(nseg); c->d_counts.reserve(nseg); c->h_counts.reserve(nseg);
@@ -312,19 +369,8 @@ void associate_slots(glio_ctx* c, const GridBuild& grid, const AssocGates& gates
   compact_run(w, c->d_segs.p, nseg, c->w_flags.p, c->w_pos.p, c->scan_tmp, c->d_dst.p, c->d_counts.p, c->st, c->lc);
   tr.mark("compact");
   GLIO_CUDA_TRY(cudaMemcpyAsync(c->h_counts.p, c->d_counts.p, nseg * sizeof(int), cudaMemcpyDeviceToHost, c->st));
-  if (keep_debug) {
-    for (int s = 0; s < nseg; ++s) {
-      Slot& sl = *slots[s];
-      const int64_t o = segs[s].offset, q = sl.Q;
-      sl.dbg_status.reserve(q); sl.dbg_idx5.reserve(5 * q); sl.dbg_sqd5.reserve(5 * q); sl.dbg_pm.reserve(q); sl.dbg_plane.reserve(4 * q);
-      GLIO_CUDA_TRY(cudaMemcpyAsync(sl.dbg_status.p, w.status + o, q, cudaMemcpyDeviceToDevice, c->st));
-      GLIO_CUDA_TRY(cudaMemcpyAsync(sl.dbg_idx5.p, w.idx5 + 5 * o, 5 * q * sizeof(int32_t), cudaMemcpyDeviceToDevice, c->st));
-      GLIO_CUDA_TRY(cudaMemcpyAsync(sl.dbg_sqd5.p, w.sqd5 + 5 * o, 5 * q * sizeof(float), cudaMemcpyDeviceToDevice, c->st));
-      GLIO_CUDA_TRY(cudaMemcpyAsync(sl.dbg_pm.p, w.pm + o, q * sizeof(float4), cudaMemcpyDeviceToDevice, c->st));
-      GLIO_CUDA_TRY(cudaMemcpyAsync(sl.dbg_plane.p, w.plane + 4 * o, 4 * q * sizeof(double), cudaMemcpyDeviceToDevice, c->st));
-      sl.dbg_Q = q;
-    }
-  }
+  if (keep_debug)
+    for (int s = 0; s < nseg; ++s) capture_debug(c, slots[s]->dbg, w, w.plane, 4, segs[s].offset, slots[s]->scan.n);
   GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
   for (int s = 0; s < nseg; ++s) {
     Slot& sl = *slots[s];
@@ -336,11 +382,11 @@ void associate_slots(glio_ctx* c, const GridBuild& grid, const AssocGates& gates
 
 // the context's own window association: its map, its gates, slots 0..
 void associate_ctx_slots(glio_ctx* c, const std::vector<int>& ids, const std::vector<std::array<double, 7>>& lidar_poses, int64_t* n_match) {
-  GLIO_REQUIRE(c->has_map, GLIO_ERR_STATE, "glio_set_map must be called before association");
+  GLIO_REQUIRE(c->map.valid, GLIO_ERR_STATE, "glio_set_map must be called before association");
   std::vector<Slot*> sl;
   for (int id : ids) sl.push_back(&c->slot(id));
   const AssocGates gates{c->prm.kd_max_radius, c->prm.surf_dist_thres, c->prm.weight_min};
-  associate_slots(c, c->map, gates, c->prm.keep_debug != 0, sl, lidar_poses, n_match);
+  associate_slots(c, c->map.grid, gates, c->prm.keep_debug != 0, sl, lidar_poses, n_match);
   c->items_dirty = true;
 }
 
@@ -416,6 +462,19 @@ EvalParams eval_params(const glio_ctx* c) {
   return ep;
 }
 
+// the W x 28 layout (per keyframe: 21 upper-triangular H, 6 g, 1 cost) as full 6x6 H, g and per-keyframe cost, each nullable
+void unpack_blocks(const double* o28, int W, double* H, double* g, double* cost) {
+  for (int k = 0; k < W; ++k) {
+    const double* o = o28 + (size_t)k * GLIO_NACC;
+    if (H) {
+      int idx = 0;
+      for (int p = 0; p < 6; ++p) for (int q = p; q < 6; ++q) { H[36 * k + 6 * p + q] = o[idx]; H[36 * k + 6 * q + p] = o[idx]; ++idx; }
+    }
+    if (g) for (int p = 0; p < 6; ++p) g[6 * k + p] = o[21 + p];
+    if (cost) cost[k] = o[27];
+  }
+}
+
 void fill_summary(const SolverSummary& S, int n, glio_solver_summary* summary, glio_iteration* iter_log, int iter_cap, double* step_log, int64_t step_cap) {
   if (summary) {
       memset(summary, 0, sizeof(*summary));
@@ -458,10 +517,10 @@ std::vector<EdgeItem> plan_edge_items(const glio_ctx* c, int W, std::vector<int>
   for (int k = 0; k < W; ++k) {
     start[k] = (int)items.size();
     if ((size_t)k >= c->slots.size() || !c->slots[k]) continue;
-    const Slot& sl = *c->slots[k];
-    for (int64_t o = 0; o < sl.n_edge; o += GLIO_ITEM_MAX) {
-      EdgeItem it; it.cps = sl.e_cps.p + o; it.pa = sl.e_pa.p + o; it.pb = sl.e_pb.p + o;
-      it.count = (int32_t)std::min<int64_t>(GLIO_ITEM_MAX, sl.n_edge - o); it.kf = k; items.push_back(it);
+    const EdgeList& e = c->slots[k]->edges;
+    for (int64_t o = 0; o < e.n; o += GLIO_ITEM_MAX) {
+      EdgeItem it; it.cps = e.cps.p + o; it.pa = e.pa.p + o; it.pb = e.pb.p + o;
+      it.count = (int32_t)std::min<int64_t>(GLIO_ITEM_MAX, e.n - o); it.kf = k; items.push_back(it);
     }
   }
   start[W] = (int)items.size();
@@ -600,32 +659,11 @@ void glio_destroy(glio_ctx* c) {
     c->marg_cv.notify_one();
     c->marg_thread.join();
   }
+  // nothing queued may still use the context's buffers when `delete c` frees them
   if (c->st_copy) cudaStreamSynchronize(c->st_copy);
   if (c->st) cudaStreamSynchronize(c->st);
-  c->map.release(); c->map_stage.release(); c->map_stage2.release(); if (c->ev_map) cudaEventDestroy(c->ev_map);
-  c->lm.release(); c->lm_stage.release();
-  c->edge_map.release(); c->edge_map_stage.release(); c->elm.release(); c->elm_stage.release();
-  c->w_pa.release(); c->w_pb.release(); c->w_eig.release(); c->d_edst.release();
-  c->se_items.release(); c->se_start.release(); c->se_part.release(); c->se_out.release(); c->se_poses.release(); c->h_eout.release();
-  for (auto& f : c->frames) f.second->release();
-  for (auto& p : c->pairs) p->release();
-  c->d_bedge_items.release(); c->d_bedge_pstart.release(); c->d_bedge_partials.release(); c->d_bedge_sums.release();
-  c->d_bin_items.release(); c->d_pair_item_start.release(); c->d_kf_inc_start.release(); c->d_inc.release(); c->d_bin_partials.release();
-  c->d_pair_sums.release(); c->d_bin_diag.release(); c->d_bin_off.release(); c->d_bin_poses.release(); c->h_bin_diag.release(); c->h_bin_off.release(); c->h_bin_poses.release();
-  for (auto& s : c->slots) if (s) s->release();
-  c->w_pm.release(); c->w_pmq.release(); c->w_nsd.release(); c->w_seg.release(); c->w_status.release(); c->w_weight.release();
-  c->w_nc.release(); c->w_plane.release(); c->w_idx5.release(); c->w_sqd5.release(); c->w_flags.release(); c->w_pos.release();
-  c->cell_count.release(); c->cell_pos.release(); c->scan_tmp.release(); c->d_segs.release(); c->d_dst.release(); c->d_counts.release();
-  c->h_counts.release(); c->d_bad.release(); c->d_items.release(); c->d_kf_item_start.release();
-  c->d_partials.release(); c->d_out.release(); c->d_poses.release(); c->d_r.release(); c->d_J.release(); c->h_out.release();
-  c->h_poses.release(); c->h_flag.release(); c->d_ticket.release(); c->w_knn_idx.release(); c->w_knn_sqd.release();
-  c->f_cloud.release(); c->f_curv.release(); c->f_label.release(); c->f_picked.release(); c->f_scan.release(); c->f_ring.release(); c->f_lf.release(); c->f_counts.release(); c->f_out.release(); c->f_ds.release(); c->f_outds.release();
-  c->sp_raw.release(); c->sp_ori.release(); c->sp_ring.release(); c->sp_hist.release(); c->sp_hscan.release(); c->sp_small.release();
-  c->sp_scan_tmp.release(); c->sp_consts.release(); c->sp_out.release(); c->sp_hits.release();
-  c->e_items.release(); c->e_start.release(); c->e_part.release(); c->e_out.release(); c->e_poses.release();
-  c->icp.release(); c->icp_src.release(); c->icp_tgt.release();
-  c->vsort.release(); c->vs_stage.release(); c->gm_cat.release(); c->gm_segs.release();
-  c->d_sel_segs.release(); c->h_sel_segs.release(); if (c->ev_sel) cudaEventDestroy(c->ev_sel);
+  if (c->ev_map) cudaEventDestroy(c->ev_map);
+  if (c->ev_sel) cudaEventDestroy(c->ev_sel);
   for (auto& r : c->lc.recs) { cudaEventDestroy(r.a); cudaEventDestroy(r.b); }
   for (auto& e : c->lc.pool) cudaEventDestroy(e);
   c->lc.recs.clear(); c->lc.pool.clear();
@@ -722,6 +760,16 @@ void glio_lidar_pose(const glio_params* prm, const double pose_body[7], double t
   lidar_pose_in_map(prm->q_lb, prm->t_lb, pose_body, t2, q2);
 }
 
+}  // extern "C"
+
+// M points on the device become the map's grid (glio_set_map, glio_set_edge_map and the local-map builds)
+static void map_build(glio_ctx* c, FeatureMap& m, const float* d, int stride, int64_t M) {
+  grid_build(m.grid, d, stride, M, nullptr, nullptr, c->prm.cell_size, c->pts_per_cell, c->st, c->lc);
+  m.valid = true; m.n = M;
+}
+
+extern "C" {
+
 int glio_set_map(glio_ctx* c, const float* xyz, int64_t M, int stride, int mem) {
   if (!c) return GLIO_ERR_ARG;
   return guarded(c, [&] {
@@ -730,12 +778,11 @@ int glio_set_map(glio_ctx* c, const float* xyz, int64_t M, int stride, int mem) 
     if (mem != GLIO_DEVICE && c->pf_ptr == xyz && c->pf_M == M && c->pf_stride == stride) {
       // the upload was started by glio_map_prefetch: wait for it on the main stream, no second copy
       GLIO_CUDA_TRY(cudaStreamWaitEvent(c->st, c->ev_map, 0));
-      std::swap(c->map_stage, c->map_stage2);
-      d = c->map_stage.p;
-    } else d = stage_points(c, c->map_stage, xyz, M, stride, mem);
+      std::swap(c->map.stage, c->map_stage2);
+      d = c->map.stage.p;
+    } else d = stage_points(c, c->map.stage, xyz, M, stride, mem);
     c->pf_ptr = nullptr;
-    grid_build(c->map, d, stride, M, nullptr, nullptr, c->prm.cell_size, c->pts_per_cell, c->st, c->lc);
-    c->has_map = true; c->map_n = M;
+    map_build(c, c->map, d, stride, M);
   });
 }
 
@@ -755,31 +802,41 @@ int glio_map_prefetch(glio_ctx* c, const float* xyz, int64_t M, int stride) {
 
 }  // extern "C"
 
-// the context's two local maps (surf: lm, corner: elm) share these
-static int localmap_clear(glio_ctx* c, LocalMap& lm) {
-  if (!c) return GLIO_ERR_ARG;
+// the context's two local maps (surf and corner) share these
+static int localmap_clear(glio_ctx* c, FeatureMap& m) {
   return guarded(c, [&] {
     GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
-    lm.clear();
+    m.lm.clear();
   });
 }
 
-static int localmap_push(glio_ctx* c, LocalMap& lm, DevBuf<float>& stage, int at_front, const float* cloud_xyz, int64_t n, int stride, int mem,
-                         const double t[3], const double q[4]) {
-  if (!c) return GLIO_ERR_ARG;
+static int localmap_push(glio_ctx* c, FeatureMap& m, int at_front, const float* cloud_xyz, int64_t n, int stride, int mem, const double t[3],
+                         const double q[4]) {
   return guarded(c, [&] {
     GLIO_REQUIRE(t && q, GLIO_ERR_ARG, "null pose");
-    const float* d = stage_points(c, stage, cloud_xyz, n, stride, mem);
-    lm.push(at_front != 0, d, stride, n, t, q, c->st, c->lc);                // transformCloud: float(q*double(p)+t)
+    const float* d = stage_points(c, m.lm_stage, cloud_xyz, n, stride, mem);
+    m.lm.push(at_front != 0, d, stride, n, t, q, c->st, c->lc);              // transformCloud: float(q*double(p)+t)
     if (mem != GLIO_DEVICE) GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));    // the staging buffer is reused by the next push
   });
 }
 
-static int localmap_pop_front(glio_ctx* c, LocalMap& lm) {
-  if (!c) return GLIO_ERR_ARG;
+static int localmap_pop_front(glio_ctx* c, FeatureMap& m) {
   return guarded(c, [&] {
-    GLIO_REQUIRE(!lm.frames.empty(), GLIO_ERR_STATE, "local map holds no keyframe cloud");
-    lm.pop_front();
+    GLIO_REQUIRE(!m.lm.frames.empty(), GLIO_ERR_STATE, "local map holds no keyframe cloud");
+    m.lm.pop_front();
+  });
+}
+
+// *surf_local_map += *recent_surf_keyframes[i] (Estimator.cpp:3605-3608), ds_filter_surf_map.filter (:3617-3618); leaf <= 0, or
+// PCL's pass-through when the voxel grid would overflow, leaves the concatenation as it is.  name: "local map" or "corner local map"
+static int localmap_build(glio_ctx* c, FeatureMap& m, const char* name, float leaf, int64_t* n_map) {
+  return guarded(c, [&] {
+    GLIO_REQUIRE(m.lm.n_points() >= 5, GLIO_ERR_STATE, std::string(name) + " needs at least 5 points");
+    const float* pts = nullptr; int stride = 0; bool filtered = false;
+    const int64_t n = m.lm.build(leaf, &pts, &stride, &filtered, c->st, c->lc);
+    GLIO_REQUIRE(!filtered || n >= 5, GLIO_ERR_STATE, "down-sampled " + std::string(name) + " has fewer than 5 points");
+    map_build(c, m, pts, stride, n);                                          // kd_tree_surf_local_map->setInputCloud
+    if (n_map) *n_map = n;
   });
 }
 
@@ -788,53 +845,42 @@ extern "C" {
 // ---- local map maintenance on the device (Estimator.cpp:3529-3631 buildLocalMapWithLandMark, :3615-3618 downSampleCloud) ----
 int glio_localmap_clear(glio_ctx* c) {
   if (!c) return GLIO_ERR_ARG;
-  return localmap_clear(c, c->lm);
+  return localmap_clear(c, c->map);
 }
 
 int glio_localmap_push(glio_ctx* c, int at_front, const float* cloud_xyz, int64_t n, int stride, int mem, const double t[3], const double q[4]) {
   if (!c) return GLIO_ERR_ARG;
-  return localmap_push(c, c->lm, c->lm_stage, at_front, cloud_xyz, n, stride, mem, t, q);
+  return localmap_push(c, c->map, at_front, cloud_xyz, n, stride, mem, t, q);
 }
 
 int glio_localmap_pop_front(glio_ctx* c) {
   if (!c) return GLIO_ERR_ARG;
-  return localmap_pop_front(c, c->lm);
+  return localmap_pop_front(c, c->map);
 }
 
 int glio_localmap_size(glio_ctx* c, int* n_frames, int64_t* n_points) {
   if (!c) return GLIO_ERR_ARG;
-  if (n_frames) *n_frames = (int)c->lm.frames.size();
-  if (n_points) *n_points = c->lm.n_points();
+  if (n_frames) *n_frames = (int)c->map.lm.frames.size();
+  if (n_points) *n_points = c->map.lm.n_points();
   return GLIO_OK;
 }
 
 int glio_localmap_build(glio_ctx* c, float leaf, int64_t* n_map) {
   if (!c) return GLIO_ERR_ARG;
-  return guarded(c, [&] {
-    GLIO_REQUIRE(c->lm.n_points() >= 5, GLIO_ERR_STATE, "local map needs at least 5 points");
-    // *surf_local_map += *recent_surf_keyframes[i] (:3605-3608), ds_filter_surf_map.filter (:3617-3618); leaf <= 0, or PCL's
-    // pass-through when the voxel grid would overflow, leaves the concatenation as it is
-    const float* pts = nullptr; int stride = 0; bool filtered = false;
-    const int64_t m = c->lm.build(leaf, &pts, &stride, &filtered, c->st, c->lc);
-    GLIO_REQUIRE(!filtered || m >= 5, GLIO_ERR_STATE, "down-sampled local map has fewer than 5 points");
-    grid_build(c->map, pts, stride, m, nullptr, nullptr, c->prm.cell_size, c->pts_per_cell, c->st, c->lc);   // kd_tree_surf_local_map->setInputCloud
-    c->map_n = m;
-    c->has_map = true;
-    if (n_map) *n_map = c->map_n;
-  });
+  return localmap_build(c, c->map, "local map", leaf, n_map);
 }
 
 int glio_get_map(glio_ctx* c, int64_t capacity, float* xyz, int64_t* n_out) {
   if (!c) return GLIO_ERR_ARG;
   return guarded(c, [&] {
-    GLIO_REQUIRE(c->has_map, GLIO_ERR_STATE, "no map set");
-    const int64_t n = std::min<int64_t>(capacity, c->map_n);
-    if (n_out) *n_out = c->map_n;
+    GLIO_REQUIRE(c->map.valid, GLIO_ERR_STATE, "no map set");
+    const int64_t n = std::min<int64_t>(capacity, c->map.n);
+    if (n_out) *n_out = c->map.n;
     if (n <= 0 || !xyz) return;
-    std::vector<float> h((size_t)n * 4);
-    GLIO_CUDA_TRY(cudaMemcpyAsync(h.data(), c->map.tmp4.p, (size_t)n * sizeof(float4), cudaMemcpyDeviceToHost, c->st));
+    std::vector<float4> h((size_t)n);
+    GLIO_CUDA_TRY(cudaMemcpyAsync(h.data(), c->map.grid.tmp4.p, (size_t)n * sizeof(float4), cudaMemcpyDeviceToHost, c->st));
     GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
-    for (int64_t i = 0; i < n; ++i) { xyz[3 * i] = h[4 * i]; xyz[3 * i + 1] = h[4 * i + 1]; xyz[3 * i + 2] = h[4 * i + 2]; }
+    unpack_float4(h.data(), n, xyz);
   });
 }
 
@@ -843,9 +889,7 @@ int glio_assoc_scan_to_map(glio_ctx* c, int slot, const float* scan_xyz, int64_t
   if (!c) return GLIO_ERR_ARG;
   return guarded(c, [&] {
     GLIO_REQUIRE(t && q, GLIO_ERR_ARG, "null pose");
-    Slot& sl = c->slot(slot);
-    sl.scan_ptr = stage_points(c, sl.scan, scan_xyz, Q, stride, mem);
-    sl.Q = Q; sl.stride = stride;
+    stage_points(c, c->slot(slot).scan, scan_xyz, Q, stride, mem);
     std::vector<std::array<double, 7>> lp(1);
     for (int k = 0; k < 3; ++k) lp[0][k] = t[k];
     for (int k = 0; k < 4; ++k) lp[0][3 + k] = q[k];
@@ -858,25 +902,15 @@ int glio_window_set_scans(glio_ctx* c, int W, const float* const* scans, const i
   return guarded(c, [&] {
     GLIO_REQUIRE(W > 0 && scans && Q, GLIO_ERR_ARG, "bad window arguments");
     GLIO_REQUIRE(stride >= 3 && stride <= 64, GLIO_ERR_ARG, "stride_floats must be in [3,64]");
-    // Host scans are uploaded on the copy stream: the call returns at once and the next association waits for the
-    // event.  The matches of the previous association stay valid (they hold their own copies of the points), so the
-    // scans of the NEXT window can be handed over while the current window is still being solved.
-    if (mem != GLIO_DEVICE) {
-      GLIO_CUDA_TRY(cudaEventRecord(c->ev_main, c->st));
-      GLIO_CUDA_TRY(cudaStreamWaitEvent(c->st_copy, c->ev_main, 0));      // nothing queued on the main stream may still read the slot buffers
-    }
+    // The call returns at once and the next association waits for the uploads.  The matches of the previous association stay
+    // valid (they hold their own copies of the points), so the scans of the NEXT window can be handed over while the current
+    // window is still being solved.
+    std::vector<PointSet*> sets(W);
     for (int k = 0; k < W; ++k) {
-      Slot& sl = c->slot(k);
+      sets[k] = &c->slot(k).scan;
       GLIO_REQUIRE(scans[k] != nullptr && Q[k] > 0, GLIO_ERR_ARG, "null or empty point array");
-      if (mem == GLIO_DEVICE) sl.scan_ptr = scans[k];
-      else {
-        sl.scan.reserve((size_t)Q[k] * stride);
-        GLIO_CUDA_TRY(cudaMemcpyAsync(sl.scan.p, scans[k], (size_t)Q[k] * stride * sizeof(float), cudaMemcpyHostToDevice, c->st_copy));
-        sl.scan_ptr = sl.scan.p;
-      }
-      sl.Q = Q[k]; sl.stride = stride;
     }
-    if (mem != GLIO_DEVICE) { GLIO_CUDA_TRY(cudaEventRecord(c->ev_scans, c->st_copy)); c->scans_pending = true; }
+    upload_points_async(c, sets, scans, Q, stride, mem);
   });
 }
 
@@ -887,17 +921,7 @@ int glio_window_set_scan(glio_ctx* c, int slot, const float* scan, int64_t Q, in
   return guarded(c, [&] {
     GLIO_REQUIRE(scan != nullptr && Q > 0, GLIO_ERR_ARG, "null or empty point array");
     GLIO_REQUIRE(stride >= 3 && stride <= 64, GLIO_ERR_ARG, "stride_floats must be in [3,64]");
-    Slot& sl = c->slot(slot);
-    if (mem == GLIO_DEVICE) sl.scan_ptr = scan;
-    else {
-      GLIO_CUDA_TRY(cudaEventRecord(c->ev_main, c->st));
-      GLIO_CUDA_TRY(cudaStreamWaitEvent(c->st_copy, c->ev_main, 0));
-      sl.scan.reserve((size_t)Q * stride);
-      GLIO_CUDA_TRY(cudaMemcpyAsync(sl.scan.p, scan, (size_t)Q * stride * sizeof(float), cudaMemcpyHostToDevice, c->st_copy));
-      sl.scan_ptr = sl.scan.p;
-      GLIO_CUDA_TRY(cudaEventRecord(c->ev_scans, c->st_copy)); c->scans_pending = true;
-    }
-    sl.Q = Q; sl.stride = stride;
+    upload_points_async(c, {&c->slot(slot).scan}, &scan, &Q, stride, mem);
   });
 }
 
@@ -915,9 +939,9 @@ int glio_window_slide(glio_ctx* c, int W) {
     c->slots[W - 1] = std::move(first);                       // its buffers are reused by the next upload
     if (c->slots[W - 1]) {
       Slot& s = *c->slots[W - 1];
-      s.Q = 0; s.scan_ptr = nullptr; s.n_match = 0; s.n_sel = -1;
-      s.eQ = 0; s.escan_ptr = nullptr; s.n_edge = 0; s.e_has_src = false;   // the dropped keyframe's corners and edges leave with it
-      s.dbg_Q = 0; s.edbg_Q = 0;                                              // and its debug views
+      s.scan.clear(); s.n_match = 0; s.n_sel = -1;
+      s.corners.clear(); s.edges.clear();                 // the dropped keyframe's corners and edges leave with it
+      s.dbg.Q = 0; s.edge_dbg.Q = 0;                      // and its debug views
     }
     c->items_dirty = true; c->edge_items_dirty = true;
   });
@@ -929,17 +953,7 @@ int glio_window_set_edge_scan(glio_ctx* c, int slot, const float* xyz, int64_t Q
   return guarded(c, [&] {
     GLIO_REQUIRE(xyz != nullptr && Q > 0, GLIO_ERR_ARG, "null or empty point array");
     GLIO_REQUIRE(stride >= 3 && stride <= 64, GLIO_ERR_ARG, "stride_floats must be in [3,64]");
-    Slot& sl = c->slot(slot);
-    if (mem == GLIO_DEVICE) sl.escan_ptr = xyz;
-    else {
-      GLIO_CUDA_TRY(cudaEventRecord(c->ev_main, c->st));
-      GLIO_CUDA_TRY(cudaStreamWaitEvent(c->st_copy, c->ev_main, 0));
-      sl.escan.reserve((size_t)Q * stride);
-      GLIO_CUDA_TRY(cudaMemcpyAsync(sl.escan.p, xyz, (size_t)Q * stride * sizeof(float), cudaMemcpyHostToDevice, c->st_copy));
-      sl.escan_ptr = sl.escan.p;
-      GLIO_CUDA_TRY(cudaEventRecord(c->ev_scans, c->st_copy)); c->scans_pending = true;
-    }
-    sl.eQ = Q; sl.estride = stride;
+    upload_points_async(c, {&c->slot(slot).corners}, &xyz, &Q, stride, mem);
   });
 }
 
@@ -961,6 +975,31 @@ glio_edge_options edge_options_or_default(const glio_edge_options* options) {
   return o;
 }
 
+// K1e / K1be over planned segments: ensure_work, one search + line-fit launch against `grid` (pair mode when oth_local is set),
+// compaction of every segment's valid records into dst[segment] and one host synchronisation; c->h_counts then holds the
+// per-segment edge counts.  dbg (window mode, keep_debug): each segment's debug views, captured from the work space.
+void edge_assoc_launch(glio_ctx* c, const GridBuild& grid, const std::vector<SegDesc>& segs, const std::vector<EdgeDst>& dst, int64_t Qt,
+                       const glio_edge_options& o, const float* oth_local, int oth_stride, const std::vector<AssocDebug*>* dbg) {
+  const int nseg = (int)segs.size();
+  const bool keep_debug = dbg != nullptr;
+  ensure_work(c, Qt, false, keep_debug);
+  c->w_pa.reserve((size_t)Qt); c->w_pb.reserve((size_t)Qt);
+  if (keep_debug) c->w_eig.reserve((size_t)Qt * 3);
+  c->d_segs.reserve(nseg); c->d_edst.reserve(nseg); c->d_counts.reserve(nseg); c->h_counts.reserve(nseg);
+  GLIO_CUDA_TRY(cudaMemcpyAsync(c->d_segs.p, segs.data(), nseg * sizeof(SegDesc), cudaMemcpyHostToDevice, c->st));
+  GLIO_CUDA_TRY(cudaMemcpyAsync(c->d_edst.p, dst.data(), nseg * sizeof(EdgeDst), cudaMemcpyHostToDevice, c->st));
+  AssocWork w = make_work(c, Qt, false, keep_debug);
+  const EdgeFitParams ep{o.max_sqdist, o.min_ratio, o.half_length};
+  edge_assoc_run(grid, c->d_segs.p, nseg, w, ep, c->w_pa.p, c->w_pb.p, keep_debug ? c->w_eig.p : nullptr, oth_local, oth_stride, c->cell_count,
+                 c->cell_pos, c->scan_tmp, c->st, c->lc);
+  compact_count(w, c->d_segs.p, nseg, c->w_flags.p, c->w_pos.p, c->scan_tmp, c->d_counts.p, c->st, c->lc);
+  compact_edge_scatter(w, c->d_segs.p, c->w_pos.p, c->w_pa.p, c->w_pb.p, (float)o.score, c->d_edst.p, c->st, c->lc);
+  GLIO_CUDA_TRY(cudaMemcpyAsync(c->h_counts.p, c->d_counts.p, nseg * sizeof(int), cudaMemcpyDeviceToHost, c->st));
+  if (keep_debug)
+    for (int s = 0; s < nseg; ++s) capture_debug(c, *(*dbg)[s], w, c->w_eig.p, 3, segs[s].offset, segs[s].count);
+  GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
+}
+
 }  // namespace
 
 extern "C" {
@@ -969,38 +1008,28 @@ int glio_set_edge_map(glio_ctx* c, const float* xyz, int64_t M, int stride, int 
   if (!c) return GLIO_ERR_ARG;
   return guarded(c, [&] {
     GLIO_REQUIRE(M >= 5, GLIO_ERR_ARG, "corner map needs at least 5 points");
-    const float* d = stage_points(c, c->edge_map_stage, xyz, M, stride, mem);
-    grid_build(c->edge_map, d, stride, M, nullptr, nullptr, c->prm.cell_size, c->pts_per_cell, c->st, c->lc);
-    c->has_edge_map = true;
+    map_build(c, c->edge_map, stage_points(c, c->edge_map.stage, xyz, M, stride, mem), stride, M);
   });
 }
 
 int glio_edge_localmap_clear(glio_ctx* c) {
   if (!c) return GLIO_ERR_ARG;
-  return localmap_clear(c, c->elm);
+  return localmap_clear(c, c->edge_map);
 }
 
 int glio_edge_localmap_push(glio_ctx* c, int at_front, const float* cloud_xyz, int64_t n, int stride, int mem, const double t[3], const double q[4]) {
   if (!c) return GLIO_ERR_ARG;
-  return localmap_push(c, c->elm, c->elm_stage, at_front, cloud_xyz, n, stride, mem, t, q);
+  return localmap_push(c, c->edge_map, at_front, cloud_xyz, n, stride, mem, t, q);
 }
 
 int glio_edge_localmap_pop_front(glio_ctx* c) {
   if (!c) return GLIO_ERR_ARG;
-  return localmap_pop_front(c, c->elm);
+  return localmap_pop_front(c, c->edge_map);
 }
 
 int glio_edge_localmap_build(glio_ctx* c, float leaf, int64_t* n_map) {
   if (!c) return GLIO_ERR_ARG;
-  return guarded(c, [&] {
-    GLIO_REQUIRE(c->elm.n_points() >= 5, GLIO_ERR_STATE, "corner local map needs at least 5 points");
-    const float* pts = nullptr; int stride = 0; bool filtered = false;
-    const int64_t m = c->elm.build(leaf, &pts, &stride, &filtered, c->st, c->lc);
-    GLIO_REQUIRE(!filtered || m >= 5, GLIO_ERR_STATE, "down-sampled corner local map has fewer than 5 points");
-    grid_build(c->edge_map, pts, stride, m, nullptr, nullptr, c->prm.cell_size, c->pts_per_cell, c->st, c->lc);
-    c->has_edge_map = true;
-    if (n_map) *n_map = m;
-  });
+  return localmap_build(c, c->edge_map, "corner local map", leaf, n_map);
 }
 
 int glio_window_associate_edges(glio_ctx* c, int W, const double* poses_body, const glio_edge_options* options, int64_t* n_edge) {
@@ -1008,61 +1037,36 @@ int glio_window_associate_edges(glio_ctx* c, int W, const double* poses_body, co
   return guarded(c, [&] {
     GLIO_REQUIRE(W > 0 && W <= 4096 && poses_body, GLIO_ERR_ARG, "bad window arguments");
     const glio_edge_options o = edge_options_or_default(options);
-    GLIO_REQUIRE(c->has_edge_map, GLIO_ERR_STATE, "glio_set_edge_map must be called before edge association");
+    GLIO_REQUIRE(c->edge_map.valid, GLIO_ERR_STATE, "glio_set_edge_map must be called before edge association");
     for (int k = 0; k < W; ++k)
-      GLIO_REQUIRE((size_t)k < c->slots.size() && c->slots[k] && c->slots[k]->eQ > 0 && c->slots[k]->escan_ptr, GLIO_ERR_STATE, "slot has no corner scan");
+      GLIO_REQUIRE((size_t)k < c->slots.size() && c->slots[k] && c->slots[k]->corners.n > 0 && c->slots[k]->corners.ptr, GLIO_ERR_STATE,
+                   "slot has no corner scan");
     if (c->scans_pending) { GLIO_CUDA_TRY(cudaStreamWaitEvent(c->st, c->ev_scans, 0)); c->scans_pending = false; }
-    const bool keep_debug = c->prm.keep_debug != 0;
     std::vector<SegDesc> segs(W);
-    std::vector<EdgeDst> dst(W);
     int64_t Qt = 0;
     for (int k = 0; k < W; ++k) {
-      Slot& sl = *c->slots[k];
-      segs[k].src = sl.escan_ptr; segs[k].stride = sl.estride; segs[k].count = sl.eQ; segs[k].offset = Qt;
-      lidar_pose_in_map(c->prm.q_lb, c->prm.t_lb, poses_body + 7 * k, segs[k].t, segs[k].q);   // Estimator.cpp:2216-2217
-      Qt += sl.eQ;
+      double lp[7];
+      lidar_pose_in_map(c->prm.q_lb, c->prm.t_lb, poses_body + 7 * k, lp, lp + 3);   // Estimator.cpp:2216-2217
+      segs[k] = make_seg(c->slots[k]->corners, Qt, lp);
+      Qt += c->slots[k]->corners.n;
     }
     GLIO_REQUIRE(Qt < ((int64_t)1 << 31), GLIO_ERR_ARG, "glio_window_associate_edges: too many corner points in one window");
-    ensure_work(c, Qt, false, keep_debug);
-    c->w_pa.reserve((size_t)Qt); c->w_pb.reserve((size_t)Qt);
-    if (keep_debug) c->w_eig.reserve((size_t)Qt * 3);
-    c->d_segs.reserve(W); c->d_edst.reserve(W); c->d_counts.reserve(W); c->h_counts.reserve(W);
-    // the slots' edge lists are replaced from here on: a reserve may drop their old contents, so they count as empty until the
-    // counts arrive (an error below leaves them empty, never pointing at memory that does not hold them)
+    // the slots' edge lists are replaced from here on: they count as empty until the counts arrive (an error below leaves them
+    // empty, never pointing at memory that does not hold them)
     c->edge_items_dirty = true;
+    std::vector<EdgeDst> dst(W);
+    std::vector<AssocDebug*> dbg(W);
     for (int k = 0; k < W; ++k) {
       Slot& sl = *c->slots[k];
-      sl.n_edge = 0; sl.e_has_src = false;
-      sl.e_cps.reserve((size_t)sl.eQ); sl.e_pa.reserve((size_t)sl.eQ); sl.e_pb.reserve((size_t)sl.eQ); sl.e_src.reserve((size_t)sl.eQ);
-      dst[k].cps = sl.e_cps.p; dst[k].pa = sl.e_pa.p; dst[k].pb = sl.e_pb.p; dst[k].src = sl.e_src.p;
+      sl.edges.clear();
+      dst[k] = sl.edges.reserve(sl.corners.n);
+      dbg[k] = &sl.edge_dbg;
     }
-    GLIO_CUDA_TRY(cudaMemcpyAsync(c->d_segs.p, segs.data(), W * sizeof(SegDesc), cudaMemcpyHostToDevice, c->st));
-    GLIO_CUDA_TRY(cudaMemcpyAsync(c->d_edst.p, dst.data(), W * sizeof(EdgeDst), cudaMemcpyHostToDevice, c->st));
-    AssocWork w = make_work(c, Qt, false, keep_debug);
-    const EdgeFitParams ep{o.max_sqdist, o.min_ratio, o.half_length};
-    edge_assoc_run(c->edge_map, c->d_segs.p, W, w, ep, c->w_pa.p, c->w_pb.p, keep_debug ? c->w_eig.p : nullptr, nullptr, 0, c->cell_count,
-                   c->cell_pos, c->scan_tmp, c->st, c->lc);
-    compact_count(w, c->d_segs.p, W, c->w_flags.p, c->w_pos.p, c->scan_tmp, c->d_counts.p, c->st, c->lc);
-    compact_edge_scatter(w, c->d_segs.p, c->w_pos.p, c->w_pa.p, c->w_pb.p, (float)o.score, c->d_edst.p, c->st, c->lc);
-    GLIO_CUDA_TRY(cudaMemcpyAsync(c->h_counts.p, c->d_counts.p, W * sizeof(int), cudaMemcpyDeviceToHost, c->st));
-    if (keep_debug) {
-      for (int k = 0; k < W; ++k) {
-        Slot& sl = *c->slots[k];
-        const int64_t off = segs[k].offset, q = sl.eQ;
-        sl.edbg_status.reserve(q); sl.edbg_idx5.reserve(5 * q); sl.edbg_sqd5.reserve(5 * q); sl.edbg_pm.reserve(q); sl.edbg_eig.reserve(3 * q);
-        GLIO_CUDA_TRY(cudaMemcpyAsync(sl.edbg_status.p, w.status + off, q, cudaMemcpyDeviceToDevice, c->st));
-        GLIO_CUDA_TRY(cudaMemcpyAsync(sl.edbg_idx5.p, w.idx5 + 5 * off, 5 * q * sizeof(int32_t), cudaMemcpyDeviceToDevice, c->st));
-        GLIO_CUDA_TRY(cudaMemcpyAsync(sl.edbg_sqd5.p, w.sqd5 + 5 * off, 5 * q * sizeof(float), cudaMemcpyDeviceToDevice, c->st));
-        GLIO_CUDA_TRY(cudaMemcpyAsync(sl.edbg_pm.p, w.pm + off, q * sizeof(float4), cudaMemcpyDeviceToDevice, c->st));
-        GLIO_CUDA_TRY(cudaMemcpyAsync(sl.edbg_eig.p, c->w_eig.p + 3 * off, 3 * q * sizeof(double), cudaMemcpyDeviceToDevice, c->st));
-        sl.edbg_Q = q;
-      }
-    }
-    GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
+    edge_assoc_launch(c, c->edge_map.grid, segs, dst, Qt, o, nullptr, 0, c->prm.keep_debug ? &dbg : nullptr);
     for (int k = 0; k < W; ++k) {
-      Slot& sl = *c->slots[k];
-      sl.n_edge = c->h_counts.p[k]; sl.e_has_src = true;
-      if (n_edge) n_edge[k] = sl.n_edge;
+      EdgeList& e = c->slots[k]->edges;
+      e.n = c->h_counts.p[k]; e.has_src = true;
+      if (n_edge) n_edge[k] = e.n;
     }
   });
 }
@@ -1072,30 +1076,29 @@ int glio_window_associate_edges(glio_ctx* c, int W, const double* poses_body, co
 namespace {
 
 // copy-out of an edge list (glio_get_edges / glio_batch_get_edges): all arrays NULL only counts
-void copy_edges_out(glio_ctx* c, int64_t n, const float4* d_cps, const float4* d_pa, const float4* d_pb, const int32_t* d_src, bool has_src,
-                    int64_t capacity, float* cp, float* pa, float* pb, double* s, int32_t* src, int64_t* n_out) {
+void copy_edges_out(glio_ctx* c, const EdgeList& e, int64_t capacity, float* cp, float* pa, float* pb, double* s, int32_t* src, int64_t* n_out) {
+  const int64_t n = e.n;
   if (n_out) *n_out = n;
   if (!cp && !pa && !pb && !s && !src) return;             // a count query
   GLIO_REQUIRE(capacity >= n, GLIO_ERR_ARG, "capacity smaller than the edge count");
   if (n == 0) return;
   std::vector<float4> h0(n), h1(n), h2(n);
-  GLIO_CUDA_TRY(cudaMemcpyAsync(h0.data(), d_cps, n * sizeof(float4), cudaMemcpyDeviceToHost, c->st));
-  GLIO_CUDA_TRY(cudaMemcpyAsync(h1.data(), d_pa, n * sizeof(float4), cudaMemcpyDeviceToHost, c->st));
-  GLIO_CUDA_TRY(cudaMemcpyAsync(h2.data(), d_pb, n * sizeof(float4), cudaMemcpyDeviceToHost, c->st));
-  if (src && has_src) GLIO_CUDA_TRY(cudaMemcpyAsync(src, d_src, n * sizeof(int32_t), cudaMemcpyDeviceToHost, c->st));
+  GLIO_CUDA_TRY(cudaMemcpyAsync(h0.data(), e.cps.p, n * sizeof(float4), cudaMemcpyDeviceToHost, c->st));
+  GLIO_CUDA_TRY(cudaMemcpyAsync(h1.data(), e.pa.p, n * sizeof(float4), cudaMemcpyDeviceToHost, c->st));
+  GLIO_CUDA_TRY(cudaMemcpyAsync(h2.data(), e.pb.p, n * sizeof(float4), cudaMemcpyDeviceToHost, c->st));
+  if (src && e.has_src) GLIO_CUDA_TRY(cudaMemcpyAsync(src, e.src.p, n * sizeof(int32_t), cudaMemcpyDeviceToHost, c->st));
   GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
+  unpack_float4(h0.data(), n, cp);
+  unpack_float4(h1.data(), n, pa);
+  unpack_float4(h2.data(), n, pb);
   for (int64_t i = 0; i < n; ++i) {
-    if (cp) { cp[3 * i] = h0[i].x; cp[3 * i + 1] = h0[i].y; cp[3 * i + 2] = h0[i].z; }
-    if (pa) { pa[3 * i] = h1[i].x; pa[3 * i + 1] = h1[i].y; pa[3 * i + 2] = h1[i].z; }
-    if (pb) { pb[3 * i] = h2[i].x; pb[3 * i + 1] = h2[i].y; pb[3 * i + 2] = h2[i].z; }
     if (s) s[i] = (double)h0[i].w;
-    if (src && !has_src) src[i] = -1;
+    if (src && !e.has_src) src[i] = -1;
   }
 }
 
 // upload of an edge list (glio_set_edges / glio_batch_set_pair_edges): (cp, s) / pa / pb as float4, n > 0
-void upload_edges(glio_ctx* c, int64_t n, const float* cp, const float* pa, const float* pb, const double* s, DevBuf<float4>& d_cps,
-                  DevBuf<float4>& d_pa, DevBuf<float4>& d_pb) {
+void upload_edges(glio_ctx* c, EdgeList& e, int64_t n, const float* cp, const float* pa, const float* pb, const double* s) {
   GLIO_REQUIRE(cp && pa && pb && s, GLIO_ERR_ARG, "null edge arrays");
   std::vector<float4> h0(n), h1(n), h2(n);
   for (int64_t i = 0; i < n; ++i) {
@@ -1103,11 +1106,30 @@ void upload_edges(glio_ctx* c, int64_t n, const float* cp, const float* pa, cons
     h1[i] = make_float4(pa[3 * i], pa[3 * i + 1], pa[3 * i + 2], 0.f);
     h2[i] = make_float4(pb[3 * i], pb[3 * i + 1], pb[3 * i + 2], 0.f);
   }
-  d_cps.reserve(n); d_pa.reserve(n); d_pb.reserve(n);
-  GLIO_CUDA_TRY(cudaMemcpyAsync(d_cps.p, h0.data(), n * sizeof(float4), cudaMemcpyHostToDevice, c->st));
-  GLIO_CUDA_TRY(cudaMemcpyAsync(d_pa.p, h1.data(), n * sizeof(float4), cudaMemcpyHostToDevice, c->st));
-  GLIO_CUDA_TRY(cudaMemcpyAsync(d_pb.p, h2.data(), n * sizeof(float4), cudaMemcpyHostToDevice, c->st));
+  e.cps.reserve(n); e.pa.reserve(n); e.pb.reserve(n);
+  GLIO_CUDA_TRY(cudaMemcpyAsync(e.cps.p, h0.data(), n * sizeof(float4), cudaMemcpyHostToDevice, c->st));
+  GLIO_CUDA_TRY(cudaMemcpyAsync(e.pa.p, h1.data(), n * sizeof(float4), cudaMemcpyHostToDevice, c->st));
+  GLIO_CUDA_TRY(cudaMemcpyAsync(e.pb.p, h2.data(), n * sizeof(float4), cudaMemcpyHostToDevice, c->st));
   GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
+}
+
+// glio_get_assoc_debug / glio_get_edge_debug: a slot's views of its last plane (nfit = 4) or edge (nfit = 3) association
+int read_assoc_debug(glio_ctx* c, int slot, AssocDebug Slot::*view, int nfit, const char* q_mismatch, int64_t Q, uint8_t* status, int32_t* idx5,
+                     float* sqd5, float* pm, double* fit) {
+  if (!c) return GLIO_ERR_ARG;
+  return guarded(c, [&] {
+    GLIO_REQUIRE(c->prm.keep_debug, GLIO_ERR_STATE, "context was created without keep_debug");
+    const AssocDebug& d = c->slot(slot).*view;
+    GLIO_REQUIRE(d.Q == Q && Q > 0, GLIO_ERR_ARG, q_mismatch);
+    if (status) GLIO_CUDA_TRY(cudaMemcpyAsync(status, d.status.p, Q, cudaMemcpyDeviceToHost, c->st));
+    if (idx5) GLIO_CUDA_TRY(cudaMemcpyAsync(idx5, d.idx5.p, 5 * Q * sizeof(int32_t), cudaMemcpyDeviceToHost, c->st));
+    if (sqd5) GLIO_CUDA_TRY(cudaMemcpyAsync(sqd5, d.sqd5.p, 5 * Q * sizeof(float), cudaMemcpyDeviceToHost, c->st));
+    if (fit) GLIO_CUDA_TRY(cudaMemcpyAsync(fit, d.fit.p, nfit * Q * sizeof(double), cudaMemcpyDeviceToHost, c->st));
+    std::vector<float4> h;
+    if (pm) { h.resize(Q); GLIO_CUDA_TRY(cudaMemcpyAsync(h.data(), d.pm.p, Q * sizeof(float4), cudaMemcpyDeviceToHost, c->st)); }
+    GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
+    if (pm) unpack_float4(h.data(), Q, pm);
+  });
 }
 
 }  // namespace
@@ -1117,26 +1139,12 @@ extern "C" {
 int glio_get_edges(glio_ctx* c, int slot, int64_t capacity, float* cp, float* pa, float* pb, double* s, int32_t* src, int64_t* n_out) {
   if (!c) return GLIO_ERR_ARG;
   return guarded(c, [&] {
-    Slot& sl = c->slot(slot);
-    copy_edges_out(c, sl.n_edge, sl.e_cps.p, sl.e_pa.p, sl.e_pb.p, sl.e_src.p, sl.e_has_src, capacity, cp, pa, pb, s, src, n_out);
+    copy_edges_out(c, c->slot(slot).edges, capacity, cp, pa, pb, s, src, n_out);
   });
 }
 
 int glio_get_edge_debug(glio_ctx* c, int slot, int64_t Q, uint8_t* status, int32_t* idx5, float* sqd5, float* pm, double* eig) {
-  if (!c) return GLIO_ERR_ARG;
-  return guarded(c, [&] {
-    GLIO_REQUIRE(c->prm.keep_debug, GLIO_ERR_STATE, "context was created without keep_debug");
-    Slot& sl = c->slot(slot);
-    GLIO_REQUIRE(sl.edbg_Q == Q && Q > 0, GLIO_ERR_ARG, "Q does not match the slot's last edge association");
-    if (status) GLIO_CUDA_TRY(cudaMemcpyAsync(status, sl.edbg_status.p, Q, cudaMemcpyDeviceToHost, c->st));
-    if (idx5) GLIO_CUDA_TRY(cudaMemcpyAsync(idx5, sl.edbg_idx5.p, 5 * Q * sizeof(int32_t), cudaMemcpyDeviceToHost, c->st));
-    if (sqd5) GLIO_CUDA_TRY(cudaMemcpyAsync(sqd5, sl.edbg_sqd5.p, 5 * Q * sizeof(float), cudaMemcpyDeviceToHost, c->st));
-    if (eig) GLIO_CUDA_TRY(cudaMemcpyAsync(eig, sl.edbg_eig.p, 3 * Q * sizeof(double), cudaMemcpyDeviceToHost, c->st));
-    std::vector<float4> h;
-    if (pm) { h.resize(Q); GLIO_CUDA_TRY(cudaMemcpyAsync(h.data(), sl.edbg_pm.p, Q * sizeof(float4), cudaMemcpyDeviceToHost, c->st)); }
-    GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
-    if (pm) for (int64_t i = 0; i < Q; ++i) { pm[3 * i] = h[i].x; pm[3 * i + 1] = h[i].y; pm[3 * i + 2] = h[i].z; }
-  });
+  return read_assoc_debug(c, slot, &Slot::edge_dbg, 3, "Q does not match the slot's last edge association", Q, status, idx5, sqd5, pm, eig);
 }
 
 int glio_window_associate(glio_ctx* c, int W, const double* poses_body, int64_t* n_match) {
@@ -1165,10 +1173,7 @@ int glio_get_matches(glio_ctx* c, int slot, int64_t capacity, float* cp, float* 
     if (cp || weight) {
       GLIO_CUDA_TRY(cudaMemcpyAsync(h.data(), sl.m_cpw.p, n * sizeof(float4), cudaMemcpyDeviceToHost, c->st));
       GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
-      for (int64_t i = 0; i < n; ++i) {
-        if (cp) { cp[3 * i] = h[i].x; cp[3 * i + 1] = h[i].y; cp[3 * i + 2] = h[i].z; }
-        if (weight) weight[i] = h[i].w;
-      }
+      unpack_float4(h.data(), n, cp, weight);
     }
     if (nsd) {
       GLIO_CUDA_TRY(cudaMemcpyAsync(nsd, sl.m_nsd.p, n * sizeof(float4), cudaMemcpyDeviceToHost, c->st));
@@ -1182,20 +1187,7 @@ int glio_get_matches(glio_ctx* c, int slot, int64_t capacity, float* cp, float* 
 }
 
 int glio_get_assoc_debug(glio_ctx* c, int slot, int64_t Q, uint8_t* status, int32_t* idx5, float* sqd5, float* pm, double* plane) {
-  if (!c) return GLIO_ERR_ARG;
-  return guarded(c, [&] {
-    GLIO_REQUIRE(c->prm.keep_debug, GLIO_ERR_STATE, "context was created without keep_debug");
-    Slot& sl = c->slot(slot);
-    GLIO_REQUIRE(sl.dbg_Q == Q && Q > 0, GLIO_ERR_ARG, "Q does not match the slot's last association");
-    if (status) GLIO_CUDA_TRY(cudaMemcpyAsync(status, sl.dbg_status.p, Q, cudaMemcpyDeviceToHost, c->st));
-    if (idx5) GLIO_CUDA_TRY(cudaMemcpyAsync(idx5, sl.dbg_idx5.p, 5 * Q * sizeof(int32_t), cudaMemcpyDeviceToHost, c->st));
-    if (sqd5) GLIO_CUDA_TRY(cudaMemcpyAsync(sqd5, sl.dbg_sqd5.p, 5 * Q * sizeof(float), cudaMemcpyDeviceToHost, c->st));
-    if (plane) GLIO_CUDA_TRY(cudaMemcpyAsync(plane, sl.dbg_plane.p, 4 * Q * sizeof(double), cudaMemcpyDeviceToHost, c->st));
-    std::vector<float4> h;
-    if (pm) { h.resize(Q); GLIO_CUDA_TRY(cudaMemcpyAsync(h.data(), sl.dbg_pm.p, Q * sizeof(float4), cudaMemcpyDeviceToHost, c->st)); }
-    GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
-    if (pm) for (int64_t i = 0; i < Q; ++i) { pm[3 * i] = h[i].x; pm[3 * i + 1] = h[i].y; pm[3 * i + 2] = h[i].z; }
-  });
+  return read_assoc_debug(c, slot, &Slot::dbg, 4, "Q does not match the slot's last association", Q, status, idx5, sqd5, pm, plane);
 }
 
 int glio_select(glio_ctx* c, int slot, const int32_t* keep, int64_t n) {
@@ -1226,15 +1218,7 @@ int glio_eval_unary(glio_ctx* c, int W, const double* poses_body, int jac_kind, 
     GLIO_REQUIRE(jac_kind == 0 || jac_kind == 1, GLIO_ERR_ARG, "jac_kind must be 0 or 1");
     const bool want_jac = (H != nullptr) || (g != nullptr);
     eval_unary_blocks(c, W, poses_body, jac_kind, want_jac);
-    for (int k = 0; k < W; ++k) {
-      const double* o = c->h_out.p + (size_t)k * GLIO_NACC;
-      if (H) {
-        int idx = 0;
-        for (int p = 0; p < 6; ++p) for (int q = p; q < 6; ++q) { H[36 * k + 6 * p + q] = o[idx]; H[36 * k + 6 * q + p] = o[idx]; ++idx; }
-      }
-      if (g) for (int p = 0; p < 6; ++p) g[6 * k + p] = o[21 + p];
-      if (cost) cost[k] = o[27];
-    }
+    unpack_blocks(c->h_out.p, W, H, g, cost);
   });
 }
 
@@ -1548,31 +1532,58 @@ static SolverOptions solver_options_from(const glio_solver_options& o) {
   return so;
 }
 
+// W keyframes as the minimizer sees them: t (3), q (4, tangent 3) and, with speed-bias, 9 more per keyframe.  The ambient
+// state holds them in that order, na doubles per keyframe; the tangent has nt per keyframe.
+struct StateLayout {
+  int W; bool sb; int nt, na;
+  StateLayout(int W_, bool sb_) : W(W_), sb(sb_), nt(sb_ ? 15 : 6), na(sb_ ? 16 : 7) {}
+  std::vector<ParamBlock> blocks() const {
+    std::vector<ParamBlock> b;
+    for (int k = 0; k < W; ++k) {
+      b.push_back(ParamBlock{na * k, 3, nt * k, 3, false, nullptr});
+      b.push_back(ParamBlock{na * k + 3, 4, nt * k + 3, 3, true, nullptr});
+      if (sb) b.push_back(ParamBlock{na * k + 7, 9, nt * k + 6, 9, false, nullptr});
+    }
+    return b;
+  }
+  // poses (W x 7) and, with speed-bias, speed_bias (W x 9) into the ambient state x
+  void pack(const double* poses, const double* speed_bias, double* x) const {
+    for (int k = 0; k < W; ++k) {
+      for (int i = 0; i < 7; ++i) x[(size_t)na * k + i] = poses[7 * k + i];
+      if (sb) for (int i = 0; i < 9; ++i) x[(size_t)na * k + 7 + i] = speed_bias[9 * k + i];
+    }
+  }
+  void unpack(const double* x, double* poses, double* speed_bias) const {
+    for (int k = 0; k < W; ++k) {
+      for (int i = 0; i < 7; ++i) poses[7 * k + i] = x[(size_t)na * k + i];
+      if (sb) for (int i = 0; i < 9; ++i) speed_bias[9 * k + i] = x[(size_t)na * k + 7 + i];
+    }
+  }
+};
+
+// each keyframe's 21 upper-triangular H entries of the W x 28 layout onto the band's diagonal blocks, nt columns per keyframe
+static void add_diag_blocks(BandMat* H, const double* o28, int W, int nt) {
+  for (int k = 0; k < W; ++k) {
+    const double* ob = o28 + (size_t)k * GLIO_NACC;
+    int idx = 0;
+    for (int p = 0; p < 6; ++p) for (int q = p; q < 6; ++q) { H->at(nt * k + q, nt * k + p) += ob[idx]; ++idx; }
+  }
+}
+
 // The minimizer over W poses (and speed-bias states) with the LiDAR blocks of `tgt` (nullptr: the context's slots and glio_params)
 // plus the host factors.  Throws on error; poses / speed_bias are in/out.
 static void solve_core(glio_ctx* c, int W, double* poses, double* speed_bias, glio_host_factors_fn host_factors, glio_host_factors_band_fn host_band,
                        int hb_hint, void* user, const SolverOptions& so, const EvalTarget* tgt, SolverSummary& S) {
     const bool sb = speed_bias != nullptr;
-    const int nt = sb ? 15 : 6, na = sb ? 16 : 7, n = W * nt;
-    std::vector<ParamBlock> blocks;
-    for (int k = 0; k < W; ++k) {
-      blocks.push_back(ParamBlock{na * k, 3, nt * k, 3, false, nullptr});
-      blocks.push_back(ParamBlock{na * k + 3, 4, nt * k + 3, 3, true, nullptr});
-      if (sb) blocks.push_back(ParamBlock{na * k + 7, 9, nt * k + 6, 9, false, nullptr});
-    }
-    TrustRegionDogleg solver(blocks, so);
-    std::vector<double> x((size_t)W * na), pz((size_t)W * 7), sz((size_t)W * 9);
-    for (int k = 0; k < W; ++k) {
-      for (int i = 0; i < 7; ++i) x[(size_t)na * k + i] = poses[7 * k + i];
-      if (sb) for (int i = 0; i < 9; ++i) x[(size_t)na * k + 7 + i] = speed_bias[9 * k + i];
-    }
+    const StateLayout L(W, sb);
+    const int nt = L.nt, n = W * nt;
+    TrustRegionDogleg solver(L.blocks(), so);
+    std::vector<double> x((size_t)W * L.na), pz((size_t)W * 7), sz((size_t)W * 9);
+    L.pack(poses, speed_bias, x.data());
     std::vector<double> Hd;       // dense scratch for the host callback's n x n interface
     int hb_fixed = -1;
     EvalFn eval = [&](const double* xa, bool want_jac, double* cost, BandMat* H, double* g) -> bool {
-      for (int k = 0; k < W; ++k) {
-        for (int i = 0; i < 7; ++i) pz[7 * k + i] = xa[(size_t)na * k + i];
-        if (sb) for (int i = 0; i < 9; ++i) sz[9 * k + i] = xa[(size_t)na * k + 7 + i];
-      }
+      L.unpack(xa, pz.data(), sz.data());
       // the device evaluates the LiDAR residuals while the host evaluates its own factors
       const unsigned int epoch = eval_unary_launch(c, W, pz.data(), 0, want_jac, tgt, true);
       double ct = 0;
@@ -1588,11 +1599,7 @@ static void solve_core(glio_ctx* c, int W, double* poses, double* speed_bias, gl
         const int hrc = host_band(user, W, pz.data(), sb ? sz.data() : nullptr, want_jac ? 1 : 0, want_jac ? H->a.data() : nullptr, want_jac ? H->hb : 0, g, &ct);
         add_device();
         if (hrc != 0) return false;
-        if (want_jac) for (int k = 0; k < W; ++k) {
-          const double* ob = c->h_out.p + (size_t)k * GLIO_NACC;
-          int idx = 0;
-          for (int p = 0; p < 6; ++p) for (int q = p; q < 6; ++q) { H->at(nt * k + q, nt * k + p) += ob[idx]; ++idx; }
-        }
+        if (want_jac) add_diag_blocks(H, c->h_out.p, W, nt);
         *cost = ct;
         return std::isfinite(ct);
       }
@@ -1614,20 +1621,13 @@ static void solve_core(glio_ctx* c, int W, double* poses, double* speed_bias, gl
         H->reset(n, hb_fixed);
         const int hb = H->hb;
         if (host_factors) for (int i = 0; i < n; ++i) for (int j = std::max(0, i - hb); j <= i; ++j) H->at(i, j) = Hd[(size_t)i * n + j];
-        for (int k = 0; k < W; ++k) {
-          const double* ob = c->h_out.p + (size_t)k * GLIO_NACC;
-          int idx = 0;
-          for (int p = 0; p < 6; ++p) for (int q = p; q < 6; ++q) { H->at(nt * k + q, nt * k + p) += ob[idx]; ++idx; }
-        }
+        add_diag_blocks(H, c->h_out.p, W, nt);
       }
       *cost = ct;
       return std::isfinite(ct);
     };
     solver.solve(x.data(), eval, &S);
-    for (int k = 0; k < W; ++k) {
-      for (int i = 0; i < 7; ++i) poses[7 * k + i] = x[(size_t)na * k + i];
-      if (sb) for (int i = 0; i < 9; ++i) speed_bias[9 * k + i] = x[(size_t)na * k + 7 + i];
-    }
+    L.unpack(x.data(), poses, speed_bias);
 }
 
 static int window_solve_impl(glio_ctx* c, int W, double* poses, double* speed_bias, glio_host_factors_fn host_factors,
@@ -1686,8 +1686,6 @@ int glio_batch_clear(glio_ctx* c) {
   if (!c) return GLIO_ERR_ARG;
   return guarded(c, [&] {
     GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
-    for (auto& f : c->frames) f.second->release();
-    for (auto& p : c->pairs) p->release();
     c->frames.clear(); c->pairs.clear(); c->pair_index.clear(); c->bin_dirty = true; c->bedge_dirty = true;
   });
 }
@@ -1698,10 +1696,8 @@ int glio_batch_set_frame(glio_ctx* c, int frame, const float* scan_xyz, int64_t 
     GLIO_REQUIRE(frame >= 0 && pose, GLIO_ERR_ARG, "bad frame arguments");
     auto& fp = c->frames[frame];
     if (!fp) fp.reset(new glio_ctx::Frame());
-    glio_ctx::Frame& f = *fp;
-    f.scan_ptr = stage_points(c, f.scan, scan_xyz, Q, stride, mem);
-    f.Q = Q; f.stride = stride; f.grid_valid = false; f.egrid_valid = false;
-    for (int i = 0; i < 7; ++i) f.pose[i] = pose[i];
+    stage_points(c, fp->surf.pts, scan_xyz, Q, stride, mem);
+    fp->set_pose(pose);
   });
 }
 
@@ -1711,57 +1707,87 @@ int glio_batch_set_pose(glio_ctx* c, int frame, const double pose[7]) {
   return guarded(c, [&] {
     auto it = c->frames.find(frame);
     GLIO_REQUIRE(it != c->frames.end() && pose, GLIO_ERR_ARG, "unknown frame");
-    for (int i = 0; i < 7; ++i) it->second->pose[i] = pose[i];
-    it->second->grid_valid = false; it->second->egrid_valid = false;
+    it->second->set_pose(pose);
   });
 }
+
+}  // extern "C"
+
+namespace {
+
+// the listed pairs grouped by searched frame (one grid, one launch per group), each group in list order; every pair must join
+// two distinct known frames
+std::map<int, std::vector<int64_t>> pairs_by_searched_frame(glio_ctx* c, const int32_t* pairs_cur, const int32_t* pairs_oth, int64_t n_pairs) {
+  std::map<int, std::vector<int64_t>> by_oth;
+  for (int64_t i = 0; i < n_pairs; ++i) {
+    GLIO_REQUIRE(c->frames.count(pairs_cur[i]) && c->frames.count(pairs_oth[i]) && pairs_cur[i] != pairs_oth[i], GLIO_ERR_ARG,
+                 "pair references an unknown frame");
+    by_oth[pairs_oth[i]].push_back(i);
+  }
+  return by_oth;
+}
+
+// the grid of a searched frame's world cloud (body pose applied directly to the stored points, quirk Q7), built when stale
+const GridBuild& searched_grid(glio_ctx* c, const glio_ctx::Frame& f, glio_ctx::FrameCloud& fc) {
+  if (!fc.grid_valid) {
+    grid_build(fc.grid, fc.pts.ptr, fc.pts.stride, fc.pts.n, f.pose, f.pose + 3, c->prm.cell_size, c->pts_per_cell, c->st, c->lc);
+    fc.grid_valid = true;
+  }
+  return fc.grid;
+}
+
+// the pair (cur, oth) of the pair list, appended with no matches and no edges when it is not there yet
+glio_ctx::Pair& pair_entry(glio_ctx* c, int cur, int oth) {
+  const std::pair<int, int> key(cur, oth);
+  auto it = c->pair_index.find(key);
+  if (it != c->pair_index.end()) return *c->pairs[it->second];
+  c->pair_index[key] = (int)c->pairs.size();
+  c->pairs.emplace_back(new glio_ctx::Pair());
+  c->pairs.back()->cur = cur; c->pairs.back()->oth = oth;
+  c->bin_dirty = true;
+  return *c->pairs.back();
+}
+
+// the pair (cur, oth) of the pair list; GLIO_ERR_ARG when it is not there
+glio_ctx::Pair& find_pair(glio_ctx* c, int cur, int oth) {
+  auto it = c->pair_index.find(std::make_pair(cur, oth));
+  GLIO_REQUIRE(it != c->pair_index.end(), GLIO_ERR_ARG, "pair is not on the pair list");
+  return *c->pairs[it->second];
+}
+
+}  // namespace
+
+extern "C" {
 
 int glio_batch_associate_pairs(glio_ctx* c, const int32_t* pairs_cur, const int32_t* pairs_oth, int64_t n_pairs, int64_t* n_match) {
   if (!c) return GLIO_ERR_ARG;
   return guarded(c, [&] {
     GLIO_REQUIRE(n_pairs > 0 && pairs_cur && pairs_oth, GLIO_ERR_ARG, "bad pair list");
-    // group the requested pairs by the searched frame: one grid, one launch per group
-    std::map<int, std::vector<int64_t>> by_oth;
-    for (int64_t i = 0; i < n_pairs; ++i) {
-      GLIO_REQUIRE(c->frames.count(pairs_cur[i]) && c->frames.count(pairs_oth[i]) && pairs_cur[i] != pairs_oth[i], GLIO_ERR_ARG, "pair references an unknown frame");
-      by_oth[pairs_oth[i]].push_back(i);
-    }
     AssocGates gates{c->prm.batch_max_radius, c->prm.batch_dist_thres, c->prm.weight_min};
-    for (auto& grp : by_oth) {
+    for (auto& grp : pairs_by_searched_frame(c, pairs_cur, pairs_oth, n_pairs)) {
       glio_ctx::Frame& fo = *c->frames[grp.first];
-      if (!fo.grid_valid) {
-        // world cloud of the searched frame (body pose applied directly to the stored points, quirk Q7) + its grid
-        grid_build(fo.grid, fo.scan_ptr, fo.stride, fo.Q, fo.pose, fo.pose + 3, c->prm.cell_size, c->pts_per_cell, c->st, c->lc);
-        fo.grid_valid = true;
-      }
+      const GridBuild& grid = searched_grid(c, fo, fo.surf);
       const int nseg = (int)grp.second.size();
       std::vector<SegDesc> segs(nseg);
       int64_t Qt = 0;
       for (int s = 0; s < nseg; ++s) {
-        glio_ctx::Frame& fc = *c->frames[pairs_cur[grp.second[s]]];
-        segs[s].src = fc.scan_ptr; segs[s].stride = fc.stride; segs[s].count = fc.Q; segs[s].offset = Qt;
-        for (int k = 0; k < 3; ++k) segs[s].t[k] = fc.pose[k];
-        for (int k = 0; k < 4; ++k) segs[s].q[k] = fc.pose[3 + k];
-        Qt += fc.Q;
+        const glio_ctx::Frame& fc = *c->frames[pairs_cur[grp.second[s]]];
+        segs[s] = make_seg(fc.surf.pts, Qt, fc.pose);
+        Qt += fc.surf.pts.n;
       }
       ensure_work(c, Qt, true, c->prm.keep_debug != 0);
       c->d_segs.reserve(nseg); c->d_dst.reserve(nseg); c->d_counts.reserve(nseg); c->h_counts.reserve(nseg);
       GLIO_CUDA_TRY(cudaMemcpyAsync(c->d_segs.p, segs.data(), nseg * sizeof(SegDesc), cudaMemcpyHostToDevice, c->st));
       AssocWork w = make_work(c, Qt, true, c->prm.keep_debug != 0);
-      assoc_run(fo.grid, c->d_segs.p, nseg, w, gates, fo.scan_ptr, fo.stride, c->cell_count, c->cell_pos, c->scan_tmp, c->st, c->lc);
+      assoc_run(grid, c->d_segs.p, nseg, w, gates, fo.surf.pts.ptr, fo.surf.pts.stride, c->cell_count, c->cell_pos, c->scan_tmp, c->st, c->lc);
       compact_count(w, c->d_segs.p, nseg, c->w_flags.p, c->w_pos.p, c->scan_tmp, c->d_counts.p, c->st, c->lc);
       GLIO_CUDA_TRY(cudaMemcpyAsync(c->h_counts.p, c->d_counts.p, nseg * sizeof(int), cudaMemcpyDeviceToHost, c->st));
       GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
       std::vector<CompactDst> dst(nseg);
       for (int s = 0; s < nseg; ++s) {
         const int64_t i = grp.second[s];
-        const std::pair<int, int> key(pairs_cur[i], pairs_oth[i]);
-        auto pit = c->pair_index.find(key);
-        int pi;
-        if (pit == c->pair_index.end()) { pi = (int)c->pairs.size(); c->pairs.emplace_back(new glio_ctx::Pair()); c->pair_index[key] = pi; }
-        else pi = pit->second;
-        glio_ctx::Pair& pr = *c->pairs[pi];
-        pr.cur = key.first; pr.oth = key.second; pr.n_match = c->h_counts.p[s]; pr.n_sel = -1;
+        glio_ctx::Pair& pr = pair_entry(c, pairs_cur[i], pairs_oth[i]);
+        pr.n_match = c->h_counts.p[s]; pr.n_sel = -1;
         const size_t nm = (size_t)std::max<int64_t>(pr.n_match, 1);
         pr.m_cpw.reserve(nm); pr.m_nc.reserve(6 * nm); pr.m_src.reserve(nm);
         dst[s].cpw = pr.m_cpw.p; dst[s].nsd = nullptr; dst[s].nc = pr.m_nc.p; dst[s].src = pr.m_src.p;
@@ -1794,9 +1820,7 @@ int glio_batch_pair_list(glio_ctx* c, int64_t capacity, int32_t* cur, int32_t* o
 int glio_batch_get_matches(glio_ctx* c, int cur, int oth, int64_t capacity, float* cp, float* weight, double* normal_cent, int32_t* src, int64_t* n_out) {
   if (!c) return GLIO_ERR_ARG;
   return guarded(c, [&] {
-    auto it = c->pair_index.find(std::make_pair(cur, oth));
-    GLIO_REQUIRE(it != c->pair_index.end(), GLIO_ERR_ARG, "pair was not associated");
-    glio_ctx::Pair& pr = *c->pairs[it->second];
+    glio_ctx::Pair& pr = find_pair(c, cur, oth);
     const int64_t n = pr.n_match;
     if (n_out) *n_out = n;
     GLIO_REQUIRE(capacity >= n, GLIO_ERR_ARG, "capacity smaller than the match count");
@@ -1806,19 +1830,14 @@ int glio_batch_get_matches(glio_ctx* c, int cur, int oth, int64_t capacity, floa
     if (normal_cent) GLIO_CUDA_TRY(cudaMemcpyAsync(normal_cent, pr.m_nc.p, 6 * n * sizeof(double), cudaMemcpyDeviceToHost, c->st));
     if (src) GLIO_CUDA_TRY(cudaMemcpyAsync(src, pr.m_src.p, n * sizeof(int32_t), cudaMemcpyDeviceToHost, c->st));
     GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
-    for (int64_t i = 0; i < n && !h.empty(); ++i) {
-      if (cp) { cp[3 * i] = h[i].x; cp[3 * i + 1] = h[i].y; cp[3 * i + 2] = h[i].z; }
-      if (weight) weight[i] = h[i].w;
-    }
+    if (!h.empty()) unpack_float4(h.data(), n, cp, weight);
   });
 }
 
 int glio_batch_select(glio_ctx* c, int cur, int oth, const int32_t* keep, int64_t n) {
   if (!c) return GLIO_ERR_ARG;
   return guarded(c, [&] {
-    auto it = c->pair_index.find(std::make_pair(cur, oth));
-    GLIO_REQUIRE(it != c->pair_index.end(), GLIO_ERR_ARG, "pair was not associated");
-    glio_ctx::Pair& pr = *c->pairs[it->second];
+    glio_ctx::Pair& pr = find_pair(c, cur, oth);
     c->bin_dirty = true;
     if (n < 0) { pr.n_sel = -1; return; }
     GLIO_REQUIRE(n == 0 || keep, GLIO_ERR_ARG, "null selection list");
@@ -1835,26 +1854,6 @@ int glio_batch_select(glio_ctx* c, int cur, int oth, const int32_t* keep, int64_
   });
 }
 
-}  // extern "C"
-
-namespace {
-
-// the pair (cur, oth) of the pair list, appended with no matches and no edges when it is not there yet
-glio_ctx::Pair& pair_entry(glio_ctx* c, int cur, int oth) {
-  const std::pair<int, int> key(cur, oth);
-  auto it = c->pair_index.find(key);
-  if (it != c->pair_index.end()) return *c->pairs[it->second];
-  c->pair_index[key] = (int)c->pairs.size();
-  c->pairs.emplace_back(new glio_ctx::Pair());
-  c->pairs.back()->cur = cur; c->pairs.back()->oth = oth;
-  c->bin_dirty = true;
-  return *c->pairs.back();
-}
-
-}  // namespace
-
-extern "C" {
-
 // ---- K1be / K2be: scan-to-multiscan edge association and binary point-to-edge factors
 int glio_batch_set_edge_frame(glio_ctx* c, int frame, const float* xyz, int64_t Q, int stride, int mem) {
   if (!c) return GLIO_ERR_ARG;
@@ -1863,8 +1862,10 @@ int glio_batch_set_edge_frame(glio_ctx* c, int frame, const float* xyz, int64_t 
     GLIO_REQUIRE(it != c->frames.end(), GLIO_ERR_STATE, "glio_batch_set_edge_frame: frame was not set with glio_batch_set_frame");
     GLIO_REQUIRE(Q >= 0 && stride >= 3 && stride <= 64, GLIO_ERR_ARG, "glio_batch_set_edge_frame: need Q >= 0 and stride_floats in [3,64]");
     glio_ctx::Frame& f = *it->second;
-    const float* p = Q > 0 ? stage_points(c, f.escan, xyz, Q, stride, mem) : nullptr;
-    f.escan_ptr = p; f.eQ = Q; f.estride = stride; f.has_edge = true; f.egrid_valid = false;
+    PointSet& ps = f.corners.pts;
+    if (Q > 0) stage_points(c, ps, xyz, Q, stride, mem);
+    else { ps.clear(); ps.stride = stride; }
+    f.has_edge = true; f.corners.grid_valid = false;
   });
 }
 
@@ -1877,68 +1878,42 @@ int glio_batch_associate_edges_pairs(glio_ctx* c, const int32_t* pairs_cur, cons
   return guarded(c, [&] {
     GLIO_REQUIRE(n_pairs > 0 && pairs_cur && pairs_oth, GLIO_ERR_ARG, "bad pair list");
     const glio_edge_options o = edge_options_or_default(options);
-    std::map<int, std::vector<int64_t>> by_oth;
-    for (int64_t i = 0; i < n_pairs; ++i) {
-      GLIO_REQUIRE(c->frames.count(pairs_cur[i]) && c->frames.count(pairs_oth[i]) && pairs_cur[i] != pairs_oth[i], GLIO_ERR_ARG,
-                   "pair references an unknown frame");
-      by_oth[pairs_oth[i]].push_back(i);
-    }
+    const auto by_oth = pairs_by_searched_frame(c, pairs_cur, pairs_oth, n_pairs);
     for (int64_t i = 0; i < n_pairs; ++i)
       GLIO_REQUIRE(c->frames[pairs_cur[i]]->has_edge && c->frames[pairs_oth[i]]->has_edge, GLIO_ERR_STATE,
                    "pair frame has no corner scan (glio_batch_set_edge_frame)");
-    const EdgeFitParams ep{o.max_sqdist, o.min_ratio, o.half_length};
     c->bedge_dirty = true;
     for (auto& grp : by_oth) {
       glio_ctx::Frame& fo = *c->frames[grp.first];
-      // the group's pairs; their edge lists count as empty until the counts arrive (a reserve may drop the old contents)
+      // the group's pairs; their edge lists count as empty until the counts arrive
       std::vector<glio_ctx::Pair*> prs;
       for (int64_t i : grp.second) {
         glio_ctx::Pair& pr = pair_entry(c, pairs_cur[i], pairs_oth[i]);
-        pr.n_edge = 0; pr.e_has_src = false;
+        pr.edges.clear();
         prs.push_back(&pr);
         if (n_edge) n_edge[i] = 0;
       }
-      if (fo.eQ == 0) continue;                 // nothing to search: every query fails the radius gate
+      if (fo.corners.pts.n == 0) continue;      // nothing to search: every query fails the radius gate
       std::vector<SegDesc> segs;
       std::vector<EdgeDst> dst;
       std::vector<int64_t> seg_item;
       int64_t Qt = 0;
       for (size_t s = 0; s < grp.second.size(); ++s) {
         const glio_ctx::Frame& fc = *c->frames[pairs_cur[grp.second[s]]];
-        if (fc.eQ == 0) continue;
-        SegDesc sd;
-        sd.src = fc.escan_ptr; sd.stride = fc.estride; sd.count = fc.eQ; sd.offset = Qt;
-        for (int k = 0; k < 3; ++k) sd.t[k] = fc.pose[k];          // body pose applied directly to the stored points (quirk Q7)
-        for (int k = 0; k < 4; ++k) sd.q[k] = fc.pose[3 + k];
-        glio_ctx::Pair& pr = *prs[s];
-        pr.e_cps.reserve((size_t)fc.eQ); pr.e_pa.reserve((size_t)fc.eQ); pr.e_pb.reserve((size_t)fc.eQ); pr.e_src.reserve((size_t)fc.eQ);
-        dst.push_back(EdgeDst{pr.e_cps.p, pr.e_pa.p, pr.e_pb.p, pr.e_src.p});
-        segs.push_back(sd); seg_item.push_back((int64_t)s);
-        Qt += fc.eQ;
+        if (fc.corners.pts.n == 0) continue;
+        segs.push_back(make_seg(fc.corners.pts, Qt, fc.pose));     // body pose applied directly to the stored points (quirk Q7)
+        dst.push_back(prs[s]->edges.reserve(fc.corners.pts.n));
+        seg_item.push_back((int64_t)s);
+        Qt += fc.corners.pts.n;
       }
       if (segs.empty()) continue;
       GLIO_REQUIRE(Qt < ((int64_t)1 << 31), GLIO_ERR_ARG, "glio_batch_associate_edges_pairs: too many corner points searching one frame");
-      if (!fo.egrid_valid) {
-        grid_build(fo.egrid, fo.escan_ptr, fo.estride, fo.eQ, fo.pose, fo.pose + 3, c->prm.cell_size, c->pts_per_cell, c->st, c->lc);
-        fo.egrid_valid = true;
-      }
-      const int nseg = (int)segs.size();
-      ensure_work(c, Qt, false, false);
-      c->w_pa.reserve((size_t)Qt); c->w_pb.reserve((size_t)Qt);
-      c->d_segs.reserve(nseg); c->d_edst.reserve(nseg); c->d_counts.reserve(nseg); c->h_counts.reserve(nseg);
-      GLIO_CUDA_TRY(cudaMemcpyAsync(c->d_segs.p, segs.data(), nseg * sizeof(SegDesc), cudaMemcpyHostToDevice, c->st));
-      GLIO_CUDA_TRY(cudaMemcpyAsync(c->d_edst.p, dst.data(), nseg * sizeof(EdgeDst), cudaMemcpyHostToDevice, c->st));
-      AssocWork w = make_work(c, Qt, false, false);
-      edge_assoc_run(fo.egrid, c->d_segs.p, nseg, w, ep, c->w_pa.p, c->w_pb.p, nullptr, fo.escan_ptr, fo.estride, c->cell_count, c->cell_pos,
-                     c->scan_tmp, c->st, c->lc);
-      compact_count(w, c->d_segs.p, nseg, c->w_flags.p, c->w_pos.p, c->scan_tmp, c->d_counts.p, c->st, c->lc);
-      compact_edge_scatter(w, c->d_segs.p, c->w_pos.p, c->w_pa.p, c->w_pb.p, (float)o.score, c->d_edst.p, c->st, c->lc);
-      GLIO_CUDA_TRY(cudaMemcpyAsync(c->h_counts.p, c->d_counts.p, nseg * sizeof(int), cudaMemcpyDeviceToHost, c->st));
-      GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
-      for (int s = 0; s < nseg; ++s) {
-        glio_ctx::Pair& pr = *prs[seg_item[s]];
-        pr.n_edge = c->h_counts.p[s]; pr.e_has_src = true;
-        if (n_edge) n_edge[grp.second[seg_item[s]]] = pr.n_edge;
+      const GridBuild& grid = searched_grid(c, fo, fo.corners);
+      edge_assoc_launch(c, grid, segs, dst, Qt, o, fo.corners.pts.ptr, fo.corners.pts.stride, nullptr);
+      for (size_t s = 0; s < segs.size(); ++s) {
+        EdgeList& e = prs[seg_item[s]]->edges;
+        e.n = c->h_counts.p[s]; e.has_src = true;
+        if (n_edge) n_edge[grp.second[seg_item[s]]] = e.n;
       }
     }
   });
@@ -1947,10 +1922,7 @@ int glio_batch_associate_edges_pairs(glio_ctx* c, const int32_t* pairs_cur, cons
 int glio_batch_get_edges(glio_ctx* c, int cur, int oth, int64_t capacity, float* cp, float* pa, float* pb, double* s, int32_t* src, int64_t* n) {
   if (!c) return GLIO_ERR_ARG;
   return guarded(c, [&] {
-    auto it = c->pair_index.find(std::make_pair(cur, oth));
-    GLIO_REQUIRE(it != c->pair_index.end(), GLIO_ERR_ARG, "pair is not on the pair list");
-    glio_ctx::Pair& pr = *c->pairs[it->second];
-    copy_edges_out(c, pr.n_edge, pr.e_cps.p, pr.e_pa.p, pr.e_pb.p, pr.e_src.p, pr.e_has_src, capacity, cp, pa, pb, s, src, n);
+    copy_edges_out(c, find_pair(c, cur, oth).edges, capacity, cp, pa, pb, s, src, n);
   });
 }
 
@@ -1959,10 +1931,10 @@ int glio_batch_set_pair_edges(glio_ctx* c, int cur, int oth, const float* cp, co
   return guarded(c, [&] {
     GLIO_REQUIRE(cur >= 0 && oth >= 0 && cur != oth, GLIO_ERR_ARG, "bad pair");
     GLIO_REQUIRE(n >= 0 && (n == 0 || (cp && pa && pb && s)), GLIO_ERR_ARG, "null edge arrays");
-    glio_ctx::Pair& pr = pair_entry(c, cur, oth);
-    pr.n_edge = 0; pr.e_has_src = false; c->bedge_dirty = true;
-    if (n > 0) upload_edges(c, n, cp, pa, pb, s, pr.e_cps, pr.e_pa, pr.e_pb);
-    pr.n_edge = n;
+    EdgeList& e = pair_entry(c, cur, oth).edges;
+    e.clear(); c->bedge_dirty = true;
+    if (n > 0) upload_edges(c, e, n, cp, pa, pb, s);
+    e.n = n;
   });
 }
 
@@ -2049,22 +2021,20 @@ int glio_batch_select_random(glio_ctx* c, const int32_t* cur, const int32_t* oth
     GLIO_REQUIRE(mode == 0 || mode == 1, GLIO_ERR_ARG, "glio_batch_select_random: mode must be 0 (start/end) or 1 (incremental)");
     check_select_options(opt);
     const int Bn = opt->batch_feature_res_num;
-    std::vector<int> pidx((size_t)n_pairs);
-    std::vector<char> listed(c->pairs.size(), 0);
+    std::vector<glio_ctx::Pair*> prs((size_t)n_pairs);
+    std::set<const glio_ctx::Pair*> listed;
     std::set<int> runs_seen;
     for (int64_t i = 0; i < n_pairs; ++i) {
       GLIO_REQUIRE(cur[i] != oth[i], GLIO_ERR_ARG, "glio_batch_select_random: cur == oth");
-      auto it = c->pair_index.find(std::make_pair((int)cur[i], (int)oth[i]));
-      GLIO_REQUIRE(it != c->pair_index.end(), GLIO_ERR_ARG, "glio_batch_select_random: pair was not associated");
-      GLIO_REQUIRE(!listed[it->second], GLIO_ERR_ARG, "glio_batch_select_random: pair listed twice");
-      listed[it->second] = 1; pidx[i] = it->second;
+      prs[i] = &find_pair(c, cur[i], oth[i]);
+      GLIO_REQUIRE(listed.insert(prs[i]).second, GLIO_ERR_ARG, "glio_batch_select_random: pair listed twice");
       if (i == 0 || cur[i] != cur[i - 1])
         GLIO_REQUIRE(runs_seen.insert(cur[i]).second, GLIO_ERR_ARG, "glio_batch_select_random: pair list is not grouped by cur");
     }
     std::vector<int64_t> n_sel((size_t)n_pairs);
     bool stopped = false;
     for (int64_t i = 0; i < n_pairs; ++i) {
-      const int64_t n = c->pairs[pidx[i]]->n_match;
+      const int64_t n = prs[i]->n_match;
       if (i == 0 || cur[i] != cur[i - 1]) stopped = false;
       if (mode == 0) {
         if (!stopped && (n - 1 < Bn || n < 50)) stopped = true;
@@ -2076,7 +2046,7 @@ int glio_batch_select_random(glio_ctx* c, const int32_t* cur, const int32_t* oth
     std::vector<SelSeg> segs;
     for (int64_t i = 0; i < n_pairs; ++i) {
       if (n_sel[i] <= 0) continue;
-      glio_ctx::Pair& pr = *c->pairs[pidx[i]];
+      glio_ctx::Pair& pr = *prs[i];
       pr.s_cpw.reserve(Bn); pr.s_nc.reserve(6 * (size_t)Bn); pr.s_keep.reserve(Bn);
       SelSeg g{};
       g.cpw = pr.m_cpw.p; g.nsd = nullptr; g.nc = pr.m_nc.p; g.o_cpw = pr.s_cpw.p; g.o_nsd = nullptr; g.o_nc = pr.s_nc.p;
@@ -2085,7 +2055,7 @@ int glio_batch_select_random(glio_ctx* c, const int32_t* cur, const int32_t* oth
     }
     select_launch(c, segs, Bn, mode == 0 ? SEL_DOMAIN_STARTEND : SEL_DOMAIN_ADD, opt->seed, opt->nonce);
     for (int64_t i = 0; i < n_pairs; ++i) {
-      glio_ctx::Pair& pr = *c->pairs[pidx[i]];
+      glio_ctx::Pair& pr = *prs[i];
       pr.n_sel = n_sel[i];
       if (n_active) n_active[i] = n_sel[i] >= 0 ? n_sel[i] : pr.n_match;
     }
@@ -2120,9 +2090,7 @@ int glio_get_selection(glio_ctx* c, int slot, int64_t capacity, int32_t* keep, i
 int glio_batch_get_selection(glio_ctx* c, int cur, int oth, int64_t capacity, int32_t* keep, int64_t* n) {
   if (!c) return GLIO_ERR_ARG;
   return guarded(c, [&] {
-    auto it = c->pair_index.find(std::make_pair(cur, oth));
-    GLIO_REQUIRE(it != c->pair_index.end(), GLIO_ERR_ARG, "pair was not associated");
-    glio_ctx::Pair& pr = *c->pairs[it->second];
+    glio_ctx::Pair& pr = find_pair(c, cur, oth);
     copy_selection(c, pr.n_sel, pr.s_keep, capacity, keep, n);
   });
 }
@@ -2179,11 +2147,12 @@ void build_bedge_items(glio_ctx* c, int K) {
   std::vector<BinEdgeItem> items;
   std::vector<int> pstart(P + 1, 0);
   for (int p = 0; p < P; ++p) {
-    glio_ctx::Pair& pr = *c->pairs[p];
+    const glio_ctx::Pair& pr = *c->pairs[p];
+    const EdgeList& e = pr.edges;
     pstart[p] = (int)items.size();
-    for (int64_t o = 0; o < pr.n_edge; o += GLIO_ITEM_MAX) {
-      BinEdgeItem it; it.cps = pr.e_cps.p + o; it.pa = pr.e_pa.p + o; it.pb = pr.e_pb.p + o;
-      it.count = (int32_t)std::min<int64_t>(GLIO_ITEM_MAX, pr.n_edge - o); it.kf_c = pr.cur; it.kf_o = pr.oth;
+    for (int64_t o = 0; o < e.n; o += GLIO_ITEM_MAX) {
+      BinEdgeItem it; it.cps = e.cps.p + o; it.pa = e.pa.p + o; it.pb = e.pb.p + o;
+      it.count = (int32_t)std::min<int64_t>(GLIO_ITEM_MAX, e.n - o); it.kf_c = pr.cur; it.kf_o = pr.oth;
       items.push_back(it);
     }
   }
@@ -2243,13 +2212,9 @@ int eval_binary_out(glio_ctx* c, int K, const double* poses, BinBlocks what, dou
     GLIO_REQUIRE(K > 0 && poses, GLIO_ERR_ARG, "bad arguments");
     const bool want_jac = Hdiag || Hoff || g;
     eval_binary_blocks(c, K, poses, want_jac, /*no loss on batch LiDAR factors, Estimator.cpp:2768*/ 0.0, what);
+    unpack_blocks(c->h_bin_diag.p, K, Hdiag, g, nullptr);
     double ct = 0;
-    for (int k = 0; k < K; ++k) {
-      const double* o = c->h_bin_diag.p + (size_t)k * GLIO_NACC;
-      if (Hdiag) { int idx = 0; for (int p = 0; p < 6; ++p) for (int q = p; q < 6; ++q) { Hdiag[36 * k + 6 * p + q] = o[idx]; Hdiag[36 * k + 6 * q + p] = o[idx]; ++idx; } }
-      if (g) for (int p = 0; p < 6; ++p) g[6 * k + p] = o[21 + p];
-      ct += o[27];
-    }
+    for (int k = 0; k < K; ++k) ct += c->h_bin_diag.p[(size_t)k * GLIO_NACC + 27];
     if (Hoff) memcpy(Hoff, c->h_bin_off.p, c->pairs.size() * 36 * sizeof(double));
     if (cost) *cost = ct;
   });
@@ -2288,13 +2253,7 @@ int glio_batch_declare_pairs(glio_ctx* c, const int32_t* pairs_cur, const int32_
     for (int64_t i = 0; i < n_pairs; ++i)
       GLIO_REQUIRE(pairs_cur[i] >= 0 && pairs_oth[i] >= 0 && pairs_cur[i] != pairs_oth[i], GLIO_ERR_ARG,
                    "glio_batch_declare_pairs: pair indices must be >= 0 and distinct");
-    for (int64_t i = 0; i < n_pairs; ++i) {
-      const std::pair<int, int> key(pairs_cur[i], pairs_oth[i]);
-      if (c->pair_index.count(key)) continue;
-      c->pair_index[key] = (int)c->pairs.size();
-      c->pairs.emplace_back(new glio_ctx::Pair());
-      c->pairs.back()->cur = key.first; c->pairs.back()->oth = key.second;
-    }
+    for (int64_t i = 0; i < n_pairs; ++i) pair_entry(c, pairs_cur[i], pairs_oth[i]);
     c->bin_dirty = true;
   });
 }
@@ -2304,14 +2263,7 @@ int glio_batch_set_pair_matches(glio_ctx* c, int cur, int oth, const float* cp, 
   return guarded(c, [&] {
     GLIO_REQUIRE(cur >= 0 && oth >= 0 && cur != oth, GLIO_ERR_ARG, "bad pair");
     GLIO_REQUIRE(n >= 0 && (n == 0 || (cp && normal_cent && weight)), GLIO_ERR_ARG, "null match arrays");
-    const std::pair<int, int> key(cur, oth);
-    auto it = c->pair_index.find(key);
-    int pi;
-    if (it == c->pair_index.end()) {
-      pi = (int)c->pairs.size(); c->pair_index[key] = pi;
-      c->pairs.emplace_back(new glio_ctx::Pair()); c->pairs.back()->cur = cur; c->pairs.back()->oth = oth;
-    } else pi = it->second;
-    glio_ctx::Pair& pr = *c->pairs[pi];
+    glio_ctx::Pair& pr = pair_entry(c, cur, oth);
     pr.n_match = n; pr.n_sel = -1;
     if (n > 0) {
       std::vector<float> cpw((size_t)n * 4);
@@ -2337,38 +2289,16 @@ int glio_batch_solve(glio_ctx* c, int K, double* poses, double* speed_bias, glio
     if (options) o = *options;
     else { glio_default_solver_options(&o); o.dogleg_type = 1; o.use_nonmonotonic_steps = 1; o.max_num_iterations = 100; }  // Estimator.cpp:3276-3281
     const bool sb = speed_bias != nullptr;
-    const int nt = sb ? 15 : 6, na = sb ? 16 : 7, n = K * nt;
+    const StateLayout L(K, sb);
+    const int nt = L.nt, n = K * nt;
     int span = 1;
     for (auto& p : c->pairs) span = std::max(span, std::abs(p->cur - p->oth));
     const int hb = (span + 1) * nt - 1;
-    std::vector<ParamBlock> blocks;
-    for (int k = 0; k < K; ++k) {
-      blocks.push_back(ParamBlock{na * k, 3, nt * k, 3, false, nullptr});
-      blocks.push_back(ParamBlock{na * k + 3, 4, nt * k + 3, 3, true, nullptr});
-      if (sb) blocks.push_back(ParamBlock{na * k + 7, 9, nt * k + 6, 9, false, nullptr});
-    }
-    SolverOptions so;
-    so.max_num_iterations = o.max_num_iterations; so.dogleg_type = o.dogleg_type; so.use_nonmonotonic_steps = o.use_nonmonotonic_steps != 0;
-    so.max_consecutive_nonmonotonic_steps = o.max_consecutive_nonmonotonic_steps;
-    so.initial_trust_region_radius = o.initial_trust_region_radius; so.max_trust_region_radius = o.max_trust_region_radius;
-    so.min_trust_region_radius = o.min_trust_region_radius; so.min_relative_decrease = o.min_relative_decrease;
-    so.min_lm_diagonal = o.min_lm_diagonal; so.max_lm_diagonal = o.max_lm_diagonal;
-    so.max_num_consecutive_invalid_steps = o.max_num_consecutive_invalid_steps; so.jacobi_scaling = o.jacobi_scaling != 0;
-    so.function_tolerance = o.function_tolerance; so.gradient_tolerance = o.gradient_tolerance; so.parameter_tolerance = o.parameter_tolerance;
-    so.fuse_candidate_jacobian = o.fuse_candidate_jacobian != 0;
-    GLIO_REQUIRE(o.trust_region_strategy == 0 || o.trust_region_strategy == 1, GLIO_ERR_ARG, "trust_region_strategy must be 0 (DOGLEG) or 1 (LEVENBERG_MARQUARDT)");
-    so.trust_region_strategy = o.trust_region_strategy;
-    TrustRegionDogleg solver(blocks, so);
-    std::vector<double> x((size_t)K * na), pz((size_t)K * 7), sz((size_t)K * 9);
-    for (int k = 0; k < K; ++k) {
-      for (int i = 0; i < 7; ++i) x[(size_t)na * k + i] = poses[7 * k + i];
-      if (sb) for (int i = 0; i < 9; ++i) x[(size_t)na * k + 7 + i] = speed_bias[9 * k + i];
-    }
+    TrustRegionDogleg solver(L.blocks(), solver_options_from(o));
+    std::vector<double> x((size_t)K * L.na), pz((size_t)K * 7), sz((size_t)K * 9);
+    L.pack(poses, speed_bias, x.data());
     EvalFn eval = [&](const double* xa, bool want_jac, double* cost, BandMat* H, double* g) -> bool {
-      for (int k = 0; k < K; ++k) {
-        for (int i = 0; i < 7; ++i) pz[7 * k + i] = xa[(size_t)na * k + i];
-        if (sb) for (int i = 0; i < 9; ++i) sz[9 * k + i] = xa[(size_t)na * k + 7 + i];
-      }
+      L.unpack(xa, pz.data(), sz.data());
       // the device evaluates the LiDAR pairs (and a sharded run sums them over the ranks) while the host evaluates its own
       // factors into the freshly reset band; the device blocks are added when they have arrived
       eval_binary_launch(c, K, pz.data(), want_jac, 0.0, c->batch_use_edges ? BIN_PLANES_EDGES : BIN_PLANES);
@@ -2382,12 +2312,8 @@ int glio_batch_solve(glio_ctx* c, int K, double* poses, double* speed_bias, glio
       if (want_jac) {
         const int w = H->hb + 1;
         double* a = H->a.data();
-        for (int k = 0; k < K; ++k) {
-          const double* ob = c->h_bin_diag.p + (size_t)k * GLIO_NACC;
-          int idx = 0;
-          for (int p = 0; p < 6; ++p) for (int q = p; q < 6; ++q) { H->at(nt * k + q, nt * k + p) += ob[idx]; ++idx; }
-          for (int p = 0; p < 6; ++p) g[nt * k + p] += ob[21 + p];
-        }
+        add_diag_blocks(H, c->h_bin_diag.p, K, nt);
+        for (int k = 0; k < K; ++k) for (int p = 0; p < 6; ++p) g[nt * k + p] += c->h_bin_diag.p[(size_t)k * GLIO_NACC + 21 + p];
         for (size_t pi = 0; pi < c->pairs.size(); ++pi) {
           const int kc = c->pairs[pi]->cur, ko = c->pairs[pi]->oth;
           const double* ob = c->h_bin_off.p + pi * 36;                 // d2 cost / d x_cur[p] d x_oth[q]
@@ -2405,10 +2331,7 @@ int glio_batch_solve(glio_ctx* c, int K, double* poses, double* speed_bias, glio
     };
     SolverSummary S;
     solver.solve(x.data(), eval, &S);
-    for (int k = 0; k < K; ++k) {
-      for (int i = 0; i < 7; ++i) poses[7 * k + i] = x[(size_t)na * k + i];
-      if (sb) for (int i = 0; i < 9; ++i) speed_bias[9 * k + i] = x[(size_t)na * k + 7 + i];
-    }
+    L.unpack(x.data(), poses, speed_bias);
     fill_summary(S, n, summary, iter_log, iter_cap, step_log, step_cap);
   });
 }
@@ -2418,11 +2341,11 @@ int glio_batch_solve(glio_ctx* c, int K, double* poses, double* speed_bias, glio
 int glio_set_edges(glio_ctx* c, int slot, const float* cp, const float* pa, const float* pb, const double* s, int64_t n) {
   if (!c) return GLIO_ERR_ARG;
   return guarded(c, [&] {
-    Slot& sl = c->slot(slot);
-    sl.n_edge = 0; sl.e_has_src = false; c->edge_items_dirty = true;
+    EdgeList& e = c->slot(slot).edges;
+    e.clear(); c->edge_items_dirty = true;
     if (n <= 0) return;
-    upload_edges(c, n, cp, pa, pb, s, sl.e_cps, sl.e_pa, sl.e_pb);
-    sl.n_edge = n;
+    upload_edges(c, e, n, cp, pa, pb, s);
+    e.n = n;
   });
 }
 
@@ -2446,12 +2369,7 @@ static int eval_edge_impl(glio_ctx* c, int W, const double* poses_body, int jac_
     std::vector<double> ho((size_t)W * GLIO_NACC);
     GLIO_CUDA_TRY(cudaMemcpyAsync(ho.data(), d_out.p, ho.size() * sizeof(double), cudaMemcpyDeviceToHost, c->st));
     GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
-    for (int k = 0; k < W; ++k) {
-      const double* o = ho.data() + (size_t)k * GLIO_NACC;
-      if (H) { int idx = 0; for (int p = 0; p < 6; ++p) for (int q = p; q < 6; ++q) { H[36 * k + 6 * p + q] = o[idx]; H[36 * k + 6 * q + p] = o[idx]; ++idx; } }
-      if (g) for (int p = 0; p < 6; ++p) g[6 * k + p] = o[21 + p];
-      if (cost) cost[k] = o[27];
-    }
+    unpack_blocks(ho.data(), W, H, g, cost);
   });
 }
 
@@ -2507,10 +2425,6 @@ struct glio_odom {
     quat_last_kf[0] = 1.0; quat_last_kf[1] = quat_last_kf[2] = quat_last_kf[3] = 0.0;
     while (!lm.frames.empty()) lm.pop_front();   // buffers kept for the next run
     last_ds_n = 0; map_pts = nullptr; map_n = 0;
-  }
-  void release() {
-    lm.release(); scan_vox.release(); last_ds.release(); in_surf.release(); in_full.release(); out_surf.release(); out_full.release();
-    grid.release(); slot.release(); d_items.release(); d_start.release(); d_partials.release();
   }
 };
 
@@ -2582,7 +2496,7 @@ void odom_step(glio_odom* o, const float4* surf, int64_t n_surf, const float4* f
       go.trust_region_strategy = 1; go.max_num_iterations = o->opt.max_num_iter;             // Ceres defaults: LEVENBERG_MARQUARDT
       SolverOptions sopt = solver_options_from(go);
       sopt.max_solver_time_in_seconds = o->opt.max_solver_time_s;
-      o->slot.scan_ptr = scan; o->slot.stride = scan_stride; o->slot.Q = scan_n;
+      o->slot.scan.ptr = scan; o->slot.scan.stride = scan_stride; o->slot.scan.n = scan_n;
       SolverSummary S;
       for (int r = 0; r < rounds; ++r) {
         double x[7] = {o->abs_pose[4], o->abs_pose[5], o->abs_pose[6], o->abs_pose[0], o->abs_pose[1], o->abs_pose[2], o->abs_pose[3]};
@@ -2681,8 +2595,7 @@ void glio_odom_destroy(glio_odom* o) {
   if (!o) return;
   glio_ctx* c = o->ctx;
   cudaSetDevice(c->device);
-  cudaStreamSynchronize(c->st);
-  o->release();
+  cudaStreamSynchronize(c->st);          // nothing queued may still use the buffers `delete o` frees
   c->odoms.erase(std::remove(c->odoms.begin(), c->odoms.end(), o), c->odoms.end());
   delete o;
 }
@@ -2766,10 +2679,6 @@ struct glio_loop {
   const float* lat_pts = nullptr; int lat_stride = 3; int64_t lat_n = 0;
   const float* his_pts = nullptr; int his_stride = 3; int64_t his_n = 0;
   IcpWork icp;
-  void release() {
-    for (auto& k : kfs) k->xyz.release();
-    kfs.clear(); latest.release(); his.release(); icp.release();
-  }
 };
 
 namespace {
@@ -2897,7 +2806,7 @@ int glio_icp_align(glio_ctx* c, const float* src, int64_t n_src, int src_stride,
       std::vector<float4> a((size_t)n_src);
       GLIO_CUDA_TRY(cudaMemcpyAsync(a.data(), c->icp.fit.p, (size_t)n_src * sizeof(float4), cudaMemcpyDeviceToHost, c->st));
       GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
-      for (int64_t i = 0; i < n_src; ++i) { aligned_xyz[3 * i] = a[i].x; aligned_xyz[3 * i + 1] = a[i].y; aligned_xyz[3 * i + 2] = a[i].z; }
+      unpack_float4(a.data(), n_src, aligned_xyz);
     }
     const int nlog = std::min(iter_cap, h.nr_iter);
     if (iter_log && nlog > 0) {
@@ -2946,8 +2855,7 @@ void glio_loop_destroy(glio_loop* L) {
   if (!L) return;
   glio_ctx* c = L->ctx;
   cudaSetDevice(c->device);
-  cudaStreamSynchronize(c->st);
-  L->release();
+  cudaStreamSynchronize(c->st);          // nothing queued may still use the buffers `delete L` frees
   c->loops.erase(std::remove(c->loops.begin(), c->loops.end(), L), c->loops.end());
   delete L;
 }
@@ -2956,7 +2864,6 @@ int glio_loop_reset(glio_loop* L) {
   if (!L) return GLIO_ERR_ARG;
   return guarded(L->ctx, [&] {
     GLIO_CUDA_TRY(cudaStreamSynchronize(L->ctx->st));
-    for (auto& k : L->kfs) k->xyz.release();
     L->kfs.clear();
     L->time_last_loop = 0.0;
     L->lat_pts = L->his_pts = nullptr; L->lat_n = L->his_n = 0;

@@ -44,11 +44,20 @@ const char* global_error();
     if (!(cond)) throw ::glio::Error{(code), (text)};       \
   } while (0)
 
-// grow-only device buffer
+// grow-only device buffer that owns its memory: freed on destruction, moved but never copied (a copy would free it twice)
 template <class T>
 struct DevBuf {
   T* p = nullptr;
   size_t cap = 0;
+  DevBuf() = default;
+  DevBuf(const DevBuf&) = delete;
+  DevBuf& operator=(const DevBuf&) = delete;
+  DevBuf(DevBuf&& o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr; o.cap = 0; }
+  DevBuf& operator=(DevBuf&& o) noexcept {
+    if (this != &o) { release(); p = o.p; cap = o.cap; o.p = nullptr; o.cap = 0; }
+    return *this;
+  }
+  ~DevBuf() { release(); }
   void reserve(size_t n) {
     if (n <= cap) return;
     if (p) GLIO_CUDA_TRY(cudaFree(p));
@@ -57,13 +66,23 @@ struct DevBuf {
     GLIO_CUDA_TRY(cudaMalloc((void**)&p, want * sizeof(T)));
     cap = want;
   }
-  void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
+  void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }   // result ignored: runs in the destructor, which must not throw
 };
 
+// the same for page-locked host memory
 template <class T>
 struct PinnedBuf {
   T* p = nullptr;
   size_t cap = 0;
+  PinnedBuf() = default;
+  PinnedBuf(const PinnedBuf&) = delete;
+  PinnedBuf& operator=(const PinnedBuf&) = delete;
+  PinnedBuf(PinnedBuf&& o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr; o.cap = 0; }
+  PinnedBuf& operator=(PinnedBuf&& o) noexcept {
+    if (this != &o) { release(); p = o.p; cap = o.cap; o.p = nullptr; o.cap = 0; }
+    return *this;
+  }
+  ~PinnedBuf() { release(); }
   void reserve(size_t n) {
     if (n <= cap) return;
     if (p) GLIO_CUDA_TRY(cudaFreeHost(p));
@@ -72,7 +91,7 @@ struct PinnedBuf {
     GLIO_CUDA_TRY(cudaMallocHost((void**)&p, want * sizeof(T)));
     cap = want;
   }
-  void release() { if (p) cudaFreeHost(p); p = nullptr; cap = 0; }
+  void release() { if (p) cudaFreeHost(p); p = nullptr; cap = 0; }   // result ignored, as above
 };
 
 // ----------------------------------------------------------------------------------------------
@@ -169,7 +188,6 @@ struct GridBuild {
   DevBuf<int> scan_tmp;
   DevBuf<int> bounds;      // 6 order-preserving ints on device
   GridDesc desc{};
-  void release() { cell_start.release(); pts.release(); tmp4.release(); sorted_pos.release(); fill.release(); scan_tmp.release(); bounds.release(); }
 };
 void grid_build(GridBuild& gb, const float* d_xyz, int stride, int64_t n, const double* t, const double* q,
                 float cell_size_hint, float pts_per_cell, cudaStream_t st, LaunchCounter& lc);
@@ -180,7 +198,6 @@ struct VoxelWork {
   DevBuf<float4> tmp4;
   DevBuf<int> bounds, count, start, opos, order, sorted, scan_tmp, out_vox;
   DevBuf<float> out_xyz;      // filtered points, 3 floats each, ascending voxel index
-  void release() { tmp4.release(); bounds.release(); count.release(); start.release(); opos.release(); order.release(); sorted.release(); scan_tmp.release(); out_vox.release(); out_xyz.release(); }
 };
 void localmap_transform(const float* d_xyz, int stride, int64_t n, const double* t, const double* q, float4* d_out, cudaStream_t st, LaunchCounter& lc);
 // returns the number of filtered points (in w.out_xyz / w.out_vox), or -1 when PCL would pass the input through unchanged
@@ -193,10 +210,6 @@ struct VoxelSortWork {
   DevBuf<int> val0, val1;               //                       point indices
   DevBuf<int> bounds, bad, hist, flags, pos, scan_tmp;
   DevBuf<float> out_xyz;                // result, 3 floats per point
-  void release() {
-    tmp4.release(); key0.release(); key1.release(); val0.release(); val1.release(); bounds.release(); bad.release(); hist.release();
-    flags.release(); pos.release(); scan_tmp.release(); out_xyz.release();
-  }
 };
 // n (> 0, < 2^31) points stride floats apart on the device -> w.out_xyz; returns its size.  *filtered = false: PCL's leaf-size check
 // passed the input through (w.out_xyz holds the input x,y,z).  Non-finite coordinates are GLIO_ERR_ARG.
@@ -213,12 +226,11 @@ struct LocalMap {
   // transformCloud(cloud, {t, q}) = float(q*double(p)+t) on the device, then push_front / push_back
   void push(bool at_front, const float* d_xyz, int stride, int64_t n, const double* t, const double* q, cudaStream_t st, LaunchCounter& lc);
   void pop_front();            // the stream is ordered: anything still reading the popped buffer was enqueued before whatever reuses it
-  void clear();                // frees every frame buffer
+  void clear();                // drops every frame and frees its buffer
   int64_t n_points() const;
   // concatenate (oldest first) and VoxelGrid(leaf) when leaf > 0; *pts / *stride receive the device cloud.  Returns its size and
   // sets *filtered = false when leaf <= 0 or PCL's overflow rule passed the concatenation through unchanged.
   int64_t build(float leaf, const float** pts, int* stride, bool* filtered, cudaStream_t st, LaunchCounter& lc);
-  void release() { clear(); cat.release(); vox.release(); }
 };
 
 // ---- K1 / K1b (assoc.cu)
@@ -411,11 +423,6 @@ struct IcpWork {
   DevBuf<IcpState> state;
   IcpState last{};
   int64_t n_src = 0, n_tgt = 0;
-  void release() {
-    grid.release(); src0.release(); cur.release(); fit.release(); qcount.release(); qstart.release(); perm.release(); scan_tmp.release();
-    nn_idx.release(); flags.release(); pos.release(); cq.release(); cm.release(); nn_d.release(); cd.release();
-    pf0.release(); pf1.release(); pd0.release(); pd1.release(); log.release(); state.release();
-  }
 };
 // one registration of d_src (n_src points, src_stride floats apart) onto d_tgt; *out receives the final state (fitness included).
 // w.fit holds the aligned cloud (float4), w.cq / w.cm / w.cd the last correspondence list, w.log the first min(log_cap, iterations)

@@ -638,9 +638,7 @@ void LocalMap::pop_front() {
 }
 
 void LocalMap::clear() {
-  for (auto& f : frames) f->pts.release();
   frames.clear();
-  for (auto& f : spare) f->pts.release();
   spare.clear();
 }
 
