@@ -135,12 +135,18 @@ class Context:
         self._lib.glio_lidar_pose(C.byref(self.params), _ptr(pb), _ptr(t2), _ptr(q2))
         return t2, q2
 
-    KERNELS = ["k_feat_curvature", "k_feat_select", "k_feat_voxel", "k_feat_offsets", "k_feat_gather", "k_knn_box", "k_plane_fit", "k_plane_fit_pair", "k_eval_unary", "k_eval_unary_cost", "k_transform_hist", "k_order_scatter",
+    # every kernel name the library hands its launch counter (tests/test_profile_names.py keeps this list complete)
+    KERNELS = ["k_sp_bounds", "k_sp_consts", "k_sp_classify", "k_sp_ranges", "k_sp_emit",
+               "k_feat_curvature", "k_feat_select", "k_feat_voxel", "k_feat_offsets", "k_feat_gather", "k_knn_box", "k_plane_fit", "k_plane_fit_pair",
+               "k_eval_unary", "k_eval_unary_cost", "k_unary_residuals", "k_eval_edge", "k_eval_edge_cost", "k_transform_hist", "k_order_scatter",
                "k_compact", "k_flags", "k_cell_hist", "k_cell_scatter", "k_load_bounds", "k_scan_block", "k_scan_add",
-               "k_eval_binary", "k_eval_binary_cost", "k_bin_assemble", "k_gather_sel", "k_sel_sample",
+               "k_eval_binary", "k_eval_binary_cost", "k_bin_assemble", "k_bin_pair_sums", "k_gather_sel", "k_sel_sample",
                "k_lm_transform", "k_vox_hist", "k_vox_scatter", "k_vox_sort", "k_vox_flags", "k_vox_centroid", "k_init_bounds",
                "k_line_fit", "k_compact_edge", "k_seg_counts", "k_line_fit_pair", "k_eval_binary_edge", "k_eval_binary_edge_cost",
-               "k_bin_pair_add"]
+               "k_bin_pair_add", "k_odom_publish",
+               "k_lc_load", "k_lc_qhist", "k_lc_qscatter", "k_lc_init", "k_lc_nn", "k_lc_compact", "k_lc_sum0",
+               "k_lc_sum1", "k_lc_means", "k_lc_solve", "k_lc_transform", "k_lc_final", "k_lc_fitness",
+               "k_vs_key", "k_vs_hist", "k_vs_scatter", "k_vs_heads", "k_vs_centroid", "k_vs_pack", "k_gm_transform"]
 
     def lib_profile(self, on):
         self._chk(self._lib.glio_profile_enable(self._h, C.c_int(1 if on else 0)))
@@ -498,7 +504,6 @@ def _scanprep_guard_hits(self, reset=False):
 
 
 Context.prepare_scan = _prepare_scan
-Context.KERNELS = ["k_sp_bounds", "k_sp_consts", "k_sp_classify", "k_sp_ranges", "k_sp_emit"] + Context.KERNELS
 Context.scanprep_guard_hits = _scanprep_guard_hits
 
 
@@ -1111,9 +1116,6 @@ class Odometry:
         return m, s
 
 
-Context.KERNELS = Context.KERNELS + ["k_odom_publish"]
-
-
 # ---------------------------------------------------------------------------------------------------------------------------
 # loop-closure registration (detectLoopClosure / performLoopClosure, GLIO/src/Estimator.cpp:5101-5273, without the GTSAM half)
 # ---------------------------------------------------------------------------------------------------------------------------
@@ -1313,8 +1315,3 @@ class LoopClosure:
         a = np.empty((nl.value, 3), np.float32); b = np.empty((nh.value, 3), np.float32)
         self.ctx._chk(self._lib.glio_loop_get_clouds(self._h, C.c_int64(nl.value), _ptr(a), C.byref(nl), C.c_int64(nh.value), _ptr(b), C.byref(nh)))
         return a, b
-
-
-Context.KERNELS = Context.KERNELS + ["k_lc_load", "k_lc_qhist", "k_lc_qscatter", "k_lc_init", "k_lc_nn", "k_lc_compact", "k_lc_sum0",
-                                     "k_lc_sum1", "k_lc_means", "k_lc_solve", "k_lc_transform", "k_lc_final", "k_lc_fitness"]
-Context.KERNELS = Context.KERNELS + ["k_vs_key", "k_vs_hist", "k_vs_scatter", "k_vs_heads", "k_vs_centroid", "k_vs_pack", "k_gm_transform"]

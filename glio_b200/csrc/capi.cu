@@ -390,34 +390,55 @@ void associate_ctx_slots(glio_ctx* c, const std::vector<int>& ids, const std::ve
   c->items_dirty = true;
 }
 
-// evaluation work items of the given slots (slot k = keyframe k, nullptr = none): start[k] = first item of keyframe k
-std::vector<EvalItem> plan_items(const std::vector<const Slot*>& slots, int eval_slots, std::vector<int>& start) {
+// The work items of one evaluation kernel, one block each: every owner's (keyframe's or pair's) residuals cut into runs, owners in
+// order.  start[o] = first item of owner o, start[owners] = the item count.
+template <class Item>
+struct ItemPlan {
+  std::vector<Item> items;
+  std::vector<int> start;
+  explicit ItemPlan(int owners) : start(owners + 1, 0) {}
+  // owner o (called once per owner, in order) with n residuals, in runs of per; item(first, count) makes one run's item
+  template <class MakeItem>
+  void cut(int o, int64_t n, int64_t per, MakeItem item) {
+    for (int64_t f = 0; f < n; f += per) items.push_back(item(f, (int32_t)std::min<int64_t>(per, n - f)));
+    start[o + 1] = (int)items.size();
+  }
+  // items and start table into d_items / d_start, d_partials sized for nacc sums per item; synchronises (both are host vectors)
+  void upload(glio_ctx* c, DevBuf<Item>& d_items, DevBuf<int>& d_start, DevBuf<double>& d_partials, int nacc) const {
+    d_items.reserve(items.size() + 1); d_start.reserve(start.size()); d_partials.reserve((items.size() + 1) * nacc);
+    if (!items.empty()) GLIO_CUDA_TRY(cudaMemcpyAsync(d_items.p, items.data(), items.size() * sizeof(Item), cudaMemcpyHostToDevice, c->st));
+    GLIO_CUDA_TRY(cudaMemcpyAsync(d_start.p, start.data(), start.size() * sizeof(int), cudaMemcpyHostToDevice, c->st));
+    GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
+  }
+};
+
+// the ticket of the unary kernels' last-block election, zero between launches
+void init_ticket(glio_ctx* c) {
+  if (!c->d_ticket.p) { c->d_ticket.reserve(1); GLIO_CUDA_TRY(cudaMemsetAsync(c->d_ticket.p, 0, sizeof(unsigned int), c->st)); }
+}
+
+// K2 work items of the given slots (slot k = keyframe k, nullptr = none)
+ItemPlan<EvalItem> plan_items(const std::vector<const Slot*>& slots, int eval_slots) {
   const int W = (int)slots.size();
-  std::vector<EvalItem> items;
-  start.assign(W + 1, 0);
+  auto active = [](const Slot* sl) -> int64_t { return !sl ? 0 : sl->n_sel >= 0 ? sl->n_sel : sl->n_match; };
   // item size: the whole launch should be about one wave of 2 resident blocks per SM (less per-item reduction
   // overhead, no wave-quantisation tail), but never below GLIO_ITEM_MAX residuals per item
   int64_t n_total = 0;
-  for (int k = 0; k < W; ++k) if (slots[k]) n_total += slots[k]->n_sel >= 0 ? slots[k]->n_sel : slots[k]->n_match;
+  for (int k = 0; k < W; ++k) n_total += active(slots[k]);
   int64_t item_size = (n_total + eval_slots - 1) / std::max(eval_slots, 1);
   item_size = std::max<int64_t>(GLIO_ITEM_MAX, ((item_size + 255) / 256) * 256);
+  ItemPlan<EvalItem> plan(W);
   for (int k = 0; k < W; ++k) {
-    start[k] = (int)items.size();
-    if (!slots[k]) continue;
-    const Slot& sl = *slots[k];
-    const bool sel = sl.n_sel >= 0;
-    const int64_t n = sel ? sl.n_sel : sl.n_match;
-    const float4* cpw = sel ? sl.s_cpw.p : sl.m_cpw.p;
-    const float4* nsd = sel ? sl.s_nsd.p : sl.m_nsd.p;
+    const Slot* sl = slots[k];
+    const int64_t n = active(sl);
     const int64_t parts = std::max<int64_t>(1, (n + item_size - 1) / item_size);
     const int64_t per = ((n + parts - 1) / parts + 255) / 256 * 256;      // equal, 256-aligned parts
-    for (int64_t o = 0; o < n; o += per) {
-      EvalItem it; it.cpw = cpw + o; it.nsd = nsd + o; it.count = (int32_t)std::min<int64_t>(per, n - o); it.kf = k;
-      items.push_back(it);
-    }
+    plan.cut(k, n, per, [&](int64_t f, int32_t count) {
+      const bool sel = sl->n_sel >= 0;
+      return EvalItem{(sel ? sl->s_cpw.p : sl->m_cpw.p) + f, (sel ? sl->s_nsd.p : sl->m_nsd.p) + f, count, k};
+    });
   }
-  start[W] = (int)items.size();
-  return items;
+  return plan;
 }
 
 // The work items of one evaluation target in device memory, and the constants its residuals are evaluated with.
@@ -426,28 +447,22 @@ struct EvalTarget {
   EvalParams ep;
 };
 
-// uploads planned items into the given device buffers; reserves the context's per-evaluation buffers for W keyframes
-void upload_items(glio_ctx* c, int W, const std::vector<EvalItem>& items, const std::vector<int>& start, DevBuf<EvalItem>& d_items,
-                  DevBuf<int>& d_start, DevBuf<double>& d_partials) {
-  d_items.reserve(items.size() + 1); d_start.reserve(W + 1);
-  d_partials.reserve((items.size() + 1) * GLIO_NACC);
+// uploads a K2 plan into the given device buffers; reserves the context's per-evaluation buffers for W keyframes
+void upload_items(glio_ctx* c, int W, const ItemPlan<EvalItem>& plan, DevBuf<EvalItem>& d_items, DevBuf<int>& d_start,
+                  DevBuf<double>& d_partials) {
   c->d_out.reserve((size_t)W * GLIO_NACC); c->h_out.reserve((size_t)W * GLIO_NACC);
   c->d_poses.reserve((size_t)W * 7); c->h_poses.reserve((size_t)W * 7);
-  if (!c->d_ticket.p) { c->d_ticket.reserve(1); GLIO_CUDA_TRY(cudaMemsetAsync(c->d_ticket.p, 0, sizeof(unsigned int), c->st)); }
-  if (!items.empty())
-    GLIO_CUDA_TRY(cudaMemcpyAsync(d_items.p, items.data(), items.size() * sizeof(EvalItem), cudaMemcpyHostToDevice, c->st));
-  GLIO_CUDA_TRY(cudaMemcpyAsync(d_start.p, start.data(), (W + 1) * sizeof(int), cudaMemcpyHostToDevice, c->st));
-  GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));   // items/start are stack vectors
+  init_ticket(c);
+  plan.upload(c, d_items, d_start, d_partials, GLIO_NACC);
 }
 
 void build_items(glio_ctx* c, int W) {
   if (!c->items_dirty && c->items_W == W) return;
   std::vector<const Slot*> sl(W, nullptr);
   for (int k = 0; k < W && (size_t)k < c->slots.size(); ++k) sl[k] = c->slots[k].get();
-  std::vector<int> start;
-  const std::vector<EvalItem> items = plan_items(sl, c->eval_slots, start);
-  c->n_items = (int)items.size();
-  upload_items(c, W, items, start, c->d_items, c->d_kf_item_start, c->d_partials);
+  const ItemPlan<EvalItem> plan = plan_items(sl, c->eval_slots);
+  c->n_items = (int)plan.items.size();
+  upload_items(c, W, plan, c->d_items, c->d_kf_item_start, c->d_partials);
   c->items_dirty = false;
   c->items_W = W;
 }
@@ -510,38 +525,27 @@ void wait_marg_copied(glio_ctx* c) {
   }
 }
 
-// K2e work items of slots 0..W-1 (GLIO_ITEM_MAX residuals each, keyframe order); start[k] = first item of keyframe k
-std::vector<EdgeItem> plan_edge_items(const glio_ctx* c, int W, std::vector<int>& start) {
-  std::vector<EdgeItem> items;
-  start.assign(W + 1, 0);
+// K2e work items of slots 0..W-1 (GLIO_ITEM_MAX residuals each, keyframe order)
+ItemPlan<EdgeItem> plan_edge_items(const glio_ctx* c, int W) {
+  ItemPlan<EdgeItem> plan(W);
   for (int k = 0; k < W; ++k) {
-    start[k] = (int)items.size();
-    if ((size_t)k >= c->slots.size() || !c->slots[k]) continue;
-    const EdgeList& e = c->slots[k]->edges;
-    for (int64_t o = 0; o < e.n; o += GLIO_ITEM_MAX) {
-      EdgeItem it; it.cps = e.cps.p + o; it.pa = e.pa.p + o; it.pb = e.pb.p + o;
-      it.count = (int32_t)std::min<int64_t>(GLIO_ITEM_MAX, e.n - o); it.kf = k; items.push_back(it);
-    }
+    const EdgeList* e = (size_t)k < c->slots.size() && c->slots[k] ? &c->slots[k]->edges : nullptr;
+    plan.cut(k, e ? e->n : 0, GLIO_ITEM_MAX, [&](int64_t f, int32_t count) { return EdgeItem{e->cps.p + f, e->pa.p + f, e->pb.p + f, count, k}; });
   }
-  start[W] = (int)items.size();
-  return items;
+  return plan;
 }
 
 // Queues the edge blocks of one solve / marginalisation evaluation (poses already in c->h_poses): the pose upload, K2e and the copy
 // of its result into c->h_eout, all on the main stream ahead of K2.  Returns false when slots 0..W-1 hold no edge.
 bool edge_blocks_launch(glio_ctx* c, int W, int jac_kind, bool want_jac) {
   if (c->edge_items_dirty || c->edge_items_W != W) {
-    std::vector<int> start;
-    const std::vector<EdgeItem> items = plan_edge_items(c, W, start);
-    c->se_items.reserve(items.size() + 1); c->se_start.reserve(W + 1); c->se_part.reserve((items.size() + 1) * GLIO_NACC);
-    if (!items.empty()) GLIO_CUDA_TRY(cudaMemcpyAsync(c->se_items.p, items.data(), items.size() * sizeof(EdgeItem), cudaMemcpyHostToDevice, c->st));
-    GLIO_CUDA_TRY(cudaMemcpyAsync(c->se_start.p, start.data(), (W + 1) * sizeof(int), cudaMemcpyHostToDevice, c->st));
-    GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));   // items / start are stack vectors
-    c->n_edge_items = (int)items.size(); c->edge_items_W = W; c->edge_items_dirty = false;
+    const ItemPlan<EdgeItem> plan = plan_edge_items(c, W);
+    plan.upload(c, c->se_items, c->se_start, c->se_part, GLIO_NACC);
+    c->n_edge_items = (int)plan.items.size(); c->edge_items_W = W; c->edge_items_dirty = false;
   }
   if (c->n_edge_items == 0) return false;
   c->se_out.reserve((size_t)W * GLIO_NACC); c->se_poses.reserve((size_t)W * 7); c->h_eout.reserve((size_t)W * GLIO_NACC);
-  if (!c->d_ticket.p) { c->d_ticket.reserve(1); GLIO_CUDA_TRY(cudaMemsetAsync(c->d_ticket.p, 0, sizeof(unsigned int), c->st)); }
+  init_ticket(c);
   GLIO_CUDA_TRY(cudaMemcpyAsync(c->se_poses.p, c->h_poses.p, (size_t)W * 7 * sizeof(double), cudaMemcpyHostToDevice, c->st));
   eval_edge_run(c->se_items.p, c->n_edge_items, W, c->se_poses.p, eval_params(c), jac_kind, want_jac, c->se_part.p, c->se_out.p, c->se_start.p,
                 c->d_ticket.p, c->st, c->lc);
@@ -2103,39 +2107,29 @@ namespace {
 void build_bin_items(glio_ctx* c, int K) {
   if (!c->bin_dirty && c->bin_K == K) return;
   const int P = (int)c->pairs.size();
-  std::vector<BinItem> items;
-  std::vector<int> pstart(P + 1, 0);
+  ItemPlan<BinItem> plan(P);
   std::vector<std::vector<BinIncidence>> inc(K);
   for (int p = 0; p < P; ++p) {
-    glio_ctx::Pair& pr = *c->pairs[p];
+    const glio_ctx::Pair& pr = *c->pairs[p];
     GLIO_REQUIRE(pr.cur >= 0 && pr.oth >= 0 && pr.cur < K && pr.oth < K, GLIO_ERR_ARG, "pair references a keyframe outside [0, K)");
-    pstart[p] = (int)items.size();
     const bool sel = pr.n_sel >= 0;
-    const int64_t n = sel ? pr.n_sel : pr.n_match;
     const float4* cpw = sel ? pr.s_cpw.p : pr.m_cpw.p;
     const double* nc = sel ? pr.s_nc.p : pr.m_nc.p;
-    for (int64_t o = 0; o < n; o += GLIO_ITEM_MAX) {
-      BinItem it; it.cpw = cpw + o; it.nc = nc + 6 * o; it.count = (int32_t)std::min<int64_t>(GLIO_ITEM_MAX, n - o); it.kf_c = pr.cur; it.kf_o = pr.oth;
-      items.push_back(it);
-    }
+    plan.cut(p, sel ? pr.n_sel : pr.n_match, GLIO_ITEM_MAX, [&](int64_t f, int32_t count) { return BinItem{cpw + f, nc + 6 * f, count, pr.cur, pr.oth}; });
     inc[pr.cur].push_back(BinIncidence{p, 0});
     inc[pr.oth].push_back(BinIncidence{p, 1});
   }
-  pstart[P] = (int)items.size();
   std::vector<int> kstart(K + 1, 0);
   std::vector<BinIncidence> flat;
   for (int k = 0; k < K; ++k) { kstart[k] = (int)flat.size(); flat.insert(flat.end(), inc[k].begin(), inc[k].end()); }
   kstart[K] = (int)flat.size();
-  c->n_bin_items = (int)items.size();
-  c->d_bin_items.reserve(items.size() + 1); c->d_pair_item_start.reserve(P + 1); c->d_kf_inc_start.reserve(K + 1); c->d_inc.reserve(flat.size() + 1);
-  c->d_bin_partials.reserve((items.size() + 1) * GLIO_NACC_BIN); c->d_pair_sums.reserve((size_t)(P + 1) * GLIO_NACC_BIN);
+  c->n_bin_items = (int)plan.items.size();
+  c->d_kf_inc_start.reserve(K + 1); c->d_inc.reserve(flat.size() + 1); c->d_pair_sums.reserve((size_t)(P + 1) * GLIO_NACC_BIN);
   c->d_bin_diag.reserve((size_t)K * GLIO_NACC); c->d_bin_off.reserve((size_t)(P + 1) * 36); c->d_bin_poses.reserve((size_t)K * 7);
   c->h_bin_diag.reserve((size_t)K * GLIO_NACC); c->h_bin_off.reserve((size_t)(P + 1) * 36); c->h_bin_poses.reserve((size_t)K * 7);
-  if (!items.empty()) GLIO_CUDA_TRY(cudaMemcpyAsync(c->d_bin_items.p, items.data(), items.size() * sizeof(BinItem), cudaMemcpyHostToDevice, c->st));
-  GLIO_CUDA_TRY(cudaMemcpyAsync(c->d_pair_item_start.p, pstart.data(), (P + 1) * sizeof(int), cudaMemcpyHostToDevice, c->st));
   GLIO_CUDA_TRY(cudaMemcpyAsync(c->d_kf_inc_start.p, kstart.data(), (K + 1) * sizeof(int), cudaMemcpyHostToDevice, c->st));
   if (!flat.empty()) GLIO_CUDA_TRY(cudaMemcpyAsync(c->d_inc.p, flat.data(), flat.size() * sizeof(BinIncidence), cudaMemcpyHostToDevice, c->st));
-  GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
+  plan.upload(c, c->d_bin_items, c->d_pair_item_start, c->d_bin_partials, GLIO_NACC_BIN);   // its synchronisation covers kstart / flat
   c->bin_dirty = false; c->bin_K = K;
 }
 
@@ -2144,25 +2138,15 @@ void build_bin_items(glio_ctx* c, int K) {
 void build_bedge_items(glio_ctx* c, int K) {
   const int P = (int)c->pairs.size();
   if (!c->bedge_dirty && c->bedge_K == K && c->bedge_P == P) return;
-  std::vector<BinEdgeItem> items;
-  std::vector<int> pstart(P + 1, 0);
+  ItemPlan<BinEdgeItem> plan(P);
   for (int p = 0; p < P; ++p) {
     const glio_ctx::Pair& pr = *c->pairs[p];
     const EdgeList& e = pr.edges;
-    pstart[p] = (int)items.size();
-    for (int64_t o = 0; o < e.n; o += GLIO_ITEM_MAX) {
-      BinEdgeItem it; it.cps = e.cps.p + o; it.pa = e.pa.p + o; it.pb = e.pb.p + o;
-      it.count = (int32_t)std::min<int64_t>(GLIO_ITEM_MAX, e.n - o); it.kf_c = pr.cur; it.kf_o = pr.oth;
-      items.push_back(it);
-    }
+    plan.cut(p, e.n, GLIO_ITEM_MAX, [&](int64_t f, int32_t count) { return BinEdgeItem{e.cps.p + f, e.pa.p + f, e.pb.p + f, count, pr.cur, pr.oth}; });
   }
-  pstart[P] = (int)items.size();
-  c->n_bedge_items = (int)items.size();
-  c->d_bedge_items.reserve(items.size() + 1); c->d_bedge_pstart.reserve(P + 1);
-  c->d_bedge_partials.reserve((items.size() + 1) * GLIO_NACC_BIN); c->d_bedge_sums.reserve((size_t)(P + 1) * GLIO_NACC_BIN);
-  if (!items.empty()) GLIO_CUDA_TRY(cudaMemcpyAsync(c->d_bedge_items.p, items.data(), items.size() * sizeof(BinEdgeItem), cudaMemcpyHostToDevice, c->st));
-  GLIO_CUDA_TRY(cudaMemcpyAsync(c->d_bedge_pstart.p, pstart.data(), (P + 1) * sizeof(int), cudaMemcpyHostToDevice, c->st));
-  GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
+  c->n_bedge_items = (int)plan.items.size();
+  c->d_bedge_sums.reserve((size_t)(P + 1) * GLIO_NACC_BIN);
+  plan.upload(c, c->d_bedge_items, c->d_bedge_pstart, c->d_bedge_partials, GLIO_NACC_BIN);
   c->bedge_dirty = false; c->bedge_K = K; c->bedge_P = P;
 }
 
@@ -2187,8 +2171,8 @@ void eval_binary_launch(glio_ctx* c, int K, const double* poses, bool want_jac, 
     bin_assemble_run(c->d_bedge_sums.p, K, P, c->d_kf_inc_start.p, c->d_inc.p, want_jac, c->d_bin_diag.p, c->d_bin_off.p, c->st, c->lc);
   else
     eval_binary_run(c->d_bin_items.p, c->n_bin_items, c->d_pair_item_start.p, P, K, c->d_bin_poses.p, c->prm.batch_score, huber, want_jac,
-                    c->d_bin_partials.p, c->d_pair_sums.p, c->d_kf_inc_start.p, c->d_inc.p, c->d_bin_diag.p, c->d_bin_off.p, nullptr, c->st,
-                    c->lc, add_edges ? c->d_bedge_sums.p : nullptr);
+                    c->d_bin_partials.p, c->d_pair_sums.p, c->d_kf_inc_start.p, c->d_inc.p, c->d_bin_diag.p, c->d_bin_off.p, c->st, c->lc,
+                    add_edges ? c->d_bedge_sums.p : nullptr);
   if (c->allreduce) {
     // keyframe-sharded evaluation: every rank holds the same pair list but only its own pairs carry residuals;
     // one sum over ranks of the pose-block buffers per evaluation (SURVEY 8e "pose-block allreduce")
@@ -2356,18 +2340,17 @@ static int eval_edge_impl(glio_ctx* c, int W, const double* poses_body, int jac_
   return guarded(c, [&] {
     GLIO_REQUIRE(W > 0 && W <= 4096 && poses_body, GLIO_ERR_ARG, "bad arguments");
     GLIO_REQUIRE(jac_kind == 0 || jac_kind == 1, GLIO_ERR_ARG, "jac_kind must be 0 or 1");
-    std::vector<int> start;
-    const std::vector<EdgeItem> items = plan_edge_items(c, W, start);
-    DevBuf<EdgeItem>& d_items = c->e_items; DevBuf<int>& d_start = c->e_start; DevBuf<double>& d_part = c->e_part; DevBuf<double>& d_out = c->e_out; DevBuf<double>& d_poses = c->e_poses;
-    d_items.reserve(items.size() + 1); d_start.reserve(W + 1); d_part.reserve((items.size() + 1) * GLIO_NACC); d_out.reserve((size_t)W * GLIO_NACC); d_poses.reserve((size_t)W * 7);
-    if (!c->d_ticket.p) { c->d_ticket.reserve(1); GLIO_CUDA_TRY(cudaMemsetAsync(c->d_ticket.p, 0, sizeof(unsigned int), c->st)); }
-    if (!items.empty()) GLIO_CUDA_TRY(cudaMemcpyAsync(d_items.p, items.data(), items.size() * sizeof(EdgeItem), cudaMemcpyHostToDevice, c->st));
-    GLIO_CUDA_TRY(cudaMemcpyAsync(d_start.p, start.data(), (W + 1) * sizeof(int), cudaMemcpyHostToDevice, c->st));
-    GLIO_CUDA_TRY(cudaMemcpyAsync(d_poses.p, poses_body, (size_t)W * 7 * sizeof(double), cudaMemcpyHostToDevice, c->st));
+    // its own buffers: the solve path's cached K2e plan and h_eout stay untouched
+    const ItemPlan<EdgeItem> plan = plan_edge_items(c, W);
+    plan.upload(c, c->e_items, c->e_start, c->e_part, GLIO_NACC);
+    c->e_out.reserve((size_t)W * GLIO_NACC); c->e_poses.reserve((size_t)W * 7);
+    init_ticket(c);
+    GLIO_CUDA_TRY(cudaMemcpyAsync(c->e_poses.p, poses_body, (size_t)W * 7 * sizeof(double), cudaMemcpyHostToDevice, c->st));
     const bool want_jac = H || g;
-    eval_edge_run(d_items.p, (int)items.size(), W, d_poses.p, eval_params(c), jac_kind, want_jac, d_part.p, d_out.p, d_start.p, c->d_ticket.p, c->st, c->lc);
+    eval_edge_run(c->e_items.p, (int)plan.items.size(), W, c->e_poses.p, eval_params(c), jac_kind, want_jac, c->e_part.p, c->e_out.p, c->e_start.p,
+                  c->d_ticket.p, c->st, c->lc);
     std::vector<double> ho((size_t)W * GLIO_NACC);
-    GLIO_CUDA_TRY(cudaMemcpyAsync(ho.data(), d_out.p, ho.size() * sizeof(double), cudaMemcpyDeviceToHost, c->st));
+    GLIO_CUDA_TRY(cudaMemcpyAsync(ho.data(), c->e_out.p, ho.size() * sizeof(double), cudaMemcpyDeviceToHost, c->st));
     GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
     unpack_blocks(ho.data(), W, H, g, cost);
   });
@@ -2506,10 +2489,9 @@ void odom_step(glio_odom* o, const float4* surf, int64_t n_surf, const float4* f
           associate_slots(c, o->grid, gates, false, std::vector<Slot*>{&o->slot}, std::vector<std::array<double, 7>>{lp}, &nm);
         }
         if (nm > 0) {
-          std::vector<int> start;
-          const std::vector<EvalItem> items = plan_items(std::vector<const Slot*>{&o->slot}, c->eval_slots, start);
-          upload_items(c, 1, items, start, o->d_items, o->d_start, o->d_partials);
-          const EvalTarget tgt{o->d_items.p, (int)items.size(), o->d_start.p, o->d_partials.p, ep};
+          const ItemPlan<EvalItem> plan = plan_items(std::vector<const Slot*>{&o->slot}, c->eval_slots);
+          upload_items(c, 1, plan, o->d_items, o->d_start, o->d_partials);
+          const EvalTarget tgt{o->d_items.p, (int)plan.items.size(), o->d_start.p, o->d_partials.p, ep};
           solve_core(c, 1, x, nullptr, nullptr, nullptr, -1, nullptr, sopt, &tgt, S);
         } else {
           // no residual uses the pose: Ceres drops the parameter blocks and Minimize returns at once (solver.cc:410-418)

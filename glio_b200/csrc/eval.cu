@@ -7,9 +7,10 @@
 //
 // HBM traffic per unary residual: 2 x 16 B loads (cp+weight, weight*n + weight*d) = 32 B; outputs are W x 28 doubles.
 // Arithmetic is fp64 (tolerance 1e-8 rad per iteration), inputs fp32 as the reference stores them (quirk Q5).
-// Reduction: per-thread register accumulators over a run of one keyframe's residuals -> warp shuffle -> shared ->
-// one partial per work item; the last block to finish sums the partials per keyframe in a fixed order
-// (deterministic, no floating-point atomics).
+// Reduction: per-thread register accumulators over a run of one keyframe's (or pair's) residuals -> warp shuffle -> shared ->
+// one partial per work item (block_partials); for the unary kernels the last block to finish sums the partials per keyframe in
+// a fixed order (kf_sums; deterministic, no floating-point atomics).  The frame set-ups (kf_frame, pair_frame), the plane
+// residual (plane_residual) and the binary 55-sum layout (pair_accumulate) are shared by the kernels below.
 #include "common.cuh"
 
 namespace glio {
@@ -50,7 +51,7 @@ __device__ __forceinline__ double huber_scale(double r, double delta, double& sc
 }
 
 constexpr int EV_T = 256;
-constexpr int NACC = 28;   // 21 upper-triangular H + 6 g + 1 cost
+constexpr int NACC = GLIO_NACC;   // 21 upper-triangular H + 6 g + 1 cost
 
 struct KfFrame {           // per keyframe, prepared in shared memory
   double M[9];             // R(q) * R(q_lb)^-1   (maps cp - t_lb to the rotated body point a)
@@ -59,125 +60,50 @@ struct KfFrame {           // per keyframe, prepared in shared memory
   double q[4];
 };
 
-// per-residual math of the unary plane factor; M, t (and R_lb^-1, q for the marginalisation variant) live in registers
-template <bool WANT_JAC, int JAC_KIND>
-__device__ __forceinline__ void unary_accumulate(const float4 c4, const float4 n4, const double (&M)[9], const double (&t)[3],
-                                                 const KfFrame& F, const EvalParams& ep, double (&acc)[NACC]) {
-  const double s = ep.unit_score ? ep.lidar_const : ep.lidar_const * (double)c4.w;   // Estimator.cpp:3692 score = lidar_const*weight; front end: no score
-  const double dx = (double)c4.x - ep.t_lb[0], dy = (double)c4.y - ep.t_lb[1], dz = (double)c4.z - ep.t_lb[2];
-  double a[3]; mat_vec3(M, dx, dy, dz, a);                   // a = R(q) q_lb^-1 (cp - t_lb)
-  const double nx = (double)n4.x, ny = (double)n4.y, nz = (double)n4.z;
-  double r = s * (nx * (a[0] + t[0]) + ny * (a[1] + t[1]) + nz * (a[2] + t[2]) + (double)n4.w);
-  double scale;
-  acc[27] += huber_scale(r, ep.huber_delta, scale);
-  if (WANT_JAC) {
-    double J[6];
-    const double ss = s * scale;
-    J[0] = ss * nx; J[1] = ss * ny; J[2] = ss * nz;
-    if (JAC_KIND == 0) {
-      // tangent (Ceres QuaternionParameterization):  2 s (a x n)
-      const double s2 = 2.0 * ss;
-      J[3] = s2 * (a[1] * nz - a[2] * ny);
-      J[4] = s2 * (a[2] * nx - a[0] * nz);
-      J[5] = s2 * (a[0] * ny - a[1] * nx);
-    } else {
-      // ambient x,y,z columns (MarginalizationFactor.cpp:9-12):
-      //   s [ 2w (p_b x n) + 2( (u.p_b) n + (n.u) p_b - 2 (n.p_b) u ) ]
-      double pb[3]; mat_vec3(F.Rlbi, dx, dy, dz, pb);
-      const double w = F.q[0], ux = F.q[1], uy = F.q[2], uz = F.q[3];
-      const double udp = ux * pb[0] + uy * pb[1] + uz * pb[2];
-      const double ndu = nx * ux + ny * uy + nz * uz;
-      const double ndp = nx * pb[0] + ny * pb[1] + nz * pb[2];
-      J[3] = ss * (2.0 * w * (pb[1] * nz - pb[2] * ny) + 2.0 * (udp * nx + ndu * pb[0] - 2.0 * ndp * ux));
-      J[4] = ss * (2.0 * w * (pb[2] * nx - pb[0] * nz) + 2.0 * (udp * ny + ndu * pb[1] - 2.0 * ndp * uy));
-      J[5] = ss * (2.0 * w * (pb[0] * ny - pb[1] * nx) + 2.0 * (udp * nz + ndu * pb[2] - 2.0 * ndp * uz));
-    }
-    r *= scale;
-    int k = 0;
-#pragma unroll
-    for (int p = 0; p < 6; ++p)
-#pragma unroll
-      for (int c = p; c < 6; ++c) acc[k++] += J[p] * J[c];
-#pragma unroll
-    for (int p = 0; p < 6; ++p) acc[21 + p] += J[p] * r;
-  }
+// F from the pose P = (t, q) of one keyframe.  STORE_Q: also keep q (the ambient quaternion columns read it); the cost-only and
+// tangent K2e kernels leave it out, which keeps k_eval_edge<false, 0> at 60 registers.
+template <bool STORE_Q>
+__device__ __forceinline__ void kf_frame(const double* P, const EvalParams& ep, KfFrame& F) {
+  double qn[4] = {P[3], P[4], P[5], P[6]};
+  double R[9]; quat_to_mat(qn, R);
+  // q_lb^-1 = conj / |q|^2 (Eigen inverse()); rotation by it as the polynomial in its coefficients
+  const double n2 = ep.q_lb[0] * ep.q_lb[0] + ep.q_lb[1] * ep.q_lb[1] + ep.q_lb[2] * ep.q_lb[2] + ep.q_lb[3] * ep.q_lb[3];
+  double qi[4] = {ep.q_lb[0] / n2, -ep.q_lb[1] / n2, -ep.q_lb[2] / n2, -ep.q_lb[3] / n2};
+  quat_to_mat(qi, F.Rlbi);
+  mat_mul3(R, F.Rlbi, F.M);
+  F.t[0] = P[0]; F.t[1] = P[1]; F.t[2] = P[2];
+  if (STORE_Q) { F.q[0] = qn[0]; F.q[1] = qn[1]; F.q[2] = qn[2]; F.q[3] = qn[3]; }
 }
 
-// One block per work item (a run of one keyframe's residuals, sized so the whole launch is about one wave of
-// 2 blocks/SM).  Loads are issued two iterations ahead of their use (4 x 16 B in flight per thread).
-// poses of up to EV_MAXW keyframes travel in the kernel parameters (no host-to-device copy on the per-iteration path)
-struct PoseArgs { double p[EV_MAXW * 7]; };
-
-#ifndef GLIO_EVAL_MINBLOCKS
-#define GLIO_EVAL_MINBLOCKS 2
-#endif
-template <bool WANT_JAC, int JAC_KIND, bool POSE_ARGS>
-__global__ void __launch_bounds__(EV_T, GLIO_EVAL_MINBLOCKS) k_eval_unary(const EvalItem* __restrict__ items, int nitems, int W,
-                                                        const double* __restrict__ poses, const __grid_constant__ PoseArgs pa, EvalParams ep,
-                                                        double* __restrict__ partials, double* __restrict__ out,
-                                                        const int* __restrict__ kf_item_start, unsigned int* __restrict__ ticket,
-                                                        unsigned int* done_flag, unsigned int epoch) {
-  __shared__ KfFrame F;
-  __shared__ double red[EV_T / 32][NACC];
-  __shared__ bool is_last;
-  const EvalItem it = items[blockIdx.x];
-  if (threadIdx.x == 0) {
-    const double* P = POSE_ARGS ? pa.p + 7 * it.kf : poses + 7 * it.kf;
-    double qn[4] = {P[3], P[4], P[5], P[6]};
-    double R[9]; quat_to_mat(qn, R);
-    // q_lb^-1 = conj / |q|^2 (Eigen inverse()); rotation by it as the polynomial in its coefficients
-    const double n2 = ep.q_lb[0] * ep.q_lb[0] + ep.q_lb[1] * ep.q_lb[1] + ep.q_lb[2] * ep.q_lb[2] + ep.q_lb[3] * ep.q_lb[3];
-    double qi[4] = {ep.q_lb[0] / n2, -ep.q_lb[1] / n2, -ep.q_lb[2] / n2, -ep.q_lb[3] / n2};
-    quat_to_mat(qi, F.Rlbi);
-    mat_mul3(R, F.Rlbi, F.M);
-    F.t[0] = P[0]; F.t[1] = P[1]; F.t[2] = P[2];
-    F.q[0] = qn[0]; F.q[1] = qn[1]; F.q[2] = qn[2]; F.q[3] = qn[3];
-  }
-  __syncthreads();
-  double M[9], t[3];
-#pragma unroll
-  for (int k = 0; k < 9; ++k) M[k] = F.M[k];
-#pragma unroll
-  for (int k = 0; k < 3; ++k) t[k] = F.t[k];
-
-  double acc[NACC];
-#pragma unroll
-  for (int k = 0; k < NACC; ++k) acc[k] = 0.0;
-
-  const int n = it.count;
-  int i = threadIdx.x;
-  // software pipeline, depth 2
-  float4 c0, n0, c1, n1;
-  if (i < n) { c0 = __ldg(&it.cpw[i]); n0 = __ldg(&it.nsd[i]); }
-  if (i + EV_T < n) { c1 = __ldg(&it.cpw[i + EV_T]); n1 = __ldg(&it.nsd[i + EV_T]); }
-  for (; i < n; i += 2 * EV_T) {
-    const float4 ca = c0, na = n0, cb = c1, nb = n1;
-    const bool has_b = i + EV_T < n;
-    if (i + 2 * EV_T < n) { c0 = __ldg(&it.cpw[i + 2 * EV_T]); n0 = __ldg(&it.nsd[i + 2 * EV_T]); }
-    if (i + 3 * EV_T < n) { c1 = __ldg(&it.cpw[i + 3 * EV_T]); n1 = __ldg(&it.nsd[i + 3 * EV_T]); }
-    unary_accumulate<WANT_JAC, JAC_KIND>(ca, na, M, t, F, ep, acc);
-    if (has_b) unary_accumulate<WANT_JAC, JAC_KIND>(cb, nb, M, t, F, ep, acc);
-  }
-
-  // block reduction
+// Reduces the NS per-thread sums of an NT-thread block (shuffle -> shared red -> one partial per block at
+// partials[blockIdx.x * NS]).  The last sum is the cost; without WANT_JAC it is the only one reduced, the others are written as 0.
+template <int NS, int NT, bool WANT_JAC>
+__device__ __forceinline__ void block_partials(const double (&acc)[NS], double (&red)[NT / 32][NS], double* __restrict__ partials) {
+  constexpr int COST = NS - 1;
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
 #pragma unroll
-  for (int k = WANT_JAC ? 0 : 27; k < NACC; ++k) {
+  for (int k = WANT_JAC ? 0 : COST; k < NS; ++k) {
     double v = acc[k];
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
     if (lane == 0) red[wid][k] = v;
   }
   __syncthreads();
-  if (threadIdx.x < NACC) {
+  if (threadIdx.x < NS) {
     double v = 0.0;
-    if (WANT_JAC || threadIdx.x == 27) {
+    if (WANT_JAC || threadIdx.x == COST) {
 #pragma unroll
-      for (int w8 = 0; w8 < EV_T / 32; ++w8) v += red[w8][threadIdx.x];
+      for (int w = 0; w < NT / 32; ++w) v += red[w][threadIdx.x];
     }
-    partials[(size_t)blockIdx.x * NACC + threadIdx.x] = v;
+    partials[(size_t)blockIdx.x * NS + threadIdx.x] = v;
   }
-  // last block: sum the partials per keyframe, in item order
+}
+
+// After block_partials: the block that takes the last ticket sums the partials per keyframe into out (W x NACC), in item order,
+// then runs last_block() (every thread), which resets the ticket for the next launch.  is_last: the kernel's shared flag.
+template <class LastBlock>
+__device__ __forceinline__ void kf_sums(const double* __restrict__ partials, double* __restrict__ out, int W, const int* __restrict__ kf_item_start,
+                                        unsigned int* __restrict__ ticket, int nitems, bool& is_last, LastBlock last_block) {
   __threadfence();
   __syncthreads();
   if (threadIdx.x == 0) {
@@ -204,11 +130,124 @@ __global__ void __launch_bounds__(EV_T, GLIO_EVAL_MINBLOCKS) k_eval_unary(const 
       for (; b < b1; ++b) v += __ldcg(&partials[(size_t)b * NACC + k]);
       out[o] = v;
     }
+    last_block();
+  }
+}
+
+// One plane residual of the unary factor: adds its block cost to cost; r (before the Huber scale), the scale, and with WANT_JAC
+// the scaled Jacobian row J.  M, t may live in registers or in F; R_lb^-1 and q (ambient columns) are read from F.
+template <bool WANT_JAC, int JAC_KIND>
+__device__ __forceinline__ void plane_residual(const float4 c4, const float4 n4, const double (&M)[9], const double (&t)[3], const KfFrame& F,
+                                               const EvalParams& ep, double& cost, double& r, double& scale, double (&J)[6]) {
+  const double s = ep.unit_score ? ep.lidar_const : ep.lidar_const * (double)c4.w;   // Estimator.cpp:3692 score = lidar_const*weight; front end: no score
+  const double dx = (double)c4.x - ep.t_lb[0], dy = (double)c4.y - ep.t_lb[1], dz = (double)c4.z - ep.t_lb[2];
+  double a[3]; mat_vec3(M, dx, dy, dz, a);                   // a = R(q) q_lb^-1 (cp - t_lb)
+  const double nx = (double)n4.x, ny = (double)n4.y, nz = (double)n4.z;
+  r = s * (nx * (a[0] + t[0]) + ny * (a[1] + t[1]) + nz * (a[2] + t[2]) + (double)n4.w);
+  cost += huber_scale(r, ep.huber_delta, scale);
+  if (WANT_JAC) {
+    const double ss = s * scale;
+    J[0] = ss * nx; J[1] = ss * ny; J[2] = ss * nz;
+    if (JAC_KIND == 0) {
+      // tangent (Ceres QuaternionParameterization):  2 s (a x n)
+      const double s2 = 2.0 * ss;
+      J[3] = s2 * (a[1] * nz - a[2] * ny);
+      J[4] = s2 * (a[2] * nx - a[0] * nz);
+      J[5] = s2 * (a[0] * ny - a[1] * nx);
+    } else {
+      // ambient x,y,z columns (MarginalizationFactor.cpp:9-12):
+      //   s [ 2w (p_b x n) + 2( (u.p_b) n + (n.u) p_b - 2 (n.p_b) u ) ]
+      double pb[3]; mat_vec3(F.Rlbi, dx, dy, dz, pb);
+      const double w = F.q[0], ux = F.q[1], uy = F.q[2], uz = F.q[3];
+      const double udp = ux * pb[0] + uy * pb[1] + uz * pb[2];
+      const double ndu = nx * ux + ny * uy + nz * uz;
+      const double ndp = nx * pb[0] + ny * pb[1] + nz * pb[2];
+      J[3] = ss * (2.0 * w * (pb[1] * nz - pb[2] * ny) + 2.0 * (udp * nx + ndu * pb[0] - 2.0 * ndp * ux));
+      J[4] = ss * (2.0 * w * (pb[2] * nx - pb[0] * nz) + 2.0 * (udp * ny + ndu * pb[1] - 2.0 * ndp * uy));
+      J[5] = ss * (2.0 * w * (pb[0] * ny - pb[1] * nx) + 2.0 * (udp * nz + ndu * pb[2] - 2.0 * ndp * uz));
+    }
+  }
+}
+
+// the 21 upper-triangular J^T J and 6 J^T r sums of one scaled residual r with Jacobian row J
+__device__ __forceinline__ void unary_sums(const double (&J)[6], double r, double (&acc)[NACC]) {
+  int k = 0;
+#pragma unroll
+  for (int p = 0; p < 6; ++p)
+#pragma unroll
+    for (int c = p; c < 6; ++c) acc[k++] += J[p] * J[c];
+#pragma unroll
+  for (int p = 0; p < 6; ++p) acc[21 + p] += J[p] * r;
+}
+
+// per-residual math of the unary plane factor; M, t (and R_lb^-1, q for the marginalisation variant) live in registers
+template <bool WANT_JAC, int JAC_KIND>
+__device__ __forceinline__ void unary_accumulate(const float4 c4, const float4 n4, const double (&M)[9], const double (&t)[3],
+                                                 const KfFrame& F, const EvalParams& ep, double (&acc)[NACC]) {
+  double r, scale, J[6];
+  plane_residual<WANT_JAC, JAC_KIND>(c4, n4, M, t, F, ep, acc[27], r, scale, J);
+  if (WANT_JAC) unary_sums(J, r * scale, acc);
+}
+
+// One block per work item (a run of one keyframe's residuals, sized so the whole launch is about one wave of
+// 2 blocks/SM).  Loads are issued two iterations ahead of their use (4 x 16 B in flight per thread).
+// poses of up to EV_MAXW keyframes travel in the kernel parameters (no host-to-device copy on the per-iteration path)
+struct PoseArgs { double p[EV_MAXW * 7]; };
+
+#ifndef GLIO_EVAL_MINBLOCKS
+#define GLIO_EVAL_MINBLOCKS 2
+#endif
+template <bool WANT_JAC, int JAC_KIND, bool POSE_ARGS>
+__global__ void __launch_bounds__(EV_T, GLIO_EVAL_MINBLOCKS) k_eval_unary(const EvalItem* __restrict__ items, int nitems, int W,
+                                                        const double* __restrict__ poses, const __grid_constant__ PoseArgs pa, EvalParams ep,
+                                                        double* __restrict__ partials, double* __restrict__ out,
+                                                        const int* __restrict__ kf_item_start, unsigned int* __restrict__ ticket,
+                                                        unsigned int* done_flag, unsigned int epoch) {
+  __shared__ KfFrame F;
+  __shared__ double red[EV_T / 32][NACC];
+  __shared__ bool is_last;
+  const EvalItem it = items[blockIdx.x];
+  if (threadIdx.x == 0) kf_frame<true>(POSE_ARGS ? pa.p + 7 * it.kf : poses + 7 * it.kf, ep, F);
+  __syncthreads();
+  double M[9], t[3];
+#pragma unroll
+  for (int k = 0; k < 9; ++k) M[k] = F.M[k];
+#pragma unroll
+  for (int k = 0; k < 3; ++k) t[k] = F.t[k];
+
+  double acc[NACC];
+#pragma unroll
+  for (int k = 0; k < NACC; ++k) acc[k] = 0.0;
+
+  const int n = it.count;
+  int i = threadIdx.x;
+  // software pipeline, depth 2
+  float4 c0, n0, c1, n1;
+  if (i < n) { c0 = __ldg(&it.cpw[i]); n0 = __ldg(&it.nsd[i]); }
+  if (i + EV_T < n) { c1 = __ldg(&it.cpw[i + EV_T]); n1 = __ldg(&it.nsd[i + EV_T]); }
+  for (; i < n; i += 2 * EV_T) {
+    const float4 ca = c0, na = n0, cb = c1, nb = n1;
+    const bool has_b = i + EV_T < n;
+    if (i + 2 * EV_T < n) { c0 = __ldg(&it.cpw[i + 2 * EV_T]); n0 = __ldg(&it.nsd[i + 2 * EV_T]); }
+    if (i + 3 * EV_T < n) { c1 = __ldg(&it.cpw[i + 3 * EV_T]); n1 = __ldg(&it.nsd[i + 3 * EV_T]); }
+    unary_accumulate<WANT_JAC, JAC_KIND>(ca, na, M, t, F, ep, acc);
+    if (has_b) unary_accumulate<WANT_JAC, JAC_KIND>(cb, nb, M, t, F, ep, acc);
+  }
+
+  block_partials<NACC, EV_T, WANT_JAC>(acc, red, partials);
+  kf_sums(partials, out, W, kf_item_start, ticket, nitems, is_last, [&] {
     // `out` may be host-mapped pinned memory: publish the W x NACC doubles system-wide, then raise the epoch flag the
     // host spins on (no device-to-host copy, no stream synchronisation on the per-iteration path)
     if (done_flag) { __threadfence_system(); __syncthreads(); }
     if (threadIdx.x == 0) { *ticket = 0u; if (done_flag) *(volatile unsigned int*)done_flag = epoch; }
-  }
+  });
+}
+
+// the instantiation for (want_jac, jac_kind, poses in the kernel parameters)
+using UnaryKernel = decltype(&k_eval_unary<false, 0, false>);
+UnaryKernel unary_kernel(bool want_jac, int jac_kind, bool pose_args) {
+  if (pose_args) return !want_jac ? k_eval_unary<false, 0, true> : jac_kind == 0 ? k_eval_unary<true, 0, true> : k_eval_unary<true, 1, true>;
+  return !want_jac ? k_eval_unary<false, 0, false> : jac_kind == 0 ? k_eval_unary<true, 0, false> : k_eval_unary<true, 1, false>;
 }
 
 void eval_unary_run(const EvalItem* d_items, int nitems, int W, const double* d_poses, const EvalParams& ep, int jac_kind,
@@ -218,19 +257,13 @@ void eval_unary_run(const EvalItem* d_items, int nitems, int W, const double* d_
     GLIO_CUDA_TRY(cudaMemsetAsync(d_out, 0, (size_t)W * NACC * sizeof(double), st));
     return;
   }
+  static const PoseArgs none{};
+  PoseArgs pa;
+  const bool pose_args = h_poses && W <= EV_MAXW;
+  if (pose_args) memcpy(pa.p, h_poses, (size_t)W * 7 * sizeof(double));
   lc.begin(want_jac ? "k_eval_unary" : "k_eval_unary_cost", st);
-  if (h_poses && W <= EV_MAXW) {
-    PoseArgs pa;
-    memcpy(pa.p, h_poses, (size_t)W * 7 * sizeof(double));
-    if (!want_jac) k_eval_unary<false, 0, true><<<nitems, EV_T, 0, st>>>(d_items, nitems, W, nullptr, pa, ep, d_partials, d_out, d_kf_item_start, d_ticket, done_flag, epoch);
-    else if (jac_kind == 0) k_eval_unary<true, 0, true><<<nitems, EV_T, 0, st>>>(d_items, nitems, W, nullptr, pa, ep, d_partials, d_out, d_kf_item_start, d_ticket, done_flag, epoch);
-    else k_eval_unary<true, 1, true><<<nitems, EV_T, 0, st>>>(d_items, nitems, W, nullptr, pa, ep, d_partials, d_out, d_kf_item_start, d_ticket, done_flag, epoch);
-  } else {
-    static const PoseArgs none{};
-    if (!want_jac) k_eval_unary<false, 0, false><<<nitems, EV_T, 0, st>>>(d_items, nitems, W, d_poses, none, ep, d_partials, d_out, d_kf_item_start, d_ticket, done_flag, epoch);
-    else if (jac_kind == 0) k_eval_unary<true, 0, false><<<nitems, EV_T, 0, st>>>(d_items, nitems, W, d_poses, none, ep, d_partials, d_out, d_kf_item_start, d_ticket, done_flag, epoch);
-    else k_eval_unary<true, 1, false><<<nitems, EV_T, 0, st>>>(d_items, nitems, W, d_poses, none, ep, d_partials, d_out, d_kf_item_start, d_ticket, done_flag, epoch);
-  }
+  unary_kernel(want_jac, jac_kind, pose_args)<<<nitems, EV_T, 0, st>>>(d_items, nitems, W, pose_args ? nullptr : d_poses, pose_args ? pa : none, ep,
+                                                                       d_partials, d_out, d_kf_item_start, d_ticket, done_flag, epoch);
   lc.end(st);
   GLIO_CUDA_TRY(cudaGetLastError());
 }
@@ -240,45 +273,14 @@ __global__ void __launch_bounds__(256) k_unary_residuals(const float4* __restric
                                                          const double* __restrict__ pose, EvalParams ep, int jac_kind,
                                                          double* __restrict__ r_out, double* __restrict__ J_out) {
   __shared__ KfFrame F;
-  if (threadIdx.x == 0) {
-    double qn[4] = {pose[3], pose[4], pose[5], pose[6]};
-    double R[9]; quat_to_mat(qn, R);
-    const double n2 = ep.q_lb[0] * ep.q_lb[0] + ep.q_lb[1] * ep.q_lb[1] + ep.q_lb[2] * ep.q_lb[2] + ep.q_lb[3] * ep.q_lb[3];
-    double qi[4] = {ep.q_lb[0] / n2, -ep.q_lb[1] / n2, -ep.q_lb[2] / n2, -ep.q_lb[3] / n2};
-    quat_to_mat(qi, F.Rlbi);
-    mat_mul3(R, F.Rlbi, F.M);
-    F.t[0] = pose[0]; F.t[1] = pose[1]; F.t[2] = pose[2];
-    F.q[0] = qn[0]; F.q[1] = qn[1]; F.q[2] = qn[2]; F.q[3] = qn[3];
-  }
+  if (threadIdx.x == 0) kf_frame<true>(pose, ep, F);
   __syncthreads();
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  const float4 c4 = cpw[i];
-  const float4 n4 = nsd[i];
-  const double s = ep.unit_score ? ep.lidar_const : ep.lidar_const * (double)c4.w;
-  const double dx = (double)c4.x - ep.t_lb[0], dy = (double)c4.y - ep.t_lb[1], dz = (double)c4.z - ep.t_lb[2];
-  double a[3]; mat_vec3(F.M, dx, dy, dz, a);
-  const double nx = (double)n4.x, ny = (double)n4.y, nz = (double)n4.z;
-  double r = s * (nx * (a[0] + F.t[0]) + ny * (a[1] + F.t[1]) + nz * (a[2] + F.t[2]) + (double)n4.w);
-  double scale;
-  huber_scale(r, ep.huber_delta, scale);
-  const double ss = s * scale;
-  double J[6];
-  J[0] = ss * nx; J[1] = ss * ny; J[2] = ss * nz;
-  if (jac_kind == 0) {
-    J[3] = 2.0 * ss * (a[1] * nz - a[2] * ny);
-    J[4] = 2.0 * ss * (a[2] * nx - a[0] * nz);
-    J[5] = 2.0 * ss * (a[0] * ny - a[1] * nx);
-  } else {
-    double pb[3]; mat_vec3(F.Rlbi, dx, dy, dz, pb);
-    const double w = F.q[0], ux = F.q[1], uy = F.q[2], uz = F.q[3];
-    const double udp = ux * pb[0] + uy * pb[1] + uz * pb[2];
-    const double ndu = nx * ux + ny * uy + nz * uz;
-    const double ndp = nx * pb[0] + ny * pb[1] + nz * pb[2];
-    J[3] = ss * (2.0 * w * (pb[1] * nz - pb[2] * ny) + 2.0 * (udp * nx + ndu * pb[0] - 2.0 * ndp * ux));
-    J[4] = ss * (2.0 * w * (pb[2] * nx - pb[0] * nz) + 2.0 * (udp * ny + ndu * pb[1] - 2.0 * ndp * uy));
-    J[5] = ss * (2.0 * w * (pb[0] * ny - pb[1] * nx) + 2.0 * (udp * nz + ndu * pb[2] - 2.0 * ndp * uz));
-  }
+  const float4 c4 = cpw[i], n4 = nsd[i];
+  double cost = 0.0, r, scale, J[6];
+  if (jac_kind == 0) plane_residual<true, 0>(c4, n4, F.M, F.t, F, ep, cost, r, scale, J);
+  else plane_residual<true, 1>(c4, n4, F.M, F.t, F, ep, cost, r, scale, J);
   r_out[i] = r * scale;
 #pragma unroll
   for (int k = 0; k < 6; ++k) J_out[6 * i + k] = J[k];
@@ -309,17 +311,7 @@ __global__ void __launch_bounds__(EV_T) k_eval_edge(const EdgeItem* __restrict__
   __shared__ double red[EV_T / 32][NACC];
   __shared__ bool is_last;
   const EdgeItem it = items[blockIdx.x];
-  if (threadIdx.x == 0) {
-    const double* P = poses + 7 * it.kf;
-    double qn[4] = {P[3], P[4], P[5], P[6]};
-    double R[9]; quat_to_mat(qn, R);
-    const double n2 = ep.q_lb[0] * ep.q_lb[0] + ep.q_lb[1] * ep.q_lb[1] + ep.q_lb[2] * ep.q_lb[2] + ep.q_lb[3] * ep.q_lb[3];
-    double qi[4] = {ep.q_lb[0] / n2, -ep.q_lb[1] / n2, -ep.q_lb[2] / n2, -ep.q_lb[3] / n2};
-    quat_to_mat(qi, F.Rlbi);
-    mat_mul3(R, F.Rlbi, F.M);
-    F.t[0] = P[0]; F.t[1] = P[1]; F.t[2] = P[2];
-    if (JAC_KIND == 1) { F.q[0] = qn[0]; F.q[1] = qn[1]; F.q[2] = qn[2]; F.q[3] = qn[3]; }
-  }
+  if (threadIdx.x == 0) kf_frame<JAC_KIND == 1>(poses + 7 * it.kf, ep, F);
   __syncthreads();
   double acc[NACC];
 #pragma unroll
@@ -355,67 +347,24 @@ __global__ void __launch_bounds__(EV_T) k_eval_edge(const EdgeItem* __restrict__
         J[4] = 2.0 * w * (pb[2] * gv[0] - pb[0] * gv[2]) + 2.0 * (udp * gv[1] + gdu * pb[1] - 2.0 * gdp * uy);
         J[5] = 2.0 * w * (pb[0] * gv[1] - pb[1] * gv[0]) + 2.0 * (udp * gv[2] + gdu * pb[2] - 2.0 * gdp * uz);
       }
-      r *= scale;
-      int kk = 0;
-#pragma unroll
-      for (int p = 0; p < 6; ++p)
-#pragma unroll
-        for (int c = p; c < 6; ++c) acc[kk++] += J[p] * J[c];
-#pragma unroll
-      for (int p = 0; p < 6; ++p) acc[21 + p] += J[p] * r;
+      unary_sums(J, r * scale, acc);
     }
   }
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-#pragma unroll
-  for (int k = WANT_JAC ? 0 : 27; k < NACC; ++k) {
-    double v = acc[k];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    if (lane == 0) red[wid][k] = v;
-  }
-  __syncthreads();
-  if (threadIdx.x < NACC) {
-    double v = 0.0;
-    if (WANT_JAC || threadIdx.x == 27) {
-#pragma unroll
-      for (int w8 = 0; w8 < EV_T / 32; ++w8) v += red[w8][threadIdx.x];
-    }
-    partials[(size_t)blockIdx.x * NACC + threadIdx.x] = v;
-  }
-  __threadfence();
-  __syncthreads();
-  if (threadIdx.x == 0) { const unsigned int tk = atomicAdd(ticket, 1u); is_last = (tk == (unsigned)nitems - 1); }
-  __syncthreads();
-  if (is_last) {
-    __threadfence();
-    for (int o = threadIdx.x; o < W * NACC; o += EV_T) {
-      const int kf = o / NACC, k = o - kf * NACC;
-      // same left-to-right order as a plain loop, but eight independent L2 loads in flight at a time: this tail is a serial
-      // chain of ~15 dependent loads per output otherwise (the last block runs alone on the GPU)
-      double v = 0.0;
-      int b = kf_item_start[kf];
-      const int b1 = kf_item_start[kf + 1];
-      for (; b + 8 <= b1; b += 8) {
-        double p[8];
-#pragma unroll
-        for (int u = 0; u < 8; ++u) p[u] = __ldcg(&partials[(size_t)(b + u) * NACC + k]);
-#pragma unroll
-        for (int u = 0; u < 8; ++u) v += p[u];
-      }
-      for (; b < b1; ++b) v += __ldcg(&partials[(size_t)b * NACC + k]);
-      out[o] = v;
-    }
-    if (threadIdx.x == 0) *ticket = 0u;
-  }
+  block_partials<NACC, EV_T, WANT_JAC>(acc, red, partials);
+  kf_sums(partials, out, W, kf_item_start, ticket, nitems, is_last, [&] { if (threadIdx.x == 0) *ticket = 0u; });
+}
+
+// the instantiation for (want_jac, jac_kind)
+using EdgeKernel = decltype(&k_eval_edge<false, 0>);
+EdgeKernel edge_kernel(bool want_jac, int jac_kind) {
+  return !want_jac ? k_eval_edge<false, 0> : jac_kind == 0 ? k_eval_edge<true, 0> : k_eval_edge<true, 1>;
 }
 
 void eval_edge_run(const EdgeItem* d_items, int nitems, int W, const double* d_poses, const EvalParams& ep, int jac_kind, bool want_jac,
                    double* d_partials, double* d_out, const int* d_kf_item_start, unsigned int* d_ticket, cudaStream_t st, LaunchCounter& lc) {
   if (nitems <= 0) { GLIO_CUDA_TRY(cudaMemsetAsync(d_out, 0, (size_t)W * NACC * sizeof(double), st)); return; }
   lc.begin(want_jac ? "k_eval_edge" : "k_eval_edge_cost", st);
-  if (!want_jac) k_eval_edge<false, 0><<<nitems, EV_T, 0, st>>>(d_items, nitems, W, d_poses, ep, d_partials, d_out, d_kf_item_start, d_ticket);
-  else if (jac_kind == 0) k_eval_edge<true, 0><<<nitems, EV_T, 0, st>>>(d_items, nitems, W, d_poses, ep, d_partials, d_out, d_kf_item_start, d_ticket);
-  else k_eval_edge<true, 1><<<nitems, EV_T, 0, st>>>(d_items, nitems, W, d_poses, ep, d_partials, d_out, d_kf_item_start, d_ticket);
+  edge_kernel(want_jac, jac_kind)<<<nitems, EV_T, 0, st>>>(d_items, nitems, W, d_poses, ep, d_partials, d_out, d_kf_item_start, d_ticket);
   lc.end(st);
   GLIO_CUDA_TRY(cudaGetLastError());
 }
@@ -424,7 +373,8 @@ void eval_edge_run(const EdgeItem* d_items, int nitems, int W, const double* d_p
 // K2b: binary (scan-to-multiscan) plane factors, BinaryLidarPlaneNormFactor (LidarKeyframeFactor.h:124-164):
 //   p_w = R(q_c) cp + t_c ;  N = R(q_o) n_l ;  c_w = R(q_o) c_l + t_o ;  r = s N.(p_w - c_w),  s = batch_score * weight
 // tangent Jacobians (SURVEY 8 a-5):  J_c = [u | v],  J_o = [-u | z]  with  u = s N,  v = 2 s (R(q_c)cp x N),  z = 2 s (N x (p_w - t_o)).
-// Because J_o's translation part is -u, the 12x12 outer product needs only 45 distinct sums (+9 for J^T r, +1 cost).
+// Because J_o's translation part is -u, the 12x12 outer product needs only 45 distinct sums (+9 for J^T r, +1 cost): the
+// GLIO_NACC_BIN layout, accumulated by pair_accumulate.
 // HBM traffic per residual: 16 B (cp, weight) + 48 B (n_l, c_l as the reference stores them: double) = 64 B.
 // ---------------------------------------------------------------------------------------------------------------
 constexpr int NB = GLIO_NACC_BIN;
@@ -432,18 +382,51 @@ constexpr int BIN_T = 128;
 
 struct PairFrame { double R1[9], t1[3], R2[9], t2[3]; };
 
+// F from the poses P1 of cur and P2 of oth
+__device__ __forceinline__ void pair_frame(const double* P1, const double* P2, PairFrame& F) {
+  double q1[4] = {P1[3], P1[4], P1[5], P1[6]}, q2[4] = {P2[3], P2[4], P2[5], P2[6]};
+  quat_to_mat(q1, F.R1); quat_to_mat(q2, F.R2);
+  F.t1[0] = P1[0]; F.t1[1] = P1[1]; F.t1[2] = P1[2]; F.t2[0] = P2[0]; F.t2[1] = P2[1]; F.t2[2] = P2[2];
+}
+
+// the 54 J^T J / J^T r sums of one residual r with J_c = [u | v], J_o = [-u | z] (GLIO_NACC_BIN, common.cuh; the cost is the caller's)
+__device__ __forceinline__ void pair_accumulate(const double (&u)[3], const double (&v)[3], const double (&z)[3], double r, double (&acc)[NB]) {
+  int k = 0;
+#pragma unroll
+  for (int a = 0; a < 3; ++a)
+#pragma unroll
+    for (int b = a; b < 3; ++b) acc[k++] += u[a] * u[b];          // uu  [0,6)
+#pragma unroll
+  for (int a = 0; a < 3; ++a)
+#pragma unroll
+    for (int b = 0; b < 3; ++b) acc[k++] += u[a] * v[b];          // uv  [6,15)
+#pragma unroll
+  for (int a = 0; a < 3; ++a)
+#pragma unroll
+    for (int b = a; b < 3; ++b) acc[k++] += v[a] * v[b];          // vv  [15,21)
+#pragma unroll
+  for (int a = 0; a < 3; ++a)
+#pragma unroll
+    for (int b = 0; b < 3; ++b) acc[k++] += u[a] * z[b];          // uz  [21,30)
+#pragma unroll
+  for (int a = 0; a < 3; ++a)
+#pragma unroll
+    for (int b = 0; b < 3; ++b) acc[k++] += v[a] * z[b];          // vz  [30,39)
+#pragma unroll
+  for (int a = 0; a < 3; ++a)
+#pragma unroll
+    for (int b = a; b < 3; ++b) acc[k++] += z[a] * z[b];          // zz  [39,45)
+#pragma unroll
+  for (int a = 0; a < 3; ++a) { acc[45 + a] += r * u[a]; acc[48 + a] += r * v[a]; acc[51 + a] += r * z[a]; }
+}
+
 template <bool WANT_JAC>
 __global__ void __launch_bounds__(BIN_T) k_eval_binary(const BinItem* __restrict__ items, const double* __restrict__ poses, double score_scale,
                                                        double huber_delta, double* __restrict__ partials) {
   __shared__ PairFrame F;
   __shared__ double red[BIN_T / 32][NB];
   const BinItem it = items[blockIdx.x];
-  if (threadIdx.x == 0) {
-    const double* P1 = poses + 7 * it.kf_c; const double* P2 = poses + 7 * it.kf_o;
-    double q1[4] = {P1[3], P1[4], P1[5], P1[6]}, q2[4] = {P2[3], P2[4], P2[5], P2[6]};
-    quat_to_mat(q1, F.R1); quat_to_mat(q2, F.R2);
-    F.t1[0] = P1[0]; F.t1[1] = P1[1]; F.t1[2] = P1[2]; F.t2[0] = P2[0]; F.t2[1] = P2[1]; F.t2[2] = P2[2];
-  }
+  if (threadIdx.x == 0) pair_frame(poses + 7 * it.kf_c, poses + 7 * it.kf_o, F);
   __syncthreads();
   double acc[NB];
 #pragma unroll
@@ -467,53 +450,10 @@ __global__ void __launch_bounds__(BIN_T) k_eval_binary(const BinItem* __restrict
       const double u[3] = {ss * N[0], ss * N[1], ss * N[2]};
       const double v[3] = {2.0 * ss * (a1[1] * N[2] - a1[2] * N[1]), 2.0 * ss * (a1[2] * N[0] - a1[0] * N[2]), 2.0 * ss * (a1[0] * N[1] - a1[1] * N[0])};
       const double z[3] = {2.0 * ss * (N[1] * pm[2] - N[2] * pm[1]), 2.0 * ss * (N[2] * pm[0] - N[0] * pm[2]), 2.0 * ss * (N[0] * pm[1] - N[1] * pm[0])};
-      r *= scale;
-      int k = 0;
-#pragma unroll
-      for (int a = 0; a < 3; ++a)
-#pragma unroll
-        for (int b = a; b < 3; ++b) acc[k++] += u[a] * u[b];          // uu  [0,6)
-#pragma unroll
-      for (int a = 0; a < 3; ++a)
-#pragma unroll
-        for (int b = 0; b < 3; ++b) acc[k++] += u[a] * v[b];          // uv  [6,15)
-#pragma unroll
-      for (int a = 0; a < 3; ++a)
-#pragma unroll
-        for (int b = a; b < 3; ++b) acc[k++] += v[a] * v[b];          // vv  [15,21)
-#pragma unroll
-      for (int a = 0; a < 3; ++a)
-#pragma unroll
-        for (int b = 0; b < 3; ++b) acc[k++] += u[a] * z[b];          // uz  [21,30)
-#pragma unroll
-      for (int a = 0; a < 3; ++a)
-#pragma unroll
-        for (int b = 0; b < 3; ++b) acc[k++] += v[a] * z[b];          // vz  [30,39)
-#pragma unroll
-      for (int a = 0; a < 3; ++a)
-#pragma unroll
-        for (int b = a; b < 3; ++b) acc[k++] += z[a] * z[b];          // zz  [39,45)
-#pragma unroll
-      for (int a = 0; a < 3; ++a) { acc[45 + a] += r * u[a]; acc[48 + a] += r * v[a]; acc[51 + a] += r * z[a]; }
+      pair_accumulate(u, v, z, r * scale, acc);
     }
   }
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-#pragma unroll
-  for (int k = WANT_JAC ? 0 : 54; k < NB; ++k) {
-    double v = acc[k];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    if (lane == 0) red[wid][k] = v;
-  }
-  __syncthreads();
-  if (threadIdx.x < NB) {
-    double v = 0.0;
-    if (WANT_JAC || threadIdx.x == 54) {
-#pragma unroll
-      for (int w4 = 0; w4 < BIN_T / 32; ++w4) v += red[w4][threadIdx.x];
-    }
-    partials[(size_t)blockIdx.x * NB + threadIdx.x] = v;
-  }
+  block_partials<NB, BIN_T, WANT_JAC>(acc, red, partials);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -532,12 +472,7 @@ __global__ void __launch_bounds__(BIN_T) k_eval_binary_edge(const BinEdgeItem* _
   __shared__ PairFrame F;
   __shared__ double red[BIN_T / 32][NB];
   const BinEdgeItem it = items[blockIdx.x];
-  if (threadIdx.x == 0) {
-    const double* P1 = poses + 7 * it.kf_c; const double* P2 = poses + 7 * it.kf_o;
-    double q1[4] = {P1[3], P1[4], P1[5], P1[6]}, q2[4] = {P2[3], P2[4], P2[5], P2[6]};
-    quat_to_mat(q1, F.R1); quat_to_mat(q2, F.R2);
-    F.t1[0] = P1[0]; F.t1[1] = P1[1]; F.t1[2] = P1[2]; F.t2[0] = P2[0]; F.t2[1] = P2[1]; F.t2[2] = P2[2];
-  }
+  if (threadIdx.x == 0) pair_frame(poses + 7 * it.kf_c, poses + 7 * it.kf_o, F);
   __syncthreads();
   double acc[NB];
 #pragma unroll
@@ -564,52 +499,10 @@ __global__ void __launch_bounds__(BIN_T) k_eval_binary_edge(const BinEdgeItem* _
       const double gv[3] = {k * (de[1] * e[2] - de[2] * e[1]), k * (de[2] * e[0] - de[0] * e[2]), k * (de[0] * e[1] - de[1] * e[0])};
       const double v[3] = {2.0 * (a1[1] * gv[2] - a1[2] * gv[1]), 2.0 * (a1[2] * gv[0] - a1[0] * gv[2]), 2.0 * (a1[0] * gv[1] - a1[1] * gv[0])};
       const double z[3] = {2.0 * (gv[1] * pm[2] - gv[2] * pm[1]), 2.0 * (gv[2] * pm[0] - gv[0] * pm[2]), 2.0 * (gv[0] * pm[1] - gv[1] * pm[0])};
-      int kk = 0;
-#pragma unroll
-      for (int a = 0; a < 3; ++a)
-#pragma unroll
-        for (int b = a; b < 3; ++b) acc[kk++] += gv[a] * gv[b];       // uu  [0,6)
-#pragma unroll
-      for (int a = 0; a < 3; ++a)
-#pragma unroll
-        for (int b = 0; b < 3; ++b) acc[kk++] += gv[a] * v[b];        // uv  [6,15)
-#pragma unroll
-      for (int a = 0; a < 3; ++a)
-#pragma unroll
-        for (int b = a; b < 3; ++b) acc[kk++] += v[a] * v[b];         // vv  [15,21)
-#pragma unroll
-      for (int a = 0; a < 3; ++a)
-#pragma unroll
-        for (int b = 0; b < 3; ++b) acc[kk++] += gv[a] * z[b];        // uz  [21,30)
-#pragma unroll
-      for (int a = 0; a < 3; ++a)
-#pragma unroll
-        for (int b = 0; b < 3; ++b) acc[kk++] += v[a] * z[b];         // vz  [30,39)
-#pragma unroll
-      for (int a = 0; a < 3; ++a)
-#pragma unroll
-        for (int b = a; b < 3; ++b) acc[kk++] += z[a] * z[b];         // zz  [39,45)
-#pragma unroll
-      for (int a = 0; a < 3; ++a) { acc[45 + a] += r * gv[a]; acc[48 + a] += r * v[a]; acc[51 + a] += r * z[a]; }
+      pair_accumulate(gv, v, z, r, acc);
     }
   }
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-#pragma unroll
-  for (int k = WANT_JAC ? 0 : 54; k < NB; ++k) {
-    double v = acc[k];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    if (lane == 0) red[wid][k] = v;
-  }
-  __syncthreads();
-  if (threadIdx.x < NB) {
-    double v = 0.0;
-    if (WANT_JAC || threadIdx.x == 54) {
-#pragma unroll
-      for (int w4 = 0; w4 < BIN_T / 32; ++w4) v += red[w4][threadIdx.x];
-    }
-    partials[(size_t)blockIdx.x * NB + threadIdx.x] = v;
-  }
+  block_partials<NB, BIN_T, WANT_JAC>(acc, red, partials);
 }
 
 // S += S_edge over n_pairs x NB sums (the binary plane and edge factors of a pair share one block assembly)
@@ -633,8 +526,7 @@ __device__ __forceinline__ int sym3(int a, int b) { return a <= b ? (a * 3 - a *
 // block assembly: blocks [0,K) -> diagonal 6x6 (21 upper-tri) + g (6) + per-KF cost share (cost is attributed to cur);
 // blocks [K, K+n_pairs) -> off-diagonal 6x6 (row = cur tangent, col = oth tangent)
 __global__ void __launch_bounds__(64) k_bin_assemble(const double* __restrict__ S, int K, int n_pairs, const int* __restrict__ kf_inc_start,
-                                                     const BinIncidence* __restrict__ inc, const int* __restrict__ pair_kf /*2 per pair*/,
-                                                     double* __restrict__ diag, double* __restrict__ off) {
+                                                     const BinIncidence* __restrict__ inc, double* __restrict__ diag, double* __restrict__ off) {
   const int b = blockIdx.x, e = threadIdx.x;
   if (b < K) {
     if (e >= GLIO_NACC) return;
@@ -672,13 +564,11 @@ __global__ void __launch_bounds__(64) k_bin_assemble(const double* __restrict__ 
 
 void eval_binary_run(const BinItem* d_items, int nitems, const int* d_pair_item_start, int n_pairs, int K, const double* d_poses,
                      double score_scale, double huber_delta, bool want_jac, double* d_partials, double* d_pair_sums,
-                     const int* d_kf_inc_start, const BinIncidence* d_inc, double* d_diag, double* d_off, double* d_cost,
+                     const int* d_kf_inc_start, const BinIncidence* d_inc, double* d_diag, double* d_off,
                      cudaStream_t st, LaunchCounter& lc, const double* d_pair_sums_edge) {
-  (void)d_cost;
   if (nitems > 0) {
     lc.begin(want_jac ? "k_eval_binary" : "k_eval_binary_cost", st);
-    if (want_jac) k_eval_binary<true><<<nitems, BIN_T, 0, st>>>(d_items, d_poses, score_scale, huber_delta, d_partials);
-    else k_eval_binary<false><<<nitems, BIN_T, 0, st>>>(d_items, d_poses, score_scale, huber_delta, d_partials);
+    (want_jac ? k_eval_binary<true> : k_eval_binary<false>)<<<nitems, BIN_T, 0, st>>>(d_items, d_poses, score_scale, huber_delta, d_partials);
     lc.end(st);
   }
   if (n_pairs > 0) {
@@ -694,7 +584,7 @@ void eval_binary_run(const BinItem* d_items, int nitems, const int* d_pair_item_
 void bin_assemble_run(const double* d_pair_sums, int K, int n_pairs, const int* d_kf_inc_start, const BinIncidence* d_inc, bool want_jac,
                       double* d_diag, double* d_off, cudaStream_t st, LaunchCounter& lc) {
   lc.begin("k_bin_assemble", st);
-  k_bin_assemble<<<K + (want_jac ? n_pairs : 0), 64, 0, st>>>(d_pair_sums, K, n_pairs, d_kf_inc_start, d_inc, nullptr, d_diag, d_off);
+  k_bin_assemble<<<K + (want_jac ? n_pairs : 0), 64, 0, st>>>(d_pair_sums, K, n_pairs, d_kf_inc_start, d_inc, d_diag, d_off);
   lc.end(st);
   GLIO_CUDA_TRY(cudaGetLastError());
 }
@@ -703,8 +593,7 @@ void eval_binary_edge_run(const BinEdgeItem* d_items, int nitems, const int* d_p
                           bool want_jac, double* d_partials, double* d_pair_sums, cudaStream_t st, LaunchCounter& lc) {
   if (nitems > 0) {
     lc.begin(want_jac ? "k_eval_binary_edge" : "k_eval_binary_edge_cost", st);
-    if (want_jac) k_eval_binary_edge<true><<<nitems, BIN_T, 0, st>>>(d_items, d_poses, d_partials);
-    else k_eval_binary_edge<false><<<nitems, BIN_T, 0, st>>>(d_items, d_poses, d_partials);
+    (want_jac ? k_eval_binary_edge<true> : k_eval_binary_edge<false>)<<<nitems, BIN_T, 0, st>>>(d_items, d_poses, d_partials);
     lc.end(st);
   }
   if (n_pairs > 0) {
