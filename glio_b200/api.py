@@ -991,10 +991,47 @@ def _batch_get_selection(self, cur, oth):
     return _selection_out(lambda cap, p, n: self._chk(self._lib.glio_batch_get_selection(self._h, C.c_int(cur), C.c_int(oth), cap, p, n)))
 
 
+def _select_random_edges(self, stream_ids, options=None, **kw):
+    """glio_select_random_edges: featureSelection's rule and sampler on the edge lists of slots 0..len(stream_ids)-1 (domain 3);
+    returns the active edge counts."""
+    ids = np.ascontiguousarray(stream_ids, np.int64)
+    opt = options if options is not None else select_default_options(**kw)
+    na = np.zeros(len(ids), np.int64)
+    self._chk(self._lib.glio_select_random_edges(self._h, C.c_int(len(ids)), _ptr(ids), C.byref(opt), _ptr(na)))
+    return na
+
+
+def _batch_select_random_edges(self, cur, oth, mode, options=None, **kw):
+    """glio_batch_select_random_edges: the batch rules and sampler on the edge lists of pairs (cur[i], oth[i]) (domains 4 / 5);
+    returns the active edge counts."""
+    cur = np.ascontiguousarray(cur, np.int32); oth = np.ascontiguousarray(oth, np.int32)
+    if len(cur) != len(oth):
+        raise ValueError("cur and oth must have the same length")
+    opt = options if options is not None else select_default_options(**kw)
+    na = np.zeros(len(cur), np.int64)
+    self._chk(self._lib.glio_batch_select_random_edges(self._h, _ptr(cur), _ptr(oth), C.c_int64(len(cur)), C.c_int(mode), C.byref(opt),
+                                                       _ptr(na)))
+    return na
+
+
+def _get_edge_selection(self, slot):
+    """The selected edge indices of a slot in draw order (int32 array), or None when all its edges are active."""
+    return _selection_out(lambda cap, p, n: self._chk(self._lib.glio_get_edge_selection(self._h, C.c_int(slot), cap, p, n)))
+
+
+def _batch_get_edge_selection(self, cur, oth):
+    """The selected edge indices of pair (cur, oth) in draw order, or None when all its edges are active."""
+    return _selection_out(lambda cap, p, n: self._chk(self._lib.glio_batch_get_edge_selection(self._h, C.c_int(cur), C.c_int(oth), cap, p, n)))
+
+
 Context.select_random = _select_random
 Context.batch_select_random = _batch_select_random
 Context.get_selection = _get_selection
 Context.batch_get_selection = _batch_get_selection
+Context.select_random_edges = _select_random_edges
+Context.batch_select_random_edges = _batch_select_random_edges
+Context.get_edge_selection = _get_edge_selection
+Context.batch_get_edge_selection = _batch_get_edge_selection
 Context.batch_declare_pairs = _batch_declare_pairs
 Context.batch_solve = _batch_solve
 Context.set_allreduce = _set_allreduce

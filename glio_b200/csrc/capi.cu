@@ -44,13 +44,25 @@ struct AssocDebug {
   int64_t Q = 0;
 };
 
+// the edges an evaluation reads: n records of cp with s in .w and line points pa / pb
+struct EdgeView {
+  const float4* cps; const float4* pa; const float4* pb;
+  int64_t n;
+};
+
 // edge correspondences: cp with s in .w, line points pa / pb; src = scan index of each edge when an association produced them
 struct EdgeList {
   DevBuf<float4> cps, pa, pb;
   DevBuf<int32_t> src;
   int64_t n = 0;
   bool has_src = false;
-  void clear() { n = 0; has_src = false; }
+  DevBuf<float4> s_cps, s_pa, s_pb;   // selected subset (glio_select_random_edges / glio_batch_select_random_edges), draw order
+  DevBuf<int32_t> s_keep;             // its edge indices
+  int64_t n_sel = -1;                 // -1: no selection -> all edges are active
+  // replacing the list drops its selection
+  void clear() { n = 0; has_src = false; n_sel = -1; }
+  // what every consumer evaluates: the selected subset if there is one, otherwise all edges
+  EdgeView active() const { return n_sel >= 0 ? EdgeView{s_cps.p, s_pa.p, s_pb.p, n_sel} : EdgeView{cps.p, pa.p, pb.p, n}; }
   // room for q edges; a reserve may drop the old contents, so the list must count as empty until it is refilled
   EdgeDst reserve(int64_t q) {
     cps.reserve((size_t)q); pa.reserve((size_t)q); pb.reserve((size_t)q); src.reserve((size_t)q);
@@ -525,12 +537,12 @@ void wait_marg_copied(glio_ctx* c) {
   }
 }
 
-// K2e work items of slots 0..W-1 (GLIO_ITEM_MAX residuals each, keyframe order)
+// K2e work items of slots 0..W-1 (GLIO_ITEM_MAX residuals each, keyframe order) over their active edges
 ItemPlan<EdgeItem> plan_edge_items(const glio_ctx* c, int W) {
   ItemPlan<EdgeItem> plan(W);
   for (int k = 0; k < W; ++k) {
-    const EdgeList* e = (size_t)k < c->slots.size() && c->slots[k] ? &c->slots[k]->edges : nullptr;
-    plan.cut(k, e ? e->n : 0, GLIO_ITEM_MAX, [&](int64_t f, int32_t count) { return EdgeItem{e->cps.p + f, e->pa.p + f, e->pb.p + f, count, k}; });
+    const EdgeView e = (size_t)k < c->slots.size() && c->slots[k] ? c->slots[k]->edges.active() : EdgeView{nullptr, nullptr, nullptr, 0};
+    plan.cut(k, e.n, GLIO_ITEM_MAX, [&](int64_t f, int32_t count) { return EdgeItem{e.cps + f, e.pa + f, e.pb + f, count, k}; });
   }
   return plan;
 }
@@ -1946,7 +1958,11 @@ int glio_batch_set_pair_edges(glio_ctx* c, int cur, int oth, const float* cp, co
 
 namespace {
 
-enum { SEL_DOMAIN_WINDOW = 0, SEL_DOMAIN_STARTEND = 1, SEL_DOMAIN_ADD = 2 };
+// Philox key domains: one per rule and record kind, so plane and edge samples with the same seed, stream and nonce are independent
+enum {
+  SEL_DOMAIN_WINDOW = 0, SEL_DOMAIN_STARTEND = 1, SEL_DOMAIN_ADD = 2,
+  SEL_DOMAIN_WINDOW_EDGES = 3, SEL_DOMAIN_STARTEND_EDGES = 4, SEL_DOMAIN_ADD_EDGES = 5
+};
 
 void check_select_options(const glio_select_options* o) {
   GLIO_REQUIRE(o != nullptr, GLIO_ERR_ARG, "null selection options");
@@ -1969,6 +1985,62 @@ void select_launch(glio_ctx* c, const std::vector<SelSeg>& segs, int k_max, uint
   select_sample_run(c->d_sel_segs.p, (int)segs.size(), k_max, seed, domain, nonce, c->st, c->lc);
 }
 
+// featureSelection's outcome (Estimator.cpp:3894-3992) for a list of n records, which follows from n alone: -1 keeps all of them
+// (the reference returns), F keeps the F sampled ones, 0 keeps none (random_select off: the loop never runs)
+int64_t window_select_count(int64_t n, const glio_select_options* o) {
+  const int F = o->feature_res_num;
+  return (n < 1 || n - 1 < F) ? -1 : o->random_select ? F : 0;
+}
+
+// the pairs (cur[i], oth[i]) of a batch selection call `fn`, with its arguments checked before anything changes: mode 0 or 1, the
+// options, no pair with cur == oth or off the pair list, none listed twice, the list grouped by cur
+std::vector<glio_ctx::Pair*> batch_select_pairs(glio_ctx* c, const std::string& fn, const int32_t* cur, const int32_t* oth, int64_t n_pairs,
+                                                int mode, const glio_select_options* opt) {
+  GLIO_REQUIRE(n_pairs >= 0 && (n_pairs == 0 || (cur && oth)), GLIO_ERR_ARG, fn + ": null pair arrays");
+  GLIO_REQUIRE(mode == 0 || mode == 1, GLIO_ERR_ARG, fn + ": mode must be 0 (start/end) or 1 (incremental)");
+  check_select_options(opt);
+  std::vector<glio_ctx::Pair*> prs((size_t)n_pairs);
+  std::set<const glio_ctx::Pair*> listed;
+  std::set<int> runs_seen;
+  for (int64_t i = 0; i < n_pairs; ++i) {
+    GLIO_REQUIRE(cur[i] != oth[i], GLIO_ERR_ARG, fn + ": cur == oth");
+    prs[i] = &find_pair(c, cur[i], oth[i]);
+    GLIO_REQUIRE(listed.insert(prs[i]).second, GLIO_ERR_ARG, fn + ": pair listed twice");
+    if (i == 0 || cur[i] != cur[i - 1])
+      GLIO_REQUIRE(runs_seen.insert(cur[i]).second, GLIO_ERR_ARG, fn + ": pair list is not grouped by cur");
+  }
+  return prs;
+}
+
+// globalFeatureSelection_Batch (mode 0, Estimator.cpp:3994-4055) / globalFeatureSelectionAdd_Batch (mode 1, :4057-4116) for the
+// listed pairs' record counts n[i], visited in list order: -1 keeps all records, B the B sampled ones.  A start/end pair that fails
+// the size test ends the run of its cur (the reference's `return`), an incremental one only skips itself (`continue`).
+std::vector<int64_t> batch_select_counts(const int32_t* cur, const std::vector<int64_t>& n, int mode, int B) {
+  std::vector<int64_t> n_sel(n.size());
+  bool stopped = false;
+  for (size_t i = 0; i < n.size(); ++i) {
+    if (i == 0 || cur[i] != cur[i - 1]) stopped = false;
+    if (mode == 0) {
+      if (!stopped && (n[i] - 1 < B || n[i] < 50)) stopped = true;
+      n_sel[i] = stopped ? -1 : B;
+    } else {
+      n_sel[i] = n[i] <= B ? -1 : B;
+    }
+  }
+  return n_sel;
+}
+
+// a k_sel_sample segment that draws k of the edges of e into its selection buffers
+SelSeg edge_select_seg(EdgeList& e, int k, uint64_t stream) {
+  e.s_cps.reserve(k); e.s_pa.reserve(k); e.s_pb.reserve(k); e.s_keep.reserve(k);
+  SelSeg g{};
+  g.cpw = e.cps.p; g.pa = e.pa.p; g.pb = e.pb.p; g.o_cpw = e.s_cps.p; g.o_pa = e.s_pa.p; g.o_pb = e.s_pb.p;
+  g.keep = e.s_keep.p; g.n = e.n; g.stream = stream; g.k = k;
+  return g;
+}
+
+uint64_t pair_stream(int32_t cur, int32_t oth) { return ((uint64_t)(uint32_t)cur << 32) | (uint32_t)oth; }
+
 }  // namespace
 
 extern "C" {
@@ -1989,10 +2061,7 @@ int glio_select_random(glio_ctx* c, int W, const int64_t* stream_ids, const glio
     check_select_options(opt);
     const int F = opt->feature_res_num;
     std::vector<int64_t> n_sel(W);
-    for (int k = 0; k < W; ++k) {
-      const int64_t n = (size_t)k < c->slots.size() && c->slots[k] ? c->slots[k]->n_match : 0;
-      n_sel[k] = (n < 1 || n - 1 < F) ? -1 : opt->random_select ? F : 0;    // return / sample F / the loop never runs
-    }
+    for (int k = 0; k < W; ++k) n_sel[k] = window_select_count((size_t)k < c->slots.size() && c->slots[k] ? c->slots[k]->n_match : 0, opt);
     std::vector<SelSeg> segs;
     for (int k = 0; k < W; ++k) {
       Slot& sl = c->slot(k);
@@ -2014,39 +2083,40 @@ int glio_select_random(glio_ctx* c, int W, const int64_t* stream_ids, const glio
   });
 }
 
-// globalFeatureSelection_Batch (mode 0, Estimator.cpp:3994-4055) / globalFeatureSelectionAdd_Batch (mode 1, :4057-4116) for the
-// listed pairs, visited in list order; a start/end pair that fails the size test ends the run of its cur (the reference's
-// `return`), an incremental one only skips itself (`continue`).
+// featureSelection's rule and sampler on the edge lists of slots 0..W-1 (domain 3)
+int glio_select_random_edges(glio_ctx* c, int W, const int64_t* stream_ids, const glio_select_options* opt, int64_t* n_active) {
+  if (!c) return GLIO_ERR_ARG;
+  return guarded(c, [&] {
+    GLIO_REQUIRE(W > 0 && W <= 4096 && stream_ids, GLIO_ERR_ARG, "glio_select_random_edges: bad window arguments");
+    check_select_options(opt);
+    const int F = opt->feature_res_num;
+    std::vector<int64_t> n_sel(W);
+    std::vector<SelSeg> segs;
+    for (int k = 0; k < W; ++k) {
+      EdgeList& e = c->slot(k).edges;
+      n_sel[k] = window_select_count(e.n, opt);
+      if (n_sel[k] > 0) segs.push_back(edge_select_seg(e, F, (uint64_t)stream_ids[k]));
+    }
+    select_launch(c, segs, F, SEL_DOMAIN_WINDOW_EDGES, opt->seed, opt->nonce);
+    for (int k = 0; k < W; ++k) {
+      EdgeList& e = c->slot(k).edges;
+      e.n_sel = n_sel[k];
+      if (n_active) n_active[k] = n_sel[k] >= 0 ? n_sel[k] : e.n;
+    }
+    c->edge_items_dirty = true;
+  });
+}
+
+// globalFeatureSelection_Batch (mode 0) / globalFeatureSelectionAdd_Batch (mode 1) for the listed pairs' plane matches
 int glio_batch_select_random(glio_ctx* c, const int32_t* cur, const int32_t* oth, int64_t n_pairs, int mode, const glio_select_options* opt,
                              int64_t* n_active) {
   if (!c) return GLIO_ERR_ARG;
   return guarded(c, [&] {
-    GLIO_REQUIRE(n_pairs >= 0 && (n_pairs == 0 || (cur && oth)), GLIO_ERR_ARG, "glio_batch_select_random: null pair arrays");
-    GLIO_REQUIRE(mode == 0 || mode == 1, GLIO_ERR_ARG, "glio_batch_select_random: mode must be 0 (start/end) or 1 (incremental)");
-    check_select_options(opt);
+    const std::vector<glio_ctx::Pair*> prs = batch_select_pairs(c, "glio_batch_select_random", cur, oth, n_pairs, mode, opt);
     const int Bn = opt->batch_feature_res_num;
-    std::vector<glio_ctx::Pair*> prs((size_t)n_pairs);
-    std::set<const glio_ctx::Pair*> listed;
-    std::set<int> runs_seen;
-    for (int64_t i = 0; i < n_pairs; ++i) {
-      GLIO_REQUIRE(cur[i] != oth[i], GLIO_ERR_ARG, "glio_batch_select_random: cur == oth");
-      prs[i] = &find_pair(c, cur[i], oth[i]);
-      GLIO_REQUIRE(listed.insert(prs[i]).second, GLIO_ERR_ARG, "glio_batch_select_random: pair listed twice");
-      if (i == 0 || cur[i] != cur[i - 1])
-        GLIO_REQUIRE(runs_seen.insert(cur[i]).second, GLIO_ERR_ARG, "glio_batch_select_random: pair list is not grouped by cur");
-    }
-    std::vector<int64_t> n_sel((size_t)n_pairs);
-    bool stopped = false;
-    for (int64_t i = 0; i < n_pairs; ++i) {
-      const int64_t n = prs[i]->n_match;
-      if (i == 0 || cur[i] != cur[i - 1]) stopped = false;
-      if (mode == 0) {
-        if (!stopped && (n - 1 < Bn || n < 50)) stopped = true;
-        n_sel[i] = stopped ? -1 : Bn;
-      } else {
-        n_sel[i] = n <= Bn ? -1 : Bn;
-      }
-    }
+    std::vector<int64_t> n((size_t)n_pairs);
+    for (int64_t i = 0; i < n_pairs; ++i) n[i] = prs[i]->n_match;
+    const std::vector<int64_t> n_sel = batch_select_counts(cur, n, mode, Bn);
     std::vector<SelSeg> segs;
     for (int64_t i = 0; i < n_pairs; ++i) {
       if (n_sel[i] <= 0) continue;
@@ -2054,7 +2124,7 @@ int glio_batch_select_random(glio_ctx* c, const int32_t* cur, const int32_t* oth
       pr.s_cpw.reserve(Bn); pr.s_nc.reserve(6 * (size_t)Bn); pr.s_keep.reserve(Bn);
       SelSeg g{};
       g.cpw = pr.m_cpw.p; g.nsd = nullptr; g.nc = pr.m_nc.p; g.o_cpw = pr.s_cpw.p; g.o_nsd = nullptr; g.o_nc = pr.s_nc.p;
-      g.keep = pr.s_keep.p; g.n = pr.n_match; g.stream = ((uint64_t)(uint32_t)cur[i] << 32) | (uint32_t)oth[i]; g.k = Bn;
+      g.keep = pr.s_keep.p; g.n = pr.n_match; g.stream = pair_stream(cur[i], oth[i]); g.k = Bn;
       segs.push_back(g);
     }
     select_launch(c, segs, Bn, mode == 0 ? SEL_DOMAIN_STARTEND : SEL_DOMAIN_ADD, opt->seed, opt->nonce);
@@ -2064,6 +2134,29 @@ int glio_batch_select_random(glio_ctx* c, const int32_t* cur, const int32_t* oth
       if (n_active) n_active[i] = n_sel[i] >= 0 ? n_sel[i] : pr.n_match;
     }
     c->bin_dirty = true;
+  });
+}
+
+// the same rules and sampler for the listed pairs' edge lists (domains 4 and 5)
+int glio_batch_select_random_edges(glio_ctx* c, const int32_t* cur, const int32_t* oth, int64_t n_pairs, int mode, const glio_select_options* opt,
+                                   int64_t* n_active) {
+  if (!c) return GLIO_ERR_ARG;
+  return guarded(c, [&] {
+    const std::vector<glio_ctx::Pair*> prs = batch_select_pairs(c, "glio_batch_select_random_edges", cur, oth, n_pairs, mode, opt);
+    const int Bn = opt->batch_feature_res_num;
+    std::vector<int64_t> n((size_t)n_pairs);
+    for (int64_t i = 0; i < n_pairs; ++i) n[i] = prs[i]->edges.n;
+    const std::vector<int64_t> n_sel = batch_select_counts(cur, n, mode, Bn);
+    std::vector<SelSeg> segs;
+    for (int64_t i = 0; i < n_pairs; ++i)
+      if (n_sel[i] > 0) segs.push_back(edge_select_seg(prs[i]->edges, Bn, pair_stream(cur[i], oth[i])));
+    select_launch(c, segs, Bn, mode == 0 ? SEL_DOMAIN_STARTEND_EDGES : SEL_DOMAIN_ADD_EDGES, opt->seed, opt->nonce);
+    for (int64_t i = 0; i < n_pairs; ++i) {
+      EdgeList& e = prs[i]->edges;
+      e.n_sel = n_sel[i];
+      if (n_active) n_active[i] = n_sel[i] >= 0 ? n_sel[i] : e.n;
+    }
+    c->bedge_dirty = true;
   });
 }
 
@@ -2096,6 +2189,22 @@ int glio_batch_get_selection(glio_ctx* c, int cur, int oth, int64_t capacity, in
   return guarded(c, [&] {
     glio_ctx::Pair& pr = find_pair(c, cur, oth);
     copy_selection(c, pr.n_sel, pr.s_keep, capacity, keep, n);
+  });
+}
+
+int glio_get_edge_selection(glio_ctx* c, int slot, int64_t capacity, int32_t* keep, int64_t* n) {
+  if (!c) return GLIO_ERR_ARG;
+  return guarded(c, [&] {
+    const EdgeList& e = c->slot(slot).edges;
+    copy_selection(c, e.n_sel, e.s_keep, capacity, keep, n);
+  });
+}
+
+int glio_batch_get_edge_selection(glio_ctx* c, int cur, int oth, int64_t capacity, int32_t* keep, int64_t* n) {
+  if (!c) return GLIO_ERR_ARG;
+  return guarded(c, [&] {
+    const EdgeList& e = find_pair(c, cur, oth).edges;
+    copy_selection(c, e.n_sel, e.s_keep, capacity, keep, n);
   });
 }
 
@@ -2133,16 +2242,17 @@ void build_bin_items(glio_ctx* c, int K) {
   c->bin_dirty = false; c->bin_K = K;
 }
 
-// work items of the binary edge evaluation: each pair's edge list in runs of GLIO_ITEM_MAX, pairs in pair-list order (rebuilt when
-// an edge list, K or the pair count changes, or the switch is turned; build_bin_items runs first and checks the pairs against K)
+// work items of the binary edge evaluation: each pair's active edges in runs of GLIO_ITEM_MAX, pairs in pair-list order (rebuilt
+// when an edge list or its selection, K or the pair count changes, or the switch is turned; build_bin_items runs first and checks
+// the pairs against K)
 void build_bedge_items(glio_ctx* c, int K) {
   const int P = (int)c->pairs.size();
   if (!c->bedge_dirty && c->bedge_K == K && c->bedge_P == P) return;
   ItemPlan<BinEdgeItem> plan(P);
   for (int p = 0; p < P; ++p) {
     const glio_ctx::Pair& pr = *c->pairs[p];
-    const EdgeList& e = pr.edges;
-    plan.cut(p, e.n, GLIO_ITEM_MAX, [&](int64_t f, int32_t count) { return BinEdgeItem{e.cps.p + f, e.pa.p + f, e.pb.p + f, count, pr.cur, pr.oth}; });
+    const EdgeView e = pr.edges.active();
+    plan.cut(p, e.n, GLIO_ITEM_MAX, [&](int64_t f, int32_t count) { return BinEdgeItem{e.cps + f, e.pa + f, e.pb + f, count, pr.cur, pr.oth}; });
   }
   c->n_bedge_items = (int)plan.items.size();
   c->d_bedge_sums.reserve((size_t)(P + 1) * GLIO_NACC_BIN);

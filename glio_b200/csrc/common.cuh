@@ -267,14 +267,17 @@ void edge_assoc_run(const GridBuild& gb, const SegDesc* d_segs, int nseg, const 
 void compact_edge_scatter(const AssocWork& w, const SegDesc* d_segs, const int* d_pos, const float4* pa, const float4* pb, float score,
                           const EdgeDst* d_dst, cudaStream_t st, LaunchCounter& lc);
 
-// ---- feature selection (select.cu): one segment = one slot's or one pair's seeded sample of k of its n matches
+// ---- feature selection (select.cu): one segment = one slot's or one pair's seeded sample of k of its n plane matches or edges
 struct SelSeg {
-  const float4* cpw;    // the segment's matches (cp.xyz, weight)
-  const float4* nsd;    // (n_s.xyz, d_s), window slots; nullptr for pairs
-  const double* nc;     // 6 per match, pairs; nullptr for slots
+  const float4* cpw;    // the segment's records: plane matches (cp.xyz, weight) or edges (cp.xyz, s)
+  const float4* nsd;    // (n_s.xyz, d_s), window plane matches; nullptr otherwise
+  const double* nc;     // 6 per match, pair plane matches; nullptr otherwise
+  const float4* pa;     // edges: the line points pa and pb; nullptr for plane matches
+  const float4* pb;
   float4* o_cpw; float4* o_nsd; double* o_nc;   // the selection buffers (same layout as gather_selection writes)
-  int32_t* keep;        // [k] the selected match indices in draw order
-  int64_t n;            // matches; the draws come from 0 .. n-2
+  float4* o_pa; float4* o_pb;
+  int32_t* keep;        // [k] the selected record indices in draw order
+  int64_t n;            // records; the draws come from 0 .. n-2
   uint64_t stream;
   int32_t k, pad;
 };

@@ -1,7 +1,8 @@
 // select.cu — the Estimator's random feature selection (Estimator.cpp:3894-4116) as a seeded sampler on the device.
 //
 // Every selection the reference makes (window featureSelection, batch start/end and incremental) is an ordered uniform sample
-// without replacement of k positions out of 0 .. n-2 (DESIGN 2).  Draw j of a segment takes
+// without replacement of k positions out of 0 .. n-2 (DESIGN 2); edge lists are selected by the same rules and draws, in domains
+// of their own, and a segment gathers either plane matches or edges.  Draw j of a segment takes
 //   r_j = mulhi64(u_j, n-1-j),  u_j = word j % 4 of Philox4x64-10 at counter (j/4 + 1, stream, nonce, 0), key (seed, domain)
 // and selects the r_j-th (0-based) value of 0 .. n-2 not chosen yet.  mulhi64 without rejection is uniform up to a relative
 // bias below (n-1)/2^64 < 2^-33 for n < 2^31.  Integer arithmetic only: the result is the same bits on every device.
@@ -78,6 +79,7 @@ __global__ void __launch_bounds__(32) k_sel_sample(const SelSeg* __restrict__ se
 #pragma unroll
       for (int c = 0; c < 6; ++c) sg.o_nc[6 * (int64_t)j + c] = sg.nc[6 * src + c];
     }
+    if (sg.pa) { sg.o_pa[j] = sg.pa[src]; sg.o_pb[j] = sg.pb[src]; }
   }
 }
 

@@ -195,7 +195,7 @@ int glio_select(glio_ctx* ctx, int slot, const int32_t* keep, int64_t n);
  *         numpy.random.Philox(key=[seed, domain], counter=[0, stream, nonce, 0]).random_raw();
  *   r_j = mulhi64(u_j, n-1-j), no rejection: uniform on [0, n-1-j) up to a bias below 2^-33 for n < 2^31;
  *   index = the r_j-th (0-based) position of 0 .. n-2 not chosen yet, ascending.
- * domain: 0 window, 1 batch start/end, 2 batch incremental.  stream: the caller's id per window slot (the keyframe index, so a
+ * domain: 0 window, 1 batch start/end, 2 batch incremental (3 to 5: the edge selections, glio_select_random_edges).  stream: the caller's id per window slot (the keyframe index, so a
  * keyframe's sample does not depend on its slot), (uint64)cur << 32 | oth per pair (so a sharded run selects what one context
  * selects).  nonce: per call, for the reference's fresh draws per solve or batch round (e.g. activation * 4 + iterCount).
  * One k_sel_sample launch per call covers every sampled slot or pair; its table goes up in one copy and the call does not
@@ -733,8 +733,9 @@ int glio_batch_set_edge_frame(glio_ctx* ctx, int frame, const float* xyz, int64_
  * the pair list yet is appended, with no plane matches (as glio_batch_set_pair_matches appends one).  Pairs are grouped by oth: one
  * search launch and one host synchronisation (for the counts) per group, besides the grid build's own when oth's grid is built.
  * n_edge[n_pairs] (may be NULL) receives the counts.  options NULL = the defaults.  An unknown frame, cur == oth or bad options is
- * GLIO_ERR_ARG, a cur or oth without a corner scan is GLIO_ERR_STATE; both change nothing.  Feature selection
- * (glio_batch_select*) leaves edge lists alone: all edges of a pair are evaluated. */
+ * GLIO_ERR_ARG, a cur or oth without a corner scan is GLIO_ERR_STATE; both change nothing.  The plane selection calls
+ * (glio_batch_select*) leave edge lists alone; glio_batch_select_random_edges selects edges.  Without an edge selection all edges of
+ * a pair are evaluated. */
 int glio_batch_associate_edges_pairs(glio_ctx* ctx, const int32_t* cur, const int32_t* oth, int64_t n_pairs, const glio_edge_options* options,
                                      int64_t* n_edge);
 /* copy-out of the edge list of pair (cur, oth), the conventions of glio_get_edges (pa / pb in oth's frame); a pair not on the pair
@@ -758,6 +759,35 @@ int glio_eval_binary_edge(glio_ctx* ctx, int K, const double* poses, double* Hdi
  * glio_eval_binary never includes edges.  The edge work-item plan is rebuilt only when an edge list, K, the pair count or this
  * switch changes. */
 int glio_batch_use_edges(glio_ctx* ctx, int on);
+
+/* ---- seeded device selection of EDGE correspondences.  The reference selects plane matches only; this library applies the same
+ * rules and the same sampler (glio_select_random / glio_batch_select_random, k_sel_sample) to edge lists, with the sizes of a
+ * glio_select_options passed to these calls, so edge sizes are set independently of plane sizes:
+ *   window (glio_select_random_edges): featureSelection's rule on the slot's edge count n: keep all edges when n < 1 or n - 1 < F,
+ *     none when random_select is 0, else the F sampled edges in draw order;
+ *   batch mode 0 (start/end): the run rule of glio_batch_select_random on edge counts (n - 1 < B or n < 50 ends the run of its cur,
+ *     whose later pairs keep all their edges); mode 1 (incremental): keep all edges when n <= B, else sample B.
+ * Draws as for plane matches, from positions 0 .. n-2: the last edge of a list is never chosen.  That quirk of the reference's plane
+ * selection is carried over on purpose, so that one kernel and one reference serve both.  Philox domains: 3 window edges, 4 batch
+ * start/end edges, 5 batch incremental edges; the streams are those of the plane calls (the keyframe id per slot, cur << 32 | oth
+ * per pair), so an edge sample is independent of the plane sample with the same seed, stream and nonce, and a sharded run selects
+ * what one context selects.  One k_sel_sample launch per call, no stream synchronisation (as the plane calls).
+ * Every consumer of an edge list evaluates its active edges: the selected subset in draw order if there is one, else all edges --
+ * glio_eval_edge / glio_eval_edge_kind, the edge blocks of glio_window_solve, glio_window_solve_band, glio_window_marginalize and
+ * glio_window_marginalize_async, glio_eval_binary_edge and the edge blocks of glio_batch_solve.  glio_get_edges / glio_batch_get_edges
+ * return the full list.  Replacing a list (glio_set_edges, glio_window_associate_edges, glio_batch_associate_edges_pairs,
+ * glio_batch_set_pair_edges, glio_batch_clear) drops its selection; glio_window_slide moves a selection with its slot and leaves the
+ * recycled last slot with none.  Plane selection calls leave edge selections alone, and these calls leave plane matches, plane
+ * selections and the plane evaluations alone.  n_active (may be NULL) receives the active edge counts.  The batch call returns
+ * GLIO_ERR_ARG, with nothing changed, on the cases glio_batch_select_random refuses; the window call on bad W, stream_ids or
+ * options. */
+int glio_select_random_edges(glio_ctx* ctx, int W, const int64_t* stream_ids, const glio_select_options* options, int64_t* n_active);
+int glio_batch_select_random_edges(glio_ctx* ctx, const int32_t* cur, const int32_t* oth, int64_t n_pairs, int mode,
+                                   const glio_select_options* options, int64_t* n_active);
+/* The selected edge indices of a slot / pair in draw order, with glio_get_selection's conventions: *n = -1 when all edges are
+ * active; a pair not on the pair list is GLIO_ERR_ARG. */
+int glio_get_edge_selection(glio_ctx* ctx, int slot, int64_t capacity, int32_t* keep, int64_t* n);
+int glio_batch_get_edge_selection(glio_ctx* ctx, int cur, int oth, int64_t capacity, int32_t* keep, int64_t* n);
 
 /* ---- batch minimizer (replaces ceres::Solve of optimizeBatchWithLandMark, Estimator.cpp:3275-3284: SUBSPACE_DOGLEG,
  * nonmonotonic steps, max_num_iter iterations; options == NULL selects exactly those).  The normal equations are
