@@ -11,7 +11,9 @@
 // What is different underneath: ceres::Solve runs glio's trust-region / dogleg restatement (glio_b200/csrc/solver.h)
 // on the normal equations, and residual blocks whose cost function can describe itself as one of GLIO's LiDAR factors
 // (glio::DeviceFactorTraits<Functor>, see INTEGRATION.md) are not evaluated one virtual call at a time on the host:
-// they are uploaded once to a glio_ctx and evaluated by the CUDA kernels (K2 / K2b), which return 6x6 pose blocks.
+// they are uploaded once to a glio_ctx and evaluated by the CUDA kernels, which return 6x6 pose blocks: K2 for the plane
+// factors (LidarPlaneNormFactor, and LidarPlaneNormIncreFactor in a front-end context), K2e for LidarEdgeFactor, K2b for
+// BinaryLidarPlaneNormFactor.
 // Every other cost function (IMU, marginalisation prior, GNSS ...) is evaluated on the host through its own
 // Evaluate(), exactly as Ceres would.  Without a glio_ctx attached everything runs on the host (used by CPU tests).
 #ifndef GLIO_SHIM_CERES_CERES_H_
@@ -36,16 +38,17 @@
 
 namespace glio {
 // ---- self-description of device-evaluable LiDAR factors --------------------------------------------------------
-enum FactorKind { FACTOR_NONE = 0, FACTOR_PLANE_UNARY = 1, FACTOR_PLANE_BINARY = 2 };
+enum FactorKind { FACTOR_NONE = 0, FACTOR_PLANE_UNARY = 1, FACTOR_PLANE_BINARY = 2, FACTOR_EDGE_UNARY = 3, FACTOR_PLANE_INCRE = 4 };
 struct FactorDesc {
   int kind = FACTOR_NONE;
   double cp[3] = {0, 0, 0};           // current point (scan / body frame)
-  double n[3] = {0, 0, 0}, d = 0;     // unary: weight*normal, weight*d  (LidarPlaneNormFactor members)
+  double n[3] = {0, 0, 0}, d = 0;     // unary / incre: weight*normal, weight*d  (LidarPlaneNormFactor, LidarPlaneNormIncreFactor)
   double q_lb[4] = {1, 0, 0, 0}, t_lb[3] = {0, 0, 0};
   double nc[6] = {0, 0, 0, 0, 0, 0};  // binary: local normal + centroid (BinaryLidarPlaneNormFactor)
-  double score = 0;
+  double score = 0;                   // unary / binary: score; edge: the weight s
+  double pa[3] = {0, 0, 0}, pb[3] = {0, 0, 0};   // edge: two points of the map line (LidarEdgeFactor last_point_a / _b)
 };
-// Specialise for the reference's functors (INTEGRATION.md shows the 10 lines for LidarPlaneNormFactor):
+// Specialise for the reference's functors (INTEGRATION.md shows the lines for each LiDAR functor):
 //   template <> struct glio::DeviceFactorTraits<LidarPlaneNormFactor> { static bool describe(const LidarPlaneNormFactor&, FactorDesc*); };
 template <class Functor> struct DeviceFactorTraits { static bool describe(const Functor&, FactorDesc*) { return false; } };
 }  // namespace glio
@@ -259,6 +262,7 @@ class Solver {
     double total_time_in_seconds = -1.0;
     int num_parameter_blocks = -1, num_parameters = -1, num_effective_parameters = -1, num_residual_blocks = -1, num_residuals = -1;
     int num_device_residual_blocks = 0;     // glio extension: residual blocks evaluated by the CUDA kernels
+    int num_device_edge_residual_blocks = 0;   // glio extension: the LidarEdgeFactor blocks among them (K2e)
     bool IsSolutionUsable() const { return termination_type == CONVERGENCE || termination_type == NO_CONVERGENCE || termination_type == USER_SUCCESS; }
     std::string BriefReport() const {
       char b[256];

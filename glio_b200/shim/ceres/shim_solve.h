@@ -60,8 +60,10 @@ inline void Solve(const Solver::Options& options, Problem* problem, Solver::Summ
   const int n = P.n_tan;
   if (n == 0) { S.termination_type = CONVERGENCE; S.message = "no free parameters"; S.initial_cost = S.final_cost = 0; return; }
 
-  // ---- split residual blocks: device-evaluable unary plane factors vs host ----
-  struct Slot { double* t; double* q; std::vector<float> cp, nsd, w; };
+  // ---- split residual blocks: device-evaluable unary factors (plane, edge, incre) vs binary plane factors vs host ----
+  // one slot per keyframe (t, q): its plane matches (LidarPlaneNormFactor, LidarPlaneNormIncreFactor) go to K2, its edges
+  // (LidarEdgeFactor) to K2e
+  struct Slot { double* t; double* q; std::vector<float> cp, nsd, w, ecp, epa, epb; std::vector<double> es; };
   std::vector<Slot> slots;
   std::map<std::pair<double*, double*>, int> slot_of;
   std::vector<const Problem::Residual*> host_blocks;
@@ -73,6 +75,34 @@ inline void Solve(const Solver::Options& options, Problem* problem, Solver::Summ
   glio_ctx* ctx = problem->ctx_;
   glio_params gp;
   if (ctx && glio_get_params(ctx, &gp) != GLIO_OK) ctx = nullptr;
+  auto slot_at = [&](double* t, double* q) -> Slot& {
+    auto key = std::make_pair(t, q);
+    auto it = slot_of.find(key);
+    if (it != slot_of.end()) return slots[it->second];
+    slot_of[key] = (int)slots.size(); slots.push_back(Slot{t, q, {}, {}, {}, {}, {}, {}, {}});
+    return slots.back();
+  };
+  // the kernels apply the context's Huber(huber_delta), or no loss when huber_delta <= 0
+  auto loss_ok = [&](const LossFunction* loss) {
+    const HuberLoss* hl = dynamic_cast<const HuberLoss*>(loss);
+    return (loss == nullptr && gp.huber_delta <= 0) || (hl && hl->a() == gp.huber_delta);
+  };
+  auto quat_ok = [&](double* q) {
+    return P.index.count(q) && problem->blocks_.at(q).size == 4 && dynamic_cast<QuaternionParameterization*>(problem->blocks_.at(q).param) != nullptr;
+  };
+  auto ext_ok = [&](const double* q_lb, const double* t_lb) {
+    bool ok = true;
+    for (int k = 0; k < 4; ++k) ok = ok && q_lb[k] == gp.q_lb[k];
+    for (int k = 0; k < 3; ++k) ok = ok && t_lb[k] == gp.t_lb[k];
+    return ok;
+  };
+  auto f32_3 = [](const double* v) { return is_f32(v[0]) && is_f32(v[1]) && is_f32(v[2]); };
+  auto add_plane = [](Slot& sl, const glio::FactorDesc& d, double w) {
+    for (int k = 0; k < 3; ++k) sl.cp.push_back((float)d.cp[k]);
+    for (int k = 0; k < 3; ++k) sl.nsd.push_back((float)d.n[k]);
+    sl.nsd.push_back((float)d.d); sl.w.push_back((float)w);
+  };
+  int n_edge_dev = 0;
   for (auto& rbp : problem->residual_blocks_) {
     const Problem::Residual* rb = rbp.get();
     glio::FactorDesc d;
@@ -81,26 +111,40 @@ inline void Solve(const Solver::Options& options, Problem* problem, Solver::Summ
     if (!described) d.kind = glio::FACTOR_NONE;
     if (described && d.kind == glio::FACTOR_PLANE_UNARY && rb->params.size() == 2) {
       double* t = rb->params[0]; double* q = rb->params[1];
-      const HuberLoss* hl = dynamic_cast<const HuberLoss*>(rb->loss);
-      const bool loss_ok = (rb->loss == nullptr && gp.huber_delta <= 0) || (hl && hl->a() == gp.huber_delta);
-      const bool blocks_ok = P.index.count(t) && P.index.count(q) && problem->blocks_.at(t).size == 3 && problem->blocks_.at(q).size == 4 &&
-                             dynamic_cast<QuaternionParameterization*>(problem->blocks_.at(q).param) != nullptr;
-      bool ext_ok = true;
-      for (int k = 0; k < 4; ++k) ext_ok = ext_ok && d.q_lb[k] == gp.q_lb[k];
-      for (int k = 0; k < 3; ++k) ext_ok = ext_ok && d.t_lb[k] == gp.t_lb[k];
+      const bool blocks_ok = P.index.count(t) && problem->blocks_.at(t).size == 3 && quat_ok(q);
       // unit_score contexts evaluate every match with score = lidar_const (front-end factor): only blocks with exactly that score qualify
       const double w = gp.unit_score ? 1.0 : d.score / gp.lidar_const;
-      const bool repr = (gp.unit_score ? d.score == gp.lidar_const : (is_f32(w) && gp.lidar_const * (double)(float)w == d.score)) && is_f32(d.cp[0]) && is_f32(d.cp[1]) && is_f32(d.cp[2]) &&
-                        is_f32(d.n[0]) && is_f32(d.n[1]) && is_f32(d.n[2]) && is_f32(d.d);
-      if (loss_ok && blocks_ok && ext_ok && repr) {
-        auto key = std::make_pair(t, q);
-        auto it = slot_of.find(key);
-        int si;
-        if (it == slot_of.end()) { si = (int)slots.size(); slot_of[key] = si; slots.push_back(Slot{t, q, {}, {}, {}}); } else si = it->second;
-        Slot& sl = slots[si];
-        for (int k = 0; k < 3; ++k) sl.cp.push_back((float)d.cp[k]);
-        for (int k = 0; k < 3; ++k) sl.nsd.push_back((float)d.n[k]);
-        sl.nsd.push_back((float)d.d); sl.w.push_back((float)w);
+      const bool repr = (gp.unit_score ? d.score == gp.lidar_const : (is_f32(w) && gp.lidar_const * (double)(float)w == d.score)) && f32_3(d.cp) &&
+                        f32_3(d.n) && is_f32(d.d);
+      if (loss_ok(rb->loss) && blocks_ok && ext_ok(d.q_lb, d.t_lb) && repr) {
+        add_plane(slot_at(t, q), d, w);
+        dev = true;
+      }
+    }
+    // LidarEdgeFactor (LidarKeyframeFactor.h:12-70): blocks (t, q), t without a local parameterization; K2e stores the weight s
+    // as a float, so it has to be one as well
+    if (described && d.kind == glio::FACTOR_EDGE_UNARY && rb->params.size() == 2) {
+      double* t = rb->params[0]; double* q = rb->params[1];
+      const bool blocks_ok = P.index.count(t) && problem->blocks_.at(t).size == 3 && problem->blocks_.at(t).param == nullptr && quat_ok(q);
+      const bool repr = f32_3(d.cp) && f32_3(d.pa) && f32_3(d.pb) && is_f32(d.score);
+      if (loss_ok(rb->loss) && blocks_ok && ext_ok(d.q_lb, d.t_lb) && repr) {
+        Slot& sl = slot_at(t, q);
+        for (int k = 0; k < 3; ++k) { sl.ecp.push_back((float)d.cp[k]); sl.epa.push_back((float)d.pa[k]); sl.epb.push_back((float)d.pb[k]); }
+        sl.es.push_back(d.score);
+        ++n_edge_dev;
+        dev = true;
+      }
+    }
+    // LidarPlaneNormIncreFactor (LidarKeyframeFactor.h:222-257): blocks in the order (q, t), no score and no extrinsic -- K2 computes
+    // exactly that residual in a front-end context (unit_score = 1, lidar_const = 1, identity extrinsic)
+    if (described && d.kind == glio::FACTOR_PLANE_INCRE && rb->params.size() == 2) {
+      double* q = rb->params[0]; double* t = rb->params[1];
+      const double ident_q[4] = {1, 0, 0, 0}, zero_t[3] = {0, 0, 0};
+      const bool ctx_ok = gp.unit_score && gp.lidar_const == 1.0 && ext_ok(ident_q, zero_t);
+      const bool blocks_ok = P.index.count(t) && problem->blocks_.at(t).size == 3 && problem->blocks_.at(t).param == nullptr && quat_ok(q);
+      const bool repr = f32_3(d.cp) && f32_3(d.n) && is_f32(d.d);
+      if (ctx_ok && loss_ok(rb->loss) && blocks_ok && repr) {
+        add_plane(slot_at(t, q), d, 1.0);
         dev = true;
       }
     }
@@ -152,6 +196,18 @@ inline void Solve(const Solver::Options& options, Problem* problem, Solver::Summ
     }
     S.num_device_residual_blocks += (int)slots[k].w.size();
   }
+  // edges: every slot's list is replaced (an empty one where the slot has no edge), so lists and selections that an earlier
+  // Solve or a direct caller left in the context are never evaluated.  A problem without routed edges makes no edge call at all.
+  const bool with_edges = n_edge_dev > 0;
+  if (with_edges) {
+    for (int k = 0; k < W; ++k) {
+      const Slot& sl = slots[k];
+      if (glio_set_edges(ctx, k, sl.ecp.data(), sl.epa.data(), sl.epb.data(), sl.es.data(), (int64_t)sl.es.size()) != GLIO_OK) {
+        S.termination_type = FAILURE; S.message = std::string("glio_set_edges: ") + glio_last_error(ctx); return;
+      }
+    }
+    S.num_device_residual_blocks += n_edge_dev; S.num_device_edge_residual_blocks = n_edge_dev;
+  }
 
   // ---- band of J^T J from the block structure ----
   int hb = 0;
@@ -187,6 +243,7 @@ inline void Solve(const Solver::Options& options, Problem* problem, Solver::Summ
   std::vector<double> x(P.n_amb);
   for (const ActiveBlock& a : P.active) std::memcpy(&x[a.amb_off], a.user, sizeof(double) * a.size);
   std::vector<double> poses((size_t)std::max(W, 1) * 7), Hd((size_t)std::max(W, 1) * 36), gd((size_t)std::max(W, 1) * 6), cd(std::max(W, 1));
+  std::vector<double> He(with_edges ? Hd.size() : 0), ge(with_edges ? gd.size() : 0), ce(with_edges ? cd.size() : 0);
   std::vector<double> bposes((size_t)std::max(KB, 1) * 7), bHd((size_t)std::max(KB, 1) * 36), bHo((size_t)std::max(PB, 1) * 36), bg((size_t)std::max(KB, 1) * 6);
   double fixed_cost = 0; bool fixed_done = false;
 
@@ -201,6 +258,14 @@ inline void Solve(const Solver::Options& options, Problem* problem, Solver::Summ
         for (int i = 0; i < 4; ++i) poses[7 * k + 3 + i] = xa[aq.amb_off + i];
       }
       if (glio_eval_unary(ctx, W, poses.data(), 0, want_jac ? Hd.data() : nullptr, want_jac ? gd.data() : nullptr, cd.data()) != GLIO_OK) return false;
+      if (with_edges) {                      // each keyframe's edge blocks join its plane blocks, as in glio_window_solve
+        if (glio_eval_edge(ctx, W, poses.data(), want_jac ? He.data() : nullptr, want_jac ? ge.data() : nullptr, ce.data()) != GLIO_OK) return false;
+        for (int k = 0; k < W; ++k) cd[k] += ce[k];
+        if (want_jac) {
+          for (size_t i = 0; i < (size_t)W * 36; ++i) Hd[i] += He[i];
+          for (size_t i = 0; i < (size_t)W * 6; ++i) gd[i] += ge[i];
+        }
+      }
       for (int k = 0; k < W; ++k) {
         ct += cd[k];
         if (!want_jac) continue;
