@@ -146,7 +146,8 @@ class Context:
                "k_bin_pair_add", "k_odom_publish",
                "k_lc_load", "k_lc_qhist", "k_lc_qscatter", "k_lc_init", "k_lc_nn", "k_lc_compact", "k_lc_sum0",
                "k_lc_sum1", "k_lc_means", "k_lc_solve", "k_lc_transform", "k_lc_final", "k_lc_fitness",
-               "k_vs_key", "k_vs_hist", "k_vs_scatter", "k_vs_heads", "k_vs_centroid", "k_vs_pack", "k_gm_transform"]
+               "k_vs_key", "k_vs_hist", "k_vs_scatter", "k_vs_heads", "k_vs_centroid", "k_vs_pack", "k_gm_transform",
+               "k_pose_pair_sums", "k_pose_pair_sums_cost", "k_pose_assemble"]
 
     def lib_profile(self, on):
         self._chk(self._lib.glio_profile_enable(self._h, C.c_int(1 if on else 0)))
@@ -929,6 +930,66 @@ Context.batch_get_edges = _batch_get_edges
 Context.batch_set_pair_edges = _batch_set_pair_edges
 Context.eval_binary_edge = _eval_binary_edge
 Context.batch_use_edges = _batch_use_edges
+
+
+# ---------------------------------------------------------------------------------------------------
+# the batch refinement's pose factors (K2p): LidarPoseFactorBatchRelativeAutoDiff and delta_q_factor_auto
+# ---------------------------------------------------------------------------------------------------
+POSE_RELATIVE, POSE_DELTA_Q = 0, 1
+POSE_MAX_KF = 1 << 22                     # keyframe indices of a pose factor are below this (GLIO_POSE_MAX_KF)
+# glio_pose_factor: i, j, kind, active (int32), dq (w, x, y, z), dp (float64)
+POSE_FACTOR_DTYPE = np.dtype([("i", "<i4"), ("j", "<i4"), ("kind", "<i4"), ("active", "<i4"), ("dq", "<f8", (4,)), ("dp", "<f8", (3,))])
+assert POSE_FACTOR_DTYPE.itemsize == 72
+
+
+def pose_factor_records(i, j, kind, dq, dp=None, active=None):
+    """A glio_pose_factor array from per-factor columns (dp defaults to 0, active to 1)."""
+    n = len(i)
+    f = np.zeros(n, POSE_FACTOR_DTYPE)
+    f["i"], f["j"], f["kind"] = i, j, kind
+    f["dq"] = np.asarray(dq, np.float64).reshape(n, 4)
+    if dp is not None:
+        f["dp"] = np.asarray(dp, np.float64).reshape(n, 3)
+    f["active"] = 1 if active is None else np.asarray(active, np.int32)
+    return f
+
+
+def _batch_set_pose_factors(self, factors):
+    """glio_batch_set_pose_factors: replace the pose-factor list (a POSE_FACTOR_DTYPE array; empty empties it)."""
+    f = np.ascontiguousarray(factors, POSE_FACTOR_DTYPE)
+    self._chk(self._lib.glio_batch_set_pose_factors(self._h, _ptr(f) if len(f) else None, C.c_int64(len(f))))
+
+
+def _batch_pose_pair_list(self):
+    """The pose-pair table (a, b), a < b, in order of first appearance."""
+    n = C.c_int64(0)
+    self._chk(self._lib.glio_batch_pose_pair_list(self._h, C.c_int64(0), None, None, C.byref(n)))
+    a = np.zeros(n.value, np.int32); b = np.zeros(n.value, np.int32)
+    self._chk(self._lib.glio_batch_pose_pair_list(self._h, C.c_int64(len(a)), _ptr(a), _ptr(b), C.byref(n)))
+    return a, b
+
+
+def _eval_pose_factors(self, poses, want_jac=True):
+    """glio_eval_pose_factors: the pose blocks alone; Hoff in pose-pair order (d2 cost / d x_a d x_b, rows for a)."""
+    pb = np.ascontiguousarray(poses, np.float64).reshape(-1, 7); K = len(pb)
+    n = C.c_int64(0)
+    self._chk(self._lib.glio_batch_pose_pair_list(self._h, C.c_int64(0), None, None, C.byref(n)))
+    P = int(n.value)
+    Hd = np.zeros((K, 6, 6)) if want_jac else None; Ho = np.zeros((P, 6, 6)) if want_jac else None
+    g = np.zeros((K, 6)) if want_jac else None; cost = np.zeros(1)
+    self._chk(self._lib.glio_eval_pose_factors(self._h, C.c_int(K), _ptr(pb), _ptr(Hd), _ptr(Ho), _ptr(g), _ptr(cost)))
+    return dict(Hdiag=Hd, Hoff=Ho, g=g, cost=float(cost[0]))
+
+
+def _batch_use_pose_factors(self, on):
+    """glio_batch_use_pose_factors: batch solves add the pose blocks (default off)."""
+    self._chk(self._lib.glio_batch_use_pose_factors(self._h, C.c_int(1 if on else 0)))
+
+
+Context.batch_set_pose_factors = _batch_set_pose_factors
+Context.batch_pose_pair_list = _batch_pose_pair_list
+Context.eval_pose_factors = _eval_pose_factors
+Context.batch_use_pose_factors = _batch_use_pose_factors
 
 
 # ---------------------------------------------------------------------------------------------------

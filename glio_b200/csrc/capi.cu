@@ -166,6 +166,11 @@ struct glio_ctx {
   // the pair count or the switch changes; its per-pair sums are added to the plane sums before the one block assembly
   bool batch_use_edges = false, bedge_dirty = true; int bedge_K = -1, bedge_P = -1, n_bedge_items = 0;
   DevBuf<BinEdgeItem> d_bedge_items; DevBuf<int> d_bedge_pstart; DevBuf<double> d_bedge_partials, d_bedge_sums;
+  // pose factors (glio_batch_set_pose_factors, K2p): the pose-pair table, the largest keyframe referenced, and the device plan built
+  // when the list is set: active factors grouped by pair in list order, per-pair starts, per-keyframe incidence lists, pair sums
+  bool batch_use_pose = false;
+  std::vector<std::pair<int, int>> pose_pairs; int pose_max_kf = -1;
+  DevBuf<PoseFactor> d_pose_f; DevBuf<int> d_pose_fstart, d_pose_inc_start; DevBuf<BinIncidence> d_pose_inc; DevBuf<double> d_pose_sums;
 
   // association workspace
   DevBuf<float4> w_pm, w_pmq, w_nsd;
@@ -1703,6 +1708,7 @@ int glio_batch_clear(glio_ctx* c) {
   return guarded(c, [&] {
     GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
     c->frames.clear(); c->pairs.clear(); c->pair_index.clear(); c->bin_dirty = true; c->bedge_dirty = true;
+    c->pose_pairs.clear(); c->pose_max_kf = -1;
   });
 }
 
@@ -2267,11 +2273,14 @@ enum BinBlocks { BIN_PLANES = 0, BIN_PLANES_EDGES = 1, BIN_EDGES = 2 };
 // device evaluation of all active binary residuals -> c->h_bin_diag (K x 28), c->h_bin_off (P x 36): everything is queued
 // (kernels, the all-reduce of a sharded run, the copies to pinned host memory); eval_binary_wait makes the result visible.
 // With edges, each pair's sums are S_plane + S_edge before the one block assembly, so the all-reduce is the same as without.
-void eval_binary_launch(glio_ctx* c, int K, const double* poses, bool want_jac, double huber, BinBlocks what = BIN_PLANES) {
+// add_pose: the pose blocks of K2p are added to the diagonal buffer and stored after the P pair blocks of the off-diagonal one
+void eval_binary_launch(glio_ctx* c, int K, const double* poses, bool want_jac, double huber, BinBlocks what = BIN_PLANES, bool add_pose = false) {
   build_bin_items(c, K);
   if (what != BIN_PLANES) build_bedge_items(c, K);
   const bool add_edges = what == BIN_PLANES_EDGES && c->n_bedge_items > 0;   // no edges: exactly the plane launches
   const int P = (int)c->pairs.size();
+  const int Pp = add_pose ? (int)c->pose_pairs.size() : 0, Pt = P + Pp;
+  if (Pp > 0) { c->d_bin_off.reserve((size_t)(Pt + 1) * 36); c->h_bin_off.reserve((size_t)(Pt + 1) * 36); }
   memcpy(c->h_bin_poses.p, poses, (size_t)K * 7 * sizeof(double));
   GLIO_CUDA_TRY(cudaMemcpyAsync(c->d_bin_poses.p, c->h_bin_poses.p, (size_t)K * 7 * sizeof(double), cudaMemcpyHostToDevice, c->st));
   if (what == BIN_EDGES || add_edges)
@@ -2283,15 +2292,18 @@ void eval_binary_launch(glio_ctx* c, int K, const double* poses, bool want_jac, 
     eval_binary_run(c->d_bin_items.p, c->n_bin_items, c->d_pair_item_start.p, P, K, c->d_bin_poses.p, c->prm.batch_score, huber, want_jac,
                     c->d_bin_partials.p, c->d_pair_sums.p, c->d_kf_inc_start.p, c->d_inc.p, c->d_bin_diag.p, c->d_bin_off.p, c->st, c->lc,
                     add_edges ? c->d_bedge_sums.p : nullptr);
+  if (add_pose)
+    eval_pose_run(c->d_pose_f.p, c->d_pose_fstart.p, Pp, K, c->pose_max_kf + 1, c->d_pose_inc_start.p, c->d_pose_inc.p, c->d_bin_poses.p,
+                  want_jac, /*add*/ true, c->d_pose_sums.p, c->d_bin_diag.p, c->d_bin_off.p + (size_t)P * 36, c->st, c->lc);
   if (c->allreduce) {
     // keyframe-sharded evaluation: every rank holds the same pair list but only its own pairs carry residuals;
     // one sum over ranks of the pose-block buffers per evaluation (SURVEY 8e "pose-block allreduce")
     GLIO_REQUIRE(c->allreduce(c->allreduce_user, c->d_bin_diag.p, (int64_t)K * GLIO_NACC, (void*)c->st) == 0, GLIO_ERR_NCCL, "allreduce hook failed (diag)");
-    if (want_jac && P > 0)
-      GLIO_REQUIRE(c->allreduce(c->allreduce_user, c->d_bin_off.p, (int64_t)P * 36, (void*)c->st) == 0, GLIO_ERR_NCCL, "allreduce hook failed (off)");
+    if (want_jac && Pt > 0)
+      GLIO_REQUIRE(c->allreduce(c->allreduce_user, c->d_bin_off.p, (int64_t)Pt * 36, (void*)c->st) == 0, GLIO_ERR_NCCL, "allreduce hook failed (off)");
   }
   GLIO_CUDA_TRY(cudaMemcpyAsync(c->h_bin_diag.p, c->d_bin_diag.p, (size_t)K * GLIO_NACC * sizeof(double), cudaMemcpyDeviceToHost, c->st));
-  if (want_jac && P > 0) GLIO_CUDA_TRY(cudaMemcpyAsync(c->h_bin_off.p, c->d_bin_off.p, (size_t)P * 36 * sizeof(double), cudaMemcpyDeviceToHost, c->st));
+  if (want_jac && Pt > 0) GLIO_CUDA_TRY(cudaMemcpyAsync(c->h_bin_off.p, c->d_bin_off.p, (size_t)Pt * 36 * sizeof(double), cudaMemcpyDeviceToHost, c->st));
 }
 void eval_binary_wait(glio_ctx* c) { GLIO_CUDA_TRY(cudaStreamSynchronize(c->st)); }
 void eval_binary_blocks(glio_ctx* c, int K, const double* poses, bool want_jac, double huber, BinBlocks what = BIN_PLANES) {
@@ -2329,6 +2341,109 @@ int glio_eval_binary_edge(glio_ctx* c, int K, const double* poses, double* Hdiag
 int glio_batch_use_edges(glio_ctx* c, int on) {
   if (!c) return GLIO_ERR_ARG;
   c->batch_use_edges = on != 0; c->bedge_dirty = true;
+  return GLIO_OK;
+}
+
+static_assert(sizeof(glio_pose_factor) == sizeof(PoseFactor) && offsetof(glio_pose_factor, dq) == offsetof(PoseFactor, dq) &&
+              offsetof(glio_pose_factor, dp) == offsetof(PoseFactor, dp), "PoseFactor must have glio_pose_factor's layout");
+
+int glio_batch_set_pose_factors(glio_ctx* c, const glio_pose_factor* f, int64_t n) {
+  if (!c) return GLIO_ERR_ARG;
+  return guarded(c, [&] {
+    // validate the whole list first: a refused call leaves the previous list in place
+    GLIO_REQUIRE(n >= 0 && (n == 0 || f), GLIO_ERR_ARG, "glio_batch_set_pose_factors: null factor array");
+    GLIO_REQUIRE(n < ((int64_t)1 << 31), GLIO_ERR_ARG, "glio_batch_set_pose_factors: too many factors");
+    for (int64_t k = 0; k < n; ++k)
+      GLIO_REQUIRE(f[k].i >= 0 && f[k].j >= 0 && f[k].i < GLIO_POSE_MAX_KF && f[k].j < GLIO_POSE_MAX_KF && f[k].i != f[k].j &&
+                   (f[k].kind == GLIO_POSE_RELATIVE || f[k].kind == GLIO_POSE_DELTA_Q),
+                   GLIO_ERR_ARG, "glio_batch_set_pose_factors: need i != j, both in [0, GLIO_POSE_MAX_KF), and a known kind");
+    // pair table in order of first appearance; the active factors grouped by pair, list order inside a pair
+    std::map<std::pair<int, int>, int> index;
+    std::vector<std::pair<int, int>> pairs;
+    std::vector<int> fpair((size_t)n), count;
+    int max_kf = -1;
+    for (int64_t k = 0; k < n; ++k) {
+      const std::pair<int, int> key(std::min(f[k].i, f[k].j), std::max(f[k].i, f[k].j));
+      auto it = index.emplace(key, (int)pairs.size()).first;
+      if (it->second == (int)pairs.size()) { pairs.push_back(key); count.push_back(0); }
+      fpair[k] = it->second;
+      if (f[k].active) ++count[it->second];
+      max_kf = std::max(max_kf, key.second);
+    }
+    const int Pp = (int)pairs.size();
+    std::vector<int> fstart(Pp + 1, 0);
+    for (int p = 0; p < Pp; ++p) fstart[p + 1] = fstart[p] + count[p];
+    std::vector<PoseFactor> grouped((size_t)fstart[Pp]);
+    std::vector<int> pos(fstart.begin(), fstart.end() - 1);
+    for (int64_t k = 0; k < n; ++k)
+      if (f[k].active) memcpy(&grouped[pos[fpair[k]]++], &f[k], sizeof(PoseFactor));
+    // per keyframe 0 .. max_kf its pairs in table order (role 0 = a, 1 = b): a counting sort over the keyframes
+    std::vector<int> kstart((size_t)max_kf + 2, 0);
+    for (const auto& pr : pairs) { ++kstart[(size_t)pr.first + 1]; ++kstart[(size_t)pr.second + 1]; }
+    for (size_t k = 1; k < kstart.size(); ++k) kstart[k] += kstart[k - 1];
+    std::vector<BinIncidence> flat((size_t)2 * Pp);
+    std::vector<int> fill(kstart.begin(), kstart.end() - 1);
+    for (int p = 0; p < Pp; ++p) { flat[fill[pairs[p].first]++] = BinIncidence{p, 0}; flat[fill[pairs[p].second]++] = BinIncidence{p, 1}; }
+    // the new plan goes to buffers of its own; the context takes them only when every upload has completed, so a failed call
+    // leaves the previous list and its buffers as they were
+    DevBuf<PoseFactor> d_f; DevBuf<int> d_fstart, d_kstart; DevBuf<BinIncidence> d_inc; DevBuf<double> d_sums;
+    d_f.reserve(grouped.size() + 1); d_fstart.reserve(fstart.size()); d_kstart.reserve(kstart.size());
+    d_inc.reserve(flat.size() + 1); d_sums.reserve((size_t)(Pp + 1) * GLIO_NACC_POSE);
+    if (!grouped.empty()) GLIO_CUDA_TRY(cudaMemcpyAsync(d_f.p, grouped.data(), grouped.size() * sizeof(PoseFactor), cudaMemcpyHostToDevice, c->st));
+    GLIO_CUDA_TRY(cudaMemcpyAsync(d_fstart.p, fstart.data(), fstart.size() * sizeof(int), cudaMemcpyHostToDevice, c->st));
+    GLIO_CUDA_TRY(cudaMemcpyAsync(d_kstart.p, kstart.data(), kstart.size() * sizeof(int), cudaMemcpyHostToDevice, c->st));
+    if (!flat.empty()) GLIO_CUDA_TRY(cudaMemcpyAsync(d_inc.p, flat.data(), flat.size() * sizeof(BinIncidence), cudaMemcpyHostToDevice, c->st));
+    GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));   // also: no evaluation still reads the buffers released below
+    c->d_pose_f = std::move(d_f); c->d_pose_fstart = std::move(d_fstart); c->d_pose_inc_start = std::move(d_kstart);
+    c->d_pose_inc = std::move(d_inc); c->d_pose_sums = std::move(d_sums);
+    c->pose_pairs.swap(pairs); c->pose_max_kf = max_kf;
+  });
+}
+
+int glio_batch_pose_pair_list(glio_ctx* c, int64_t capacity, int32_t* a, int32_t* b, int64_t* n_pairs) {
+  if (!c) return GLIO_ERR_ARG;
+  return guarded(c, [&] {
+    const int64_t P = (int64_t)c->pose_pairs.size();
+    if (n_pairs) *n_pairs = P;
+    if (!a && !b) return;
+    GLIO_REQUIRE(capacity >= P, GLIO_ERR_ARG, "glio_batch_pose_pair_list: capacity too small");
+    for (int64_t k = 0; k < P; ++k) { if (a) a[k] = c->pose_pairs[k].first; if (b) b[k] = c->pose_pairs[k].second; }
+  });
+}
+
+int glio_eval_pose_factors(glio_ctx* c, int K, const double* poses, double* Hdiag, double* Hoff, double* g, double* cost) {
+  if (!c) return GLIO_ERR_ARG;
+  return guarded(c, [&] {
+    GLIO_REQUIRE(K > 0 && poses, GLIO_ERR_ARG, "bad arguments");
+    GLIO_REQUIRE(c->pose_max_kf < K, GLIO_ERR_ARG, "glio_eval_pose_factors: a pose factor references a keyframe outside [0, K)");
+    const int Pp = (int)c->pose_pairs.size();
+    const bool want_jac = Hdiag || Hoff || g;
+    c->d_bin_diag.reserve((size_t)K * GLIO_NACC); c->h_bin_diag.reserve((size_t)K * GLIO_NACC);
+    c->d_bin_off.reserve((size_t)(Pp + 1) * 36); c->h_bin_off.reserve((size_t)(Pp + 1) * 36);
+    c->d_bin_poses.reserve((size_t)K * 7); c->h_bin_poses.reserve((size_t)K * 7);
+    memcpy(c->h_bin_poses.p, poses, (size_t)K * 7 * sizeof(double));
+    GLIO_CUDA_TRY(cudaMemcpyAsync(c->d_bin_poses.p, c->h_bin_poses.p, (size_t)K * 7 * sizeof(double), cudaMemcpyHostToDevice, c->st));
+    eval_pose_run(c->d_pose_f.p, c->d_pose_fstart.p, Pp, K, c->pose_max_kf + 1, c->d_pose_inc_start.p, c->d_pose_inc.p, c->d_bin_poses.p,
+                  want_jac, /*add*/ false, c->d_pose_sums.p, c->d_bin_diag.p, c->d_bin_off.p, c->st, c->lc);
+    if (c->allreduce) {
+      GLIO_REQUIRE(c->allreduce(c->allreduce_user, c->d_bin_diag.p, (int64_t)K * GLIO_NACC, (void*)c->st) == 0, GLIO_ERR_NCCL, "allreduce hook failed (diag)");
+      if (want_jac && Pp > 0)
+        GLIO_REQUIRE(c->allreduce(c->allreduce_user, c->d_bin_off.p, (int64_t)Pp * 36, (void*)c->st) == 0, GLIO_ERR_NCCL, "allreduce hook failed (off)");
+    }
+    GLIO_CUDA_TRY(cudaMemcpyAsync(c->h_bin_diag.p, c->d_bin_diag.p, (size_t)K * GLIO_NACC * sizeof(double), cudaMemcpyDeviceToHost, c->st));
+    if (want_jac && Pp > 0) GLIO_CUDA_TRY(cudaMemcpyAsync(c->h_bin_off.p, c->d_bin_off.p, (size_t)Pp * 36 * sizeof(double), cudaMemcpyDeviceToHost, c->st));
+    GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
+    unpack_blocks(c->h_bin_diag.p, K, Hdiag, g, nullptr);
+    double ct = 0;
+    for (int k = 0; k < K; ++k) ct += c->h_bin_diag.p[(size_t)k * GLIO_NACC + 27];
+    if (Hoff) memcpy(Hoff, c->h_bin_off.p, (size_t)Pp * 36 * sizeof(double));
+    if (cost) *cost = ct;
+  });
+}
+
+int glio_batch_use_pose_factors(glio_ctx* c, int on) {
+  if (!c) return GLIO_ERR_ARG;
+  c->batch_use_pose = on != 0;
   return GLIO_OK;
 }
 
@@ -2385,8 +2500,11 @@ int glio_batch_solve(glio_ctx* c, int K, double* poses, double* speed_bias, glio
     const bool sb = speed_bias != nullptr;
     const StateLayout L(K, sb);
     const int nt = L.nt, n = K * nt;
+    const bool add_pose = c->batch_use_pose && !c->pose_pairs.empty();
+    GLIO_REQUIRE(!add_pose || c->pose_max_kf < K, GLIO_ERR_ARG, "glio_batch_solve: a pose factor references a keyframe outside [0, K)");
     int span = 1;
     for (auto& p : c->pairs) span = std::max(span, std::abs(p->cur - p->oth));
+    if (add_pose) for (auto& p : c->pose_pairs) span = std::max(span, p.second - p.first);
     const int hb = (span + 1) * nt - 1;
     TrustRegionDogleg solver(L.blocks(), solver_options_from(o));
     std::vector<double> x((size_t)K * L.na), pz((size_t)K * 7), sz((size_t)K * 9);
@@ -2395,7 +2513,7 @@ int glio_batch_solve(glio_ctx* c, int K, double* poses, double* speed_bias, glio
       L.unpack(xa, pz.data(), sz.data());
       // the device evaluates the LiDAR pairs (and a sharded run sums them over the ranks) while the host evaluates its own
       // factors into the freshly reset band; the device blocks are added when they have arrived
-      eval_binary_launch(c, K, pz.data(), want_jac, 0.0, c->batch_use_edges ? BIN_PLANES_EDGES : BIN_PLANES);
+      eval_binary_launch(c, K, pz.data(), want_jac, 0.0, c->batch_use_edges ? BIN_PLANES_EDGES : BIN_PLANES, add_pose);
       double ct = 0;
       int hrc = 0;
       if (want_jac) { H->reset(n, hb); std::fill(g, g + n, 0.0); }
@@ -2408,8 +2526,9 @@ int glio_batch_solve(glio_ctx* c, int K, double* poses, double* speed_bias, glio
         double* a = H->a.data();
         add_diag_blocks(H, c->h_bin_diag.p, K, nt);
         for (int k = 0; k < K; ++k) for (int p = 0; p < 6; ++p) g[nt * k + p] += c->h_bin_diag.p[(size_t)k * GLIO_NACC + 21 + p];
-        for (size_t pi = 0; pi < c->pairs.size(); ++pi) {
-          const int kc = c->pairs[pi]->cur, ko = c->pairs[pi]->oth;
+        const size_t P = c->pairs.size(), Pt = P + (add_pose ? c->pose_pairs.size() : 0);
+        for (size_t pi = 0; pi < Pt; ++pi) {                           // LiDAR pairs (cur, oth), then pose pairs (a, b)
+          const int kc = pi < P ? c->pairs[pi]->cur : c->pose_pairs[pi - P].first, ko = pi < P ? c->pairs[pi]->oth : c->pose_pairs[pi - P].second;
           const double* ob = c->h_bin_off.p + pi * 36;                 // d2 cost / d x_cur[p] d x_oth[q]
           if (kc > ko) {                                               // rows of cur, six contiguous band entries each
             for (int p = 0; p < 6; ++p) { double* row = a + (size_t)(nt * kc + p) * w + (nt * ko - (nt * kc + p) + H->hb); for (int q = 0; q < 6; ++q) row[q] += ob[6 * p + q]; }

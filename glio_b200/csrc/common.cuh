@@ -349,6 +349,20 @@ struct BinEdgeItem {
 void eval_binary_edge_run(const BinEdgeItem* d_items, int nitems, const int* d_pair_item_start, int n_pairs, const double* d_poses,
                           bool want_jac, double* d_partials, double* d_pair_sums, cudaStream_t st, LaunchCounter& lc);
 
+// ---- K2p (eval.cu): the batch refinement's pose factors, LidarPoseFactorBatchRelativeAutoDiff (kind 0, 6 rows) and
+// delta_q_factor_auto (kind 1, 3 rows); the layout of the public glio_pose_factor
+struct PoseFactor { int32_t i, j, kind, active; double dq[4]; double dp[3]; };
+// Per distinct keyframe pair (a, b), a < b, the sums of its factors' 12 x 12 J^T J, J^T r and cost over the tangent columns
+// (t_a, d_a, t_b, d_b): aa upper-triangular (21), bb upper-triangular (21), ab row-major (36), g (12), cost.
+constexpr int GLIO_NACC_POSE = 91;
+// k_pose_pair_sums: the factors of pair p are f[fstart[p] .. fstart[p+1]) in list order -> d_sums (n_pairs x 91);
+// k_pose_assemble: per keyframe k < n_inc_kf the pairs of its incidence list (role 0 = a, 1 = b), in order, summed into d_diag
+// (K x 28, added to its contents when add, else written; the cost goes to a) and, with want_jac, the ab blocks -> d_off (n_pairs x 36).
+// Two launches whatever K; with n_pairs = 0 only the assembly runs.
+void eval_pose_run(const PoseFactor* d_f, const int* d_fstart, int n_pairs, int K, int n_inc_kf, const int* d_kf_inc_start,
+                   const BinIncidence* d_inc, const double* d_poses, bool want_jac, bool add, double* d_sums, double* d_diag, double* d_off,
+                   cudaStream_t st, LaunchCounter& lc);
+
 // ---- front-end feature extraction (features.cu; Preprocessing.cpp:529-655)
 constexpr int FEAT_MAX_SHARP = 12, FEAT_MAX_LESS_SHARP = 60, FEAT_MAX_FLAT = 24;   // per ring: 6 sectors x (2, 10, 4)
 struct FeatArgs {

@@ -602,4 +602,182 @@ void eval_binary_edge_run(const BinEdgeItem* d_items, int nitems, const int* d_p
   GLIO_CUDA_TRY(cudaGetLastError());
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// K2p: the batch refinement's pose factors (glio_batch_set_pose_factors), as their AutoDiff functors evaluate them with Eigen:
+//   relative  (LidarPoseFactorBatchRelativeAutoDiff, LidarPoseFactor.h:54-95; blocks t_i, q_i, t_j, q_j):
+//     E = (dq^-1 q_i^-1) q_j,  r[0..2] = 10 (2 vec(E)),  r[3..5] = 20 (q_i^-1 (t_j - t_i) - dp)
+//   attitude  (delta_q_factor_auto, LidarKeyframeFactor.h:281-303; blocks q_i, q_j):  r = 10000 vec(E)
+// with q^-1 = conj(q) / |q|^2 (0 for q = 0) and q v = v + 2w (u x v) + 2 u x (u x v), for any (not necessarily unit) q.
+// Tangent columns: the directional derivative of r along Ceres' QuaternionParameterization column k, d q = [0, e_k] (x) q, i.e. the
+// ambient Jacobian times the 4 x 3 local Jacobian, exact at non-unit quaternions too.
+// Layout: one half-warp per distinct pair (a, b); lane l < 12 owns tangent column l of (t_a, d_a, t_b, d_b), walks the pair's
+// factors in list order and keeps row l of the pair's 12 x 12 J^T J and entry l of J^T r in registers (12 + 1 doubles); the other
+// columns come by shuffle.  k_pose_assemble then sums each keyframe's pairs in incidence order.  No floating-point atomics.
+// ---------------------------------------------------------------------------------------------------------------
+constexpr int NP = GLIO_NACC_POSE;
+constexpr int POSE_T = 128;   // 8 pairs per block
+
+__device__ __forceinline__ void qmul(const double a[4], const double b[4], double o[4]) {   // Eigen's quaternion product, (w, x, y, z)
+  o[0] = a[0] * b[0] - a[1] * b[1] - a[2] * b[2] - a[3] * b[3];
+  o[1] = a[0] * b[1] + a[1] * b[0] + a[2] * b[3] - a[3] * b[2];
+  o[2] = a[0] * b[2] + a[2] * b[0] + a[3] * b[1] - a[1] * b[3];
+  o[3] = a[0] * b[3] + a[3] * b[0] + a[1] * b[2] - a[2] * b[1];
+}
+// Eigen's q * v:  uv = 2 (u x v);  v + w uv + u x uv
+__device__ __forceinline__ void qrot(const double q[4], const double v[3], double o[3]) {
+  const double uv[3] = {2.0 * (q[2] * v[2] - q[3] * v[1]), 2.0 * (q[3] * v[0] - q[1] * v[2]), 2.0 * (q[1] * v[1] - q[2] * v[0])};
+  o[0] = v[0] + q[0] * uv[0] + (q[2] * uv[2] - q[3] * uv[1]);
+  o[1] = v[1] + q[0] * uv[1] + (q[3] * uv[0] - q[1] * uv[2]);
+  o[2] = v[2] + q[0] * uv[2] + (q[1] * uv[1] - q[2] * uv[0]);
+}
+// derivative of q * v along d q (v fixed): dw uv + w duv + du x uv + u x duv,  duv = 2 (du x v)
+__device__ __forceinline__ void qrot_d(const double q[4], const double d[4], const double v[3], double o[3]) {
+  const double uv[3] = {2.0 * (q[2] * v[2] - q[3] * v[1]), 2.0 * (q[3] * v[0] - q[1] * v[2]), 2.0 * (q[1] * v[1] - q[2] * v[0])};
+  const double du[3] = {2.0 * (d[2] * v[2] - d[3] * v[1]), 2.0 * (d[3] * v[0] - d[1] * v[2]), 2.0 * (d[1] * v[1] - d[2] * v[0])};
+  o[0] = d[0] * uv[0] + q[0] * du[0] + (d[2] * uv[2] - d[3] * uv[1]) + (q[2] * du[2] - q[3] * du[1]);
+  o[1] = d[0] * uv[1] + q[0] * du[1] + (d[3] * uv[0] - d[1] * uv[2]) + (q[3] * du[0] - q[1] * du[2]);
+  o[2] = d[0] * uv[2] + q[0] * du[2] + (d[1] * uv[1] - d[2] * uv[0]) + (q[1] * du[1] - q[2] * du[0]);
+}
+
+__device__ __forceinline__ int sym6(int p, int q) { return p * 6 - p * (p - 1) / 2 + (q - p); }   // p <= q
+
+template <bool WANT_JAC>
+__global__ void __launch_bounds__(POSE_T) k_pose_pair_sums(const PoseFactor* __restrict__ fl, const int* __restrict__ fstart, int n_pairs,
+                                                           const double* __restrict__ poses, double* __restrict__ sums) {
+  const int p = blockIdx.x * (POSE_T / 16) + (threadIdx.x >> 4);
+  if (p >= n_pairs) return;                       // a half-warp leaves as a whole; the shuffles below stay inside it
+  const unsigned mask = 0xffffu << (threadIdx.x & 16);
+  const int l = threadIdx.x & 15, comp = l % 6;
+  double H[12], gl = 0.0, cost = 0.0;
+#pragma unroll
+  for (int m = 0; m < 12; ++m) H[m] = 0.0;
+  const int f1 = fstart[p + 1];
+  for (int k = fstart[p]; k < f1; ++k) {
+    const PoseFactor F = fl[k];
+    const double* Pi = poses + 7 * F.i;
+    const double* Pj = poses + 7 * F.j;
+    const double qi[4] = {Pi[3], Pi[4], Pi[5], Pi[6]}, qj[4] = {Pj[3], Pj[4], Pj[5], Pj[6]};
+    const double v[3] = {Pj[0] - Pi[0], Pj[1] - Pi[1], Pj[2] - Pi[2]};
+    const double nd = F.dq[0] * F.dq[0] + F.dq[1] * F.dq[1] + F.dq[2] * F.dq[2] + F.dq[3] * F.dq[3];
+    double A[4] = {0.0, 0.0, 0.0, 0.0};
+    if (nd > 0.0) { A[0] = F.dq[0] / nd; A[1] = -F.dq[1] / nd; A[2] = -F.dq[2] / nd; A[3] = -F.dq[3] / nd; }
+    const double n2 = qi[0] * qi[0] + qi[1] * qi[1] + qi[2] * qi[2] + qi[3] * qi[3];
+    double B[4] = {0.0, 0.0, 0.0, 0.0};
+    if (n2 > 0.0) { B[0] = qi[0] / n2; B[1] = -qi[1] / n2; B[2] = -qi[2] / n2; B[3] = -qi[3] / n2; }
+    double AB[4], E[4]; qmul(A, B, AB); qmul(AB, qj, E);
+    const bool rel = F.kind == 0;
+    double r[6];
+    if (rel) {
+      double Bv[3]; qrot(B, v, Bv);
+#pragma unroll
+      for (int m = 0; m < 3; ++m) { r[m] = 10.0 * (2.0 * E[1 + m]); r[3 + m] = 20.0 * (Bv[m] - F.dp[m]); }
+    } else {
+#pragma unroll
+      for (int m = 0; m < 3; ++m) { r[m] = 10000.0 * E[1 + m]; r[3 + m] = 0.0; }
+    }
+    cost += 0.5 * (r[0] * r[0] + r[1] * r[1] + r[2] * r[2] + r[3] * r[3] + r[4] * r[4] + r[5] * r[5]);
+    if (WANT_JAC) {
+      double c[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};   // column l of J
+      const bool is_i = (l < 6) == (F.i < F.j);
+      if (l < 12 && comp < 3) {
+        if (rel) {
+          const double e[3] = {comp == 0 ? 1.0 : 0.0, comp == 1 ? 1.0 : 0.0, comp == 2 ? 1.0 : 0.0};
+          double Be[3]; qrot(B, e, Be);
+          const double s = is_i ? -20.0 : 20.0;
+          c[3] = s * Be[0]; c[4] = s * Be[1]; c[5] = s * Be[2];
+        }
+      } else if (l < 12) {
+        const double w = is_i ? qi[0] : qj[0], x = is_i ? qi[1] : qj[1], y = is_i ? qi[2] : qj[2], z = is_i ? qi[3] : qj[3];
+        // [0, e_k] (x) q, k = comp - 3 (the columns of QuaternionParameterization::ComputeJacobian)
+        const double d[4] = {comp == 3 ? -x : comp == 4 ? -y : -z, comp == 3 ? w : comp == 4 ? z : -y,
+                             comp == 3 ? -z : comp == 4 ? w : x, comp == 3 ? y : comp == 4 ? -x : w};
+        double dE[4];
+        if (is_i) {
+          // d(conj(q) / |q|^2) = (conj(d) - B d|q|^2) / |q|^2, as the Jet quotient forms it
+          double dB[4] = {0.0, 0.0, 0.0, 0.0};
+          if (n2 > 0.0) {
+            const double dn = 2.0 * (qi[0] * d[0] + qi[1] * d[1] + qi[2] * d[2] + qi[3] * d[3]);
+            dB[0] = (d[0] - B[0] * dn) / n2; dB[1] = (-d[1] - B[1] * dn) / n2; dB[2] = (-d[2] - B[2] * dn) / n2; dB[3] = (-d[3] - B[3] * dn) / n2;
+          }
+          double t4[4]; qmul(A, dB, t4); qmul(t4, qj, dE);
+          if (rel) { double dBv[3]; qrot_d(B, dB, v, dBv); c[3] = 20.0 * dBv[0]; c[4] = 20.0 * dBv[1]; c[5] = 20.0 * dBv[2]; }
+        } else {
+          qmul(AB, d, dE);
+        }
+        const double s = rel ? 20.0 : 10000.0;
+        c[0] = s * dE[1]; c[1] = s * dE[2]; c[2] = s * dE[3];
+      }
+      gl += c[0] * r[0] + c[1] * r[1] + c[2] * r[2] + c[3] * r[3] + c[4] * r[4] + c[5] * r[5];
+#pragma unroll
+      for (int m = 0; m < 12; ++m) {
+        double s = 0.0;
+#pragma unroll
+        for (int q = 0; q < 6; ++q) s += c[q] * __shfl_sync(mask, c[q], m, 16);
+        H[m] += s;
+      }
+    }
+  }
+  double* S = sums + (size_t)p * NP;
+  if (WANT_JAC) {
+    if (l < 6) {
+#pragma unroll
+      for (int m = 0; m < 6; ++m) if (m >= l) S[sym6(l, m)] = H[m];
+#pragma unroll
+      for (int m = 0; m < 6; ++m) S[42 + 6 * l + m] = H[6 + m];
+    } else if (l < 12) {
+#pragma unroll
+      for (int m = 6; m < 12; ++m) if (m >= l) S[21 + sym6(l - 6, m - 6)] = H[m];
+    }
+    if (l < 12) S[78 + l] = gl;
+  }
+  if (l == 0) S[90] = cost;
+}
+
+// thread t < K*28: diag entry (kf, e) (the GLIO_NACC layout) from the kf's pairs in incidence order; then, with WANT_JAC, one
+// thread per entry of the n_pairs ab blocks
+template <bool WANT_JAC>
+__global__ void __launch_bounds__(256) k_pose_assemble(const double* __restrict__ S, int K, int n_pairs, int n_inc_kf,
+                                                       const int* __restrict__ kf_inc_start, const BinIncidence* __restrict__ inc, bool add,
+                                                       double* __restrict__ diag, double* __restrict__ off) {
+  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const int64_t nd = (int64_t)K * GLIO_NACC;
+  if (t < nd) {
+    const int kf = (int)(t / GLIO_NACC), e = (int)(t - (int64_t)kf * GLIO_NACC);
+    double v = 0.0;
+    if (kf < n_inc_kf && (WANT_JAC || e == 27)) {
+      for (int i = kf_inc_start[kf]; i < kf_inc_start[kf + 1]; ++i) {
+        const double* s = S + (size_t)inc[i].pair * NP;
+        const int role = inc[i].role;
+        if (e < 21) v += s[21 * role + e];                       // aa | bb
+        else if (e < 27) v += s[78 + 6 * role + (e - 21)];      // g_a | g_b
+        else if (role == 0) v += s[90];                         // the cost goes to a
+      }
+    }
+    diag[t] = add ? diag[t] + v : v;
+  } else if (WANT_JAC) {
+    const int64_t o = t - nd;
+    if (o < (int64_t)n_pairs * 36) {
+      const int64_t pr = o / 36;
+      off[o] = S[pr * NP + 42 + (o - pr * 36)];
+    }
+  }
+}
+
+void eval_pose_run(const PoseFactor* d_f, const int* d_fstart, int n_pairs, int K, int n_inc_kf, const int* d_kf_inc_start,
+                   const BinIncidence* d_inc, const double* d_poses, bool want_jac, bool add, double* d_sums, double* d_diag, double* d_off,
+                   cudaStream_t st, LaunchCounter& lc) {
+  if (n_pairs > 0) {
+    const int nb = (n_pairs + POSE_T / 16 - 1) / (POSE_T / 16);
+    lc.begin(want_jac ? "k_pose_pair_sums" : "k_pose_pair_sums_cost", st);
+    (want_jac ? k_pose_pair_sums<true> : k_pose_pair_sums<false>)<<<nb, POSE_T, 0, st>>>(d_f, d_fstart, n_pairs, d_poses, d_sums);
+    lc.end(st);
+  }
+  const int64_t n = (int64_t)K * GLIO_NACC + (want_jac ? (int64_t)n_pairs * 36 : 0);
+  lc.begin("k_pose_assemble", st);
+  (want_jac ? k_pose_assemble<true> : k_pose_assemble<false>)<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(
+      d_sums, K, n_pairs, n_inc_kf, d_kf_inc_start, d_inc, add, d_diag, d_off);
+  lc.end(st);
+  GLIO_CUDA_TRY(cudaGetLastError());
+}
+
 }  // namespace glio

@@ -38,6 +38,13 @@ def owner_of(cur, K, world):
     return np.searchsorted(bounds, cur, side="right") - 1
 
 
+def pose_factor_active(i, j, K, world, rank):
+    """The active mask of one rank's pose-factor list: a factor belongs to the rank that owns its lower keyframe (owner_of's
+    contiguous ranges).  Every rank passes the same list, so every rank gets the same pose-pair layout."""
+    lo = np.minimum(np.asarray(i), np.asarray(j))
+    return (owner_of(lo, K, world) == rank).astype(np.int32)
+
+
 def frames_needed(cur, oth, owned_mask):
     """Frames a rank must hold: its own cur frames plus the searched frames of its pairs (the +-2*search_range halo)."""
     return np.unique(np.concatenate([cur[owned_mask], oth[owned_mask]]))

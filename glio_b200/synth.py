@@ -237,6 +237,81 @@ def batch_edge_problem(K=200, Q=10_000, seed=SEED0 + 3, search_range=6, frames=N
     return dict(corner_scans=scans, poses_true=truth, poses_init=init, K=K, Q=Q, search_range=search_range, seed=seed)
 
 
+def _unify(q):
+    """unifyQuaternion: w >= 0."""
+    return q if q[0] >= 0 else -q
+
+
+def _qinv(q):
+    return quat_conj(q) / np.dot(q, q)
+
+
+def attitude_factors(kf, search_range, start_idx=0, end=None):
+    """The delta_q_factor_auto list of optimizeBatchWithLandMark (Estimator.cpp:2831-2891, added at both fusion levels) over
+    keyframe poses kf (K, 7) = (t, q w x y z), i.e. pose_info_keyframe: per i a backward and then a forward walk, each accepted j a
+    factor (i, j, dq = unify(q_i)^-1 q_j).  p_range > 5 / search_range is integer division; p_tmp and factor_count carry over
+    from the backward into the forward walk, which a full backward walk resets.  Returns (i, j, dq (n, 4))."""
+    end = len(kf) if end is None else end
+    thr = 5 // search_range
+    I, J, DQ = [], [], []
+    for i in range(start_idx, end):
+        qi = _unify(kf[i, 3:]); p_tmp = kf[i, :3]
+        count = 0
+        for walk in (range(i, start_idx - 1, -1), range(i, end)):
+            for j in walk:
+                if count == search_range:
+                    count = 0
+                    break
+                if j == i:
+                    continue
+                pj = kf[j, :3]
+                if np.linalg.norm(p_tmp - pj) > thr:
+                    p_tmp = pj
+                    I.append(i); J.append(j); DQ.append(quat_mul(_qinv(qi), kf[j, 3:]))
+                    count += 1
+    return np.asarray(I, np.int32), np.asarray(J, np.int32), np.asarray(DQ, np.float64).reshape(-1, 4)
+
+
+def relative_pose_factors(kf, search_range, start_idx=0, end=None):
+    """The LidarPoseFactorBatchRelativeAutoDiff list of sms_fusion_level 0 (Estimator.cpp:2897-2954): two loops over
+    ms_i = 1 .. search_range - 1, so interior pairs appear twice, always with i < j; dq = q_i^-1 q_j, dp = q_i^-1 (p_j - p_i).
+    Returns (i, j, dq (n, 4), dp (n, 3))."""
+    end = len(kf) if end is None else end
+    pairs = [(idx - m, idx) for idx in range(start_idx + search_range, end) for m in range(1, search_range)]
+    pairs += [(idx, idx + m) for idx in range(start_idx, end - search_range) for m in range(1, search_range)]
+    I, J, DQ, DP = [], [], [], []
+    for i, j in pairs:
+        qinv = _qinv(kf[i, 3:])
+        I.append(i); J.append(j); DQ.append(quat_mul(qinv, kf[j, 3:]))
+        DP.append(quat_to_R(qinv) @ (kf[j, :3] - kf[i, :3]))
+    return (np.asarray(I, np.int32), np.asarray(J, np.int32), np.asarray(DQ, np.float64).reshape(-1, 4),
+            np.asarray(DP, np.float64).reshape(-1, 3))
+
+
+def pose_graph_problem(K=200, seed=SEED0 + 16, search_range=6, level=0, sig_t=0.03, sig_r_deg=0.2):
+    """The batch refinement's pose factors on a seeded trajectory.  kf: the keyframe poses the factors are measured from
+    (pose_info_keyframe: truth + N(0, 0.01 m), N(0, 0.05 deg)); poses_init: the states (truth + N(0, sig_t), N(0, sig_r_deg)).
+    level 0: the attitude factors, then the relative factors, in the Estimator's order, as columns i, j, kind, dq, dp (see
+    api.pose_factor_records); level 1: the attitude factors alone, and the LiDAR pairs dist.batch_pairs(K, search_range)."""
+    rng = np.random.default_rng(seed)
+    truth = trajectory(K, rng)
+    kf = perturb(truth, rng, sig_t=0.01, sig_r_deg=0.05)
+    init = perturb(truth, rng, sig_t=sig_t, sig_r_deg=sig_r_deg)
+    ai, aj, adq = attitude_factors(kf, search_range)
+    if level == 0:
+        ri, rj, rdq, rdp = relative_pose_factors(kf, search_range)
+    else:
+        ri, rj, rdq, rdp = (np.zeros(0, np.int32),) * 2 + (np.zeros((0, 4)), np.zeros((0, 3)))
+    out = dict(K=K, poses_true=truth, kf=kf, poses_init=init, search_range=search_range, seed=seed, level=level,
+               i=np.concatenate([ai, ri]), j=np.concatenate([aj, rj]),
+               kind=np.concatenate([np.ones(len(ai), np.int32), np.zeros(len(ri), np.int32)]),
+               dq=np.concatenate([adq, rdq]), dp=np.concatenate([np.zeros((len(ai), 3)), rdp]))
+    if level == 1:
+        from .dist import batch_pairs
+        out["pairs"] = batch_pairs(K, search_range)
+    return out
+
+
 def raw_elevations(n_rings):
     """Elevation table (degrees) of a raw sweep for the ring rules of Preprocessing.cpp:441-483: every line sits inside its ring's
     interval, plus lines each rule treats specially.  16: VLP-16's -15..15 step 2, one line at -16.5 that int() truncates toward

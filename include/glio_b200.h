@@ -616,7 +616,7 @@ int glio_batch_select_random(glio_ctx* ctx, const int32_t* cur, const int32_t* o
                              const glio_select_options* options, int64_t* n_active);
 int glio_batch_get_selection(glio_ctx* ctx, int cur, int oth, int64_t capacity, int32_t* keep, int64_t* n);
 int glio_batch_pair_list(glio_ctx* ctx, int64_t capacity, int32_t* cur, int32_t* oth, int64_t* n_pairs);
-int glio_batch_clear(glio_ctx* ctx);
+int glio_batch_clear(glio_ctx* ctx);   /* also empties the pose-factor list (glio_batch_set_pose_factors) */
 
 /* Creates (empty) pair entries in the given order without associating them: on a keyframe-sharded multi-GPU run
  * every rank declares the SAME global pair list and then associates only the pairs it owns, so the block
@@ -759,6 +759,40 @@ int glio_eval_binary_edge(glio_ctx* ctx, int K, const double* poses, double* Hdi
  * glio_eval_binary never includes edges.  The edge work-item plan is rebuilt only when an edge list, K, the pair count or this
  * switch changes. */
 int glio_batch_use_edges(glio_ctx* ctx, int on);
+
+/* ---- K2p: the batch refinement's pose factors (optimizeBatchWithLandMark, Estimator.cpp:2831-2954), evaluated on the device.
+ *   GLIO_POSE_RELATIVE (LidarPoseFactorBatchRelativeAutoDiff, blocks t_i, q_i, t_j, q_j, 6 rows, no loss):
+ *     r[0..2] = 10 (2 vec(dq^-1 q_i^-1 q_j)),  r[3..5] = 20 (q_i^-1 (t_j - t_i) - dp)
+ *   GLIO_POSE_DELTA_Q (delta_q_factor_auto, blocks q_i, q_j, 3 rows, no loss):  r = 10000 vec(dq^-1 q_i^-1 q_j)
+ * with Eigen's semantics at any quaternion: q^-1 = conj(q) / |q|^2 (0 for q = 0), q v = v + 2w (u x v) + 2 u x (u x v).  dq is
+ * (w, x, y, z); dp is read by the relative kind only.  The Jacobian columns are the tangent columns of Ceres'
+ * QuaternionParameterization (ambient Jacobian times its 4 x 3 local Jacobian at the current q) and the translation columns.
+ * The weights are the reference's, fixed per kind.  active = 0: the factor is not evaluated by this context, but it still makes
+ * its pair entry, so keyframe-sharded ranks that pass one list with their own active masks share one pair layout. */
+enum { GLIO_POSE_RELATIVE = 0, GLIO_POSE_DELTA_Q = 1 };
+/* keyframe indices of a pose factor are < GLIO_POSE_MAX_KF (the host plan holds one incidence start per keyframe up to the largest) */
+enum { GLIO_POSE_MAX_KF = 1 << 22 };
+typedef struct { int32_t i, j, kind, active; double dq[4]; /* w,x,y,z */ double dp[3]; } glio_pose_factor;
+/* Replaces the pose-factor list (n = 0 empties it; glio_batch_clear empties it too).  The whole list is checked first (i != j, both
+ * in [0, GLIO_POSE_MAX_KF), a known kind; f may be NULL only when n = 0); a refused call (GLIO_ERR_ARG) leaves the previous list in place.  The
+ * distinct unordered pairs (a, b), a = min(i, j) < b, form the pose-pair table in order of first appearance.  Device buffers are
+ * allocated and filled here, and the context takes the new list only once they are complete: a call that fails for any reason
+ * leaves the previous list in place.  Evaluations allocate nothing for the list. */
+int glio_batch_set_pose_factors(glio_ctx* ctx, const glio_pose_factor* f, int64_t n);
+/* the pose-pair table (a[k] < b[k]), glio_batch_pair_list's conventions: NULL arrays only count */
+int glio_batch_pose_pair_list(glio_ctx* ctx, int64_t capacity, int32_t* a, int32_t* b, int64_t* n_pairs);
+/* The pose blocks alone, for the active factors: Hdiag[K*36] (per keyframe 6 x 6 over (t, delta)), Hoff[n_pose_pairs*36]
+ * (block k = d2 cost / d x_a d x_b of pose pair k, rows for a), g[K*6], cost (attributed to a); NULL outputs are skipped and
+ * without Hdiag, Hoff and g only the cost is formed.  Per pair the factors are summed in list order, per keyframe the pairs in
+ * table order.  With the all-reduce hook set, the K x 28 and n_pose_pairs x 36 buffers are summed over the ranks, as in
+ * glio_eval_binary.  A list that references a keyframe >= K is GLIO_ERR_ARG. */
+int glio_eval_pose_factors(glio_ctx* ctx, int K, const double* poses, double* Hdiag, double* Hoff, double* g, double* cost);
+/* on != 0: every evaluation inside glio_batch_solve adds the pose blocks of the active factors to the LiDAR pair blocks, before the
+ * all-reduce: a sharded run then sums K x 28 and (P + P_pose) x 36 doubles, one call per buffer.  The band's half bandwidth covers
+ * the pose pairs' span, and the solve works with no LiDAR pair at all (the reference's sms_fusion_level 0 problem).  Default off;
+ * with the switch off or an empty list glio_batch_solve launches what it launches without pose factors.  A list that references
+ * a keyframe >= K makes glio_batch_solve return GLIO_ERR_ARG.  glio_eval_binary and glio_eval_binary_edge never add pose blocks. */
+int glio_batch_use_pose_factors(glio_ctx* ctx, int on);
 
 /* ---- seeded device selection of EDGE correspondences.  The reference selects plane matches only; this library applies the same
  * rules and the same sampler (glio_select_random / glio_batch_select_random, k_sel_sample) to edge lists, with the sizes of a
