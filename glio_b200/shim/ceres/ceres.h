@@ -13,7 +13,8 @@
 // (glio::DeviceFactorTraits<Functor>, see INTEGRATION.md) are not evaluated one virtual call at a time on the host:
 // they are uploaded once to a glio_ctx and evaluated by the CUDA kernels, which return 6x6 pose blocks: K2 for the plane
 // factors (LidarPlaneNormFactor, and LidarPlaneNormIncreFactor in a front-end context), K2e for LidarEdgeFactor, K2b for
-// BinaryLidarPlaneNormFactor.
+// BinaryLidarPlaneNormFactor, K2p for the batch refinement's pose factors (LidarPoseFactorBatchRelativeAutoDiff,
+// delta_q_factor_auto).
 // Every other cost function (IMU, marginalisation prior, GNSS ...) is evaluated on the host through its own
 // Evaluate(), exactly as Ceres would.  Without a glio_ctx attached everything runs on the host (used by CPU tests).
 #ifndef GLIO_SHIM_CERES_CERES_H_
@@ -38,7 +39,8 @@
 
 namespace glio {
 // ---- self-description of device-evaluable LiDAR factors --------------------------------------------------------
-enum FactorKind { FACTOR_NONE = 0, FACTOR_PLANE_UNARY = 1, FACTOR_PLANE_BINARY = 2, FACTOR_EDGE_UNARY = 3, FACTOR_PLANE_INCRE = 4 };
+enum FactorKind { FACTOR_NONE = 0, FACTOR_PLANE_UNARY = 1, FACTOR_PLANE_BINARY = 2, FACTOR_EDGE_UNARY = 3, FACTOR_PLANE_INCRE = 4,
+                  FACTOR_POSE_RELATIVE = 5, FACTOR_POSE_DELTA_Q = 6 };
 struct FactorDesc {
   int kind = FACTOR_NONE;
   double cp[3] = {0, 0, 0};           // current point (scan / body frame)
@@ -47,6 +49,7 @@ struct FactorDesc {
   double nc[6] = {0, 0, 0, 0, 0, 0};  // binary: local normal + centroid (BinaryLidarPlaneNormFactor)
   double score = 0;                   // unary / binary: score; edge: the weight s
   double pa[3] = {0, 0, 0}, pb[3] = {0, 0, 0};   // edge: two points of the map line (LidarEdgeFactor last_point_a / _b)
+  double dq[4] = {1, 0, 0, 0}, dp[3] = {0, 0, 0};  // pose factors: the measured delta_q (w, x, y, z) and, relative kind, delta_p
 };
 // Specialise for the reference's functors (INTEGRATION.md shows the lines for each LiDAR functor):
 //   template <> struct glio::DeviceFactorTraits<LidarPlaneNormFactor> { static bool describe(const LidarPlaneNormFactor&, FactorDesc*); };
@@ -263,6 +266,7 @@ class Solver {
     int num_parameter_blocks = -1, num_parameters = -1, num_effective_parameters = -1, num_residual_blocks = -1, num_residuals = -1;
     int num_device_residual_blocks = 0;     // glio extension: residual blocks evaluated by the CUDA kernels
     int num_device_edge_residual_blocks = 0;   // glio extension: the LidarEdgeFactor blocks among them (K2e)
+    int num_device_pose_residual_blocks = 0;   // glio extension: the relative-pose and delta_q blocks among them (K2p)
     bool IsSolutionUsable() const { return termination_type == CONVERGENCE || termination_type == NO_CONVERGENCE || termination_type == USER_SUCCESS; }
     std::string BriefReport() const {
       char b[256];

@@ -96,6 +96,7 @@ inline void Solve(const Solver::Options& options, Problem* problem, Solver::Summ
     for (int k = 0; k < 3; ++k) ok = ok && t_lb[k] == gp.t_lb[k];
     return ok;
   };
+  auto trans_ok = [&](double* t) { return P.index.count(t) && problem->blocks_.at(t).size == 3 && problem->blocks_.at(t).param == nullptr; };
   auto f32_3 = [](const double* v) { return is_f32(v[0]) && is_f32(v[1]) && is_f32(v[2]); };
   auto add_plane = [](Slot& sl, const glio::FactorDesc& d, double w) {
     for (int k = 0; k < 3; ++k) sl.cp.push_back((float)d.cp[k]);
@@ -103,6 +104,9 @@ inline void Solve(const Solver::Options& options, Problem* problem, Solver::Summ
     sl.nsd.push_back((float)d.d); sl.w.push_back((float)w);
   };
   int n_edge_dev = 0;
+  // pose-factor candidates: routed after the loop, once every keyframe (t, q) pairing of the problem is known
+  struct PoseCand { const Problem::Residual* rb; glio::FactorDesc d; };
+  std::vector<PoseCand> pose_cands;
   for (auto& rbp : problem->residual_blocks_) {
     const Problem::Residual* rb = rbp.get();
     glio::FactorDesc d;
@@ -177,10 +181,60 @@ inline void Solve(const Solver::Options& options, Problem* problem, Solver::Summ
         dev = true;
       }
     }
+    // LidarPoseFactorBatchRelativeAutoDiff (LidarPoseFactor.h:54-95, blocks t_i, q_i, t_j, q_j) and delta_q_factor_auto
+    // (LidarKeyframeFactor.h:281-304, blocks q_i, q_j), both added without a loss (Estimator.cpp:2863, :2924): K2p evaluates them
+    // when every block is active, each q a QuaternionParameterization and each t a plain 3-vector.  A candidate stays in
+    // host_blocks until the keyframe table below takes it.
+    if (!dev && rb->loss == nullptr &&
+        ((d.kind == glio::FACTOR_POSE_RELATIVE && rb->params.size() == 4 && trans_ok(rb->params[0]) && quat_ok(rb->params[1]) &&
+          trans_ok(rb->params[2]) && quat_ok(rb->params[3])) ||
+         (d.kind == glio::FACTOR_POSE_DELTA_Q && rb->params.size() == 2 && quat_ok(rb->params[0]) && quat_ok(rb->params[1]))))
+      pose_cands.push_back(PoseCand{rb, d});
     if (!dev) host_blocks.push_back(rb);
   }
   const int W = (int)slots.size();
   const int KB = (int)bkfs.size(), PB = (int)bpairs.size();
+
+  // ---- pose factors on the batch keyframe table ----
+  // Binary-plane and pose blocks that share a (t, q) pair share one keyframe; a q seen only in delta_q blocks is a keyframe of
+  // its own without a t (t = NULL: rotation columns only).  A q paired with two t blocks, or a t with two q blocks, has no single
+  // keyframe: the pose blocks that touch it stay on the host.  So do blocks whose two sides are one keyframe.
+  std::vector<glio_pose_factor> pose_list;
+  {
+    std::map<double*, std::set<double*>> ts_of_q, qs_of_t;
+    auto pairing = [&](double* t, double* q) { ts_of_q[q].insert(t); qs_of_t[t].insert(q); };
+    for (const auto& kf : bkfs) pairing(kf.first, kf.second);
+    for (const PoseCand& c : pose_cands)
+      if (c.d.kind == glio::FACTOR_POSE_RELATIVE) { pairing(c.rb->params[0], c.rb->params[1]); pairing(c.rb->params[2], c.rb->params[3]); }
+    auto q_single = [&](double* q) {
+      auto it = ts_of_q.find(q);
+      if (it == ts_of_q.end()) return true;
+      return it->second.size() == 1 && qs_of_t.at(*it->second.begin()).size() == 1;
+    };
+    auto kf_of_q = [&](double* q) {
+      auto it = ts_of_q.find(q);
+      auto key = std::make_pair(it == ts_of_q.end() ? (double*)nullptr : *it->second.begin(), q);
+      auto kit = bkf_of.find(key);
+      if (kit != bkf_of.end()) return kit->second;
+      const int k = (int)bkfs.size(); bkf_of[key] = k; bkfs.push_back(key); return k;
+    };
+    std::set<const Problem::Residual*> routed;
+    for (const PoseCand& c : pose_cands) {
+      const bool rel = c.d.kind == glio::FACTOR_POSE_RELATIVE;
+      double* qi = c.rb->params[rel ? 1 : 0]; double* qj = c.rb->params[rel ? 3 : 1];
+      if (qi == qj || !q_single(qi) || !q_single(qj)) continue;
+      glio_pose_factor f;
+      f.i = kf_of_q(qi); f.j = kf_of_q(qj); f.kind = rel ? GLIO_POSE_RELATIVE : GLIO_POSE_DELTA_Q; f.active = 1;
+      for (int k = 0; k < 4; ++k) f.dq[k] = c.d.dq[k];
+      for (int k = 0; k < 3; ++k) f.dp[k] = rel ? c.d.dp[k] : 0.0;
+      pose_list.push_back(f);
+      routed.insert(c.rb);
+    }
+    if (!routed.empty())
+      host_blocks.erase(std::remove_if(host_blocks.begin(), host_blocks.end(), [&](const Problem::Residual* rb) { return routed.count(rb) != 0; }),
+                        host_blocks.end());
+  }
+  const int KT = (int)bkfs.size(), NP = (int)pose_list.size();   // keyframes of K2b (the first KB) and K2p; routed pose blocks
   if (PB > 0) {
     if (glio_batch_clear(ctx) != GLIO_OK) { S.termination_type = FAILURE; S.message = std::string("glio_batch_clear: ") + glio_last_error(ctx); return; }
     for (int p = 0; p < PB; ++p) {
@@ -208,6 +262,22 @@ inline void Solve(const Solver::Options& options, Problem* problem, Solver::Summ
     }
     S.num_device_residual_blocks += n_edge_dev; S.num_device_edge_residual_blocks = n_edge_dev;
   }
+  // pose factors: the context's list is replaced after glio_batch_clear (which empties it) and the pair uploads.  A problem
+  // without routed pose blocks makes no pose call at all.  glio_eval_binary never adds pose blocks, so glio_batch_use_pose_factors
+  // does not change what is computed here.
+  std::vector<int32_t> pp_a, pp_b;                               // the pose-pair table (glio_batch_pose_pair_list)
+  if (NP > 0) {
+    int64_t npp = 0;
+    if (glio_batch_set_pose_factors(ctx, pose_list.data(), NP) != GLIO_OK || glio_batch_pose_pair_list(ctx, 0, nullptr, nullptr, &npp) != GLIO_OK) {
+      S.termination_type = FAILURE; S.message = std::string("glio_batch_set_pose_factors: ") + glio_last_error(ctx); return;
+    }
+    pp_a.resize(npp); pp_b.resize(npp);
+    if (glio_batch_pose_pair_list(ctx, npp, pp_a.data(), pp_b.data(), &npp) != GLIO_OK) {
+      S.termination_type = FAILURE; S.message = std::string("glio_batch_pose_pair_list: ") + glio_last_error(ctx); return;
+    }
+    S.num_device_residual_blocks += NP; S.num_device_pose_residual_blocks = NP;
+  }
+  const int PP = (int)pp_a.size();
 
   // ---- band of J^T J from the block structure ----
   int hb = 0;
@@ -244,7 +314,8 @@ inline void Solve(const Solver::Options& options, Problem* problem, Solver::Summ
   for (const ActiveBlock& a : P.active) std::memcpy(&x[a.amb_off], a.user, sizeof(double) * a.size);
   std::vector<double> poses((size_t)std::max(W, 1) * 7), Hd((size_t)std::max(W, 1) * 36), gd((size_t)std::max(W, 1) * 6), cd(std::max(W, 1));
   std::vector<double> He(with_edges ? Hd.size() : 0), ge(with_edges ? gd.size() : 0), ce(with_edges ? cd.size() : 0);
-  std::vector<double> bposes((size_t)std::max(KB, 1) * 7), bHd((size_t)std::max(KB, 1) * 36), bHo((size_t)std::max(PB, 1) * 36), bg((size_t)std::max(KB, 1) * 6);
+  std::vector<double> bposes((size_t)std::max(KT, 1) * 7), bHd((size_t)std::max(KB, 1) * 36), bHo((size_t)std::max(PB, 1) * 36), bg((size_t)std::max(KB, 1) * 6);
+  std::vector<double> pHd(NP > 0 ? (size_t)KT * 36 : 0), pHo(NP > 0 ? (size_t)std::max(PP, 1) * 36 : 0), pg(NP > 0 ? (size_t)KT * 6 : 0);
   double fixed_cost = 0; bool fixed_done = false;
 
   glio::EvalFn eval = [&](const double* xa, bool want_jac, double* cost, glio::BandMat* H, double* g) -> bool {
@@ -277,17 +348,22 @@ inline void Solve(const Solver::Options& options, Problem* problem, Solver::Summ
         }
       }
     }
-    if (PB > 0) {
-      for (int k = 0; k < KB; ++k) {
-        const ActiveBlock& at = P.active[P.index[bkfs[k].first]]; const ActiveBlock& aq = P.active[P.index[bkfs[k].second]];
-        for (int i = 0; i < 3; ++i) bposes[7 * k + i] = xa[at.amb_off + i];
+    // batch keyframe k: tangent column of its 6-vector entry p (t then delta); -1 for the t entries of a keyframe without a t
+    auto toff = [&](int kf, int p) {
+      double* u = p < 3 ? bkfs[kf].first : bkfs[kf].second;
+      return u ? P.active[P.index[u]].tan_off + p % 3 : -1;
+    };
+    if (PB > 0 || NP > 0)
+      for (int k = 0; k < KT; ++k) {
+        for (int i = 0; i < 3; ++i) bposes[7 * k + i] = bkfs[k].first ? xa[P.active[P.index[bkfs[k].first]].amb_off + i] : 0.0;
+        const ActiveBlock& aq = P.active[P.index[bkfs[k].second]];
         for (int i = 0; i < 4; ++i) bposes[7 * k + 3 + i] = xa[aq.amb_off + i];
       }
+    if (PB > 0) {
       double bc = 0;
       if (glio_eval_binary(ctx, KB, bposes.data(), want_jac ? bHd.data() : nullptr, want_jac ? bHo.data() : nullptr, want_jac ? bg.data() : nullptr, &bc) != GLIO_OK) return false;
       ct += bc;
       if (want_jac) {
-        auto toff = [&](int kf, int p) { return (p < 3 ? P.active[P.index[bkfs[kf].first]].tan_off : P.active[P.index[bkfs[kf].second]].tan_off) + p % 3; };
         for (int k = 0; k < KB; ++k)
           for (int p = 0; p < 6; ++p) {
             const int ip = toff(k, p);
@@ -298,6 +374,27 @@ inline void Solve(const Solver::Options& options, Problem* problem, Solver::Summ
           for (int p = 0; p < 6; ++p) for (int q = 0; q < 6; ++q) {
             const int ip = toff(bpairs[pr].kc, p), iq = toff(bpairs[pr].ko, q);
             const double v = bHo[36 * pr + 6 * p + q];
+            if (ip >= iq) H->at(ip, iq) += v; else H->at(iq, ip) += v;
+          }
+      }
+    }
+    if (NP > 0) {                            // K2p: Hdiag, g and cost into the band, Hoff over the pose-pair table as the bpairs
+      double pc = 0;
+      if (glio_eval_pose_factors(ctx, KT, bposes.data(), want_jac ? pHd.data() : nullptr, want_jac ? pHo.data() : nullptr, want_jac ? pg.data() : nullptr, &pc) != GLIO_OK) return false;
+      ct += pc;
+      if (want_jac) {
+        for (int k = 0; k < KT; ++k)
+          for (int p = 0; p < 6; ++p) {
+            const int ip = toff(k, p);
+            if (ip < 0) continue;
+            g[ip] += pg[6 * k + p];
+            for (int q = 0; q < 6; ++q) { const int iq = toff(k, q); if (iq >= 0 && ip >= iq) H->at(ip, iq) += pHd[36 * k + 6 * p + q]; }
+          }
+        for (int pr = 0; pr < PP; ++pr)                       // block (a, b): row = a tangent, col = b tangent
+          for (int p = 0; p < 6; ++p) for (int q = 0; q < 6; ++q) {
+            const int ip = toff(pp_a[pr], p), iq = toff(pp_b[pr], q);
+            if (ip < 0 || iq < 0) continue;
+            const double v = pHo[36 * pr + 6 * p + q];
             if (ip >= iq) H->at(ip, iq) += v; else H->at(iq, ip) += v;
           }
       }

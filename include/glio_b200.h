@@ -825,8 +825,9 @@ int glio_batch_get_edge_selection(glio_ctx* ctx, int cur, int oth, int64_t capac
 
 /* ---- batch minimizer (replaces ceres::Solve of optimizeBatchWithLandMark, Estimator.cpp:3275-3284: SUBSPACE_DOGLEG,
  * nonmonotonic steps, max_num_iter iterations; options == NULL selects exactly those).  The normal equations are
- * block-banded (half bandwidth (max|cur-oth|+1)*nt - 1) and stored/factored in band form.  Host factors (IMU chain,
- * delta_q, DD pseudorange: host C++ by design) accumulate into the same LOWER-BAND storage:
+ * block-banded (half bandwidth (max|cur-oth|+1)*nt - 1) and stored/factored in band form.  Host factors (IMU chain, DD
+ * pseudorange: host C++ by design; the pose factors run on the device through glio_batch_use_pose_factors) accumulate into the
+ * same LOWER-BAND storage:
  * entry (i,j), i-hb <= j <= i, lives at Hband[i*(hb+1) + (j-i+hb)]. */
 int glio_hf_evaluate_band(void* user, int K, const double* poses, const double* speed_bias, int want_jac, double* Hband, int hb,
                           double* g, double* cost);
