@@ -147,7 +147,8 @@ class Context:
                "k_lc_load", "k_lc_qhist", "k_lc_qscatter", "k_lc_init", "k_lc_nn", "k_lc_compact", "k_lc_sum0",
                "k_lc_sum1", "k_lc_means", "k_lc_solve", "k_lc_transform", "k_lc_final", "k_lc_fitness",
                "k_vs_key", "k_vs_hist", "k_vs_scatter", "k_vs_heads", "k_vs_centroid", "k_vs_pack", "k_gm_transform",
-               "k_pose_pair_sums", "k_pose_pair_sums_cost", "k_pose_assemble"]
+               "k_pose_pair_sums", "k_pose_pair_sums_cost", "k_pose_assemble",
+               "k_psr_pair_sums", "k_psr_pair_sums_cost", "k_psr_assemble"]
 
     def lib_profile(self, on):
         self._chk(self._lib.glio_profile_enable(self._h, C.c_int(1 if on else 0)))
@@ -990,6 +991,88 @@ Context.batch_set_pose_factors = _batch_set_pose_factors
 Context.batch_pose_pair_list = _batch_pose_pair_list
 Context.eval_pose_factors = _eval_pose_factors
 Context.batch_use_pose_factors = _batch_use_pose_factors
+
+
+# ---------------------------------------------------------------------------------------------------
+# the batch refinement's double-differenced pseudorange factors (K2g): dd_psr_factor_20
+# ---------------------------------------------------------------------------------------------------
+DD_PSR_MAX_SAT = 20                       # GLIO_DD_PSR_MAX_SAT: the reference's 19-row buffer
+DD_PSR_MAX_KF = 1 << 22                   # GLIO_DD_PSR_MAX_KF
+# glio_dd_psr_factor: i, j, n_sat, master, active, reserved (int32), sat_offset, w_offset (int64; -1 = identity), ratio,
+# threshold, station (float64)
+DD_PSR_FACTOR_DTYPE = np.dtype([("i", "<i4"), ("j", "<i4"), ("n_sat", "<i4"), ("master", "<i4"), ("active", "<i4"), ("reserved", "<i4"),
+                                ("sat_offset", "<i8"), ("w_offset", "<i8"), ("ratio", "<f8"), ("threshold", "<f8"), ("station", "<f8", (3,))])
+assert DD_PSR_FACTOR_DTYPE.itemsize == 80
+# glio_dd_psr_sat: sat_user, sat_ref (ECEF, m), psr_user, psr_ref (m)
+DD_PSR_SAT_DTYPE = np.dtype([("sat_user", "<f8", (3,)), ("sat_ref", "<f8", (3,)), ("psr_user", "<f8"), ("psr_ref", "<f8")])
+assert DD_PSR_SAT_DTYPE.itemsize == 64
+
+
+def dd_psr_factor_records(i, j, n_sat, master, ratio, threshold, station, sat_offset=None, w_offset=None, active=None):
+    """A glio_dd_psr_factor array from per-factor columns.  sat_offset defaults to the running sum of n_sat (each factor's
+    satellites follow the previous factor's), w_offset to -1 (identity), active to 1; threshold and station may be scalars /
+    one 3-vector for all factors."""
+    n = len(i)
+    f = np.zeros(n, DD_PSR_FACTOR_DTYPE)
+    f["i"], f["j"], f["n_sat"], f["master"] = i, j, n_sat, master
+    f["ratio"], f["threshold"] = ratio, threshold
+    f["station"] = np.broadcast_to(np.asarray(station, np.float64), (n, 3))
+    if sat_offset is None:
+        sat_offset = np.cumsum(f["n_sat"].astype(np.int64)) - f["n_sat"]
+    f["sat_offset"] = sat_offset
+    f["w_offset"] = -1 if w_offset is None else w_offset
+    f["active"] = 1 if active is None else np.asarray(active, np.int32)
+    return f
+
+
+def dd_psr_sat_records(sat_user, sat_ref, psr_user, psr_ref):
+    """A glio_dd_psr_sat array from columns (n, 3), (n, 3), (n,), (n,)."""
+    s = np.zeros(len(psr_user), DD_PSR_SAT_DTYPE)
+    s["sat_user"], s["sat_ref"], s["psr_user"], s["psr_ref"] = sat_user, sat_ref, psr_user, psr_ref
+    return s
+
+
+def _batch_set_dd_psr_factors(self, factors, sats, R_ecef_local, anchor_ecef, W=None):
+    """glio_batch_set_dd_psr_factors: replace the DD-pseudorange list (an empty factor array empties it)."""
+    f = np.ascontiguousarray(factors, DD_PSR_FACTOR_DTYPE)
+    s = np.ascontiguousarray(sats, DD_PSR_SAT_DTYPE)
+    w = np.zeros(0) if W is None else np.ascontiguousarray(W, np.float64).ravel()
+    R = np.ascontiguousarray(R_ecef_local, np.float64).reshape(9)
+    a = np.ascontiguousarray(anchor_ecef, np.float64).reshape(3)
+    self._chk(self._lib.glio_batch_set_dd_psr_factors(self._h, _ptr(f) if len(f) else None, C.c_int64(len(f)), _ptr(s) if len(s) else None,
+                                                      C.c_int64(len(s)), _ptr(w) if len(w) else None, C.c_int64(len(w)), _ptr(R), _ptr(a)))
+
+
+def _batch_dd_psr_pair_list(self):
+    """The DD pair table (a, b), a < b, in order of first appearance."""
+    n = C.c_int64(0)
+    self._chk(self._lib.glio_batch_dd_psr_pair_list(self._h, C.c_int64(0), None, None, C.byref(n)))
+    a = np.zeros(n.value, np.int32); b = np.zeros(n.value, np.int32)
+    self._chk(self._lib.glio_batch_dd_psr_pair_list(self._h, C.c_int64(len(a)), _ptr(a), _ptr(b), C.byref(n)))
+    return a, b
+
+
+def _eval_dd_psr_factors(self, poses, want_jac=True):
+    """glio_eval_dd_psr_factors: the DD blocks alone; Hoff in DD-pair order (d2 cost / d x_a d x_b, rows for a)."""
+    pb = np.ascontiguousarray(poses, np.float64).reshape(-1, 7); K = len(pb)
+    n = C.c_int64(0)
+    self._chk(self._lib.glio_batch_dd_psr_pair_list(self._h, C.c_int64(0), None, None, C.byref(n)))
+    P = int(n.value)
+    Hd = np.zeros((K, 6, 6)) if want_jac else None; Ho = np.zeros((P, 6, 6)) if want_jac else None
+    g = np.zeros((K, 6)) if want_jac else None; cost = np.zeros(1)
+    self._chk(self._lib.glio_eval_dd_psr_factors(self._h, C.c_int(K), _ptr(pb), _ptr(Hd), _ptr(Ho), _ptr(g), _ptr(cost)))
+    return dict(Hdiag=Hd, Hoff=Ho, g=g, cost=float(cost[0]))
+
+
+def _batch_use_dd_psr_factors(self, on):
+    """glio_batch_use_dd_psr_factors: batch solves add the DD blocks (default off)."""
+    self._chk(self._lib.glio_batch_use_dd_psr_factors(self._h, C.c_int(1 if on else 0)))
+
+
+Context.batch_set_dd_psr_factors = _batch_set_dd_psr_factors
+Context.batch_dd_psr_pair_list = _batch_dd_psr_pair_list
+Context.eval_dd_psr_factors = _eval_dd_psr_factors
+Context.batch_use_dd_psr_factors = _batch_use_dd_psr_factors
 
 
 # ---------------------------------------------------------------------------------------------------

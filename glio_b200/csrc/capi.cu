@@ -171,6 +171,12 @@ struct glio_ctx {
   bool batch_use_pose = false;
   std::vector<std::pair<int, int>> pose_pairs; int pose_max_kf = -1;
   DevBuf<PoseFactor> d_pose_f; DevBuf<int> d_pose_fstart, d_pose_inc_start; DevBuf<BinIncidence> d_pose_inc; DevBuf<double> d_pose_sums;
+  // DD pseudorange factors (glio_batch_set_dd_psr_factors, K2g): the same plan as the pose factors, plus the list's satellites,
+  // weights and frame constants
+  bool batch_use_dd = false;
+  std::vector<std::pair<int, int>> dd_pairs; int dd_max_kf = -1; DdPsrFrame dd_frame{};
+  DevBuf<DdPsrFactor> d_dd_f; DevBuf<int> d_dd_fstart, d_dd_inc_start; DevBuf<BinIncidence> d_dd_inc; DevBuf<DdPsrSat> d_dd_sats;
+  DevBuf<double> d_dd_w, d_dd_sums;
 
   // association workspace
   DevBuf<float4> w_pm, w_pmq, w_nsd;
@@ -1709,6 +1715,7 @@ int glio_batch_clear(glio_ctx* c) {
     GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
     c->frames.clear(); c->pairs.clear(); c->pair_index.clear(); c->bin_dirty = true; c->bedge_dirty = true;
     c->pose_pairs.clear(); c->pose_max_kf = -1;
+    c->dd_pairs.clear(); c->dd_max_kf = -1;
   });
 }
 
@@ -2273,14 +2280,16 @@ enum BinBlocks { BIN_PLANES = 0, BIN_PLANES_EDGES = 1, BIN_EDGES = 2 };
 // device evaluation of all active binary residuals -> c->h_bin_diag (K x 28), c->h_bin_off (P x 36): everything is queued
 // (kernels, the all-reduce of a sharded run, the copies to pinned host memory); eval_binary_wait makes the result visible.
 // With edges, each pair's sums are S_plane + S_edge before the one block assembly, so the all-reduce is the same as without.
-// add_pose: the pose blocks of K2p are added to the diagonal buffer and stored after the P pair blocks of the off-diagonal one
-void eval_binary_launch(glio_ctx* c, int K, const double* poses, bool want_jac, double huber, BinBlocks what = BIN_PLANES, bool add_pose = false) {
+// add_pose: the pose blocks of K2p are added to the diagonal buffer and stored after the P pair blocks of the off-diagonal one;
+// add_dd: the DD blocks of K2g likewise, after the pose pair blocks
+void eval_binary_launch(glio_ctx* c, int K, const double* poses, bool want_jac, double huber, BinBlocks what = BIN_PLANES, bool add_pose = false,
+                        bool add_dd = false) {
   build_bin_items(c, K);
   if (what != BIN_PLANES) build_bedge_items(c, K);
   const bool add_edges = what == BIN_PLANES_EDGES && c->n_bedge_items > 0;   // no edges: exactly the plane launches
   const int P = (int)c->pairs.size();
-  const int Pp = add_pose ? (int)c->pose_pairs.size() : 0, Pt = P + Pp;
-  if (Pp > 0) { c->d_bin_off.reserve((size_t)(Pt + 1) * 36); c->h_bin_off.reserve((size_t)(Pt + 1) * 36); }
+  const int Pp = add_pose ? (int)c->pose_pairs.size() : 0, Pd = add_dd ? (int)c->dd_pairs.size() : 0, Pt = P + Pp + Pd;
+  if (Pp + Pd > 0) { c->d_bin_off.reserve((size_t)(Pt + 1) * 36); c->h_bin_off.reserve((size_t)(Pt + 1) * 36); }
   memcpy(c->h_bin_poses.p, poses, (size_t)K * 7 * sizeof(double));
   GLIO_CUDA_TRY(cudaMemcpyAsync(c->d_bin_poses.p, c->h_bin_poses.p, (size_t)K * 7 * sizeof(double), cudaMemcpyHostToDevice, c->st));
   if (what == BIN_EDGES || add_edges)
@@ -2295,6 +2304,10 @@ void eval_binary_launch(glio_ctx* c, int K, const double* poses, bool want_jac, 
   if (add_pose)
     eval_pose_run(c->d_pose_f.p, c->d_pose_fstart.p, Pp, K, c->pose_max_kf + 1, c->d_pose_inc_start.p, c->d_pose_inc.p, c->d_bin_poses.p,
                   want_jac, /*add*/ true, c->d_pose_sums.p, c->d_bin_diag.p, c->d_bin_off.p + (size_t)P * 36, c->st, c->lc);
+  if (add_dd)
+    eval_dd_psr_run(c->d_dd_f.p, c->d_dd_fstart.p, c->d_dd_sats.p, c->d_dd_w.p, c->dd_frame, Pd, K, c->dd_max_kf + 1, c->d_dd_inc_start.p,
+                    c->d_dd_inc.p, c->d_bin_poses.p, want_jac, /*add*/ true, c->d_dd_sums.p, c->d_bin_diag.p,
+                    c->d_bin_off.p + (size_t)(P + Pp) * 36, c->st, c->lc);
   if (c->allreduce) {
     // keyframe-sharded evaluation: every rank holds the same pair list but only its own pairs carry residuals;
     // one sum over ranks of the pose-block buffers per evaluation (SURVEY 8e "pose-block allreduce")
@@ -2324,6 +2337,70 @@ int eval_binary_out(glio_ctx* c, int K, const double* poses, BinBlocks what, dou
     if (Hoff) memcpy(Hoff, c->h_bin_off.p, c->pairs.size() * 36 * sizeof(double));
     if (cost) *cost = ct;
   });
+}
+
+// The pair plan of a factor list with keyframes i, j and an active flag (pose and DD factors): the distinct unordered pairs
+// (a, b), a < b, in order of first appearance; the active factors' list positions grouped by pair, list order inside a pair
+// (order[fstart[p] .. fstart[p+1])); per keyframe 0 .. max_kf its pairs in table order (role 0 = a, 1 = b), by a counting sort.
+struct PairPlan {
+  std::vector<std::pair<int, int>> pairs;
+  std::vector<int> fstart, order, kstart;
+  std::vector<BinIncidence> inc;
+  int max_kf = -1;
+};
+template <class F>
+PairPlan plan_factor_pairs(const F* f, int64_t n) {
+  PairPlan pl;
+  std::map<std::pair<int, int>, int> index;
+  std::vector<int> fpair((size_t)n), count;
+  for (int64_t k = 0; k < n; ++k) {
+    const std::pair<int, int> key(std::min(f[k].i, f[k].j), std::max(f[k].i, f[k].j));
+    auto it = index.emplace(key, (int)pl.pairs.size()).first;
+    if (it->second == (int)pl.pairs.size()) { pl.pairs.push_back(key); count.push_back(0); }
+    fpair[k] = it->second;
+    if (f[k].active) ++count[it->second];
+    pl.max_kf = std::max(pl.max_kf, key.second);
+  }
+  const int Pn = (int)pl.pairs.size();
+  pl.fstart.assign(Pn + 1, 0);
+  for (int p = 0; p < Pn; ++p) pl.fstart[p + 1] = pl.fstart[p] + count[p];
+  pl.order.resize((size_t)pl.fstart[Pn]);
+  std::vector<int> pos(pl.fstart.begin(), pl.fstart.end() - 1);
+  for (int64_t k = 0; k < n; ++k)
+    if (f[k].active) pl.order[pos[fpair[k]]++] = (int)k;
+  pl.kstart.assign((size_t)pl.max_kf + 2, 0);
+  for (const auto& pr : pl.pairs) { ++pl.kstart[(size_t)pr.first + 1]; ++pl.kstart[(size_t)pr.second + 1]; }
+  for (size_t k = 1; k < pl.kstart.size(); ++k) pl.kstart[k] += pl.kstart[k - 1];
+  pl.inc.resize((size_t)2 * Pn);
+  std::vector<int> fill(pl.kstart.begin(), pl.kstart.end() - 1);
+  for (int p = 0; p < Pn; ++p) { pl.inc[fill[pl.pairs[p].first]++] = BinIncidence{p, 0}; pl.inc[fill[pl.pairs[p].second]++] = BinIncidence{p, 1}; }
+  return pl;
+}
+
+// the blocks of one device factor list alone (glio_eval_pose_factors, glio_eval_dd_psr_factors): run queues the kernels into the
+// K x 28 / n_pairs x 36 buffers, then the all-reduce of a sharded run, the copy-out and the unpacking
+template <class Run>
+void eval_factor_blocks(glio_ctx* c, int K, const double* poses, int n_pairs, Run run, double* Hdiag, double* Hoff, double* g, double* cost) {
+  const bool want_jac = Hdiag || Hoff || g;
+  c->d_bin_diag.reserve((size_t)K * GLIO_NACC); c->h_bin_diag.reserve((size_t)K * GLIO_NACC);
+  c->d_bin_off.reserve((size_t)(n_pairs + 1) * 36); c->h_bin_off.reserve((size_t)(n_pairs + 1) * 36);
+  c->d_bin_poses.reserve((size_t)K * 7); c->h_bin_poses.reserve((size_t)K * 7);
+  memcpy(c->h_bin_poses.p, poses, (size_t)K * 7 * sizeof(double));
+  GLIO_CUDA_TRY(cudaMemcpyAsync(c->d_bin_poses.p, c->h_bin_poses.p, (size_t)K * 7 * sizeof(double), cudaMemcpyHostToDevice, c->st));
+  run(want_jac);
+  if (c->allreduce) {
+    GLIO_REQUIRE(c->allreduce(c->allreduce_user, c->d_bin_diag.p, (int64_t)K * GLIO_NACC, (void*)c->st) == 0, GLIO_ERR_NCCL, "allreduce hook failed (diag)");
+    if (want_jac && n_pairs > 0)
+      GLIO_REQUIRE(c->allreduce(c->allreduce_user, c->d_bin_off.p, (int64_t)n_pairs * 36, (void*)c->st) == 0, GLIO_ERR_NCCL, "allreduce hook failed (off)");
+  }
+  GLIO_CUDA_TRY(cudaMemcpyAsync(c->h_bin_diag.p, c->d_bin_diag.p, (size_t)K * GLIO_NACC * sizeof(double), cudaMemcpyDeviceToHost, c->st));
+  if (want_jac && n_pairs > 0) GLIO_CUDA_TRY(cudaMemcpyAsync(c->h_bin_off.p, c->d_bin_off.p, (size_t)n_pairs * 36 * sizeof(double), cudaMemcpyDeviceToHost, c->st));
+  GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
+  unpack_blocks(c->h_bin_diag.p, K, Hdiag, g, nullptr);
+  double ct = 0;
+  for (int k = 0; k < K; ++k) ct += c->h_bin_diag.p[(size_t)k * GLIO_NACC + 27];
+  if (Hoff) memcpy(Hoff, c->h_bin_off.p, (size_t)n_pairs * 36 * sizeof(double));
+  if (cost) *cost = ct;
 }
 
 }  // namespace
@@ -2358,32 +2435,11 @@ int glio_batch_set_pose_factors(glio_ctx* c, const glio_pose_factor* f, int64_t 
                    (f[k].kind == GLIO_POSE_RELATIVE || f[k].kind == GLIO_POSE_DELTA_Q),
                    GLIO_ERR_ARG, "glio_batch_set_pose_factors: need i != j, both in [0, GLIO_POSE_MAX_KF), and a known kind");
     // pair table in order of first appearance; the active factors grouped by pair, list order inside a pair
-    std::map<std::pair<int, int>, int> index;
-    std::vector<std::pair<int, int>> pairs;
-    std::vector<int> fpair((size_t)n), count;
-    int max_kf = -1;
-    for (int64_t k = 0; k < n; ++k) {
-      const std::pair<int, int> key(std::min(f[k].i, f[k].j), std::max(f[k].i, f[k].j));
-      auto it = index.emplace(key, (int)pairs.size()).first;
-      if (it->second == (int)pairs.size()) { pairs.push_back(key); count.push_back(0); }
-      fpair[k] = it->second;
-      if (f[k].active) ++count[it->second];
-      max_kf = std::max(max_kf, key.second);
-    }
-    const int Pp = (int)pairs.size();
-    std::vector<int> fstart(Pp + 1, 0);
-    for (int p = 0; p < Pp; ++p) fstart[p + 1] = fstart[p] + count[p];
-    std::vector<PoseFactor> grouped((size_t)fstart[Pp]);
-    std::vector<int> pos(fstart.begin(), fstart.end() - 1);
-    for (int64_t k = 0; k < n; ++k)
-      if (f[k].active) memcpy(&grouped[pos[fpair[k]]++], &f[k], sizeof(PoseFactor));
-    // per keyframe 0 .. max_kf its pairs in table order (role 0 = a, 1 = b): a counting sort over the keyframes
-    std::vector<int> kstart((size_t)max_kf + 2, 0);
-    for (const auto& pr : pairs) { ++kstart[(size_t)pr.first + 1]; ++kstart[(size_t)pr.second + 1]; }
-    for (size_t k = 1; k < kstart.size(); ++k) kstart[k] += kstart[k - 1];
-    std::vector<BinIncidence> flat((size_t)2 * Pp);
-    std::vector<int> fill(kstart.begin(), kstart.end() - 1);
-    for (int p = 0; p < Pp; ++p) { flat[fill[pairs[p].first]++] = BinIncidence{p, 0}; flat[fill[pairs[p].second]++] = BinIncidence{p, 1}; }
+    PairPlan pl = plan_factor_pairs(f, n);
+    const int Pp = (int)pl.pairs.size();
+    const std::vector<int>& fstart = pl.fstart; const std::vector<int>& kstart = pl.kstart; const std::vector<BinIncidence>& flat = pl.inc;
+    std::vector<PoseFactor> grouped(pl.order.size());
+    for (size_t q = 0; q < grouped.size(); ++q) memcpy(&grouped[q], &f[pl.order[q]], sizeof(PoseFactor));
     // the new plan goes to buffers of its own; the context takes them only when every upload has completed, so a failed call
     // leaves the previous list and its buffers as they were
     DevBuf<PoseFactor> d_f; DevBuf<int> d_fstart, d_kstart; DevBuf<BinIncidence> d_inc; DevBuf<double> d_sums;
@@ -2396,7 +2452,7 @@ int glio_batch_set_pose_factors(glio_ctx* c, const glio_pose_factor* f, int64_t 
     GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));   // also: no evaluation still reads the buffers released below
     c->d_pose_f = std::move(d_f); c->d_pose_fstart = std::move(d_fstart); c->d_pose_inc_start = std::move(d_kstart);
     c->d_pose_inc = std::move(d_inc); c->d_pose_sums = std::move(d_sums);
-    c->pose_pairs.swap(pairs); c->pose_max_kf = max_kf;
+    c->pose_pairs.swap(pl.pairs); c->pose_max_kf = pl.max_kf;
   });
 }
 
@@ -2417,33 +2473,96 @@ int glio_eval_pose_factors(glio_ctx* c, int K, const double* poses, double* Hdia
     GLIO_REQUIRE(K > 0 && poses, GLIO_ERR_ARG, "bad arguments");
     GLIO_REQUIRE(c->pose_max_kf < K, GLIO_ERR_ARG, "glio_eval_pose_factors: a pose factor references a keyframe outside [0, K)");
     const int Pp = (int)c->pose_pairs.size();
-    const bool want_jac = Hdiag || Hoff || g;
-    c->d_bin_diag.reserve((size_t)K * GLIO_NACC); c->h_bin_diag.reserve((size_t)K * GLIO_NACC);
-    c->d_bin_off.reserve((size_t)(Pp + 1) * 36); c->h_bin_off.reserve((size_t)(Pp + 1) * 36);
-    c->d_bin_poses.reserve((size_t)K * 7); c->h_bin_poses.reserve((size_t)K * 7);
-    memcpy(c->h_bin_poses.p, poses, (size_t)K * 7 * sizeof(double));
-    GLIO_CUDA_TRY(cudaMemcpyAsync(c->d_bin_poses.p, c->h_bin_poses.p, (size_t)K * 7 * sizeof(double), cudaMemcpyHostToDevice, c->st));
-    eval_pose_run(c->d_pose_f.p, c->d_pose_fstart.p, Pp, K, c->pose_max_kf + 1, c->d_pose_inc_start.p, c->d_pose_inc.p, c->d_bin_poses.p,
-                  want_jac, /*add*/ false, c->d_pose_sums.p, c->d_bin_diag.p, c->d_bin_off.p, c->st, c->lc);
-    if (c->allreduce) {
-      GLIO_REQUIRE(c->allreduce(c->allreduce_user, c->d_bin_diag.p, (int64_t)K * GLIO_NACC, (void*)c->st) == 0, GLIO_ERR_NCCL, "allreduce hook failed (diag)");
-      if (want_jac && Pp > 0)
-        GLIO_REQUIRE(c->allreduce(c->allreduce_user, c->d_bin_off.p, (int64_t)Pp * 36, (void*)c->st) == 0, GLIO_ERR_NCCL, "allreduce hook failed (off)");
-    }
-    GLIO_CUDA_TRY(cudaMemcpyAsync(c->h_bin_diag.p, c->d_bin_diag.p, (size_t)K * GLIO_NACC * sizeof(double), cudaMemcpyDeviceToHost, c->st));
-    if (want_jac && Pp > 0) GLIO_CUDA_TRY(cudaMemcpyAsync(c->h_bin_off.p, c->d_bin_off.p, (size_t)Pp * 36 * sizeof(double), cudaMemcpyDeviceToHost, c->st));
-    GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
-    unpack_blocks(c->h_bin_diag.p, K, Hdiag, g, nullptr);
-    double ct = 0;
-    for (int k = 0; k < K; ++k) ct += c->h_bin_diag.p[(size_t)k * GLIO_NACC + 27];
-    if (Hoff) memcpy(Hoff, c->h_bin_off.p, (size_t)Pp * 36 * sizeof(double));
-    if (cost) *cost = ct;
+    eval_factor_blocks(c, K, poses, Pp, [&](bool want_jac) {
+      eval_pose_run(c->d_pose_f.p, c->d_pose_fstart.p, Pp, K, c->pose_max_kf + 1, c->d_pose_inc_start.p, c->d_pose_inc.p, c->d_bin_poses.p,
+                    want_jac, /*add*/ false, c->d_pose_sums.p, c->d_bin_diag.p, c->d_bin_off.p, c->st, c->lc);
+    }, Hdiag, Hoff, g, cost);
   });
 }
 
 int glio_batch_use_pose_factors(glio_ctx* c, int on) {
   if (!c) return GLIO_ERR_ARG;
   c->batch_use_pose = on != 0;
+  return GLIO_OK;
+}
+
+static_assert(sizeof(glio_dd_psr_factor) == sizeof(DdPsrFactor) && offsetof(glio_dd_psr_factor, sat_offset) == offsetof(DdPsrFactor, sat_offset) &&
+              offsetof(glio_dd_psr_factor, ratio) == offsetof(DdPsrFactor, ratio) && offsetof(glio_dd_psr_factor, station) == offsetof(DdPsrFactor, station),
+              "DdPsrFactor must have glio_dd_psr_factor's layout");
+static_assert(sizeof(glio_dd_psr_sat) == sizeof(DdPsrSat) && offsetof(glio_dd_psr_sat, psr_user) == offsetof(DdPsrSat, psr_user),
+              "DdPsrSat must have glio_dd_psr_sat's layout");
+
+int glio_batch_set_dd_psr_factors(glio_ctx* c, const glio_dd_psr_factor* f, int64_t n, const glio_dd_psr_sat* sats, int64_t n_sats,
+                                  const double* W, int64_t n_w, const double* R_ecef_local, const double* anchor_ecef) {
+  if (!c) return GLIO_ERR_ARG;
+  return guarded(c, [&] {
+    // validate the whole list first: a refused call leaves the previous list in place
+    GLIO_REQUIRE(n >= 0 && (n == 0 || (f && R_ecef_local && anchor_ecef)), GLIO_ERR_ARG, "glio_batch_set_dd_psr_factors: null factor array or frame");
+    GLIO_REQUIRE(n < ((int64_t)1 << 31), GLIO_ERR_ARG, "glio_batch_set_dd_psr_factors: too many factors");
+    GLIO_REQUIRE(n_sats >= 0 && (n_sats == 0 || sats) && n_w >= 0 && (n_w == 0 || W), GLIO_ERR_ARG,
+                 "glio_batch_set_dd_psr_factors: null satellite or weight array");
+    for (int64_t k = 0; k < n; ++k) {
+      const glio_dd_psr_factor& F = f[k];
+      GLIO_REQUIRE(F.i >= 0 && F.j >= 0 && F.i < GLIO_DD_PSR_MAX_KF && F.j < GLIO_DD_PSR_MAX_KF && F.i != F.j, GLIO_ERR_ARG,
+                   "glio_batch_set_dd_psr_factors: need i != j, both in [0, GLIO_DD_PSR_MAX_KF)");
+      GLIO_REQUIRE(F.n_sat >= 2 && F.n_sat <= GLIO_DD_PSR_MAX_SAT && F.master >= 0 && F.master < F.n_sat, GLIO_ERR_ARG,
+                   "glio_batch_set_dd_psr_factors: need 2 <= n_sat <= GLIO_DD_PSR_MAX_SAT and 0 <= master < n_sat");
+      GLIO_REQUIRE(F.sat_offset >= 0 && F.sat_offset <= n_sats - F.n_sat, GLIO_ERR_ARG, "glio_batch_set_dd_psr_factors: satellites outside [0, n_sats)");
+      const int64_t nw = (int64_t)(F.n_sat - 1) * (F.n_sat - 1);
+      GLIO_REQUIRE(F.w_offset == -1 || (F.w_offset >= 0 && F.w_offset <= n_w - nw), GLIO_ERR_ARG,
+                   "glio_batch_set_dd_psr_factors: weight outside [0, n_w) and not -1");
+    }
+    PairPlan pl = plan_factor_pairs(f, n);
+    const int Pd = (int)pl.pairs.size();
+    std::vector<DdPsrFactor> grouped(pl.order.size());
+    for (size_t q = 0; q < grouped.size(); ++q) memcpy(&grouped[q], &f[pl.order[q]], sizeof(DdPsrFactor));
+    DdPsrFrame fr{};
+    if (n > 0) { memcpy(fr.R, R_ecef_local, sizeof(fr.R)); memcpy(fr.anchor, anchor_ecef, sizeof(fr.anchor)); }
+    // the new plan goes to buffers of its own; the context takes them only when every upload has completed
+    DevBuf<DdPsrFactor> d_f; DevBuf<int> d_fstart, d_kstart; DevBuf<BinIncidence> d_inc; DevBuf<DdPsrSat> d_sats; DevBuf<double> d_w, d_sums;
+    d_f.reserve(grouped.size() + 1); d_fstart.reserve(pl.fstart.size()); d_kstart.reserve(pl.kstart.size());
+    d_inc.reserve(pl.inc.size() + 1); d_sats.reserve((size_t)n_sats + 1); d_w.reserve((size_t)n_w + 1);
+    d_sums.reserve((size_t)(Pd + 1) * GLIO_NACC_DD);
+    if (!grouped.empty()) GLIO_CUDA_TRY(cudaMemcpyAsync(d_f.p, grouped.data(), grouped.size() * sizeof(DdPsrFactor), cudaMemcpyHostToDevice, c->st));
+    GLIO_CUDA_TRY(cudaMemcpyAsync(d_fstart.p, pl.fstart.data(), pl.fstart.size() * sizeof(int), cudaMemcpyHostToDevice, c->st));
+    GLIO_CUDA_TRY(cudaMemcpyAsync(d_kstart.p, pl.kstart.data(), pl.kstart.size() * sizeof(int), cudaMemcpyHostToDevice, c->st));
+    if (!pl.inc.empty()) GLIO_CUDA_TRY(cudaMemcpyAsync(d_inc.p, pl.inc.data(), pl.inc.size() * sizeof(BinIncidence), cudaMemcpyHostToDevice, c->st));
+    if (n_sats > 0) GLIO_CUDA_TRY(cudaMemcpyAsync(d_sats.p, sats, (size_t)n_sats * sizeof(DdPsrSat), cudaMemcpyHostToDevice, c->st));
+    if (n_w > 0) GLIO_CUDA_TRY(cudaMemcpyAsync(d_w.p, W, (size_t)n_w * sizeof(double), cudaMemcpyHostToDevice, c->st));
+    GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));   // also: no evaluation still reads the buffers released below
+    c->d_dd_f = std::move(d_f); c->d_dd_fstart = std::move(d_fstart); c->d_dd_inc_start = std::move(d_kstart);
+    c->d_dd_inc = std::move(d_inc); c->d_dd_sats = std::move(d_sats); c->d_dd_w = std::move(d_w); c->d_dd_sums = std::move(d_sums);
+    c->dd_pairs.swap(pl.pairs); c->dd_max_kf = pl.max_kf; c->dd_frame = fr;
+  });
+}
+
+int glio_batch_dd_psr_pair_list(glio_ctx* c, int64_t capacity, int32_t* a, int32_t* b, int64_t* n_pairs) {
+  if (!c) return GLIO_ERR_ARG;
+  return guarded(c, [&] {
+    const int64_t P = (int64_t)c->dd_pairs.size();
+    if (n_pairs) *n_pairs = P;
+    if (!a && !b) return;
+    GLIO_REQUIRE(capacity >= P, GLIO_ERR_ARG, "glio_batch_dd_psr_pair_list: capacity too small");
+    for (int64_t k = 0; k < P; ++k) { if (a) a[k] = c->dd_pairs[k].first; if (b) b[k] = c->dd_pairs[k].second; }
+  });
+}
+
+int glio_eval_dd_psr_factors(glio_ctx* c, int K, const double* poses, double* Hdiag, double* Hoff, double* g, double* cost) {
+  if (!c) return GLIO_ERR_ARG;
+  return guarded(c, [&] {
+    GLIO_REQUIRE(K > 0 && poses, GLIO_ERR_ARG, "bad arguments");
+    GLIO_REQUIRE(c->dd_max_kf < K, GLIO_ERR_ARG, "glio_eval_dd_psr_factors: a DD factor references a keyframe outside [0, K)");
+    const int Pd = (int)c->dd_pairs.size();
+    eval_factor_blocks(c, K, poses, Pd, [&](bool want_jac) {
+      eval_dd_psr_run(c->d_dd_f.p, c->d_dd_fstart.p, c->d_dd_sats.p, c->d_dd_w.p, c->dd_frame, Pd, K, c->dd_max_kf + 1, c->d_dd_inc_start.p,
+                      c->d_dd_inc.p, c->d_bin_poses.p, want_jac, /*add*/ false, c->d_dd_sums.p, c->d_bin_diag.p, c->d_bin_off.p, c->st, c->lc);
+    }, Hdiag, Hoff, g, cost);
+  });
+}
+
+int glio_batch_use_dd_psr_factors(glio_ctx* c, int on) {
+  if (!c) return GLIO_ERR_ARG;
+  c->batch_use_dd = on != 0;
   return GLIO_OK;
 }
 
@@ -2505,6 +2624,9 @@ int glio_batch_solve(glio_ctx* c, int K, double* poses, double* speed_bias, glio
     int span = 1;
     for (auto& p : c->pairs) span = std::max(span, std::abs(p->cur - p->oth));
     if (add_pose) for (auto& p : c->pose_pairs) span = std::max(span, p.second - p.first);
+    const bool add_dd = c->batch_use_dd && !c->dd_pairs.empty();
+    GLIO_REQUIRE(!add_dd || c->dd_max_kf < K, GLIO_ERR_ARG, "glio_batch_solve: a DD factor references a keyframe outside [0, K)");
+    if (add_dd) for (auto& p : c->dd_pairs) span = std::max(span, p.second - p.first);
     const int hb = (span + 1) * nt - 1;
     TrustRegionDogleg solver(L.blocks(), solver_options_from(o));
     std::vector<double> x((size_t)K * L.na), pz((size_t)K * 7), sz((size_t)K * 9);
@@ -2513,7 +2635,7 @@ int glio_batch_solve(glio_ctx* c, int K, double* poses, double* speed_bias, glio
       L.unpack(xa, pz.data(), sz.data());
       // the device evaluates the LiDAR pairs (and a sharded run sums them over the ranks) while the host evaluates its own
       // factors into the freshly reset band; the device blocks are added when they have arrived
-      eval_binary_launch(c, K, pz.data(), want_jac, 0.0, c->batch_use_edges ? BIN_PLANES_EDGES : BIN_PLANES, add_pose);
+      eval_binary_launch(c, K, pz.data(), want_jac, 0.0, c->batch_use_edges ? BIN_PLANES_EDGES : BIN_PLANES, add_pose, add_dd);
       double ct = 0;
       int hrc = 0;
       if (want_jac) { H->reset(n, hb); std::fill(g, g + n, 0.0); }
@@ -2526,9 +2648,11 @@ int glio_batch_solve(glio_ctx* c, int K, double* poses, double* speed_bias, glio
         double* a = H->a.data();
         add_diag_blocks(H, c->h_bin_diag.p, K, nt);
         for (int k = 0; k < K; ++k) for (int p = 0; p < 6; ++p) g[nt * k + p] += c->h_bin_diag.p[(size_t)k * GLIO_NACC + 21 + p];
-        const size_t P = c->pairs.size(), Pt = P + (add_pose ? c->pose_pairs.size() : 0);
-        for (size_t pi = 0; pi < Pt; ++pi) {                           // LiDAR pairs (cur, oth), then pose pairs (a, b)
-          const int kc = pi < P ? c->pairs[pi]->cur : c->pose_pairs[pi - P].first, ko = pi < P ? c->pairs[pi]->oth : c->pose_pairs[pi - P].second;
+        const size_t P = c->pairs.size(), Pp = add_pose ? c->pose_pairs.size() : 0, Pt = P + Pp + (add_dd ? c->dd_pairs.size() : 0);
+        for (size_t pi = 0; pi < Pt; ++pi) {                           // LiDAR pairs (cur, oth), then pose pairs (a, b), then DD pairs (a, b)
+          const std::pair<int, int> ab = pi < P ? std::pair<int, int>(c->pairs[pi]->cur, c->pairs[pi]->oth)
+                                                : pi < P + Pp ? c->pose_pairs[pi - P] : c->dd_pairs[pi - P - Pp];
+          const int kc = ab.first, ko = ab.second;
           const double* ob = c->h_bin_off.p + pi * 36;                 // d2 cost / d x_cur[p] d x_oth[q]
           if (kc > ko) {                                               // rows of cur, six contiguous band entries each
             for (int p = 0; p < 6; ++p) { double* row = a + (size_t)(nt * kc + p) * w + (nt * ko - (nt * kc + p) + H->hb); for (int q = 0; q < 6; ++q) row[q] += ob[6 * p + q]; }

@@ -363,6 +363,22 @@ void eval_pose_run(const PoseFactor* d_f, const int* d_fstart, int n_pairs, int 
                    const BinIncidence* d_inc, const double* d_poses, bool want_jac, bool add, double* d_sums, double* d_diag, double* d_off,
                    cudaStream_t st, LaunchCounter& lc);
 
+// ---- K2g (eval.cu): the batch refinement's double-differenced pseudorange factors (dd_psr_factor_20); the layouts of the public
+// glio_dd_psr_factor and glio_dd_psr_sat
+struct DdPsrFactor { int32_t i, j, n_sat, master, active, reserved; int64_t sat_offset, w_offset; double ratio, threshold, station[3]; };
+struct DdPsrSat { double sat_user[3], sat_ref[3], psr_user, psr_ref; };
+// the per-list constants: R_ecef_local (row-major) and the anchor, passed by value
+struct DdPsrFrame { double R[9]; double anchor[3]; };
+// Per distinct keyframe pair (a, b), a < b, the sums of its factors' 6 x 6 J^T J, J^T r and cost over (t_a, t_b): aa and bb
+// upper-triangular (6 + 6), ab row-major (9), g (3 + 3), cost.
+constexpr int GLIO_NACC_DD = 28;
+// k_psr_pair_sums: the factors of pair p are f[fstart[p] .. fstart[p+1]) in list order, their satellites and weights read at the
+// records' offsets in d_sats / d_w -> d_sums (n_pairs x 28); k_psr_assemble: as k_pose_assemble, the t columns only.
+// Two launches whatever K; with n_pairs = 0 only the assembly runs.
+void eval_dd_psr_run(const DdPsrFactor* d_f, const int* d_fstart, const DdPsrSat* d_sats, const double* d_w, const DdPsrFrame& frame,
+                     int n_pairs, int K, int n_inc_kf, const int* d_kf_inc_start, const BinIncidence* d_inc, const double* d_poses,
+                     bool want_jac, bool add, double* d_sums, double* d_diag, double* d_off, cudaStream_t st, LaunchCounter& lc);
+
 // ---- front-end feature extraction (features.cu; Preprocessing.cpp:529-655)
 constexpr int FEAT_MAX_SHARP = 12, FEAT_MAX_LESS_SHARP = 60, FEAT_MAX_FLAT = 24;   // per ring: 6 sectors x (2, 10, 4)
 struct FeatArgs {

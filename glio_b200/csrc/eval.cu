@@ -780,4 +780,171 @@ void eval_pose_run(const PoseFactor* d_f, const int* d_fstart, int n_pairs, int 
   GLIO_CUDA_TRY(cudaGetLastError());
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// K2g: the batch refinement's double-differenced pseudorange factors (glio_batch_set_dd_psr_factors), as dd_psr_factor_20's
+// Evaluate forms them (dd_psr_factor.hpp:25-171; blocks t_i, t_j, and the constant yaw and anchor folded into R and anchor):
+//   P = R (ratio t_i + (1 - ratio) t_j) + anchor;  row k <-> satellite s = k + (k >= m), m the master:
+//   e_k = (|su_s - P| - |sr_s - st|) - (|su_m - P| - |sr_m - st|) - ((pu_s - pr_s) - (pu_m - pr_m)),  w_k = |e_k| > thr ? 0.05 : 1
+//   r_k = w_k e_k,  J_i row k = (-u_s^T R w_k ratio) - (-u_m^T R w_k ratio), J_j the same with (1 - ratio),  u = normalized(su - P)
+//   then r = W r, J = W J when the factor has a weight matrix.  normalized() is Eigen 3.3's: d / |d| if |d|^2 > 0, else d.
+// Layout: one warp per distinct pair (a, b); lane k owns row k, walks the pair's factors in list order and accumulates its row's
+// contributions to the 28 pair sums (aa, bb upper-triangular over t, ab, g, cost) in registers; W is applied by broadcasting the
+// raw rows with __shfl_sync in index order; one butterfly reduction over the lanes at the end.  k_psr_assemble then sums each
+// keyframe's pairs in incidence order into the t columns of the K x 28 layout.  No floating-point atomics.
+// ---------------------------------------------------------------------------------------------------------------
+constexpr int ND = GLIO_NACC_DD;
+constexpr int PSR_T = 128;   // 4 pairs per block
+
+// d = a - b and |d|^2 with the roundings pinned: equal arguments give equal bits wherever they are formed
+__device__ __forceinline__ double psr_diff_sq(const double a[3], const double b[3], double d[3]) {
+  d[0] = __dsub_rn(a[0], b[0]); d[1] = __dsub_rn(a[1], b[1]); d[2] = __dsub_rn(a[2], b[2]);
+  return __fma_rn(d[2], d[2], __fma_rn(d[1], d[1], __dmul_rn(d[0], d[0])));
+}
+
+template <bool WANT_JAC>
+__global__ void __launch_bounds__(PSR_T) k_psr_pair_sums(const DdPsrFactor* __restrict__ fl, const int* __restrict__ fstart,
+                                                         const DdPsrSat* __restrict__ sats, const double* __restrict__ Wm, const DdPsrFrame fr,
+                                                         int n_pairs, const double* __restrict__ poses, double* __restrict__ sums) {
+  const int p = blockIdx.x * (PSR_T / 32) + (threadIdx.x >> 5);
+  if (p >= n_pairs) return;                       // a warp leaves as a whole; the shuffles below use the full mask
+  const int k = threadIdx.x & 31;
+  double acc[ND];
+#pragma unroll
+  for (int e = 0; e < ND; ++e) acc[e] = 0.0;
+  const int f1 = fstart[p];
+  for (int f = f1, f2 = fstart[p + 1]; f < f2; ++f) {
+    const DdPsrFactor F = fl[f];
+    const double* ti = poses + 7 * F.i;
+    const double* tj = poses + 7 * F.j;
+    const double ra = F.ratio, rb = 1.0 - F.ratio;
+    double loc[3], P[3];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) loc[c] = ra * ti[c] + rb * tj[c];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) P[c] = fr.R[3 * c] * loc[0] + fr.R[3 * c + 1] * loc[1] + fr.R[3 * c + 2] * loc[2] + fr.anchor[c];
+    const int nr = F.n_sat - 1, m = F.master;
+    const DdPsrSat* S = sats + F.sat_offset;
+    double r = 0.0, J[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+    if (k < nr) {
+      const DdPsrSat Sm = S[m], Ss = S[k + (k >= m ? 1 : 0)];
+      double dus[3], dum[3], drs[3], drm[3];
+      const double zus = psr_diff_sq(Ss.sat_user, P, dus), zum = psr_diff_sq(Sm.sat_user, P, dum);
+      const double zrs = psr_diff_sq(Ss.sat_ref, F.station, drs), zrm = psr_diff_sq(Sm.sat_ref, F.station, drm);
+      const double nus = sqrt(zus), num = sqrt(zum);
+      const double dd_est = (nus - sqrt(zrs)) - (num - sqrt(zrm));
+      const double dd_psr = (Ss.psr_user - Ss.psr_ref) - (Sm.psr_user - Sm.psr_ref);
+      const double e = dd_est - dd_psr;
+      const double w = fabs(e) > F.threshold ? 0.05 : 1.0;
+      r = w * e;
+      if (WANT_JAC) {
+#pragma unroll
+        for (int c = 0; c < 3; ++c) {
+          if (zus > 0.0) dus[c] = dus[c] / nus;
+          if (zum > 0.0) dum[c] = dum[c] / num;
+        }
+#pragma unroll
+        for (int c = 0; c < 3; ++c) {
+          const double as = -dus[0] * fr.R[c] - dus[1] * fr.R[3 + c] - dus[2] * fr.R[6 + c];   // (-u_s^T R)[c]
+          const double am = -dum[0] * fr.R[c] - dum[1] * fr.R[3 + c] - dum[2] * fr.R[6 + c];   // (-u_m^T R)[c]
+          J[c] = as * w * ra - am * w * ra;
+          J[3 + c] = as * w * rb - am * w * rb;
+        }
+      }
+    }
+    if (F.w_offset >= 0) {                        // r = W r, J = W J: row l broadcast from lane l, in index order
+      const double* Wf = Wm + F.w_offset;
+      double rw = 0.0, Jw[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+      for (int l = 0; l < nr; ++l) {
+        const double wl = k < nr ? Wf[k * nr + l] : 0.0;
+        rw += wl * __shfl_sync(0xffffffffu, r, l);
+        if (WANT_JAC) {
+#pragma unroll
+          for (int q = 0; q < 6; ++q) Jw[q] += wl * __shfl_sync(0xffffffffu, J[q], l);
+        }
+      }
+      r = rw;
+#pragma unroll
+      for (int q = 0; q < 6; ++q) J[q] = Jw[q];
+    }
+    acc[27] += 0.5 * r * r;
+    if (WANT_JAC) {
+      const bool ilo = F.i < F.j;
+      const double Ja[3] = {ilo ? J[0] : J[3], ilo ? J[1] : J[4], ilo ? J[2] : J[5]};
+      const double Jb[3] = {ilo ? J[3] : J[0], ilo ? J[4] : J[1], ilo ? J[5] : J[2]};
+      int s = 0;
+#pragma unroll
+      for (int a = 0; a < 3; ++a)
+#pragma unroll
+        for (int b = a; b < 3; ++b, ++s) { acc[s] += Ja[a] * Ja[b]; acc[6 + s] += Jb[a] * Jb[b]; }
+#pragma unroll
+      for (int a = 0; a < 3; ++a) {
+#pragma unroll
+        for (int b = 0; b < 3; ++b) acc[12 + 3 * a + b] += Ja[a] * Jb[b];
+        acc[21 + a] += Ja[a] * r;
+        acc[24 + a] += Jb[a] * r;
+      }
+    }
+  }
+  // butterfly over the 32 lanes: a lane and its partner add the same two values, so every lane ends with the same bits
+#pragma unroll
+  for (int e = WANT_JAC ? 0 : 27; e < ND; ++e)
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) acc[e] += __shfl_xor_sync(0xffffffffu, acc[e], o);
+  double* Sp = sums + (size_t)p * ND;
+#pragma unroll
+  for (int e = WANT_JAC ? 0 : 27; e < ND; ++e)
+    if (k == e) Sp[e] = acc[e];
+}
+
+// thread t < K*28: diag entry (kf, e) (the GLIO_NACC layout) from the kf's pairs in incidence order, the t rows and columns only;
+// then, with WANT_JAC, one thread per entry of the n_pairs 6 x 6 ab blocks
+template <bool WANT_JAC>
+__global__ void __launch_bounds__(256) k_psr_assemble(const double* __restrict__ S, int K, int n_pairs, int n_inc_kf,
+                                                      const int* __restrict__ kf_inc_start, const BinIncidence* __restrict__ inc, bool add,
+                                                      double* __restrict__ diag, double* __restrict__ off) {
+  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const int64_t nd = (int64_t)K * GLIO_NACC;
+  if (t < nd) {
+    const int kf = (int)(t / GLIO_NACC), e = (int)(t - (int64_t)kf * GLIO_NACC);
+    // 6 x 6 upper triangle -> the 3 x 3 t block: (0,0..2) = 0..2, (1,1..2) = 6..7, (2,2) = 11; g_t = 21..23; cost = 27
+    const int src = e <= 2 ? e : e == 6 || e == 7 ? e - 3 : e == 11 ? 5 : -1;
+    double v = 0.0;
+    if (kf < n_inc_kf && ((WANT_JAC && (src >= 0 || (e >= 21 && e < 24))) || e == 27)) {
+      for (int i = kf_inc_start[kf]; i < kf_inc_start[kf + 1]; ++i) {
+        const double* s = S + (size_t)inc[i].pair * ND;
+        const int role = inc[i].role;
+        if (e < 21) v += s[6 * role + src];                     // aa | bb
+        else if (e < 27) v += s[21 + 3 * role + (e - 21)];     // g_a | g_b
+        else if (role == 0) v += s[27];                         // the cost goes to a
+      }
+    }
+    diag[t] = add ? diag[t] + v : v;
+  } else if (WANT_JAC) {
+    const int64_t o = t - nd;
+    if (o < (int64_t)n_pairs * 36) {
+      const int64_t pr = o / 36;
+      const int q = (int)(o - pr * 36), row = q / 6, col = q - 6 * row;
+      off[o] = row < 3 && col < 3 ? S[pr * ND + 12 + 3 * row + col] : 0.0;
+    }
+  }
+}
+
+void eval_dd_psr_run(const DdPsrFactor* d_f, const int* d_fstart, const DdPsrSat* d_sats, const double* d_w, const DdPsrFrame& frame,
+                     int n_pairs, int K, int n_inc_kf, const int* d_kf_inc_start, const BinIncidence* d_inc, const double* d_poses,
+                     bool want_jac, bool add, double* d_sums, double* d_diag, double* d_off, cudaStream_t st, LaunchCounter& lc) {
+  if (n_pairs > 0) {
+    const int nb = (n_pairs + PSR_T / 32 - 1) / (PSR_T / 32);
+    lc.begin(want_jac ? "k_psr_pair_sums" : "k_psr_pair_sums_cost", st);
+    (want_jac ? k_psr_pair_sums<true> : k_psr_pair_sums<false>)<<<nb, PSR_T, 0, st>>>(d_f, d_fstart, d_sats, d_w, frame, n_pairs,
+                                                                                     d_poses, d_sums);
+    lc.end(st);
+  }
+  const int64_t n = (int64_t)K * GLIO_NACC + (want_jac ? (int64_t)n_pairs * 36 : 0);
+  lc.begin("k_psr_assemble", st);
+  (want_jac ? k_psr_assemble<true> : k_psr_assemble<false>)<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(
+      d_sums, K, n_pairs, n_inc_kf, d_kf_inc_start, d_inc, add, d_diag, d_off);
+  lc.end(st);
+  GLIO_CUDA_TRY(cudaGetLastError());
+}
+
 }  // namespace glio

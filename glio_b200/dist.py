@@ -39,8 +39,8 @@ def owner_of(cur, K, world):
 
 
 def pose_factor_active(i, j, K, world, rank):
-    """The active mask of one rank's pose-factor list: a factor belongs to the rank that owns its lower keyframe (owner_of's
-    contiguous ranges).  Every rank passes the same list, so every rank gets the same pose-pair layout."""
+    """The active mask of one rank's pose-factor or DD-pseudorange list: a factor belongs to the rank that owns its lower keyframe
+    (owner_of's contiguous ranges).  Every rank passes the same list, so every rank gets the same pair layout."""
     lo = np.minimum(np.asarray(i), np.asarray(j))
     return (owner_of(lo, K, world) == rank).astype(np.int32)
 

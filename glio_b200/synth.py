@@ -312,6 +312,175 @@ def pose_graph_problem(K=200, seed=SEED0 + 16, search_range=6, level=0, sig_t=0.
     return out
 
 
+# ---------------------------------------------------------------------------------------------------------------------------
+# GNSS double-differenced pseudorange factors of the batch refinement (dd_psr_factor_20, Estimator.cpp:3086-3272)
+# ---------------------------------------------------------------------------------------------------------------------------
+WGS84_A, WGS84_E2 = 6378137.0, 6.69437999014e-3            # gnss_constant.hpp: EARTH_SEMI_MAJOR, EARTH_ECCE_2
+_PI = 3.1415926535897932
+_R2D, _D2R = 180.0 / _PI, _PI / 180.0
+DD_PSR_THRESHOLDS = (1e9, 10.0, 8.0, 6.0)                   # DDpsr_threshold of the 4 outer passes (Estimator.cpp:2764-2765)
+# one GNSS_Raw of an epoch: the PRN, the satellite's ECEF position, the raw pseudorange and the elevation seen by the receiver
+GNSS_RAW_DTYPE = np.dtype([("prn", "<i4"), ("sat_pos", "<f8", (3,)), ("psr", "<f8"), ("elevation", "<f8")])
+
+
+# the constellation of a PRN (gnss_tools.h:1116-1168, PRN 84 counts as GPS and as Galileo there) in the Estimator's order
+def prn_is_gps(prn): return prn <= 32 or prn == 84
+def prn_is_bds(prn): return 87 <= prn <= 121
+def prn_is_glo(prn): return 32 < prn <= 56
+def prn_is_gal(prn): return 56 < prn < 87
+
+
+# (predicate, the pseudorange > 1000 check): prepareGPS/BDSDDPsrData check it, prepareGLO/GALDDPsrData do not
+DD_PSR_SYSTEMS = ((prn_is_gps, True), (prn_is_bds, True), (prn_is_glo, False), (prn_is_gal, False))
+
+
+def geo_to_ecef(lat_deg, lon_deg, h):
+    lat, lon = np.deg2rad(lat_deg), np.deg2rad(lon_deg)
+    N = WGS84_A / np.sqrt(1.0 - WGS84_E2 * np.sin(lat) ** 2)
+    return np.array([(N + h) * np.cos(lat) * np.cos(lon), (N + h) * np.cos(lat) * np.sin(lon), (N * (1.0 - WGS84_E2) + h) * np.sin(lat)])
+
+
+def ecef_local_rotation(anchor, yaw):
+    """R_ecef_local = ecef2rotation(anchor) * R_enu_local(yaw), gnss_comm's closed form (gnss_utility.cpp:347-388, :738-753): Bowring's
+    latitude, atan2 longitude (through degrees, as ecef2geo returns them), the ENU -> ECEF columns, times Rz(yaw)."""
+    x, y, z = (float(v) for v in anchor)
+    a, e2 = WGS84_A, WGS84_E2
+    a2 = a * a; b2 = a2 * (1 - e2); b = np.sqrt(b2); ep2 = (a2 - b2) / b2
+    p = np.hypot(x, y)
+    s1, s2 = z * a, p * b
+    h = np.sqrt(s1 * s1 + s2 * s2)
+    sin_t, cos_t = s1 / h, s2 / h
+    s1 = z + ep2 * b * sin_t ** 3
+    s2 = p - a * e2 * cos_t ** 3
+    lat = np.arctan(s1 / s2) * _R2D * _D2R
+    lon = np.arctan2(y, x) * _R2D * _D2R
+    sl, cl, so, co = np.sin(lat), np.cos(lat), np.sin(lon), np.cos(lon)
+    R_ecef_enu = np.array([[-so, -sl * co, cl * co], [co, -sl * so, cl * so], [0.0, cl, sl]])
+    cy, sy = np.cos(yaw), np.sin(yaw)
+    return R_ecef_enu @ np.array([[cy, -sy, 0.0], [sy, cy, 0.0], [0.0, 0.0, 1.0]])
+
+
+def gnss_epochs(kf_times, truth_t, R, anchor, station, rng, rate=10.0, outlier_frac=0.03, drop_frac=0.05):
+    """Seeded rover and station GNSS epochs at `rate` Hz over the keyframe times.  Satellites of GPS, GLONASS, Galileo and BeiDou
+    (MEO, plus two BeiDou IGSO) on orbits of their systems' radii move slowly across the sky; the station's satellite positions differ
+    from the rover's by up to a few metres (their own transmit times).  Pseudoranges = range + receiver clock - satellite clock
+    (both cancel in the double difference) + noise (rover 1.5 m, station 0.3 m) + on a fraction of rover rows a multipath excess of
+    20 .. 60 m; a few rover rows carry a zero pseudorange and a few satellites are missing from one receiver.  The rover's position
+    is the true trajectory, linear in time between keyframes, through R and anchor.  Returns a list of (time, user, ref) with
+    GNSS_RAW_DTYPE arrays (elevations in degrees, seen from the anchor)."""
+    R_enu = ecef_local_rotation(anchor, 0.0)                      # ENU -> ECEF at the anchor
+    sats = []                                                   # (prn, radius, azimuth0, elevation0, d az, d el) per satellite
+    for prns, radius in ((range(1, 33), 26_560e3), (range(33, 57), 25_510e3), (range(57, 87), 29_600e3), (range(87, 122), 27_900e3)):
+        for prn in rng.choice(list(prns), 11, replace=False):
+            sats.append((int(prn), radius, rng.uniform(0, 2 * np.pi), rng.uniform(np.deg2rad(12), np.deg2rad(85)),
+                         rng.normal(0, 2e-5), rng.normal(0, 1e-5)))
+    for prn in (120, 121):                                      # BeiDou IGSO / GEO radius
+        if all(s[0] != prn for s in sats):
+            sats.append((prn, 42_164e3, rng.uniform(0, 2 * np.pi), rng.uniform(np.deg2rad(30), np.deg2rad(60)), 0.0, 0.0))
+    prn, radius, az0, el0, daz, d_el = (np.array(c) for c in zip(*sats))
+    ns = len(prn)
+    sat_clock = rng.uniform(-3e5, 3e5, ns)
+    # zero pseudoranges only where every system's filter drops them: PRN 84 is Galileo too, whose filter keeps it
+    zero_ok = np.array([(prn_is_gps(p) or prn_is_bds(p)) and not (prn_is_glo(p) or prn_is_gal(p)) for p in prn])
+    t0, t1 = kf_times[0], kf_times[-1]
+    times = t0 - 0.05 + np.arange(int(np.ceil((t1 - t0 + 0.1) * rate)) + 1) / rate
+    out = []
+    for t in times:
+        k = int(np.clip(np.searchsorted(kf_times, t) - 1, 0, len(kf_times) - 2))
+        u = np.clip((t - kf_times[k]) / (kf_times[k + 1] - kf_times[k]), 0.0, 1.0)
+        P = R @ ((1 - u) * truth_t[k] + u * truth_t[k + 1]) + anchor
+        clk_u, clk_r = rng.uniform(-3e5, 3e5, 2)
+        az, el = az0 + daz * (t - t0), np.clip(el0 + d_el * (t - t0), np.deg2rad(10), np.deg2rad(89))
+        d = np.stack([np.sin(az) * np.cos(el), np.cos(az) * np.cos(el), np.sin(el)], axis=1) @ R_enu.T
+        bd = d @ anchor                                         # |anchor + rho d| = radius
+        rho = -bd + np.sqrt(bd * bd - (anchor @ anchor - radius * radius))
+        su = anchor + rho[:, None] * d
+        sr = su + rng.uniform(-3.0, 3.0, (ns, 3))
+        pu = np.linalg.norm(su - P, axis=1) + clk_u - sat_clock + rng.normal(0, 1.5, ns)
+        pu += np.where(rng.random(ns) < outlier_frac, rng.uniform(20.0, 60.0, ns), 0.0)
+        pu = np.where((rng.random(ns) < 0.01) & zero_ok, 0.0, pu)
+        pr = np.linalg.norm(sr - station, axis=1) + clk_r - sat_clock + rng.normal(0, 0.3, ns)
+        user = np.zeros(ns, GNSS_RAW_DTYPE); ref = np.zeros(ns, GNSS_RAW_DTYPE)
+        user["prn"], user["sat_pos"], user["psr"], user["elevation"] = prn, su, pu, np.rad2deg(el)
+        ref["prn"], ref["sat_pos"], ref["psr"], ref["elevation"] = prn, sr, pr, np.rad2deg(el)
+        user = user[rng.random(ns) >= drop_frac]; ref = ref[rng.random(ns) >= drop_frac]
+        out.append((float(t), user[rng.permutation(len(user))], ref))   # the rover lists its satellites in its own order
+    return out
+
+
+def _lower_upper(kf_times, t):
+    """getGlobalLowerUpperIdx (Estimator.cpp:1635-1662) with keyframe_idx[0] = 1: the keyframes k = 0 .. K-2 closest to t strictly
+    before and strictly after it, or -1."""
+    cand = np.asarray(kf_times[:-1])
+    before, after = np.nonzero(cand < t)[0], np.nonzero(cand > t)[0]
+    lo = int(before[np.argmin(t - cand[before])]) if len(before) else -1
+    hi = int(after[np.argmin(cand[after] - t)]) if len(after) else -1
+    return lo, hi
+
+
+def dd_psr_factors(epochs, kf_times, trans, station, threshold):
+    """The dd_psr_factor_20 list of one outer pass of optimizeBatchWithLandMark (Estimator.cpp:3086-3272) over GNSS epochs
+    (gnss_epochs' format): an epoch inside the keyframe times is bracketed by getGlobalLowerUpperIdx (left = i, right = j, ratio =
+    (t_j - t) / (t_j - t_i)); it is kept only when the right keyframe's current translation trans[j] is at least 1 m from the
+    last kept one (P_add_idx, starting at 0).  Per constellation (GPS, BeiDou, GLONASS, Galileo) the rover's satellites also seen by
+    the station (GPS and BeiDou: rover pseudorange > 1000) in the rover's order, the master the first with the largest elevation by
+    the reference's |ele| > maxEle test, and a factor when more than 2 satellites remain.  Weight identity.  Returns the columns of
+    api.dd_psr_factor_records (sat_offset in order) and the satellites (sat_user, sat_ref, psr_user, psr_ref)."""
+    cols = dict(i=[], j=[], n_sat=[], master=[], ratio=[], threshold=[], station=[])
+    su, sr, pu, pr = [], [], [], []
+    p_add = np.zeros(3)
+    for t, user, ref in epochs:
+        if t > kf_times[-1] or t < kf_times[0]:
+            continue
+        lo, hi = _lower_upper(kf_times, t)
+        if lo < 0 or hi < 0:
+            continue
+        ratio = (kf_times[hi] - t) / (kf_times[hi] - kf_times[lo])
+        if np.linalg.norm(trans[hi] - p_add) < 1:
+            continue
+        p_add = np.array(trans[hi], np.float64)
+        ref_of = {}
+        for b, prn in enumerate(ref["prn"].tolist()):
+            ref_of.setdefault(prn, []).append(b)
+        for is_sys, psr_check in DD_PSR_SYSTEMS:
+            pick = [(a, b) for a, prn in enumerate(user["prn"].tolist()) for b in ref_of.get(prn, ())
+                    if is_sys(prn) and (not psr_check or user[a]["psr"] > 1000)]
+            if len(pick) <= 2:
+                continue
+            ele = [float(user[a]["elevation"]) for a, _ in pick]
+            master, max_ele = -1, 0.0
+            for m, e in enumerate(ele):
+                if abs(e) > max_ele:
+                    max_ele, master = e, m
+            if master < 0 or len(pick) > 20:
+                raise ValueError("an epoch the reference cannot evaluate (no master, or more than 20 satellites)")
+            cols["i"].append(lo); cols["j"].append(hi); cols["n_sat"].append(len(pick)); cols["master"].append(master)
+            cols["ratio"].append(ratio); cols["threshold"].append(threshold); cols["station"].append(np.asarray(station, np.float64))
+            for a, b in pick:
+                su.append(user[a]["sat_pos"]); sr.append(ref[b]["sat_pos"]); pu.append(user[a]["psr"]); pr.append(ref[b]["psr"])
+    cols = {k: np.asarray(v) for k, v in cols.items()}
+    cols["station"] = cols["station"].reshape(-1, 3)
+    return cols, dict(sat_user=np.asarray(su).reshape(-1, 3), sat_ref=np.asarray(sr).reshape(-1, 3), psr_user=np.asarray(pu, np.float64),
+                      psr_ref=np.asarray(pr, np.float64))
+
+
+def dd_psr_problem(K=200, seed=SEED0 + 17, search_range=6, outer_pass=1, yaw=0.3):
+    """The level-0 batch refinement problem with its GNSS factors: pose_graph_problem's pose factors and trajectory, keyframe times
+    0.25 .. 0.45 s apart (about 3 Hz), an anchor in Hong Kong with the local frame rotated by `yaw` from ENU, a station 3 km away, the
+    epochs of gnss_epochs and the DD list of outer pass `outer_pass` (threshold DD_PSR_THRESHOLDS[outer_pass]) built against
+    poses_init.  Adds R (R_ecef_local), anchor, station, kf_times, epochs, dd (the factor columns) and dd_sats."""
+    P = pose_graph_problem(K=K, seed=seed, search_range=search_range)
+    rng = np.random.default_rng([seed, 1])
+    kf_times = 1_600_000_000.0 + np.concatenate([[0.0], np.cumsum(rng.uniform(0.25, 0.45, K - 1))])
+    anchor = geo_to_ecef(22.3, 114.18, 5.0)
+    station = anchor + ecef_local_rotation(anchor, 0.0) @ np.array([2400.0, -1800.0, 25.0])
+    R = ecef_local_rotation(anchor, yaw)
+    epochs = gnss_epochs(kf_times, P["poses_true"][:, :3], R, anchor, station, rng)
+    dd, sats = dd_psr_factors(epochs, kf_times, P["poses_init"][:, :3], station, DD_PSR_THRESHOLDS[outer_pass])
+    P.update(R=R, anchor=anchor, station=station, kf_times=kf_times, epochs=epochs, dd=dd, dd_sats=sats, outer_pass=outer_pass)
+    return P
+
+
 def raw_elevations(n_rings):
     """Elevation table (degrees) of a raw sweep for the ring rules of Preprocessing.cpp:441-483: every line sits inside its ring's
     interval, plus lines each rule treats specially.  16: VLP-16's -15..15 step 2, one line at -16.5 that int() truncates toward

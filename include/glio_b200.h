@@ -616,7 +616,8 @@ int glio_batch_select_random(glio_ctx* ctx, const int32_t* cur, const int32_t* o
                              const glio_select_options* options, int64_t* n_active);
 int glio_batch_get_selection(glio_ctx* ctx, int cur, int oth, int64_t capacity, int32_t* keep, int64_t* n);
 int glio_batch_pair_list(glio_ctx* ctx, int64_t capacity, int32_t* cur, int32_t* oth, int64_t* n_pairs);
-int glio_batch_clear(glio_ctx* ctx);   /* also empties the pose-factor list (glio_batch_set_pose_factors) */
+int glio_batch_clear(glio_ctx* ctx);   /* also empties the pose-factor and DD-pseudorange lists (glio_batch_set_pose_factors,
+                                          glio_batch_set_dd_psr_factors) */
 
 /* Creates (empty) pair entries in the given order without associating them: on a keyframe-sharded multi-GPU run
  * every rank declares the SAME global pair list and then associates only the pairs it owns, so the block
@@ -794,6 +795,53 @@ int glio_eval_pose_factors(glio_ctx* ctx, int K, const double* poses, double* Hd
  * a keyframe >= K makes glio_batch_solve return GLIO_ERR_ARG.  glio_eval_binary and glio_eval_binary_edge never add pose blocks. */
 int glio_batch_use_pose_factors(glio_ctx* ctx, int on);
 
+/* ---- K2g: the batch refinement's double-differenced pseudorange factors (dd_psr_factor_20, added per epoch and constellation by
+ * optimizeBatchWithLandMark through addDDPsrResFactor_gl, Estimator.cpp:3086-3272 and :1902-1913), evaluated on the device.
+ * Per list: R = R_ecef_local (row-major 3 x 3) = ecef2rotation(anchor) * R_enu_local(yaw), and anchor = anchor_ecef; the caller
+ * forms R once, since the yaw and anchor blocks are constant in the batch.  Per factor: keyframes i != j, ratio, threshold,
+ * station (the factor's Station_pos), n_sat satellites (2 <= n_sat <= GLIO_DD_PSR_MAX_SAT: the reference's fixed buffer holds 19
+ * rows) at sats[sat_offset .. sat_offset + n_sat), the master 0 <= master < n_sat, and a dense row-major (n_sat-1) x (n_sat-1)
+ * weight W at W[w_offset ..], or w_offset = -1 for identity (the batch passes identity).  Rows k = 0 .. n_sat-2 belong to the
+ * satellites s != master in index order:
+ *   local = ratio t_i + (1 - ratio) t_j,  P = R local + anchor
+ *   e_k = (|sat_user_s - P| - |sat_ref_s - station|) - (|sat_user_m - P| - |sat_ref_m - station|)
+ *         - ((psr_user_s - psr_ref_s) - (psr_user_m - psr_ref_m))
+ *   w_k = 0.05 if |e_k| > threshold else 1 (strict, on the raw residual, before W),  r_k = w_k e_k
+ *   J_i row k = (-u_s^T R w_k ratio) - (-u_m^T R w_k ratio),  J_j row k the same with (1 - ratio),  u = normalized(sat_user - P)
+ *   r = W r_raw,  J = W J_raw,  cost = 0.5 |r|^2 (no loss function)
+ * normalized() is Eigen 3.3's: v / |v| when |v|^2 > 0, else v itself (the zero vector for a zero-length line of sight).  Only the
+ * t columns of the (t, delta) keyframe layout are non-zero.  The threshold is the factor's own: the reference sets it per outer
+ * pass from {1e9, 10, 8, 6}.  active = 0: as for the pose factors, the factor makes its pair entry but is not evaluated here. */
+enum { GLIO_DD_PSR_MAX_SAT = 20, GLIO_DD_PSR_MAX_KF = 1 << 22 };
+typedef struct {
+  int32_t i, j, n_sat, master, active, reserved;   /* reserved: 0 */
+  int64_t sat_offset, w_offset;                    /* w_offset = -1: identity */
+  double ratio, threshold, station[3];
+} glio_dd_psr_factor;
+typedef struct { double sat_user[3], sat_ref[3], psr_user, psr_ref; } glio_dd_psr_sat;
+/* Replaces the DD-pseudorange list (n = 0 empties it; glio_batch_clear empties it too).  The whole list is checked first: i != j,
+ * both in [0, GLIO_DD_PSR_MAX_KF), 2 <= n_sat <= GLIO_DD_PSR_MAX_SAT, 0 <= master < n_sat, the satellites inside [0, n_sats), the
+ * weight inside [0, n_w) or w_offset = -1, and R_ecef_local and anchor_ecef given when n > 0; a refused call (GLIO_ERR_ARG) leaves
+ * the previous list in place.  The distinct unordered pairs (a, b), a = min(i, j) < b, form the DD pair table in order of first
+ * appearance.  The list, the satellites and the weights are copied to device buffers allocated here; the context takes them only
+ * once complete, so a call that fails for any reason leaves the previous list in place.  Evaluations allocate nothing for it. */
+int glio_batch_set_dd_psr_factors(glio_ctx* ctx, const glio_dd_psr_factor* f, int64_t n, const glio_dd_psr_sat* sats, int64_t n_sats,
+                                  const double* W, int64_t n_w, const double* R_ecef_local, const double* anchor_ecef);
+/* the DD pair table (a[k] < b[k]), glio_batch_pair_list's conventions: NULL arrays only count */
+int glio_batch_dd_psr_pair_list(glio_ctx* ctx, int64_t capacity, int32_t* a, int32_t* b, int64_t* n_pairs);
+/* The DD blocks alone, for the active factors, in glio_eval_pose_factors' layout: Hdiag[K*36], Hoff[n_dd_pairs*36] (rows for a),
+ * g[K*6], cost (attributed to a); NULL outputs are skipped and without Hdiag, Hoff and g only the cost is formed.  Per pair the
+ * factors are summed in list order, per keyframe the pairs in table order.  With the all-reduce hook set, the K x 28 and
+ * n_dd_pairs x 36 buffers are summed over the ranks.  A list that references a keyframe >= K is GLIO_ERR_ARG. */
+int glio_eval_dd_psr_factors(glio_ctx* ctx, int K, const double* poses, double* Hdiag, double* Hoff, double* g, double* cost);
+/* on != 0: every evaluation inside glio_batch_solve adds the DD blocks of the active factors before the all-reduce.  The
+ * off-diagonal buffer holds the LiDAR pairs, then the pose pairs (glio_batch_use_pose_factors on), then the DD pairs: a sharded run
+ * sums K x 28 and (P + P_pose + P_dd) x 36 doubles, one call per buffer.  The band's half bandwidth covers the DD pairs' span, and
+ * the solve works with no LiDAR pair.  Default off; with the switch off or an empty list glio_batch_solve launches what it launches
+ * without DD factors.  A list that references a keyframe >= K makes glio_batch_solve return GLIO_ERR_ARG.  glio_eval_binary,
+ * glio_eval_binary_edge and glio_eval_pose_factors never add DD blocks. */
+int glio_batch_use_dd_psr_factors(glio_ctx* ctx, int on);
+
 /* ---- seeded device selection of EDGE correspondences.  The reference selects plane matches only; this library applies the same
  * rules and the same sampler (glio_select_random / glio_batch_select_random, k_sel_sample) to edge lists, with the sizes of a
  * glio_select_options passed to these calls, so edge sizes are set independently of plane sizes:
@@ -825,9 +873,9 @@ int glio_batch_get_edge_selection(glio_ctx* ctx, int cur, int oth, int64_t capac
 
 /* ---- batch minimizer (replaces ceres::Solve of optimizeBatchWithLandMark, Estimator.cpp:3275-3284: SUBSPACE_DOGLEG,
  * nonmonotonic steps, max_num_iter iterations; options == NULL selects exactly those).  The normal equations are
- * block-banded (half bandwidth (max|cur-oth|+1)*nt - 1) and stored/factored in band form.  Host factors (IMU chain, DD
- * pseudorange: host C++ by design; the pose factors run on the device through glio_batch_use_pose_factors) accumulate into the
- * same LOWER-BAND storage:
+ * block-banded (half bandwidth (max|cur-oth|+1)*nt - 1) and stored/factored in band form.  Host factors (IMU chain, prior;
+ * the pose factors run on the device through glio_batch_use_pose_factors, the DD pseudorange factors through
+ * glio_batch_use_dd_psr_factors) accumulate into the same LOWER-BAND storage:
  * entry (i,j), i-hb <= j <= i, lives at Hband[i*(hb+1) + (j-i+hb)]. */
 int glio_hf_evaluate_band(void* user, int K, const double* poses, const double* speed_bias, int want_jac, double* Hband, int hb,
                           double* g, double* cost);

@@ -1,0 +1,90 @@
+"""Worker of tests/test_gpu_dist_dd_psr_factors.py: one rank of a keyframe-sharded batch solve with LiDAR plane pairs, pose factors
+and DD pseudorange factors.  Every rank declares the same pairs and passes the same pose and DD lists; a rank uploads the plane
+matches of the pairs whose cur it owns (dist.owner_of) and marks active the pose and DD factors whose lower keyframe it owns
+(dist.pose_factor_active).  Both ranks may share one GPU: the all-reduce hook stages the device buffer through the host and sums it
+with torch.distributed (gloo), as in batch_shard_worker.py.  Writes the solve and one glio_eval_dd_psr_factors result."""
+import ctypes as C
+import json
+import os
+import sys
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+sys.path.insert(0, ROOT)
+
+
+def main():
+    out_path = sys.argv[1]
+    import torch
+    import torch.distributed as dist
+    from glio_b200 import api, dist as gdist, synth
+    from tests import eval_reference as er
+    rank = int(os.environ.get("RANK", 0)); world = int(os.environ.get("WORLD_SIZE", 1))
+    if world > 1:
+        dist.init_process_group("gloo")
+    torch.cuda.set_device(0)
+    cudart = C.CDLL("libcudart.so")
+    K, sr = 30, 3
+    P = synth.dd_psr_problem(K=K, search_range=sr, seed=91)
+    cur, oth = gdist.batch_pairs(K, sr)
+    own = gdist.owner_of(cur, K, world) == rank
+    pf = api.pose_factor_records(P["i"], P["j"], P["kind"], P["dq"], P["dp"], active=gdist.pose_factor_active(P["i"], P["j"], K, world, rank))
+    active = gdist.pose_factor_active(P["dd"]["i"], P["dd"]["j"], K, world, rank)
+    f = api.dd_psr_factor_records(**P["dd"], active=active)
+    sats = api.dd_psr_sat_records(**P["dd_sats"])
+    ctx = api.Context(0)
+    calls, counts = [0], []
+
+    def hook(user, d_buf, count, stream):
+        try:
+            n = int(count)
+            h = np.empty(n, np.float64)
+            s = C.c_void_p(stream)
+            assert cudart.cudaMemcpyAsync(h.ctypes.data_as(C.c_void_p), C.c_void_p(d_buf), C.c_size_t(8 * n), C.c_int(2), s) == 0
+            assert cudart.cudaStreamSynchronize(s) == 0
+            t = torch.from_numpy(h)
+            dist.all_reduce(t)
+            assert cudart.cudaMemcpyAsync(C.c_void_p(d_buf), h.ctypes.data_as(C.c_void_p), C.c_size_t(8 * n), C.c_int(1), s) == 0
+            assert cudart.cudaStreamSynchronize(s) == 0
+            calls[0] += 1; counts.append(n)
+            return 0
+        except Exception:
+            return -1
+    cb = api.ALLREDUCE_FN(hook)
+    if world > 1:
+        ctx.set_allreduce(cb, None)
+    ctx.batch_declare_pairs(cur, oth)
+    n_match = 0
+    for k, (a, b) in enumerate(zip(cur, oth)):
+        if own[k]:
+            m = er.make_pair(np.random.default_rng([91, int(a), int(b)]), P["poses_true"][a], P["poses_true"][b], 30, noise=0.02)
+            ctx.batch_set_pair_matches(int(a), int(b), m["cp"], m["nc"], m["weight"]); n_match += 30
+    ctx.batch_set_pose_factors(pf)
+    ctx.batch_use_pose_factors(True)
+    ctx.batch_set_dd_psr_factors(f, sats, P["R"], P["anchor"])
+    ctx.batch_use_dd_psr_factors(True)
+    e = ctx.eval_dd_psr_factors(P["poses_init"])
+    n_eval_calls = calls[0]
+    hf = api.HostFactorSet(); T = P["poses_true"]; rng = np.random.default_rng(7)
+    sw = np.concatenate([np.full(3, 10.0), np.full(3, 30.0), np.zeros(9)])
+    hf.add_prior(0, T[0, :3], T[0, 3:], None, sw * 3)
+    for i in range(K - 1):
+        dq = synth.quat_mul(synth.quat_conj(T[i, 3:]), T[i + 1, 3:]); dp = synth.quat_to_R(T[i, 3:]).T @ (T[i + 1, :3] - T[i, :3])
+        hf.add_between(i, i + 1, dp + rng.normal(0, 0.005, 3), dq, np.zeros(3), 0.1, sw)
+    r = ctx.batch_solve(P["poses_init"], None, hf, api.batch_solver_options(max_num_iterations=12))
+    s = r["summary"]
+    res = dict(rank=rank, world=world, n_match_own=n_match, n_active=int(active.sum()), n_factors=len(f), n_pairs=len(cur),
+               n_pose_pairs=len(ctx.batch_pose_pair_list()[0]), n_dd_pairs=len(ctx.batch_dd_psr_pair_list()[0]), hook_calls=calls[0],
+               eval_hook_calls=n_eval_calls, hook_counts=sorted(set(counts)),
+               eval=dict(Hdiag=e["Hdiag"].tolist(), Hoff=e["Hoff"].tolist(), g=e["g"].tolist(), cost=e["cost"]),
+               initial_cost=float(s.initial_cost), final_cost=float(s.final_cost), iterations=int(s.num_iterations), poses=r["poses"].tolist())
+    ctx.close()
+    if world > 1:
+        dist.destroy_process_group()
+    with open(out_path + f".rank{rank}.json", "w") as fo:
+        json.dump(res, fo)
+
+
+if __name__ == "__main__":
+    main()
