@@ -659,12 +659,30 @@ def _batch_select(self, cur, oth, keep):
     self._chk(self._lib.glio_batch_select(self._h, C.c_int(cur), C.c_int(oth), _ptr(k), C.c_int64(len(k))))
 
 
-def _batch_pair_list(self):
+def _pair_table(self, pair_list):
+    """The two int32 columns of a pair table read through a glio_*pair_list entry point: the count, then the table."""
     n = C.c_int64(0)
-    self._chk(self._lib.glio_batch_pair_list(self._h, C.c_int64(0), None, None, C.byref(n)))
-    cur = np.zeros(n.value, np.int32); oth = np.zeros(n.value, np.int32)
-    self._chk(self._lib.glio_batch_pair_list(self._h, C.c_int64(n.value), _ptr(cur), _ptr(oth), C.byref(n)))
-    return cur, oth
+    self._chk(pair_list(self._h, C.c_int64(0), None, None, C.byref(n)))
+    a = np.zeros(n.value, np.int32); b = np.zeros(n.value, np.int32)
+    self._chk(pair_list(self._h, C.c_int64(n.value), _ptr(a), _ptr(b), C.byref(n)))
+    return a, b
+
+
+def _eval_blocks(self, eval_fn, pair_list, poses, want_jac):
+    """The blocks of a glio_eval_* entry point, Hoff sized by the pair table of pair_list: Hdiag (K,6,6), Hoff (P,6,6) and g (K,6)
+    (None without want_jac), and the cost."""
+    pb = np.ascontiguousarray(poses, np.float64).reshape(-1, 7); K = len(pb)
+    n = C.c_int64(0)
+    self._chk(pair_list(self._h, C.c_int64(0), None, None, C.byref(n)))
+    P = int(n.value)
+    Hd = np.zeros((K, 6, 6)) if want_jac else None; Ho = np.zeros((P, 6, 6)) if want_jac else None
+    g = np.zeros((K, 6)) if want_jac else None; cost = np.zeros(1)
+    self._chk(eval_fn(self._h, C.c_int(K), _ptr(pb), _ptr(Hd), _ptr(Ho), _ptr(g), _ptr(cost)))
+    return dict(Hdiag=Hd, Hoff=Ho, g=g, cost=float(cost[0]))
+
+
+def _batch_pair_list(self):
+    return _pair_table(self, self._lib.glio_batch_pair_list)
 
 
 def _batch_clear(self):
@@ -672,14 +690,7 @@ def _batch_clear(self):
 
 
 def _eval_binary(self, poses, want_jac=True):
-    pb = np.ascontiguousarray(poses, np.float64).reshape(-1, 7); K = len(pb)
-    n = C.c_int64(0)
-    self._chk(self._lib.glio_batch_pair_list(self._h, C.c_int64(0), None, None, C.byref(n)))
-    P = int(n.value)
-    Hd = np.zeros((K, 6, 6)) if want_jac else None; Ho = np.zeros((P, 6, 6)) if want_jac else None
-    g = np.zeros((K, 6)) if want_jac else None; cost = np.zeros(1)
-    self._chk(self._lib.glio_eval_binary(self._h, C.c_int(K), _ptr(pb), _ptr(Hd), _ptr(Ho), _ptr(g), _ptr(cost)))
-    return dict(Hdiag=Hd, Hoff=Ho, g=g, cost=float(cost[0]))
+    return _eval_blocks(self, self._lib.glio_eval_binary, self._lib.glio_batch_pair_list, poses, want_jac)
 
 
 HOST_FACTORS_BAND_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_int,
@@ -910,14 +921,7 @@ def _batch_set_pair_edges(self, cur, oth, cp, pa, pb, s):
 
 def _eval_binary_edge(self, poses, want_jac=True):
     """glio_eval_binary_edge: the binary edge blocks alone, in eval_binary's layout and pair order."""
-    pb = np.ascontiguousarray(poses, np.float64).reshape(-1, 7); K = len(pb)
-    n = C.c_int64(0)
-    self._chk(self._lib.glio_batch_pair_list(self._h, C.c_int64(0), None, None, C.byref(n)))
-    P = int(n.value)
-    Hd = np.zeros((K, 6, 6)) if want_jac else None; Ho = np.zeros((P, 6, 6)) if want_jac else None
-    g = np.zeros((K, 6)) if want_jac else None; cost = np.zeros(1)
-    self._chk(self._lib.glio_eval_binary_edge(self._h, C.c_int(K), _ptr(pb), _ptr(Hd), _ptr(Ho), _ptr(g), _ptr(cost)))
-    return dict(Hdiag=Hd, Hoff=Ho, g=g, cost=float(cost[0]))
+    return _eval_blocks(self, self._lib.glio_eval_binary_edge, self._lib.glio_batch_pair_list, poses, want_jac)
 
 
 def _batch_use_edges(self, on):
@@ -963,23 +967,12 @@ def _batch_set_pose_factors(self, factors):
 
 def _batch_pose_pair_list(self):
     """The pose-pair table (a, b), a < b, in order of first appearance."""
-    n = C.c_int64(0)
-    self._chk(self._lib.glio_batch_pose_pair_list(self._h, C.c_int64(0), None, None, C.byref(n)))
-    a = np.zeros(n.value, np.int32); b = np.zeros(n.value, np.int32)
-    self._chk(self._lib.glio_batch_pose_pair_list(self._h, C.c_int64(len(a)), _ptr(a), _ptr(b), C.byref(n)))
-    return a, b
+    return _pair_table(self, self._lib.glio_batch_pose_pair_list)
 
 
 def _eval_pose_factors(self, poses, want_jac=True):
     """glio_eval_pose_factors: the pose blocks alone; Hoff in pose-pair order (d2 cost / d x_a d x_b, rows for a)."""
-    pb = np.ascontiguousarray(poses, np.float64).reshape(-1, 7); K = len(pb)
-    n = C.c_int64(0)
-    self._chk(self._lib.glio_batch_pose_pair_list(self._h, C.c_int64(0), None, None, C.byref(n)))
-    P = int(n.value)
-    Hd = np.zeros((K, 6, 6)) if want_jac else None; Ho = np.zeros((P, 6, 6)) if want_jac else None
-    g = np.zeros((K, 6)) if want_jac else None; cost = np.zeros(1)
-    self._chk(self._lib.glio_eval_pose_factors(self._h, C.c_int(K), _ptr(pb), _ptr(Hd), _ptr(Ho), _ptr(g), _ptr(cost)))
-    return dict(Hdiag=Hd, Hoff=Ho, g=g, cost=float(cost[0]))
+    return _eval_blocks(self, self._lib.glio_eval_pose_factors, self._lib.glio_batch_pose_pair_list, poses, want_jac)
 
 
 def _batch_use_pose_factors(self, on):
@@ -1045,23 +1038,12 @@ def _batch_set_dd_psr_factors(self, factors, sats, R_ecef_local, anchor_ecef, W=
 
 def _batch_dd_psr_pair_list(self):
     """The DD pair table (a, b), a < b, in order of first appearance."""
-    n = C.c_int64(0)
-    self._chk(self._lib.glio_batch_dd_psr_pair_list(self._h, C.c_int64(0), None, None, C.byref(n)))
-    a = np.zeros(n.value, np.int32); b = np.zeros(n.value, np.int32)
-    self._chk(self._lib.glio_batch_dd_psr_pair_list(self._h, C.c_int64(len(a)), _ptr(a), _ptr(b), C.byref(n)))
-    return a, b
+    return _pair_table(self, self._lib.glio_batch_dd_psr_pair_list)
 
 
 def _eval_dd_psr_factors(self, poses, want_jac=True):
     """glio_eval_dd_psr_factors: the DD blocks alone; Hoff in DD-pair order (d2 cost / d x_a d x_b, rows for a)."""
-    pb = np.ascontiguousarray(poses, np.float64).reshape(-1, 7); K = len(pb)
-    n = C.c_int64(0)
-    self._chk(self._lib.glio_batch_dd_psr_pair_list(self._h, C.c_int64(0), None, None, C.byref(n)))
-    P = int(n.value)
-    Hd = np.zeros((K, 6, 6)) if want_jac else None; Ho = np.zeros((P, 6, 6)) if want_jac else None
-    g = np.zeros((K, 6)) if want_jac else None; cost = np.zeros(1)
-    self._chk(self._lib.glio_eval_dd_psr_factors(self._h, C.c_int(K), _ptr(pb), _ptr(Hd), _ptr(Ho), _ptr(g), _ptr(cost)))
-    return dict(Hdiag=Hd, Hoff=Ho, g=g, cost=float(cost[0]))
+    return _eval_blocks(self, self._lib.glio_eval_dd_psr_factors, self._lib.glio_batch_dd_psr_pair_list, poses, want_jac)
 
 
 def _batch_use_dd_psr_factors(self, on):

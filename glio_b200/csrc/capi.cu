@@ -70,6 +70,18 @@ struct EdgeList {
   }
 };
 
+// A device pair-factor list of the batch solve (pose factors, DD pseudorange factors): its switch, its pair table, the largest
+// keyframe referenced, and the plan built when the list is set: per-pair starts into the active records (grouped by pair in list
+// order; the records sit beside the list in the context), per-keyframe incidence lists and the pair sums
+struct PairFactorList {
+  bool use = false;                                  // glio_batch_use_*: glio_batch_solve adds the list's blocks
+  std::vector<std::pair<int, int>> pairs; int max_kf = -1;
+  DevBuf<int> d_fstart, d_inc_start; DevBuf<BinIncidence> d_inc; DevBuf<double> d_sums;
+  void clear() { pairs.clear(); max_kf = -1; }
+  // a new list's table and buffers; the switch stays as it was
+  void take(PairFactorList&& o) { const bool u = use; *this = std::move(o); use = u; }
+};
+
 struct Slot {
   PointSet scan;                 // surf scan
   DevBuf<float4> m_cpw, m_nsd;   // compacted matches, scan order
@@ -166,17 +178,11 @@ struct glio_ctx {
   // the pair count or the switch changes; its per-pair sums are added to the plane sums before the one block assembly
   bool batch_use_edges = false, bedge_dirty = true; int bedge_K = -1, bedge_P = -1, n_bedge_items = 0;
   DevBuf<BinEdgeItem> d_bedge_items; DevBuf<int> d_bedge_pstart; DevBuf<double> d_bedge_partials, d_bedge_sums;
-  // pose factors (glio_batch_set_pose_factors, K2p): the pose-pair table, the largest keyframe referenced, and the device plan built
-  // when the list is set: active factors grouped by pair in list order, per-pair starts, per-keyframe incidence lists, pair sums
-  bool batch_use_pose = false;
-  std::vector<std::pair<int, int>> pose_pairs; int pose_max_kf = -1;
-  DevBuf<PoseFactor> d_pose_f; DevBuf<int> d_pose_fstart, d_pose_inc_start; DevBuf<BinIncidence> d_pose_inc; DevBuf<double> d_pose_sums;
-  // DD pseudorange factors (glio_batch_set_dd_psr_factors, K2g): the same plan as the pose factors, plus the list's satellites,
-  // weights and frame constants
-  bool batch_use_dd = false;
-  std::vector<std::pair<int, int>> dd_pairs; int dd_max_kf = -1; DdPsrFrame dd_frame{};
-  DevBuf<DdPsrFactor> d_dd_f; DevBuf<int> d_dd_fstart, d_dd_inc_start; DevBuf<BinIncidence> d_dd_inc; DevBuf<DdPsrSat> d_dd_sats;
-  DevBuf<double> d_dd_w, d_dd_sums;
+  // pose factors (glio_batch_set_pose_factors, K2p): the list and its active records
+  PairFactorList pose; DevBuf<PoseFactor> d_pose_f;
+  // DD pseudorange factors (glio_batch_set_dd_psr_factors, K2g): the list, its active records, and the list's satellites, weights
+  // and frame constants
+  PairFactorList dd; DevBuf<DdPsrFactor> d_dd_f; DevBuf<DdPsrSat> d_dd_sats; DevBuf<double> d_dd_w; DdPsrFrame dd_frame{};
 
   // association workspace
   DevBuf<float4> w_pm, w_pmq, w_nsd;
@@ -1714,8 +1720,7 @@ int glio_batch_clear(glio_ctx* c) {
   return guarded(c, [&] {
     GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
     c->frames.clear(); c->pairs.clear(); c->pair_index.clear(); c->bin_dirty = true; c->bedge_dirty = true;
-    c->pose_pairs.clear(); c->pose_max_kf = -1;
-    c->dd_pairs.clear(); c->dd_max_kf = -1;
+    c->pose.clear(); c->dd.clear();
   });
 }
 
@@ -1784,6 +1789,24 @@ glio_ctx::Pair& find_pair(glio_ctx* c, int cur, int oth) {
   return *c->pairs[it->second];
 }
 
+// the LiDAR pair list as (cur, oth)
+std::vector<std::pair<int, int>> lidar_pairs(const glio_ctx* c) {
+  std::vector<std::pair<int, int>> t;
+  t.reserve(c->pairs.size());
+  for (const auto& p : c->pairs) t.emplace_back(p->cur, p->oth);
+  return t;
+}
+
+// a pair table into the caller's arrays (glio_batch_pair_list, glio_batch_pose_pair_list, glio_batch_dd_psr_pair_list): NULL
+// arrays only count; a capacity below the pair count is GLIO_ERR_ARG with the text err
+void copy_pair_table(const std::vector<std::pair<int, int>>& t, int64_t capacity, int32_t* a, int32_t* b, int64_t* n_pairs, const char* err) {
+  const int64_t n = (int64_t)t.size();
+  if (n_pairs) *n_pairs = n;
+  if (!a && !b) return;
+  GLIO_REQUIRE(capacity >= n, GLIO_ERR_ARG, err);
+  for (int64_t k = 0; k < n; ++k) { if (a) a[k] = t[k].first; if (b) b[k] = t[k].second; }
+}
+
 }  // namespace
 
 extern "C" {
@@ -1838,12 +1861,7 @@ int glio_batch_associate(glio_ctx* c, int cur, const int32_t* oth, int n_oth, in
 
 int glio_batch_pair_list(glio_ctx* c, int64_t capacity, int32_t* cur, int32_t* oth, int64_t* n_pairs) {
   if (!c) return GLIO_ERR_ARG;
-  return guarded(c, [&] {
-    const int64_t n = (int64_t)c->pairs.size();
-    if (n_pairs) *n_pairs = n;
-    GLIO_REQUIRE(capacity >= n || (!cur && !oth), GLIO_ERR_ARG, "capacity smaller than the pair count");
-    for (int64_t i = 0; i < n; ++i) { if (cur) cur[i] = c->pairs[i]->cur; if (oth) oth[i] = c->pairs[i]->oth; }
-  });
+  return guarded(c, [&] { copy_pair_table(lidar_pairs(c), capacity, cur, oth, n_pairs, "capacity smaller than the pair count"); });
 }
 
 int glio_batch_get_matches(glio_ctx* c, int cur, int oth, int64_t capacity, float* cp, float* weight, double* normal_cent, int32_t* src, int64_t* n_out) {
@@ -2273,43 +2291,45 @@ void build_bedge_items(glio_ctx* c, int K) {
   c->bedge_dirty = false; c->bedge_K = K; c->bedge_P = P;
 }
 
-// what a binary evaluation returns: the plane blocks (glio_eval_binary), plane + edge blocks (glio_batch_solve with
-// glio_batch_use_edges on), or the edge blocks alone (glio_eval_binary_edge)
-enum BinBlocks { BIN_PLANES = 0, BIN_PLANES_EDGES = 1, BIN_EDGES = 2 };
+// the LiDAR part of a batch block evaluation: none (glio_eval_pose_factors, glio_eval_dd_psr_factors), the plane blocks
+// (glio_eval_binary), plane + edge blocks (glio_batch_solve with glio_batch_use_edges on), or the edge blocks alone
+// (glio_eval_binary_edge)
+enum BinBlocks { BIN_NONE, BIN_PLANES, BIN_PLANES_EDGES, BIN_EDGES };
 
-// device evaluation of all active binary residuals -> c->h_bin_diag (K x 28), c->h_bin_off (P x 36): everything is queued
-// (kernels, the all-reduce of a sharded run, the copies to pinned host memory); eval_binary_wait makes the result visible.
-// With edges, each pair's sums are S_plane + S_edge before the one block assembly, so the all-reduce is the same as without.
-// add_pose: the pose blocks of K2p are added to the diagonal buffer and stored after the P pair blocks of the off-diagonal one;
-// add_dd: the DD blocks of K2g likewise, after the pose pair blocks
-void eval_binary_launch(glio_ctx* c, int K, const double* poses, bool want_jac, double huber, BinBlocks what = BIN_PLANES, bool add_pose = false,
-                        bool add_dd = false) {
-  build_bin_items(c, K);
-  if (what != BIN_PLANES) build_bedge_items(c, K);
-  const bool add_edges = what == BIN_PLANES_EDGES && c->n_bedge_items > 0;   // no edges: exactly the plane launches
-  const int P = (int)c->pairs.size();
-  const int Pp = add_pose ? (int)c->pose_pairs.size() : 0, Pd = add_dd ? (int)c->dd_pairs.size() : 0, Pt = P + Pp + Pd;
-  if (Pp + Pd > 0) { c->d_bin_off.reserve((size_t)(Pt + 1) * 36); c->h_bin_off.reserve((size_t)(Pt + 1) * 36); }
+// Device evaluation of the batch blocks -> c->h_bin_diag (K x 28), c->h_bin_off: the LiDAR part, then the pose list when add_pose,
+// then the DD list when add_dd.  The first group queued writes the diagonal buffer and the later ones add to it; the off-diagonal
+// blocks of each group follow those of the groups before it.  With edges, each LiDAR pair's sums are S_plane + S_edge before the one
+// block assembly, so the all-reduce is the same as without.  Everything is queued (kernels, the all-reduce of a sharded run, the
+// copies to pinned host memory); a synchronisation of the stream makes the result visible.  Returns the off-diagonal block count.
+// Without a LiDAR part the LiDAR pairs are neither read nor checked against K.
+int eval_blocks_launch(glio_ctx* c, int K, const double* poses, bool want_jac, BinBlocks lidar, bool add_pose, bool add_dd) {
+  if (lidar != BIN_NONE) build_bin_items(c, K);
+  if (lidar == BIN_PLANES_EDGES || lidar == BIN_EDGES) build_bedge_items(c, K);
+  const int P = lidar == BIN_NONE ? 0 : (int)c->pairs.size(), Pp = add_pose ? (int)c->pose.pairs.size() : 0;
+  const int Pd = add_dd ? (int)c->dd.pairs.size() : 0, Pt = P + Pp + Pd;
+  c->d_bin_diag.reserve((size_t)K * GLIO_NACC); c->d_bin_off.reserve((size_t)(Pt + 1) * 36); c->d_bin_poses.reserve((size_t)K * 7);
+  c->h_bin_diag.reserve((size_t)K * GLIO_NACC); c->h_bin_off.reserve((size_t)(Pt + 1) * 36); c->h_bin_poses.reserve((size_t)K * 7);
   memcpy(c->h_bin_poses.p, poses, (size_t)K * 7 * sizeof(double));
   GLIO_CUDA_TRY(cudaMemcpyAsync(c->d_bin_poses.p, c->h_bin_poses.p, (size_t)K * 7 * sizeof(double), cudaMemcpyHostToDevice, c->st));
-  if (what == BIN_EDGES || add_edges)
+  const bool add_edges = lidar == BIN_PLANES_EDGES && c->n_bedge_items > 0;   // no edges: exactly the plane launches
+  if (lidar == BIN_EDGES || add_edges)
     eval_binary_edge_run(c->d_bedge_items.p, c->n_bedge_items, c->d_bedge_pstart.p, P, c->d_bin_poses.p, want_jac, c->d_bedge_partials.p,
                          c->d_bedge_sums.p, c->st, c->lc);
-  if (what == BIN_EDGES)
+  if (lidar == BIN_EDGES)
     bin_assemble_run(c->d_bedge_sums.p, K, P, c->d_kf_inc_start.p, c->d_inc.p, want_jac, c->d_bin_diag.p, c->d_bin_off.p, c->st, c->lc);
-  else
-    eval_binary_run(c->d_bin_items.p, c->n_bin_items, c->d_pair_item_start.p, P, K, c->d_bin_poses.p, c->prm.batch_score, huber, want_jac,
-                    c->d_bin_partials.p, c->d_pair_sums.p, c->d_kf_inc_start.p, c->d_inc.p, c->d_bin_diag.p, c->d_bin_off.p, c->st, c->lc,
-                    add_edges ? c->d_bedge_sums.p : nullptr);
+  else if (lidar != BIN_NONE)
+    eval_binary_run(c->d_bin_items.p, c->n_bin_items, c->d_pair_item_start.p, P, K, c->d_bin_poses.p, c->prm.batch_score,
+                    /*no loss on batch LiDAR factors, Estimator.cpp:2768*/ 0.0, want_jac, c->d_bin_partials.p, c->d_pair_sums.p,
+                    c->d_kf_inc_start.p, c->d_inc.p, c->d_bin_diag.p, c->d_bin_off.p, c->st, c->lc, add_edges ? c->d_bedge_sums.p : nullptr);
   if (add_pose)
-    eval_pose_run(c->d_pose_f.p, c->d_pose_fstart.p, Pp, K, c->pose_max_kf + 1, c->d_pose_inc_start.p, c->d_pose_inc.p, c->d_bin_poses.p,
-                  want_jac, /*add*/ true, c->d_pose_sums.p, c->d_bin_diag.p, c->d_bin_off.p + (size_t)P * 36, c->st, c->lc);
+    eval_pose_run(c->d_pose_f.p, c->pose.d_fstart.p, Pp, K, c->pose.max_kf + 1, c->pose.d_inc_start.p, c->pose.d_inc.p, c->d_bin_poses.p,
+                  want_jac, /*add*/ lidar != BIN_NONE, c->pose.d_sums.p, c->d_bin_diag.p, c->d_bin_off.p + (size_t)P * 36, c->st, c->lc);
   if (add_dd)
-    eval_dd_psr_run(c->d_dd_f.p, c->d_dd_fstart.p, c->d_dd_sats.p, c->d_dd_w.p, c->dd_frame, Pd, K, c->dd_max_kf + 1, c->d_dd_inc_start.p,
-                    c->d_dd_inc.p, c->d_bin_poses.p, want_jac, /*add*/ true, c->d_dd_sums.p, c->d_bin_diag.p,
-                    c->d_bin_off.p + (size_t)(P + Pp) * 36, c->st, c->lc);
+    eval_dd_psr_run(c->d_dd_f.p, c->dd.d_fstart.p, c->d_dd_sats.p, c->d_dd_w.p, c->dd_frame, Pd, K, c->dd.max_kf + 1,
+                    c->dd.d_inc_start.p, c->dd.d_inc.p, c->d_bin_poses.p, want_jac, /*add*/ lidar != BIN_NONE || add_pose, c->dd.d_sums.p,
+                    c->d_bin_diag.p, c->d_bin_off.p + (size_t)(P + Pp) * 36, c->st, c->lc);
   if (c->allreduce) {
-    // keyframe-sharded evaluation: every rank holds the same pair list but only its own pairs carry residuals;
+    // keyframe-sharded evaluation: every rank holds the same pair lists but only its own pairs and factors carry residuals;
     // one sum over ranks of the pose-block buffers per evaluation (SURVEY 8e "pose-block allreduce")
     GLIO_REQUIRE(c->allreduce(c->allreduce_user, c->d_bin_diag.p, (int64_t)K * GLIO_NACC, (void*)c->st) == 0, GLIO_ERR_NCCL, "allreduce hook failed (diag)");
     if (want_jac && Pt > 0)
@@ -2317,24 +2337,29 @@ void eval_binary_launch(glio_ctx* c, int K, const double* poses, bool want_jac, 
   }
   GLIO_CUDA_TRY(cudaMemcpyAsync(c->h_bin_diag.p, c->d_bin_diag.p, (size_t)K * GLIO_NACC * sizeof(double), cudaMemcpyDeviceToHost, c->st));
   if (want_jac && Pt > 0) GLIO_CUDA_TRY(cudaMemcpyAsync(c->h_bin_off.p, c->d_bin_off.p, (size_t)Pt * 36 * sizeof(double), cudaMemcpyDeviceToHost, c->st));
-}
-void eval_binary_wait(glio_ctx* c) { GLIO_CUDA_TRY(cudaStreamSynchronize(c->st)); }
-void eval_binary_blocks(glio_ctx* c, int K, const double* poses, bool want_jac, double huber, BinBlocks what = BIN_PLANES) {
-  eval_binary_launch(c, K, poses, want_jac, huber, what);
-  eval_binary_wait(c);
+  return Pt;
 }
 
-// glio_eval_binary / glio_eval_binary_edge: the blocks as 6x6 / 6 / total cost on the host
-int eval_binary_out(glio_ctx* c, int K, const double* poses, BinBlocks what, double* Hdiag, double* Hoff, double* g, double* cost) {
+// an evaluation that adds a pair-factor list referencing a keyframe >= K is GLIO_ERR_ARG; who names the call
+void require_lists_within(const glio_ctx* c, int K, bool add_pose, bool add_dd, const char* who) {
+  GLIO_REQUIRE(!add_pose || c->pose.max_kf < K, GLIO_ERR_ARG, std::string(who) + ": a pose factor references a keyframe outside [0, K)");
+  GLIO_REQUIRE(!add_dd || c->dd.max_kf < K, GLIO_ERR_ARG, std::string(who) + ": a DD factor references a keyframe outside [0, K)");
+}
+
+// glio_eval_binary, glio_eval_binary_edge, glio_eval_pose_factors, glio_eval_dd_psr_factors: one evaluation, its blocks on the host
+// as 6x6 Hdiag / 6 g / total cost and the off-diagonal blocks
+int eval_blocks_out(glio_ctx* c, const char* who, int K, const double* poses, BinBlocks lidar, bool add_pose, bool add_dd, double* Hdiag,
+                    double* Hoff, double* g, double* cost) {
   if (!c) return GLIO_ERR_ARG;
   return guarded(c, [&] {
     GLIO_REQUIRE(K > 0 && poses, GLIO_ERR_ARG, "bad arguments");
-    const bool want_jac = Hdiag || Hoff || g;
-    eval_binary_blocks(c, K, poses, want_jac, /*no loss on batch LiDAR factors, Estimator.cpp:2768*/ 0.0, what);
+    require_lists_within(c, K, add_pose, add_dd, who);
+    const int n_off = eval_blocks_launch(c, K, poses, Hdiag || Hoff || g, lidar, add_pose, add_dd);
+    GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
     unpack_blocks(c->h_bin_diag.p, K, Hdiag, g, nullptr);
     double ct = 0;
     for (int k = 0; k < K; ++k) ct += c->h_bin_diag.p[(size_t)k * GLIO_NACC + 27];
-    if (Hoff) memcpy(Hoff, c->h_bin_off.p, c->pairs.size() * 36 * sizeof(double));
+    if (Hoff) memcpy(Hoff, c->h_bin_off.p, (size_t)n_off * 36 * sizeof(double));
     if (cost) *cost = ct;
   });
 }
@@ -2377,30 +2402,26 @@ PairPlan plan_factor_pairs(const F* f, int64_t n) {
   return pl;
 }
 
-// the blocks of one device factor list alone (glio_eval_pose_factors, glio_eval_dd_psr_factors): run queues the kernels into the
-// K x 28 / n_pairs x 36 buffers, then the all-reduce of a sharded run, the copy-out and the unpacking
-template <class Run>
-void eval_factor_blocks(glio_ctx* c, int K, const double* poses, int n_pairs, Run run, double* Hdiag, double* Hoff, double* g, double* cost) {
-  const bool want_jac = Hdiag || Hoff || g;
-  c->d_bin_diag.reserve((size_t)K * GLIO_NACC); c->h_bin_diag.reserve((size_t)K * GLIO_NACC);
-  c->d_bin_off.reserve((size_t)(n_pairs + 1) * 36); c->h_bin_off.reserve((size_t)(n_pairs + 1) * 36);
-  c->d_bin_poses.reserve((size_t)K * 7); c->h_bin_poses.reserve((size_t)K * 7);
-  memcpy(c->h_bin_poses.p, poses, (size_t)K * 7 * sizeof(double));
-  GLIO_CUDA_TRY(cudaMemcpyAsync(c->d_bin_poses.p, c->h_bin_poses.p, (size_t)K * 7 * sizeof(double), cudaMemcpyHostToDevice, c->st));
-  run(want_jac);
-  if (c->allreduce) {
-    GLIO_REQUIRE(c->allreduce(c->allreduce_user, c->d_bin_diag.p, (int64_t)K * GLIO_NACC, (void*)c->st) == 0, GLIO_ERR_NCCL, "allreduce hook failed (diag)");
-    if (want_jac && n_pairs > 0)
-      GLIO_REQUIRE(c->allreduce(c->allreduce_user, c->d_bin_off.p, (int64_t)n_pairs * 36, (void*)c->st) == 0, GLIO_ERR_NCCL, "allreduce hook failed (off)");
-  }
-  GLIO_CUDA_TRY(cudaMemcpyAsync(c->h_bin_diag.p, c->d_bin_diag.p, (size_t)K * GLIO_NACC * sizeof(double), cudaMemcpyDeviceToHost, c->st));
-  if (want_jac && n_pairs > 0) GLIO_CUDA_TRY(cudaMemcpyAsync(c->h_bin_off.p, c->d_bin_off.p, (size_t)n_pairs * 36 * sizeof(double), cudaMemcpyDeviceToHost, c->st));
-  GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
-  unpack_blocks(c->h_bin_diag.p, K, Hdiag, g, nullptr);
-  double ct = 0;
-  for (int k = 0; k < K; ++k) ct += c->h_bin_diag.p[(size_t)k * GLIO_NACC + 27];
-  if (Hoff) memcpy(Hoff, c->h_bin_off.p, (size_t)n_pairs * 36 * sizeof(double));
-  if (cost) *cost = ct;
+// A new pair-factor list from n records (glio_batch_set_pose_factors, glio_batch_set_dd_psr_factors), after the checks every
+// record shares (i != j, both in [0, max_kf); ij_err otherwise): its pair plan, and its active records grouped by pair into d_f,
+// queued on the stream into buffers of their own.  The caller queues its own payload, synchronises, and only then hands the
+// buffers to the context, so a failed call leaves the previous list and its buffers as they were.
+template <class F, class Rec>
+PairFactorList upload_pair_factors(glio_ctx* c, const Rec* f, int64_t n, int max_kf, int nacc, const char* ij_err, DevBuf<F>& d_f) {
+  for (int64_t k = 0; k < n; ++k)
+    GLIO_REQUIRE(f[k].i >= 0 && f[k].j >= 0 && f[k].i < max_kf && f[k].j < max_kf && f[k].i != f[k].j, GLIO_ERR_ARG, ij_err);
+  PairPlan pl = plan_factor_pairs(f, n);
+  std::vector<F> grouped(pl.order.size());
+  for (size_t q = 0; q < grouped.size(); ++q) memcpy(&grouped[q], &f[pl.order[q]], sizeof(F));
+  PairFactorList l;
+  d_f.reserve(grouped.size() + 1); l.d_fstart.reserve(pl.fstart.size()); l.d_inc_start.reserve(pl.kstart.size());
+  l.d_inc.reserve(pl.inc.size() + 1); l.d_sums.reserve((pl.pairs.size() + 1) * nacc);
+  if (!grouped.empty()) GLIO_CUDA_TRY(cudaMemcpyAsync(d_f.p, grouped.data(), grouped.size() * sizeof(F), cudaMemcpyHostToDevice, c->st));
+  GLIO_CUDA_TRY(cudaMemcpyAsync(l.d_fstart.p, pl.fstart.data(), pl.fstart.size() * sizeof(int), cudaMemcpyHostToDevice, c->st));
+  GLIO_CUDA_TRY(cudaMemcpyAsync(l.d_inc_start.p, pl.kstart.data(), pl.kstart.size() * sizeof(int), cudaMemcpyHostToDevice, c->st));
+  if (!pl.inc.empty()) GLIO_CUDA_TRY(cudaMemcpyAsync(l.d_inc.p, pl.inc.data(), pl.inc.size() * sizeof(BinIncidence), cudaMemcpyHostToDevice, c->st));
+  l.pairs.swap(pl.pairs); l.max_kf = pl.max_kf;
+  return l;
 }
 
 }  // namespace
@@ -2408,11 +2429,11 @@ void eval_factor_blocks(glio_ctx* c, int K, const double* poses, int n_pairs, Ru
 extern "C" {
 
 int glio_eval_binary(glio_ctx* c, int K, const double* poses, double* Hdiag, double* Hoff, double* g, double* cost) {
-  return eval_binary_out(c, K, poses, BIN_PLANES, Hdiag, Hoff, g, cost);
+  return eval_blocks_out(c, "glio_eval_binary", K, poses, BIN_PLANES, false, false, Hdiag, Hoff, g, cost);
 }
 
 int glio_eval_binary_edge(glio_ctx* c, int K, const double* poses, double* Hdiag, double* Hoff, double* g, double* cost) {
-  return eval_binary_out(c, K, poses, BIN_EDGES, Hdiag, Hoff, g, cost);
+  return eval_blocks_out(c, "glio_eval_binary_edge", K, poses, BIN_EDGES, false, false, Hdiag, Hoff, g, cost);
 }
 
 int glio_batch_use_edges(glio_ctx* c, int on) {
@@ -2431,58 +2452,27 @@ int glio_batch_set_pose_factors(glio_ctx* c, const glio_pose_factor* f, int64_t 
     GLIO_REQUIRE(n >= 0 && (n == 0 || f), GLIO_ERR_ARG, "glio_batch_set_pose_factors: null factor array");
     GLIO_REQUIRE(n < ((int64_t)1 << 31), GLIO_ERR_ARG, "glio_batch_set_pose_factors: too many factors");
     for (int64_t k = 0; k < n; ++k)
-      GLIO_REQUIRE(f[k].i >= 0 && f[k].j >= 0 && f[k].i < GLIO_POSE_MAX_KF && f[k].j < GLIO_POSE_MAX_KF && f[k].i != f[k].j &&
-                   (f[k].kind == GLIO_POSE_RELATIVE || f[k].kind == GLIO_POSE_DELTA_Q),
-                   GLIO_ERR_ARG, "glio_batch_set_pose_factors: need i != j, both in [0, GLIO_POSE_MAX_KF), and a known kind");
-    // pair table in order of first appearance; the active factors grouped by pair, list order inside a pair
-    PairPlan pl = plan_factor_pairs(f, n);
-    const int Pp = (int)pl.pairs.size();
-    const std::vector<int>& fstart = pl.fstart; const std::vector<int>& kstart = pl.kstart; const std::vector<BinIncidence>& flat = pl.inc;
-    std::vector<PoseFactor> grouped(pl.order.size());
-    for (size_t q = 0; q < grouped.size(); ++q) memcpy(&grouped[q], &f[pl.order[q]], sizeof(PoseFactor));
-    // the new plan goes to buffers of its own; the context takes them only when every upload has completed, so a failed call
-    // leaves the previous list and its buffers as they were
-    DevBuf<PoseFactor> d_f; DevBuf<int> d_fstart, d_kstart; DevBuf<BinIncidence> d_inc; DevBuf<double> d_sums;
-    d_f.reserve(grouped.size() + 1); d_fstart.reserve(fstart.size()); d_kstart.reserve(kstart.size());
-    d_inc.reserve(flat.size() + 1); d_sums.reserve((size_t)(Pp + 1) * GLIO_NACC_POSE);
-    if (!grouped.empty()) GLIO_CUDA_TRY(cudaMemcpyAsync(d_f.p, grouped.data(), grouped.size() * sizeof(PoseFactor), cudaMemcpyHostToDevice, c->st));
-    GLIO_CUDA_TRY(cudaMemcpyAsync(d_fstart.p, fstart.data(), fstart.size() * sizeof(int), cudaMemcpyHostToDevice, c->st));
-    GLIO_CUDA_TRY(cudaMemcpyAsync(d_kstart.p, kstart.data(), kstart.size() * sizeof(int), cudaMemcpyHostToDevice, c->st));
-    if (!flat.empty()) GLIO_CUDA_TRY(cudaMemcpyAsync(d_inc.p, flat.data(), flat.size() * sizeof(BinIncidence), cudaMemcpyHostToDevice, c->st));
+      GLIO_REQUIRE(f[k].kind == GLIO_POSE_RELATIVE || f[k].kind == GLIO_POSE_DELTA_Q, GLIO_ERR_ARG, "glio_batch_set_pose_factors: need a known kind");
+    DevBuf<PoseFactor> d_f;
+    PairFactorList l = upload_pair_factors(c, f, n, GLIO_POSE_MAX_KF, GLIO_NACC_POSE,
+                                           "glio_batch_set_pose_factors: need i != j, both in [0, GLIO_POSE_MAX_KF)", d_f);
     GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));   // also: no evaluation still reads the buffers released below
-    c->d_pose_f = std::move(d_f); c->d_pose_fstart = std::move(d_fstart); c->d_pose_inc_start = std::move(d_kstart);
-    c->d_pose_inc = std::move(d_inc); c->d_pose_sums = std::move(d_sums);
-    c->pose_pairs.swap(pl.pairs); c->pose_max_kf = pl.max_kf;
+    c->d_pose_f = std::move(d_f); c->pose.take(std::move(l));
   });
 }
 
 int glio_batch_pose_pair_list(glio_ctx* c, int64_t capacity, int32_t* a, int32_t* b, int64_t* n_pairs) {
   if (!c) return GLIO_ERR_ARG;
-  return guarded(c, [&] {
-    const int64_t P = (int64_t)c->pose_pairs.size();
-    if (n_pairs) *n_pairs = P;
-    if (!a && !b) return;
-    GLIO_REQUIRE(capacity >= P, GLIO_ERR_ARG, "glio_batch_pose_pair_list: capacity too small");
-    for (int64_t k = 0; k < P; ++k) { if (a) a[k] = c->pose_pairs[k].first; if (b) b[k] = c->pose_pairs[k].second; }
-  });
+  return guarded(c, [&] { copy_pair_table(c->pose.pairs, capacity, a, b, n_pairs, "glio_batch_pose_pair_list: capacity too small"); });
 }
 
 int glio_eval_pose_factors(glio_ctx* c, int K, const double* poses, double* Hdiag, double* Hoff, double* g, double* cost) {
-  if (!c) return GLIO_ERR_ARG;
-  return guarded(c, [&] {
-    GLIO_REQUIRE(K > 0 && poses, GLIO_ERR_ARG, "bad arguments");
-    GLIO_REQUIRE(c->pose_max_kf < K, GLIO_ERR_ARG, "glio_eval_pose_factors: a pose factor references a keyframe outside [0, K)");
-    const int Pp = (int)c->pose_pairs.size();
-    eval_factor_blocks(c, K, poses, Pp, [&](bool want_jac) {
-      eval_pose_run(c->d_pose_f.p, c->d_pose_fstart.p, Pp, K, c->pose_max_kf + 1, c->d_pose_inc_start.p, c->d_pose_inc.p, c->d_bin_poses.p,
-                    want_jac, /*add*/ false, c->d_pose_sums.p, c->d_bin_diag.p, c->d_bin_off.p, c->st, c->lc);
-    }, Hdiag, Hoff, g, cost);
-  });
+  return eval_blocks_out(c, "glio_eval_pose_factors", K, poses, BIN_NONE, true, false, Hdiag, Hoff, g, cost);
 }
 
 int glio_batch_use_pose_factors(glio_ctx* c, int on) {
   if (!c) return GLIO_ERR_ARG;
-  c->batch_use_pose = on != 0;
+  c->pose.use = on != 0;
   return GLIO_OK;
 }
 
@@ -2503,8 +2493,6 @@ int glio_batch_set_dd_psr_factors(glio_ctx* c, const glio_dd_psr_factor* f, int6
                  "glio_batch_set_dd_psr_factors: null satellite or weight array");
     for (int64_t k = 0; k < n; ++k) {
       const glio_dd_psr_factor& F = f[k];
-      GLIO_REQUIRE(F.i >= 0 && F.j >= 0 && F.i < GLIO_DD_PSR_MAX_KF && F.j < GLIO_DD_PSR_MAX_KF && F.i != F.j, GLIO_ERR_ARG,
-                   "glio_batch_set_dd_psr_factors: need i != j, both in [0, GLIO_DD_PSR_MAX_KF)");
       GLIO_REQUIRE(F.n_sat >= 2 && F.n_sat <= GLIO_DD_PSR_MAX_SAT && F.master >= 0 && F.master < F.n_sat, GLIO_ERR_ARG,
                    "glio_batch_set_dd_psr_factors: need 2 <= n_sat <= GLIO_DD_PSR_MAX_SAT and 0 <= master < n_sat");
       GLIO_REQUIRE(F.sat_offset >= 0 && F.sat_offset <= n_sats - F.n_sat, GLIO_ERR_ARG, "glio_batch_set_dd_psr_factors: satellites outside [0, n_sats)");
@@ -2512,57 +2500,31 @@ int glio_batch_set_dd_psr_factors(glio_ctx* c, const glio_dd_psr_factor* f, int6
       GLIO_REQUIRE(F.w_offset == -1 || (F.w_offset >= 0 && F.w_offset <= n_w - nw), GLIO_ERR_ARG,
                    "glio_batch_set_dd_psr_factors: weight outside [0, n_w) and not -1");
     }
-    PairPlan pl = plan_factor_pairs(f, n);
-    const int Pd = (int)pl.pairs.size();
-    std::vector<DdPsrFactor> grouped(pl.order.size());
-    for (size_t q = 0; q < grouped.size(); ++q) memcpy(&grouped[q], &f[pl.order[q]], sizeof(DdPsrFactor));
-    DdPsrFrame fr{};
-    if (n > 0) { memcpy(fr.R, R_ecef_local, sizeof(fr.R)); memcpy(fr.anchor, anchor_ecef, sizeof(fr.anchor)); }
-    // the new plan goes to buffers of its own; the context takes them only when every upload has completed
-    DevBuf<DdPsrFactor> d_f; DevBuf<int> d_fstart, d_kstart; DevBuf<BinIncidence> d_inc; DevBuf<DdPsrSat> d_sats; DevBuf<double> d_w, d_sums;
-    d_f.reserve(grouped.size() + 1); d_fstart.reserve(pl.fstart.size()); d_kstart.reserve(pl.kstart.size());
-    d_inc.reserve(pl.inc.size() + 1); d_sats.reserve((size_t)n_sats + 1); d_w.reserve((size_t)n_w + 1);
-    d_sums.reserve((size_t)(Pd + 1) * GLIO_NACC_DD);
-    if (!grouped.empty()) GLIO_CUDA_TRY(cudaMemcpyAsync(d_f.p, grouped.data(), grouped.size() * sizeof(DdPsrFactor), cudaMemcpyHostToDevice, c->st));
-    GLIO_CUDA_TRY(cudaMemcpyAsync(d_fstart.p, pl.fstart.data(), pl.fstart.size() * sizeof(int), cudaMemcpyHostToDevice, c->st));
-    GLIO_CUDA_TRY(cudaMemcpyAsync(d_kstart.p, pl.kstart.data(), pl.kstart.size() * sizeof(int), cudaMemcpyHostToDevice, c->st));
-    if (!pl.inc.empty()) GLIO_CUDA_TRY(cudaMemcpyAsync(d_inc.p, pl.inc.data(), pl.inc.size() * sizeof(BinIncidence), cudaMemcpyHostToDevice, c->st));
+    DevBuf<DdPsrFactor> d_f; DevBuf<DdPsrSat> d_sats; DevBuf<double> d_w;
+    PairFactorList l = upload_pair_factors(c, f, n, GLIO_DD_PSR_MAX_KF, GLIO_NACC_DD,
+                                           "glio_batch_set_dd_psr_factors: need i != j, both in [0, GLIO_DD_PSR_MAX_KF)", d_f);
+    d_sats.reserve((size_t)n_sats + 1); d_w.reserve((size_t)n_w + 1);
     if (n_sats > 0) GLIO_CUDA_TRY(cudaMemcpyAsync(d_sats.p, sats, (size_t)n_sats * sizeof(DdPsrSat), cudaMemcpyHostToDevice, c->st));
     if (n_w > 0) GLIO_CUDA_TRY(cudaMemcpyAsync(d_w.p, W, (size_t)n_w * sizeof(double), cudaMemcpyHostToDevice, c->st));
+    DdPsrFrame fr{};
+    if (n > 0) { memcpy(fr.R, R_ecef_local, sizeof(fr.R)); memcpy(fr.anchor, anchor_ecef, sizeof(fr.anchor)); }
     GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));   // also: no evaluation still reads the buffers released below
-    c->d_dd_f = std::move(d_f); c->d_dd_fstart = std::move(d_fstart); c->d_dd_inc_start = std::move(d_kstart);
-    c->d_dd_inc = std::move(d_inc); c->d_dd_sats = std::move(d_sats); c->d_dd_w = std::move(d_w); c->d_dd_sums = std::move(d_sums);
-    c->dd_pairs.swap(pl.pairs); c->dd_max_kf = pl.max_kf; c->dd_frame = fr;
+    c->d_dd_f = std::move(d_f); c->d_dd_sats = std::move(d_sats); c->d_dd_w = std::move(d_w); c->dd_frame = fr; c->dd.take(std::move(l));
   });
 }
 
 int glio_batch_dd_psr_pair_list(glio_ctx* c, int64_t capacity, int32_t* a, int32_t* b, int64_t* n_pairs) {
   if (!c) return GLIO_ERR_ARG;
-  return guarded(c, [&] {
-    const int64_t P = (int64_t)c->dd_pairs.size();
-    if (n_pairs) *n_pairs = P;
-    if (!a && !b) return;
-    GLIO_REQUIRE(capacity >= P, GLIO_ERR_ARG, "glio_batch_dd_psr_pair_list: capacity too small");
-    for (int64_t k = 0; k < P; ++k) { if (a) a[k] = c->dd_pairs[k].first; if (b) b[k] = c->dd_pairs[k].second; }
-  });
+  return guarded(c, [&] { copy_pair_table(c->dd.pairs, capacity, a, b, n_pairs, "glio_batch_dd_psr_pair_list: capacity too small"); });
 }
 
 int glio_eval_dd_psr_factors(glio_ctx* c, int K, const double* poses, double* Hdiag, double* Hoff, double* g, double* cost) {
-  if (!c) return GLIO_ERR_ARG;
-  return guarded(c, [&] {
-    GLIO_REQUIRE(K > 0 && poses, GLIO_ERR_ARG, "bad arguments");
-    GLIO_REQUIRE(c->dd_max_kf < K, GLIO_ERR_ARG, "glio_eval_dd_psr_factors: a DD factor references a keyframe outside [0, K)");
-    const int Pd = (int)c->dd_pairs.size();
-    eval_factor_blocks(c, K, poses, Pd, [&](bool want_jac) {
-      eval_dd_psr_run(c->d_dd_f.p, c->d_dd_fstart.p, c->d_dd_sats.p, c->d_dd_w.p, c->dd_frame, Pd, K, c->dd_max_kf + 1, c->d_dd_inc_start.p,
-                      c->d_dd_inc.p, c->d_bin_poses.p, want_jac, /*add*/ false, c->d_dd_sums.p, c->d_bin_diag.p, c->d_bin_off.p, c->st, c->lc);
-    }, Hdiag, Hoff, g, cost);
-  });
+  return eval_blocks_out(c, "glio_eval_dd_psr_factors", K, poses, BIN_NONE, false, true, Hdiag, Hoff, g, cost);
 }
 
 int glio_batch_use_dd_psr_factors(glio_ctx* c, int on) {
   if (!c) return GLIO_ERR_ARG;
-  c->batch_use_dd = on != 0;
+  c->dd.use = on != 0;
   return GLIO_OK;
 }
 
@@ -2619,14 +2581,15 @@ int glio_batch_solve(glio_ctx* c, int K, double* poses, double* speed_bias, glio
     const bool sb = speed_bias != nullptr;
     const StateLayout L(K, sb);
     const int nt = L.nt, n = K * nt;
-    const bool add_pose = c->batch_use_pose && !c->pose_pairs.empty();
-    GLIO_REQUIRE(!add_pose || c->pose_max_kf < K, GLIO_ERR_ARG, "glio_batch_solve: a pose factor references a keyframe outside [0, K)");
+    const bool add_pose = c->pose.use && !c->pose.pairs.empty(), add_dd = c->dd.use && !c->dd.pairs.empty();
+    require_lists_within(c, K, add_pose, add_dd, "glio_batch_solve");
+    // the keyframe pair of each off-diagonal block, in the evaluation's order: LiDAR pairs (cur, oth), then pose pairs (a, b), then
+    // DD pairs (a, b)
+    std::vector<std::pair<int, int>> off = lidar_pairs(c);
+    if (add_pose) off.insert(off.end(), c->pose.pairs.begin(), c->pose.pairs.end());
+    if (add_dd) off.insert(off.end(), c->dd.pairs.begin(), c->dd.pairs.end());
     int span = 1;
-    for (auto& p : c->pairs) span = std::max(span, std::abs(p->cur - p->oth));
-    if (add_pose) for (auto& p : c->pose_pairs) span = std::max(span, p.second - p.first);
-    const bool add_dd = c->batch_use_dd && !c->dd_pairs.empty();
-    GLIO_REQUIRE(!add_dd || c->dd_max_kf < K, GLIO_ERR_ARG, "glio_batch_solve: a DD factor references a keyframe outside [0, K)");
-    if (add_dd) for (auto& p : c->dd_pairs) span = std::max(span, p.second - p.first);
+    for (const auto& p : off) span = std::max(span, std::abs(p.first - p.second));
     const int hb = (span + 1) * nt - 1;
     TrustRegionDogleg solver(L.blocks(), solver_options_from(o));
     std::vector<double> x((size_t)K * L.na), pz((size_t)K * 7), sz((size_t)K * 9);
@@ -2635,12 +2598,12 @@ int glio_batch_solve(glio_ctx* c, int K, double* poses, double* speed_bias, glio
       L.unpack(xa, pz.data(), sz.data());
       // the device evaluates the LiDAR pairs (and a sharded run sums them over the ranks) while the host evaluates its own
       // factors into the freshly reset band; the device blocks are added when they have arrived
-      eval_binary_launch(c, K, pz.data(), want_jac, 0.0, c->batch_use_edges ? BIN_PLANES_EDGES : BIN_PLANES, add_pose, add_dd);
+      eval_blocks_launch(c, K, pz.data(), want_jac, c->batch_use_edges ? BIN_PLANES_EDGES : BIN_PLANES, add_pose, add_dd);
       double ct = 0;
       int hrc = 0;
       if (want_jac) { H->reset(n, hb); std::fill(g, g + n, 0.0); }
       if (host_factors) hrc = host_factors(user, K, pz.data(), sb ? sz.data() : nullptr, want_jac ? 1 : 0, want_jac ? H->a.data() : nullptr, want_jac ? H->hb : 0, g, &ct);
-      eval_binary_wait(c);
+      GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
       if (hrc != 0) return false;
       for (int k = 0; k < K; ++k) ct += c->h_bin_diag.p[(size_t)k * GLIO_NACC + 27];
       if (want_jac) {
@@ -2648,11 +2611,8 @@ int glio_batch_solve(glio_ctx* c, int K, double* poses, double* speed_bias, glio
         double* a = H->a.data();
         add_diag_blocks(H, c->h_bin_diag.p, K, nt);
         for (int k = 0; k < K; ++k) for (int p = 0; p < 6; ++p) g[nt * k + p] += c->h_bin_diag.p[(size_t)k * GLIO_NACC + 21 + p];
-        const size_t P = c->pairs.size(), Pp = add_pose ? c->pose_pairs.size() : 0, Pt = P + Pp + (add_dd ? c->dd_pairs.size() : 0);
-        for (size_t pi = 0; pi < Pt; ++pi) {                           // LiDAR pairs (cur, oth), then pose pairs (a, b), then DD pairs (a, b)
-          const std::pair<int, int> ab = pi < P ? std::pair<int, int>(c->pairs[pi]->cur, c->pairs[pi]->oth)
-                                                : pi < P + Pp ? c->pose_pairs[pi - P] : c->dd_pairs[pi - P - Pp];
-          const int kc = ab.first, ko = ab.second;
+        for (size_t pi = 0; pi < off.size(); ++pi) {
+          const int kc = off[pi].first, ko = off[pi].second;
           const double* ob = c->h_bin_off.p + pi * 36;                 // d2 cost / d x_cur[p] d x_oth[q]
           if (kc > ko) {                                               // rows of cur, six contiguous band entries each
             for (int p = 0; p < 6; ++p) { double* row = a + (size_t)(nt * kc + p) * w + (nt * ko - (nt * kc + p) + H->hb); for (int q = 0; q < 6; ++q) row[q] += ob[6 * p + q]; }

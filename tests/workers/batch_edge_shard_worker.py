@@ -1,8 +1,6 @@
 """Worker of tests/test_gpu_dist_batch_edges.py: one rank of a keyframe-sharded batch solve with binary edge factors
 (glio_batch_set_edge_frame, glio_batch_associate_edges_pairs on owned pairs, glio_batch_use_edges, glio_batch_solve).  Both ranks
-may share one GPU: the all-reduce hook is a ctypes callback that stages the device buffer through the host and sums it with
-torch.distributed (gloo), as in batch_shard_worker.py."""
-import ctypes as C
+may share one GPU through tests/gloo_hook.py's all-reduce hook."""
 import json
 import os
 import sys
@@ -18,11 +16,11 @@ def main():
     import torch
     import torch.distributed as dist
     from glio_b200 import api, dist as gdist, synth
+    from tests import gloo_hook
     rank = int(os.environ.get("RANK", 0)); world = int(os.environ.get("WORLD_SIZE", 1))
     if world > 1:
         dist.init_process_group("gloo")
     torch.cuda.set_device(0)
-    cudart = C.CDLL("libcudart.so")
     K, sr = 10, 2
     cur, oth = gdist.batch_pairs(K, sr)
     own = gdist.owner_of(cur, K, world) == rank
@@ -30,24 +28,7 @@ def main():
     B = synth.batch_problem(K=K, Q=3000, seed=78, search_range=sr, rng_range=6.0, frames=need)
     E = synth.batch_edge_problem(K=K, Q=2000, seed=78, search_range=sr, frames=need, rng_range=6.0)
     ctx = api.Context(0)
-    calls = [0]
-
-    def hook(user, d_buf, count, stream):
-        try:
-            n = int(count)
-            h = np.empty(n, np.float64)
-            s = C.c_void_p(stream)
-            assert cudart.cudaMemcpyAsync(h.ctypes.data_as(C.c_void_p), C.c_void_p(d_buf), C.c_size_t(8 * n), C.c_int(2), s) == 0
-            assert cudart.cudaStreamSynchronize(s) == 0
-            t = torch.from_numpy(h)
-            dist.all_reduce(t)
-            assert cudart.cudaMemcpyAsync(C.c_void_p(d_buf), h.ctypes.data_as(C.c_void_p), C.c_size_t(8 * n), C.c_int(1), s) == 0
-            assert cudart.cudaStreamSynchronize(s) == 0
-            calls[0] += 1
-            return 0
-        except Exception:
-            return -1
-    cb = api.ALLREDUCE_FN(hook)
+    cb, calls, _ = gloo_hook.staging_allreduce()
     if world > 1:
         ctx.set_allreduce(cb, None)
     for k in need:

@@ -1,9 +1,6 @@
 """Worker of tests/test_gpu_dist_product.py: one rank of a keyframe-sharded batch solve of the PRODUCT (glio_set_allreduce,
 glio_batch_declare_pairs, glio_batch_associate_pairs on owned pairs, glio_batch_solve).  Both ranks may share one GPU: the
-all-reduce hook handed to the library is a ctypes callback that stages the device buffer through the host and sums it with
-torch.distributed (gloo) - the C-ABI contract of glio_allreduce_fn, with any transport underneath (libglio_nccl.so is the NCCL
-one; two NCCL ranks cannot share a device, so the single-GPU test box uses this one)."""
-import ctypes as C
+all-reduce hook is tests/gloo_hook.py's, which stages the device buffer through the host and sums it with torch.distributed (gloo)."""
 import json
 import os
 import sys
@@ -19,36 +16,18 @@ def main():
     import torch
     import torch.distributed as dist
     from glio_b200 import api, dist as gdist, synth
+    from tests import gloo_hook
     rank = int(os.environ.get("RANK", 0)); world = int(os.environ.get("WORLD_SIZE", 1))
     if world > 1:
         dist.init_process_group("gloo")
     torch.cuda.set_device(0)
-    cudart = C.CDLL("libcudart.so")
     K, Q, sr = 10, 3000, 2
     cur, oth = gdist.batch_pairs(K, sr)
     own = gdist.owner_of(cur, K, world) == rank
     need = gdist.frames_needed(cur, oth, own)
     B = synth.batch_problem(K=K, Q=Q, seed=77, search_range=sr, rng_range=6.0, frames=need)
     ctx = api.Context(0)
-    calls = [0]
-
-    def hook(user, d_buf, count, stream):
-        try:
-            n = int(count)
-            h = np.empty(n, np.float64)
-            # everything on the library's own (non-blocking) stream: a copy on the NULL stream would not be ordered with it
-            s = C.c_void_p(stream)
-            assert cudart.cudaMemcpyAsync(h.ctypes.data_as(C.c_void_p), C.c_void_p(d_buf), C.c_size_t(8 * n), C.c_int(2), s) == 0
-            assert cudart.cudaStreamSynchronize(s) == 0
-            t = torch.from_numpy(h)
-            dist.all_reduce(t)
-            assert cudart.cudaMemcpyAsync(C.c_void_p(d_buf), h.ctypes.data_as(C.c_void_p), C.c_size_t(8 * n), C.c_int(1), s) == 0
-            assert cudart.cudaStreamSynchronize(s) == 0
-            calls[0] += 1
-            return 0
-        except Exception:
-            return -1
-    cb = api.ALLREDUCE_FN(hook)
+    cb, calls, _ = gloo_hook.staging_allreduce()
     if world > 1:
         ctx.set_allreduce(cb, None)
     for k in need:
