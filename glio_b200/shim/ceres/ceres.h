@@ -14,9 +14,10 @@
 // they are uploaded once to a glio_ctx and evaluated by the CUDA kernels, which return 6x6 pose blocks: K2 for the plane
 // factors (LidarPlaneNormFactor, and LidarPlaneNormIncreFactor in a front-end context), K2e for LidarEdgeFactor, K2b for
 // BinaryLidarPlaneNormFactor, K2p for the batch refinement's pose factors (LidarPoseFactorBatchRelativeAutoDiff,
-// delta_q_factor_auto).
-// Every other cost function (IMU, marginalisation prior, GNSS ...) is evaluated on the host through its own
-// Evaluate(), exactly as Ceres would.  Without a glio_ctx attached everything runs on the host (used by CPU tests).
+// delta_q_factor_auto), and K2g for its GNSS double-differenced pseudorange factor dd_psr_factor_20, a SizedCostFunction
+// that describes itself through glio::DeviceCostTraits<Cost>, looked up by the static type AddResidualBlock is given.
+// Every other cost function (IMU, marginalisation prior, the window's GNSS factors ...) is evaluated on the host through its
+// own Evaluate(), exactly as Ceres would.  Without a glio_ctx attached everything runs on the host (used by CPU tests).
 #ifndef GLIO_SHIM_CERES_CERES_H_
 #define GLIO_SHIM_CERES_CERES_H_
 
@@ -30,12 +31,15 @@
 #include <memory>
 #include <set>
 #include <string>
+#include <type_traits>
 #include <utility>
 #include <vector>
 
 #include "../../../include/glio_b200.h"
 #include "../../csrc/solver.h"
 #include "jet.h"
+
+namespace ceres { class CostFunction; }
 
 namespace glio {
 // ---- self-description of device-evaluable LiDAR factors --------------------------------------------------------
@@ -54,6 +58,41 @@ struct FactorDesc {
 // Specialise for the reference's functors (INTEGRATION.md shows the lines for each LiDAR functor):
 //   template <> struct glio::DeviceFactorTraits<LidarPlaneNormFactor> { static bool describe(const LidarPlaneNormFactor&, FactorDesc*); };
 template <class Functor> struct DeviceFactorTraits { static bool describe(const Functor&, FactorDesc*) { return false; } };
+
+// ---- self-description of device-evaluable cost functions that are not AutoDiffCostFunctions ----------------------------
+// dd_psr_factor_20 (dd_psr_factor.hpp) is a SizedCostFunction<19, 3, 3, 1, 3> with its own Evaluate: blocks t_i, t_j, yaw, anchor.
+// Its description is the factor's data; the rows it evaluates are those of K2g (glio_batch_set_dd_psr_factors in glio_b200.h).
+struct DdPsrDesc {
+  int n_sat = 0, master = -1;         // satellites (the rows of GNSS_Raws); master: the reference's mPrn, an index into them
+  double ratio = 0, threshold = 0, station[3] = {0, 0, 0};
+  double sat_user[GLIO_DD_PSR_MAX_SAT][3], sat_ref[GLIO_DD_PSR_MAX_SAT][3];   // ECEF satellite positions: rover, station
+  double psr_user[GLIO_DD_PSR_MAX_SAT], psr_ref[GLIO_DD_PSR_MAX_SAT];         // raw pseudoranges: rover, station
+  double W[(GLIO_DD_PSR_MAX_SAT - 1) * (GLIO_DD_PSR_MAX_SAT - 1)];             // the (n_sat-1) x (n_sat-1) weight, row-major
+  int w_identity = 0;                 // 1: W is exactly the identity (uploaded as w_offset = -1)
+};
+// Specialise for the cost function's class, next to its header (INTEGRATION.md shows the lines for dd_psr_factor_20):
+//   template <> struct glio::DeviceCostTraits<dd_psr_factor_20> {
+//     static bool describe(const dd_psr_factor_20&, DdPsrDesc*);                 // false: the block stays on the host
+//     static void frame(const double* yaw, const double* anchor, double R_ecef_local[9]);   // row-major, the factor's own R
+//   };
+// Problem::AddResidualBlock looks the traits up by the cost function's static type.  The default describes nothing.
+template <class Cost> struct DeviceCostTraits {};
+
+// what AddResidualBlock records for a cost function whose static type has a DeviceCostTraits specialisation
+struct CostDescriber {
+  bool (*describe)(const ceres::CostFunction* cost, DdPsrDesc*);
+  void (*frame)(const double* yaw, const double* anchor, double R_ecef_local[9]);
+};
+namespace detail {
+template <class Cost, class = void> struct HasCostTraits : std::false_type {};
+template <class Cost>
+struct HasCostTraits<Cost, decltype((void)&DeviceCostTraits<Cost>::describe, (void)&DeviceCostTraits<Cost>::frame)> : std::true_type {};
+template <class Cost> const CostDescriber* cost_describer() {
+  static const CostDescriber d{[](const ceres::CostFunction* c, DdPsrDesc* out) { return DeviceCostTraits<Cost>::describe(*static_cast<const Cost*>(c), out); },
+                               &DeviceCostTraits<Cost>::frame};
+  return &d;
+}
+}  // namespace detail
 }  // namespace glio
 
 namespace ceres {
@@ -267,6 +306,7 @@ class Solver {
     int num_device_residual_blocks = 0;     // glio extension: residual blocks evaluated by the CUDA kernels
     int num_device_edge_residual_blocks = 0;   // glio extension: the LidarEdgeFactor blocks among them (K2e)
     int num_device_pose_residual_blocks = 0;   // glio extension: the relative-pose and delta_q blocks among them (K2p)
+    int num_device_dd_psr_residual_blocks = 0;   // glio extension: the dd_psr_factor_20 blocks among them (K2g)
     bool IsSolutionUsable() const { return termination_type == CONVERGENCE || termination_type == NO_CONVERGENCE || termination_type == USER_SUCCESS; }
     std::string BriefReport() const {
       char b[256];
@@ -325,17 +365,22 @@ class Problem {
   bool HasParameterBlock(const double* values) const { return blocks_.count(const_cast<double*>(values)) != 0; }
 
   ResidualBlockId AddResidualBlock(CostFunction* cost, LossFunction* loss, const std::vector<double*>& parameter_blocks) {
-    const std::vector<int32_t>& sizes = cost->parameter_block_sizes();
-    if (sizes.size() != parameter_blocks.size()) { fprintf(stderr, "ceres(glio shim): parameter block count mismatch\n"); return nullptr; }
-    for (size_t i = 0; i < sizes.size(); ++i) AddParameterBlock(parameter_blocks[i], sizes[i], nullptr);
-    std::unique_ptr<Residual> rb(new Residual());
-    rb->cost = cost; rb->loss = loss; rb->params = parameter_blocks;
-    residual_blocks_.push_back(std::move(rb));
-    return residual_blocks_.back().get();
+    return AddResidual(cost, loss, parameter_blocks, nullptr);
   }
   template <typename... Ts>
   ResidualBlockId AddResidualBlock(CostFunction* cost, LossFunction* loss, double* x0, Ts*... xs) {
-    return AddResidualBlock(cost, loss, std::vector<double*>{x0, xs...});
+    return AddResidual(cost, loss, std::vector<double*>{x0, xs...}, nullptr);
+  }
+  // glio extension: a cost function whose static type has a glio::DeviceCostTraits specialisation (dd_psr_factor_20) is
+  // recorded with its describer.  These overloads exist only for such types, so every other call resolves as above; a
+  // described cost function passed as a plain CostFunction* is recorded without one and stays on the host.
+  template <class Cost, typename std::enable_if<glio::detail::HasCostTraits<Cost>::value, int>::type = 0>
+  ResidualBlockId AddResidualBlock(Cost* cost, LossFunction* loss, const std::vector<double*>& parameter_blocks) {
+    return AddResidual(cost, loss, parameter_blocks, glio::detail::cost_describer<Cost>());
+  }
+  template <class Cost, typename... Ts, typename std::enable_if<glio::detail::HasCostTraits<Cost>::value, int>::type = 0>
+  ResidualBlockId AddResidualBlock(Cost* cost, LossFunction* loss, double* x0, Ts*... xs) {
+    return AddResidual(cost, loss, std::vector<double*>{x0, xs...}, glio::detail::cost_describer<Cost>());
   }
 
   int NumParameterBlocks() const { return (int)blocks_.size(); }
@@ -353,7 +398,16 @@ class Problem {
  private:
   friend void Solve(const Solver::Options&, Problem*, Solver::Summary*);
   struct Block { double* values = nullptr; int size = 0; LocalParameterization* param = nullptr; bool constant = false; int order = 0; };
-  struct Residual { CostFunction* cost = nullptr; LossFunction* loss = nullptr; std::vector<double*> params; };
+  struct Residual { CostFunction* cost = nullptr; LossFunction* loss = nullptr; std::vector<double*> params; const glio::CostDescriber* describer = nullptr; };
+  ResidualBlockId AddResidual(CostFunction* cost, LossFunction* loss, const std::vector<double*>& parameter_blocks, const glio::CostDescriber* describer) {
+    const std::vector<int32_t>& sizes = cost->parameter_block_sizes();
+    if (sizes.size() != parameter_blocks.size()) { fprintf(stderr, "ceres(glio shim): parameter block count mismatch\n"); return nullptr; }
+    for (size_t i = 0; i < sizes.size(); ++i) AddParameterBlock(parameter_blocks[i], sizes[i], nullptr);
+    std::unique_ptr<Residual> rb(new Residual());
+    rb->cost = cost; rb->loss = loss; rb->params = parameter_blocks; rb->describer = describer;
+    residual_blocks_.push_back(std::move(rb));
+    return residual_blocks_.back().get();
+  }
   Options options_;
   std::map<double*, Block> blocks_;
   std::vector<double*> order_;

@@ -107,6 +107,13 @@ inline void Solve(const Solver::Options& options, Problem* problem, Solver::Summ
   // pose-factor candidates: routed after the loop, once every keyframe (t, q) pairing of the problem is known
   struct PoseCand { const Problem::Residual* rb; glio::FactorDesc d; };
   std::vector<PoseCand> pose_cands;
+  // DD-pseudorange candidates: routed after the pose factors, on the same keyframe table.  Each candidate's satellites and
+  // weight go into the arrays glio_batch_set_dd_psr_factors takes; those of candidates left on the host stay there unused.
+  struct DdCand { const Problem::Residual* rb; glio_dd_psr_factor f; };
+  std::vector<DdCand> dd_cands;
+  std::vector<glio_dd_psr_sat> dd_sats;
+  std::vector<double> dd_W;
+  std::unique_ptr<glio::DdPsrDesc> dd_desc(new glio::DdPsrDesc());
   for (auto& rbp : problem->residual_blocks_) {
     const Problem::Residual* rb = rbp.get();
     glio::FactorDesc d;
@@ -190,6 +197,35 @@ inline void Solve(const Solver::Options& options, Problem* problem, Solver::Summ
           trans_ok(rb->params[2]) && quat_ok(rb->params[3])) ||
          (d.kind == glio::FACTOR_POSE_DELTA_Q && rb->params.size() == 2 && quat_ok(rb->params[0]) && quat_ok(rb->params[1]))))
       pose_cands.push_back(PoseCand{rb, d});
+    // dd_psr_factor_20 (dd_psr_factor.hpp, added without a loss at Estimator.cpp:1910): K2g computes exactly its residual when the
+    // blocks are (t_i, t_j, yaw, anchor) of sizes (3, 3, 1, 3), both t active plain 3-vectors of different keyframes, yaw and
+    // anchor constant, and the description within K2g's limits.  A candidate stays in host_blocks until the keyframe table takes it.
+    if (!dev && ctx && rb->describer && rb->loss == nullptr && rb->params.size() == 4) {
+      const std::vector<int32_t>& sz = rb->cost->parameter_block_sizes();
+      double* const* b = rb->params.data();
+      const bool shape = sz[0] == 3 && sz[1] == 3 && sz[2] == 1 && sz[3] == 3 && problem->blocks_.at(b[2]).size == 1 &&
+                         problem->blocks_.at(b[3]).size == 3 && trans_ok(b[0]) && trans_ok(b[1]) && b[0] != b[1] &&
+                         !P.index.count(b[2]) && !P.index.count(b[3]);
+      if (shape) *dd_desc = glio::DdPsrDesc();
+      if (shape && rb->describer->describe(rb->cost, dd_desc.get()) && dd_desc->n_sat >= 2 && dd_desc->n_sat <= GLIO_DD_PSR_MAX_SAT &&
+          dd_desc->master >= 0 && dd_desc->master < dd_desc->n_sat) {
+        const glio::DdPsrDesc& dd = *dd_desc;
+        glio_dd_psr_factor f;
+        f.i = f.j = -1; f.n_sat = dd.n_sat; f.master = dd.master; f.active = 1; f.reserved = 0;
+        f.sat_offset = (int64_t)dd_sats.size();
+        f.w_offset = dd.w_identity ? -1 : (int64_t)dd_W.size();
+        f.ratio = dd.ratio; f.threshold = dd.threshold;
+        for (int k = 0; k < 3; ++k) f.station[k] = dd.station[k];
+        for (int s_ = 0; s_ < dd.n_sat; ++s_) {
+          glio_dd_psr_sat sat;
+          for (int k = 0; k < 3; ++k) { sat.sat_user[k] = dd.sat_user[s_][k]; sat.sat_ref[k] = dd.sat_ref[s_][k]; }
+          sat.psr_user = dd.psr_user[s_]; sat.psr_ref = dd.psr_ref[s_];
+          dd_sats.push_back(sat);
+        }
+        if (!dd.w_identity) dd_W.insert(dd_W.end(), dd.W, dd.W + (size_t)(dd.n_sat - 1) * (dd.n_sat - 1));
+        dd_cands.push_back(DdCand{rb, f});
+      }
+    }
     if (!dev) host_blocks.push_back(rb);
   }
   const int W = (int)slots.size();
@@ -200,8 +236,8 @@ inline void Solve(const Solver::Options& options, Problem* problem, Solver::Summ
   // its own without a t (t = NULL: rotation columns only).  A q paired with two t blocks, or a t with two q blocks, has no single
   // keyframe: the pose blocks that touch it stay on the host.  So do blocks whose two sides are one keyframe.
   std::vector<glio_pose_factor> pose_list;
+  std::map<double*, std::set<double*>> ts_of_q, qs_of_t;
   {
-    std::map<double*, std::set<double*>> ts_of_q, qs_of_t;
     auto pairing = [&](double* t, double* q) { ts_of_q[q].insert(t); qs_of_t[t].insert(q); };
     for (const auto& kf : bkfs) pairing(kf.first, kf.second);
     for (const PoseCand& c : pose_cands)
@@ -234,7 +270,49 @@ inline void Solve(const Solver::Options& options, Problem* problem, Solver::Summ
       host_blocks.erase(std::remove_if(host_blocks.begin(), host_blocks.end(), [&](const Problem::Residual* rb) { return routed.count(rb) != 0; }),
                         host_blocks.end());
   }
-  const int KT = (int)bkfs.size(), NP = (int)pose_list.size();   // keyframes of K2b (the first KB) and K2p; routed pose blocks
+
+  // ---- DD pseudorange factors on the same table ----
+  // A t paired with one q by the binary-plane or pose blocks (and that q with no other t) is the keyframe (t, q); a t seen in no
+  // such pairing is a keyframe of its own without a q (q = NULL: translation columns only, an identity quaternion in the pose
+  // array, which K2g does not read).  A t with two q blocks, or whose q has two t blocks, keeps its DD blocks on the host.  K2g
+  // takes one R and anchor per list: only the blocks that share the first candidate's constant yaw and anchor blocks (and frame())
+  // are routed.
+  std::vector<glio_dd_psr_factor> dd_list;
+  double dd_R[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1}, dd_anchor[3] = {0, 0, 0};
+  {
+    auto t_single = [&](double* t) {
+      auto it = qs_of_t.find(t);
+      return it == qs_of_t.end() || (it->second.size() == 1 && ts_of_q.at(*it->second.begin()).size() == 1);
+    };
+    auto kf_of_t = [&](double* t) {
+      auto it = qs_of_t.find(t);
+      auto key = std::make_pair(t, it == qs_of_t.end() ? (double*)nullptr : *it->second.begin());
+      auto kit = bkf_of.find(key);
+      if (kit != bkf_of.end()) return kit->second;
+      const int k = (int)bkfs.size(); bkf_of[key] = k; bkfs.push_back(key); return k;
+    };
+    std::set<const Problem::Residual*> routed;
+    const Problem::Residual* first = nullptr;
+    for (const DdCand& c : dd_cands) {
+      double* const* b = c.rb->params.data();
+      if (first && (b[2] != first->params[2] || b[3] != first->params[3] || c.rb->describer->frame != first->describer->frame)) continue;
+      if (!t_single(b[0]) || !t_single(b[1])) continue;
+      if (!first) {
+        first = c.rb;
+        c.rb->describer->frame(b[2], b[3], dd_R);
+        for (int k = 0; k < 3; ++k) dd_anchor[k] = b[3][k];
+      }
+      glio_dd_psr_factor f = c.f;
+      f.i = kf_of_t(b[0]); f.j = kf_of_t(b[1]);
+      dd_list.push_back(f);
+      routed.insert(c.rb);
+    }
+    if (!routed.empty())
+      host_blocks.erase(std::remove_if(host_blocks.begin(), host_blocks.end(), [&](const Problem::Residual* rb) { return routed.count(rb) != 0; }),
+                        host_blocks.end());
+  }
+  // keyframes of K2b (the first KB), K2p and K2g; routed pose and DD blocks
+  const int KT = (int)bkfs.size(), NP = (int)pose_list.size(), ND = (int)dd_list.size();
   if (PB > 0) {
     if (glio_batch_clear(ctx) != GLIO_OK) { S.termination_type = FAILURE; S.message = std::string("glio_batch_clear: ") + glio_last_error(ctx); return; }
     for (int p = 0; p < PB; ++p) {
@@ -278,6 +356,24 @@ inline void Solve(const Solver::Options& options, Problem* problem, Solver::Summ
     S.num_device_residual_blocks += NP; S.num_device_pose_residual_blocks = NP;
   }
   const int PP = (int)pp_a.size();
+  // DD factors: the context's list is replaced after the clear, pair and pose uploads.  A problem without routed DD blocks makes
+  // no DD call.  glio_eval_binary and glio_eval_pose_factors never add DD blocks, so glio_batch_use_dd_psr_factors does not change
+  // what is computed here.
+  std::vector<int32_t> dp_a, dp_b;                               // the DD pair table (glio_batch_dd_psr_pair_list)
+  if (ND > 0) {
+    int64_t ndp = 0;
+    if (glio_batch_set_dd_psr_factors(ctx, dd_list.data(), ND, dd_sats.data(), (int64_t)dd_sats.size(), dd_W.empty() ? nullptr : dd_W.data(),
+                                      (int64_t)dd_W.size(), dd_R, dd_anchor) != GLIO_OK ||
+        glio_batch_dd_psr_pair_list(ctx, 0, nullptr, nullptr, &ndp) != GLIO_OK) {
+      S.termination_type = FAILURE; S.message = std::string("glio_batch_set_dd_psr_factors: ") + glio_last_error(ctx); return;
+    }
+    dp_a.resize(ndp); dp_b.resize(ndp);
+    if (glio_batch_dd_psr_pair_list(ctx, ndp, dp_a.data(), dp_b.data(), &ndp) != GLIO_OK) {
+      S.termination_type = FAILURE; S.message = std::string("glio_batch_dd_psr_pair_list: ") + glio_last_error(ctx); return;
+    }
+    S.num_device_residual_blocks += ND; S.num_device_dd_psr_residual_blocks = ND;
+  }
+  const int DP = (int)dp_a.size();
 
   // ---- band of J^T J from the block structure ----
   int hb = 0;
@@ -316,6 +412,7 @@ inline void Solve(const Solver::Options& options, Problem* problem, Solver::Summ
   std::vector<double> He(with_edges ? Hd.size() : 0), ge(with_edges ? gd.size() : 0), ce(with_edges ? cd.size() : 0);
   std::vector<double> bposes((size_t)std::max(KT, 1) * 7), bHd((size_t)std::max(KB, 1) * 36), bHo((size_t)std::max(PB, 1) * 36), bg((size_t)std::max(KB, 1) * 6);
   std::vector<double> pHd(NP > 0 ? (size_t)KT * 36 : 0), pHo(NP > 0 ? (size_t)std::max(PP, 1) * 36 : 0), pg(NP > 0 ? (size_t)KT * 6 : 0);
+  std::vector<double> dHd(ND > 0 ? (size_t)KT * 36 : 0), dHo(ND > 0 ? (size_t)std::max(DP, 1) * 36 : 0), dg(ND > 0 ? (size_t)KT * 6 : 0);
   double fixed_cost = 0; bool fixed_done = false;
 
   glio::EvalFn eval = [&](const double* xa, bool want_jac, double* cost, glio::BandMat* H, double* g) -> bool {
@@ -353,9 +450,10 @@ inline void Solve(const Solver::Options& options, Problem* problem, Solver::Summ
       double* u = p < 3 ? bkfs[kf].first : bkfs[kf].second;
       return u ? P.active[P.index[u]].tan_off + p % 3 : -1;
     };
-    if (PB > 0 || NP > 0)
+    if (PB > 0 || NP > 0 || ND > 0)
       for (int k = 0; k < KT; ++k) {
         for (int i = 0; i < 3; ++i) bposes[7 * k + i] = bkfs[k].first ? xa[P.active[P.index[bkfs[k].first]].amb_off + i] : 0.0;
+        if (!bkfs[k].second) { bposes[7 * k + 3] = 1.0; bposes[7 * k + 4] = bposes[7 * k + 5] = bposes[7 * k + 6] = 0.0; continue; }
         const ActiveBlock& aq = P.active[P.index[bkfs[k].second]];
         for (int i = 0; i < 4; ++i) bposes[7 * k + 3 + i] = xa[aq.amb_off + i];
       }
@@ -395,6 +493,26 @@ inline void Solve(const Solver::Options& options, Problem* problem, Solver::Summ
             const int ip = toff(pp_a[pr], p), iq = toff(pp_b[pr], q);
             if (ip < 0 || iq < 0) continue;
             const double v = pHo[36 * pr + 6 * p + q];
+            if (ip >= iq) H->at(ip, iq) += v; else H->at(iq, ip) += v;
+          }
+      }
+    }
+    if (ND > 0) {                            // K2g: Hdiag, g and cost into the band (t columns only), Hoff over the DD pair table
+      double dc = 0;
+      if (glio_eval_dd_psr_factors(ctx, KT, bposes.data(), want_jac ? dHd.data() : nullptr, want_jac ? dHo.data() : nullptr, want_jac ? dg.data() : nullptr, &dc) != GLIO_OK) return false;
+      ct += dc;
+      if (want_jac) {
+        for (int k = 0; k < KT; ++k)
+          for (int p = 0; p < 3; ++p) {
+            const int ip = toff(k, p);
+            if (ip < 0) continue;                 // a rotation-only keyframe of the pose factors
+            g[ip] += dg[6 * k + p];
+            for (int q = 0; q <= p; ++q) H->at(ip, toff(k, q)) += dHd[36 * k + 6 * p + q];
+          }
+        for (int pr = 0; pr < DP; ++pr)                       // block (a, b): row = a tangent, col = b tangent
+          for (int p = 0; p < 3; ++p) for (int q = 0; q < 3; ++q) {
+            const int ip = toff(dp_a[pr], p), iq = toff(dp_b[pr], q);
+            const double v = dHo[36 * pr + 6 * p + q];
             if (ip >= iq) H->at(ip, iq) += v; else H->at(iq, ip) += v;
           }
       }
