@@ -76,7 +76,7 @@ __global__ void __launch_bounds__(128, 6) k_knn_box(SearchArgs a) {
   const float qx = q4.x, qy = q4.y, qz = q4.z;
   Top5 t; top5_init(t);
   const int cx = cell_coord(qx, g.ox, g.inv_cell), cy = cell_coord(qy, g.oy, g.inv_cell), cz = cell_coord(qz, g.oz, g.inv_cell);
-  const float gate_r = sqrtf(a.gate_sq) + 2e-3f;
+  const float gate_r = sqrtf(a.gate_sq) + g.slack;
   const int rmax = (int)ceilf(gate_r * g.inv_cell) + 1;
   const bool far_out = cx < -rmax || cy < -rmax || cz < -rmax || cx >= g.nx + rmax || cy >= g.ny + rmax || cz >= g.nz + rmax;
   float d4f = __int_as_float(0x7f800000);

@@ -102,6 +102,10 @@ struct PinnedBuf {
 struct GridDesc {
   float ox, oy, oz;     // origin (min corner of cell (0,0,0))
   float cell, inv_cell;
+  // margin (metres) the kNN face tests take off a float face distance before they call a face closed: a point that
+  // cell_coord puts beyond a face can lie up to a few float spacings of the grid's coordinates nearer than the face
+  // as computed (grid_build)
+  float slack;
   int nx, ny, nz;
   int64_t npts;
   const int* cell_start;   // [nx*ny*nz + 1]

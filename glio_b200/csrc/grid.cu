@@ -190,6 +190,22 @@ __global__ void __launch_bounds__(256) k_cell_scatter(const float4* __restrict__
   }
 }
 
+// The face tests (box_face_open, axis_gap, nn_face_open) compute a face as ox + (float)k * cell and a point's cell as
+// floor((x - ox) * inv_cell), each rounded in float.  The two roundings can disagree near a face: a point up to a few
+// spacings of the float grid (ulp) nearer than the computed face can be counted beyond it.  The face distances are
+// therefore shrunk by this slack: the 2 mm of old while every face and cell corner of the grid stays below 2^12 m in
+// magnitude, 8 ulp(M) above (M: the largest |ox|, |ox + n*cell| over the axes), which covers the worst disagreement of
+// tests/test_knn_margins.py with room to spare.  Queries add no term: the face distance b = face - q is rounded
+// relative to b, which the 0.999 factor covers.
+static float face_slack(const GridDesc& g) {
+  const float o[3] = {g.ox, g.oy, g.oz};
+  const int n[3] = {g.nx, g.ny, g.nz};
+  float M = 0.f;
+  for (int d = 0; d < 3; ++d) M = std::max(M, std::max(std::fabs(o[d]), std::fabs(o[d] + (float)n[d] * g.cell)));
+  const float ulp = std::nextafter(M, INFINITY) - M;
+  return std::max(2e-3f, 8.f * ulp);
+}
+
 void grid_build(GridBuild& gb, const float* d_xyz, int stride, int64_t n, const double* t, const double* q,
                 float cell_size_hint, float pts_per_cell, cudaStream_t st, LaunchCounter& lc) {
   GLIO_REQUIRE(n > 0 && n < (int64_t)1 << 31, GLIO_ERR_ARG, "grid_build: point count out of range");
@@ -234,6 +250,7 @@ void grid_build(GridBuild& gb, const float* d_xyz, int stride, int64_t n, const 
   g.ny = (int)std::floor((mx[1] - g.oy) / cell) + 2;
   g.nz = (int)std::floor((mx[2] - g.oz) / cell) + 2;
   g.npts = n;
+  g.slack = face_slack(g);
   const int64_t ncell = (int64_t)g.nx * g.ny * g.nz;
   gb.cell_start.reserve((size_t)ncell + 2);
   gb.fill.reserve((size_t)ncell + 2);

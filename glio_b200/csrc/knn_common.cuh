@@ -97,9 +97,9 @@ __device__ __forceinline__ void scan_start_box(const GridDesc& g, float qx, floa
 // the same margins as the face test, strict inequality, so nothing that could enter the top-5 (ties included) is skipped;
 // (2) the bounds of up to eight surviving rows are fetched together (18 independent loads in flight) and parked in the thread's
 // shared-memory column before the rows are scanned: the chain of dependent loads per slab shrinks ~9x.
-__device__ __forceinline__ float axis_gap(float q, float lo, float hi) {
+__device__ __forceinline__ float axis_gap(float q, float lo, float hi, float slack) {
   const float d = fmaxf(lo - q, q - hi);                   // > 0 outside [lo, hi]
-  const float m = d * 0.999f - 2e-3f;
+  const float m = d * 0.999f - slack;
   return m > 0.f ? m : 0.f;
 }
 __device__ __forceinline__ void scan_rows_batched(const GridDesc& g, int x0, int x1, int y0, int y1, int z0, int z1, float qx, float qy, float qz, Top5& t, float& d4f,
@@ -107,7 +107,7 @@ __device__ __forceinline__ void scan_rows_batched(const GridDesc& g, int x0, int
   x0 = max(x0, 0); x1 = min(x1, g.nx - 1); y0 = max(y0, 0); y1 = min(y1, g.ny - 1); z0 = max(z0, 0); z1 = min(z1, g.nz - 1);
   if (x0 > x1 || y0 > y1 || z0 > z1) return;
   const int* __restrict__ cs = g.cell_start;
-  const float gx = axis_gap(qx, g.ox + (float)x0 * g.cell, g.ox + (float)(x1 + 1) * g.cell);
+  const float gx = axis_gap(qx, g.ox + (float)x0 * g.cell, g.ox + (float)(x1 + 1) * g.cell, g.slack);
   const float gx2 = gx * gx;
   const int dx1 = x1 + 1 - x0;
   constexpr int NB = 8;
@@ -118,8 +118,8 @@ __device__ __forceinline__ void scan_rows_batched(const GridDesc& g, int x0, int
     int nb = 0;
 #pragma unroll 1
     while (nb < NB && more) {
-      const float gy = axis_gap(qy, g.oy + (float)y * g.cell, g.oy + (float)(y + 1) * g.cell);
-      const float gz = axis_gap(qz, g.oz + (float)z * g.cell, g.oz + (float)(z + 1) * g.cell);
+      const float gy = axis_gap(qy, g.oy + (float)y * g.cell, g.oy + (float)(y + 1) * g.cell, g.slack);
+      const float gz = axis_gap(qz, g.oz + (float)z * g.cell, g.oz + (float)(z + 1) * g.cell, g.slack);
       if (!(d4f <= gx2 + gy * gy + gz * gz)) { sb[(2 * nb) * 128] = (z * g.ny + y) * g.nx + x0; ++nb; }
       if (++y > y1) { y = y0; if (++z > z1) more = false; }
     }
@@ -147,7 +147,7 @@ __device__ __forceinline__ bool box_face_open(const GridDesc& g, int f, float qx
   const float qa = ax == 0 ? qx : (ax == 1 ? qy : qz), oa = ax == 0 ? g.ox : (ax == 1 ? g.oy : g.oz);
   if (up ? (hi >= n - 1) : (lo <= 0)) return false;                   // nothing beyond this face
   const float b = up ? (oa + (float)(hi + 1) * g.cell) - qa : qa - (oa + (float)lo * g.cell);
-  const float bs = b * 0.999f - 2e-3f;
+  const float bs = b * 0.999f - g.slack;                              // GridDesc::slack
   if (bs >= gate_r) return false;                                     // beyond the gate radius
   if (bs > 0.f && key_dist(t.k4) <= bs * bs) return false;            // the 5th distance is inside this face
   return true;

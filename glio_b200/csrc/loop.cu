@@ -115,7 +115,7 @@ __device__ __forceinline__ bool nn_face_open(const GridDesc& g, int f, float qx,
   const float qa = ax == 0 ? qx : (ax == 1 ? qy : qz), oa = ax == 0 ? g.ox : (ax == 1 ? g.oy : g.oz);
   if (up ? (hi[ax] >= n - 1) : (lo[ax] <= 0)) return false;
   const float b = up ? (oa + (float)(hi[ax] + 1) * g.cell) - qa : qa - (oa + (float)lo[ax] * g.cell);
-  const float bs = b * 0.999f - 2e-3f;
+  const float bs = b * 0.999f - g.slack;
   if (bs >= gate_r) return false;
   if (bs > 0.f && bd <= bs * bs) return false;
   return true;
@@ -498,7 +498,7 @@ void icp_run(IcpWork& w, const float* d_src, int src_stride, int64_t n_src, cons
   lc.begin("k_lc_qscatter", st); k_lc_qscatter<<<nb, 256, 0, st>>>(g, w.src0.p, n, w.qstart.p, w.qcount.p, w.perm.p); lc.end(st);
   GLIO_CUDA_TRY(cudaMemsetAsync(w.flags.p, 0, (size_t)(n + 1) * sizeof(int), st));   // flags[n] = 0: pos[n] = count
   const double max_dist_sqr = o.max_correspondence_distance * o.max_correspondence_distance;
-  const float gate_r = (float)std::sqrt(max_dist_sqr) + 2e-3f;
+  const float gate_r = (float)std::sqrt(max_dist_sqr) + g.slack;
   IcpConvergence cc;
   cc.max_iterations = o.max_iterations;
   cc.translation_threshold = o.transformation_epsilon;              // icp.hpp: setTranslationThreshold (transformation_epsilon_)

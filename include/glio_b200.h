@@ -99,7 +99,12 @@ int glio_get_match_counts(glio_ctx* ctx, int W, int64_t* n_match, int64_t* n_act
 void glio_lidar_pose(const glio_params* prm, const double pose_body[7], double t2[3], double q2[4]);
 
 /* ---- K0: local-map upload + uniform-grid build.
- * Replaces kd_tree_surf_local_map->setInputCloud(surf_local_map_ds)  (Estimator.cpp:2056). */
+ * Replaces kd_tree_surf_local_map->setInputCloud(surf_local_map_ds)  (Estimator.cpp:2056).
+ * Coordinate domain of every grid kNN search (surf / corner association, pair mode, loop-closure ICP): any finite float
+ * coordinates.  The searches stay exact (bit-identical to brute force) at any world offset and grid extent: their face
+ * tests keep a margin of max(2 mm, 8 float spacings of the grid's largest coordinate), 2 mm while the grid stays within
+ * 2^12 m of the origin.  Above that the margin grows with the coordinates (6 cm at 2^16 m, 1 m at 2^20 m), and with it the
+ * cells a query scans; results do not change.  Tested to 2^18 m offsets and 200 km wide grids. */
 int glio_set_map(glio_ctx* ctx, const float* xyz, int64_t M, int stride_floats, int mem);
 /* start the upload of the NEXT map from (pinned) host memory on the copy stream and return; the following glio_set_map with the same
  * pointer / count / stride uses the staged copy.  The poses a map is built from are final when the solve returns, so a caller can
