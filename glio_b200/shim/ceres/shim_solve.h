@@ -97,6 +97,15 @@ inline void Solve(const Solver::Options& options, Problem* problem, Solver::Summ
     return ok;
   };
   auto trans_ok = [&](double* t) { return P.index.count(t) && problem->blocks_.at(t).size == 3 && problem->blocks_.at(t).param == nullptr; };
+  // the plane routes' keyframe (t, q): unlike trans_ok, t may have a local parameterization
+  auto tq_ok = [&](double* t, double* q) { return P.index.count(t) && problem->blocks_.at(t).size == 3 && quat_ok(q); };
+  // the batch keyframe table's index of (t, q), appended if new
+  auto kf_index = [&](double* t, double* q) {
+    auto key = std::make_pair(t, q);
+    auto it = bkf_of.find(key);
+    if (it != bkf_of.end()) return it->second;
+    const int k = (int)bkfs.size(); bkf_of[key] = k; bkfs.push_back(key); return k;
+  };
   auto f32_3 = [](const double* v) { return is_f32(v[0]) && is_f32(v[1]) && is_f32(v[2]); };
   auto add_plane = [](Slot& sl, const glio::FactorDesc& d, double w) {
     for (int k = 0; k < 3; ++k) sl.cp.push_back((float)d.cp[k]);
@@ -122,12 +131,11 @@ inline void Solve(const Solver::Options& options, Problem* problem, Solver::Summ
     if (!described) d.kind = glio::FACTOR_NONE;
     if (described && d.kind == glio::FACTOR_PLANE_UNARY && rb->params.size() == 2) {
       double* t = rb->params[0]; double* q = rb->params[1];
-      const bool blocks_ok = P.index.count(t) && problem->blocks_.at(t).size == 3 && quat_ok(q);
       // unit_score contexts evaluate every match with score = lidar_const (front-end factor): only blocks with exactly that score qualify
       const double w = gp.unit_score ? 1.0 : d.score / gp.lidar_const;
       const bool repr = (gp.unit_score ? d.score == gp.lidar_const : (is_f32(w) && gp.lidar_const * (double)(float)w == d.score)) && f32_3(d.cp) &&
                         f32_3(d.n) && is_f32(d.d);
-      if (loss_ok(rb->loss) && blocks_ok && ext_ok(d.q_lb, d.t_lb) && repr) {
+      if (loss_ok(rb->loss) && tq_ok(t, q) && ext_ok(d.q_lb, d.t_lb) && repr) {
         add_plane(slot_at(t, q), d, w);
         dev = true;
       }
@@ -136,9 +144,8 @@ inline void Solve(const Solver::Options& options, Problem* problem, Solver::Summ
     // as a float, so it has to be one as well
     if (described && d.kind == glio::FACTOR_EDGE_UNARY && rb->params.size() == 2) {
       double* t = rb->params[0]; double* q = rb->params[1];
-      const bool blocks_ok = P.index.count(t) && problem->blocks_.at(t).size == 3 && problem->blocks_.at(t).param == nullptr && quat_ok(q);
       const bool repr = f32_3(d.cp) && f32_3(d.pa) && f32_3(d.pb) && is_f32(d.score);
-      if (loss_ok(rb->loss) && blocks_ok && ext_ok(d.q_lb, d.t_lb) && repr) {
+      if (loss_ok(rb->loss) && trans_ok(t) && quat_ok(q) && ext_ok(d.q_lb, d.t_lb) && repr) {
         Slot& sl = slot_at(t, q);
         for (int k = 0; k < 3; ++k) { sl.ecp.push_back((float)d.cp[k]); sl.epa.push_back((float)d.pa[k]); sl.epb.push_back((float)d.pb[k]); }
         sl.es.push_back(d.score);
@@ -152,9 +159,8 @@ inline void Solve(const Solver::Options& options, Problem* problem, Solver::Summ
       double* q = rb->params[0]; double* t = rb->params[1];
       const double ident_q[4] = {1, 0, 0, 0}, zero_t[3] = {0, 0, 0};
       const bool ctx_ok = gp.unit_score && gp.lidar_const == 1.0 && ext_ok(ident_q, zero_t);
-      const bool blocks_ok = P.index.count(t) && problem->blocks_.at(t).size == 3 && problem->blocks_.at(t).param == nullptr && quat_ok(q);
       const bool repr = f32_3(d.cp) && f32_3(d.n) && is_f32(d.d);
-      if (ctx_ok && loss_ok(rb->loss) && blocks_ok && repr) {
+      if (ctx_ok && loss_ok(rb->loss) && trans_ok(t) && quat_ok(q) && repr) {
         add_plane(slot_at(t, q), d, 1.0);
         dev = true;
       }
@@ -163,20 +169,10 @@ inline void Solve(const Solver::Options& options, Problem* problem, Solver::Summ
     // (Estimator.cpp:2768); grouped by keyframe pair and evaluated by K2b
     if (!dev && ctx && d.kind == glio::FACTOR_PLANE_BINARY && rb->params.size() == 4 && rb->loss == nullptr && gp.batch_score != 0.0) {
       double* tc = rb->params[0]; double* qc = rb->params[1]; double* to = rb->params[2]; double* qo = rb->params[3];
-      auto blk_ok = [&](double* t, double* q) {
-        return P.index.count(t) && P.index.count(q) && problem->blocks_.at(t).size == 3 && problem->blocks_.at(q).size == 4 &&
-               dynamic_cast<QuaternionParameterization*>(problem->blocks_.at(q).param) != nullptr;
-      };
       const double w = d.score / gp.batch_score;
       const bool repr = is_f32(w) && gp.batch_score * (double)(float)w == d.score && is_f32(d.cp[0]) && is_f32(d.cp[1]) && is_f32(d.cp[2]);
-      if (blk_ok(tc, qc) && blk_ok(to, qo) && !(tc == to && qc == qo) && repr) {
-        auto kf_of = [&](double* t, double* q) {
-          auto key = std::make_pair(t, q);
-          auto it = bkf_of.find(key);
-          if (it != bkf_of.end()) return it->second;
-          const int k = (int)bkfs.size(); bkf_of[key] = k; bkfs.push_back(key); return k;
-        };
-        const int kc = kf_of(tc, qc), ko = kf_of(to, qo);
+      if (tq_ok(tc, qc) && tq_ok(to, qo) && !(tc == to && qc == qo) && repr) {
+        const int kc = kf_index(tc, qc), ko = kf_index(to, qo);
         auto pkey = std::make_pair(kc, ko);
         auto pit = bpair_of.find(pkey);
         int pi;
@@ -237,6 +233,7 @@ inline void Solve(const Solver::Options& options, Problem* problem, Solver::Summ
   // keyframe: the pose blocks that touch it stay on the host.  So do blocks whose two sides are one keyframe.
   std::vector<glio_pose_factor> pose_list;
   std::map<double*, std::set<double*>> ts_of_q, qs_of_t;
+  std::set<const Problem::Residual*> routed;                     // pose and DD blocks the keyframe table takes off the host
   {
     auto pairing = [&](double* t, double* q) { ts_of_q[q].insert(t); qs_of_t[t].insert(q); };
     for (const auto& kf : bkfs) pairing(kf.first, kf.second);
@@ -249,12 +246,8 @@ inline void Solve(const Solver::Options& options, Problem* problem, Solver::Summ
     };
     auto kf_of_q = [&](double* q) {
       auto it = ts_of_q.find(q);
-      auto key = std::make_pair(it == ts_of_q.end() ? (double*)nullptr : *it->second.begin(), q);
-      auto kit = bkf_of.find(key);
-      if (kit != bkf_of.end()) return kit->second;
-      const int k = (int)bkfs.size(); bkf_of[key] = k; bkfs.push_back(key); return k;
+      return kf_index(it == ts_of_q.end() ? nullptr : *it->second.begin(), q);
     };
-    std::set<const Problem::Residual*> routed;
     for (const PoseCand& c : pose_cands) {
       const bool rel = c.d.kind == glio::FACTOR_POSE_RELATIVE;
       double* qi = c.rb->params[rel ? 1 : 0]; double* qj = c.rb->params[rel ? 3 : 1];
@@ -266,9 +259,6 @@ inline void Solve(const Solver::Options& options, Problem* problem, Solver::Summ
       pose_list.push_back(f);
       routed.insert(c.rb);
     }
-    if (!routed.empty())
-      host_blocks.erase(std::remove_if(host_blocks.begin(), host_blocks.end(), [&](const Problem::Residual* rb) { return routed.count(rb) != 0; }),
-                        host_blocks.end());
   }
 
   // ---- DD pseudorange factors on the same table ----
@@ -286,12 +276,8 @@ inline void Solve(const Solver::Options& options, Problem* problem, Solver::Summ
     };
     auto kf_of_t = [&](double* t) {
       auto it = qs_of_t.find(t);
-      auto key = std::make_pair(t, it == qs_of_t.end() ? (double*)nullptr : *it->second.begin());
-      auto kit = bkf_of.find(key);
-      if (kit != bkf_of.end()) return kit->second;
-      const int k = (int)bkfs.size(); bkf_of[key] = k; bkfs.push_back(key); return k;
+      return kf_index(t, it == qs_of_t.end() ? nullptr : *it->second.begin());
     };
-    std::set<const Problem::Residual*> routed;
     const Problem::Residual* first = nullptr;
     for (const DdCand& c : dd_cands) {
       double* const* b = c.rb->params.data();
@@ -307,25 +293,37 @@ inline void Solve(const Solver::Options& options, Problem* problem, Solver::Summ
       dd_list.push_back(f);
       routed.insert(c.rb);
     }
-    if (!routed.empty())
-      host_blocks.erase(std::remove_if(host_blocks.begin(), host_blocks.end(), [&](const Problem::Residual* rb) { return routed.count(rb) != 0; }),
-                        host_blocks.end());
   }
+  if (!routed.empty())
+    host_blocks.erase(std::remove_if(host_blocks.begin(), host_blocks.end(), [&](const Problem::Residual* rb) { return routed.count(rb) != 0; }),
+                      host_blocks.end());
   // keyframes of K2b (the first KB), K2p and K2g; routed pose and DD blocks
   const int KT = (int)bkfs.size(), NP = (int)pose_list.size(), ND = (int)dd_list.size();
+  auto fail = [&](const char* call) { S.termination_type = FAILURE; S.message = std::string(call) + ": " + glio_last_error(ctx); };
+  // the batch evaluations of the present kinds, in the order eval adds them (K2b, K2p, K2g): the glio_eval_* call, its keyframe
+  // count, its Hoff pair table (block (a, b): row = a tangent, col = b tangent) and the columns it fills of each keyframe's 6
+  struct BatchEval { decltype(&glio_eval_binary) fn; int K; std::vector<int32_t> a, b; int nc; };
+  std::vector<BatchEval> batch;
+  // a glio_batch_*_pair_list table: its size, then its entries
+  auto fetch_pairs = [&](decltype(&glio_batch_pose_pair_list) list, BatchEval& be) {
+    int64_t np = 0;
+    if (list(ctx, 0, nullptr, nullptr, &np) != GLIO_OK) return false;
+    be.a.resize(np); be.b.resize(np);
+    return list(ctx, np, be.a.data(), be.b.data(), &np) == GLIO_OK;
+  };
   if (PB > 0) {
-    if (glio_batch_clear(ctx) != GLIO_OK) { S.termination_type = FAILURE; S.message = std::string("glio_batch_clear: ") + glio_last_error(ctx); return; }
+    if (glio_batch_clear(ctx) != GLIO_OK) return fail("glio_batch_clear");
+    batch.push_back(BatchEval{glio_eval_binary, KB, {}, {}, 6});
     for (int p = 0; p < PB; ++p) {
-      if (glio_batch_set_pair_matches(ctx, bpairs[p].kc, bpairs[p].ko, bpairs[p].cp.data(), bpairs[p].nc.data(), bpairs[p].w.data(), (int64_t)bpairs[p].w.size()) != GLIO_OK) {
-        S.termination_type = FAILURE; S.message = std::string("glio_batch_set_pair_matches: ") + glio_last_error(ctx); return;
-      }
+      if (glio_batch_set_pair_matches(ctx, bpairs[p].kc, bpairs[p].ko, bpairs[p].cp.data(), bpairs[p].nc.data(), bpairs[p].w.data(), (int64_t)bpairs[p].w.size()) != GLIO_OK)
+        return fail("glio_batch_set_pair_matches");
+      batch.back().a.push_back(bpairs[p].kc); batch.back().b.push_back(bpairs[p].ko);
       S.num_device_residual_blocks += (int)bpairs[p].w.size();
     }
   }
   for (int k = 0; k < W; ++k) {
-    if (glio_set_matches(ctx, k, slots[k].cp.data(), slots[k].nsd.data(), slots[k].w.data(), (int64_t)slots[k].w.size()) != GLIO_OK) {
-      S.termination_type = FAILURE; S.message = std::string("glio_set_matches: ") + glio_last_error(ctx); return;
-    }
+    if (glio_set_matches(ctx, k, slots[k].cp.data(), slots[k].nsd.data(), slots[k].w.data(), (int64_t)slots[k].w.size()) != GLIO_OK)
+      return fail("glio_set_matches");
     S.num_device_residual_blocks += (int)slots[k].w.size();
   }
   // edges: every slot's list is replaced (an empty one where the slot has no edge), so lists and selections that an earlier
@@ -334,46 +332,31 @@ inline void Solve(const Solver::Options& options, Problem* problem, Solver::Summ
   if (with_edges) {
     for (int k = 0; k < W; ++k) {
       const Slot& sl = slots[k];
-      if (glio_set_edges(ctx, k, sl.ecp.data(), sl.epa.data(), sl.epb.data(), sl.es.data(), (int64_t)sl.es.size()) != GLIO_OK) {
-        S.termination_type = FAILURE; S.message = std::string("glio_set_edges: ") + glio_last_error(ctx); return;
-      }
+      if (glio_set_edges(ctx, k, sl.ecp.data(), sl.epa.data(), sl.epb.data(), sl.es.data(), (int64_t)sl.es.size()) != GLIO_OK)
+        return fail("glio_set_edges");
     }
     S.num_device_residual_blocks += n_edge_dev; S.num_device_edge_residual_blocks = n_edge_dev;
   }
   // pose factors: the context's list is replaced after glio_batch_clear (which empties it) and the pair uploads.  A problem
   // without routed pose blocks makes no pose call at all.  glio_eval_binary never adds pose blocks, so glio_batch_use_pose_factors
   // does not change what is computed here.
-  std::vector<int32_t> pp_a, pp_b;                               // the pose-pair table (glio_batch_pose_pair_list)
   if (NP > 0) {
-    int64_t npp = 0;
-    if (glio_batch_set_pose_factors(ctx, pose_list.data(), NP) != GLIO_OK || glio_batch_pose_pair_list(ctx, 0, nullptr, nullptr, &npp) != GLIO_OK) {
-      S.termination_type = FAILURE; S.message = std::string("glio_batch_set_pose_factors: ") + glio_last_error(ctx); return;
-    }
-    pp_a.resize(npp); pp_b.resize(npp);
-    if (glio_batch_pose_pair_list(ctx, npp, pp_a.data(), pp_b.data(), &npp) != GLIO_OK) {
-      S.termination_type = FAILURE; S.message = std::string("glio_batch_pose_pair_list: ") + glio_last_error(ctx); return;
-    }
+    if (glio_batch_set_pose_factors(ctx, pose_list.data(), NP) != GLIO_OK) return fail("glio_batch_set_pose_factors");
+    batch.push_back(BatchEval{glio_eval_pose_factors, KT, {}, {}, 6});
+    if (!fetch_pairs(glio_batch_pose_pair_list, batch.back())) return fail("glio_batch_pose_pair_list");
     S.num_device_residual_blocks += NP; S.num_device_pose_residual_blocks = NP;
   }
-  const int PP = (int)pp_a.size();
   // DD factors: the context's list is replaced after the clear, pair and pose uploads.  A problem without routed DD blocks makes
   // no DD call.  glio_eval_binary and glio_eval_pose_factors never add DD blocks, so glio_batch_use_dd_psr_factors does not change
-  // what is computed here.
-  std::vector<int32_t> dp_a, dp_b;                               // the DD pair table (glio_batch_dd_psr_pair_list)
+  // what is computed here.  K2g fills only the t columns; restricting it to them keeps its pairs off q columns outside the band.
   if (ND > 0) {
-    int64_t ndp = 0;
     if (glio_batch_set_dd_psr_factors(ctx, dd_list.data(), ND, dd_sats.data(), (int64_t)dd_sats.size(), dd_W.empty() ? nullptr : dd_W.data(),
-                                      (int64_t)dd_W.size(), dd_R, dd_anchor) != GLIO_OK ||
-        glio_batch_dd_psr_pair_list(ctx, 0, nullptr, nullptr, &ndp) != GLIO_OK) {
-      S.termination_type = FAILURE; S.message = std::string("glio_batch_set_dd_psr_factors: ") + glio_last_error(ctx); return;
-    }
-    dp_a.resize(ndp); dp_b.resize(ndp);
-    if (glio_batch_dd_psr_pair_list(ctx, ndp, dp_a.data(), dp_b.data(), &ndp) != GLIO_OK) {
-      S.termination_type = FAILURE; S.message = std::string("glio_batch_dd_psr_pair_list: ") + glio_last_error(ctx); return;
-    }
+                                      (int64_t)dd_W.size(), dd_R, dd_anchor) != GLIO_OK)
+      return fail("glio_batch_set_dd_psr_factors");
+    batch.push_back(BatchEval{glio_eval_dd_psr_factors, KT, {}, {}, 3});
+    if (!fetch_pairs(glio_batch_dd_psr_pair_list, batch.back())) return fail("glio_batch_dd_psr_pair_list");
     S.num_device_residual_blocks += ND; S.num_device_dd_psr_residual_blocks = ND;
   }
-  const int DP = (int)dp_a.size();
 
   // ---- band of J^T J from the block structure ----
   int hb = 0;
@@ -410,14 +393,40 @@ inline void Solve(const Solver::Options& options, Problem* problem, Solver::Summ
   for (const ActiveBlock& a : P.active) std::memcpy(&x[a.amb_off], a.user, sizeof(double) * a.size);
   std::vector<double> poses((size_t)std::max(W, 1) * 7), Hd((size_t)std::max(W, 1) * 36), gd((size_t)std::max(W, 1) * 6), cd(std::max(W, 1));
   std::vector<double> He(with_edges ? Hd.size() : 0), ge(with_edges ? gd.size() : 0), ce(with_edges ? cd.size() : 0);
-  std::vector<double> bposes((size_t)std::max(KT, 1) * 7), bHd((size_t)std::max(KB, 1) * 36), bHo((size_t)std::max(PB, 1) * 36), bg((size_t)std::max(KB, 1) * 6);
-  std::vector<double> pHd(NP > 0 ? (size_t)KT * 36 : 0), pHo(NP > 0 ? (size_t)std::max(PP, 1) * 36 : 0), pg(NP > 0 ? (size_t)KT * 6 : 0);
-  std::vector<double> dHd(ND > 0 ? (size_t)KT * 36 : 0), dHo(ND > 0 ? (size_t)std::max(DP, 1) * 36 : 0), dg(ND > 0 ? (size_t)KT * 6 : 0);
+  size_t max_pairs = 1;
+  for (const BatchEval& be : batch) max_pairs = std::max(max_pairs, be.a.size());
+  std::vector<double> bposes((size_t)std::max(KT, 1) * 7), bHd((size_t)std::max(KT, 1) * 36), bHo(max_pairs * 36), bg((size_t)std::max(KT, 1) * 6);
+  // tangent column of each unary slot's and each batch keyframe's 6-vector entries (t, then the rotation's delta); -1 for the
+  // entries of a keyframe without a t (seen only in delta_q blocks) or without a q (seen only in DD blocks)
+  auto cols_of = [&](double* t, double* q, std::vector<int>& col) {
+    for (int p = 0; p < 6; ++p) { double* u = p < 3 ? t : q; col.push_back(u ? P.active[P.index[u]].tan_off + p % 3 : -1); }
+  };
+  std::vector<int> ucol, bcol;
+  for (const Slot& sl : slots) cols_of(sl.t, sl.q, ucol);
+  for (const auto& kf : bkfs) cols_of(kf.first, kf.second, bcol);
   double fixed_cost = 0; bool fixed_done = false;
 
   glio::EvalFn eval = [&](const double* xa, bool want_jac, double* cost, glio::BandMat* H, double* g) -> bool {
     double ct = 0;
     if (want_jac) { H->reset(n, hb); std::fill(g, g + n, 0.0); }
+    // adds K keyframes' Hdiag (K x 36) and g (K x 6), then np Hoff blocks (block i: row = keyframe a[i], col = keyframe b[i]) to
+    // the band's lower triangle, over the first nc of each keyframe's 6 entries; entries without a column are skipped
+    auto scatter = [&](const int* col, int K, int nc, const double* Hk, const double* gk, int np, const int32_t* a, const int32_t* b, const double* Ho) {
+      for (int k = 0; k < K; ++k)
+        for (int p = 0; p < nc; ++p) {
+          const int ip = col[6 * k + p];
+          if (ip < 0) continue;
+          g[ip] += gk[6 * k + p];
+          for (int q = 0; q < nc; ++q) { const int iq = col[6 * k + q]; if (iq >= 0 && ip >= iq) H->at(ip, iq) += Hk[36 * k + 6 * p + q]; }
+        }
+      for (int pr = 0; pr < np; ++pr)
+        for (int p = 0; p < nc; ++p) for (int q = 0; q < nc; ++q) {
+          const int ip = col[6 * a[pr] + p], iq = col[6 * b[pr] + q];
+          if (ip < 0 || iq < 0) continue;
+          const double v = Ho[36 * pr + 6 * p + q];
+          if (ip >= iq) H->at(ip, iq) += v; else H->at(iq, ip) += v;
+        }
+    };
     // device blocks
     if (W > 0) {
       for (int k = 0; k < W; ++k) {
@@ -434,88 +443,21 @@ inline void Solve(const Solver::Options& options, Problem* problem, Solver::Summ
           for (size_t i = 0; i < (size_t)W * 6; ++i) gd[i] += ge[i];
         }
       }
-      for (int k = 0; k < W; ++k) {
-        ct += cd[k];
-        if (!want_jac) continue;
-        const int off[2] = {P.active[P.index[slots[k].t]].tan_off, P.active[P.index[slots[k].q]].tan_off};
-        for (int p = 0; p < 6; ++p) {
-          const int ip = off[p / 3] + p % 3;
-          g[ip] += gd[6 * k + p];
-          for (int q = 0; q < 6; ++q) { const int iq = off[q / 3] + q % 3; if (ip >= iq) H->at(ip, iq) += Hd[36 * k + 6 * p + q]; }
-        }
-      }
+      for (int k = 0; k < W; ++k) ct += cd[k];
+      if (want_jac) scatter(ucol.data(), W, 6, Hd.data(), gd.data(), 0, nullptr, nullptr, nullptr);
     }
-    // batch keyframe k: tangent column of its 6-vector entry p (t then delta); -1 for the t entries of a keyframe without a t
-    auto toff = [&](int kf, int p) {
-      double* u = p < 3 ? bkfs[kf].first : bkfs[kf].second;
-      return u ? P.active[P.index[u]].tan_off + p % 3 : -1;
-    };
-    if (PB > 0 || NP > 0 || ND > 0)
+    if (!batch.empty())
       for (int k = 0; k < KT; ++k) {
         for (int i = 0; i < 3; ++i) bposes[7 * k + i] = bkfs[k].first ? xa[P.active[P.index[bkfs[k].first]].amb_off + i] : 0.0;
         if (!bkfs[k].second) { bposes[7 * k + 3] = 1.0; bposes[7 * k + 4] = bposes[7 * k + 5] = bposes[7 * k + 6] = 0.0; continue; }
         const ActiveBlock& aq = P.active[P.index[bkfs[k].second]];
         for (int i = 0; i < 4; ++i) bposes[7 * k + 3 + i] = xa[aq.amb_off + i];
       }
-    if (PB > 0) {
+    for (const BatchEval& be : batch) {
       double bc = 0;
-      if (glio_eval_binary(ctx, KB, bposes.data(), want_jac ? bHd.data() : nullptr, want_jac ? bHo.data() : nullptr, want_jac ? bg.data() : nullptr, &bc) != GLIO_OK) return false;
+      if (be.fn(ctx, be.K, bposes.data(), want_jac ? bHd.data() : nullptr, want_jac ? bHo.data() : nullptr, want_jac ? bg.data() : nullptr, &bc) != GLIO_OK) return false;
       ct += bc;
-      if (want_jac) {
-        for (int k = 0; k < KB; ++k)
-          for (int p = 0; p < 6; ++p) {
-            const int ip = toff(k, p);
-            g[ip] += bg[6 * k + p];
-            for (int q = 0; q < 6; ++q) { const int iq = toff(k, q); if (ip >= iq) H->at(ip, iq) += bHd[36 * k + 6 * p + q]; }
-          }
-        for (int pr = 0; pr < PB; ++pr)                       // block (cur, oth): row = cur tangent, col = oth tangent; lower triangle holds it once
-          for (int p = 0; p < 6; ++p) for (int q = 0; q < 6; ++q) {
-            const int ip = toff(bpairs[pr].kc, p), iq = toff(bpairs[pr].ko, q);
-            const double v = bHo[36 * pr + 6 * p + q];
-            if (ip >= iq) H->at(ip, iq) += v; else H->at(iq, ip) += v;
-          }
-      }
-    }
-    if (NP > 0) {                            // K2p: Hdiag, g and cost into the band, Hoff over the pose-pair table as the bpairs
-      double pc = 0;
-      if (glio_eval_pose_factors(ctx, KT, bposes.data(), want_jac ? pHd.data() : nullptr, want_jac ? pHo.data() : nullptr, want_jac ? pg.data() : nullptr, &pc) != GLIO_OK) return false;
-      ct += pc;
-      if (want_jac) {
-        for (int k = 0; k < KT; ++k)
-          for (int p = 0; p < 6; ++p) {
-            const int ip = toff(k, p);
-            if (ip < 0) continue;
-            g[ip] += pg[6 * k + p];
-            for (int q = 0; q < 6; ++q) { const int iq = toff(k, q); if (iq >= 0 && ip >= iq) H->at(ip, iq) += pHd[36 * k + 6 * p + q]; }
-          }
-        for (int pr = 0; pr < PP; ++pr)                       // block (a, b): row = a tangent, col = b tangent
-          for (int p = 0; p < 6; ++p) for (int q = 0; q < 6; ++q) {
-            const int ip = toff(pp_a[pr], p), iq = toff(pp_b[pr], q);
-            if (ip < 0 || iq < 0) continue;
-            const double v = pHo[36 * pr + 6 * p + q];
-            if (ip >= iq) H->at(ip, iq) += v; else H->at(iq, ip) += v;
-          }
-      }
-    }
-    if (ND > 0) {                            // K2g: Hdiag, g and cost into the band (t columns only), Hoff over the DD pair table
-      double dc = 0;
-      if (glio_eval_dd_psr_factors(ctx, KT, bposes.data(), want_jac ? dHd.data() : nullptr, want_jac ? dHo.data() : nullptr, want_jac ? dg.data() : nullptr, &dc) != GLIO_OK) return false;
-      ct += dc;
-      if (want_jac) {
-        for (int k = 0; k < KT; ++k)
-          for (int p = 0; p < 3; ++p) {
-            const int ip = toff(k, p);
-            if (ip < 0) continue;                 // a rotation-only keyframe of the pose factors
-            g[ip] += dg[6 * k + p];
-            for (int q = 0; q <= p; ++q) H->at(ip, toff(k, q)) += dHd[36 * k + 6 * p + q];
-          }
-        for (int pr = 0; pr < DP; ++pr)                       // block (a, b): row = a tangent, col = b tangent
-          for (int p = 0; p < 3; ++p) for (int q = 0; q < 3; ++q) {
-            const int ip = toff(dp_a[pr], p), iq = toff(dp_b[pr], q);
-            const double v = dHo[36 * pr + 6 * p + q];
-            if (ip >= iq) H->at(ip, iq) += v; else H->at(iq, ip) += v;
-          }
-      }
+      if (want_jac) scatter(bcol.data(), be.K, be.nc, bHd.data(), bg.data(), (int)be.a.size(), be.a.data(), be.b.data(), bHo.data());
     }
     // host blocks (ResidualBlock::Evaluate, ceres.tgz::internal/ceres/residual_block.cc:70-197)
     std::vector<const double*> pp; std::vector<double*> jj; std::vector<std::vector<double>> Jamb, Jloc; std::vector<double> r;

@@ -15,13 +15,13 @@ sys.path.insert(0, ROOT)
 import numpy as np
 import torch
 from glio_b200 import api, synth
+from tests import shim_common as sc
 from tests import test_shim_dd_psr_routes as td
 
 
 def timed(exe, mode, path, reps, iters, *flags):
-    out = subprocess.check_output([exe, mode, *flags, "--repeat", str(reps + 1), "--max-iter", str(iters), path], text=True)
-    rows = [l.split() for l in out.splitlines() if l.startswith("time ")][1:]          # the first solve warms up
-    ms = [float(r[1]) for r in rows]; its = [int(r[2]) for r in rows]
+    rows = sc.run_driver(exe, mode, [path], *flags, "--repeat", str(reps + 1), "--max-iter", str(iters))[0]["times"][1:]   # the first solve warms up
+    ms = [r[0] for r in rows]; its = [r[1] for r in rows]
     return dict(median_ms=float(np.median(ms)), iterations=sorted(set(its)), median_ms_per_iteration=float(np.median([m / max(i, 1) for m, i in zip(ms, its)])))
 
 
@@ -36,7 +36,7 @@ def main():
     gpu = subprocess.check_output(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"], text=True).strip()
     print("gpu:", gpu, flush=True)
     with tempfile.TemporaryDirectory() as tmp:
-        exe = td.build_driver(tmp)
+        exe = sc.build_driver(tmp, "shim_dd_psr_routes_test")
         out = dict(gpu=gpu, iteration_cap=a.iters, cases={})
         for K in (200, 2000, 3457):
             name = f"level0_k{K}"
@@ -46,8 +46,8 @@ def main():
             dds = td.dd_from_records(f, api.dd_psr_sat_records(s["sat_user"], s["sat_ref"], s["psr_user"], s["psr_ref"]))
             path = os.path.join(tmp, name + ".bin")
             td.write_problem(path, P["poses_init"], pose=P, dds=dds, frames=[(0.3, P["anchor"], 1, 1)], max_iter=a.iters)
-            dev = td.run(exe, "device", [path])[0]
-            host = td.run(exe, "host", [path])[0]
+            dev = sc.run_driver(exe, "device", [path])[0]
+            host = sc.run_driver(exe, "host", [path])[0]
             if dev["device_dd"] != len(dds) or dev["device_blocks"] != dev["blocks"]:
                 sys.exit(f"{name}: {dev['device_blocks']} of {dev['blocks']} blocks ({dev['device_dd']} of {len(dds)} DD) were routed to the device")
             if (dev["n_iters"], dev["termination"]) != (host["n_iters"], host["termination"]):

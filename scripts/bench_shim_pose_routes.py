@@ -14,13 +14,13 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import numpy as np
 import torch
+from tests import shim_common as sc
 from tests import test_shim_pose_routes as tp
 
 
 def timed(exe, mode, path, reps, iters):
-    out = subprocess.check_output([exe, mode, "--repeat", str(reps + 1), "--max-iter", str(iters), path], text=True)
-    rows = [l.split() for l in out.splitlines() if l.startswith("time ")][1:]          # the first solve warms up
-    ms = [float(r[1]) for r in rows]; its = [int(r[2]) for r in rows]
+    rows = sc.run_driver(exe, mode, [path], "--repeat", str(reps + 1), "--max-iter", str(iters))[0]["times"][1:]   # the first solve warms up
+    ms = [r[0] for r in rows]; its = [r[1] for r in rows]
     return dict(median_ms=float(np.median(ms)), iterations=sorted(set(its)), median_ms_per_iteration=float(np.median([m / max(i, 1) for m, i in zip(ms, its)])))
 
 
@@ -35,14 +35,14 @@ def main():
     gpu = subprocess.check_output(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"], text=True).strip()
     print("gpu:", gpu, flush=True)
     with tempfile.TemporaryDirectory() as tmp:
-        exe = tp.build_driver(tmp)
+        exe = sc.build_driver(tmp, "shim_pose_routes_test")
         out = dict(gpu=gpu, iteration_cap=a.iters, cases={})
         for name, level, K in (("level0_k200", 0, 200), ("level0_k2000", 0, 2000), ("level0_k3457", 0, 3457), ("level1_k200", 1, 200)):
             c = tp.level0(K) if level == 0 else tp.level1(K)
             path = os.path.join(tmp, name + ".bin")
             tp.write_case(path, c)
             n_pose = len(c["pose"])
-            r = tp.run(exe, "device", [path], "--max-iter", "1")[0]
+            r = sc.run_driver(exe, "device", [path], "--max-iter", "1")[0]
             if r["device_pose"] != n_pose:
                 sys.exit(f"{name}: {r['device_pose']} of {n_pose} pose blocks were routed to the device")
             info = dict(pose_blocks=n_pose, binary_blocks=len(c["kw"].get("binary", ())))

@@ -19,6 +19,7 @@ import torch
 from glio_b200 import synth
 from oracle import pyoracle as oracle
 from tests import eval_reference as er
+from tests import shim_common as sc
 from tests import test_shim_routes as tr
 
 
@@ -56,9 +57,8 @@ def window_problem(path, n_plane, n_edge, W=20, seed=11):
 
 
 def timed(exe, mode, path, reps):
-    out = subprocess.check_output([exe, mode, "--repeat", str(reps + 1), path], text=True)
-    rows = [l.split() for l in out.splitlines() if l.startswith("time ")][1:]          # the first solve warms up
-    return dict(median_ms=float(np.median([float(r[1]) for r in rows])), iterations=sorted({int(r[2]) for r in rows}))
+    rows = sc.run_driver(exe, mode, [path], "--repeat", str(reps + 1))[0]["times"][1:]          # the first solve warms up
+    return dict(median_ms=float(np.median([r[0] for r in rows])), iterations=sorted({r[1] for r in rows}))
 
 
 def main():
@@ -72,7 +72,7 @@ def main():
     print("gpu:", gpu, flush=True)
     oracle.build()
     with tempfile.TemporaryDirectory() as tmp:
-        exe = tr.build_driver(tmp)
+        exe = sc.build_driver(tmp, "shim_routes_test")
         out = dict(gpu=gpu, cases={})
         cases = [("front_end_incre", None, 0.015), ("front_end_incre_no_time_limit", None, 1e9), ("window_w20_100p_100e", (100, 100), None),
                  ("window_w20_10000p_8000e", (10_000, 8_000), None)]
@@ -86,7 +86,7 @@ def main():
                 window_problem(path, *shape)
                 info["blocks_per_keyframe"] = dict(plane=shape[0], edge=shape[1])
                 n_lidar = 20 * (shape[0] + shape[1])
-            routed = tr.run(exe, "device", [path])[0]["device_blocks"]
+            routed = sc.run_driver(exe, "device", [path])[0]["device_blocks"]
             if routed != n_lidar:
                 sys.exit(f"{name}: {routed} of {n_lidar} LiDAR blocks were routed to the device")
             host_reps = a.host_reps_large if shape is not None and shape[0] >= 1000 else a.reps

@@ -30,6 +30,7 @@
 #include <vector>
 
 #include "ceres/ceres.h"
+#include "shim_driver.h"
 
 // ---- the parts of Eigen, nlosExclusion and gnss_comm the factor and its trait use ----------------------------------------------
 struct Quaterniond {
@@ -307,10 +308,6 @@ template <int N> struct PriorN {
   template <typename T> bool operator()(const T* x, T* r) const { for (int k = 0; k < N; ++k) r[k] = T(10.0) * (x[k] - T(x0[k])); return true; }
 };
 
-template <class T> static void rd(FILE* f, T* p, size_t n) {
-  if (fread(p, sizeof(T), n, f) != n) { fprintf(stderr, "shim_dd_psr_routes_test: truncated problem file\n"); exit(2); }
-}
-
 // one problem file (written by tests/test_shim_dd_psr_routes.py: write_problem)
 struct Spec {
   int32_t K = 0;
@@ -486,11 +483,6 @@ static Result solve(const Spec& s, glio_ctx* ctx, Mode mode = SOLVE, int max_ite
   return R;
 }
 
-static int64_t launches(glio_ctx* ctx, std::initializer_list<const char*> names) {
-  int64_t n = 0;
-  for (const char* k : names) { int64_t c = 0; glio_profile_get(ctx, k, nullptr, &c); n += c; }
-  return n;
-}
 static int64_t dd_launches(glio_ctx* ctx) { return launches(ctx, {"k_psr_pair_sums", "k_psr_pair_sums_cost", "k_psr_assemble"}); }
 static int64_t pose_launches(glio_ctx* ctx) { return launches(ctx, {"k_pose_pair_sums", "k_pose_pair_sums_cost", "k_pose_assemble"}); }
 
@@ -517,8 +509,7 @@ int main(int argc, char** argv) {
   glio_ctx* ctx = nullptr;
   if (device) {
     glio_params prm; glio_default_params(&prm);
-    if (glio_create(0, &prm, &ctx) != GLIO_OK) { fprintf(stderr, "glio_create: %s\n", glio_last_error(nullptr)); return 3; }
-    if (!repeat && glio_profile_enable(ctx, 1) != GLIO_OK) return 3;   // launch counts; timed runs leave the profiler off
+    ctx = create_context(prm, !repeat);
     if (preload > 0) {
       // factors between keyframes 1 .. 9 whose satellites sit 1 km from a far-off anchor: any of them evaluated would add cost
       std::vector<glio_dd_psr_factor> f(preload);
@@ -560,12 +551,11 @@ int main(int argc, char** argv) {
       continue;
     }
     g_gate_margin = std::numeric_limits<double>::infinity();
-    const int64_t d0 = ctx ? dd_launches(ctx) : 0, p0 = ctx ? pose_launches(ctx) : 0;
+    const int64_t d0 = dd_launches(ctx), p0 = pose_launches(ctx);
     const Result R = solve(s, ctx, SOLVE, max_iter);
-    const int64_t d1 = ctx ? dd_launches(ctx) : 0, p1 = ctx ? pose_launches(ctx) : 0;
+    const int64_t d1 = dd_launches(ctx), p1 = pose_launches(ctx);
     const ceres::Solver::Summary& S = R.summary;
-    printf("termination %d\n", (int)S.termination_type);
-    printf("iters %d\n", (int)S.iterations.size());
+    print_solve_head(S);
     printf("blocks %d\n", S.num_residual_blocks);
     printf("device_blocks %d\n", S.num_device_residual_blocks);
     printf("device_pose %d\n", S.num_device_pose_residual_blocks);
@@ -573,10 +563,7 @@ int main(int argc, char** argv) {
     printf("dd_launches %lld\n", (long long)(d1 - d0));
     printf("pose_launches %lld\n", (long long)(p1 - p0));
     printf("gate_margin %.17g\n", g_gate_margin);
-    printf("cost %.17g %.17g\n", S.initial_cost, S.final_cost);
-    for (auto& it : S.iterations) printf("it %d %d %.17g %.17g\n", it.iteration, (int)it.step_is_successful, it.cost, it.trust_region_radius);
-    for (int k = 0; k < s.K; ++k)
-      printf("pose %d %.17g %.17g %.17g %.17g %.17g %.17g %.17g\n", k, R.t[3 * k], R.t[3 * k + 1], R.t[3 * k + 2], R.q[4 * k], R.q[4 * k + 1], R.q[4 * k + 2], R.q[4 * k + 3]);
+    print_solve_tail(S, s.K, R.t, R.q, nullptr);
   }
   if (ctx) glio_destroy(ctx);
   return 0;

@@ -28,6 +28,7 @@
 
 #include "ceres/ceres.h"
 #include "ceres/rotation.h"
+#include "shim_driver.h"
 
 // the parts of Eigen::Quaterniond / Eigen::Vector3d the factors and their traits use
 struct Quaterniond {
@@ -211,10 +212,6 @@ struct DDF {
   }
 };
 
-template <class T> static void rd(FILE* f, T* p, size_t n) {
-  if (fread(p, sizeof(T), n, f) != n) { fprintf(stderr, "shim_pose_routes_test: truncated problem file\n"); exit(2); }
-}
-
 // one problem file (written by tests/test_shim_pose_routes.py: write_problem)
 struct Spec {
   int32_t K = 0, n_rcv = 0, epoch = 0;
@@ -361,11 +358,7 @@ static Result solve(const Spec& s, glio_ctx* ctx, Mode mode = SOLVE, int max_ite
   return R;
 }
 
-static int64_t pose_launches(glio_ctx* ctx) {
-  int64_t n = 0;
-  for (const char* k : {"k_pose_pair_sums", "k_pose_pair_sums_cost", "k_pose_assemble"}) { int64_t c = 0; glio_profile_get(ctx, k, nullptr, &c); n += c; }
-  return n;
-}
+static int64_t pose_launches(glio_ctx* ctx) { return launches(ctx, {"k_pose_pair_sums", "k_pose_pair_sums_cost", "k_pose_assemble"}); }
 
 int main(int argc, char** argv) {
   if (argc < 3) { fprintf(stderr, "usage: shim_pose_routes_test host|device|evaluate|describe [--repeat R] [--max-iter M] [--use-pose] [--preload-pose N] problem.bin...\n"); return 2; }
@@ -385,8 +378,7 @@ int main(int argc, char** argv) {
   glio_ctx* ctx = nullptr;
   if (device) {
     glio_params prm; glio_default_params(&prm);
-    if (glio_create(0, &prm, &ctx) != GLIO_OK) { fprintf(stderr, "glio_create: %s\n", glio_last_error(nullptr)); return 3; }
-    if (!repeat && glio_profile_enable(ctx, 1) != GLIO_OK) return 3;   // launch counts; timed runs leave the profiler off
+    ctx = create_context(prm, !repeat);
     if (preload > 0) {
       // relative factors between keyframes 1 .. 9 with a large measured offset: any of them evaluated would add cost
       std::vector<glio_pose_factor> f(preload);
@@ -416,21 +408,15 @@ int main(int argc, char** argv) {
       }
       continue;
     }
-    const int64_t l0 = ctx ? pose_launches(ctx) : 0;
+    const int64_t l0 = pose_launches(ctx);
     const Result R = solve(s, ctx, SOLVE, max_iter);
-    const int64_t l1 = ctx ? pose_launches(ctx) : 0;
+    const int64_t l1 = pose_launches(ctx);
     const ceres::Solver::Summary& S = R.summary;
-    printf("termination %d\n", (int)S.termination_type);
-    printf("iters %d\n", (int)S.iterations.size());
+    print_solve_head(S);
     printf("device_blocks %d\n", S.num_device_residual_blocks);
     printf("device_pose %d\n", S.num_device_pose_residual_blocks);
     printf("pose_launches %lld\n", (long long)(l1 - l0));
-    printf("cost %.17g %.17g\n", S.initial_cost, S.final_cost);
-    for (auto& it : S.iterations) printf("it %d %d %.17g %.17g\n", it.iteration, (int)it.step_is_successful, it.cost, it.trust_region_radius);
-    for (int k = 0; k < s.K; ++k) {
-      printf("pose %d %.17g %.17g %.17g %.17g %.17g %.17g %.17g\n", k, R.t[3 * k], R.t[3 * k + 1], R.t[3 * k + 2], R.q[4 * k], R.q[4 * k + 1], R.q[4 * k + 2], R.q[4 * k + 3]);
-      printf("sb %d", k); for (int i = 0; i < 9; ++i) printf(" %.17g", R.sb[9 * k + i]); printf("\n");
-    }
+    print_solve_tail(S, s.K, R.t, R.q, &R.sb);
   }
   if (ctx) glio_destroy(ctx);
   return 0;

@@ -24,6 +24,7 @@
 
 #include "ceres/ceres.h"
 #include "ceres/rotation.h"
+#include "shim_driver.h"
 
 template <typename T> static void Rotate(const T q[4], const T v[3], T o[3]) {   // q v q^-1 for any q: v + 2w (u x v) + 2 u x (u x v)
   T uv[3] = {q[2] * v[2] - q[3] * v[1], q[3] * v[0] - q[1] * v[2], q[1] * v[1] - q[2] * v[0]};
@@ -169,10 +170,6 @@ struct RangeF {
   }
 };
 
-template <class T> static void rd(FILE* f, T* p, size_t n) {
-  if (fread(p, sizeof(T), n, f) != n) { fprintf(stderr, "shim_routes_test: truncated problem file\n"); exit(2); }
-}
-
 // one problem file (written by tests/test_shim_routes.py: write_problem)
 struct Spec {
   int32_t W = 0, use_sb = 0;
@@ -308,11 +305,7 @@ static Result solve(const Spec& s, glio_ctx* ctx, bool evaluate_only = false) {
   return R;
 }
 
-static int64_t edge_launches(glio_ctx* ctx) {
-  int64_t a = 0, b = 0;
-  glio_profile_get(ctx, "k_eval_edge", nullptr, &a); glio_profile_get(ctx, "k_eval_edge_cost", nullptr, &b);
-  return a + b;
-}
+static int64_t edge_launches(glio_ctx* ctx) { return launches(ctx, {"k_eval_edge", "k_eval_edge_cost"}); }
 
 int main(int argc, char** argv) {
   if (argc < 3) { fprintf(stderr, "usage: shim_routes_test host|device|evaluate [--repeat R] [--use-edges] [--preload-edges N] problem.bin...\n"); return 2; }
@@ -334,9 +327,8 @@ int main(int argc, char** argv) {
     for (int k = 0; k < 4; ++k) prm.q_lb[k] = s0.q_lb[k];
     for (int k = 0; k < 3; ++k) prm.t_lb[k] = s0.t_lb[k];
     prm.lidar_const = s0.lidar_const; prm.huber_delta = s0.huber; prm.unit_score = s0.unit_score;
-    if (glio_create(0, &prm, &ctx) != GLIO_OK) { fprintf(stderr, "glio_create: %s\n", glio_last_error(nullptr)); return 3; }
+    ctx = create_context(prm, !repeat);
     if (use_edges && glio_window_use_edges(ctx, 1) != GLIO_OK) return 3;
-    if (!repeat && glio_profile_enable(ctx, 1) != GLIO_OK) return 3;   // launch counts; timed runs leave the profiler off
     if (preload > 0) {
       // points 1 m off the x axis, against the x axis as the line: every edge has a residual at any pose near the identity
       std::vector<float> cp(3 * (size_t)preload), pa(3 * (size_t)preload, 0.f), pb(3 * (size_t)preload, 0.f);
@@ -371,22 +363,16 @@ int main(int argc, char** argv) {
       }
       continue;
     }
-    const int64_t e0 = ctx ? edge_launches(ctx) : 0;
+    const int64_t e0 = edge_launches(ctx);
     const Result R = solve(s, ctx);
-    const int64_t e1 = ctx ? edge_launches(ctx) : 0;
+    const int64_t e1 = edge_launches(ctx);
     const ceres::Solver::Summary& S = R.summary;
     const int dev_edges = S.num_device_edge_residual_blocks;
-    printf("termination %d\n", (int)S.termination_type);
-    printf("iters %d\n", (int)S.iterations.size());
+    print_solve_head(S);
     printf("device_blocks %d\n", S.num_device_residual_blocks);
     printf("device_kinds %d %d\n", S.num_device_residual_blocks - dev_edges, dev_edges);
     printf("edge_launches %lld\n", (long long)(e1 - e0));
-    printf("cost %.17g %.17g\n", S.initial_cost, S.final_cost);
-    for (auto& it : S.iterations) printf("it %d %d %.17g %.17g\n", it.iteration, (int)it.step_is_successful, it.cost, it.trust_region_radius);
-    for (int k = 0; k < s.W; ++k) {
-      printf("pose %d %.17g %.17g %.17g %.17g %.17g %.17g %.17g\n", k, R.t[3 * k], R.t[3 * k + 1], R.t[3 * k + 2], R.q[4 * k], R.q[4 * k + 1], R.q[4 * k + 2], R.q[4 * k + 3]);
-      printf("sb %d", k); for (int i = 0; i < 9; ++i) printf(" %.17g", R.sb[9 * k + i]); printf("\n");
-    }
+    print_solve_tail(S, s.W, R.t, R.q, &R.sb);
   }
   if (ctx) glio_destroy(ctx);
   return 0;

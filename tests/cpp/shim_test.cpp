@@ -129,10 +129,10 @@ struct RangeF {
 template <class T> static bool rd(FILE* f, T* p, size_t n) { return fread(p, sizeof(T), n, f) == n; }
 
 int main(int argc, char** argv) {
-  if (argc < 3) { fprintf(stderr, "usage: shim_test problem.bin host|device\n"); return 2; }
-  FILE* f = fopen(argv[1], "rb");
+  if (argc < 3) { fprintf(stderr, "usage: shim_test host|device problem.bin\n"); return 2; }
+  FILE* f = fopen(argv[2], "rb");
   if (!f) return 2;
-  const bool device = std::string(argv[2]) == "device";
+  const bool device = std::string(argv[1]) == "device";
   int32_t W, use_sb;
   rd(f, &W, 1); rd(f, &use_sb, 1);
   std::vector<double> poses(7 * W), sb(9 * W);
@@ -219,6 +219,7 @@ int main(int argc, char** argv) {
     options.use_nonmonotonic_steps = false;
     ceres::Solve(options, &problem, &summary);
   }
+  printf("solve\n");
   printf("termination %d\n", (int)summary.termination_type);
   printf("iters %d\n", (int)summary.iterations.size());
   printf("device_blocks %d\n", summary.num_device_residual_blocks);

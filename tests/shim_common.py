@@ -1,20 +1,84 @@
-"""Helpers for the Ceres-shim tests: serialise a window problem, build and run tests/cpp/shim_test."""
+"""Helpers for the Ceres-shim tests: build and run the shim drivers under tests/cpp, serialise tests/cpp/shim_test's window
+problem, compare two solves."""
 import os
 import struct
 import subprocess
 
 import numpy as np
+import pytest
+
+from glio_b200 import synth
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def build_shim_test(tmpdir):
-    exe = os.path.join(str(tmpdir), "shim_test")
-    cmd = ["/usr/bin/g++", "-O2", "-std=c++17", "-I", os.path.join(ROOT, "glio_b200", "shim"), os.path.join(ROOT, "tests", "cpp", "shim_test.cpp"),
+def build_driver(tmpdir, name):
+    """compile tests/cpp/<name>.cpp against the shim headers and the in-tree libglio_b200.so"""
+    exe = os.path.join(str(tmpdir), name)
+    cmd = ["/usr/bin/g++", "-O2", "-std=c++17", "-I", os.path.join(ROOT, "glio_b200", "shim"), os.path.join(ROOT, "tests", "cpp", name + ".cpp"),
            "-o", exe, "-L", os.path.join(ROOT, "glio_b200"), "-lglio_b200", "-Wl,-rpath," + os.path.join(ROOT, "glio_b200"),
            "-L/usr/local/cuda/lib64", "-Wl,-rpath,/usr/local/cuda/lib64", "-lcudart"]
     subprocess.check_call(cmd)
     return exe
+
+
+def run_driver(exe, mode, paths, *flags, desc_ints=0):
+    """run a shim driver on problem files; one record per `solve` line it prints, each with the lines that follow as `text`.
+    desc_ints: how many leading integers the driver's `desc` lines have before their hex-float values"""
+    out = subprocess.check_output([exe, mode, *flags, *[str(p) for p in paths]], text=True)
+    res, head = [], {}
+    for line in out.splitlines():
+        key, *v = line.split()
+        if key == "preload_cost":
+            head["preload_cost"] = float(v[0])
+        if key.startswith("preload"):
+            continue
+        if key == "solve":
+            res.append(dict(iters=[], poses={}, sb={}, text=[], desc=[], frames=[], times=[])); continue
+        r = res[-1]
+        r["text"].append(line)
+        if key == "iters": r["n_iters"] = int(v[0])
+        elif key in ("termination", "blocks") or key.startswith("device_") or key.endswith("_launches"):
+            r[key] = int(v[0]) if len(v) == 1 else tuple(int(x) for x in v)
+        elif key in ("cost", "const"): r[key] = (float(v[0]), float(v[1]))
+        elif key in ("eval_cost", "gate_margin"): r[key] = float(v[0])
+        elif key == "it": r["iters"].append((int(v[0]), int(v[1]), float(v[2]), float(v[3])))
+        elif key in ("pose", "sb"): r["poses" if key == "pose" else "sb"][int(v[0])] = np.array([float(x) for x in v[1:]])
+        elif key == "gradient": r["gradient"] = np.array([float(x) for x in v])
+        elif key == "frame": r["frames"].append(np.array([float.fromhex(x) for x in v]).reshape(3, 3))
+        elif key == "time": r["times"].append((float(v[0]), *(int(x) for x in v[1:])))
+        elif key == "desc": r["desc"].append((*(int(x) for x in v[:desc_ints]), [float.fromhex(x) for x in v[desc_ints:]]))
+    for r in res:
+        if r["poses"]:
+            r["poses"] = np.array([r["poses"][k] for k in sorted(r["poses"])]); r["sb"] = np.array([r["sb"][k] for k in sorted(r["sb"])])
+    if res:
+        res[0].update(head)
+    return res
+
+
+def rot_err(qa, qb):
+    """rotation angle between two sets of unit quaternions (N, 4)"""
+    qa = np.atleast_2d(qa); qb = np.atleast_2d(qb)
+    d = np.array([synth.quat_mul(synth.quat_conj(a), b) for a, b in zip(qa, qb)])
+    return float(np.max(2.0 * np.linalg.norm(d[:, 1:], axis=1)))
+
+
+def assert_same_solve(a, b, sb=True, iterate_abs=0.0):
+    """same termination, iterations and accept/reject decisions, initial and final cost rel 1e-9, poses 1e-6 m / 1e-8 rad,
+    speed-bias 1e-6 (sb).  Iterates compare within 1e-9 relative plus iterate_abs of the initial cost: an iterate's cost carries
+    the rounding of the steps, taken at the scale of the initial cost, and the batch problems' attitude factors (weight 10^4) make
+    the first step drop the cost by three to five orders of magnitude."""
+    assert a["termination"] == b["termination"]
+    assert a["n_iters"] == b["n_iters"] >= 2
+    assert [i[1] for i in a["iters"]] == [i[1] for i in b["iters"]]
+    assert a["cost"][0] == pytest.approx(b["cost"][0], rel=1e-9)
+    for x, y in zip(a["iters"], b["iters"]):
+        assert x[2] == pytest.approx(y[2], rel=1e-9, abs=iterate_abs * b["cost"][0])
+    assert a["cost"][1] == pytest.approx(b["cost"][1], rel=1e-9)
+    assert np.max(np.abs(a["poses"][:, :3] - b["poses"][:, :3])) <= 1e-6
+    assert rot_err(a["poses"][:, 3:], b["poses"][:, 3:]) <= 1e-8
+    if sb:
+        assert np.max(np.abs(a["sb"] - b["sb"])) <= 1e-6
 
 
 def write_problem(path, poses, sb, q_lb, t_lb, lidar_const, huber, kf, cp, nsd, w, priors, betweens, ranges, binary=None):
@@ -46,24 +110,6 @@ def write_problem(path, poses, sb, q_lb, t_lb, lidar_const, huber, kf, cp, nsd, 
             f.write(np.ascontiguousarray(kc, np.int32).tobytes()); f.write(np.ascontiguousarray(ko, np.int32).tobytes())
             f.write(np.ascontiguousarray(bcp, np.float32).tobytes()); f.write(np.ascontiguousarray(bnc, np.float64).tobytes())
             f.write(np.ascontiguousarray(bsc, np.float64).tobytes())
-
-
-def run_shim(exe, path, mode):
-    out = subprocess.check_output([exe, path, mode], text=True)
-    res = dict(iters=[], poses={}, sb={})
-    for line in out.splitlines():
-        p = line.split()
-        if p[0] == "termination": res["termination"] = int(p[1])
-        elif p[0] == "iters": res["n_iters"] = int(p[1])
-        elif p[0] == "device_blocks": res["device_blocks"] = int(p[1])
-        elif p[0] == "blocks": res["blocks"] = (int(p[1]), int(p[2]))
-        elif p[0] == "it": res["iters"].append((int(p[1]), int(p[2]), float(p[3]), float(p[4])))
-        elif p[0] == "pose": res["poses"][int(p[1])] = np.array([float(v) for v in p[2:]])
-        elif p[0] == "sb": res["sb"][int(p[1])] = np.array([float(v) for v in p[2:]])
-        elif p[0] == "const": res["const"] = (float(p[1]), float(p[2]))
-    res["poses"] = np.array([res["poses"][k] for k in sorted(res["poses"])])
-    res["sb"] = np.array([res["sb"][k] for k in sorted(res["sb"])])
-    return res
 
 
 def make_problem(oracle, synth, W=4, Q=800, M=20000, seed=17, n_sel=150):

@@ -23,36 +23,36 @@ def _check(res, ro, W):
 
 
 def test_shim_host_only_matches_oracle(tmp_path, oracle):
-    exe = sc.build_shim_test(tmp_path)
+    exe = sc.build_driver(tmp_path, "shim_test")
     P, kf, cp, nsd, w, sb0, priors, betweens, ranges = sc.make_problem(oracle, synth)
     path = str(tmp_path / "p.bin")
     sc.write_problem(path, P["poses_init"], sb0, P["q_lb"], P["t_lb"], 7.5, 1.0, kf, cp, nsd, w, priors, betweens, ranges)
     ro = sc.oracle_solve(oracle, P, kf, cp, nsd, w, sb0, priors, betweens, ranges)
-    res = sc.run_shim(exe, path, "host")
+    res = sc.run_driver(exe, "host", [path])[0]
     assert res["device_blocks"] == 0
     _check(res, ro, 4)
 
 
 @pytest.mark.gpu
 def test_shim_device_routing_matches_oracle(tmp_path, oracle):
-    exe = sc.build_shim_test(tmp_path)
+    exe = sc.build_driver(tmp_path, "shim_test")
     P, kf, cp, nsd, w, sb0, priors, betweens, ranges = sc.make_problem(oracle, synth)
     path = str(tmp_path / "p.bin")
     sc.write_problem(path, P["poses_init"], sb0, P["q_lb"], P["t_lb"], 7.5, 1.0, kf, cp, nsd, w, priors, betweens, ranges)
     ro = sc.oracle_solve(oracle, P, kf, cp, nsd, w, sb0, priors, betweens, ranges)
-    res = sc.run_shim(exe, path, "device")
+    res = sc.run_driver(exe, "device", [path])[0]
     assert res["device_blocks"] == len(kf)                 # every LidarPlaneNormFactor block ran on the GPU
     _check(res, ro, 4)
 
 
 def _binary_case(tmp_path, oracle, mode):
-    exe = sc.build_shim_test(tmp_path)
+    exe = sc.build_driver(tmp_path, "shim_test")
     P, kf, cp, nsd, w, sb0, priors, betweens, ranges = sc.make_problem(oracle, synth)
     binary = sc.make_binary(oracle, synth, P)
     path = str(tmp_path / "pb.bin")
     sc.write_problem(path, P["poses_init"], sb0, P["q_lb"], P["t_lb"], 7.5, 1.0, kf, cp, nsd, w, priors, betweens, ranges, binary=binary)
     ro = sc.oracle_solve(oracle, P, kf, cp, nsd, w, sb0, priors, betweens, ranges, binary=binary)
-    res = sc.run_shim(exe, path, mode)
+    res = sc.run_driver(exe, mode, [path])[0]
     return res, ro, len(kf), len(binary[0])
 
 

@@ -2,9 +2,7 @@
 tests/cpp/shim_dd_psr_routes_test.cpp: problems built with optimizeBatchWithLandMark's call sequence give the same iterates
 host-only and device-routed and through glio_batch_solve, a level-0 problem routes every residual block, blocks K2g cannot
 evaluate exactly stay on the host, and problems without DD blocks launch no K2g kernel."""
-import os
 import struct
-import subprocess
 
 import numpy as np
 import pytest
@@ -12,21 +10,12 @@ import pytest
 from glio_b200 import synth
 from tests import dd_psr_reference as dr
 from tests import eval_reference as er
-from tests.test_shim_pose_routes import assert_same_solve, binary_records, curved_pose_graph
+from tests import shim_common as sc
+from tests.test_shim_pose_routes import binary_records, curved_pose_graph
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 YAW = 0.3
 REL, DQ = 0, 1                                  # the driver's pose record kinds (synth's kind column: 1 = attitude)
 BIN_DTYPE = np.dtype([("kc", "<i4"), ("ko", "<i4"), ("cp", "<f8", (3,)), ("nc", "<f8", (6,)), ("score", "<f8")])
-
-
-def build_driver(tmpdir):
-    exe = os.path.join(str(tmpdir), "shim_dd_psr_routes_test")
-    cmd = ["/usr/bin/g++", "-O2", "-std=c++17", "-I", os.path.join(ROOT, "glio_b200", "shim"),
-           os.path.join(ROOT, "tests", "cpp", "shim_dd_psr_routes_test.cpp"), "-o", exe, "-L", os.path.join(ROOT, "glio_b200"), "-lglio_b200",
-           "-Wl,-rpath," + os.path.join(ROOT, "glio_b200"), "-L/usr/local/cuda/lib64", "-Wl,-rpath,/usr/local/cuda/lib64", "-lcudart"]
-    subprocess.check_call(cmd)
-    return exe
 
 
 # ---------------------------------------------------------------------------------------------------------------------------
@@ -99,35 +88,6 @@ def write_problem(path, poses, pose=None, binary=None, dds=(), frames=None, t_co
         f.write(struct.pack("<id", max_iter, time_limit))
 
 
-def run(exe, mode, paths, *flags):
-    out = subprocess.check_output([exe, mode, *flags, *[str(p) for p in paths]], text=True)
-    res = []
-    ints = ("termination", "blocks", "device_blocks", "device_pose", "device_dd", "dd_launches", "pose_launches")
-    for line in out.splitlines():
-        p = line.split()
-        if p[0] == "preload":
-            continue
-        if p[0] == "solve":
-            res.append(dict(iters=[], poses={}, text=[], desc=[], frames=[], times=[])); continue
-        r = res[-1]
-        r["text"].append(line)
-        if p[0] in ints: r[p[0]] = int(p[1])
-        elif p[0] == "iters": r["n_iters"] = int(p[1])
-        elif p[0] == "gate_margin": r["gate_margin"] = float(p[1])
-        elif p[0] == "cost": r["cost"] = (float(p[1]), float(p[2]))
-        elif p[0] == "it": r["iters"].append((int(p[1]), int(p[2]), float(p[3]), float(p[4])))
-        elif p[0] == "pose": r["poses"][int(p[1])] = np.array([float(v) for v in p[2:]])
-        elif p[0] == "eval_cost": r["eval_cost"] = float(p[1])
-        elif p[0] == "gradient": r["gradient"] = np.array([float(v) for v in p[1:]])
-        elif p[0] == "desc": r["desc"].append((int(p[1]), int(p[2]), int(p[3]), int(p[4]), [float.fromhex(v) for v in p[5:]]))
-        elif p[0] == "frame": r["frames"].append(np.array([float.fromhex(v) for v in p[1:]]).reshape(3, 3))
-        elif p[0] == "time": r["times"].append((float(p[1]), int(p[2]), int(p[3]), int(p[4])))
-    for r in res:
-        if r["poses"]:
-            r["poses"] = np.array([r["poses"][k] for k in sorted(r["poses"])])
-    return res
-
-
 # ---------------------------------------------------------------------------------------------------------------------------
 # problems
 # ---------------------------------------------------------------------------------------------------------------------------
@@ -191,7 +151,7 @@ def n_pose(c):
 def test_host_evaluate_dd_factor(tmp_path):
     """Problem::Evaluate of a DD-only problem (the restated factor, host) against the longdouble reference: n_sat 2 .. 20, the master
     anywhere, i < j and i > j, identity and dense W, the 1e9 / 10 / 8 / 6 gates"""
-    exe = build_driver(tmp_path)
+    exe = sc.build_driver(tmp_path, "shim_dd_psr_routes_test")
     rng = np.random.default_rng(21)
     K = 6
     truth = synth.trajectory(K, rng)
@@ -200,8 +160,8 @@ def test_host_evaluate_dd_factor(tmp_path):
     f, sats, W, _, anchor = dr.random_list(rng, truth, ij, np.array([2, 3, 19, 20, 7, 11, 5, 9]), with_w=True)
     dds = dd_from_records(f, sats, W)
     write_problem(tmp_path / "e.bin", poses, dds=dds)
-    frame = run(exe, "describe", [tmp_path / "e.bin"])[0]["frames"][0]
-    r = run(exe, "evaluate", [tmp_path / "e.bin"])[0]
+    frame = sc.run_driver(exe, "describe", [tmp_path / "e.bin"], desc_ints=4)[0]["frames"][0]
+    r = sc.run_driver(exe, "evaluate", [tmp_path / "e.bin"])[0]
     ref = dr.dd_blocks(poses, f, sats, frame, anchor, W)
     er.assert_within(r["eval_cost"], ref["cost"], ref["Mcost"], "cost")
     g = r["gradient"][:6 * K].reshape(K, 6)                        # per keyframe t, q (tangent); then yaw and anchor
@@ -212,11 +172,11 @@ def test_host_evaluate_dd_factor(tmp_path):
 
 def test_ecef2rotation_matches_synth(tmp_path):
     """the driver's gnss_comm ecef2rotation * R_enu_local(yaw) (the trait's frame()) against synth.ecef_local_rotation"""
-    exe = build_driver(tmp_path)
+    exe = sc.build_driver(tmp_path, "shim_dd_psr_routes_test")
     frames = [(y, synth.geo_to_ecef(lat, lon, h), 1, 1) for y, lat, lon, h in
               ((0.3, 22.3, 114.18, 5.0), (-2.0, -33.9, 151.2, 40.0), (1.1, 64.1, -21.9, 0.0), (0.0, 0.5, -179.0, 1200.0), (3.0, -80.0, 10.0, 5.0))]
     write_problem(tmp_path / "f.bin", np.tile([0, 0, 0, 1, 0, 0, 0], (2, 1)), frames=frames)
-    got = run(exe, "describe", [tmp_path / "f.bin"])[0]["frames"]
+    got = sc.run_driver(exe, "describe", [tmp_path / "f.bin"], desc_ints=4)[0]["frames"]
     assert len(got) == len(frames)
     for R, (yaw, anchor, _, _) in zip(got, frames):
         np.testing.assert_allclose(R, synth.ecef_local_rotation(anchor, yaw), rtol=0, atol=4e-16)
@@ -233,7 +193,7 @@ def _desc_case(rng, n_sat, master, W=None, n_ref=None):
 def test_descriptions_are_the_constructor_arguments(tmp_path):
     """the trait returns the factor's private data bit for bit, read through the explicit-instantiation idiom; it refuses what K2g
     cannot evaluate: n_sat 1 and 21, a master out of range, a W of the wrong size, station data of another length"""
-    exe = build_driver(tmp_path)
+    exe = sc.build_driver(tmp_path, "shim_dd_psr_routes_test")
     rng = np.random.default_rng(5)
     good = []
     for n_sat in (2, 3, 19, 20):
@@ -247,7 +207,7 @@ def test_descriptions_are_the_constructor_arguments(tmp_path):
     bad = [_desc_case(rng, 1, 0), _desc_case(rng, 21, 3), _desc_case(rng, 6, 6), _desc_case(rng, 6, -1),
            _desc_case(rng, 6, 2, W=np.eye(4)), _desc_case(rng, 6, 2, W=np.eye(6)), _desc_case(rng, 6, 2, n_ref=7), _desc_case(rng, 6, 2, n_ref=5)]
     write_problem(tmp_path / "d.bin", np.tile([0, 0, 0, 1, 0, 0, 0], (2, 1)), dds=good + bad)
-    desc = run(exe, "describe", [tmp_path / "d.bin"])[0]["desc"]
+    desc = sc.run_driver(exe, "describe", [tmp_path / "d.bin"], desc_ints=4)[0]["desc"]
     assert len(desc) == len(good) + len(bad)
     for d, (ok, n_sat, master, ident, v) in zip(good, desc):
         n = len(d["user"])
@@ -267,10 +227,10 @@ def test_descriptions_are_the_constructor_arguments(tmp_path):
 def test_host_solve_level0(tmp_path):
     """the level-0 problem with its DD factors solved on the host only (no context): no device block, a cost that drops, and a gate
     margin the driver reports"""
-    exe = build_driver(tmp_path)
+    exe = sc.build_driver(tmp_path, "shim_dd_psr_routes_test")
     c = level0(30)
     write_case(tmp_path / "h.bin", c)
-    r = run(exe, "host", [tmp_path / "h.bin"])[0]
+    r = sc.run_driver(exe, "host", [tmp_path / "h.bin"])[0]
     assert r["device_blocks"] == 0 and r["device_dd"] == 0 and r["dd_launches"] == 0
     assert r["blocks"] == n_pose(c) + len(c["dds"]) and len(c["dds"]) > 0
     assert r["cost"][1] < 1e-2 * r["cost"][0]
@@ -292,22 +252,22 @@ def assert_gate_clear(h):
 def test_device_matches_host(tmp_path, K, outer_pass):
     """level-0 problems (attitude, relative and DD blocks) at each outer pass's threshold: every residual block is routed, and the
     device-routed solve agrees with the host-routed one"""
-    exe = build_driver(tmp_path)
+    exe = sc.build_driver(tmp_path, "shim_dd_psr_routes_test")
     # K = 7 uses seed SEED0 + 29 in place of the default SEED0 + 16: at that size the pass-0 problem (every outlier row at full
     # weight) of the default seed ends without convergence after its 10 iterations, and its nonmonotonic steps carried the DD
     # rows' rounding (a few 1e-11 of the cost per evaluation) to 3e-9 of an iterate's cost; seed 29's problems converge at every pass
     c = level0(K, seed=synth.SEED0 + (29 if K == 7 else 16), outer_pass=outer_pass)
     path = tmp_path / "p.bin"
     write_case(path, c)
-    dev = run(exe, "device", [path])[0]
-    host = run(exe, "host", [path])[0]
+    dev = sc.run_driver(exe, "device", [path])[0]
+    host = sc.run_driver(exe, "host", [path])[0]
     n_dd = len(c["dds"])
     assert n_dd > 0 and host["device_blocks"] == 0
     assert dev["device_blocks"] == dev["blocks"] == n_pose(c) + n_dd
     assert dev["device_dd"] == n_dd and dev["device_pose"] == n_pose(c)
     assert dev["dd_launches"] >= dev["n_iters"]                     # K2g runs in every evaluation
     assert_gate_clear(host)
-    assert_same_solve(dev, host)
+    sc.assert_same_solve(dev, host, sb=False, iterate_abs=1e-10)
 
 
 @pytest.mark.gpu
@@ -316,14 +276,14 @@ def test_device_matches_glio_batch_solve(tmp_path, outer_pass):
     """the device-routed solve against glio_batch_solve with glio_batch_use_pose_factors(1) and glio_batch_use_dd_psr_factors(1) on
     the same pose and DD lists, with the R the trait's frame() gives"""
     from glio_b200 import api
-    exe = build_driver(tmp_path)
+    exe = sc.build_driver(tmp_path, "shim_dd_psr_routes_test")
     max_iter = 8
     c = level0(40, outer_pass=outer_pass)
     path = tmp_path / "p.bin"
     write_case(path, c, max_iter=max_iter)
-    dev = run(exe, "device", [path])[0]
-    host = run(exe, "host", [path])[0]
-    R = run(exe, "describe", [path])[0]["frames"][0]
+    dev = sc.run_driver(exe, "device", [path])[0]
+    host = sc.run_driver(exe, "host", [path])[0]
+    R = sc.run_driver(exe, "describe", [path], desc_ints=4)[0]["frames"][0]
     P = c["P"]
     f, sats, W = records_from_dd(c["dds"])
     ctx = api.Context(0)
@@ -340,14 +300,14 @@ def test_device_matches_glio_batch_solve(tmp_path, outer_pass):
               iters=[(i["iteration"], int(i["step_is_successful"]), i["cost"], i["trust_region_radius"]) for i in out["iterations"]])
     assert dev["device_dd"] == len(c["dds"]) and dev["device_blocks"] == dev["blocks"]
     assert_gate_clear(host)
-    assert_same_solve(dev, bs)
+    sc.assert_same_solve(dev, bs, sb=False, iterate_abs=1e-10)
 
 
 @pytest.mark.gpu
 def test_dd_pair_counts_and_translation_only_keyframes(tmp_path):
     """DD-only problems (every keyframe translation-only: its q blocks are unused) with exactly 1, 3, 4, 5, 8 and 9 distinct DD pairs
     (K2g gives 4 pairs to a block), i < j and i > j, solved in turn on one context and on the host; one of them with dense W"""
-    exe = build_driver(tmp_path)
+    exe = sc.build_driver(tmp_path, "shim_dd_psr_routes_test")
     paths = []
     for n_pairs in (1, 3, 4, 5, 8, 9):
         c = dd_chain(n_pairs, synth.SEED0 + 60 + n_pairs, with_w=n_pairs == 5)
@@ -355,12 +315,12 @@ def test_dd_pair_counts_and_translation_only_keyframes(tmp_path):
         path = tmp_path / f"c{n_pairs}.bin"
         write_case(path, c)
         paths.append((path, len(c["dds"])))
-    dev = run(exe, "device", [p for p, _ in paths])
-    host = run(exe, "host", [p for p, _ in paths])
+    dev = sc.run_driver(exe, "device", [p for p, _ in paths])
+    host = sc.run_driver(exe, "host", [p for p, _ in paths])
     for d, h, (_, n) in zip(dev, host, paths):
         assert d["device_dd"] == d["device_blocks"] == d["blocks"] == n and d["device_pose"] == 0
         assert_gate_clear(h)
-        assert_same_solve(d, h)
+        sc.assert_same_solve(d, h, sb=False, iterate_abs=1e-10)
 
 
 @pytest.mark.gpu
@@ -368,7 +328,7 @@ def test_level1_shape_and_dense_weights(tmp_path):
     """a level-1-shaped problem (BinaryLidarPlaneNormFactor blocks of the batch pairs, attitude and DD blocks: DD keyframes shared
     with the binary-plane keyframes), and a level-0 problem whose DD factors carry dense, non-identity weights"""
     from glio_b200.dist import batch_pairs
-    exe = build_driver(tmp_path)
+    exe = sc.build_driver(tmp_path, "shim_dd_psr_routes_test")
     K = 30
     c = level0(K, seed=synth.SEED0 + 18)
     P = dict(c["P"]); P["pairs"] = batch_pairs(K, 6)
@@ -384,13 +344,13 @@ def test_level1_shape_and_dense_weights(tmp_path):
         d["W"] = np.eye(m) + rng.normal(0, 0.1, (m, m))
     path2 = tmp_path / "w.bin"
     write_case(path2, c, dds=dds)
-    dev = run(exe, "device", [path1, path2])
-    host = run(exe, "host", [path1, path2])
+    dev = sc.run_driver(exe, "device", [path1, path2])
+    host = sc.run_driver(exe, "host", [path1, path2])
     assert dev[0]["device_blocks"] == dev[0]["blocks"] == len(B) + int(att.sum()) + len(c["dds"])
     assert dev[1]["device_blocks"] == dev[1]["blocks"] and dev[1]["device_dd"] == len(dds)
     for d, h in zip(dev, host):
         assert_gate_clear(h)
-        assert_same_solve(d, h)
+        sc.assert_same_solve(d, h, sb=False, iterate_abs=1e-10)
 
 
 @pytest.mark.gpu
@@ -398,7 +358,7 @@ def test_blocks_that_stay_on_the_host(tmp_path):
     """DD blocks K2g cannot evaluate exactly stay on the host, next to routed ones: a variable yaw, a variable anchor, a loss, t_i ==
     t_j, a constant t (keyframe 0 gauge-fixed), a second constant (yaw, anchor) pair, a t paired with two q blocks, and a factor
     added through a ceres::CostFunction*.  The DD device count is exactly the routable one, and the solve agrees with the host one."""
-    exe = build_driver(tmp_path)
+    exe = sc.build_driver(tmp_path, "shim_dd_psr_routes_test")
     K = 30
     c = level0(K)
     base = c["dds"]
@@ -425,13 +385,13 @@ def test_blocks_that_stay_on_the_host(tmp_path):
     assert 0 < expect < len(dds) - len(extra) + 1 and expect < len(base)
     path = tmp_path / "m.bin"
     write_problem(path, c["poses"], pose=pose, dds=dds, frames=frames, t_const=t_const, q_alt=q_alt)
-    dev = run(exe, "device", [path])[0]
-    host = run(exe, "host", [path])[0]
+    dev = sc.run_driver(exe, "device", [path])[0]
+    host = sc.run_driver(exe, "host", [path])[0]
     assert host["device_blocks"] == 0
     assert dev["device_dd"] == expect
     assert dev["device_blocks"] == dev["device_dd"] + dev["device_pose"] < dev["blocks"]
     assert_gate_clear(host)
-    assert_same_solve(dev, host)
+    sc.assert_same_solve(dev, host, sb=False, iterate_abs=1e-10)
     assert np.array_equal(dev["poses"][0, :3], c["poses"][0, :3])                  # the constant t stayed put
 
 
@@ -440,18 +400,18 @@ def test_solve_sequences_on_one_context(tmp_path):
     """DD problem -> pose-only problem -> DD-only problem -> DD problem on one context print the same text (%.17g) as fresh contexts,
     also with both switches on and after a direct caller left another DD list with the switch on; the pose-only problem launches no
     K2g kernel"""
-    exe = build_driver(tmp_path)
+    exe = sc.build_driver(tmp_path, "shim_dd_psr_routes_test")
     paths = [tmp_path / f"s{i}.bin" for i in range(4)]
     write_case(paths[0], level0(40))
     c1 = level0(30, seed=synth.SEED0 + 19)
     write_case(paths[1], c1, dds=[])
     write_case(paths[2], dd_chain(9, synth.SEED0 + 70))
     write_case(paths[3], level0(25, seed=synth.SEED0 + 17, outer_pass=3))
-    fresh = [run(exe, "device", [p])[0] for p in paths]
+    fresh = [sc.run_driver(exe, "device", [p])[0] for p in paths]
     assert [f["dd_launches"] > 0 for f in fresh] == [True, False, True, True]
     assert fresh[1]["device_dd"] == 0 and fresh[1]["device_pose"] > 0
     for flags in ((), ("--use-pose", "--use-dd"), ("--preload-dd", "40")):
-        seq = run(exe, "device", paths, *flags)
+        seq = sc.run_driver(exe, "device", paths, *flags)
         assert len(seq) == 4
         for a, b in zip(seq, fresh):
             assert a["text"] == b["text"]

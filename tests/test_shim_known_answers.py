@@ -1,16 +1,12 @@
 """Ceres' own unit-test expectations (loss_function_test.cc, corrector_test.cc, local_parameterization_test.cc, rotation /
 jet checks; the reference vendors Ceres 2.0.0) against the PRODUCT's Ceres-API shim (glio_b200/shim/ceres)."""
-import os
 import subprocess
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+from tests import shim_common as sc
 
 
 def test_shim_against_ceres_known_answers(tmp_path):
-    exe = str(tmp_path / "shim_ka")
-    subprocess.check_call(["/usr/bin/g++", "-O2", "-std=c++17", "-I", os.path.join(ROOT, "glio_b200", "shim"), os.path.join(ROOT, "tests", "cpp", "shim_known_answers.cpp"),
-                           "-o", exe, "-L", os.path.join(ROOT, "glio_b200"), "-lglio_b200", "-Wl,-rpath," + os.path.join(ROOT, "glio_b200"),
-                           "-L/usr/local/cuda/lib64", "-Wl,-rpath,/usr/local/cuda/lib64", "-lcudart"])
+    exe = sc.build_driver(tmp_path, "shim_known_answers")
     p = subprocess.run([exe], text=True, capture_output=True)
     lines = p.stdout.splitlines()
     assert len(lines) == 38, p.stdout + p.stderr

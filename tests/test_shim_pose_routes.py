@@ -3,9 +3,7 @@ driven by tests/cpp/shim_pose_routes_test.cpp: problems built with optimizeBatch
 host-only and device-routed and through glio_batch_solve, blocks K2p cannot evaluate exactly stay on the host, and problems without
 pose blocks launch no K2p kernel."""
 import ctypes as C
-import os
 import struct
-import subprocess
 
 import numpy as np
 import pytest
@@ -13,8 +11,8 @@ import pytest
 from glio_b200 import synth
 from tests import eval_reference as er
 from tests import pose_factor_reference as pr
+from tests import shim_common as sc
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 REL, DQ, LOOKALIKE = 0, 1, 2                      # the driver's pose record kinds (2: LidarPoseFactorAutoDiff, no trait)
 YAW, ANCHOR = 0.3, np.array([12.0, -7.0, 3.0])    # the constant yaw offset and anchor of the level-0 problems
 PAIR_DTYPE = np.dtype([("kind", "<i4"), ("i", "<i4"), ("j", "<i4"), ("alt", "<i4"), ("dq", "<f8", (4,)), ("dp", "<f8", (3,)),
@@ -22,15 +20,6 @@ PAIR_DTYPE = np.dtype([("kind", "<i4"), ("i", "<i4"), ("j", "<i4"), ("alt", "<i4
 BIN_DTYPE = np.dtype([("kc", "<i4"), ("ko", "<i4"), ("cp", "<f8", (3,)), ("nc", "<f8", (6,)), ("score", "<f8")])
 DD_DTYPE = np.dtype([("i", "<i4"), ("j", "<i4"), ("s1", "<f8", (3,)), ("s2", "<f8", (3,)), ("rho_i", "<f8"), ("rho_j", "<f8"),
                      ("w", "<f8")])
-
-
-def build_driver(tmpdir):
-    exe = os.path.join(str(tmpdir), "shim_pose_routes_test")
-    cmd = ["/usr/bin/g++", "-O2", "-std=c++17", "-I", os.path.join(ROOT, "glio_b200", "shim"),
-           os.path.join(ROOT, "tests", "cpp", "shim_pose_routes_test.cpp"), "-o", exe, "-L", os.path.join(ROOT, "glio_b200"), "-lglio_b200",
-           "-Wl,-rpath," + os.path.join(ROOT, "glio_b200"), "-L/usr/local/cuda/lib64", "-Wl,-rpath,/usr/local/cuda/lib64", "-lcudart"]
-    subprocess.check_call(cmd)
-    return exe
 
 
 def pose_records(i, j, kind, dq, dp=None, alt=None, loss=-1.0):
@@ -70,57 +59,6 @@ def write_problem(path, poses, pose, sb=None, n_rcv=0, epoch=0, t_param=None, q_
             f.write(np.asarray(dv, np.float64).tobytes()); f.write(struct.pack("<d", dt)); f.write(np.asarray(sw, np.float64).tobytes())
         f.write(struct.pack("<i", len(dds))); f.write(np.ascontiguousarray(dds, DD_DTYPE).tobytes())
         f.write(struct.pack("<id", max_iter, time_limit))
-
-
-def run(exe, mode, paths, *flags):
-    out = subprocess.check_output([exe, mode, *flags, *[str(p) for p in paths]], text=True)
-    res = []
-    for line in out.splitlines():
-        p = line.split()
-        if p[0] == "preload":
-            continue
-        if p[0] == "solve":
-            res.append(dict(iters=[], poses={}, sb={}, text=[], desc=[], times=[])); continue
-        r = res[-1]
-        r["text"].append(line)
-        if p[0] == "termination": r["termination"] = int(p[1])
-        elif p[0] == "iters": r["n_iters"] = int(p[1])
-        elif p[0] == "device_blocks": r["device_blocks"] = int(p[1])
-        elif p[0] == "device_pose": r["device_pose"] = int(p[1])
-        elif p[0] == "pose_launches": r["pose_launches"] = int(p[1])
-        elif p[0] == "cost": r["cost"] = (float(p[1]), float(p[2]))
-        elif p[0] == "it": r["iters"].append((int(p[1]), int(p[2]), float(p[3]), float(p[4])))
-        elif p[0] == "pose": r["poses"][int(p[1])] = np.array([float(v) for v in p[2:]])
-        elif p[0] == "sb": r["sb"][int(p[1])] = np.array([float(v) for v in p[2:]])
-        elif p[0] == "eval_cost": r["eval_cost"] = float(p[1])
-        elif p[0] == "gradient": r["gradient"] = np.array([float(v) for v in p[1:]])
-        elif p[0] == "desc": r["desc"].append((int(p[1]), int(p[2]), [float.fromhex(v) for v in p[3:]]))
-        elif p[0] == "time": r["times"].append((float(p[1]), int(p[2]), int(p[3])))
-    for r in res:
-        if r["poses"]:
-            r["poses"] = np.array([r["poses"][k] for k in sorted(r["poses"])]); r["sb"] = np.array([r["sb"][k] for k in sorted(r["sb"])])
-    return res
-
-
-def rot_err(qa, qb):
-    d = np.array([synth.quat_mul(synth.quat_conj(a), b) for a, b in zip(np.atleast_2d(qa), np.atleast_2d(qb))])
-    return float(np.max(2.0 * np.linalg.norm(d[:, 1:], axis=1)))
-
-
-def assert_same_solve(a, b):
-    """same termination, iterations and accept/reject decisions, initial and final cost rel 1e-9, poses 1e-6 m / 1e-8 rad.  An
-    iterate's cost carries the rounding of the steps, taken at the scale of the initial cost: the attitude factors' weight 10^4
-    makes the first step drop the cost by three to five orders of magnitude, so iterates compare within 1e-9 relative plus 1e-10
-    of the initial cost."""
-    assert a["termination"] == b["termination"]
-    assert a["n_iters"] == b["n_iters"] >= 2
-    assert [i[1] for i in a["iters"]] == [i[1] for i in b["iters"]]
-    assert a["cost"][0] == pytest.approx(b["cost"][0], rel=1e-9)
-    for x, y in zip(a["iters"], b["iters"]):
-        assert x[2] == pytest.approx(y[2], rel=1e-9, abs=1e-10 * b["cost"][0])
-    assert a["cost"][1] == pytest.approx(b["cost"][1], rel=1e-9)
-    assert np.max(np.abs(a["poses"][:, :3] - b["poses"][:, :3])) <= 1e-6
-    assert rot_err(a["poses"][:, 3:], b["poses"][:, 3:]) <= 1e-8
 
 
 # ---------------------------------------------------------------------------------------------------------------------------
@@ -252,7 +190,7 @@ POSES = {"near": dict(offset=0.0), "3km": dict(offset=3000.0), "20km": dict(offs
 def test_host_evaluate_pose_functors(tmp_path, fx):
     """Problem::Evaluate of a pose-only problem (host Jets) against the longdouble reference of both functors: pins the restated
     functors and their block order"""
-    exe = build_driver(tmp_path)
+    exe = sc.build_driver(tmp_path, "shim_pose_routes_test")
     rng = np.random.default_rng(11)
     K = 9
     kw = dict(POSES[fx])
@@ -265,7 +203,7 @@ def test_host_evaluate_pose_functors(tmp_path, fx):
     kind = rng.choice([REL, DQ], n)
     dp = rng.normal(0, 1.5, (n, 3))
     write_problem(tmp_path / "p.bin", poses, pose_records(i, j, kind, dq, dp))
-    r = run(exe, "evaluate", [tmp_path / "p.bin"])[0]
+    r = sc.run_driver(exe, "evaluate", [tmp_path / "p.bin"])[0]
     from glio_b200 import api
     f = api.pose_factor_records(i, j, np.where(kind == REL, api.POSE_RELATIVE, api.POSE_DELTA_Q), dq, np.where((kind == REL)[:, None], dp, 0.0))
     ref = pr.pose_blocks(poses, f)
@@ -279,7 +217,7 @@ def test_host_evaluate_pose_functors(tmp_path, fx):
 def test_trait_descriptions_are_the_constructor_arguments(tmp_path):
     """both traits return dq / dp bit for bit (values that are not floats, signed zeros, a subnormal, a non-unit dq), the private
     members of LidarPoseFactorBatchRelativeAutoDiff read through the explicit-instantiation idiom; the look-alike has no trait"""
-    exe = build_driver(tmp_path)
+    exe = sc.build_driver(tmp_path, "shim_pose_routes_test")
     rng = np.random.default_rng(4)
     n = 12
     dq = rng.normal(size=(n, 4)) * 0.7; dp = rng.normal(0, 1e3, (n, 3))
@@ -287,7 +225,7 @@ def test_trait_descriptions_are_the_constructor_arguments(tmp_path):
     kind = np.array([REL, DQ] * (n // 2))
     kind[-1] = LOOKALIKE
     write_problem(tmp_path / "d.bin", er.make_poses(2, rng), pose_records(np.zeros(n, int), np.ones(n, int), kind, dq, dp))
-    desc = run(exe, "describe", [tmp_path / "d.bin"])[0]["desc"]
+    desc = sc.run_driver(exe, "describe", [tmp_path / "d.bin"], desc_ints=2)[0]["desc"]
     assert len(desc) == n
     for k, (ok, fk, v) in enumerate(desc):
         if kind[k] == LOOKALIKE:
@@ -302,10 +240,10 @@ def test_trait_descriptions_are_the_constructor_arguments(tmp_path):
 def test_host_solve_level0(tmp_path):
     """the level-0 problem solved on the host only (no context): no device block, and the solve removes almost all of the
     attitude factors' initial cost (the initial rotations are 0.2 degrees off, the factors' keyframe poses 0.05 degrees)"""
-    exe = build_driver(tmp_path)
+    exe = sc.build_driver(tmp_path, "shim_pose_routes_test")
     c = level0(30)
     write_case(tmp_path / "h.bin", c)
-    r = run(exe, "host", [tmp_path / "h.bin"])[0]
+    r = sc.run_driver(exe, "host", [tmp_path / "h.bin"])[0]
     assert r["device_blocks"] == 0 and r["device_pose"] == 0 and r["pose_launches"] == 0
     assert r["cost"][1] < 1e-3 * r["cost"][0]
 
@@ -316,18 +254,18 @@ def test_host_solve_level0(tmp_path):
 @pytest.mark.gpu
 @pytest.mark.parametrize("level,K", [(0, 2), (0, 7), (0, 40), (0, 200), (1, 13), (1, 40), (1, 200)])
 def test_device_matches_host(tmp_path, level, K):
-    exe = build_driver(tmp_path)
+    exe = sc.build_driver(tmp_path, "shim_pose_routes_test")
     c = level0(K) if level == 0 else level1(K)
     path = tmp_path / "p.bin"
     write_case(path, c)
-    dev = run(exe, "device", [path])[0]
-    host = run(exe, "host", [path])[0]
+    dev = sc.run_driver(exe, "device", [path])[0]
+    host = sc.run_driver(exe, "host", [path])[0]
     n_pose = len(c["pose"])
     nb = len(c["kw"].get("binary", ()))
     assert n_pose > 0 and host["device_blocks"] == 0
     assert dev["device_pose"] == n_pose and dev["device_blocks"] == n_pose + nb
     assert dev["pose_launches"] >= dev["n_iters"]                 # K2p runs in every evaluation
-    assert_same_solve(dev, host)
+    sc.assert_same_solve(dev, host, sb=False, iterate_abs=1e-10)
 
 
 def _dd_band_callback(api, ctx, hf, dds, nt):
@@ -370,13 +308,13 @@ def test_device_matches_glio_batch_solve(tmp_path, level):
     """the device-routed solve against glio_batch_solve with glio_batch_use_pose_factors(1), the same pose list and LiDAR pairs,
     and the host stand-ins passed through the band callback"""
     from glio_b200 import api
-    exe = build_driver(tmp_path)
+    exe = sc.build_driver(tmp_path, "shim_pose_routes_test")
     K = 40
     c = level0(K) if level == 0 else level1(K)
     max_iter = 8
     path = tmp_path / "p.bin"
     write_case(path, c, max_iter=max_iter)
-    dev = run(exe, "device", [path])[0]
+    dev = sc.run_driver(exe, "device", [path])[0]
     P = c["P"]
     ctx = api.Context(0)
     hf = None
@@ -408,14 +346,14 @@ def test_device_matches_glio_batch_solve(tmp_path, level):
     bs = dict(termination=int(summ.termination), n_iters=summ.num_iterations, cost=(summ.initial_cost, summ.final_cost), poses=pb,
               iters=[(i["iteration"], int(i["step_is_successful"]), i["cost"], i["trust_region_radius"]) for i in its])
     assert dev["device_pose"] == len(c["pose"])
-    assert_same_solve(dev, bs)
+    sc.assert_same_solve(dev, bs, sb=False, iterate_abs=1e-10)
 
 
 @pytest.mark.gpu
 def test_blocks_that_stay_on_the_host(tmp_path):
     """pose blocks K2p cannot evaluate exactly stay on the host: the device count is exactly the routable one and the solve agrees
     with the host-only one"""
-    exe = build_driver(tmp_path)
+    exe = sc.build_driver(tmp_path, "shim_pose_routes_test")
     K = 30
     c = level0(K)
     base = c["pose"]
@@ -434,11 +372,11 @@ def test_blocks_that_stay_on_the_host(tmp_path):
     assert 0 < expect < len(pose) - 40
     path = tmp_path / "m.bin"
     write_problem(path, c["poses"], pose, t_param=t_param, q_const=q_const, q_ident=q_ident, alt_t=alt_t, **c["kw"])
-    dev = run(exe, "device", [path])[0]
-    host = run(exe, "host", [path])[0]
+    dev = sc.run_driver(exe, "device", [path])[0]
+    host = sc.run_driver(exe, "host", [path])[0]
     assert host["device_blocks"] == 0
     assert dev["device_pose"] == dev["device_blocks"] == expect
-    assert_same_solve(dev, host)
+    sc.assert_same_solve(dev, host, sb=False, iterate_abs=1e-10)
     assert np.array_equal(dev["poses"][5, 3:], c["poses"][5, 3:])                  # the constant q stayed put
 
     # delta_q-only keyframes: the attitude factors alone, the positions held by the stand-ins and a prior; K2p adds rotation
@@ -448,17 +386,17 @@ def test_blocks_that_stay_on_the_host(tmp_path):
     priors, _ = imu_chain(P["poses_true"], None)
     path = tmp_path / "dq.bin"
     write_problem(path, c1["poses"], c1["pose"], sb=np.zeros((K, 9)), priors=priors, dds=dd_records(P["poses_true"], 5))
-    dev = run(exe, "device", [path])[0]
-    host = run(exe, "host", [path])[0]
+    dev = sc.run_driver(exe, "device", [path])[0]
+    host = sc.run_driver(exe, "host", [path])[0]
     assert dev["device_pose"] == dev["device_blocks"] == len(c1["pose"]) == routable(c1["pose"], K)
-    assert_same_solve(dev, host)
+    sc.assert_same_solve(dev, host, sb=False, iterate_abs=1e-10)
 
 
 @pytest.mark.gpu
 def test_pose_pair_counts_around_the_kernel_block(tmp_path):
     """chains with exactly 1, 7, 8, 9, 16 and 17 distinct pose pairs (K2p gives 8 pairs to a block), relative and delta_q factors
     on each pair, solved in turn on one context and on the host"""
-    exe = build_driver(tmp_path)
+    exe = sc.build_driver(tmp_path, "shim_pose_routes_test")
     paths = []
     for n_pairs in (1, 7, 8, 9, 16, 17):
         c = level0(n_pairs + 1, seed=synth.SEED0 + 40 + n_pairs)
@@ -468,11 +406,11 @@ def test_pose_pair_counts_around_the_kernel_block(tmp_path):
         path = tmp_path / f"c{n_pairs}.bin"
         write_problem(path, c["poses"], p, **c["kw"])
         paths.append((path, len(p)))
-    dev = run(exe, "device", [p for p, _ in paths])
-    host = run(exe, "host", [p for p, _ in paths])
+    dev = sc.run_driver(exe, "device", [p for p, _ in paths])
+    host = sc.run_driver(exe, "host", [p for p, _ in paths])
     for d, h, (_, n) in zip(dev, host, paths):
         assert d["device_pose"] == n
-        assert_same_solve(d, h)
+        sc.assert_same_solve(d, h, sb=False, iterate_abs=1e-10)
 
 
 @pytest.mark.gpu
@@ -480,17 +418,17 @@ def test_solve_sequences_on_one_context(tmp_path):
     """pose problem -> binary-only problem -> pose problem on one context print the same text (%.17g) as fresh contexts, also with
     glio_batch_use_pose_factors(1) set and after a direct caller left another pose list with the switch on; the binary-only
     problem launches no K2p kernel"""
-    exe = build_driver(tmp_path)
+    exe = sc.build_driver(tmp_path, "shim_pose_routes_test")
     paths = [tmp_path / f"s{i}.bin" for i in range(4)]
     write_case(paths[0], level0(40))
     write_case(paths[1], level1(30, attitude=False))
     write_case(paths[2], level1(30))
     write_case(paths[3], level0(25, seed=synth.SEED0 + 17))
-    fresh = [run(exe, "device", [p])[0] for p in paths]
+    fresh = [sc.run_driver(exe, "device", [p])[0] for p in paths]
     assert [f["pose_launches"] > 0 for f in fresh] == [True, False, True, True]
     assert fresh[1]["device_pose"] == 0 and fresh[1]["device_blocks"] > 0
     for flags in ((), ("--use-pose",), ("--preload-pose", "40")):
-        seq = run(exe, "device", paths, *flags)
+        seq = sc.run_driver(exe, "device", paths, *flags)
         assert len(seq) == 4
         for a, b in zip(seq, fresh):
             assert a["text"] == b["text"]

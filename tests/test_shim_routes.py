@@ -1,9 +1,7 @@
 """Ceres-API shim routes for LidarEdgeFactor (K2e) and LidarPlaneNormIncreFactor (K2 in a front-end context), driven by
 tests/cpp/shim_routes_test.cpp: problems built with the reference's call sequences give the same iterates host-only and
 device-routed, blocks the kernels cannot evaluate exactly stay on the host, and plane-only problems launch no edge kernel."""
-import os
 import struct
-import subprocess
 
 import numpy as np
 import pytest
@@ -15,15 +13,6 @@ from tests import shim_common as sc
 PLANE, BINARY, EDGE, INCRE = 1, 2, 3, 4          # glio::FactorKind
 IDENT_Q, ZERO_T = np.array([1.0, 0.0, 0.0, 0.0]), np.zeros(3)
 LIDAR_CONST, HUBER = 7.5, 1.0
-
-
-def build_driver(tmpdir):
-    exe = os.path.join(str(tmpdir), "shim_routes_test")
-    cmd = ["/usr/bin/g++", "-O2", "-std=c++17", "-I", os.path.join(sc.ROOT, "glio_b200", "shim"),
-           os.path.join(sc.ROOT, "tests", "cpp", "shim_routes_test.cpp"), "-o", exe, "-L", os.path.join(sc.ROOT, "glio_b200"), "-lglio_b200",
-           "-Wl,-rpath," + os.path.join(sc.ROOT, "glio_b200"), "-L/usr/local/cuda/lib64", "-Wl,-rpath,/usr/local/cuda/lib64", "-lcudart"]
-    subprocess.check_call(cmd)
-    return exe
 
 
 def lidar_records(kind, kf, cp, a=None, b=None, d=None, s=None, q_lb=IDENT_Q, t_lb=ZERO_T, loss=-1.0, kf2=None):
@@ -67,58 +56,6 @@ def write_problem(path, poses, lidar, ctx, sb=None, priors=(), betweens=(), rang
             f.write(struct.pack("<i", k)); f.write(np.asarray(lever, np.float64).tobytes()); f.write(np.asarray(sat, np.float64).tobytes())
             f.write(struct.pack("<dd", rho, w_))
         f.write(struct.pack("<iid", strategy, max_iter, time_limit))
-
-
-def run(exe, mode, paths, *flags):
-    out = subprocess.check_output([exe, mode, *flags, *[str(p) for p in paths]], text=True)
-    res, head = [], {}
-    for line in out.splitlines():
-        p = line.split()
-        if p[0] == "preload_cost":
-            head["preload_cost"] = float(p[1]); continue
-        if p[0] == "solve":
-            res.append(dict(iters=[], poses={}, sb={}, text=[])); continue
-        r = res[-1]
-        r["text"].append(line)
-        if p[0] == "termination": r["termination"] = int(p[1])
-        elif p[0] == "iters": r["n_iters"] = int(p[1])
-        elif p[0] == "device_blocks": r["device_blocks"] = int(p[1])
-        elif p[0] == "device_kinds": r["device_kinds"] = (int(p[1]), int(p[2]))
-        elif p[0] == "edge_launches": r["edge_launches"] = int(p[1])
-        elif p[0] == "cost": r["cost"] = (float(p[1]), float(p[2]))
-        elif p[0] == "it": r["iters"].append((int(p[1]), int(p[2]), float(p[3]), float(p[4])))
-        elif p[0] == "pose": r["poses"][int(p[1])] = np.array([float(v) for v in p[2:]])
-        elif p[0] == "sb": r["sb"][int(p[1])] = np.array([float(v) for v in p[2:]])
-        elif p[0] == "eval_cost": r["eval_cost"] = float(p[1])
-        elif p[0] == "gradient": r["gradient"] = np.array([float(v) for v in p[1:]])
-    for r in res:
-        if r["poses"]:
-            r["poses"] = np.array([r["poses"][k] for k in sorted(r["poses"])]); r["sb"] = np.array([r["sb"][k] for k in sorted(r["sb"])])
-    if res:
-        res[0].update(head)
-    return res
-
-
-def rot_err(qa, qb):
-    """rotation angle between two sets of unit quaternions (N, 4)"""
-    qa = np.atleast_2d(qa); qb = np.atleast_2d(qb)
-    d = np.array([synth.quat_mul(synth.quat_conj(a), b) for a, b in zip(qa, qb)])
-    return float(np.max(2.0 * np.linalg.norm(d[:, 1:], axis=1)))
-
-
-def assert_same_solve(a, b, sb=True):
-    """the bars of test_front_end_scan_matcher_settings / test_shim: same termination, iterations and accept/reject decisions,
-    cost rel 1e-9, poses 1e-6 m / 1e-8 rad, speed-bias 1e-6"""
-    assert a["termination"] == b["termination"]
-    assert a["n_iters"] == b["n_iters"] >= 2
-    assert [i[1] for i in a["iters"]] == [i[1] for i in b["iters"]]
-    for x, y in zip(a["iters"], b["iters"]):
-        assert x[2] == pytest.approx(y[2], rel=1e-9)
-    assert a["cost"][1] == pytest.approx(b["cost"][1], rel=1e-9)
-    assert np.max(np.abs(a["poses"][:, :3] - b["poses"][:, :3])) <= 1e-6
-    assert rot_err(a["poses"][:, 3:], b["poses"][:, 3:]) <= 1e-8
-    if sb:
-        assert np.max(np.abs(a["sb"] - b["sb"])) <= 1e-6
 
 
 # ---------------------------------------------------------------------------------------------------------------------------
@@ -220,7 +157,7 @@ def write_window(path, c, W=4, with_edges=True, extra=None, **kw):
 # ---------------------------------------------------------------------------------------------------------------------------
 def test_host_evaluate_edge_and_incre_functors(tmp_path):
     """Problem::Evaluate of edge-only and Incre-only problems against the extended-precision reference: pins the functors"""
-    exe = build_driver(tmp_path)
+    exe = sc.build_driver(tmp_path, "shim_routes_test")
     rng = np.random.default_rng(5)
     poses = er.make_poses(2, rng)
     q_lb, t_lb = er.Q_LB_NONUNIT, er.T_LB
@@ -228,7 +165,7 @@ def test_host_evaluate_edge_and_incre_functors(tmp_path):
     E = [er.make_edges(rng, poses[k], 300, q_lb, t_lb) for k in range(2)]
     lid = np.concatenate([lidar_records(EDGE, k, E[k]["cp"], a=E[k]["pa"], b=E[k]["pb"], s=E[k]["s"], q_lb=q_lb, t_lb=t_lb, loss=0.3) for k in range(2)])
     write_problem(tmp_path / "e.bin", poses, lid, ctx)
-    r = run(exe, "evaluate", [tmp_path / "e.bin"])[0]
+    r = sc.run_driver(exe, "evaluate", [tmp_path / "e.bin"])[0]
     ref = er.unary_blocks(poses, E, q_lb, t_lb, LIDAR_CONST, 0.3, fn="edge")
     er.assert_within(r["eval_cost"], ref["cost"].sum(), ref["Mcost"].sum(), "edge cost")
     er.assert_within(r["gradient"], ref["g"].ravel(), ref["Mg"].ravel(), "edge gradient")      # blocks t, q per keyframe
@@ -240,7 +177,7 @@ def test_host_evaluate_edge_and_incre_functors(tmp_path):
         u["weight"] = np.ones(len(u["cp"]), np.float32)
     lid = np.concatenate([incre_records(U[k]["cp"], U[k]["nsd"], kf=k) for k in range(2)])
     write_problem(tmp_path / "i.bin", poses, lid, FRONT_CTX, strategy=1)
-    r = run(exe, "evaluate", [tmp_path / "i.bin"])[0]
+    r = sc.run_driver(exe, "evaluate", [tmp_path / "i.bin"])[0]
     ref = er.unary_blocks(poses, U, IDENT_Q, ZERO_T, 1.0, 0.1, unit_score=True)
     er.assert_within(r["eval_cost"], ref["cost"].sum(), ref["Mcost"].sum(), "incre cost")
     g = r["gradient"].reshape(2, 6)[:, [3, 4, 5, 0, 1, 2]]                                  # blocks q, t -> t, q
@@ -255,11 +192,11 @@ def _front_end_check(res, ro):
     for (i, ok, cost, radius), io in zip(res["iters"], ro["iterations"]):
         assert cost == pytest.approx(io["cost"], rel=1e-9)
     assert np.max(np.abs(res["poses"][:, :3] - ro["poses"][:, :3])) <= 1e-6
-    assert rot_err(res["poses"][:, 3:], ro["poses"][:, 3:]) <= 1e-8
+    assert sc.rot_err(res["poses"][:, 3:], ro["poses"][:, 3:]) <= 1e-8
 
 
 def _front_end_case(tmp_path, oracle, mode):
-    exe = build_driver(tmp_path)
+    exe = sc.build_driver(tmp_path, "shim_routes_test")
     state, cp, nsd = front_end_problem(oracle)
     prob = oracle.WindowProblem(state, None, IDENT_Q, ZERO_T, huber_delta=0.1)
     prob.add_unary(np.zeros(len(cp), np.int32), cp, nsd, np.ones(len(cp)))
@@ -268,7 +205,7 @@ def _front_end_case(tmp_path, oracle, mode):
         write_problem(path, state, incre_records(cp, nsd), FRONT_CTX, strategy=1, max_iter=max_it)
         prob.reset_state(state)
         ro = prob.solve(oracle.solver_options(reserved=2, max_num_iterations=max_it), mode=0)
-        res = run(exe, mode, [path])[0]
+        res = sc.run_driver(exe, mode, [path])[0]
         _front_end_check(res, ro)
         assert res["device_blocks"] == (len(cp) if mode == "device" else 0)
         if mode == "device":
@@ -291,17 +228,17 @@ def test_front_end_incre_device_matches_oracle(tmp_path, oracle):
 @pytest.mark.gpu
 def test_window_with_edges_device_host_and_window_solve(tmp_path, oracle):
     from glio_b200 import api
-    exe = build_driver(tmp_path)
+    exe = sc.build_driver(tmp_path, "shim_routes_test")
     c = window_case(oracle)
     path = tmp_path / "w.bin"
     write_window(path, c)
-    dev = run(exe, "device", [path])[0]
-    host = run(exe, "host", [path])[0]
+    dev = sc.run_driver(exe, "device", [path])[0]
+    host = sc.run_driver(exe, "host", [path])[0]
     n_planes, n_edges = len(c["kf"]), sum(len(e) for e in c["edges"].values())
     assert host["device_blocks"] == 0
     assert dev["device_blocks"] == n_planes + n_edges and dev["device_kinds"] == (n_planes, n_edges)
     assert dev["edge_launches"] >= dev["n_iters"]                 # K2e runs in every evaluation: at least one per iteration
-    assert_same_solve(dev, host)
+    sc.assert_same_solve(dev, host)
 
     # the same lists through glio_set_matches / glio_set_edges and glio_window_use_edges(1), host factors in the callback
     P = c["P"]
@@ -326,14 +263,14 @@ def test_window_with_edges_device_host_and_window_solve(tmp_path, oracle):
     ws = dict(termination=int(rw["summary"].termination), n_iters=rw["summary"].num_iterations,
               iters=[(i["iteration"], int(i["step_is_successful"]), i["cost"], i["trust_region_radius"]) for i in rw["iterations"]],
               cost=(rw["summary"].initial_cost, rw["summary"].final_cost), poses=rw["poses"], sb=rw["speed_bias"])
-    assert_same_solve(dev, ws)
+    sc.assert_same_solve(dev, ws)
 
 
 @pytest.mark.gpu
 def test_blocks_that_stay_on_the_host(tmp_path, oracle):
     """edge blocks the kernels cannot evaluate exactly stay on the host; the count of device blocks is exactly the routable ones
     and the solve agrees with the host-only one"""
-    exe = build_driver(tmp_path)
+    exe = sc.build_driver(tmp_path, "shim_routes_test")
     c = window_case(oracle)
     P = c["P"]
     ql, tl = P["q_lb"], P["t_lb"]
@@ -369,11 +306,11 @@ def test_blocks_that_stay_on_the_host(tmp_path, oracle):
         lid = np.concatenate([window_lidar(c), extra])
         write_problem(path, P["poses_init"], lid, ctx, sb=c["sb0"], priors=c["priors"], betweens=c["betweens"], ranges=c["ranges"],
                       t_param=t_param, q_const=q_const)
-        dev = run(exe, "device", [path])[0]
-        host = run(exe, "host", [path])[0]
+        dev = sc.run_driver(exe, "device", [path])[0]
+        host = sc.run_driver(exe, "host", [path])[0]
         assert host["device_blocks"] == 0
         assert dev["device_blocks"] == n_dev and dev["device_kinds"] == kinds
-        assert_same_solve(dev, host)
+        sc.assert_same_solve(dev, host)
         assert np.array_equal(dev["poses"][2, 3:], P["poses_init"][2, 3:])          # the constant q stayed put
 
 
@@ -381,7 +318,7 @@ def test_blocks_that_stay_on_the_host(tmp_path, oracle):
 def test_incre_blocks_outside_a_front_end_context(tmp_path, oracle):
     """LidarPlaneNormIncreFactor blocks go to K2 only in a front-end context: each context below differs from it in exactly one
     field, and the device count then excludes exactly the Incre blocks (the edge blocks of the same problem stay routed)"""
-    exe = build_driver(tmp_path)
+    exe = sc.build_driver(tmp_path, "shim_routes_test")
     state, cp, nsd = front_end_problem(oracle)
     e = er.make_edges(np.random.default_rng(23), state[0], 200, IDENT_Q, ZERO_T, noise=0.03)
     cases = [
@@ -395,11 +332,11 @@ def test_incre_blocks_outside_a_front_end_context(tmp_path, oracle):
         edges = lidar_records(EDGE, 0, e["cp"], a=e["pa"], b=e["pb"], s=e["s"], q_lb=ctx["q_lb"], t_lb=ctx["t_lb"], loss=0.1)
         path = tmp_path / f"{name}.bin"
         write_problem(path, state, [incre_records(cp, nsd), edges], ctx, strategy=1)
-        dev = run(exe, "device", [path])[0]
-        host = run(exe, "host", [path])[0]
+        dev = sc.run_driver(exe, "device", [path])[0]
+        host = sc.run_driver(exe, "host", [path])[0]
         assert dev["device_kinds"] == ((len(cp) if incre_dev else 0), len(e["cp"])), name
         assert dev["device_blocks"] == (len(cp) if incre_dev else 0) + len(e["cp"])
-        assert_same_solve(dev, host, sb=False)
+        sc.assert_same_solve(dev, host, sb=False)
 
 
 def _shim_problem(tmp_path, oracle, binary):
@@ -425,11 +362,11 @@ def _shim_problem(tmp_path, oracle, binary):
 @pytest.mark.parametrize("binary", [False, True])
 def test_plane_only_problems_launch_no_edge_kernel(tmp_path, oracle, binary):
     """test_shim.py's two problems: the device block counts are unchanged and no K2e kernel is launched"""
-    exe = build_driver(tmp_path)
-    old = sc.build_shim_test(tmp_path)
+    exe = sc.build_driver(tmp_path, "shim_routes_test")
+    old = sc.build_driver(tmp_path, "shim_test")
     path, path_old, nu, nb = _shim_problem(tmp_path, oracle, binary)
-    dev = run(exe, "device", [path])[0]
-    ref = sc.run_shim(old, str(path_old), "device")
+    dev = sc.run_driver(exe, "device", [path])[0]
+    ref = sc.run_driver(old, "device", [path_old])[0]
     assert dev["device_blocks"] == ref["device_blocks"] == nu + nb
     assert dev["edge_launches"] == 0
     assert dev["n_iters"] == ref["n_iters"]
@@ -443,19 +380,19 @@ def test_solve_sequences_on_one_context(tmp_path, oracle):
     list left in it would be evaluated: every solve on one context is bit-identical to the same solve on a fresh context, with or
     without glio_window_use_edges(1) set beforehand, and after a direct caller left selected edge lists in every slot
     (glio_set_edges + glio_select_random_edges; the first solve has to clear slot 1's)"""
-    exe = build_driver(tmp_path)
+    exe = sc.build_driver(tmp_path, "shim_routes_test")
     c = window_case(oracle)
     paths = [tmp_path / f"s{i}.bin" for i in range(4)]
     write_window(paths[0], c, W=4)
     write_window(paths[1], c, W=3, with_edges=False)
     write_window(paths[2], c, W=2)
     write_window(paths[3], c, W=4, with_edges={0})
-    fresh = [run(exe, "device", [p])[0] for p in paths]
+    fresh = [sc.run_driver(exe, "device", [p])[0] for p in paths]
     assert [f["device_kinds"][1] for f in fresh] == [sum(len(e) for e in c["edges"].values()), 0, len(c["edges"][0]), len(c["edges"][0])]
     assert [f["edge_launches"] > 0 for f in fresh] == [True, False, True, True]
     assert fresh[3]["cost"][0] < fresh[0]["cost"][0]      # the last problem really lacks the edges of slots 2 and 3
     for flags in ((), ("--use-edges",), ("--use-edges", "--preload-edges", "150")):
-        seq = run(exe, "device", paths, *flags)
+        seq = sc.run_driver(exe, "device", paths, *flags)
         assert len(seq) == 4
         if "--preload-edges" in flags:
             assert seq[0]["preload_cost"] > 1.0               # the left-over lists would add cost if they were evaluated
