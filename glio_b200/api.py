@@ -148,7 +148,8 @@ class Context:
                "k_lc_sum1", "k_lc_means", "k_lc_solve", "k_lc_transform", "k_lc_final", "k_lc_fitness",
                "k_vs_key", "k_vs_hist", "k_vs_scatter", "k_vs_heads", "k_vs_centroid", "k_vs_pack", "k_gm_transform",
                "k_pose_pair_sums", "k_pose_pair_sums_cost", "k_pose_assemble",
-               "k_psr_pair_sums", "k_psr_pair_sums_cost", "k_psr_assemble"]
+               "k_psr_pair_sums", "k_psr_pair_sums_cost", "k_psr_assemble",
+               "k_imu_pair_sums", "k_imu_pair_sums_cost", "k_imu_assemble"]
 
     def lib_profile(self, on):
         self._chk(self._lib.glio_profile_enable(self._h, C.c_int(1 if on else 0)))
@@ -1055,6 +1056,70 @@ Context.batch_set_dd_psr_factors = _batch_set_dd_psr_factors
 Context.batch_dd_psr_pair_list = _batch_dd_psr_pair_list
 Context.eval_dd_psr_factors = _eval_dd_psr_factors
 Context.batch_use_dd_psr_factors = _batch_use_dd_psr_factors
+
+
+# ---------------------------------------------------------------------------------------------------
+# the batch refinement's IMU factors (K2i): ImuFactor from the caller's pre-integration
+# ---------------------------------------------------------------------------------------------------
+IMU_MAX_KF = 1 << 22                      # keyframe indices of an IMU factor are below this (GLIO_IMU_MAX_KF)
+# glio_imu_factor: i, j, active, reserved (int32), then float64: sum_dt, g_vec, delta_p, delta_q (w, x, y, z), delta_v,
+# linearized_ba, linearized_bg, the jacobian_ blocks dp_dba, dp_dbg, dq_dbg, dv_dba, dv_dbg (3 x 3) and sqrt_info (15 x 15), row-major
+IMU_FACTOR_DTYPE = np.dtype([("i", "<i4"), ("j", "<i4"), ("active", "<i4"), ("reserved", "<i4"), ("sum_dt", "<f8"), ("g_vec", "<f8", (3,)),
+                             ("delta_p", "<f8", (3,)), ("delta_q", "<f8", (4,)), ("delta_v", "<f8", (3,)),
+                             ("linearized_ba", "<f8", (3,)), ("linearized_bg", "<f8", (3,)),
+                             ("dp_dba", "<f8", (3, 3)), ("dp_dbg", "<f8", (3, 3)), ("dq_dbg", "<f8", (3, 3)), ("dv_dba", "<f8", (3, 3)),
+                             ("dv_dbg", "<f8", (3, 3)), ("sqrt_info", "<f8", (15, 15))])
+assert IMU_FACTOR_DTYPE.itemsize == 2336
+
+
+def imu_factor_records(i, j, sum_dt, g_vec, delta_p, delta_q, delta_v, linearized_ba, linearized_bg, dp_dba, dp_dbg, dq_dbg, dv_dba,
+                       dv_dbg, sqrt_info, active=None):
+    """A glio_imu_factor array from per-factor columns (g_vec may be one vector for all; active defaults to 1)."""
+    n = len(i)
+    f = np.zeros(n, IMU_FACTOR_DTYPE)
+    f["i"], f["j"], f["sum_dt"] = i, j, sum_dt
+    f["g_vec"] = np.broadcast_to(np.asarray(g_vec, np.float64), (n, 3))
+    for name, val, shape in (("delta_p", delta_p, (3,)), ("delta_q", delta_q, (4,)), ("delta_v", delta_v, (3,)),
+                             ("linearized_ba", linearized_ba, (3,)), ("linearized_bg", linearized_bg, (3,)), ("dp_dba", dp_dba, (3, 3)),
+                             ("dp_dbg", dp_dbg, (3, 3)), ("dq_dbg", dq_dbg, (3, 3)), ("dv_dba", dv_dba, (3, 3)), ("dv_dbg", dv_dbg, (3, 3)),
+                             ("sqrt_info", sqrt_info, (15, 15))):
+        f[name] = np.asarray(val, np.float64).reshape((n,) + shape)
+    f["active"] = 1 if active is None else np.asarray(active, np.int32)
+    return f
+
+
+def _batch_set_imu_factors(self, factors):
+    """glio_batch_set_imu_factors: replace the IMU list (an IMU_FACTOR_DTYPE array; empty empties it)."""
+    f = np.ascontiguousarray(factors, IMU_FACTOR_DTYPE)
+    self._chk(self._lib.glio_batch_set_imu_factors(self._h, _ptr(f) if len(f) else None, C.c_int64(len(f))))
+
+
+def _batch_imu_pair_list(self):
+    """The IMU pair table (a, b), a < b, in order of first appearance."""
+    return _pair_table(self, self._lib.glio_batch_imu_pair_list)
+
+
+def _eval_imu_factors(self, poses, speed_bias, want_jac=True):
+    """glio_eval_imu_factors: the IMU blocks alone at poses (K, 7) and speed_bias (K, 9): Hdiag (K,15,15), Hoff (P,15,15) in
+    IMU-pair order (d2 cost / d x_a d x_b, rows for a) and g (K,15) (None without want_jac), and the cost."""
+    pb = np.ascontiguousarray(poses, np.float64).reshape(-1, 7); K = len(pb)
+    sb = np.ascontiguousarray(speed_bias, np.float64).reshape(K, 9)
+    P = len(_pair_table(self, self._lib.glio_batch_imu_pair_list)[0])
+    Hd = np.zeros((K, 15, 15)) if want_jac else None; Ho = np.zeros((P, 15, 15)) if want_jac else None
+    g = np.zeros((K, 15)) if want_jac else None; cost = np.zeros(1)
+    self._chk(self._lib.glio_eval_imu_factors(self._h, C.c_int(K), _ptr(pb), _ptr(sb), _ptr(Hd), _ptr(Ho), _ptr(g), _ptr(cost)))
+    return dict(Hdiag=Hd, Hoff=Ho, g=g, cost=float(cost[0]))
+
+
+def _batch_use_imu_factors(self, on):
+    """glio_batch_use_imu_factors: batch solves add the IMU blocks (default off; they need speed_bias)."""
+    self._chk(self._lib.glio_batch_use_imu_factors(self._h, C.c_int(1 if on else 0)))
+
+
+Context.batch_set_imu_factors = _batch_set_imu_factors
+Context.batch_imu_pair_list = _batch_imu_pair_list
+Context.eval_imu_factors = _eval_imu_factors
+Context.batch_use_imu_factors = _batch_use_imu_factors
 
 
 # ---------------------------------------------------------------------------------------------------

@@ -183,6 +183,10 @@ struct glio_ctx {
   // DD pseudorange factors (glio_batch_set_dd_psr_factors, K2g): the list, its active records, and the list's satellites, weights
   // and frame constants
   PairFactorList dd; DevBuf<DdPsrFactor> d_dd_f; DevBuf<DdPsrSat> d_dd_sats; DevBuf<double> d_dd_w; DdPsrFrame dd_frame{};
+  // IMU factors (glio_batch_set_imu_factors, K2i): the list and its active records; the speed-bias states of an evaluation and the
+  // IMU blocks (K x 241 and n_imu_pairs x 225), kept apart from the 6-column buffers above
+  PairFactorList imu; DevBuf<ImuFactor> d_imu_f;
+  DevBuf<double> d_imu_sb, d_imu_diag, d_imu_off; PinnedBuf<double> h_imu_sb, h_imu_diag, h_imu_off;
 
   // association workspace
   DevBuf<float4> w_pm, w_pmq, w_nsd;
@@ -1720,7 +1724,7 @@ int glio_batch_clear(glio_ctx* c) {
   return guarded(c, [&] {
     GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
     c->frames.clear(); c->pairs.clear(); c->pair_index.clear(); c->bin_dirty = true; c->bedge_dirty = true;
-    c->pose.clear(); c->dd.clear();
+    c->pose.clear(); c->dd.clear(); c->imu.clear();
   });
 }
 
@@ -2364,6 +2368,31 @@ int eval_blocks_out(glio_ctx* c, const char* who, int K, const double* poses, Bi
   });
 }
 
+// Device evaluation of the IMU blocks -> c->h_imu_diag (K x 241), c->h_imu_off (n_imu_pairs x 225), at the poses already queued
+// into c->d_bin_poses and speed_bias, which is queued here.  The IMU buffers are summed over the ranks of a sharded run after
+// whatever the caller queued before, one call per buffer.  Queued only; a synchronisation of the stream makes the result visible.
+// Returns the off-diagonal block count.
+int imu_blocks_launch(glio_ctx* c, int K, const double* speed_bias, bool want_jac) {
+  const int Pi = (int)c->imu.pairs.size();
+  c->d_imu_sb.reserve((size_t)K * 9); c->h_imu_sb.reserve((size_t)K * 9);
+  c->d_imu_diag.reserve((size_t)K * GLIO_NACC_IMU_KF); c->h_imu_diag.reserve((size_t)K * GLIO_NACC_IMU_KF);
+  c->d_imu_off.reserve((size_t)(Pi + 1) * 225); c->h_imu_off.reserve((size_t)(Pi + 1) * 225);
+  memcpy(c->h_imu_sb.p, speed_bias, (size_t)K * 9 * sizeof(double));
+  GLIO_CUDA_TRY(cudaMemcpyAsync(c->d_imu_sb.p, c->h_imu_sb.p, (size_t)K * 9 * sizeof(double), cudaMemcpyHostToDevice, c->st));
+  eval_imu_run(c->d_imu_f.p, c->imu.d_fstart.p, Pi, K, c->imu.max_kf + 1, c->imu.d_inc_start.p, c->imu.d_inc.p, c->d_bin_poses.p,
+               c->d_imu_sb.p, want_jac, c->imu.d_sums.p, c->d_imu_diag.p, c->d_imu_off.p, c->st, c->lc);
+  if (c->allreduce) {
+    GLIO_REQUIRE(c->allreduce(c->allreduce_user, c->d_imu_diag.p, (int64_t)K * GLIO_NACC_IMU_KF, (void*)c->st) == 0, GLIO_ERR_NCCL,
+                 "allreduce hook failed (IMU diag)");
+    if (want_jac && Pi > 0)
+      GLIO_REQUIRE(c->allreduce(c->allreduce_user, c->d_imu_off.p, (int64_t)Pi * 225, (void*)c->st) == 0, GLIO_ERR_NCCL,
+                   "allreduce hook failed (IMU off)");
+  }
+  GLIO_CUDA_TRY(cudaMemcpyAsync(c->h_imu_diag.p, c->d_imu_diag.p, (size_t)K * GLIO_NACC_IMU_KF * sizeof(double), cudaMemcpyDeviceToHost, c->st));
+  if (want_jac && Pi > 0) GLIO_CUDA_TRY(cudaMemcpyAsync(c->h_imu_off.p, c->d_imu_off.p, (size_t)Pi * 225 * sizeof(double), cudaMemcpyDeviceToHost, c->st));
+  return Pi;
+}
+
 // The pair plan of a factor list with keyframes i, j and an active flag (pose and DD factors): the distinct unordered pairs
 // (a, b), a < b, in order of first appearance; the active factors' list positions grouped by pair, list order inside a pair
 // (order[fstart[p] .. fstart[p+1])); per keyframe 0 .. max_kf its pairs in table order (role 0 = a, 1 = b), by a counting sort.
@@ -2528,6 +2557,64 @@ int glio_batch_use_dd_psr_factors(glio_ctx* c, int on) {
   return GLIO_OK;
 }
 
+static_assert(sizeof(glio_imu_factor) == sizeof(ImuFactor) && offsetof(glio_imu_factor, sum_dt) == offsetof(ImuFactor, sum_dt) &&
+              offsetof(glio_imu_factor, delta_q) == offsetof(ImuFactor, delta_q) && offsetof(glio_imu_factor, dp_dba) == offsetof(ImuFactor, dp_dba) &&
+              offsetof(glio_imu_factor, dv_dbg) == offsetof(ImuFactor, dv_dbg) && offsetof(glio_imu_factor, sqrt_info) == offsetof(ImuFactor, sqrt_info),
+              "ImuFactor must have glio_imu_factor's layout");
+
+int glio_batch_set_imu_factors(glio_ctx* c, const glio_imu_factor* f, int64_t n) {
+  if (!c) return GLIO_ERR_ARG;
+  return guarded(c, [&] {
+    // validate the whole list first: a refused call leaves the previous list in place
+    GLIO_REQUIRE(n >= 0 && (n == 0 || f), GLIO_ERR_ARG, "glio_batch_set_imu_factors: null factor array");
+    GLIO_REQUIRE(n < ((int64_t)1 << 31), GLIO_ERR_ARG, "glio_batch_set_imu_factors: too many factors");
+    constexpr int nd = (int)((sizeof(glio_imu_factor) - offsetof(glio_imu_factor, sum_dt)) / sizeof(double));
+    for (int64_t k = 0; k < n; ++k) {
+      const double* d = &f[k].sum_dt;
+      for (int m = 0; m < nd; ++m) GLIO_REQUIRE(std::isfinite(d[m]), GLIO_ERR_ARG, "glio_batch_set_imu_factors: a non-finite field");
+    }
+    DevBuf<ImuFactor> d_f;
+    PairFactorList l = upload_pair_factors(c, f, n, GLIO_IMU_MAX_KF, GLIO_NACC_IMU,
+                                           "glio_batch_set_imu_factors: need i != j, both in [0, GLIO_IMU_MAX_KF)", d_f);
+    GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));   // also: no evaluation still reads the buffers released below
+    c->d_imu_f = std::move(d_f); c->imu.take(std::move(l));
+  });
+}
+
+int glio_batch_imu_pair_list(glio_ctx* c, int64_t capacity, int32_t* a, int32_t* b, int64_t* n_pairs) {
+  if (!c) return GLIO_ERR_ARG;
+  return guarded(c, [&] { copy_pair_table(c->imu.pairs, capacity, a, b, n_pairs, "glio_batch_imu_pair_list: capacity too small"); });
+}
+
+int glio_eval_imu_factors(glio_ctx* c, int K, const double* poses, const double* speed_bias, double* Hdiag, double* Hoff, double* g,
+                          double* cost) {
+  if (!c) return GLIO_ERR_ARG;
+  return guarded(c, [&] {
+    GLIO_REQUIRE(K > 0 && poses && speed_bias, GLIO_ERR_ARG, "glio_eval_imu_factors: need K > 0, poses and speed_bias");
+    GLIO_REQUIRE(c->imu.max_kf < K, GLIO_ERR_ARG, "glio_eval_imu_factors: an IMU factor references a keyframe outside [0, K)");
+    c->d_bin_poses.reserve((size_t)K * 7); c->h_bin_poses.reserve((size_t)K * 7);
+    memcpy(c->h_bin_poses.p, poses, (size_t)K * 7 * sizeof(double));
+    GLIO_CUDA_TRY(cudaMemcpyAsync(c->d_bin_poses.p, c->h_bin_poses.p, (size_t)K * 7 * sizeof(double), cudaMemcpyHostToDevice, c->st));
+    const int n_off = imu_blocks_launch(c, K, speed_bias, Hdiag || Hoff || g);
+    GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
+    double ct = 0;
+    for (int k = 0; k < K; ++k) {
+      const double* o = c->h_imu_diag.p + (size_t)k * GLIO_NACC_IMU_KF;
+      if (Hdiag) memcpy(Hdiag + (size_t)225 * k, o, 225 * sizeof(double));
+      if (g) memcpy(g + (size_t)15 * k, o + 225, 15 * sizeof(double));
+      ct += o[240];
+    }
+    if (Hoff && n_off > 0) memcpy(Hoff, c->h_imu_off.p, (size_t)n_off * 225 * sizeof(double));
+    if (cost) *cost = ct;
+  });
+}
+
+int glio_batch_use_imu_factors(glio_ctx* c, int on) {
+  if (!c) return GLIO_ERR_ARG;
+  c->imu.use = on != 0;
+  return GLIO_OK;
+}
+
 
 int glio_set_allreduce(glio_ctx* c, glio_allreduce_fn fn, void* user) {
   if (!c) return GLIO_ERR_ARG;
@@ -2582,7 +2669,10 @@ int glio_batch_solve(glio_ctx* c, int K, double* poses, double* speed_bias, glio
     const StateLayout L(K, sb);
     const int nt = L.nt, n = K * nt;
     const bool add_pose = c->pose.use && !c->pose.pairs.empty(), add_dd = c->dd.use && !c->dd.pairs.empty();
+    const bool add_imu = c->imu.use && !c->imu.pairs.empty();
     require_lists_within(c, K, add_pose, add_dd, "glio_batch_solve");
+    GLIO_REQUIRE(!add_imu || sb, GLIO_ERR_ARG, "glio_batch_solve: the IMU factors need speed_bias");
+    GLIO_REQUIRE(!add_imu || c->imu.max_kf < K, GLIO_ERR_ARG, "glio_batch_solve: an IMU factor references a keyframe outside [0, K)");
     // the keyframe pair of each off-diagonal block, in the evaluation's order: LiDAR pairs (cur, oth), then pose pairs (a, b), then
     // DD pairs (a, b)
     std::vector<std::pair<int, int>> off = lidar_pairs(c);
@@ -2590,6 +2680,7 @@ int glio_batch_solve(glio_ctx* c, int K, double* poses, double* speed_bias, glio
     if (add_dd) off.insert(off.end(), c->dd.pairs.begin(), c->dd.pairs.end());
     int span = 1;
     for (const auto& p : off) span = std::max(span, std::abs(p.first - p.second));
+    if (add_imu) for (const auto& p : c->imu.pairs) span = std::max(span, p.second - p.first);
     const int hb = (span + 1) * nt - 1;
     TrustRegionDogleg solver(L.blocks(), solver_options_from(o));
     std::vector<double> x((size_t)K * L.na), pz((size_t)K * 7), sz((size_t)K * 9);
@@ -2599,6 +2690,7 @@ int glio_batch_solve(glio_ctx* c, int K, double* poses, double* speed_bias, glio
       // the device evaluates the LiDAR pairs (and a sharded run sums them over the ranks) while the host evaluates its own
       // factors into the freshly reset band; the device blocks are added when they have arrived
       eval_blocks_launch(c, K, pz.data(), want_jac, c->batch_use_edges ? BIN_PLANES_EDGES : BIN_PLANES, add_pose, add_dd);
+      if (add_imu) imu_blocks_launch(c, K, sz.data(), want_jac);
       double ct = 0;
       int hrc = 0;
       if (want_jac) { H->reset(n, hb); std::fill(g, g + n, 0.0); }
@@ -2620,6 +2712,28 @@ int glio_batch_solve(glio_ctx* c, int K, double* poses, double* speed_bias, glio
             for (int q = 0; q < 6; ++q) { double* row = a + (size_t)(nt * ko + q) * w + (nt * kc - (nt * ko + q) + H->hb); for (int p = 0; p < 6; ++p) row[p] += ob[6 * p + q]; }
           } else {
             for (int p = 0; p < 6; ++p) for (int q = 0; q < 6; ++q) H->add_sym(nt * kc + p, nt * ko + q, ob[6 * p + q]);
+          }
+        }
+      }
+      if (add_imu) {
+        // the IMU blocks after all others: each keyframe's 15 x 15 lower triangle, g and cost, then each pair's (a, b) block,
+        // stored transposed (rows of b, a < b)
+        for (int k = 0; k < K; ++k) ct += c->h_imu_diag.p[(size_t)k * GLIO_NACC_IMU_KF + 240];
+        if (want_jac) {
+          const int w = H->hb + 1;
+          double* a = H->a.data();
+          for (int k = 0; k < K; ++k) {
+            const double* o = c->h_imu_diag.p + (size_t)k * GLIO_NACC_IMU_KF;
+            for (int p = 0; p < 15; ++p) {
+              double* row = a + (size_t)(15 * k + p) * w + (H->hb - p);
+              for (int q = 0; q <= p; ++q) row[q] += o[15 * p + q];
+              g[15 * k + p] += o[225 + p];
+            }
+          }
+          for (size_t pi = 0; pi < c->imu.pairs.size(); ++pi) {
+            const int ka = c->imu.pairs[pi].first, kb = c->imu.pairs[pi].second;
+            const double* ob = c->h_imu_off.p + pi * 225;              // d2 cost / d x_a[p] d x_b[q]
+            for (int q = 0; q < 15; ++q) { double* row = a + (size_t)(15 * kb + q) * w + (15 * ka - (15 * kb + q) + H->hb); for (int p = 0; p < 15; ++p) row[p] += ob[15 * p + q]; }
           }
         }
       }

@@ -383,6 +383,29 @@ void eval_dd_psr_run(const DdPsrFactor* d_f, const int* d_fstart, const DdPsrSat
                      int n_pairs, int K, int n_inc_kf, const int* d_kf_inc_start, const BinIncidence* d_inc, const double* d_poses,
                      bool want_jac, bool add, double* d_sums, double* d_diag, double* d_off, cudaStream_t st, LaunchCounter& lc);
 
+// ---- K2i (eval.cu): the batch refinement's IMU factors (ImuFactor) from the caller's pre-integration; the layout of the public
+// glio_imu_factor.  The 3 x 3 jacobian_ blocks and sqrt_info are row-major.
+struct ImuFactor {
+  int32_t i, j, active, reserved;
+  double sum_dt, g_vec[3];
+  double delta_p[3], delta_q[4], delta_v[3];
+  double linearized_ba[3], linearized_bg[3];
+  double dp_dba[9], dp_dbg[9], dq_dbg[9], dv_dba[9], dv_dbg[9];
+  double sqrt_info[225];
+};
+// Per distinct keyframe pair (a, b), a < b, the sums of its factors' 30 x 30 J^T J, J^T r and cost over the tangent columns
+// (x_a, x_b), x = [t, delta, v, ba, bg]: aa (225), bb (225), ab (225), all row-major, g (15 + 15), cost.
+constexpr int GLIO_NACC_IMU = 706;
+// Per keyframe: its 15 x 15 diagonal block (row-major), g (15) and cost.
+constexpr int GLIO_NACC_IMU_KF = 241;
+// k_imu_pair_sums: the factors of pair p are f[fstart[p] .. fstart[p+1]) in list order, at poses (K x 7) and speed_bias (K x 9)
+// -> d_sums (n_pairs x 706); k_imu_assemble: per keyframe k < n_inc_kf the pairs of its incidence list, in order, written into
+// d_diag (K x 241; the cost goes to a) and, with want_jac, the ab blocks -> d_off (n_pairs x 225).  Two launches whatever K; with
+// n_pairs = 0 only the assembly runs.
+void eval_imu_run(const ImuFactor* d_f, const int* d_fstart, int n_pairs, int K, int n_inc_kf, const int* d_kf_inc_start,
+                  const BinIncidence* d_inc, const double* d_poses, const double* d_sb, bool want_jac, double* d_sums, double* d_diag,
+                  double* d_off, cudaStream_t st, LaunchCounter& lc);
+
 // ---- front-end feature extraction (features.cu; Preprocessing.cpp:529-655)
 constexpr int FEAT_MAX_SHARP = 12, FEAT_MAX_LESS_SHARP = 60, FEAT_MAX_FLAT = 24;   // per ring: 6 sectors x (2, 10, 4)
 struct FeatArgs {

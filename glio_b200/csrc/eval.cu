@@ -947,4 +947,251 @@ void eval_dd_psr_run(const DdPsrFactor* d_f, const int* d_fstart, const DdPsrSat
   GLIO_CUDA_TRY(cudaGetLastError());
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// K2i: the batch refinement's IMU factors (glio_batch_set_imu_factors), as ImuFactor::Evaluate writes them (ImuFactor.h:21-171,
+// the residual of Preintegration::evaluate, Preintegration.h:196-235; blocks P_i, Q_i, SB_i, P_j, Q_j, SB_j), from the caller's
+// pre-integration.  Q_i and Q_j are normalised first; inverse() = conj / |q|^2 and q v are Eigen's; deltaQ(theta) = (1, theta / 2):
+//   dba = Ba_i - lin_ba,  dbg = Bg_i - lin_bg,  cdq = delta_q deltaQ(dq_dbg dbg),  cdv / cdp = delta_v / delta_p + dv_dba / dp_dba dba
+//   + dv_dbg / dp_dbg dbg;  r_P = Q_i^-1 (-g T^2 / 2 + P_j - P_i - V_i T) - cdp,  r_R = 2 vec(normalized(cdq^-1 (Q_i^-1 Q_j))),
+//   r_V = Q_i^-1 (-g T + V_j - V_i) - cdv,  r_BA = Ba_j - Ba_i,  r_BG = Bg_j - Bg_i,  r = sqrt_info r_raw,  cost = |r|^2 / 2.
+// The Jacobian is ImuFactor's analytic one (not the derivative of r): its ambient 15 x 4 quaternion blocks times Ceres'
+// QuaternionParameterization local Jacobian at the unnormalised parameter, [0, e_k] (x) q, then sqrt_info times every column.
+// Layout: one warp per distinct pair (a, b); lane l < 30 owns tangent column l of (x_a, x_b), x = [t, delta, v, ba, bg], walks the
+// pair's factors in list order and keeps row l of the pair's 30 x 30 J^T J and entry l of J^T r in registers; the other columns,
+// and row a of r from lane a, come by shuffle; the lanes' cost shares are summed by one butterfly at the end.  k_imu_assemble then sums each keyframe's pairs in incidence order.  No floating-point atomics.
+// ---------------------------------------------------------------------------------------------------------------
+constexpr int NI = GLIO_NACC_IMU, NIK = GLIO_NACC_IMU_KF;
+constexpr int IMU_T = 128;   // 4 pairs per block
+
+__device__ __forceinline__ void qnormalize(const double q[4], double o[4]) {   // Eigen's normalize(): unchanged when |q|^2 = 0
+  const double n2 = q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3];
+  const double n = n2 > 0.0 ? sqrt(n2) : 1.0;
+#pragma unroll
+  for (int m = 0; m < 4; ++m) o[m] = n2 > 0.0 ? q[m] / n : q[m];
+}
+__device__ __forceinline__ void qinverse(const double q[4], double o[4]) {     // Eigen's inverse(): conj / |q|^2, 0 for q = 0
+  const double n2 = q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3];
+  o[0] = n2 > 0.0 ? q[0] / n2 : 0.0; o[1] = n2 > 0.0 ? -q[1] / n2 : 0.0; o[2] = n2 > 0.0 ? -q[2] / n2 : 0.0; o[3] = n2 > 0.0 ? -q[3] / n2 : 0.0;
+}
+// y = M x for a row-major 3 x 3 M
+__device__ __forceinline__ void mat3v(const double* M, const double x[3], double y[3]) {
+#pragma unroll
+  for (int m = 0; m < 3; ++m) y[m] = M[3 * m] * x[0] + M[3 * m + 1] * x[1] + M[3 * m + 2] * x[2];
+}
+// column e of Eigen's toRotationMatrix() of q
+__device__ __forceinline__ void rotmat_col(const double q[4], int e, double o[3]) {
+  const double tx = 2.0 * q[1], ty = 2.0 * q[2], tz = 2.0 * q[3];
+  const double twx = tx * q[0], twy = ty * q[0], twz = tz * q[0], txx = tx * q[1], txy = ty * q[1], txz = tz * q[1];
+  const double tyy = ty * q[2], tyz = tz * q[2], tzz = tz * q[3];
+  if (e == 0) { o[0] = 1.0 - (tyy + tzz); o[1] = txy + twz; o[2] = txz - twy; }
+  else if (e == 1) { o[0] = txy - twz; o[1] = 1.0 - (txx + tzz); o[2] = tyz + twx; }
+  else { o[0] = txz + twy; o[1] = tyz - twx; o[2] = 1.0 - (txx + tyy); }
+}
+// ImuFactor's P / V rows of the Q_i block along d:  2 (d_w (w t + u x t) + (u.t) d_u + u (t.d_u) - t (u.d_u) - w (t x d_u))
+__device__ __forceinline__ void imu_qi_rows(const double q[4], const double t[3], const double d[4], double o[3]) {
+  const double ut = q[1] * t[0] + q[2] * t[1] + q[3] * t[2], td = t[0] * d[1] + t[1] * d[2] + t[2] * d[3];
+  const double ud = q[1] * d[1] + q[2] * d[2] + q[3] * d[3];
+  const double uxt[3] = {q[2] * t[2] - q[3] * t[1], q[3] * t[0] - q[1] * t[2], q[1] * t[1] - q[2] * t[0]};
+  const double txd[3] = {t[1] * d[3] - t[2] * d[2], t[2] * d[1] - t[0] * d[3], t[0] * d[2] - t[1] * d[1]};
+#pragma unroll
+  for (int m = 0; m < 3; ++m) o[m] = 2.0 * (d[0] * (q[0] * t[m] + uxt[m]) + ut * d[1 + m] + q[1 + m] * td - t[m] * ud - q[0] * txd[m]);
+}
+
+template <bool WANT_JAC>
+__global__ void __launch_bounds__(IMU_T) k_imu_pair_sums(const ImuFactor* __restrict__ fl, const int* __restrict__ fstart, int n_pairs,
+                                                         const double* __restrict__ poses, const double* __restrict__ sb,
+                                                         double* __restrict__ sums) {
+  const int p = blockIdx.x * (IMU_T / 32) + (threadIdx.x >> 5);
+  if (p >= n_pairs) return;                       // a warp leaves as a whole
+  const int l = threadIdx.x & 31, half = l >= 15 ? 1 : 0, comp = l - 15 * half, blk = comp / 3, e = comp - 3 * blk;
+  double H[30], gl = 0.0, cost = 0.0;
+#pragma unroll
+  for (int m = 0; m < 30; ++m) H[m] = 0.0;
+  const int f1 = fstart[p + 1];
+  for (int k = fstart[p]; k < f1; ++k) {
+    const ImuFactor& F = fl[k];
+    const double* Pi = poses + 7 * F.i;
+    const double* Pj = poses + 7 * F.j;
+    const double* Si = sb + 9 * F.i;
+    const double* Sj = sb + 9 * F.j;
+    double qi[4], qj[4], qii[4];
+    { const double a[4] = {Pi[3], Pi[4], Pi[5], Pi[6]}, b[4] = {Pj[3], Pj[4], Pj[5], Pj[6]}; qnormalize(a, qi); qnormalize(b, qj); }
+    qinverse(qi, qii);
+    const double T = F.sum_dt;
+    double dba[3], dbg[3], th[3], ca[3], cb[3];
+#pragma unroll
+    for (int m = 0; m < 3; ++m) { dba[m] = Si[3 + m] - F.linearized_ba[m]; dbg[m] = Si[6 + m] - F.linearized_bg[m]; }
+    mat3v(F.dq_dbg, dbg, th);
+    const double dQ[4] = {1.0, th[0] / 2.0, th[1] / 2.0, th[2] / 2.0};
+    double cdq[4]; qmul(F.delta_q, dQ, cdq);
+    double raw[15], tmp[3], tmp1[3];
+#pragma unroll
+    for (int m = 0; m < 3; ++m) {
+      tmp[m] = -0.5 * F.g_vec[m] * T * T + Pj[m] - Pi[m] - Si[m] * T;
+      tmp1[m] = -F.g_vec[m] * T + Sj[m] - Si[m];
+    }
+    {
+      double rp[3], rv[3];
+      qrot(qii, tmp, rp); qrot(qii, tmp1, rv);
+      mat3v(F.dp_dba, dba, ca); mat3v(F.dp_dbg, dbg, cb);
+#pragma unroll
+      for (int m = 0; m < 3; ++m) raw[m] = rp[m] - (F.delta_p[m] + ca[m] + cb[m]);
+      mat3v(F.dv_dba, dba, ca); mat3v(F.dv_dbg, dbg, cb);
+#pragma unroll
+      for (int m = 0; m < 3; ++m) raw[6 + m] = rv[m] - (F.delta_v[m] + ca[m] + cb[m]);
+      double cinv[4], qij[4], E[4], En[4];
+      qinverse(cdq, cinv); qmul(qii, qj, qij); qmul(cinv, qij, E); qnormalize(E, En);
+#pragma unroll
+      for (int m = 0; m < 3; ++m) {
+        raw[3 + m] = 2.0 * En[1 + m];
+        raw[9 + m] = Sj[3 + m] - Si[3 + m];
+        raw[12 + m] = Sj[6 + m] - Si[6 + m];
+      }
+    }
+    // lane l < 15 owns row l of r = sqrt_info r_raw (the other rows come by shuffle); its cost share is summed over the lanes
+    // once, at the end
+    double rl = 0.0;
+    if (l < 15) {
+#pragma unroll
+      for (int b = 0; b < 15; ++b) rl += F.sqrt_info[15 * l + b] * raw[b];
+    }
+    cost += 0.5 * (rl * rl);
+    if (WANT_JAC) {
+      double u[15];   // column l of the Jacobian before sqrt_info
+#pragma unroll
+      for (int m = 0; m < 15; ++m) u[m] = 0.0;
+      const bool is_i = (half == 0) == (F.i < F.j);
+      if (l < 30) {
+        if (blk == 0 || blk == 2) {                                  // t, v: columns of +-R(Q_i^-1) (times T for v in the P rows)
+          double c3[3]; rotmat_col(qii, e, c3);
+          const double s = is_i ? -1.0 : 1.0;
+#pragma unroll
+          for (int m = 0; m < 3; ++m) {
+            if (blk == 0) u[m] = s * c3[m];
+            else if (is_i) { u[m] = -c3[m] * T; u[6 + m] = -c3[m]; }
+            else u[6 + m] = c3[m];
+          }
+        } else if (blk == 1) {                                       // delta: the ambient block along [0, e_k] (x) q
+          const double* qr = is_i ? Pi + 3 : Pj + 3;
+          const double w = qr[0], x = qr[1], y = qr[2], z = qr[3];
+          const double d[4] = {e == 0 ? -x : e == 1 ? -y : -z, e == 0 ? w : e == 1 ? z : -y,
+                               e == 0 ? -z : e == 1 ? w : x, e == 0 ? y : e == 1 ? -x : w};
+          double t4[4], o4[4];
+          if (is_i) {
+            imu_qi_rows(qi, tmp, d, u); imu_qi_rows(qi, tmp1, d, u + 6);
+            double qji[4]; qinverse(qj, qji);
+            qmul(d, cdq, t4); qmul(qji, t4, o4);                     // Qleft(Q_j^-1) Qright(cdq) d
+#pragma unroll
+            for (int m = 0; m < 3; ++m) u[3 + m] = -2.0 * o4[1 + m];
+          } else {
+            double cinv[4]; qinverse(cdq, cinv); qmul(cinv, qii, t4); qmul(t4, d, o4);   // Qleft(cdq^-1 Q_i^-1) d
+#pragma unroll
+            for (int m = 0; m < 3; ++m) u[3 + m] = 2.0 * o4[1 + m];
+          }
+        } else if (blk == 3) {                                       // ba
+          if (is_i) {
+#pragma unroll
+            for (int m = 0; m < 3; ++m) { u[m] = -F.dp_dba[3 * m + e]; u[6 + m] = -F.dv_dba[3 * m + e]; }
+            u[9 + e] = -1.0;
+          } else {
+            u[9 + e] = 1.0;
+          }
+        } else {                                                     // bg
+          if (is_i) {
+            double qji[4], t4[4], M[4]; qinverse(qj, qji); qmul(qji, qi, t4); qmul(t4, cdq, M);
+            const double c3[3] = {F.dq_dbg[e], F.dq_dbg[3 + e], F.dq_dbg[6 + e]};
+            // -(w I + [v]x) c:  LeftQuatMatrix's top-left 3 x 3
+            u[3] = -(M[0] * c3[0] + (M[2] * c3[2] - M[3] * c3[1]));
+            u[4] = -(M[0] * c3[1] + (M[3] * c3[0] - M[1] * c3[2]));
+            u[5] = -(M[0] * c3[2] + (M[1] * c3[1] - M[2] * c3[0]));
+#pragma unroll
+            for (int m = 0; m < 3; ++m) { u[m] = -F.dp_dbg[3 * m + e]; u[6 + m] = -F.dv_dbg[3 * m + e]; }
+            u[12 + e] = -1.0;
+          } else {
+            u[12 + e] = 1.0;
+          }
+        }
+      }
+      double c[15];
+#pragma unroll
+      for (int a = 0; a < 15; ++a) {
+        double s = 0.0;
+#pragma unroll
+        for (int b = 0; b < 15; ++b) s += F.sqrt_info[15 * a + b] * u[b];
+        c[a] = s;
+      }
+#pragma unroll
+      for (int a = 0; a < 15; ++a) gl += c[a] * __shfl_sync(0xffffffffu, rl, a);
+#pragma unroll
+      for (int m = 0; m < 30; ++m) {
+        double s = 0.0;
+#pragma unroll
+        for (int a = 0; a < 15; ++a) s += c[a] * __shfl_sync(0xffffffffu, c[a], m);
+        H[m] += s;
+      }
+    }
+  }
+  double* S = sums + (size_t)p * NI;
+  if (WANT_JAC) {
+    if (l < 15) {
+#pragma unroll
+      for (int m = 0; m < 15; ++m) { S[15 * l + m] = H[m]; S[450 + 15 * l + m] = H[15 + m]; }
+    } else if (l < 30) {
+#pragma unroll
+      for (int m = 0; m < 15; ++m) S[225 + 15 * (l - 15) + m] = H[15 + m];
+    }
+    if (l < 30) S[675 + l] = gl;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) cost += __shfl_xor_sync(0xffffffffu, cost, o);
+  if (l == 0) S[705] = cost;
+}
+
+// thread t < K*241: diag entry (kf, e) from the kf's pairs in incidence order; then, with WANT_JAC, one thread per entry of the
+// n_pairs ab blocks
+template <bool WANT_JAC>
+__global__ void __launch_bounds__(256) k_imu_assemble(const double* __restrict__ S, int K, int n_pairs, int n_inc_kf,
+                                                      const int* __restrict__ kf_inc_start, const BinIncidence* __restrict__ inc,
+                                                      double* __restrict__ diag, double* __restrict__ off) {
+  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const int64_t nd = (int64_t)K * NIK;
+  if (t < nd) {
+    const int kf = (int)(t / NIK), e = (int)(t - (int64_t)kf * NIK);
+    double v = 0.0;
+    if (kf < n_inc_kf && (WANT_JAC || e == 240)) {
+      for (int i = kf_inc_start[kf]; i < kf_inc_start[kf + 1]; ++i) {
+        const double* s = S + (size_t)inc[i].pair * NI;
+        const int role = inc[i].role;
+        if (e < 225) v += s[225 * role + e];                     // aa | bb
+        else if (e < 240) v += s[675 + 15 * role + (e - 225)];  // g_a | g_b
+        else if (role == 0) v += s[705];                        // the cost goes to a
+      }
+    }
+    diag[t] = v;
+  } else if (WANT_JAC) {
+    const int64_t o = t - nd;
+    if (o < (int64_t)n_pairs * 225) {
+      const int64_t pr = o / 225;
+      off[o] = S[pr * NI + 450 + (o - pr * 225)];
+    }
+  }
+}
+
+void eval_imu_run(const ImuFactor* d_f, const int* d_fstart, int n_pairs, int K, int n_inc_kf, const int* d_kf_inc_start,
+                  const BinIncidence* d_inc, const double* d_poses, const double* d_sb, bool want_jac, double* d_sums, double* d_diag,
+                  double* d_off, cudaStream_t st, LaunchCounter& lc) {
+  if (n_pairs > 0) {
+    const int nb = (n_pairs + IMU_T / 32 - 1) / (IMU_T / 32);
+    lc.begin(want_jac ? "k_imu_pair_sums" : "k_imu_pair_sums_cost", st);
+    (want_jac ? k_imu_pair_sums<true> : k_imu_pair_sums<false>)<<<nb, IMU_T, 0, st>>>(d_f, d_fstart, n_pairs, d_poses, d_sb, d_sums);
+    lc.end(st);
+  }
+  const int64_t n = (int64_t)K * NIK + (want_jac ? (int64_t)n_pairs * 225 : 0);
+  lc.begin("k_imu_assemble", st);
+  (want_jac ? k_imu_assemble<true> : k_imu_assemble<false>)<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(
+      d_sums, K, n_pairs, n_inc_kf, d_kf_inc_start, d_inc, d_diag, d_off);
+  lc.end(st);
+  GLIO_CUDA_TRY(cudaGetLastError());
+}
+
 }  // namespace glio

@@ -313,6 +313,77 @@ def pose_graph_problem(K=200, seed=SEED0 + 16, search_range=6, level=0, sig_t=0.
 
 
 # ---------------------------------------------------------------------------------------------------------------------------
+# IMU factors of the batch refinement at sms_fusion_level 1 (ImuFactor between consecutive keyframes, Estimator.cpp:2993-3001)
+# ---------------------------------------------------------------------------------------------------------------------------
+IMU_GRAVITY = np.array([0.0, 0.0, 9.81])
+
+
+def _skew(v):
+    return np.array([[0.0, -v[2], v[1]], [v[2], 0.0, -v[0]], [-v[1], v[0], 0.0]])
+
+
+def imu_problem(K=200, seed=SEED0 + 18, search_range=6, sig_p=0.02, sig_r=0.005, sig_v=0.03, sig_ba=0.02, sig_bg=0.002):
+    """A level-1-shaped batch problem with IMU factors.  This is generated data, not a pre-integration: no IMU samples are
+    integrated.  pose_graph_problem(level=1)'s trajectory, attitude factors and LiDAR pairs; keyframe times 0.25 .. 0.45 s apart
+    (as in dd_psr_problem); true velocities (central differences of the positions over the times) and slowly drifting biases
+    (sb_true, K x 9: V, Ba, Bg); perturbed initial speed-bias states (sb_init).  One factor per consecutive pair (k, k+1), in
+    order, with T = t_{k+1} - t_k, g = IMU_GRAVITY, linearisation biases off the truth by a little (so Bg_i != linearized_bg),
+    first-order jacobian_ blocks (dp_dba = -T^2/2 I, dv_dba = -T I, dq_dbg = -T I, dp_dbg and dv_dbg of the order of T^2 and T
+    times a small random rotation term), and deltas chosen so that the raw residual at the truth is N(0, sigma) noise.  The
+    covariance is diag(sigma^2) with mild correlations (SPD), and sqrt_info = LLT(covariance^-1).matrixL()^T as ImuFactor forms it.
+    Adds kf_times, sb_true, sb_init, cov (n x 15 x 15) and imu (the factor columns of api.imu_factor_records)."""
+    P = pose_graph_problem(K=K, seed=seed, search_range=search_range, level=1)
+    rng = np.random.default_rng([seed, 2])
+    kf_times = 1_600_000_000.0 + np.concatenate([[0.0], np.cumsum(rng.uniform(0.25, 0.45, K - 1))])
+    T = P["poses_true"]
+    V = np.gradient(T[:, :3], kf_times, axis=0) if K > 1 else np.zeros((K, 3))
+    ba = np.array([0.05, -0.03, 0.02]) + np.cumsum(rng.normal(0.0, 1e-4, (K, 3)), axis=0)
+    bg = np.array([0.002, -0.001, 0.0015]) + np.cumsum(rng.normal(0.0, 1e-5, (K, 3)), axis=0)
+    sb_true = np.concatenate([V, ba, bg], axis=1)
+    sb_init = sb_true + np.concatenate([rng.normal(0.0, 0.1, (K, 3)), rng.normal(0.0, 0.01, (K, 3)), rng.normal(0.0, 1e-3, (K, 3))], axis=1)
+    n = K - 1
+    sig = np.concatenate([np.full(3, sig_p), np.full(3, sig_r), np.full(3, sig_v), np.full(3, sig_ba), np.full(3, sig_bg)])
+    cols = {k: [] for k in ("i", "j", "sum_dt", "delta_p", "delta_q", "delta_v", "linearized_ba", "linearized_bg", "dp_dba", "dp_dbg",
+                            "dq_dbg", "dv_dba", "dv_dbg", "sqrt_info")}
+    covs = []
+    g = IMU_GRAVITY
+    for k in range(n):
+        i, j = k, k + 1
+        dt = kf_times[j] - kf_times[i]
+        qi, qj = T[i, 3:], T[j, 3:]
+        Ri = quat_to_R(qi)
+        lin_ba = ba[i] + rng.normal(0.0, 0.005, 3); lin_bg = bg[i] + rng.normal(0.0, 5e-4, 3)
+        dp_dba = -0.5 * dt * dt * np.eye(3); dv_dba = -dt * np.eye(3); dq_dbg = -dt * np.eye(3)
+        dp_dbg = dt * dt * _skew(rng.normal(0.0, 0.3, 3)); dv_dbg = dt * _skew(rng.normal(0.0, 0.5, 3))
+        dba, dbg = ba[i] - lin_ba, bg[i] - lin_bg
+        e = rng.normal(0.0, 1.0, 15) * sig
+        dp = Ri.T @ (-0.5 * g * dt * dt + T[j, :3] - T[i, :3] - V[i] * dt) - dp_dba @ dba - dp_dbg @ dbg + e[:3]
+        dv = Ri.T @ (-g * dt + V[j] - V[i]) - dv_dba @ dba - dv_dbg @ dbg + e[6:9]
+        # delta_q deltaQ(dq_dbg dbg) = q_i^-1 q_j (x) exp(e_R / 2) up to normalisation
+        dQ = np.concatenate([[1.0], 0.5 * (dq_dbg @ dbg)])
+        target = quat_mul(quat_mul(quat_conj(qi), qj), quat_from_rotvec(e[3:6]))
+        dq = quat_mul(target, quat_conj(dQ) / np.dot(dQ, dQ))
+        dq /= np.linalg.norm(dq)
+        C = rng.normal(0.0, 0.1, (15, 15)); C = 0.5 * (C + C.T); np.fill_diagonal(C, 1.0)
+        w, U = np.linalg.eigh(C); C = U @ np.diag(np.maximum(w, 0.2)) @ U.T
+        d = np.sqrt(np.diag(C)); C = C / np.outer(d, d)
+        cov = np.outer(sig, sig) * C
+        L = np.linalg.cholesky(np.linalg.inv(cov))
+        for name, val in (("i", i), ("j", j), ("sum_dt", dt), ("delta_p", dp), ("delta_q", dq), ("delta_v", dv), ("linearized_ba", lin_ba),
+                          ("linearized_bg", lin_bg), ("dp_dba", dp_dba), ("dp_dbg", dp_dbg), ("dq_dbg", dq_dbg), ("dv_dba", dv_dba),
+                          ("dv_dbg", dv_dbg), ("sqrt_info", L.T)):
+            cols[name].append(val)
+        covs.append(cov)
+    imu = {k: np.asarray(v, np.int32 if k in ("i", "j") else np.float64) for k, v in cols.items()}
+    for k, shape in (("delta_p", (3,)), ("delta_q", (4,)), ("delta_v", (3,)), ("linearized_ba", (3,)), ("linearized_bg", (3,)),
+                     ("dp_dba", (3, 3)), ("dp_dbg", (3, 3)), ("dq_dbg", (3, 3)), ("dv_dba", (3, 3)), ("dv_dbg", (3, 3)), ("sqrt_info", (15, 15))):
+        imu[k] = imu[k].reshape((n,) + shape)
+    imu["g_vec"] = np.broadcast_to(g, (n, 3)).copy()
+    P.update(kf_times=kf_times, sb_true=sb_true, sb_init=sb_init, cov=np.asarray(covs).reshape(n, 15, 15), imu=imu)
+    return P
+
+
+# ---------------------------------------------------------------------------------------------------------------------------
 # GNSS double-differenced pseudorange factors of the batch refinement (dd_psr_factor_20, Estimator.cpp:3086-3272)
 # ---------------------------------------------------------------------------------------------------------------------------
 WGS84_A, WGS84_E2 = 6378137.0, 6.69437999014e-3            # gnss_constant.hpp: EARTH_SEMI_MAJOR, EARTH_ECCE_2

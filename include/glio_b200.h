@@ -621,8 +621,8 @@ int glio_batch_select_random(glio_ctx* ctx, const int32_t* cur, const int32_t* o
                              const glio_select_options* options, int64_t* n_active);
 int glio_batch_get_selection(glio_ctx* ctx, int cur, int oth, int64_t capacity, int32_t* keep, int64_t* n);
 int glio_batch_pair_list(glio_ctx* ctx, int64_t capacity, int32_t* cur, int32_t* oth, int64_t* n_pairs);
-int glio_batch_clear(glio_ctx* ctx);   /* also empties the pose-factor and DD-pseudorange lists (glio_batch_set_pose_factors,
-                                          glio_batch_set_dd_psr_factors) */
+int glio_batch_clear(glio_ctx* ctx);   /* also empties the pose-factor, DD-pseudorange and IMU lists (glio_batch_set_pose_factors,
+                                          glio_batch_set_dd_psr_factors, glio_batch_set_imu_factors) */
 
 /* Creates (empty) pair entries in the given order without associating them: on a keyframe-sharded multi-GPU run
  * every rank declares the SAME global pair list and then associates only the pairs it owns, so the block
@@ -847,6 +847,54 @@ int glio_eval_dd_psr_factors(glio_ctx* ctx, int K, const double* poses, double* 
  * glio_eval_binary_edge and glio_eval_pose_factors never add DD blocks. */
 int glio_batch_use_dd_psr_factors(glio_ctx* ctx, int on);
 
+/* ---- K2i: the batch refinement's IMU factors (ImuFactor between consecutive keyframes at sms_fusion_level 1,
+ * Estimator.cpp:2993-3001), evaluated on the device from the caller's pre-integration: the library integrates no IMU samples
+ * and inverts no covariance.  Per factor, with T = sum_dt, g = g_vec, Q_i and Q_j normalised (Eigen's normalize()), q^-1 =
+ * conj(q) / |q|^2, q v Eigen's rotation, deltaQ(theta) = (1, theta / 2) (not normalised), and the speed-bias state
+ * SB = [V(3), Ba(3), Bg(3)]:
+ *   dba = Ba_i - linearized_ba,  dbg = Bg_i - linearized_bg,  cdq = delta_q deltaQ(dq_dbg dbg)
+ *   cdp = delta_p + dp_dba dba + dp_dbg dbg,  cdv = delta_v + dv_dba dba + dv_dbg dbg
+ *   r_P = Q_i^-1 (-g T^2 / 2 + P_j - P_i - V_i T) - cdp,  r_R = 2 vec(normalized(cdq^-1 (Q_i^-1 Q_j)))
+ *   r_V = Q_i^-1 (-g T + V_j - V_i) - cdv,  r_BA = Ba_j - Ba_i,  r_BG = Bg_j - Bg_i
+ *   r = sqrt_info r_raw,  cost = |r|^2 / 2 (no loss function)
+ * The Jacobian is ImuFactor's analytic one, which is not the exact derivative of r (its rotation rows, its bias columns and the
+ * missing normalisation term are kept as written), each column multiplied by sqrt_info.  The quaternion columns are its ambient
+ * 15 x 4 blocks times Ceres' QuaternionParameterization local Jacobian at the unnormalised parameter q.  Tangent order per
+ * keyframe: [t(3), delta(3), v(3), ba(3), bg(3)], glio_batch_solve's 15 columns with speed-bias.  active = 0: as for the pose
+ * factors, the factor makes its pair entry but is not evaluated here.  sqrt_info is what ImuFactor forms from the covariance,
+ * LLT(covariance.inverse()).matrixL().transpose(); the jacobian_ blocks and sqrt_info are row-major. */
+enum { GLIO_IMU_MAX_KF = 1 << 22 };
+typedef struct {
+  int32_t i, j, active, reserved;                 /* reserved: 0 */
+  double sum_dt, g_vec[3];
+  double delta_p[3], delta_q[4] /* w,x,y,z */, delta_v[3];
+  double linearized_ba[3], linearized_bg[3];
+  double dp_dba[9], dp_dbg[9], dq_dbg[9], dv_dba[9], dv_dbg[9];
+  double sqrt_info[225];
+} glio_imu_factor;
+/* Replaces the IMU list (n = 0 empties it; glio_batch_clear empties it too).  The whole list is checked first: i != j, both in
+ * [0, GLIO_IMU_MAX_KF), every double finite, f given when n > 0; a refused call (GLIO_ERR_ARG) leaves the previous list in place.
+ * The distinct unordered pairs (a, b), a = min(i, j) < b, form the IMU pair table in order of first appearance.  The list is
+ * copied to device buffers allocated here; the context takes them only once complete, so a call that fails for any reason leaves
+ * the previous list in place.  Evaluations allocate nothing for it. */
+int glio_batch_set_imu_factors(glio_ctx* ctx, const glio_imu_factor* f, int64_t n);
+/* the IMU pair table (a[k] < b[k]), glio_batch_pair_list's conventions: NULL arrays only count */
+int glio_batch_imu_pair_list(glio_ctx* ctx, int64_t capacity, int32_t* a, int32_t* b, int64_t* n_pairs);
+/* The IMU blocks alone, for the active factors, at poses[K*7] and speed_bias[K*9] (both required): Hdiag[K*225] (per keyframe
+ * 15 x 15, row-major), Hoff[n_imu_pairs*225] (block k = d2 cost / d x_a d x_b of IMU pair k, rows for a), g[K*15], cost
+ * (attributed to a); NULL outputs are skipped and without Hdiag, Hoff and g only the cost is formed.  Per pair the factors are
+ * summed in list order, per keyframe the pairs in table order.  With the all-reduce hook set, the K x 241 (Hdiag, g, cost) and
+ * n_imu_pairs x 225 buffers are summed over the ranks.  A list that references a keyframe >= K is GLIO_ERR_ARG. */
+int glio_eval_imu_factors(glio_ctx* ctx, int K, const double* poses, const double* speed_bias, double* Hdiag, double* Hoff, double* g,
+                          double* cost);
+/* on != 0: every evaluation inside glio_batch_solve adds the IMU blocks of the active factors into the 15-column band, after the
+ * LiDAR, pose and DD blocks.  The speed-bias states are uploaded with the poses at every evaluation; a sharded run sums the IMU
+ * buffers (K x 241, then n_imu_pairs x 225) after the others, one call per buffer.  The band's half bandwidth covers the IMU pairs'
+ * span, and the solve works with no LiDAR pair.  Default off; with the switch off or an empty list glio_batch_solve launches what it
+ * launches without IMU factors.  With the switch on and a non-empty list, speed_bias == NULL or a list that references a keyframe
+ * >= K makes glio_batch_solve return GLIO_ERR_ARG.  The other glio_eval_* calls never add IMU blocks. */
+int glio_batch_use_imu_factors(glio_ctx* ctx, int on);
+
 /* ---- seeded device selection of EDGE correspondences.  The reference selects plane matches only; this library applies the same
  * rules and the same sampler (glio_select_random / glio_batch_select_random, k_sel_sample) to edge lists, with the sizes of a
  * glio_select_options passed to these calls, so edge sizes are set independently of plane sizes:
@@ -880,7 +928,7 @@ int glio_batch_get_edge_selection(glio_ctx* ctx, int cur, int oth, int64_t capac
  * nonmonotonic steps, max_num_iter iterations; options == NULL selects exactly those).  The normal equations are
  * block-banded (half bandwidth (max|cur-oth|+1)*nt - 1) and stored/factored in band form.  Host factors (IMU chain, prior;
  * the pose factors run on the device through glio_batch_use_pose_factors, the DD pseudorange factors through
- * glio_batch_use_dd_psr_factors) accumulate into the same LOWER-BAND storage:
+ * glio_batch_use_dd_psr_factors, the IMU factors through glio_batch_use_imu_factors) accumulate into the same LOWER-BAND storage:
  * entry (i,j), i-hb <= j <= i, lives at Hband[i*(hb+1) + (j-i+hb)]. */
 int glio_hf_evaluate_band(void* user, int K, const double* poses, const double* speed_bias, int want_jac, double* Hband, int hb,
                           double* g, double* cost);
