@@ -14,15 +14,17 @@
 // they are uploaded once to a glio_ctx and evaluated by the CUDA kernels, which return 6x6 pose blocks: K2 for the plane
 // factors (LidarPlaneNormFactor, and LidarPlaneNormIncreFactor in a front-end context), K2e for LidarEdgeFactor, K2b for
 // BinaryLidarPlaneNormFactor, K2p for the batch refinement's pose factors (LidarPoseFactorBatchRelativeAutoDiff,
-// delta_q_factor_auto), and K2g for its GNSS double-differenced pseudorange factor dd_psr_factor_20, a SizedCostFunction
-// that describes itself through glio::DeviceCostTraits<Cost>, looked up by the static type AddResidualBlock is given.
-// Every other cost function (IMU, marginalisation prior, the window's GNSS factors ...) is evaluated on the host through its
-// own Evaluate(), exactly as Ceres would.  Without a glio_ctx attached everything runs on the host (used by CPU tests).
+// delta_q_factor_auto), K2g for its GNSS double-differenced pseudorange factor dd_psr_factor_20 and K2i for its IMU factor
+// ImuFactor: SizedCostFunctions that describe themselves through glio::DeviceCostTraits<Cost>, looked up by the static type
+// AddResidualBlock is given.  Every other cost function (marginalisation prior, the window's GNSS factors, speed-bias priors
+// ...) is evaluated on the host through its own Evaluate(), exactly as Ceres would.  Without a glio_ctx attached everything
+// runs on the host (used by CPU tests).
 #ifndef GLIO_SHIM_CERES_CERES_H_
 #define GLIO_SHIM_CERES_CERES_H_
 
 #include <algorithm>
 #include <cmath>
+#include <cstddef>
 #include <cstdint>
 #include <cstdio>
 #include <cstring>
@@ -70,26 +72,49 @@ struct DdPsrDesc {
   double W[(GLIO_DD_PSR_MAX_SAT - 1) * (GLIO_DD_PSR_MAX_SAT - 1)];             // the (n_sat-1) x (n_sat-1) weight, row-major
   int w_identity = 0;                 // 1: W is exactly the identity (uploaded as w_offset = -1)
 };
-// Specialise for the cost function's class, next to its header (INTEGRATION.md shows the lines for dd_psr_factor_20):
+// Specialise for the cost function's class, next to its header (INTEGRATION.md shows the lines for dd_psr_factor_20 and
+// ImuFactor).  A specialisation provides one of two kinds of description:
 //   template <> struct glio::DeviceCostTraits<dd_psr_factor_20> {
 //     static bool describe(const dd_psr_factor_20&, DdPsrDesc*);                 // false: the block stays on the host
 //     static void frame(const double* yaw, const double* anchor, double R_ecef_local[9]);   // row-major, the factor's own R
 //   };
-// Problem::AddResidualBlock looks the traits up by the cost function's static type.  The default describes nothing.
+//   template <> struct glio::DeviceCostTraits<ImuFactor> {
+//     static bool describe(const ImuFactor&, glio_imu_factor*);                  // false: the block stays on the host
+//   };
+// The IMU description is K2i's record (glio_imu_factor in glio_b200.h) without i, j and active, which the shim sets: the
+// pre-integrated deltas, the five jacobian_ blocks and sqrt_info, formed on the caller's side from the covariance as the
+// factor forms it.  Problem::AddResidualBlock looks the traits up by the cost function's static type.  The default describes
+// nothing.
 template <class Cost> struct DeviceCostTraits {};
 
-// what AddResidualBlock records for a cost function whose static type has a DeviceCostTraits specialisation
+// what AddResidualBlock records for a cost function whose static type has a DeviceCostTraits specialisation: the calls of its
+// kind, the others NULL
 struct CostDescriber {
-  bool (*describe)(const ceres::CostFunction* cost, DdPsrDesc*);
+  bool (*describe_dd_psr)(const ceres::CostFunction* cost, DdPsrDesc*);
   void (*frame)(const double* yaw, const double* anchor, double R_ecef_local[9]);
+  bool (*describe_imu)(const ceres::CostFunction* cost, glio_imu_factor*);
 };
 namespace detail {
-template <class Cost, class = void> struct HasCostTraits : std::false_type {};
+template <class Cost, class = void> struct HasDdPsrTraits : std::false_type {};
 template <class Cost>
-struct HasCostTraits<Cost, decltype((void)&DeviceCostTraits<Cost>::describe, (void)&DeviceCostTraits<Cost>::frame)> : std::true_type {};
+struct HasDdPsrTraits<Cost, decltype((void)DeviceCostTraits<Cost>::describe(std::declval<const Cost&>(), (DdPsrDesc*)nullptr),
+                                     (void)&DeviceCostTraits<Cost>::frame)> : std::true_type {};
+template <class Cost, class = void> struct HasImuTraits : std::false_type {};
+template <class Cost>
+struct HasImuTraits<Cost, decltype((void)DeviceCostTraits<Cost>::describe(std::declval<const Cost&>(), (glio_imu_factor*)nullptr))>
+    : std::true_type {};
+template <class Cost> struct HasCostTraits : std::integral_constant<bool, HasDdPsrTraits<Cost>::value || HasImuTraits<Cost>::value> {};
+template <class Cost> CostDescriber make_describer(std::true_type /* DD */) {
+  return CostDescriber{[](const ceres::CostFunction* c, DdPsrDesc* out) { return DeviceCostTraits<Cost>::describe(*static_cast<const Cost*>(c), out); },
+                       &DeviceCostTraits<Cost>::frame, nullptr};
+}
+template <class Cost> CostDescriber make_describer(std::false_type /* IMU */) {
+  return CostDescriber{nullptr, nullptr, [](const ceres::CostFunction* c, glio_imu_factor* out) {
+                         return DeviceCostTraits<Cost>::describe(*static_cast<const Cost*>(c), out);
+                       }};
+}
 template <class Cost> const CostDescriber* cost_describer() {
-  static const CostDescriber d{[](const ceres::CostFunction* c, DdPsrDesc* out) { return DeviceCostTraits<Cost>::describe(*static_cast<const Cost*>(c), out); },
-                               &DeviceCostTraits<Cost>::frame};
+  static const CostDescriber d = make_describer<Cost>(HasDdPsrTraits<Cost>());
   return &d;
 }
 }  // namespace detail
@@ -307,6 +332,7 @@ class Solver {
     int num_device_edge_residual_blocks = 0;   // glio extension: the LidarEdgeFactor blocks among them (K2e)
     int num_device_pose_residual_blocks = 0;   // glio extension: the relative-pose and delta_q blocks among them (K2p)
     int num_device_dd_psr_residual_blocks = 0;   // glio extension: the dd_psr_factor_20 blocks among them (K2g)
+    int num_device_imu_residual_blocks = 0;   // glio extension: the ImuFactor blocks among them (K2i)
     bool IsSolutionUsable() const { return termination_type == CONVERGENCE || termination_type == NO_CONVERGENCE || termination_type == USER_SUCCESS; }
     std::string BriefReport() const {
       char b[256];
@@ -371,7 +397,7 @@ class Problem {
   ResidualBlockId AddResidualBlock(CostFunction* cost, LossFunction* loss, double* x0, Ts*... xs) {
     return AddResidual(cost, loss, std::vector<double*>{x0, xs...}, nullptr);
   }
-  // glio extension: a cost function whose static type has a glio::DeviceCostTraits specialisation (dd_psr_factor_20) is
+  // glio extension: a cost function whose static type has a glio::DeviceCostTraits specialisation (dd_psr_factor_20, ImuFactor) is
   // recorded with its describer.  These overloads exist only for such types, so every other call resolves as above; a
   // described cost function passed as a plain CostFunction* is recorded without one and stays on the host.
   template <class Cost, typename std::enable_if<glio::detail::HasCostTraits<Cost>::value, int>::type = 0>

@@ -123,6 +123,10 @@ inline void Solve(const Solver::Options& options, Problem* problem, Solver::Summ
   std::vector<glio_dd_psr_sat> dd_sats;
   std::vector<double> dd_W;
   std::unique_ptr<glio::DdPsrDesc> dd_desc(new glio::DdPsrDesc());
+  // ImuFactor candidates: routed after the DD factors, on the same table, with their descriptions (i, j set there)
+  struct ImuCand { const Problem::Residual* rb; glio_imu_factor f; };
+  std::vector<ImuCand> imu_cands;
+  auto sb_ok = [&](double* sb) { return P.index.count(sb) && problem->blocks_.at(sb).size == 9 && problem->blocks_.at(sb).param == nullptr; };
   for (auto& rbp : problem->residual_blocks_) {
     const Problem::Residual* rb = rbp.get();
     glio::FactorDesc d;
@@ -196,14 +200,14 @@ inline void Solve(const Solver::Options& options, Problem* problem, Solver::Summ
     // dd_psr_factor_20 (dd_psr_factor.hpp, added without a loss at Estimator.cpp:1910): K2g computes exactly its residual when the
     // blocks are (t_i, t_j, yaw, anchor) of sizes (3, 3, 1, 3), both t active plain 3-vectors of different keyframes, yaw and
     // anchor constant, and the description within K2g's limits.  A candidate stays in host_blocks until the keyframe table takes it.
-    if (!dev && ctx && rb->describer && rb->loss == nullptr && rb->params.size() == 4) {
+    if (!dev && ctx && rb->describer && rb->describer->describe_dd_psr && rb->loss == nullptr && rb->params.size() == 4) {
       const std::vector<int32_t>& sz = rb->cost->parameter_block_sizes();
       double* const* b = rb->params.data();
       const bool shape = sz[0] == 3 && sz[1] == 3 && sz[2] == 1 && sz[3] == 3 && problem->blocks_.at(b[2]).size == 1 &&
                          problem->blocks_.at(b[3]).size == 3 && trans_ok(b[0]) && trans_ok(b[1]) && b[0] != b[1] &&
                          !P.index.count(b[2]) && !P.index.count(b[3]);
       if (shape) *dd_desc = glio::DdPsrDesc();
-      if (shape && rb->describer->describe(rb->cost, dd_desc.get()) && dd_desc->n_sat >= 2 && dd_desc->n_sat <= GLIO_DD_PSR_MAX_SAT &&
+      if (shape && rb->describer->describe_dd_psr(rb->cost, dd_desc.get()) && dd_desc->n_sat >= 2 && dd_desc->n_sat <= GLIO_DD_PSR_MAX_SAT &&
           dd_desc->master >= 0 && dd_desc->master < dd_desc->n_sat) {
         const glio::DdPsrDesc& dd = *dd_desc;
         glio_dd_psr_factor f;
@@ -222,6 +226,25 @@ inline void Solve(const Solver::Options& options, Problem* problem, Solver::Summ
         dd_cands.push_back(DdCand{rb, f});
       }
     }
+    // ImuFactor (ImuFactor.h, added without a loss at Estimator.cpp:2993-3001): K2i computes exactly its residual and Jacobian when
+    // the blocks are (t_i, q_i, sb_i, t_j, q_j, sb_j) of sizes (3, 4, 9, 3, 4, 9), all active, each t a plain 3-vector, each q a
+    // QuaternionParameterization and each sb a plain 9-vector, the two keyframes different, and the description finite (K2i's
+    // list takes finite records only).  A candidate stays in host_blocks until the keyframe table takes it.
+    if (!dev && ctx && rb->describer && rb->describer->describe_imu && rb->loss == nullptr && rb->params.size() == 6) {
+      const std::vector<int32_t>& sz = rb->cost->parameter_block_sizes();
+      double* const* b = rb->params.data();
+      const bool shape = sz[0] == 3 && sz[1] == 4 && sz[2] == 9 && sz[3] == 3 && sz[4] == 4 && sz[5] == 9 && trans_ok(b[0]) && quat_ok(b[1]) &&
+                         sb_ok(b[2]) && trans_ok(b[3]) && quat_ok(b[4]) && sb_ok(b[5]) && !(b[0] == b[3] && b[1] == b[4]);
+      glio_imu_factor f;
+      std::memset(&f, 0, sizeof(f));
+      if (shape && rb->describer->describe_imu(rb->cost, &f)) {
+        bool finite = true;
+        const double* v = &f.sum_dt;
+        for (size_t k = 0; k < (sizeof(f) - offsetof(glio_imu_factor, sum_dt)) / sizeof(double); ++k) finite = finite && std::isfinite(v[k]);
+        f.i = f.j = -1; f.active = 1; f.reserved = 0;
+        if (finite) imu_cands.push_back(ImuCand{rb, f});
+      }
+    }
     if (!dev) host_blocks.push_back(rb);
   }
   const int W = (int)slots.size();
@@ -233,12 +256,13 @@ inline void Solve(const Solver::Options& options, Problem* problem, Solver::Summ
   // keyframe: the pose blocks that touch it stay on the host.  So do blocks whose two sides are one keyframe.
   std::vector<glio_pose_factor> pose_list;
   std::map<double*, std::set<double*>> ts_of_q, qs_of_t;
-  std::set<const Problem::Residual*> routed;                     // pose and DD blocks the keyframe table takes off the host
+  std::set<const Problem::Residual*> routed;                     // pose, DD and IMU blocks the keyframe table takes off the host
   {
     auto pairing = [&](double* t, double* q) { ts_of_q[q].insert(t); qs_of_t[t].insert(q); };
     for (const auto& kf : bkfs) pairing(kf.first, kf.second);
     for (const PoseCand& c : pose_cands)
       if (c.d.kind == glio::FACTOR_POSE_RELATIVE) { pairing(c.rb->params[0], c.rb->params[1]); pairing(c.rb->params[2], c.rb->params[3]); }
+    for (const ImuCand& c : imu_cands) { pairing(c.rb->params[0], c.rb->params[1]); pairing(c.rb->params[3], c.rb->params[4]); }
     auto q_single = [&](double* q) {
       auto it = ts_of_q.find(q);
       if (it == ts_of_q.end()) return true;
@@ -294,11 +318,41 @@ inline void Solve(const Solver::Options& options, Problem* problem, Solver::Summ
       routed.insert(c.rb);
     }
   }
+
+  // ---- IMU factors on the same table ----
+  // A keyframe (t, q) whose t pairs with that q alone (and that q with that t alone) takes the IMU blocks whose sb is used by IMU
+  // candidates with that keyframe only, while the keyframe is used with that sb only: then K2i's 15 columns per keyframe are
+  // [t, delta, sb], and the keyframe's sb columns are its own.  Every other IMU candidate stays on the host.
+  std::vector<glio_imu_factor> imu_list;
+  std::vector<double*> bkf_sb;                                   // each batch keyframe's sb block (NULL: none)
+  {
+    std::map<double*, std::set<std::pair<double*, double*>>> kfs_of_sb;
+    std::map<std::pair<double*, double*>, std::set<double*>> sbs_of_kf;
+    for (const ImuCand& c : imu_cands)
+      for (int s = 0; s < 2; ++s) {
+        double* const* b = c.rb->params.data() + 3 * s;
+        kfs_of_sb[b[2]].insert(std::make_pair(b[0], b[1])); sbs_of_kf[std::make_pair(b[0], b[1])].insert(b[2]);
+      }
+    auto side_ok = [&](double* const* b) {
+      return qs_of_t.at(b[0]).size() == 1 && ts_of_q.at(b[1]).size() == 1 && kfs_of_sb.at(b[2]).size() == 1 && sbs_of_kf.at(std::make_pair(b[0], b[1])).size() == 1;
+    };
+    for (const ImuCand& c : imu_cands) {
+      double* const* b = c.rb->params.data();
+      if (!side_ok(b) || !side_ok(b + 3)) continue;
+      glio_imu_factor f = c.f;
+      f.i = kf_index(b[0], b[1]); f.j = kf_index(b[3], b[4]);
+      bkf_sb.resize(bkfs.size(), nullptr);
+      bkf_sb[f.i] = b[2]; bkf_sb[f.j] = b[5];
+      imu_list.push_back(f);
+      routed.insert(c.rb);
+    }
+  }
   if (!routed.empty())
     host_blocks.erase(std::remove_if(host_blocks.begin(), host_blocks.end(), [&](const Problem::Residual* rb) { return routed.count(rb) != 0; }),
                       host_blocks.end());
-  // keyframes of K2b (the first KB), K2p and K2g; routed pose and DD blocks
-  const int KT = (int)bkfs.size(), NP = (int)pose_list.size(), ND = (int)dd_list.size();
+  // keyframes of K2b (the first KB), K2p, K2g and K2i; routed pose, DD and IMU blocks
+  const int KT = (int)bkfs.size(), NP = (int)pose_list.size(), ND = (int)dd_list.size(), NI = (int)imu_list.size();
+  bkf_sb.resize(KT, nullptr);
   auto fail = [&](const char* call) { S.termination_type = FAILURE; S.message = std::string(call) + ": " + glio_last_error(ctx); };
   // the batch evaluations of the present kinds, in the order eval adds them (K2b, K2p, K2g): the glio_eval_* call, its keyframe
   // count, its Hoff pair table (block (a, b): row = a tangent, col = b tangent) and the columns it fills of each keyframe's 6
@@ -357,6 +411,15 @@ inline void Solve(const Solver::Options& options, Problem* problem, Solver::Summ
     if (!fetch_pairs(glio_batch_dd_psr_pair_list, batch.back())) return fail("glio_batch_dd_psr_pair_list");
     S.num_device_residual_blocks += ND; S.num_device_dd_psr_residual_blocks = ND;
   }
+  // IMU factors: the context's list is replaced after the clear, pair, pose and DD uploads.  A problem without routed IMU blocks
+  // makes no IMU call.  K2i's blocks are 15 x 15 over [t, delta, v, ba, bg]; no other glio_eval_* call adds them, so
+  // glio_batch_use_imu_factors does not change what is computed here.
+  BatchEval imu{nullptr, KT, {}, {}, 15};
+  if (NI > 0) {
+    if (glio_batch_set_imu_factors(ctx, imu_list.data(), NI) != GLIO_OK) return fail("glio_batch_set_imu_factors");
+    if (!fetch_pairs(glio_batch_imu_pair_list, imu)) return fail("glio_batch_imu_pair_list");
+    S.num_device_residual_blocks += NI; S.num_device_imu_residual_blocks = NI;
+  }
 
   // ---- band of J^T J from the block structure ----
   int hb = 0;
@@ -396,6 +459,9 @@ inline void Solve(const Solver::Options& options, Problem* problem, Solver::Summ
   size_t max_pairs = 1;
   for (const BatchEval& be : batch) max_pairs = std::max(max_pairs, be.a.size());
   std::vector<double> bposes((size_t)std::max(KT, 1) * 7), bHd((size_t)std::max(KT, 1) * 36), bHo(max_pairs * 36), bg((size_t)std::max(KT, 1) * 6);
+  // K2i's inputs and outputs, allocated once per solve: speed-bias states (zeros for a keyframe without an sb, which no IMU factor
+  // references), K x 225, P_imu x 225 and K x 15
+  std::vector<double> bsb(NI > 0 ? (size_t)KT * 9 : 0), iHd(NI > 0 ? (size_t)KT * 225 : 0), iHo(imu.a.size() * 225), ig(NI > 0 ? (size_t)KT * 15 : 0);
   // tangent column of each unary slot's and each batch keyframe's 6-vector entries (t, then the rotation's delta); -1 for the
   // entries of a keyframe without a t (seen only in delta_q blocks) or without a q (seen only in DD blocks)
   auto cols_of = [&](double* t, double* q, std::vector<int>& col) {
@@ -404,26 +470,35 @@ inline void Solve(const Solver::Options& options, Problem* problem, Solver::Summ
   std::vector<int> ucol, bcol;
   for (const Slot& sl : slots) cols_of(sl.t, sl.q, ucol);
   for (const auto& kf : bkfs) cols_of(kf.first, kf.second, bcol);
+  // K2i's 15 entries per batch keyframe: [t(3), delta(3)] as above, then its sb's v(3), ba(3), bg(3)
+  std::vector<int> icol;
+  if (NI > 0)
+    for (int k = 0; k < KT; ++k) {
+      icol.insert(icol.end(), bcol.begin() + 6 * k, bcol.begin() + 6 * k + 6);
+      for (int p = 0; p < 9; ++p) icol.push_back(bkf_sb[k] ? P.active[P.index[bkf_sb[k]]].tan_off + p : -1);
+    }
   double fixed_cost = 0; bool fixed_done = false;
 
   glio::EvalFn eval = [&](const double* xa, bool want_jac, double* cost, glio::BandMat* H, double* g) -> bool {
     double ct = 0;
     if (want_jac) { H->reset(n, hb); std::fill(g, g + n, 0.0); }
-    // adds K keyframes' Hdiag (K x 36) and g (K x 6), then np Hoff blocks (block i: row = keyframe a[i], col = keyframe b[i]) to
-    // the band's lower triangle, over the first nc of each keyframe's 6 entries; entries without a column are skipped
-    auto scatter = [&](const int* col, int K, int nc, const double* Hk, const double* gk, int np, const int32_t* a, const int32_t* b, const double* Ho) {
+    // adds K keyframes' Hdiag (K x st^2) and g (K x st), then np Hoff blocks (block i: row = keyframe a[i], col = keyframe b[i],
+    // st x st) to the band's lower triangle, over the first nc of each keyframe's st entries (st = 6, or 15 for K2i); entries
+    // without a column are skipped
+    auto scatter = [&](const int* col, int st, int K, int nc, const double* Hk, const double* gk, int np, const int32_t* a, const int32_t* b,
+                       const double* Ho) {
       for (int k = 0; k < K; ++k)
         for (int p = 0; p < nc; ++p) {
-          const int ip = col[6 * k + p];
+          const int ip = col[st * k + p];
           if (ip < 0) continue;
-          g[ip] += gk[6 * k + p];
-          for (int q = 0; q < nc; ++q) { const int iq = col[6 * k + q]; if (iq >= 0 && ip >= iq) H->at(ip, iq) += Hk[36 * k + 6 * p + q]; }
+          g[ip] += gk[st * k + p];
+          for (int q = 0; q < nc; ++q) { const int iq = col[st * k + q]; if (iq >= 0 && ip >= iq) H->at(ip, iq) += Hk[(size_t)st * st * k + st * p + q]; }
         }
       for (int pr = 0; pr < np; ++pr)
         for (int p = 0; p < nc; ++p) for (int q = 0; q < nc; ++q) {
-          const int ip = col[6 * a[pr] + p], iq = col[6 * b[pr] + q];
+          const int ip = col[st * a[pr] + p], iq = col[st * b[pr] + q];
           if (ip < 0 || iq < 0) continue;
-          const double v = Ho[36 * pr + 6 * p + q];
+          const double v = Ho[(size_t)st * st * pr + st * p + q];
           if (ip >= iq) H->at(ip, iq) += v; else H->at(iq, ip) += v;
         }
     };
@@ -444,9 +519,9 @@ inline void Solve(const Solver::Options& options, Problem* problem, Solver::Summ
         }
       }
       for (int k = 0; k < W; ++k) ct += cd[k];
-      if (want_jac) scatter(ucol.data(), W, 6, Hd.data(), gd.data(), 0, nullptr, nullptr, nullptr);
+      if (want_jac) scatter(ucol.data(), 6, W, 6, Hd.data(), gd.data(), 0, nullptr, nullptr, nullptr);
     }
-    if (!batch.empty())
+    if (!batch.empty() || NI > 0)
       for (int k = 0; k < KT; ++k) {
         for (int i = 0; i < 3; ++i) bposes[7 * k + i] = bkfs[k].first ? xa[P.active[P.index[bkfs[k].first]].amb_off + i] : 0.0;
         if (!bkfs[k].second) { bposes[7 * k + 3] = 1.0; bposes[7 * k + 4] = bposes[7 * k + 5] = bposes[7 * k + 6] = 0.0; continue; }
@@ -457,7 +532,18 @@ inline void Solve(const Solver::Options& options, Problem* problem, Solver::Summ
       double bc = 0;
       if (be.fn(ctx, be.K, bposes.data(), want_jac ? bHd.data() : nullptr, want_jac ? bHo.data() : nullptr, want_jac ? bg.data() : nullptr, &bc) != GLIO_OK) return false;
       ct += bc;
-      if (want_jac) scatter(bcol.data(), be.K, be.nc, bHd.data(), bg.data(), (int)be.a.size(), be.a.data(), be.b.data(), bHo.data());
+      if (want_jac) scatter(bcol.data(), 6, be.K, be.nc, bHd.data(), bg.data(), (int)be.a.size(), be.a.data(), be.b.data(), bHo.data());
+    }
+    // K2i after K2b, K2p and K2g, the order glio_batch_solve adds them in
+    if (NI > 0) {
+      for (int k = 0; k < KT; ++k)
+        for (int i = 0; i < 9; ++i) bsb[9 * k + i] = bkf_sb[k] ? xa[P.active[P.index[bkf_sb[k]]].amb_off + i] : 0.0;
+      double ic = 0;
+      if (glio_eval_imu_factors(ctx, KT, bposes.data(), bsb.data(), want_jac ? iHd.data() : nullptr, want_jac ? iHo.data() : nullptr,
+                                want_jac ? ig.data() : nullptr, &ic) != GLIO_OK)
+        return false;
+      ct += ic;
+      if (want_jac) scatter(icol.data(), 15, KT, 15, iHd.data(), ig.data(), (int)imu.a.size(), imu.a.data(), imu.b.data(), iHo.data());
     }
     // host blocks (ResidualBlock::Evaluate, ceres.tgz::internal/ceres/residual_block.cc:70-197)
     std::vector<const double*> pp; std::vector<double*> jj; std::vector<std::vector<double>> Jamb, Jloc; std::vector<double> r;
