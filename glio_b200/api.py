@@ -149,7 +149,7 @@ class Context:
                "k_vs_key", "k_vs_hist", "k_vs_scatter", "k_vs_heads", "k_vs_centroid", "k_vs_pack", "k_gm_transform",
                "k_pose_pair_sums", "k_pose_pair_sums_cost", "k_pose_assemble",
                "k_psr_pair_sums", "k_psr_pair_sums_cost", "k_psr_assemble",
-               "k_imu_pair_sums", "k_imu_pair_sums_cost", "k_imu_assemble"]
+               "k_imu_pair_sums", "k_imu_pair_sums_cost", "k_imu_pair_sums_ambient", "k_imu_assemble"]
 
     def lib_profile(self, on):
         self._chk(self._lib.glio_profile_enable(self._h, C.c_int(1 if on else 0)))
@@ -1120,6 +1120,47 @@ Context.batch_set_imu_factors = _batch_set_imu_factors
 Context.batch_imu_pair_list = _batch_imu_pair_list
 Context.eval_imu_factors = _eval_imu_factors
 Context.batch_use_imu_factors = _batch_use_imu_factors
+
+
+# the window's IMU chain (K2i in the sliding window): its own list of IMU_FACTOR_DTYPE records, i and j window slots
+WINDOW_MAX_SLOTS = 4096                   # window slots of an IMU factor are below this
+
+
+def _window_set_imu_factors(self, factors):
+    """glio_window_set_imu_factors: replace the window IMU list (an IMU_FACTOR_DTYPE array; empty empties it).  The batch list
+    is left alone."""
+    f = np.ascontiguousarray(factors, IMU_FACTOR_DTYPE)
+    self._chk(self._lib.glio_window_set_imu_factors(self._h, _ptr(f) if len(f) else None, C.c_int64(len(f))))
+
+
+def _window_imu_pair_list(self):
+    """The window IMU pair table (a, b), a < b, in order of first appearance."""
+    return _pair_table(self, self._lib.glio_window_imu_pair_list)
+
+
+def _eval_window_imu_factors(self, poses, speed_bias, jac_kind=0, want_jac=True):
+    """glio_eval_window_imu_factors: the window IMU blocks alone at poses (W, 7) and speed_bias (W, 9), eval_imu_factors' layout.
+    jac_kind 0: tangent quaternion columns; 1: the ambient x, y, z columns the marginalisation reads."""
+    pb = np.ascontiguousarray(poses, np.float64).reshape(-1, 7); W = len(pb)
+    sb = np.ascontiguousarray(speed_bias, np.float64).reshape(W, 9)
+    P = len(_pair_table(self, self._lib.glio_window_imu_pair_list)[0])
+    Hd = np.zeros((W, 15, 15)) if want_jac else None; Ho = np.zeros((P, 15, 15)) if want_jac else None
+    g = np.zeros((W, 15)) if want_jac else None; cost = np.zeros(1)
+    self._chk(self._lib.glio_eval_window_imu_factors(self._h, C.c_int(W), _ptr(pb), _ptr(sb), C.c_int(jac_kind), _ptr(Hd), _ptr(Ho),
+                                                     _ptr(g), _ptr(cost)))
+    return dict(Hdiag=Hd, Hoff=Ho, g=g, cost=float(cost[0]))
+
+
+def _window_use_imu_factors(self, on):
+    """glio_window_use_imu_factors: window solves and marginalisations take the IMU chain from the device (default off; they
+    need speed_bias)."""
+    self._chk(self._lib.glio_window_use_imu_factors(self._h, C.c_int(1 if on else 0)))
+
+
+Context.window_set_imu_factors = _window_set_imu_factors
+Context.window_imu_pair_list = _window_imu_pair_list
+Context.eval_window_imu_factors = _eval_window_imu_factors
+Context.window_use_imu_factors = _window_use_imu_factors
 
 
 # ---------------------------------------------------------------------------------------------------

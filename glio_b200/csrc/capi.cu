@@ -82,6 +82,13 @@ struct PairFactorList {
   void take(PairFactorList&& o) { const bool u = use; *this = std::move(o); use = u; }
 };
 
+// An IMU factor list (K2i): the pair-factor list, its active records, and the buffers of one evaluation: the speed-bias states and
+// the IMU blocks (K x 241 and n_pairs x 225), on the device and in pinned memory.  The batch solve and the window keep one each.
+struct ImuFactorList : PairFactorList {
+  DevBuf<ImuFactor> d_f;
+  DevBuf<double> d_sb, d_diag, d_off; PinnedBuf<double> h_sb, h_diag, h_off;
+};
+
 struct Slot {
   PointSet scan;                 // surf scan
   DevBuf<float4> m_cpw, m_nsd;   // compacted matches, scan order
@@ -123,6 +130,8 @@ struct glio_marg_job {
   int rc = 0;
   std::string err;
   glio_marg_prior* prior = nullptr;
+  bool with_imu = false;               // the device half queued the window IMU factor KF0 -> KF1
+  std::vector<double> imu;             // snapshot of its pair sums (706)
 };
 
 struct glio_ctx {
@@ -183,10 +192,8 @@ struct glio_ctx {
   // DD pseudorange factors (glio_batch_set_dd_psr_factors, K2g): the list, its active records, and the list's satellites, weights
   // and frame constants
   PairFactorList dd; DevBuf<DdPsrFactor> d_dd_f; DevBuf<DdPsrSat> d_dd_sats; DevBuf<double> d_dd_w; DdPsrFrame dd_frame{};
-  // IMU factors (glio_batch_set_imu_factors, K2i): the list and its active records; the speed-bias states of an evaluation and the
-  // IMU blocks (K x 241 and n_imu_pairs x 225), kept apart from the 6-column buffers above
-  PairFactorList imu; DevBuf<ImuFactor> d_imu_f;
-  DevBuf<double> d_imu_sb, d_imu_diag, d_imu_off; PinnedBuf<double> h_imu_sb, h_imu_diag, h_imu_off;
+  // IMU factors (glio_batch_set_imu_factors, K2i), kept apart from the 6-column buffers above
+  ImuFactorList imu;
 
   // association workspace
   DevBuf<float4> w_pm, w_pmq, w_nsd;
@@ -244,6 +251,16 @@ struct glio_ctx {
   bool items_dirty = true;
   int items_W = -1;
   int n_items = 0;
+
+  // the window's IMU chain (glio_window_set_imu_factors, glio_window_use_imu_factors), separate from the batch list: its poses
+  // travel from pinned memory; a marginalisation copies pair {0, 1}'s ambient-column sums into h_wimu_marg, which an asynchronous
+  // marginalisation owns until its worker has copied it (wait_marg_copied).  Kept after the members above, whose layout stays as
+  // it was without the window chain.
+  ImuFactorList window_imu;
+  DevBuf<double> wimu_poses; PinnedBuf<double> h_wimu_poses, h_wimu_marg;
+  // what the marginalisation needs of the list's slot 0: the index of pair {0, 1} when an active factor joins slots 0 and 1 (-1
+  // otherwise), and whether an active factor joins slot 0 to another slot
+  int wimu_pair01 = -1; bool wimu_slot0_elsewhere = false;
 
   Slot& slot(int k) {
     GLIO_REQUIRE(k >= 0 && k < 4096, GLIO_ERR_ARG, "slot index out of range");
@@ -645,6 +662,109 @@ void eval_unary_wait(glio_ctx* c, unsigned int epoch) {
 // device evaluation of all active unary residuals -> c->h_out (W x 28: 21 upper-tri H, 6 g, 1 cost), synchronised
 void eval_unary_blocks(glio_ctx* c, int W, const double* poses_body, int jac_kind, bool want_jac) {
   eval_unary_wait(c, eval_unary_launch(c, W, poses_body, jac_kind, want_jac));
+}
+
+// Device evaluation of the IMU blocks of list L -> L.h_diag (K x 241), L.h_off (n_pairs x 225), at the poses d_poses (already queued)
+// and speed_bias, which is queued here; jac_kind 1 gives the ambient x, y, z quaternion columns.  With reduce (the batch list) the
+// IMU buffers are summed over the ranks of a sharded run after whatever the caller queued before, one call per buffer.  Queued only;
+// a synchronisation of the stream, or the completion flag of a K2 queued after it, makes the result visible.  Returns the
+// off-diagonal block count.
+int imu_blocks_launch(glio_ctx* c, ImuFactorList& L, int K, const double* d_poses, const double* speed_bias, int jac_kind, bool want_jac,
+                      bool reduce) {
+  const int Pi = (int)L.pairs.size();
+  L.d_sb.reserve((size_t)K * 9); L.h_sb.reserve((size_t)K * 9);
+  L.d_diag.reserve((size_t)K * GLIO_NACC_IMU_KF); L.h_diag.reserve((size_t)K * GLIO_NACC_IMU_KF);
+  L.d_off.reserve((size_t)(Pi + 1) * 225); L.h_off.reserve((size_t)(Pi + 1) * 225);
+  memcpy(L.h_sb.p, speed_bias, (size_t)K * 9 * sizeof(double));
+  GLIO_CUDA_TRY(cudaMemcpyAsync(L.d_sb.p, L.h_sb.p, (size_t)K * 9 * sizeof(double), cudaMemcpyHostToDevice, c->st));
+  eval_imu_run(L.d_f.p, L.d_fstart.p, Pi, K, L.max_kf + 1, L.d_inc_start.p, L.d_inc.p, d_poses, L.d_sb.p, jac_kind, want_jac, L.d_sums.p,
+               L.d_diag.p, L.d_off.p, c->st, c->lc);
+  if (reduce && c->allreduce) {
+    GLIO_REQUIRE(c->allreduce(c->allreduce_user, L.d_diag.p, (int64_t)K * GLIO_NACC_IMU_KF, (void*)c->st) == 0, GLIO_ERR_NCCL,
+                 "allreduce hook failed (IMU diag)");
+    if (want_jac && Pi > 0)
+      GLIO_REQUIRE(c->allreduce(c->allreduce_user, L.d_off.p, (int64_t)Pi * 225, (void*)c->st) == 0, GLIO_ERR_NCCL,
+                   "allreduce hook failed (IMU off)");
+  }
+  GLIO_CUDA_TRY(cudaMemcpyAsync(L.h_diag.p, L.d_diag.p, (size_t)K * GLIO_NACC_IMU_KF * sizeof(double), cudaMemcpyDeviceToHost, c->st));
+  if (want_jac && Pi > 0) GLIO_CUDA_TRY(cudaMemcpyAsync(L.h_off.p, L.d_off.p, (size_t)Pi * 225 * sizeof(double), cudaMemcpyDeviceToHost, c->st));
+  return Pi;
+}
+
+// the half bandwidth of list L's blocks at 15 columns per keyframe: (the widest pair's span + 1) * 15 - 1, 0 for no pair
+int imu_half_bandwidth(const ImuFactorList& L) {
+  int span = 0;
+  for (const auto& p : L.pairs) span = std::max(span, p.second - p.first);
+  return span > 0 ? (span + 1) * 15 - 1 : 0;
+}
+
+// list L's blocks of an evaluation that has arrived into the 15-column band: the cost, then with want_jac each keyframe's 15 x 15
+// lower triangle and g, then each pair's (a, b) block, stored transposed (rows of b, a < b)
+void add_imu_blocks(const ImuFactorList& L, int K, bool want_jac, BandMat* H, double* g, double& ct) {
+  for (int k = 0; k < K; ++k) ct += L.h_diag.p[(size_t)k * GLIO_NACC_IMU_KF + 240];
+  if (!want_jac) return;
+  const int w = H->hb + 1;
+  double* a = H->a.data();
+  for (int k = 0; k < K; ++k) {
+    const double* o = L.h_diag.p + (size_t)k * GLIO_NACC_IMU_KF;
+    for (int p = 0; p < 15; ++p) {
+      double* row = a + (size_t)(15 * k + p) * w + (H->hb - p);
+      for (int q = 0; q <= p; ++q) row[q] += o[15 * p + q];
+      g[15 * k + p] += o[225 + p];
+    }
+  }
+  for (size_t pi = 0; pi < L.pairs.size(); ++pi) {
+    const int ka = L.pairs[pi].first, kb = L.pairs[pi].second;
+    const double* ob = L.h_off.p + pi * 225;              // d2 cost / d x_a[p] d x_b[q]
+    for (int q = 0; q < 15; ++q) { double* row = a + (size_t)(15 * kb + q) * w + (15 * ka - (15 * kb + q) + H->hb); for (int p = 0; p < 15; ++p) row[p] += ob[15 * p + q]; }
+  }
+}
+
+// the W window poses into the device buffer the window's K2i reads, from pinned memory
+void upload_window_imu_poses(glio_ctx* c, int W, const double* poses) {
+  c->wimu_poses.reserve((size_t)W * 7); c->h_wimu_poses.reserve((size_t)W * 7);
+  memcpy(c->h_wimu_poses.p, poses, (size_t)W * 7 * sizeof(double));
+  GLIO_CUDA_TRY(cudaMemcpyAsync(c->wimu_poses.p, c->h_wimu_poses.p, (size_t)W * 7 * sizeof(double), cudaMemcpyHostToDevice, c->st));
+}
+
+// The window's IMU blocks at one solve evaluation (tangent columns): the poses and speed-bias states, K2i and the copies of its
+// blocks into pinned memory, all queued on the main stream ahead of the K2 the caller queues next, whose completion flag covers them
+void window_imu_launch(glio_ctx* c, int W, const double* poses, const double* speed_bias, bool want_jac) {
+  wait_marg_copied(c);                   // a pending marginalisation's upload may still read the pinned buffers
+  upload_window_imu_poses(c, W, poses);
+  imu_blocks_launch(c, c->window_imu, W, c->wimu_poses.p, speed_bias, 0, want_jac, false);
+}
+
+// The marginalisation's IMU part (Estimator.cpp:2520-2534): the ImuFactor KF0 -> KF1 with the ambient x, y, z quaternion columns
+// that ThreadsConstructA reads (MarginalizationFactor.cpp:3-29).  K2i runs over pair {0, 1} alone and its 706 sums are copied into
+// c->h_wimu_marg, queued ahead of K2.  Factors that do not touch slot 0 take no part; an active factor (0, k), k != 1, is
+// GLIO_ERR_ARG: its other speed-bias block is not in the marginalisation ordering.  Returns false when no active factor is (0, 1).
+bool window_imu_marg_launch(glio_ctx* c, const double* poses, const double* speed_bias) {
+  ImuFactorList& M = c->window_imu;
+  GLIO_REQUIRE(!c->wimu_slot0_elsewhere, GLIO_ERR_ARG, "marginalisation: an active IMU factor joins slot 0 to a slot other than 1");
+  const int p01 = c->wimu_pair01;
+  if (p01 < 0) return false;
+  wait_marg_copied(c);
+  upload_window_imu_poses(c, 2, poses);
+  M.d_sb.reserve(18); M.h_sb.reserve(18); c->h_wimu_marg.reserve(GLIO_NACC_IMU);
+  memcpy(M.h_sb.p, speed_bias, 18 * sizeof(double));
+  GLIO_CUDA_TRY(cudaMemcpyAsync(M.d_sb.p, M.h_sb.p, 18 * sizeof(double), cudaMemcpyHostToDevice, c->st));
+  eval_imu_pair_sums_run(M.d_f.p, M.d_fstart.p + p01, 1, c->wimu_poses.p, M.d_sb.p, 1, true, M.d_sums.p, c->st, c->lc);
+  GLIO_CUDA_TRY(cudaMemcpyAsync(c->h_wimu_marg.p, M.d_sums.p, GLIO_NACC_IMU * sizeof(double), cudaMemcpyDeviceToHost, c->st));
+  return true;
+}
+
+// pair {0, 1}'s sums s (706: aa, bb, ab row-major, g) into A (N x N) and b at the marginalisation ordering, where KF0's
+// [t, q, sb] is [0, 15) and KF1's [15, 30) (marg.h)
+void add_marg_imu(std::vector<double>& A, std::vector<double>& b, int N, const double* s) {
+  for (int p = 0; p < 15; ++p)
+    for (int q = 0; q < 15; ++q) {
+      A[(size_t)p * N + q] += s[15 * p + q];
+      A[(size_t)(15 + p) * N + 15 + q] += s[225 + 15 * p + q];
+      A[(size_t)p * N + 15 + q] += s[450 + 15 * p + q];
+      A[(size_t)(15 + q) * N + p] += s[450 + 15 * p + q];
+    }
+  for (int l = 0; l < 30; ++l) b[l] += s[675 + l];
 }
 
 }  // namespace
@@ -1280,10 +1400,12 @@ glio_marg_prior* marg_finish_host(int W, double eps, std::vector<double>& A, std
 }
 
 // device half + the caller's host factors: queues the LiDAR re-evaluation of every keyframe with the ambient x,y,z quaternion
-// columns (Estimator.cpp:2538-2576) and evaluates the host callback while the kernel runs
+// columns (Estimator.cpp:2538-2576), after the window's IMU factor KF0 -> KF1 when glio_window_use_imu_factors is on (*with_imu
+// tells whether it was queued), and evaluates the host callback while the kernels run
 unsigned int marg_begin(glio_ctx* c, int W, const double* poses, const double* speed_bias, glio_host_marg_fn host_marg, void* user,
-                        std::vector<double>& A, std::vector<double>& b) {
+                        std::vector<double>& A, std::vector<double>& b, bool* with_imu) {
   const int N = 6 * W + 18;
+  *with_imu = c->window_imu.use && !c->window_imu.pairs.empty() && window_imu_marg_launch(c, poses, speed_bias);
   const unsigned int epoch = eval_unary_launch(c, W, poses, 1, true, nullptr, true);
   A.assign((size_t)N * N, 0.0); b.assign(N, 0.0);
   if (host_marg) GLIO_REQUIRE(host_marg(user, W, poses, speed_bias, A.data(), b.data()) == 0, GLIO_ERR_STATE, "host_marg callback failed");
@@ -1316,7 +1438,9 @@ void marg_worker(glio_ctx* c) {
     try {
       eval_unary_wait(c, j->epoch);
       j->out.assign(c->h_out.p, c->h_out.p + (size_t)j->W * GLIO_NACC);
+      if (j->with_imu) j->imu.assign(c->h_wimu_marg.p, c->h_wimu_marg.p + GLIO_NACC_IMU);
       j->copied.store(1, std::memory_order_release);
+      if (j->with_imu) add_marg_imu(j->A, j->b, 6 * j->W + 18, j->imu.data());
       j->prior = marg_finish_host(j->W, j->eps, j->A, j->b, j->out.data(), j->x0_pose.data(), j->x0_sb.data());
       if (!j->prior) { j->rc = GLIO_ERR_STATE; j->err = "marginalisation failed (decomposition or prior)"; }
     } catch (const Error& e) { j->rc = e.code; j->err = e.msg; }
@@ -1337,8 +1461,10 @@ int glio_window_marginalize(glio_ctx* c, int W, const double* poses, const doubl
   return guarded(c, [&] {
     GLIO_REQUIRE(W >= 2 && W <= 4096 && poses && speed_bias, GLIO_ERR_ARG, "glio_window_marginalize: need W >= 2, poses and speed_bias");
     std::vector<double> A, b;
-    const unsigned int epoch = marg_begin(c, W, poses, speed_bias, host_marg, user, A, b);
+    bool with_imu = false;
+    const unsigned int epoch = marg_begin(c, W, poses, speed_bias, host_marg, user, A, b, &with_imu);
     eval_unary_wait(c, epoch);
+    if (with_imu) add_marg_imu(A, b, 6 * W + 18, c->h_wimu_marg.p);
     glio_marg_prior* made = marg_finish_host(W, eps, A, b, c->h_out.p, poses + 7, speed_bias + 9);
     GLIO_REQUIRE(made != nullptr, GLIO_ERR_STATE, "marginalisation failed (decomposition or prior)");
     *prior_out = made;
@@ -1359,7 +1485,7 @@ int glio_window_marginalize_async(glio_ctx* c, int W, const double* poses, const
     std::unique_ptr<glio_marg_job> j(new glio_marg_job());
     j->ctx = c; j->W = W; j->eps = eps;
     j->x0_pose.assign(poses + 7, poses + 7 * (size_t)W); j->x0_sb.assign(speed_bias + 9, speed_bias + 18);
-    j->epoch = marg_begin(c, W, poses, speed_bias, host_marg, user, j->A, j->b);
+    j->epoch = marg_begin(c, W, poses, speed_bias, host_marg, user, j->A, j->b, &j->with_imu);
 #if defined(__linux__)
     j->submit_cpu = sched_getcpu();
 #endif
@@ -1607,13 +1733,18 @@ static void add_diag_blocks(BandMat* H, const double* o28, int W, int nt) {
   }
 }
 
-// The minimizer over W poses (and speed-bias states) with the LiDAR blocks of `tgt` (nullptr: the context's slots and glio_params)
-// plus the host factors.  Throws on error; poses / speed_bias are in/out.
+// The minimizer over W poses (and speed-bias states) with the LiDAR blocks of `tgt` (nullptr: the context's slots and glio_params,
+// plus the window's IMU chain when glio_window_use_imu_factors is on) plus the host factors.  Throws on error; poses / speed_bias
+// are in/out.
 static void solve_core(glio_ctx* c, int W, double* poses, double* speed_bias, glio_host_factors_fn host_factors, glio_host_factors_band_fn host_band,
                        int hb_hint, void* user, const SolverOptions& so, const EvalTarget* tgt, SolverSummary& S) {
     const bool sb = speed_bias != nullptr;
     const StateLayout L(W, sb);
     const int nt = L.nt, n = W * nt;
+    const bool add_imu = tgt == nullptr && c->window_imu.use && !c->window_imu.pairs.empty();
+    GLIO_REQUIRE(!add_imu || sb, GLIO_ERR_ARG, "window solve: the IMU factors need speed_bias");
+    GLIO_REQUIRE(!add_imu || c->window_imu.max_kf < W, GLIO_ERR_ARG, "window solve: an IMU factor references a slot outside [0, W)");
+    const int imu_hb = add_imu ? imu_half_bandwidth(c->window_imu) : 0;   // the band must cover the IMU pairs whatever the callback writes
     TrustRegionDogleg solver(L.blocks(), so);
     std::vector<double> x((size_t)W * L.na), pz((size_t)W * 7), sz((size_t)W * 9);
     L.pack(poses, speed_bias, x.data());
@@ -1621,7 +1752,8 @@ static void solve_core(glio_ctx* c, int W, double* poses, double* speed_bias, gl
     int hb_fixed = -1;
     EvalFn eval = [&](const double* xa, bool want_jac, double* cost, BandMat* H, double* g) -> bool {
       L.unpack(xa, pz.data(), sz.data());
-      // the device evaluates the LiDAR residuals while the host evaluates its own factors
+      // the device evaluates the IMU chain and the LiDAR residuals while the host evaluates its own factors
+      if (add_imu) window_imu_launch(c, W, pz.data(), sz.data(), want_jac);
       const unsigned int epoch = eval_unary_launch(c, W, pz.data(), 0, want_jac, tgt, true);
       double ct = 0;
       if (want_jac) std::fill(g, g + n, 0.0);
@@ -1632,11 +1764,12 @@ static void solve_core(glio_ctx* c, int W, double* poses, double* speed_bias, gl
       };
       if (host_band) {
         // host factors accumulate straight into the band matrix (no dense n x n scratch)
-        if (want_jac) H->reset(n, hb_hint >= 5 ? hb_hint : n - 1);
+        if (want_jac) H->reset(n, hb_hint >= 5 ? std::max(hb_hint, imu_hb) : n - 1);
         const int hrc = host_band(user, W, pz.data(), sb ? sz.data() : nullptr, want_jac ? 1 : 0, want_jac ? H->a.data() : nullptr, want_jac ? H->hb : 0, g, &ct);
         add_device();
         if (hrc != 0) return false;
         if (want_jac) add_diag_blocks(H, c->h_out.p, W, nt);
+        if (add_imu) add_imu_blocks(c->window_imu, W, want_jac, H, g, ct);
         *cost = ct;
         return std::isfinite(ct);
       }
@@ -1653,13 +1786,14 @@ static void solve_core(glio_ctx* c, int W, double* poses, double* speed_bias, gl
         {
           int w = 5;
           if (host_factors) for (int i = 0; i < n; ++i) for (int j = 0; j < i - w; ++j) if (Hd[(size_t)i * n + j] != 0.0 || Hd[(size_t)j * n + i] != 0.0) { w = i - j; break; }
-          hb_fixed = std::max(hb_fixed, w);
+          hb_fixed = std::max(hb_fixed, std::max(w, imu_hb));
         }
         H->reset(n, hb_fixed);
         const int hb = H->hb;
         if (host_factors) for (int i = 0; i < n; ++i) for (int j = std::max(0, i - hb); j <= i; ++j) H->at(i, j) = Hd[(size_t)i * n + j];
         add_diag_blocks(H, c->h_out.p, W, nt);
       }
+      if (add_imu) add_imu_blocks(c->window_imu, W, want_jac, H, g, ct);
       *cost = ct;
       return std::isfinite(ct);
     };
@@ -2368,31 +2502,6 @@ int eval_blocks_out(glio_ctx* c, const char* who, int K, const double* poses, Bi
   });
 }
 
-// Device evaluation of the IMU blocks -> c->h_imu_diag (K x 241), c->h_imu_off (n_imu_pairs x 225), at the poses already queued
-// into c->d_bin_poses and speed_bias, which is queued here.  The IMU buffers are summed over the ranks of a sharded run after
-// whatever the caller queued before, one call per buffer.  Queued only; a synchronisation of the stream makes the result visible.
-// Returns the off-diagonal block count.
-int imu_blocks_launch(glio_ctx* c, int K, const double* speed_bias, bool want_jac) {
-  const int Pi = (int)c->imu.pairs.size();
-  c->d_imu_sb.reserve((size_t)K * 9); c->h_imu_sb.reserve((size_t)K * 9);
-  c->d_imu_diag.reserve((size_t)K * GLIO_NACC_IMU_KF); c->h_imu_diag.reserve((size_t)K * GLIO_NACC_IMU_KF);
-  c->d_imu_off.reserve((size_t)(Pi + 1) * 225); c->h_imu_off.reserve((size_t)(Pi + 1) * 225);
-  memcpy(c->h_imu_sb.p, speed_bias, (size_t)K * 9 * sizeof(double));
-  GLIO_CUDA_TRY(cudaMemcpyAsync(c->d_imu_sb.p, c->h_imu_sb.p, (size_t)K * 9 * sizeof(double), cudaMemcpyHostToDevice, c->st));
-  eval_imu_run(c->d_imu_f.p, c->imu.d_fstart.p, Pi, K, c->imu.max_kf + 1, c->imu.d_inc_start.p, c->imu.d_inc.p, c->d_bin_poses.p,
-               c->d_imu_sb.p, want_jac, c->imu.d_sums.p, c->d_imu_diag.p, c->d_imu_off.p, c->st, c->lc);
-  if (c->allreduce) {
-    GLIO_REQUIRE(c->allreduce(c->allreduce_user, c->d_imu_diag.p, (int64_t)K * GLIO_NACC_IMU_KF, (void*)c->st) == 0, GLIO_ERR_NCCL,
-                 "allreduce hook failed (IMU diag)");
-    if (want_jac && Pi > 0)
-      GLIO_REQUIRE(c->allreduce(c->allreduce_user, c->d_imu_off.p, (int64_t)Pi * 225, (void*)c->st) == 0, GLIO_ERR_NCCL,
-                   "allreduce hook failed (IMU off)");
-  }
-  GLIO_CUDA_TRY(cudaMemcpyAsync(c->h_imu_diag.p, c->d_imu_diag.p, (size_t)K * GLIO_NACC_IMU_KF * sizeof(double), cudaMemcpyDeviceToHost, c->st));
-  if (want_jac && Pi > 0) GLIO_CUDA_TRY(cudaMemcpyAsync(c->h_imu_off.p, c->d_imu_off.p, (size_t)Pi * 225 * sizeof(double), cudaMemcpyDeviceToHost, c->st));
-  return Pi;
-}
-
 // The pair plan of a factor list with keyframes i, j and an active flag (pose and DD factors): the distinct unordered pairs
 // (a, b), a < b, in order of first appearance; the active factors' list positions grouped by pair, list order inside a pair
 // (order[fstart[p] .. fstart[p+1])); per keyframe 0 .. max_kf its pairs in table order (role 0 = a, 1 = b), by a counting sort.
@@ -2451,6 +2560,41 @@ PairFactorList upload_pair_factors(glio_ctx* c, const Rec* f, int64_t n, int max
   if (!pl.inc.empty()) GLIO_CUDA_TRY(cudaMemcpyAsync(l.d_inc.p, pl.inc.data(), pl.inc.size() * sizeof(BinIncidence), cudaMemcpyHostToDevice, c->st));
   l.pairs.swap(pl.pairs); l.max_kf = pl.max_kf;
   return l;
+}
+
+static_assert(sizeof(glio_imu_factor) == sizeof(ImuFactor) && offsetof(glio_imu_factor, sum_dt) == offsetof(ImuFactor, sum_dt) &&
+              offsetof(glio_imu_factor, delta_q) == offsetof(ImuFactor, delta_q) && offsetof(glio_imu_factor, dp_dba) == offsetof(ImuFactor, dp_dba) &&
+              offsetof(glio_imu_factor, dv_dbg) == offsetof(ImuFactor, dv_dbg) && offsetof(glio_imu_factor, sqrt_info) == offsetof(ImuFactor, sqrt_info),
+              "ImuFactor must have glio_imu_factor's layout");
+
+// Replaces IMU list L (glio_batch_set_imu_factors, glio_window_set_imu_factors; who names the call, max_name its index bound)
+void set_imu_factors(glio_ctx* c, ImuFactorList& L, const glio_imu_factor* f, int64_t n, int max_kf, const char* who, const char* max_name) {
+  const std::string w(who);
+  // validate the whole list first: a refused call leaves the previous list in place
+  GLIO_REQUIRE(n >= 0 && (n == 0 || f), GLIO_ERR_ARG, w + ": null factor array");
+  GLIO_REQUIRE(n < ((int64_t)1 << 31), GLIO_ERR_ARG, w + ": too many factors");
+  constexpr int nd = (int)((sizeof(glio_imu_factor) - offsetof(glio_imu_factor, sum_dt)) / sizeof(double));
+  for (int64_t k = 0; k < n; ++k) {
+    const double* d = &f[k].sum_dt;
+    for (int m = 0; m < nd; ++m) GLIO_REQUIRE(std::isfinite(d[m]), GLIO_ERR_ARG, w + ": a non-finite field");
+  }
+  DevBuf<ImuFactor> d_f;
+  PairFactorList l = upload_pair_factors(c, f, n, max_kf, GLIO_NACC_IMU, (w + ": need i != j, both in [0, " + max_name + ")").c_str(), d_f);
+  GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));   // also: no evaluation still reads the buffers released below
+  L.d_f = std::move(d_f); L.take(std::move(l));
+}
+
+// an IMU evaluation that has arrived, on the host: Hdiag (K x 225), Hoff (n_off x 225), g (K x 15), the total cost
+void imu_blocks_out(const ImuFactorList& L, int K, int n_off, double* Hdiag, double* Hoff, double* g, double* cost) {
+  double ct = 0;
+  for (int k = 0; k < K; ++k) {
+    const double* o = L.h_diag.p + (size_t)k * GLIO_NACC_IMU_KF;
+    if (Hdiag) memcpy(Hdiag + (size_t)225 * k, o, 225 * sizeof(double));
+    if (g) memcpy(g + (size_t)15 * k, o + 225, 15 * sizeof(double));
+    ct += o[240];
+  }
+  if (Hoff && n_off > 0) memcpy(Hoff, L.h_off.p, (size_t)n_off * 225 * sizeof(double));
+  if (cost) *cost = ct;
 }
 
 }  // namespace
@@ -2557,28 +2701,9 @@ int glio_batch_use_dd_psr_factors(glio_ctx* c, int on) {
   return GLIO_OK;
 }
 
-static_assert(sizeof(glio_imu_factor) == sizeof(ImuFactor) && offsetof(glio_imu_factor, sum_dt) == offsetof(ImuFactor, sum_dt) &&
-              offsetof(glio_imu_factor, delta_q) == offsetof(ImuFactor, delta_q) && offsetof(glio_imu_factor, dp_dba) == offsetof(ImuFactor, dp_dba) &&
-              offsetof(glio_imu_factor, dv_dbg) == offsetof(ImuFactor, dv_dbg) && offsetof(glio_imu_factor, sqrt_info) == offsetof(ImuFactor, sqrt_info),
-              "ImuFactor must have glio_imu_factor's layout");
-
 int glio_batch_set_imu_factors(glio_ctx* c, const glio_imu_factor* f, int64_t n) {
   if (!c) return GLIO_ERR_ARG;
-  return guarded(c, [&] {
-    // validate the whole list first: a refused call leaves the previous list in place
-    GLIO_REQUIRE(n >= 0 && (n == 0 || f), GLIO_ERR_ARG, "glio_batch_set_imu_factors: null factor array");
-    GLIO_REQUIRE(n < ((int64_t)1 << 31), GLIO_ERR_ARG, "glio_batch_set_imu_factors: too many factors");
-    constexpr int nd = (int)((sizeof(glio_imu_factor) - offsetof(glio_imu_factor, sum_dt)) / sizeof(double));
-    for (int64_t k = 0; k < n; ++k) {
-      const double* d = &f[k].sum_dt;
-      for (int m = 0; m < nd; ++m) GLIO_REQUIRE(std::isfinite(d[m]), GLIO_ERR_ARG, "glio_batch_set_imu_factors: a non-finite field");
-    }
-    DevBuf<ImuFactor> d_f;
-    PairFactorList l = upload_pair_factors(c, f, n, GLIO_IMU_MAX_KF, GLIO_NACC_IMU,
-                                           "glio_batch_set_imu_factors: need i != j, both in [0, GLIO_IMU_MAX_KF)", d_f);
-    GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));   // also: no evaluation still reads the buffers released below
-    c->d_imu_f = std::move(d_f); c->imu.take(std::move(l));
-  });
+  return guarded(c, [&] { set_imu_factors(c, c->imu, f, n, GLIO_IMU_MAX_KF, "glio_batch_set_imu_factors", "GLIO_IMU_MAX_KF"); });
 }
 
 int glio_batch_imu_pair_list(glio_ctx* c, int64_t capacity, int32_t* a, int32_t* b, int64_t* n_pairs) {
@@ -2595,17 +2720,9 @@ int glio_eval_imu_factors(glio_ctx* c, int K, const double* poses, const double*
     c->d_bin_poses.reserve((size_t)K * 7); c->h_bin_poses.reserve((size_t)K * 7);
     memcpy(c->h_bin_poses.p, poses, (size_t)K * 7 * sizeof(double));
     GLIO_CUDA_TRY(cudaMemcpyAsync(c->d_bin_poses.p, c->h_bin_poses.p, (size_t)K * 7 * sizeof(double), cudaMemcpyHostToDevice, c->st));
-    const int n_off = imu_blocks_launch(c, K, speed_bias, Hdiag || Hoff || g);
+    const int n_off = imu_blocks_launch(c, c->imu, K, c->d_bin_poses.p, speed_bias, 0, Hdiag || Hoff || g, true);
     GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
-    double ct = 0;
-    for (int k = 0; k < K; ++k) {
-      const double* o = c->h_imu_diag.p + (size_t)k * GLIO_NACC_IMU_KF;
-      if (Hdiag) memcpy(Hdiag + (size_t)225 * k, o, 225 * sizeof(double));
-      if (g) memcpy(g + (size_t)15 * k, o + 225, 15 * sizeof(double));
-      ct += o[240];
-    }
-    if (Hoff && n_off > 0) memcpy(Hoff, c->h_imu_off.p, (size_t)n_off * 225 * sizeof(double));
-    if (cost) *cost = ct;
+    imu_blocks_out(c->imu, K, n_off, Hdiag, Hoff, g, cost);
   });
 }
 
@@ -2615,6 +2732,46 @@ int glio_batch_use_imu_factors(glio_ctx* c, int on) {
   return GLIO_OK;
 }
 
+// ---- the window's IMU chain (Estimator.cpp:2179-2193), from the caller's pre-integration
+int glio_window_set_imu_factors(glio_ctx* c, const glio_imu_factor* f, int64_t n) {
+  if (!c) return GLIO_ERR_ARG;
+  return guarded(c, [&] {
+    set_imu_factors(c, c->window_imu, f, n, 4096, "glio_window_set_imu_factors", "4096");
+    // what the marginalisation needs of slot 0 (glio_window_marginalize)
+    bool active01 = false, slot0_elsewhere = false;
+    for (int64_t k = 0; k < n; ++k)
+      if (f[k].active && std::min(f[k].i, f[k].j) == 0) (std::max(f[k].i, f[k].j) == 1 ? active01 : slot0_elsewhere) = true;
+    c->wimu_pair01 = -1; c->wimu_slot0_elsewhere = slot0_elsewhere;
+    for (size_t p = 0; active01 && p < c->window_imu.pairs.size(); ++p)
+      if (c->window_imu.pairs[p] == std::make_pair(0, 1)) c->wimu_pair01 = (int)p;
+  });
+}
+
+int glio_window_imu_pair_list(glio_ctx* c, int64_t capacity, int32_t* a, int32_t* b, int64_t* n_pairs) {
+  if (!c) return GLIO_ERR_ARG;
+  return guarded(c, [&] { copy_pair_table(c->window_imu.pairs, capacity, a, b, n_pairs, "glio_window_imu_pair_list: capacity too small"); });
+}
+
+int glio_eval_window_imu_factors(glio_ctx* c, int W, const double* poses, const double* speed_bias, int jac_kind, double* Hdiag,
+                                 double* Hoff, double* g, double* cost) {
+  if (!c) return GLIO_ERR_ARG;
+  return guarded(c, [&] {
+    GLIO_REQUIRE(W > 0 && W <= 4096 && poses && speed_bias, GLIO_ERR_ARG, "glio_eval_window_imu_factors: need 0 < W <= 4096, poses and speed_bias");
+    GLIO_REQUIRE(jac_kind == 0 || jac_kind == 1, GLIO_ERR_ARG, "glio_eval_window_imu_factors: jac_kind must be 0 or 1");
+    GLIO_REQUIRE(c->window_imu.max_kf < W, GLIO_ERR_ARG, "glio_eval_window_imu_factors: an IMU factor references a slot outside [0, W)");
+    wait_marg_copied(c);
+    upload_window_imu_poses(c, W, poses);
+    const int n_off = imu_blocks_launch(c, c->window_imu, W, c->wimu_poses.p, speed_bias, jac_kind, Hdiag || Hoff || g, false);
+    GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
+    imu_blocks_out(c->window_imu, W, n_off, Hdiag, Hoff, g, cost);
+  });
+}
+
+int glio_window_use_imu_factors(glio_ctx* c, int on) {
+  if (!c) return GLIO_ERR_ARG;
+  c->window_imu.use = on != 0;
+  return GLIO_OK;
+}
 
 int glio_set_allreduce(glio_ctx* c, glio_allreduce_fn fn, void* user) {
   if (!c) return GLIO_ERR_ARG;
@@ -2690,7 +2847,7 @@ int glio_batch_solve(glio_ctx* c, int K, double* poses, double* speed_bias, glio
       // the device evaluates the LiDAR pairs (and a sharded run sums them over the ranks) while the host evaluates its own
       // factors into the freshly reset band; the device blocks are added when they have arrived
       eval_blocks_launch(c, K, pz.data(), want_jac, c->batch_use_edges ? BIN_PLANES_EDGES : BIN_PLANES, add_pose, add_dd);
-      if (add_imu) imu_blocks_launch(c, K, sz.data(), want_jac);
+      if (add_imu) imu_blocks_launch(c, c->imu, K, c->d_bin_poses.p, sz.data(), 0, want_jac, true);
       double ct = 0;
       int hrc = 0;
       if (want_jac) { H->reset(n, hb); std::fill(g, g + n, 0.0); }
@@ -2715,28 +2872,7 @@ int glio_batch_solve(glio_ctx* c, int K, double* poses, double* speed_bias, glio
           }
         }
       }
-      if (add_imu) {
-        // the IMU blocks after all others: each keyframe's 15 x 15 lower triangle, g and cost, then each pair's (a, b) block,
-        // stored transposed (rows of b, a < b)
-        for (int k = 0; k < K; ++k) ct += c->h_imu_diag.p[(size_t)k * GLIO_NACC_IMU_KF + 240];
-        if (want_jac) {
-          const int w = H->hb + 1;
-          double* a = H->a.data();
-          for (int k = 0; k < K; ++k) {
-            const double* o = c->h_imu_diag.p + (size_t)k * GLIO_NACC_IMU_KF;
-            for (int p = 0; p < 15; ++p) {
-              double* row = a + (size_t)(15 * k + p) * w + (H->hb - p);
-              for (int q = 0; q <= p; ++q) row[q] += o[15 * p + q];
-              g[15 * k + p] += o[225 + p];
-            }
-          }
-          for (size_t pi = 0; pi < c->imu.pairs.size(); ++pi) {
-            const int ka = c->imu.pairs[pi].first, kb = c->imu.pairs[pi].second;
-            const double* ob = c->h_imu_off.p + pi * 225;              // d2 cost / d x_a[p] d x_b[q]
-            for (int q = 0; q < 15; ++q) { double* row = a + (size_t)(15 * kb + q) * w + (15 * ka - (15 * kb + q) + H->hb); for (int p = 0; p < 15; ++p) row[p] += ob[15 * p + q]; }
-          }
-        }
-      }
+      if (add_imu) add_imu_blocks(c->imu, K, want_jac, H, g, ct);   // the IMU blocks after all others
       *cost = ct;
       return std::isfinite(ct);
     };

@@ -401,10 +401,14 @@ constexpr int GLIO_NACC_IMU_KF = 241;
 // k_imu_pair_sums: the factors of pair p are f[fstart[p] .. fstart[p+1]) in list order, at poses (K x 7) and speed_bias (K x 9)
 // -> d_sums (n_pairs x 706); k_imu_assemble: per keyframe k < n_inc_kf the pairs of its incidence list, in order, written into
 // d_diag (K x 241; the cost goes to a) and, with want_jac, the ab blocks -> d_off (n_pairs x 225).  Two launches whatever K; with
-// n_pairs = 0 only the assembly runs.
+// n_pairs = 0 only the assembly runs.  jac_kind 0: the delta columns are the tangent ones; 1: the ambient x, y, z quaternion columns
+// (k_imu_pair_sums_ambient; the cost-only launch is the same for both).
 void eval_imu_run(const ImuFactor* d_f, const int* d_fstart, int n_pairs, int K, int n_inc_kf, const int* d_kf_inc_start,
-                  const BinIncidence* d_inc, const double* d_poses, const double* d_sb, bool want_jac, double* d_sums, double* d_diag,
-                  double* d_off, cudaStream_t st, LaunchCounter& lc);
+                  const BinIncidence* d_inc, const double* d_poses, const double* d_sb, int jac_kind, bool want_jac, double* d_sums,
+                  double* d_diag, double* d_off, cudaStream_t st, LaunchCounter& lc);
+// k_imu_pair_sums alone over n_pairs pairs starting at d_fstart (a sub-range of a list's plan) -> d_sums (n_pairs x 706)
+void eval_imu_pair_sums_run(const ImuFactor* d_f, const int* d_fstart, int n_pairs, const double* d_poses, const double* d_sb, int jac_kind,
+                            bool want_jac, double* d_sums, cudaStream_t st, LaunchCounter& lc);
 
 // ---- front-end feature extraction (features.cu; Preprocessing.cpp:529-655)
 constexpr int FEAT_MAX_SHARP = 12, FEAT_MAX_LESS_SHARP = 60, FEAT_MAX_FLAT = 24;   // per ring: 6 sectors x (2, 10, 4)

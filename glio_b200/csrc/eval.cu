@@ -997,7 +997,9 @@ __device__ __forceinline__ void imu_qi_rows(const double q[4], const double t[3]
   for (int m = 0; m < 3; ++m) o[m] = 2.0 * (d[0] * (q[0] * t[m] + uxt[m]) + ut * d[1 + m] + q[1 + m] * td - t[m] * ud - q[0] * txd[m]);
 }
 
-template <bool WANT_JAC>
+// JAC_KIND 0: the tangent columns above.  JAC_KIND 1 (the window marginalisation, MarginalizationFactor.cpp:3-29): the delta lanes
+// take the ambient x, y, z columns of the 4-vector parameter, d = e_{1+k}, in place of [0, e_k] (x) q; every other column is the same.
+template <bool WANT_JAC, int JAC_KIND>
 __global__ void __launch_bounds__(IMU_T) k_imu_pair_sums(const ImuFactor* __restrict__ fl, const int* __restrict__ fstart, int n_pairs,
                                                          const double* __restrict__ poses, const double* __restrict__ sb,
                                                          double* __restrict__ sums) {
@@ -1071,11 +1073,16 @@ __global__ void __launch_bounds__(IMU_T) k_imu_pair_sums(const ImuFactor* __rest
             else if (is_i) { u[m] = -c3[m] * T; u[6 + m] = -c3[m]; }
             else u[6 + m] = c3[m];
           }
-        } else if (blk == 1) {                                       // delta: the ambient block along [0, e_k] (x) q
-          const double* qr = is_i ? Pi + 3 : Pj + 3;
-          const double w = qr[0], x = qr[1], y = qr[2], z = qr[3];
-          const double d[4] = {e == 0 ? -x : e == 1 ? -y : -z, e == 0 ? w : e == 1 ? z : -y,
-                               e == 0 ? -z : e == 1 ? w : x, e == 0 ? y : e == 1 ? -x : w};
+        } else if (blk == 1) {                                       // delta: the ambient block along [0, e_k] (x) q, or e_{1+k}
+          double d[4];
+          if (JAC_KIND == 1) {
+            d[0] = 0.0; d[1] = e == 0 ? 1.0 : 0.0; d[2] = e == 1 ? 1.0 : 0.0; d[3] = e == 2 ? 1.0 : 0.0;
+          } else {
+            const double* qr = is_i ? Pi + 3 : Pj + 3;
+            const double w = qr[0], x = qr[1], y = qr[2], z = qr[3];
+            d[0] = e == 0 ? -x : e == 1 ? -y : -z; d[1] = e == 0 ? w : e == 1 ? z : -y;
+            d[2] = e == 0 ? -z : e == 1 ? w : x; d[3] = e == 0 ? y : e == 1 ? -x : w;
+          }
           double t4[4], o4[4];
           if (is_i) {
             imu_qi_rows(qi, tmp, d, u); imu_qi_rows(qi, tmp1, d, u + 6);
@@ -1177,15 +1184,22 @@ __global__ void __launch_bounds__(256) k_imu_assemble(const double* __restrict__
   }
 }
 
+// the pair sums alone: n_pairs pairs from d_fstart, JAC_KIND jac_kind with want_jac, the cost otherwise
+void eval_imu_pair_sums_run(const ImuFactor* d_f, const int* d_fstart, int n_pairs, const double* d_poses, const double* d_sb, int jac_kind,
+                            bool want_jac, double* d_sums, cudaStream_t st, LaunchCounter& lc) {
+  if (n_pairs <= 0) return;
+  const int nb = (n_pairs + IMU_T / 32 - 1) / (IMU_T / 32);
+  lc.begin(want_jac ? (jac_kind == 1 ? "k_imu_pair_sums_ambient" : "k_imu_pair_sums") : "k_imu_pair_sums_cost", st);
+  (want_jac ? (jac_kind == 1 ? k_imu_pair_sums<true, 1> : k_imu_pair_sums<true, 0>) : k_imu_pair_sums<false, 0>)<<<nb, IMU_T, 0, st>>>(
+      d_f, d_fstart, n_pairs, d_poses, d_sb, d_sums);
+  lc.end(st);
+  GLIO_CUDA_TRY(cudaGetLastError());
+}
+
 void eval_imu_run(const ImuFactor* d_f, const int* d_fstart, int n_pairs, int K, int n_inc_kf, const int* d_kf_inc_start,
-                  const BinIncidence* d_inc, const double* d_poses, const double* d_sb, bool want_jac, double* d_sums, double* d_diag,
-                  double* d_off, cudaStream_t st, LaunchCounter& lc) {
-  if (n_pairs > 0) {
-    const int nb = (n_pairs + IMU_T / 32 - 1) / (IMU_T / 32);
-    lc.begin(want_jac ? "k_imu_pair_sums" : "k_imu_pair_sums_cost", st);
-    (want_jac ? k_imu_pair_sums<true> : k_imu_pair_sums<false>)<<<nb, IMU_T, 0, st>>>(d_f, d_fstart, n_pairs, d_poses, d_sb, d_sums);
-    lc.end(st);
-  }
+                  const BinIncidence* d_inc, const double* d_poses, const double* d_sb, int jac_kind, bool want_jac, double* d_sums,
+                  double* d_diag, double* d_off, cudaStream_t st, LaunchCounter& lc) {
+  eval_imu_pair_sums_run(d_f, d_fstart, n_pairs, d_poses, d_sb, jac_kind, want_jac, d_sums, st, lc);
   const int64_t n = (int64_t)K * NIK + (want_jac ? (int64_t)n_pairs * 225 : 0);
   lc.begin("k_imu_assemble", st);
   (want_jac ? k_imu_assemble<true> : k_imu_assemble<false>)<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(

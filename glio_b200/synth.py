@@ -322,33 +322,15 @@ def _skew(v):
     return np.array([[0.0, -v[2], v[1]], [v[2], 0.0, -v[0]], [-v[1], v[0], 0.0]])
 
 
-def imu_problem(K=200, seed=SEED0 + 18, search_range=6, sig_p=0.02, sig_r=0.005, sig_v=0.03, sig_ba=0.02, sig_bg=0.002):
-    """A level-1-shaped batch problem with IMU factors.  This is generated data, not a pre-integration: no IMU samples are
-    integrated.  pose_graph_problem(level=1)'s trajectory, attitude factors and LiDAR pairs; keyframe times 0.25 .. 0.45 s apart
-    (as in dd_psr_problem); true velocities (central differences of the positions over the times) and slowly drifting biases
-    (sb_true, K x 9: V, Ba, Bg); perturbed initial speed-bias states (sb_init).  One factor per consecutive pair (k, k+1), in
-    order, with T = t_{k+1} - t_k, g = IMU_GRAVITY, linearisation biases off the truth by a little (so Bg_i != linearized_bg),
-    first-order jacobian_ blocks (dp_dba = -T^2/2 I, dv_dba = -T I, dq_dbg = -T I, dp_dbg and dv_dbg of the order of T^2 and T
-    times a small random rotation term), and deltas chosen so that the raw residual at the truth is N(0, sigma) noise.  The
-    covariance is diag(sigma^2) with mild correlations (SPD), and sqrt_info = LLT(covariance^-1).matrixL()^T as ImuFactor forms it.
-    Adds kf_times, sb_true, sb_init, cov (n x 15 x 15) and imu (the factor columns of api.imu_factor_records)."""
-    P = pose_graph_problem(K=K, seed=seed, search_range=search_range, level=1)
-    rng = np.random.default_rng([seed, 2])
-    kf_times = 1_600_000_000.0 + np.concatenate([[0.0], np.cumsum(rng.uniform(0.25, 0.45, K - 1))])
-    T = P["poses_true"]
-    V = np.gradient(T[:, :3], kf_times, axis=0) if K > 1 else np.zeros((K, 3))
-    ba = np.array([0.05, -0.03, 0.02]) + np.cumsum(rng.normal(0.0, 1e-4, (K, 3)), axis=0)
-    bg = np.array([0.002, -0.001, 0.0015]) + np.cumsum(rng.normal(0.0, 1e-5, (K, 3)), axis=0)
-    sb_true = np.concatenate([V, ba, bg], axis=1)
-    sb_init = sb_true + np.concatenate([rng.normal(0.0, 0.1, (K, 3)), rng.normal(0.0, 0.01, (K, 3)), rng.normal(0.0, 1e-3, (K, 3))], axis=1)
-    n = K - 1
-    sig = np.concatenate([np.full(3, sig_p), np.full(3, sig_r), np.full(3, sig_v), np.full(3, sig_ba), np.full(3, sig_bg)])
+def _imu_factor_columns(T, kf_times, V, ba, bg, pairs, sig, rng):
+    """The per-factor recipe of imu_problem for the keyframe pairs (i, j) of `pairs`, in order, at the true poses T, velocities V
+    and biases ba, bg: the factor columns of api.imu_factor_records and the covariances (n x 15 x 15)."""
+    n = len(pairs)
     cols = {k: [] for k in ("i", "j", "sum_dt", "delta_p", "delta_q", "delta_v", "linearized_ba", "linearized_bg", "dp_dba", "dp_dbg",
                             "dq_dbg", "dv_dba", "dv_dbg", "sqrt_info")}
     covs = []
     g = IMU_GRAVITY
-    for k in range(n):
-        i, j = k, k + 1
+    for i, j in pairs:
         dt = kf_times[j] - kf_times[i]
         qi, qj = T[i, 3:], T[j, 3:]
         Ri = quat_to_R(qi)
@@ -379,7 +361,51 @@ def imu_problem(K=200, seed=SEED0 + 18, search_range=6, sig_p=0.02, sig_r=0.005,
                      ("dp_dba", (3, 3)), ("dp_dbg", (3, 3)), ("dq_dbg", (3, 3)), ("dv_dba", (3, 3)), ("dv_dbg", (3, 3)), ("sqrt_info", (15, 15))):
         imu[k] = imu[k].reshape((n,) + shape)
     imu["g_vec"] = np.broadcast_to(g, (n, 3)).copy()
-    P.update(kf_times=kf_times, sb_true=sb_true, sb_init=sb_init, cov=np.asarray(covs).reshape(n, 15, 15), imu=imu)
+    return imu, np.asarray(covs).reshape(n, 15, 15)
+
+
+def imu_problem(K=200, seed=SEED0 + 18, search_range=6, sig_p=0.02, sig_r=0.005, sig_v=0.03, sig_ba=0.02, sig_bg=0.002):
+    """A level-1-shaped batch problem with IMU factors.  This is generated data, not a pre-integration: no IMU samples are
+    integrated.  pose_graph_problem(level=1)'s trajectory, attitude factors and LiDAR pairs; keyframe times 0.25 .. 0.45 s apart
+    (as in dd_psr_problem); true velocities (central differences of the positions over the times) and slowly drifting biases
+    (sb_true, K x 9: V, Ba, Bg); perturbed initial speed-bias states (sb_init).  One factor per consecutive pair (k, k+1), in
+    order, with T = t_{k+1} - t_k, g = IMU_GRAVITY, linearisation biases off the truth by a little (so Bg_i != linearized_bg),
+    first-order jacobian_ blocks (dp_dba = -T^2/2 I, dv_dba = -T I, dq_dbg = -T I, dp_dbg and dv_dbg of the order of T^2 and T
+    times a small random rotation term), and deltas chosen so that the raw residual at the truth is N(0, sigma) noise.  The
+    covariance is diag(sigma^2) with mild correlations (SPD), and sqrt_info = LLT(covariance^-1).matrixL()^T as ImuFactor forms it.
+    Adds kf_times, sb_true, sb_init, cov (n x 15 x 15) and imu (the factor columns of api.imu_factor_records)."""
+    P = pose_graph_problem(K=K, seed=seed, search_range=search_range, level=1)
+    rng = np.random.default_rng([seed, 2])
+    kf_times = 1_600_000_000.0 + np.concatenate([[0.0], np.cumsum(rng.uniform(0.25, 0.45, K - 1))])
+    T = P["poses_true"]
+    V = np.gradient(T[:, :3], kf_times, axis=0) if K > 1 else np.zeros((K, 3))
+    ba = np.array([0.05, -0.03, 0.02]) + np.cumsum(rng.normal(0.0, 1e-4, (K, 3)), axis=0)
+    bg = np.array([0.002, -0.001, 0.0015]) + np.cumsum(rng.normal(0.0, 1e-5, (K, 3)), axis=0)
+    sb_true = np.concatenate([V, ba, bg], axis=1)
+    sb_init = sb_true + np.concatenate([rng.normal(0.0, 0.1, (K, 3)), rng.normal(0.0, 0.01, (K, 3)), rng.normal(0.0, 1e-3, (K, 3))], axis=1)
+    sig = np.concatenate([np.full(3, sig_p), np.full(3, sig_r), np.full(3, sig_v), np.full(3, sig_ba), np.full(3, sig_bg)])
+    imu, cov = _imu_factor_columns(T, kf_times, V, ba, bg, [(k, k + 1) for k in range(K - 1)], sig, rng)
+    P.update(kf_times=kf_times, sb_true=sb_true, sb_init=sb_init, cov=cov, imu=imu)
+    return P
+
+
+def window_imu_problem(W=20, Q=100_000, M=1_000_000, seed=SEED0 + 2, sig_p=0.02, sig_r=0.005, sig_v=0.03, sig_ba=0.02, sig_bg=0.002):
+    """window_problem(W, Q, M, seed) plus the window's IMU chain: one factor per consecutive slot pair (k, k+1), in order, by
+    imu_problem's per-factor recipe at the window's true poses.  Generated data, not a pre-integration.  Keyframe times 0.25 ..
+    0.45 s apart, true velocities (central differences), slowly drifting biases (sb_true, W x 9: V, Ba, Bg) and perturbed initial
+    speed-bias states (sb_init).  Adds kf_times, sb_true, sb_init, cov ((W-1) x 15 x 15) and imu (api.imu_factor_records columns)."""
+    P = window_problem(W=W, Q=Q, M=M, seed=seed)
+    rng = np.random.default_rng([seed, 3])
+    kf_times = 1_600_000_000.0 + np.concatenate([[0.0], np.cumsum(rng.uniform(0.25, 0.45, W - 1))])
+    T = P["poses_true"]
+    V = np.gradient(T[:, :3], kf_times, axis=0) if W > 1 else np.zeros((W, 3))
+    ba = np.array([0.05, -0.03, 0.02]) + np.cumsum(rng.normal(0.0, 1e-4, (W, 3)), axis=0)
+    bg = np.array([0.002, -0.001, 0.0015]) + np.cumsum(rng.normal(0.0, 1e-5, (W, 3)), axis=0)
+    sb_true = np.concatenate([V, ba, bg], axis=1)
+    sb_init = sb_true + np.concatenate([rng.normal(0.0, 0.1, (W, 3)), rng.normal(0.0, 0.01, (W, 3)), rng.normal(0.0, 1e-3, (W, 3))], axis=1)
+    sig = np.concatenate([np.full(3, sig_p), np.full(3, sig_r), np.full(3, sig_v), np.full(3, sig_ba), np.full(3, sig_bg)])
+    imu, cov = _imu_factor_columns(T, kf_times, V, ba, bg, [(k, k + 1) for k in range(W - 1)], sig, rng)
+    P.update(kf_times=kf_times, sb_true=sb_true, sb_init=sb_init, cov=cov, imu=imu)
     return P
 
 

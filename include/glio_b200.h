@@ -241,8 +241,10 @@ int glio_eval_unary_residuals(glio_ctx* ctx, int slot, const double pose_body[7]
 /* ---- the minimizer iteration around K2 (replaces ceres::Solve for the window problem, Estimator.cpp:2424-2433):
  * Ceres 2.0.0 TrustRegionMinimizer + DoglegStrategy + Jacobi scaling + normal-equation Cholesky semantics
  * (ceres.tgz::internal/ceres/{trust_region_minimizer,dogleg_strategy,trust_region_step_evaluator}.cc).
- * LiDAR blocks come from the device; all other factors of the problem (IMU, marginalisation prior, GNSS — host C++
- * by design) are added by the host_factors callback into the same dense tangent-space normal equations. */
+ * LiDAR blocks come from the device, and so does the IMU chain when glio_window_use_imu_factors is on (the factors from the
+ * caller's pre-integration, glio_window_set_imu_factors).  The other factors of the problem (the marginalisation prior, the
+ * first window's speed-bias prior, the IMU chain when the switch is off) are added by the host_factors callback into the same
+ * dense tangent-space normal equations. */
 typedef struct {
   int32_t max_num_iterations;            /* 15 (Estimator.cpp:2427); batch: max_num_iter */
   int32_t dogleg_type;                   /* 0 TRADITIONAL_DOGLEG (window), 1 SUBSPACE_DOGLEG (batch, Estimator.cpp:3280) */
@@ -297,7 +299,8 @@ int glio_window_solve(glio_ctx* ctx, int W, double* poses, double* speed_bias, g
 
 /* Same solve with the host factors accumulating straight into LOWER-BAND storage (entry (i,j), i-hb <= j <= i, at
  * Hband[i*(hb+1) + (j-i+hb)]): no dense n x n scratch.  half_bandwidth must cover every coupling the host factors create
- * (window: prior + IMU chain -> 2*nt-1 = 29 with speed-bias states); < 5 means dense. */
+ * (window: prior + IMU chain -> 2*nt-1 = 29 with speed-bias states); < 5 means dense.  With glio_window_use_imu_factors on, the
+ * band covers the device IMU pairs' span whatever half_bandwidth says. */
 typedef int (*glio_host_factors_band_fn)(void* user, int K, const double* poses, const double* speed_bias, int want_jac,
                                          double* Hband, int hb, double* g, double* cost);
 int glio_window_solve_band(glio_ctx* ctx, int W, double* poses, double* speed_bias, glio_host_factors_band_fn host_factors,
@@ -308,7 +311,8 @@ int glio_window_solve_band(glio_ctx* ctx, int W, double* poses, double* speed_bi
  * prior 15x[t,q,sb] (marginalisation-prior-like), between 15x[t,q,sb|t,q,sb] (IMU-chain-like), range 1x[t,q]
  * (pseudorange-like).  glio_hf_evaluate has the glio_host_factors_fn signature (user = the set).  They exist so the
  * plumbing of host factors + device LiDAR blocks can be tested and benchmarked without ROS / GNSS data; the real
- * ImuFactor / MarginalizationFactor / dd_psr_factor plug in through the same callback (or the Ceres shim). */
+ * MarginalizationFactor / dd_psr_factor plug in through the same callback (or the Ceres shim); the real ImuFactor chain also
+ * runs on the device (glio_window_use_imu_factors, glio_batch_use_imu_factors). */
 typedef struct glio_host_factor_set glio_host_factor_set;
 glio_host_factor_set* glio_hf_create(void);
 void glio_hf_destroy(glio_host_factor_set* s);
@@ -562,7 +566,8 @@ int glio_loop_global_map(glio_loop* lp, int interval, float leaf, int64_t capaci
  * block + 6-vector per keyframe), asks the host callback for the other factors, and does the small dense algebra on the host.
  * Orderings (see glio_b200/csrc/marg.h): marginalisation ordering N = 6W+18 = [KF0: t,q,sb | KF1: t,q,sb | KF k>=2: t,q];
  * the prior keeps n = 6W+3 states, numbered as the NEXT window numbers them (addr_shift, Estimator.cpp:2583-2597).
- * host_marg(user, W, poses, speed_bias, A[N*N], b[N]) ACCUMULATES the non-LiDAR factors (may be NULL). */
+ * host_marg(user, W, poses, speed_bias, A[N*N], b[N]) ACCUMULATES the non-LiDAR factors (may be NULL); with
+ * glio_window_use_imu_factors on, the window's IMU factor KF0 -> KF1 comes from the device instead (see there). */
 typedef int (*glio_host_marg_fn)(void* user, int W, const double* poses, const double* speed_bias, double* A, double* b);
 typedef struct glio_marg_prior glio_marg_prior;
 int glio_window_marginalize(glio_ctx* ctx, int W, const double* poses, const double* speed_bias, glio_host_marg_fn host_marg, void* user,
@@ -894,6 +899,36 @@ int glio_eval_imu_factors(glio_ctx* ctx, int K, const double* poses, const doubl
  * launches without IMU factors.  With the switch on and a non-empty list, speed_bias == NULL or a list that references a keyframe
  * >= K makes glio_batch_solve return GLIO_ERR_ARG.  The other glio_eval_* calls never add IMU blocks. */
 int glio_batch_use_imu_factors(glio_ctx* ctx, int on);
+
+/* ---- K2i in the sliding window: the window problem's IMU chain (Estimator.cpp:2179-2193: ImuFactor(pre_integrations[idx+1])
+ * between window slots), with the factor, the record and the Jacobian described above.  The window keeps its own list, separate
+ * from the batch one: glio_batch_clear and glio_batch_set_imu_factors leave it alone, and this list's calls leave the batch list
+ * alone.  i and j are window slots.  glio_window_slide leaves the list as it is: the reference builds a new problem per window, so
+ * a caller sets a new list for each window. */
+/* Replaces the window IMU list (n = 0 empties it).  The whole list is checked first: i != j, both in [0, 4096) (the window's
+ * size cap), every double finite; a refused or failed call leaves the previous list in place. */
+int glio_window_set_imu_factors(glio_ctx* ctx, const glio_imu_factor* f, int64_t n);
+/* the window IMU pair table (a[k] < b[k]), glio_batch_pair_list's conventions */
+int glio_window_imu_pair_list(glio_ctx* ctx, int64_t capacity, int32_t* a, int32_t* b, int64_t* n_pairs);
+/* The window IMU blocks alone at poses[W*7] and speed_bias[W*9], in glio_eval_imu_factors' layout.  jac_kind 0: the tangent
+ * columns; 1: the quaternion columns are the ambient x, y, z columns of the 15 x 4 blocks (ImuFactor.h:77-100 and :139-150,
+ * rightCols(3), times sqrt_info), what the marginalisation reads.  No all-reduce.  A list that references a slot >= W is
+ * GLIO_ERR_ARG. */
+int glio_eval_window_imu_factors(glio_ctx* ctx, int W, const double* poses, const double* speed_bias, int jac_kind, double* Hdiag,
+                                 double* Hoff, double* g, double* cost);
+/* on != 0 with a non-empty list:
+ * - glio_window_solve and glio_window_solve_band: every evaluation uploads the speed-bias states and queues K2i (tangent columns)
+ *   and the copy of its blocks on the main stream ahead of K2; the host adds the 15 x 15 diagonal and pair blocks into the band at
+ *   15 columns per keyframe, after the LiDAR blocks and the callback's factors.  The band covers the IMU pairs' span (29 for a
+ *   chain) in both forms of the solve.  speed_bias == NULL or a list slot >= W is GLIO_ERR_ARG.  A window with no LiDAR match
+ *   still solves.
+ * - glio_window_marginalize and glio_window_marginalize_async: the device half also queues K2i with the ambient columns over
+ *   the active factors of pair {0, 1} (KF0 -> KF1, Estimator.cpp:2520-2534) ahead of K2; the host half adds that pair's 30 x 30
+ *   block and 30-vector into A and b at the marginalisation ordering (KF0 [0, 15), KF1 [15, 30)), after host_marg's factors.
+ *   Factors that do not touch slot 0 take no part; an active factor between slot 0 and a slot other than 1 is GLIO_ERR_ARG.
+ *   The synchronous and asynchronous priors are the same bit for bit.
+ * Default off; with the switch off or an empty list the solve and the marginalisation launch what they launch without it. */
+int glio_window_use_imu_factors(glio_ctx* ctx, int on);
 
 /* ---- seeded device selection of EDGE correspondences.  The reference selects plane matches only; this library applies the same
  * rules and the same sampler (glio_select_random / glio_batch_select_random, k_sel_sample) to edge lists, with the sizes of a
