@@ -149,7 +149,8 @@ class Context:
                "k_vs_key", "k_vs_hist", "k_vs_scatter", "k_vs_heads", "k_vs_centroid", "k_vs_pack", "k_gm_transform",
                "k_pose_pair_sums", "k_pose_pair_sums_cost", "k_pose_assemble",
                "k_psr_pair_sums", "k_psr_pair_sums_cost", "k_psr_assemble",
-               "k_imu_pair_sums", "k_imu_pair_sums_cost", "k_imu_pair_sums_ambient", "k_imu_assemble"]
+               "k_imu_pair_sums", "k_imu_pair_sums_cost", "k_imu_pair_sums_ambient", "k_imu_assemble",
+               "k_band_chol_solve", "k_band_assemble", "k_band_assemble_g", "k_band_scale", "k_band_shift", "k_band_symv"]
 
     def lib_profile(self, on):
         self._chk(self._lib.glio_profile_enable(self._h, C.c_int(1 if on else 0)))
@@ -1161,6 +1162,51 @@ Context.window_set_imu_factors = _window_set_imu_factors
 Context.window_imu_pair_list = _window_imu_pair_list
 Context.eval_window_imu_factors = _eval_window_imu_factors
 Context.window_use_imu_factors = _window_use_imu_factors
+
+
+# K4: the band Cholesky factor-and-solve on the device
+BAND_MAX_HB = 160                         # GLIO_BAND_MAX_HB: the largest half bandwidth glio_band_solve takes
+
+
+def _band_solve(self, band, b):
+    """glio_band_solve: factor the symmetric band (n, hb+1) (lower band, glio_batch_solve's layout) and solve A x = b on the
+    device.  Returns (L, x, ok): L the factored band in the same layout, x the solution, ok False when a pivot was not positive
+    and finite or x is not finite (then L and x hold partial results)."""
+    L = np.array(band, np.float64, order="C", copy=True)
+    n, w = L.shape
+    rhs = np.ascontiguousarray(b, np.float64).reshape(n)
+    x = np.zeros(n); ok = C.c_int(0)
+    self._chk(self._lib.glio_band_solve(self._h, C.c_int(n), C.c_int(w - 1), _ptr(L), _ptr(rhs), _ptr(x), C.byref(ok)))
+    return L, x, bool(ok.value)
+
+
+Context.band_solve = _band_solve
+
+
+def _batch_use_device_solver(self, on):
+    """glio_batch_use_device_solver: batch solves run the minimizer's band algebra on the device (default off)."""
+    self._chk(self._lib.glio_batch_use_device_solver(self._h, C.c_int(1 if on else 0)))
+
+
+def _batch_normal_equations(self, poses, speed_bias=None, host_factors=None, on_device=False):
+    """glio_batch_normal_equations: (band (n, hb+1), g (n), cost) at one state, by the host path or on the device."""
+    pb = np.ascontiguousarray(poses, np.float64).reshape(-1, 7); K = len(pb)
+    sb = None if speed_bias is None else np.ascontiguousarray(speed_bias, np.float64).reshape(K, 9)
+    n = K * (15 if sb is not None else 6)
+    cap = n * n if n < 4096 else n * 256
+    H = np.zeros(cap); g = np.zeros(n); cost = np.zeros(1); hb = C.c_int(0)
+    if host_factors is None:
+        fn, user = C.cast(None, HOST_FACTORS_BAND_FN), None
+    else:
+        fn, user = C.cast(self._lib.glio_hf_evaluate_band, HOST_FACTORS_BAND_FN), host_factors._h
+    self._chk(self._lib.glio_batch_normal_equations(self._h, C.c_int(K), _ptr(pb), _ptr(sb), fn, user, C.c_int(1 if on_device else 0),
+                                                    C.c_int64(cap), _ptr(H), C.byref(hb), _ptr(g), _ptr(cost)))
+    w = hb.value + 1
+    return H[:n * w].reshape(n, w).copy(), g, float(cost[0])
+
+
+Context.batch_use_device_solver = _batch_use_device_solver
+Context.batch_normal_equations = _batch_normal_equations
 
 
 # ---------------------------------------------------------------------------------------------------

@@ -261,6 +261,12 @@ struct glio_ctx {
   // what the marginalisation needs of the list's slot 0: the index of pair {0, 1} when an active factor joins slots 0 and 1 (-1
   // otherwise), and whether an active factor joins slot 0 to another slot
   int wimu_pair01 = -1; bool wimu_slot0_elsewhere = false;
+  // glio_band_solve (K4): the band, right-hand side, solution and success flag, grown to the largest system solved
+  DevBuf<double> band_a, band_b, band_x; DevBuf<int> band_flag;
+  // glio_batch_use_device_solver: the device minimizer's bands (H, Hc, Hs, A), vectors and assembly plan, reserved per shape
+  bool batch_device_solver = false;
+  DevBuf<double> dm_H[2], dm_g, dm_Hs, dm_A, dm_v1, dm_v2, dm_v3; DevBuf<int> dm_flag;
+  DevBuf<BandBlock> dm_blocks; DevBuf<BandContrib> dm_contrib; PinnedBuf<double> dm_h1, dm_h2;
 
   Slot& slot(int k) {
     GLIO_REQUIRE(k >= 0 && k < 4096, GLIO_ERR_ARG, "slot index out of range");
@@ -2813,6 +2819,184 @@ int glio_batch_set_pair_matches(glio_ctx* c, int cur, int oth, const float* cp, 
   });
 }
 
+namespace {
+
+// One batch problem as glio_batch_solve sees it: the state layout, the off-diagonal block order, the band's half bandwidth, and
+// the evaluation of its normal equations into a host band (the host path) or into a device band (the device minimizer).
+struct BatchProblem {
+  glio_ctx* c; int K; bool sb; StateLayout L; int nt, n, hb;
+  bool add_pose, add_dd, add_imu;
+  glio_host_factors_band_fn host_factors; void* user;
+  std::vector<std::pair<int, int>> off;
+  std::vector<double> pz, sz;
+  int n_blocks = 0; bool plan_ready = false;
+  BandMat hcb;                      // the callback's band of the device path
+  BatchProblem(glio_ctx* c_, int K_, bool sb_, glio_host_factors_band_fn hf, void* u, const char* who)
+      : c(c_), K(K_), sb(sb_), L(K_, sb_), nt(L.nt), n(K_ * L.nt), host_factors(hf), user(u), pz((size_t)K_ * 7), sz((size_t)K_ * 9) {
+    add_pose = c->pose.use && !c->pose.pairs.empty(); add_dd = c->dd.use && !c->dd.pairs.empty();
+    add_imu = c->imu.use && !c->imu.pairs.empty();
+    require_lists_within(c, K, add_pose, add_dd, who);
+    GLIO_REQUIRE(!add_imu || sb, GLIO_ERR_ARG, std::string(who) + ": the IMU factors need speed_bias");
+    GLIO_REQUIRE(!add_imu || c->imu.max_kf < K, GLIO_ERR_ARG, std::string(who) + ": an IMU factor references a keyframe outside [0, K)");
+    // the keyframe pair of each off-diagonal block, in the evaluation's order: LiDAR pairs (cur, oth), then pose pairs (a, b), then
+    // DD pairs (a, b)
+    off = lidar_pairs(c);
+    if (add_pose) off.insert(off.end(), c->pose.pairs.begin(), c->pose.pairs.end());
+    if (add_dd) off.insert(off.end(), c->dd.pairs.begin(), c->dd.pairs.end());
+    int span = 1;
+    for (const auto& p : off) span = std::max(span, std::abs(p.first - p.second));
+    if (add_imu) for (const auto& p : c->imu.pairs) span = std::max(span, p.second - p.first);
+    hb = std::min((span + 1) * nt - 1, std::max(n - 1, 0));   // BandMat::reset's clamp
+  }
+  // the device blocks of one evaluation at the ambient state xa, and the host callback into the freshly reset band H (may be the
+  // callback band of the device path); the cost as the host path sums it.  false: the callback failed.
+  bool evaluate(const double* xa, bool want_jac, double* cost, BandMat* H, double* g) {
+    L.unpack(xa, pz.data(), sz.data());
+    // the device evaluates the LiDAR pairs (and a sharded run sums them over the ranks) while the host evaluates its own
+    // factors into the freshly reset band; the device blocks are added when they have arrived
+    eval_blocks_launch(c, K, pz.data(), want_jac, c->batch_use_edges ? BIN_PLANES_EDGES : BIN_PLANES, add_pose, add_dd);
+    if (add_imu) imu_blocks_launch(c, c->imu, K, c->d_bin_poses.p, sz.data(), 0, want_jac, true);
+    double ct = 0;
+    int hrc = 0;
+    if (want_jac) { H->reset(n, hb); std::fill(g, g + n, 0.0); }
+    if (host_factors) hrc = host_factors(user, K, pz.data(), sb ? sz.data() : nullptr, want_jac ? 1 : 0, want_jac ? H->a.data() : nullptr, want_jac ? H->hb : 0, g, &ct);
+    GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
+    if (hrc != 0) return false;
+    for (int k = 0; k < K; ++k) ct += c->h_bin_diag.p[(size_t)k * GLIO_NACC + 27];
+    if (add_imu) for (int k = 0; k < K; ++k) ct += c->imu.h_diag.p[(size_t)k * GLIO_NACC_IMU_KF + 240];
+    *cost = ct;
+    return std::isfinite(ct);
+  }
+  // the host path: the blocks that have arrived added into H and g in the order LiDAR / pose / DD diagonal and off-diagonal, IMU
+  void host_add(BandMat* H, double* g) {
+    const int w = H->hb + 1;
+    double* a = H->a.data();
+    add_diag_blocks(H, c->h_bin_diag.p, K, nt);
+    for (int k = 0; k < K; ++k) for (int p = 0; p < 6; ++p) g[nt * k + p] += c->h_bin_diag.p[(size_t)k * GLIO_NACC + 21 + p];
+    for (size_t pi = 0; pi < off.size(); ++pi) {
+      const int kc = off[pi].first, ko = off[pi].second;
+      const double* ob = c->h_bin_off.p + pi * 36;                 // d2 cost / d x_cur[p] d x_oth[q]
+      if (kc > ko) {                                               // rows of cur, six contiguous band entries each
+        for (int p = 0; p < 6; ++p) { double* row = a + (size_t)(nt * kc + p) * w + (nt * ko - (nt * kc + p) + H->hb); for (int q = 0; q < 6; ++q) row[q] += ob[6 * p + q]; }
+      } else if (kc < ko) {                                        // stored transposed: rows of oth
+        for (int q = 0; q < 6; ++q) { double* row = a + (size_t)(nt * ko + q) * w + (nt * kc - (nt * ko + q) + H->hb); for (int p = 0; p < 6; ++p) row[p] += ob[6 * p + q]; }
+      } else {
+        for (int p = 0; p < 6; ++p) for (int q = 0; q < 6; ++q) H->add_sym(nt * kc + p, nt * ko + q, ob[6 * p + q]);
+      }
+    }
+    if (add_imu) { double unused = 0; add_imu_blocks(c->imu, K, true, H, g, unused); }   // the IMU blocks after all others
+  }
+  bool host_eval(const double* xa, bool want_jac, double* cost, BandMat* H, double* g) {
+    if (!evaluate(xa, want_jac, cost, H, g)) return false;
+    if (want_jac) host_add(H, g);
+    return true;
+  }
+  // the assembly plan of the device path (once per problem): per band block its contributions in the host path's order
+  void build_plan() {
+    if (plan_ready) return;
+    std::map<std::pair<int, int>, std::vector<BandContrib>> per;
+    for (int k = 0; k < K; ++k) per[{k, k}].push_back(BandContrib{BAND_DIAG6, k});
+    for (size_t pi = 0; pi < off.size(); ++pi) {
+      const int kc = off[pi].first, ko = off[pi].second;
+      if (kc > ko) per[{kc, ko}].push_back(BandContrib{BAND_OFF6, (int)pi});
+      else per[{ko, kc}].push_back(BandContrib{BAND_OFF6_T, (int)pi});
+    }
+    if (add_imu) {
+      for (int k = 0; k < K; ++k) per[{k, k}].push_back(BandContrib{BAND_IMU_DIAG, k});
+      for (size_t pi = 0; pi < c->imu.pairs.size(); ++pi) per[{c->imu.pairs[pi].second, c->imu.pairs[pi].first}].push_back(BandContrib{BAND_IMU_OFF_T, (int)pi});
+    }
+    std::vector<BandBlock> blocks; std::vector<BandContrib> contrib;
+    for (auto& kv : per) {
+      blocks.push_back(BandBlock{kv.first.first, kv.first.second, (int)contrib.size(), (int)(contrib.size() + kv.second.size())});
+      contrib.insert(contrib.end(), kv.second.begin(), kv.second.end());
+    }
+    n_blocks = (int)blocks.size();
+    c->dm_blocks.reserve(blocks.size() + 1); c->dm_contrib.reserve(contrib.size() + 1);
+    GLIO_CUDA_TRY(cudaMemcpyAsync(c->dm_blocks.p, blocks.data(), blocks.size() * sizeof(BandBlock), cudaMemcpyHostToDevice, c->st));
+    GLIO_CUDA_TRY(cudaMemcpyAsync(c->dm_contrib.p, contrib.data(), contrib.size() * sizeof(BandContrib), cudaMemcpyHostToDevice, c->st));
+    GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
+    plan_ready = true;
+  }
+  // the device path: the callback's band and g uploaded, then the device blocks gathered onto them (k_band_assemble) into d_H;
+  // g comes back to the host
+  bool device_eval(const double* xa, bool want_jac, double* cost, double* d_H, double* g) {
+    if (!evaluate(xa, want_jac, cost, &hcb, g)) return false;
+    if (!want_jac) return true;
+    build_plan();
+    const size_t nb = (size_t)n * (hb + 1);
+    if (host_factors) GLIO_CUDA_TRY(cudaMemcpyAsync(d_H, hcb.a.data(), nb * sizeof(double), cudaMemcpyHostToDevice, c->st));
+    else GLIO_CUDA_TRY(cudaMemsetAsync(d_H, 0, nb * sizeof(double), c->st));
+    GLIO_CUDA_TRY(cudaMemcpyAsync(c->dm_g.p, g, (size_t)n * sizeof(double), cudaMemcpyHostToDevice, c->st));
+    band_assemble_run(d_H, hb, nt, c->dm_blocks.p, n_blocks, c->dm_contrib.p, c->d_bin_diag.p, c->d_bin_off.p,
+                      add_imu ? c->imu.d_diag.p : nullptr, add_imu ? c->imu.d_off.p : nullptr, c->dm_g.p, n, c->st, c->lc);
+    GLIO_CUDA_TRY(cudaMemcpyAsync(g, c->dm_g.p, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, c->st));
+    GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
+    return true;
+  }
+};
+
+// The minimizer's band operations on the device: H and Hc in c->dm_H, Hs, A; n-vectors through pinned staging
+struct DeviceBandOps : BandOps {
+  BatchProblem& P; glio_ctx* c; int n, hb; int cur = 0;
+  explicit DeviceBandOps(BatchProblem& p) : P(p), c(p.c), n(p.n), hb(p.hb) {
+    const size_t nb = (size_t)n * (hb + 1);
+    GLIO_REQUIRE(hb <= GLIO_BAND_MAX_HB, GLIO_ERR_ARG, "glio_batch_solve: the device solver needs a half bandwidth <= GLIO_BAND_MAX_HB (160)");
+    c->dm_H[0].reserve(nb); c->dm_H[1].reserve(nb); c->dm_Hs.reserve(nb); c->dm_A.reserve(nb);
+    c->dm_g.reserve(n); c->dm_v1.reserve(n); c->dm_v2.reserve(n); c->dm_v3.reserve(n); c->dm_flag.reserve(1);
+    c->dm_h1.reserve(n); c->dm_h2.reserve(n);
+    P.hcb.reset(n, hb);
+  }
+  bool eval(const double* x, bool want_jac, double* cost, int slot, double* g) override {
+    return P.device_eval(x, want_jac, cost, c->dm_H[slot ? 1 - cur : cur].p, g);
+  }
+  bool shape_ok(int) const override { return true; }
+  void down(const double* d, double* h) {
+    GLIO_CUDA_TRY(cudaMemcpyAsync(c->dm_h1.p, d, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, c->st));
+    GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
+    memcpy(h, c->dm_h1.p, (size_t)n * sizeof(double));
+  }
+  void up(const double* h, double* d) {
+    memcpy(c->dm_h2.p, h, (size_t)n * sizeof(double));
+    GLIO_CUDA_TRY(cudaMemcpyAsync(d, c->dm_h2.p, (size_t)n * sizeof(double), cudaMemcpyHostToDevice, c->st));
+  }
+  void diag(double* d) override {
+    GLIO_CUDA_TRY(cudaMemcpy2DAsync(c->dm_h1.p, sizeof(double), c->dm_H[cur].p + hb, (hb + 1) * sizeof(double), sizeof(double), n,
+                                    cudaMemcpyDeviceToHost, c->st));
+    GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
+    memcpy(d, c->dm_h1.p, (size_t)n * sizeof(double));
+  }
+  void scale(const double* s, double* hs_diag) override {
+    up(s, c->dm_v1.p);
+    band_scale_run(c->dm_H[cur].p, c->dm_Hs.p, c->dm_v1.p, n, hb, c->dm_v2.p, c->st, c->lc);
+    down(c->dm_v2.p, hs_diag);
+  }
+  bool shifted_solve(const double* v, const double* rhs, double* y) override {
+    up(v, c->dm_v1.p);
+    GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));   // the staging buffer is reused for rhs
+    up(rhs, c->dm_v2.p);
+    band_shift_run(c->dm_Hs.p, c->dm_A.p, c->dm_v1.p, n, hb, c->st, c->lc);
+    band_chol_solve_run(c->dm_A.p, c->dm_v2.p, c->dm_v3.p, n, hb, c->dm_flag.p, c->st, c->lc);
+    int ok = 0;
+    GLIO_CUDA_TRY(cudaMemcpyAsync(&ok, c->dm_flag.p, sizeof(int), cudaMemcpyDeviceToHost, c->st));
+    down(c->dm_v3.p, y);
+    return ok == 1;
+  }
+  void symv(const double* x, double* y) override {
+    up(x, c->dm_v1.p);
+    band_symv_run(c->dm_Hs.p, c->dm_v1.p, c->dm_v2.p, n, hb, c->st, c->lc);
+    down(c->dm_v2.p, y);
+  }
+  void swap() override { cur = 1 - cur; }
+};
+
+}  // namespace
+
+int glio_batch_use_device_solver(glio_ctx* c, int on) {
+  if (!c) return GLIO_ERR_ARG;
+  c->batch_device_solver = on != 0;
+  return GLIO_OK;
+}
+
 int glio_batch_solve(glio_ctx* c, int K, double* poses, double* speed_bias, glio_host_factors_band_fn host_factors, void* user,
                      const glio_solver_options* options, glio_solver_summary* summary, glio_iteration* iter_log, int iter_cap,
                      double* step_log, int64_t step_cap) {
@@ -2822,67 +3006,69 @@ int glio_batch_solve(glio_ctx* c, int K, double* poses, double* speed_bias, glio
     glio_solver_options o;
     if (options) o = *options;
     else { glio_default_solver_options(&o); o.dogleg_type = 1; o.use_nonmonotonic_steps = 1; o.max_num_iterations = 100; }  // Estimator.cpp:3276-3281
-    const bool sb = speed_bias != nullptr;
-    const StateLayout L(K, sb);
-    const int nt = L.nt, n = K * nt;
-    const bool add_pose = c->pose.use && !c->pose.pairs.empty(), add_dd = c->dd.use && !c->dd.pairs.empty();
-    const bool add_imu = c->imu.use && !c->imu.pairs.empty();
-    require_lists_within(c, K, add_pose, add_dd, "glio_batch_solve");
-    GLIO_REQUIRE(!add_imu || sb, GLIO_ERR_ARG, "glio_batch_solve: the IMU factors need speed_bias");
-    GLIO_REQUIRE(!add_imu || c->imu.max_kf < K, GLIO_ERR_ARG, "glio_batch_solve: an IMU factor references a keyframe outside [0, K)");
-    // the keyframe pair of each off-diagonal block, in the evaluation's order: LiDAR pairs (cur, oth), then pose pairs (a, b), then
-    // DD pairs (a, b)
-    std::vector<std::pair<int, int>> off = lidar_pairs(c);
-    if (add_pose) off.insert(off.end(), c->pose.pairs.begin(), c->pose.pairs.end());
-    if (add_dd) off.insert(off.end(), c->dd.pairs.begin(), c->dd.pairs.end());
-    int span = 1;
-    for (const auto& p : off) span = std::max(span, std::abs(p.first - p.second));
-    if (add_imu) for (const auto& p : c->imu.pairs) span = std::max(span, p.second - p.first);
-    const int hb = (span + 1) * nt - 1;
-    TrustRegionDogleg solver(L.blocks(), solver_options_from(o));
-    std::vector<double> x((size_t)K * L.na), pz((size_t)K * 7), sz((size_t)K * 9);
-    L.pack(poses, speed_bias, x.data());
-    EvalFn eval = [&](const double* xa, bool want_jac, double* cost, BandMat* H, double* g) -> bool {
-      L.unpack(xa, pz.data(), sz.data());
-      // the device evaluates the LiDAR pairs (and a sharded run sums them over the ranks) while the host evaluates its own
-      // factors into the freshly reset band; the device blocks are added when they have arrived
-      eval_blocks_launch(c, K, pz.data(), want_jac, c->batch_use_edges ? BIN_PLANES_EDGES : BIN_PLANES, add_pose, add_dd);
-      if (add_imu) imu_blocks_launch(c, c->imu, K, c->d_bin_poses.p, sz.data(), 0, want_jac, true);
-      double ct = 0;
-      int hrc = 0;
-      if (want_jac) { H->reset(n, hb); std::fill(g, g + n, 0.0); }
-      if (host_factors) hrc = host_factors(user, K, pz.data(), sb ? sz.data() : nullptr, want_jac ? 1 : 0, want_jac ? H->a.data() : nullptr, want_jac ? H->hb : 0, g, &ct);
-      GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
-      if (hrc != 0) return false;
-      for (int k = 0; k < K; ++k) ct += c->h_bin_diag.p[(size_t)k * GLIO_NACC + 27];
-      if (want_jac) {
-        const int w = H->hb + 1;
-        double* a = H->a.data();
-        add_diag_blocks(H, c->h_bin_diag.p, K, nt);
-        for (int k = 0; k < K; ++k) for (int p = 0; p < 6; ++p) g[nt * k + p] += c->h_bin_diag.p[(size_t)k * GLIO_NACC + 21 + p];
-        for (size_t pi = 0; pi < off.size(); ++pi) {
-          const int kc = off[pi].first, ko = off[pi].second;
-          const double* ob = c->h_bin_off.p + pi * 36;                 // d2 cost / d x_cur[p] d x_oth[q]
-          if (kc > ko) {                                               // rows of cur, six contiguous band entries each
-            for (int p = 0; p < 6; ++p) { double* row = a + (size_t)(nt * kc + p) * w + (nt * ko - (nt * kc + p) + H->hb); for (int q = 0; q < 6; ++q) row[q] += ob[6 * p + q]; }
-          } else if (kc < ko) {                                        // stored transposed: rows of oth
-            for (int q = 0; q < 6; ++q) { double* row = a + (size_t)(nt * ko + q) * w + (nt * kc - (nt * ko + q) + H->hb); for (int p = 0; p < 6; ++p) row[p] += ob[6 * p + q]; }
-          } else {
-            for (int p = 0; p < 6; ++p) for (int q = 0; q < 6; ++q) H->add_sym(nt * kc + p, nt * ko + q, ob[6 * p + q]);
-          }
-        }
-      }
-      if (add_imu) add_imu_blocks(c->imu, K, want_jac, H, g, ct);   // the IMU blocks after all others
-      *cost = ct;
-      return std::isfinite(ct);
-    };
+    BatchProblem P(c, K, speed_bias != nullptr, host_factors, user, "glio_batch_solve");
+    TrustRegionDogleg solver(P.L.blocks(), solver_options_from(o));
+    std::vector<double> x((size_t)K * P.L.na);
+    P.L.pack(poses, speed_bias, x.data());
     SolverSummary S;
-    solver.solve(x.data(), eval, &S);
-    L.unpack(x.data(), poses, speed_bias);
-    fill_summary(S, n, summary, iter_log, iter_cap, step_log, step_cap);
+    if (c->batch_device_solver) {
+      DeviceBandOps ops(P);
+      solver.solve(x.data(), ops, &S);
+    } else {
+      EvalFn eval = [&](const double* xa, bool want_jac, double* cost, BandMat* H, double* g) -> bool { return P.host_eval(xa, want_jac, cost, H, g); };
+      solver.solve(x.data(), eval, &S);
+    }
+    P.L.unpack(x.data(), poses, speed_bias);
+    fill_summary(S, P.n, summary, iter_log, iter_cap, step_log, step_cap);
   });
 }
 
+int glio_batch_normal_equations(glio_ctx* c, int K, const double* poses, const double* speed_bias, glio_host_factors_band_fn host_factors,
+                                void* user, int on_device, int64_t capacity, double* Hband, int* hb, double* g, double* cost) {
+  if (!c) return GLIO_ERR_ARG;
+  return guarded(c, [&] {
+    GLIO_REQUIRE(K > 0 && poses && hb && g && cost, GLIO_ERR_ARG, "glio_batch_normal_equations: need K > 0, poses, hb, g and cost");
+    BatchProblem P(c, K, speed_bias != nullptr, host_factors, user, "glio_batch_normal_equations");
+    *hb = P.hb;
+    const size_t nb = (size_t)P.n * (P.hb + 1);
+    GLIO_REQUIRE(Hband && capacity >= (int64_t)nb, GLIO_ERR_ARG, "glio_batch_normal_equations: capacity smaller than n * (hb + 1)");
+    std::vector<double> x((size_t)K * P.L.na);
+    P.L.pack(poses, speed_bias, x.data());
+    bool ok;
+    if (on_device) {
+      GLIO_REQUIRE(P.hb <= GLIO_BAND_MAX_HB, GLIO_ERR_ARG, "glio_batch_normal_equations: the device path needs hb <= GLIO_BAND_MAX_HB (160)");
+      c->dm_H[0].reserve(nb); c->dm_g.reserve(P.n); P.hcb.reset(P.n, P.hb);
+      ok = P.device_eval(x.data(), true, cost, c->dm_H[0].p, g);
+      if (ok) {
+        GLIO_CUDA_TRY(cudaMemcpyAsync(Hband, c->dm_H[0].p, nb * sizeof(double), cudaMemcpyDeviceToHost, c->st));
+        GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
+      }
+    } else {
+      BandMat H;
+      ok = P.host_eval(x.data(), true, cost, &H, g);
+      if (ok) memcpy(Hband, H.a.data(), nb * sizeof(double));
+    }
+    GLIO_REQUIRE(ok, GLIO_ERR_NUMERIC, "glio_batch_normal_equations: the host callback failed or the cost is not finite");
+  });
+}
+
+
+int glio_band_solve(glio_ctx* c, int n, int hb, double* band, const double* b, double* x, int* ok) {
+  if (!c) return GLIO_ERR_ARG;
+  return guarded(c, [&] {
+    GLIO_REQUIRE(n > 0 && band && b && x && ok, GLIO_ERR_ARG, "glio_band_solve: need n > 0 and band, b, x, ok");
+    GLIO_REQUIRE(hb >= 0 && hb <= GLIO_BAND_MAX_HB, GLIO_ERR_ARG, "glio_band_solve: need 0 <= hb <= GLIO_BAND_MAX_HB (160)");
+    const size_t nb = (size_t)n * (hb + 1);
+    c->band_a.reserve(nb); c->band_b.reserve((size_t)n); c->band_x.reserve((size_t)n); c->band_flag.reserve(1);
+    GLIO_CUDA_TRY(cudaMemcpyAsync(c->band_a.p, band, nb * sizeof(double), cudaMemcpyHostToDevice, c->st));
+    GLIO_CUDA_TRY(cudaMemcpyAsync(c->band_b.p, b, (size_t)n * sizeof(double), cudaMemcpyHostToDevice, c->st));
+    band_chol_solve_run(c->band_a.p, c->band_b.p, c->band_x.p, n, hb, c->band_flag.p, c->st, c->lc);
+    GLIO_CUDA_TRY(cudaMemcpyAsync(band, c->band_a.p, nb * sizeof(double), cudaMemcpyDeviceToHost, c->st));
+    GLIO_CUDA_TRY(cudaMemcpyAsync(x, c->band_x.p, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, c->st));
+    GLIO_CUDA_TRY(cudaMemcpyAsync(ok, c->band_flag.p, sizeof(int), cudaMemcpyDeviceToHost, c->st));
+    GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
+  });
+}
 
 // ---- K2e: edge correspondences are an input (the reference has no edge association, SURVEY fact 1)
 int glio_set_edges(glio_ctx* c, int slot, const float* cp, const float* pa, const float* pb, const double* s, int64_t n) {

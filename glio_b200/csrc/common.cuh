@@ -507,4 +507,22 @@ struct GlobalMapSeg { const float* xyz; int64_t n, off; double t[3], q[4]; };
 void loop_global_map_cloud(const GlobalMapSeg* d_segs, int nseg, int64_t n_max, const double t_first[3], const double q_first[4], float4* out,
                            cudaStream_t st, LaunchCounter& lc);
 
+// ---- K4 (band.cu): band Cholesky factor-and-solve in one thread block (glio_band_solve).  d_band[n*(hb+1)] in A, out L;
+// d_x[n] out; d_flag[0] = 1 on success, 0 on a pivot that is not positive and finite or a non-finite x.  Needs
+// band_chol_smem_bytes(hb) of shared memory; hb <= GLIO_BAND_MAX_HB fits.
+size_t band_chol_smem_bytes(int hb);
+void band_chol_solve_run(double* d_band, const double* d_b, double* d_x, int n, int hb, int* d_flag, cudaStream_t st, LaunchCounter& lc);
+// The device minimizer's band passes (glio_batch_use_device_solver).  The assembly plan: per nt x nt band block (ka, kb), ka >= kb,
+// its contributions [c0, c1) in the host path's order; BAND_*_T blocks are read transposed.
+enum BandContribKind { BAND_DIAG6 = 0, BAND_OFF6 = 1, BAND_OFF6_T = 2, BAND_IMU_DIAG = 3, BAND_IMU_OFF_T = 4 };
+struct BandContrib { int32_t kind, idx; };
+struct BandBlock { int32_t ka, kb, c0, c1; };
+// d_H / d_g already hold the host callback's band and g (or zeros)
+void band_assemble_run(double* d_H, int hb, int nt, const BandBlock* d_blocks, int n_blocks, const BandContrib* d_contrib,
+                       const double* d_diag6, const double* d_off6, const double* d_imu_diag, const double* d_imu_off, double* d_g, int n,
+                       cudaStream_t st, LaunchCounter& lc);
+void band_scale_run(const double* d_H, double* d_Hs, const double* d_s, int n, int hb, double* d_hs_diag, cudaStream_t st, LaunchCounter& lc);
+void band_shift_run(const double* d_Hs, double* d_A, const double* d_v, int n, int hb, cudaStream_t st, LaunchCounter& lc);
+void band_symv_run(const double* d_Hs, const double* d_x, double* d_y, int n, int hb, cudaStream_t st, LaunchCounter& lc);
+
 }  // namespace glio

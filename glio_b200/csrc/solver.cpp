@@ -120,11 +120,11 @@ namespace {
 inline double dot(const std::vector<double>& a, const std::vector<double>& b) { double s = 0; for (size_t i = 0; i < a.size(); ++i) s += a[i] * b[i]; return s; }
 inline double norm(const std::vector<double>& a) { return std::sqrt(dot(a, a)); }
 // y = A x for a symmetric matrix in lower-band storage
-inline void symv(const BandMat& A, const std::vector<double>& x, std::vector<double>& y) {
+inline void symv(const BandMat& A, const double* x, double* y) {
   const int n = A.n, hb = A.hb, w = hb + 1;
 #if defined(__x86_64__)
   static const bool fast = __builtin_cpu_supports("avx2") && __builtin_cpu_supports("fma") && std::getenv("GLIO_NO_AVX2") == nullptr;
-  if (fast && hb >= 4) { detail::symv_avx2(A, x.data(), y.data()); return; }
+  if (fast && hb >= 4) { detail::symv_avx2(A, x, y); return; }
 #endif
   for (int i = 0; i < n; ++i) y[i] = 0.0;
   for (int i = 0; i < n; ++i) {
@@ -153,24 +153,56 @@ struct StepEvaluator {
   }
 };
 
+// the band operations in host memory: the evaluator's BandMat, the band Cholesky and symv above
+struct HostBandOps : BandOps {
+  const EvalFn& fn;
+  BandMat H, Hc, Hs, A;
+  explicit HostBandOps(const EvalFn& f) : fn(f) {}
+  bool eval(const double* x, bool want_jac, double* cost, int slot, double* g) override {
+    return fn(x, want_jac, cost, want_jac ? (slot ? &Hc : &H) : nullptr, g);
+  }
+  bool shape_ok(int n) const override { return H.n == n; }
+  void diag(double* d) override { for (int i = 0; i < H.n; ++i) d[i] = H.at(i, i); }
+  void scale(const double* scale, double* hs_diag) override {
+    const int n = H.n, hb = H.hb, w = hb + 1;
+    Hs.n = H.n; Hs.hb = H.hb; Hs.a.resize(H.a.size());
+    for (int i = 0; i < n; ++i) {
+      const double si = scale[i];
+      for (int j = std::max(0, i - hb); j <= i; ++j) Hs.a[(size_t)i * w + (j - i + hb)] = H.a[(size_t)i * w + (j - i + hb)] * si * scale[j];
+      hs_diag[i] = Hs.at(i, i);
+    }
+  }
+  bool shifted_solve(const double* v, const double* rhs, double* y) override {
+    A = Hs;
+    for (int i = 0; i < A.n; ++i) A.at(i, i) += v[i] * v[i];
+    return detail::cholesky_solve(A, rhs, y);
+  }
+  void symv(const double* x, double* y) override { glio::symv(Hs, x, y); }
+  void swap() override { std::swap(H, Hc); }
+};
+
 }  // namespace
 
 void TrustRegionDogleg::solve(double* x_io, const EvalFn& eval_user, SolverSummary* sum) {
+  HostBandOps ops(eval_user);
+  solve(x_io, ops, sum);
+}
+
+void TrustRegionDogleg::solve(double* x_io, BandOps& ops, SolverSummary* sum) {
   const int n = n_, na = n_amb_;
   SolverSummary& S = *sum;
   S = SolverSummary();
   typedef std::chrono::steady_clock clk;
   const auto t_begin = clk::now();
-  auto eval = [&](const double* xx, bool wj, double* cst, BandMat* HH, double* gg) -> bool {
+  auto eval = [&](const double* xx, bool wj, double* cst, int slot, double* gg) -> bool {
     const auto t0 = clk::now();
-    const bool ok = eval_user(xx, wj, cst, HH, gg);
+    const bool ok = ops.eval(xx, wj, cst, slot, gg);
     S.eval_seconds += std::chrono::duration<double>(clk::now() - t0).count();
     return ok;
   };
   struct Fin { SolverSummary& s; clk::time_point t; ~Fin() { s.total_seconds = std::chrono::duration<double>(clk::now() - t).count(); } } fin{S, t_begin};
   std::vector<double> x(x_io, x_io + na), cand(na), proj(na);
-  BandMat H, Hs, Hc, A;
-  std::vector<double> g(n), gs(n), gc(n);
+  std::vector<double> g(n), gs(n), gc(n), hs_diag(n), hdiag(n), shift(n);
   std::vector<double> scale(n, 1.0), diag(n), grad_d(n), gn(n), step(n), delta(n), tmp(n), tmp2(n), y(n), negg(n);
   double x_cost = 0, cand_cost = 0, minimum_cost = std::numeric_limits<double>::max(), model_cost_change = 0;
   double x_norm = -1;  // trust_region_minimizer.cc:175 "Invalid value"
@@ -184,13 +216,8 @@ void TrustRegionDogleg::solve(double* x_io, const EvalFn& eval_user, SolverSumma
   bool sub_1d = false;
 
   auto apply_scaling = [&]() {
-    Hs.n = H.n; Hs.hb = H.hb; Hs.a.resize(H.a.size());
-    const int hb = H.hb, w = hb + 1;
-    for (int i = 0; i < n; ++i) {
-      const double si = scale[i];
-      for (int j = std::max(0, i - hb); j <= i; ++j) Hs.a[(size_t)i * w + (j - i + hb)] = H.a[(size_t)i * w + (j - i + hb)] * si * scale[j];
-      gs[i] = g[i] * si;
-    }
+    ops.scale(scale.data(), hs_diag.data());
+    for (int i = 0; i < n; ++i) gs[i] = g[i] * scale[i];
   };
   auto gradient_norms = [&](IterationRecord& it) {
     for (int i = 0; i < n; ++i) negg[i] = -g[i];
@@ -286,7 +313,7 @@ void TrustRegionDogleg::solve(double* x_io, const EvalFn& eval_user, SolverSumma
     sub_g[0] = dot(basis0, grad_d); sub_g[1] = dot(basis1, grad_d);
     for (int i = 0; i < n; ++i) { tmp[i] = basis0[i] / diag[i]; tmp2[i] = basis1[i] / diag[i]; }
     std::vector<double> h0(n), h1(n);
-    symv(Hs, tmp, h0); symv(Hs, tmp2, h1);
+    ops.symv(tmp.data(), h0.data()); ops.symv(tmp2.data(), h1.data());
     sub_B[0] = dot(tmp, h0); sub_B[1] = dot(tmp, h1); sub_B[2] = sub_B[1]; sub_B[3] = dot(tmp2, h1);
     return true;
   };
@@ -297,13 +324,12 @@ void TrustRegionDogleg::solve(double* x_io, const EvalFn& eval_user, SolverSumma
   const bool lm = opt_.trust_region_strategy == 1;
   double lm_decrease = 2.0;
   auto lm_compute_step = [&]() -> int {
-    if (!reuse) for (int i = 0; i < n; ++i) diag[i] = std::min(std::max(Hs.at(i, i), opt_.min_lm_diagonal), opt_.max_lm_diagonal);
+    if (!reuse) for (int i = 0; i < n; ++i) diag[i] = std::min(std::max(hs_diag[i], opt_.min_lm_diagonal), opt_.max_lm_diagonal);
     reuse = true;
-    A = Hs;
-    for (int i = 0; i < n; ++i) { const double d = std::sqrt(diag[i] / radius); A.at(i, i) += d * d; }
+    for (int i = 0; i < n; ++i) shift[i] = std::sqrt(diag[i] / radius);
     S.num_linear_solves++;
     const auto tl0 = clk::now();
-    const bool ok = detail::cholesky_solve(A, gs.data(), y.data());
+    const bool ok = ops.shifted_solve(shift.data(), gs.data(), y.data());
     S.linear_solver_seconds += std::chrono::duration<double>(clk::now() - tl0).count();
     if (!ok) return 1;
     for (int i = 0; i < n; ++i) step[i] = -y[i];
@@ -314,19 +340,18 @@ void TrustRegionDogleg::solve(double* x_io, const EvalFn& eval_user, SolverSumma
     if (lm) return lm_compute_step();
     if (reuse) { if (opt_.dogleg_type == 0) traditional(); else subspace(); return 0; }
     reuse = true;
-    for (int i = 0; i < n; ++i) diag[i] = std::sqrt(std::min(std::max(Hs.at(i, i), opt_.min_lm_diagonal), opt_.max_lm_diagonal));
+    for (int i = 0; i < n; ++i) diag[i] = std::sqrt(std::min(std::max(hs_diag[i], opt_.min_lm_diagonal), opt_.max_lm_diagonal));
     for (int i = 0; i < n; ++i) grad_d[i] = gs[i] / diag[i];
     for (int i = 0; i < n; ++i) tmp[i] = grad_d[i] / diag[i];
-    symv(Hs, tmp, tmp2);
+    ops.symv(tmp.data(), tmp2.data());
     alpha = dot(grad_d, grad_d) / dot(tmp, tmp2);
     bool ok = false;
     while (mu < max_mu) {
-      A = Hs;
       const double sm = std::sqrt(mu);
-      for (int i = 0; i < n; ++i) { const double lm = diag[i] * sm; A.at(i, i) += lm * lm; }
+      for (int i = 0; i < n; ++i) shift[i] = diag[i] * sm;
       S.num_linear_solves++;
       const auto tl0 = clk::now();
-      const bool chol_ok = detail::cholesky_solve(A, gs.data(), y.data());
+      const bool chol_ok = ops.shifted_solve(shift.data(), gs.data(), y.data());
       S.linear_solver_seconds += std::chrono::duration<double>(clk::now() - tl0).count();
       if (chol_ok) { ok = true; break; }
       mu *= mu_inc;
@@ -342,11 +367,11 @@ void TrustRegionDogleg::solve(double* x_io, const EvalFn& eval_user, SolverSumma
   IterationRecord it{};
   it.iteration = 0;
   S.num_evaluations++; S.num_jacobian_evaluations++;
-  if (!eval(x.data(), true, &x_cost, &H, g.data()) || H.n != n) {
+  if (!eval(x.data(), true, &x_cost, 0, g.data()) || !ops.shape_ok(n)) {
     S.termination = TERM_FAILURE; S.message = "Residual and Jacobian evaluation failed."; return;
   }
   S.initial_cost = x_cost; S.final_cost = x_cost;
-  if (opt_.jacobi_scaling) for (int i = 0; i < n; ++i) scale[i] = 1.0 / (1.0 + std::sqrt(H.at(i, i)));
+  if (opt_.jacobi_scaling) { ops.diag(hdiag.data()); for (int i = 0; i < n; ++i) scale[i] = 1.0 / (1.0 + std::sqrt(hdiag[i])); }
   apply_scaling();
   it.cost = x_cost; gradient_norms(it);
   it.step_is_valid = 1; it.step_is_successful = 1;
@@ -375,7 +400,7 @@ void TrustRegionDogleg::solve(double* x_io, const EvalFn& eval_user, SolverSumma
     const int rc = compute_step();
     bool valid = false;
     if (rc == 0) {
-      symv(Hs, step, tmp);
+      ops.symv(step.data(), tmp.data());
       model_cost_change = -(dot(step, gs) + 0.5 * dot(step, tmp));
       valid = model_cost_change > 0.0;
       if (valid) { for (int i = 0; i < n; ++i) delta[i] = step[i] * scale[i]; num_consecutive_invalid = 0; }
@@ -396,7 +421,7 @@ void TrustRegionDogleg::solve(double* x_io, const EvalFn& eval_user, SolverSumma
     plus(x.data(), delta.data(), cand.data());
     const bool fused = opt_.fuse_candidate_jacobian;
     S.num_evaluations++; if (fused) S.num_jacobian_evaluations++;
-    if (!eval(cand.data(), fused, &cand_cost, fused ? &Hc : nullptr, fused ? gc.data() : nullptr))
+    if (!eval(cand.data(), fused, &cand_cost, 1, fused ? gc.data() : nullptr))
       cand_cost = std::numeric_limits<double>::max();
     // ParameterToleranceReached (:676-693)
     { double s2 = 0; for (int i = 0; i < na; ++i) { const double d = x[i] - cand[i]; s2 += d * d; } it.step_norm = std::sqrt(s2); }
@@ -414,10 +439,10 @@ void TrustRegionDogleg::solve(double* x_io, const EvalFn& eval_user, SolverSumma
       // HandleSuccessfulStep (:757-771)
       x = cand;
       { double s2 = 0; for (int i = 0; i < na; ++i) s2 += x[i] * x[i]; x_norm = std::sqrt(s2); }
-      if (fused) { std::swap(H, Hc); g.swap(gc); x_cost = cand_cost; }
+      if (fused) { ops.swap(); g.swap(gc); x_cost = cand_cost; }
       else {
         S.num_evaluations++; S.num_jacobian_evaluations++;
-        if (!eval(x.data(), true, &x_cost, &H, g.data())) { S.termination = TERM_FAILURE; S.message = "Residual and Jacobian evaluation failed."; return; }
+        if (!eval(x.data(), true, &x_cost, 0, g.data())) { S.termination = TERM_FAILURE; S.message = "Residual and Jacobian evaluation failed."; return; }
       }
       apply_scaling();
       it.cost = x_cost; gradient_norms(it);

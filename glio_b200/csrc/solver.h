@@ -121,6 +121,22 @@ bool real_roots_deg4(const double* poly5, std::vector<double>* roots);
 
 }  // namespace detail
 
+// The band operations of the minimizer, behind one seam so the same trust-region control flow runs with its band matrices in host
+// memory (HostBandOps, below) or on the device (glio_batch_solve with glio_batch_use_device_solver).  Bands: H (slot 0) and the
+// candidate's Hc (slot 1) from the evaluator, the scaled Hs = S H S, and the shifted A = Hs + diag(v*v) that is factored.  Only
+// n-vectors cross the seam.
+struct BandOps {
+  virtual ~BandOps() = default;
+  // evaluate at x; with want_jac fill band `slot` and g (n, overwritten).  false: evaluation failed
+  virtual bool eval(const double* x, bool want_jac, double* cost, int slot, double* g) = 0;
+  virtual bool shape_ok(int n) const = 0;                  // after the first Jacobian evaluation: the band has n rows
+  virtual void diag(double* d) = 0;                        // d = diag(H)
+  virtual void scale(const double* s, double* hs_diag) = 0;  // Hs = S H S, hs_diag = diag(Hs)
+  virtual bool shifted_solve(const double* v, const double* rhs, double* y) = 0;   // A = Hs + diag(v*v); A y = rhs; false: not SPD
+  virtual void symv(const double* x, double* y) = 0;       // y = Hs x
+  virtual void swap() = 0;                                 // H <-> Hc (an accepted fused candidate)
+};
+
 class TrustRegionDogleg {
  public:
   TrustRegionDogleg(const std::vector<ParamBlock>& blocks, const SolverOptions& opt) : blocks_(blocks), opt_(opt) {
@@ -140,6 +156,8 @@ class TrustRegionDogleg {
 
   // x: ambient state, in/out (on return: the lowest-cost accepted point, like Ceres' `parameters`)
   void solve(double* x_inout, const EvalFn& eval, SolverSummary* sum);
+  // the same minimizer over any band implementation
+  void solve(double* x_inout, BandOps& ops, SolverSummary* sum);
 
  private:
   std::vector<ParamBlock> blocks_;

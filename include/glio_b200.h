@@ -86,7 +86,7 @@ int64_t glio_launch_count(const glio_ctx* ctx);
  * front end k_feat_curvature, k_feat_select, k_feat_voxel, k_feat_offsets, k_feat_gather; sweep preparation k_sp_bounds,
  * k_sp_consts, k_sp_classify, k_sp_ranges, k_sp_emit; odometry k_odom_publish; loop-closure registration k_lc_load, k_lc_qhist,
  * k_lc_qscatter, k_lc_init, k_lc_nn, k_lc_compact, k_lc_sum0, k_lc_sum1, k_lc_means, k_lc_solve, k_lc_transform, k_lc_final,
- * k_lc_fitness). */
+ * k_lc_fitness; band Cholesky k_band_chol_solve). */
 int glio_profile_enable(glio_ctx* ctx, int on);
 int glio_profile_get(glio_ctx* ctx, const char* kernel_name, double* ms_total, int64_t* launches);
 /* statistics: number of queries a first kNN search pass handed to a second pass.  The box search has no second pass, so
@@ -970,6 +970,32 @@ int glio_hf_evaluate_band(void* user, int K, const double* poses, const double* 
 int glio_batch_solve(glio_ctx* ctx, int K, double* poses, double* speed_bias, glio_host_factors_band_fn host_factors, void* user,
                      const glio_solver_options* options, glio_solver_summary* summary, glio_iteration* iter_log, int iter_cap,
                      double* step_log, int64_t step_cap);
+
+/* on != 0: every glio_batch_solve on this context runs the minimizer's band algebra on the device.  Each Jacobian evaluation
+ * uploads the host callback's band (a zeroed band with the usual contract; none when host_factors is NULL) and gathers the device
+ * blocks onto it (k_band_assemble, each entry in the host path's order, so the band is the host path's bit for bit); the Jacobi
+ * scaling, the shifted factor-and-solve (K4, below) and the band products run on the device, and only n-vectors cross PCIe.
+ * The back-substitution and the band product sum in another order than the host's, so results differ from the host path by
+ * rounding.  Needs a half bandwidth <= GLIO_BAND_MAX_HB (GLIO_ERR_ARG otherwise).  Default off: glio_batch_solve then runs exactly
+ * the host path.  Kernel names for glio_profile_get: k_band_assemble, k_band_assemble_g, k_band_scale, k_band_shift, k_band_symv. */
+int glio_batch_use_device_solver(glio_ctx* ctx, int on);
+/* The batch normal equations at one state: the band (n x (hb+1), n = K * (speed_bias ? 15 : 6), capacity >= n * (hb+1) doubles),
+ * *hb, g (n) and the cost, assembled by the host path (on_device = 0) or by k_band_assemble (on_device != 0), with the switches and
+ * lists glio_batch_solve would use.  A failing callback or a non-finite cost is GLIO_ERR_NUMERIC. */
+int glio_batch_normal_equations(glio_ctx* ctx, int K, const double* poses, const double* speed_bias, glio_host_factors_band_fn host_factors,
+                                void* user, int on_device, int64_t capacity, double* Hband, int* hb, double* g, double* cost);
+
+/* ---- K4: the band Cholesky factor-and-solve on the device, one system at a time.  band[n*(hb+1)] holds the lower band of a
+ * symmetric A in glio_batch_solve's layout (entry (i,j), i-hb <= j <= i, at band[i*(hb+1) + (j-i+hb)]); on return it holds L,
+ * A = L L^T, in the same layout, and x[n] solves A x = b.  Slots of the layout with j < 0 are left as they are.  The factor and
+ * the forward half follow the scalar host band Cholesky's operation order (right-looking, updates in ascending column order, one
+ * 1.0 / l per column), so L is bit-identical to it; the backward substitution is in axpy form over descending rows, so x differs
+ * from the host's by rounding.  *ok = 1 on success; *ok = 0 when a pivot is not positive and finite or x is not finite (the
+ * host's LINEAR_SOLVER_FAILURE), and then band and x hold partial results.  Bad arguments, and 0 > hb or hb > GLIO_BAND_MAX_HB
+ * (the shared-memory window of one thread block), are GLIO_ERR_ARG.  Host buffers in and out; the call returns when x and *ok
+ * have arrived.  Kernel name for glio_profile_get: k_band_chol_solve. */
+enum { GLIO_BAND_MAX_HB = 160 };
+int glio_band_solve(glio_ctx* ctx, int n, int hb, double* band, const double* b, double* x, int* ok);
 
 /* ---- multi-GPU (batch path only; the window path is "replicas only", SURVEY 8e).
  * Keyframe-sharded ranks sum their pose-block buffers once per evaluation.  The library does not link NCCL: the
