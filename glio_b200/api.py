@@ -1183,6 +1183,22 @@ def _band_solve(self, band, b):
 Context.band_solve = _band_solve
 
 
+def _band_ops(self, H, s, v, x):
+    """glio_band_ops: the device minimizer's scale, shift and product on the band H (n, hb+1) and the n-vectors s, v and x.
+    Returns (Hs, hs_diag, A, y): Hs = S H S, hs_diag its diagonal, A = Hs + diag(v*v) and y = Hs x.  The slots of Hs and A with
+    j < 0 are unspecified."""
+    Hb = np.ascontiguousarray(H, np.float64)
+    n, w = Hb.shape
+    s, v, x = (np.ascontiguousarray(a, np.float64).reshape(n) for a in (s, v, x))
+    Hs = np.zeros((n, w)); A = np.zeros((n, w)); hs_diag = np.zeros(n); y = np.zeros(n)
+    self._chk(self._lib.glio_band_ops(self._h, C.c_int(n), C.c_int(w - 1), _ptr(Hb), _ptr(s), _ptr(v), _ptr(x), _ptr(Hs),
+                                      _ptr(hs_diag), _ptr(A), _ptr(y)))
+    return Hs, hs_diag, A, y
+
+
+Context.band_ops = _band_ops
+
+
 def _batch_use_device_solver(self, on):
     """glio_batch_use_device_solver: batch solves run the minimizer's band algebra on the device (default off)."""
     self._chk(self._lib.glio_batch_use_device_solver(self._h, C.c_int(1 if on else 0)))

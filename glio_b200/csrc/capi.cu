@@ -3070,6 +3070,33 @@ int glio_band_solve(glio_ctx* c, int n, int hb, double* band, const double* b, d
   });
 }
 
+// DeviceBandOps' scale, shift and symv on host buffers, in the device minimizer's own buffers (every solve fills them afresh) and
+// with its staging pattern: s, then v, then x in dm_v1; hs_diag, then y in dm_v2.  One stream orders every reuse.
+int glio_band_ops(glio_ctx* c, int n, int hb, const double* H, const double* s, const double* v, const double* x, double* Hs,
+                  double* hs_diag, double* A, double* y) {
+  if (!c) return GLIO_ERR_ARG;
+  return guarded(c, [&] {
+    GLIO_REQUIRE(n > 0 && H && s && v && x && Hs && hs_diag && A && y, GLIO_ERR_ARG,
+                 "glio_band_ops: need n > 0 and H, s, v, x, Hs, hs_diag, A, y");
+    GLIO_REQUIRE(hb >= 0 && hb <= GLIO_BAND_MAX_HB, GLIO_ERR_ARG, "glio_band_ops: need 0 <= hb <= GLIO_BAND_MAX_HB (160)");
+    const size_t nb = (size_t)n * (hb + 1), bb = nb * sizeof(double), vb = (size_t)n * sizeof(double);
+    c->dm_H[0].reserve(nb); c->dm_Hs.reserve(nb); c->dm_A.reserve(nb); c->dm_v1.reserve(n); c->dm_v2.reserve(n);
+    GLIO_CUDA_TRY(cudaMemcpyAsync(c->dm_H[0].p, H, bb, cudaMemcpyHostToDevice, c->st));
+    GLIO_CUDA_TRY(cudaMemcpyAsync(c->dm_v1.p, s, vb, cudaMemcpyHostToDevice, c->st));
+    band_scale_run(c->dm_H[0].p, c->dm_Hs.p, c->dm_v1.p, n, hb, c->dm_v2.p, c->st, c->lc);
+    GLIO_CUDA_TRY(cudaMemcpyAsync(hs_diag, c->dm_v2.p, vb, cudaMemcpyDeviceToHost, c->st));
+    GLIO_CUDA_TRY(cudaMemcpyAsync(c->dm_v1.p, v, vb, cudaMemcpyHostToDevice, c->st));
+    band_shift_run(c->dm_Hs.p, c->dm_A.p, c->dm_v1.p, n, hb, c->st, c->lc);
+    GLIO_CUDA_TRY(cudaMemcpyAsync(c->dm_v1.p, x, vb, cudaMemcpyHostToDevice, c->st));
+    band_symv_run(c->dm_Hs.p, c->dm_v1.p, c->dm_v2.p, n, hb, c->st, c->lc);
+    GLIO_CUDA_TRY(cudaMemcpyAsync(y, c->dm_v2.p, vb, cudaMemcpyDeviceToHost, c->st));
+    GLIO_CUDA_TRY(cudaMemcpyAsync(Hs, c->dm_Hs.p, bb, cudaMemcpyDeviceToHost, c->st));
+    GLIO_CUDA_TRY(cudaMemcpyAsync(A, c->dm_A.p, bb, cudaMemcpyDeviceToHost, c->st));
+    GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
+    GLIO_CUDA_TRY(cudaGetLastError());
+  });
+}
+
 // ---- K2e: edge correspondences are an input (the reference has no edge association, SURVEY fact 1)
 int glio_set_edges(glio_ctx* c, int slot, const float* cp, const float* pa, const float* pb, const double* s, int64_t n) {
   if (!c) return GLIO_ERR_ARG;

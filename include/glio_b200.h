@@ -996,6 +996,14 @@ int glio_batch_normal_equations(glio_ctx* ctx, int K, const double* poses, const
  * have arrived.  Kernel name for glio_profile_get: k_band_chol_solve. */
 enum { GLIO_BAND_MAX_HB = 160 };
 int glio_band_solve(glio_ctx* ctx, int n, int hb, double* band, const double* b, double* x, int* ok);
+/* The device minimizer's three small band passes on host buffers, in the order a solve uses them: Hs = S H S (entry (i,j) is
+ * (H_ij * s_i) * s_j) and hs_diag = diag(Hs); A = Hs + diag(v * v); y = Hs x, per row the columns max(0, i-hb) .. i from row i and
+ * then i+1 .. min(n-1, i+hb) from the rows below, each term one rounded product and one rounded sum, starting from 0.0.  H, Hs
+ * and A are n x (hb+1) in glio_band_solve's layout; s, v, x, hs_diag and y have n entries.  H's slots with j < 0 are never read,
+ * and those of Hs and A are left unspecified.  Same argument checks as glio_band_solve.  Kernel names for glio_profile_get:
+ * k_band_scale, k_band_shift, k_band_symv. */
+int glio_band_ops(glio_ctx* ctx, int n, int hb, const double* H, const double* s, const double* v, const double* x, double* Hs,
+                  double* hs_diag, double* A, double* y);
 
 /* ---- multi-GPU (batch path only; the window path is "replicas only", SURVEY 8e).
  * Keyframe-sharded ranks sum their pose-block buffers once per evaluation.  The library does not link NCCL: the

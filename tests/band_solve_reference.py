@@ -62,6 +62,47 @@ def band_cholesky_solve(band, b):
     return a, y, x, bool(np.all(np.isfinite(x)))
 
 
+def _offsets(n, hb):
+    """(i, j) index grids of the band layout and the mask of its slots with j >= 0"""
+    i = np.arange(n)[:, None]
+    j = i - hb + np.arange(hb + 1)[None, :]
+    return i, j, j >= 0
+
+
+def band_scale(H, s):
+    """k_band_scale: (Hs, hs_diag), Hs_ij = (H_ij * s_i) * s_j on the slots with j >= 0; the others hold 0.0 here (the device
+    leaves them unspecified)"""
+    n, w = H.shape
+    i, j, ok = _offsets(n, w - 1)
+    Hs = np.zeros((n, w))
+    Hs[ok] = (H[ok] * s[np.broadcast_to(i, ok.shape)[ok]]) * s[j[ok]]
+    return Hs, Hs[:, w - 1].copy()
+
+
+def band_shift(Hs, v):
+    """k_band_shift: A = Hs + diag(v * v)"""
+    A = np.array(Hs, dtype=np.float64, copy=True)
+    A[:, -1] = Hs[:, -1] + v * v
+    return A
+
+
+def band_symv(Hs, x):
+    """k_band_symv: y = Hs x in the kernel's order.  Row i starts from 0.0 and adds, one rounded product and one rounded sum per
+    term, the columns max(0, i-hb) .. i from row i, then i+1 .. min(n-1, i+hb) from the rows below.  The sum never becomes -0.0, so
+    adding +0.0 in place of a term outside the matrix changes no bit; every row therefore runs the same 2hb+1 terms."""
+    n, w = Hs.shape
+    hb = w - 1
+    rows = np.arange(n)
+    y = np.zeros(n)
+    for d in range(-hb, hb + 1):                    # column j = i + d, ascending
+        j = rows + d
+        valid = (j >= 0) & (j < n)
+        jc = np.clip(j, 0, n - 1)
+        h = Hs[rows, hb + d] if d <= 0 else Hs[jc, hb - d]
+        y = y + np.where(valid, np.where(valid, h, 0.0) * x[jc], 0.0)
+    return y
+
+
 def band_to_dense(band):
     """the symmetric dense matrix of a lower band"""
     n, w = band.shape
@@ -71,6 +112,44 @@ def band_to_dense(band):
         for j in range(max(0, i - hb), i + 1):
             A[i, j] = A[j, i] = band[i, j - i + hb]
     return A
+
+
+PREFETCH = 8                                        # kBandPrefetch: K4's ring holds R = hb + 1 + PREFETCH rows
+
+
+def ring_edge_sizes(hb):
+    """the sizes where K4's ring is most fragile: n = hb+1 .. hb+18 (the prologue loads every row up to n = R-1 and the sweep's
+    own loads start just above) and n = 2R-1, 2R, 2R+1 (every slot refilled once)"""
+    R = hb + 1 + PREFETCH
+    return sorted(set(range(hb + 1, hb + 19)) | {2 * R - 1, 2 * R, 2 * R + 1})
+
+
+def block_band(K, nt, span, rng, zero_frac=0.4):
+    """a positive definite band shaped like the batch normal equations: K blocks of nt columns, half bandwidth (span+1) nt - 1,
+    nt x nt blocks coupling keyframes up to span apart, of which about zero_frac are whole zero blocks, and the last nt - 6 columns
+    of every block row empty (speed-bias columns without a factor) but for the diagonal.  Slots with j < 0 hold NaN."""
+    n, hb = K * nt, min((span + 1) * nt - 1, K * nt - 1)
+    band = np.zeros((n, hb + 1))
+    for ka in range(K):
+        for kb in range(max(0, ka - span), ka + 1):
+            if ka != kb and rng.uniform() < zero_frac:
+                continue
+            blk = rng.uniform(-1.0, 1.0, (nt, nt))
+            blk[:, 6:] = 0.0; blk[6:, :] = 0.0
+            for p in range(nt):
+                for q in range(nt):
+                    i, j = nt * ka + p, nt * kb + q
+                    if j <= i:
+                        band[i, j - i + hb] = blk[p, q]
+    i = np.arange(n)[:, None]
+    j = i - hb + np.arange(hb + 1)[None, :]
+    off = (j >= 0) & (j < i)
+    rowsum = np.zeros(n)
+    np.add.at(rowsum, np.broadcast_to(i, band.shape)[off], np.abs(band[off]))
+    np.add.at(rowsum, j[off], np.abs(band[off]))
+    band[:, hb] = rowsum + rng.uniform(1e-3, 1.0, n)
+    band[j < 0] = np.nan
+    return band
 
 
 def random_spd_band(n, hb, rng, scale_exp=0.0):
