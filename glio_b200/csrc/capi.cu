@@ -44,29 +44,62 @@ struct AssocDebug {
   int64_t Q = 0;
 };
 
-// the edges an evaluation reads: n records of cp with s in .w and line points pa / pb
-struct EdgeView {
-  const float4* cps; const float4* pa; const float4* pb;
+// the records an evaluation or a selection reads: n records, a column the list's kind does not use is nullptr
+struct CorrView {
+  const float4* cpw; const float4* nsd; const double* nc; const float4* pa; const float4* pb;
   int64_t n;
 };
 
-// edge correspondences: cp with s in .w, line points pa / pb; src = scan index of each edge when an association produced them
-struct EdgeList {
-  DevBuf<float4> cps, pa, pb;
-  DevBuf<int32_t> src;
-  int64_t n = 0;
-  bool has_src = false;
-  DevBuf<float4> s_cps, s_pa, s_pb;   // selected subset (glio_select_random_edges / glio_batch_select_random_edges), draw order
-  DevBuf<int32_t> s_keep;             // its edge indices
-  int64_t n_sel = -1;                 // -1: no selection -> all edges are active
+// the three kinds of correspondence list and their columns
+enum CorrKind {
+  CORR_WINDOW_PLANES,   // a slot's plane matches: cpw = (cp.xyz, weight), nsd = (n_s.xyz, d_s)
+  CORR_PAIR_PLANES,     // a pair's plane matches: cpw, nc = 6 doubles per record (local-frame unit normal, local-frame centroid)
+  CORR_EDGES            // a slot's or a pair's edges: cpw = (cp.xyz, s), line points pa / pb
+};
+
+// the record columns of one list; only the columns of its kind are ever reserved
+struct CorrCols {
+  DevBuf<float4> cpw, nsd, pa, pb;
+  DevBuf<double> nc;
+  void reserve(CorrKind kind, int64_t q) {
+    cpw.reserve((size_t)q);
+    if (kind == CORR_WINDOW_PLANES) nsd.reserve((size_t)q);
+    if (kind == CORR_PAIR_PLANES) nc.reserve(6 * (size_t)q);
+    if (kind == CORR_EDGES) { pa.reserve((size_t)q); pb.reserve((size_t)q); }
+  }
+  CorrView view(int64_t n) const { return CorrView{cpw.p, nsd.p, nc.p, pa.p, pb.p, n}; }
+};
+
+// One correspondence list: n records (rec), src = the scan index of each record (has_src: for edges, whether an association wrote
+// it), and the selected subset: n_sel records in keep order (a keep list or the sampler's draws), -1 when there is none and every
+// record is active.  Every change of the list marks `plan`, the owner's work-item plan that reads it, stale (nullptr: the owner
+// cuts its plan afresh for every evaluation).
+struct CorrList {
+  const CorrKind kind;
+  bool* const plan;
+  CorrCols rec; DevBuf<int32_t> src; int64_t n = 0; bool has_src = false;
+  CorrCols sel; DevBuf<int32_t> keep; int64_t n_sel = -1;
+  CorrList(CorrKind k, bool* p) : kind(k), plan(p) {}
+  void set_selection(int64_t m) { n_sel = m; if (plan) *plan = true; }
   // replacing the list drops its selection
-  void clear() { n = 0; has_src = false; n_sel = -1; }
-  // what every consumer evaluates: the selected subset if there is one, otherwise all edges
-  EdgeView active() const { return n_sel >= 0 ? EdgeView{s_cps.p, s_pa.p, s_pb.p, n_sel} : EdgeView{cps.p, pa.p, pb.p, n}; }
-  // room for q edges; a reserve may drop the old contents, so the list must count as empty until it is refilled
-  EdgeDst reserve(int64_t q) {
-    cps.reserve((size_t)q); pa.reserve((size_t)q); pb.reserve((size_t)q); src.reserve((size_t)q);
-    return EdgeDst{cps.p, pa.p, pb.p, src.p};
+  void clear() { n = 0; has_src = false; set_selection(-1); }
+  int64_t n_active() const { return n_sel >= 0 ? n_sel : n; }
+  // what every consumer reads: the selected subset if there is one, otherwise the whole list
+  CorrView active() const { return n_sel >= 0 ? sel.view(n_sel) : rec.view(n); }
+  // room for q records and their src, which drops the selection; a reserve may drop the old contents, so the caller clears the
+  // list first or sets n before the records are written
+  void reserve(int64_t q) { set_selection(-1); rec.reserve(kind, q); src.reserve((size_t)q); }
+  // the destination of an association's compacted records
+  CompactDst plane_dst(int64_t q) { reserve(q); return CompactDst{rec.cpw.p, rec.nsd.p, rec.nc.p, src.p}; }
+  EdgeDst edge_dst(int64_t q) { reserve(q); return EdgeDst{rec.cpw.p, rec.pa.p, rec.pb.p, src.p}; }
+  // the k_sel_sample segment that draws k of the records into the selection columns
+  SelSeg sample_seg(int k, uint64_t stream) {
+    sel.reserve(kind, k); keep.reserve((size_t)k);
+    SelSeg g{};
+    g.cpw = rec.cpw.p; g.nsd = rec.nsd.p; g.nc = rec.nc.p; g.pa = rec.pa.p; g.pb = rec.pb.p;
+    g.o_cpw = sel.cpw.p; g.o_nsd = sel.nsd.p; g.o_nc = sel.nc.p; g.o_pa = sel.pa.p; g.o_pb = sel.pb.p;
+    g.keep = keep.p; g.n = n; g.stream = stream; g.k = k;
+    return g;
   }
 };
 
@@ -91,15 +124,11 @@ struct ImuFactorList : PairFactorList {
 
 struct Slot {
   PointSet scan;                 // surf scan
-  DevBuf<float4> m_cpw, m_nsd;   // compacted matches, scan order
-  DevBuf<int32_t> m_src;
-  int64_t n_match = 0;
-  DevBuf<float4> s_cpw, s_nsd;   // selected subset
-  DevBuf<int32_t> s_keep;        // its match indices (glio_select's list or the sampler's draws, glio_get_selection)
-  int64_t n_sel = -1;            // -1: no selection -> all matches are active
-  EdgeList edges;                // glio_set_edges or glio_window_associate_edges
+  CorrList planes;               // glio_window_associate (scan order) or glio_set_matches
+  CorrList edges;                // glio_set_edges or glio_window_associate_edges
   PointSet corners;              // corner scan (glio_window_set_edge_scan)
   AssocDebug dbg, edge_dbg;      // keep_debug: the last plane and the last edge association
+  explicit Slot(bool* plane_plan = nullptr, bool* edge_plan = nullptr) : planes(CORR_WINDOW_PLANES, plane_plan), edges(CORR_EDGES, edge_plan) {}
 };
 
 // a map the window associates against (surf or corner points): its grid, and the local map that can build it
@@ -171,9 +200,9 @@ struct glio_ctx {
   };
   struct Pair {
     int cur = 0, oth = 0;
-    DevBuf<float4> m_cpw; DevBuf<double> m_nc; DevBuf<int32_t> m_src; int64_t n_match = 0;
-    DevBuf<float4> s_cpw; DevBuf<double> s_nc; DevBuf<int32_t> s_keep; int64_t n_sel = -1;
-    EdgeList edges;              // glio_batch_associate_edges_pairs or glio_batch_set_pair_edges: cp in cur's frame, pa / pb in oth's
+    CorrList planes;             // glio_batch_associate_pairs or glio_batch_set_pair_matches
+    CorrList edges;              // glio_batch_associate_edges_pairs or glio_batch_set_pair_edges: cp in cur's frame, pa / pb in oth's
+    Pair(int c, int o, bool* plane_plan, bool* edge_plan) : cur(c), oth(o), planes(CORR_PAIR_PLANES, plane_plan), edges(CORR_EDGES, edge_plan) {}
   };
   std::map<int, std::unique_ptr<Frame>> frames;
   std::vector<std::unique_ptr<Pair>> pairs;
@@ -271,7 +300,7 @@ struct glio_ctx {
   Slot& slot(int k) {
     GLIO_REQUIRE(k >= 0 && k < 4096, GLIO_ERR_ARG, "slot index out of range");
     if ((size_t)k >= slots.size()) slots.resize((size_t)k + 1);
-    if (!slots[k]) slots[k].reset(new Slot());
+    if (!slots[k]) slots[k].reset(new Slot(&items_dirty, &edge_items_dirty));
     return *slots[k];
   }
 };
@@ -365,6 +394,71 @@ void unpack_float4(const float4* h, int64_t n, float* xyz, float* w = nullptr) {
   }
 }
 
+// copy-out of a plane match list (glio_get_matches: nsd; glio_batch_get_matches: nc), every array nullable
+void copy_matches_out(glio_ctx* c, const CorrList& l, int64_t capacity, float* cp, float* weight, float* nsd, double* nc, int32_t* src,
+                      int64_t* n_out) {
+  const int64_t n = l.n;
+  if (n_out) *n_out = n;
+  GLIO_REQUIRE(capacity >= n, GLIO_ERR_ARG, "capacity smaller than the match count");
+  if (n == 0) return;
+  std::vector<float4> h(cp || weight ? n : 0);
+  if (!h.empty()) GLIO_CUDA_TRY(cudaMemcpyAsync(h.data(), l.rec.cpw.p, n * sizeof(float4), cudaMemcpyDeviceToHost, c->st));
+  if (nsd) GLIO_CUDA_TRY(cudaMemcpyAsync(nsd, l.rec.nsd.p, n * sizeof(float4), cudaMemcpyDeviceToHost, c->st));
+  if (nc) GLIO_CUDA_TRY(cudaMemcpyAsync(nc, l.rec.nc.p, 6 * n * sizeof(double), cudaMemcpyDeviceToHost, c->st));
+  if (src) GLIO_CUDA_TRY(cudaMemcpyAsync(src, l.src.p, n * sizeof(int32_t), cudaMemcpyDeviceToHost, c->st));
+  GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
+  unpack_float4(h.data(), (int64_t)h.size(), cp, weight);
+}
+
+// upload of n > 0 plane matches into a cleared list: cp and weight, with nsd (4 floats per match) into a slot's list, where src is
+// 0 (glio_set_matches), or nc (6 doubles per match) into a pair's, where src is the match index (glio_batch_set_pair_matches)
+void upload_matches(glio_ctx* c, CorrList& l, int64_t n, const float* cp, const float* weight, const float* nsd, const double* nc) {
+  const bool window = l.kind == CORR_WINDOW_PLANES;
+  std::vector<float4> h0(n), h1(window ? n : 0);
+  std::vector<int32_t> hs(window ? 0 : n);
+  for (int64_t i = 0; i < n; ++i) {
+    h0[i] = make_float4(cp[3 * i], cp[3 * i + 1], cp[3 * i + 2], weight[i]);
+    if (window) h1[i] = make_float4(nsd[4 * i], nsd[4 * i + 1], nsd[4 * i + 2], nsd[4 * i + 3]);
+    else hs[i] = (int32_t)i;
+  }
+  l.reserve(n);
+  GLIO_CUDA_TRY(cudaMemcpyAsync(l.rec.cpw.p, h0.data(), n * sizeof(float4), cudaMemcpyHostToDevice, c->st));
+  if (window) {
+    GLIO_CUDA_TRY(cudaMemcpyAsync(l.rec.nsd.p, h1.data(), n * sizeof(float4), cudaMemcpyHostToDevice, c->st));
+    GLIO_CUDA_TRY(cudaMemsetAsync(l.src.p, 0, n * sizeof(int32_t), c->st));
+  } else {
+    GLIO_CUDA_TRY(cudaMemcpyAsync(l.rec.nc.p, nc, 6 * n * sizeof(double), cudaMemcpyHostToDevice, c->st));
+    GLIO_CUDA_TRY(cudaMemcpyAsync(l.src.p, hs.data(), n * sizeof(int32_t), cudaMemcpyHostToDevice, c->st));
+  }
+  GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
+  l.n = n;
+}
+
+// glio_select / glio_batch_select: the plane matches keep[0..n) become the list's selection (n < 0: no selection)
+void select_keep(glio_ctx* c, CorrList& l, const int32_t* keep, int64_t n) {
+  if (n < 0) { l.set_selection(-1); return; }
+  GLIO_REQUIRE(n == 0 || keep, GLIO_ERR_ARG, "null selection list");
+  l.set_selection(n);
+  if (n == 0) return;
+  l.keep.reserve(n); c->d_bad.reserve(1); l.sel.reserve(l.kind, n);
+  GLIO_CUDA_TRY(cudaMemcpyAsync(l.keep.p, keep, n * sizeof(int32_t), cudaMemcpyHostToDevice, c->st));
+  GLIO_CUDA_TRY(cudaMemsetAsync(c->d_bad.p, 0, sizeof(int), c->st));
+  gather_selection(l.keep.p, n, l.n, l.rec.cpw.p, l.rec.nsd.p, l.rec.nc.p, l.sel.cpw.p, l.sel.nsd.p, l.sel.nc.p, c->d_bad.p, c->st, c->lc);
+  int bad = 0;
+  GLIO_CUDA_TRY(cudaMemcpyAsync(&bad, c->d_bad.p, sizeof(int), cudaMemcpyDeviceToHost, c->st));
+  GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
+  if (bad) { l.set_selection(-1); throw Error{GLIO_ERR_ARG, "selection index out of range"}; }
+}
+
+// the *_get_selection calls: the selection's record indices (a count query when out is NULL)
+void copy_selection(glio_ctx* c, const CorrList& l, int64_t cap, int32_t* out, int64_t* n) {
+  if (n) *n = l.n_sel;
+  if (l.n_sel <= 0 || !out) return;
+  GLIO_REQUIRE(cap >= l.n_sel, GLIO_ERR_ARG, "capacity smaller than the selection");
+  GLIO_CUDA_TRY(cudaMemcpyAsync(out, l.keep.p, l.n_sel * sizeof(int32_t), cudaMemcpyDeviceToHost, c->st));
+  GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
+}
+
 // queues the copy of the association's per-query views [off, off + q) from the work space into d (fit: nfit doubles per query)
 void capture_debug(glio_ctx* c, AssocDebug& d, const AssocWork& w, const double* fit, int nfit, int64_t off, int64_t q) {
   d.status.reserve(q); d.idx5.reserve(5 * q); d.sqd5.reserve(5 * q); d.pm.reserve(q); d.fit.reserve(nfit * q);
@@ -409,9 +503,7 @@ void associate_slots(glio_ctx* c, const GridBuild& grid, const AssocGates& gates
     Slot& sl = *slots[s];
     GLIO_REQUIRE(sl.scan.n > 0 && sl.scan.ptr, GLIO_ERR_STATE, "slot has no scan");
     segs[s] = make_seg(sl.scan, Qt, lidar_poses[s].data());
-    sl.m_cpw.reserve((size_t)sl.scan.n); sl.m_nsd.reserve((size_t)sl.scan.n); sl.m_src.reserve((size_t)sl.scan.n);
-    dst[s].cpw = sl.m_cpw.p; dst[s].nsd = sl.m_nsd.p; dst[s].nc = nullptr; dst[s].src = sl.m_src.p;
-    sl.n_sel = -1;
+    dst[s] = sl.planes.plane_dst(sl.scan.n);
     Qt += sl.scan.n;
   }
   ensure_work(c, Qt, false, keep_debug);
@@ -429,9 +521,9 @@ void associate_slots(glio_ctx* c, const GridBuild& grid, const AssocGates& gates
     for (int s = 0; s < nseg; ++s) capture_debug(c, slots[s]->dbg, w, w.plane, 4, segs[s].offset, slots[s]->scan.n);
   GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
   for (int s = 0; s < nseg; ++s) {
-    Slot& sl = *slots[s];
-    sl.n_match = c->h_counts.p[s];
-    if (n_match) n_match[s] = sl.n_match;
+    CorrList& l = slots[s]->planes;
+    l.n = c->h_counts.p[s];
+    if (n_match) n_match[s] = l.n;
   }
   tr.mark("done");
 }
@@ -443,7 +535,6 @@ void associate_ctx_slots(glio_ctx* c, const std::vector<int>& ids, const std::ve
   for (int id : ids) sl.push_back(&c->slot(id));
   const AssocGates gates{c->prm.kd_max_radius, c->prm.surf_dist_thres, c->prm.weight_min};
   associate_slots(c, c->map.grid, gates, c->prm.keep_debug != 0, sl, lidar_poses, n_match);
-  c->items_dirty = true;
 }
 
 // The work items of one evaluation kernel, one block each: every owner's (keyframe's or pair's) residuals cut into runs, owners in
@@ -476,23 +567,19 @@ void init_ticket(glio_ctx* c) {
 // K2 work items of the given slots (slot k = keyframe k, nullptr = none)
 ItemPlan<EvalItem> plan_items(const std::vector<const Slot*>& slots, int eval_slots) {
   const int W = (int)slots.size();
-  auto active = [](const Slot* sl) -> int64_t { return !sl ? 0 : sl->n_sel >= 0 ? sl->n_sel : sl->n_match; };
+  auto active = [](const Slot* sl) { return sl ? sl->planes.active() : CorrView{}; };
   // item size: the whole launch should be about one wave of 2 resident blocks per SM (less per-item reduction
   // overhead, no wave-quantisation tail), but never below GLIO_ITEM_MAX residuals per item
   int64_t n_total = 0;
-  for (int k = 0; k < W; ++k) n_total += active(slots[k]);
+  for (int k = 0; k < W; ++k) n_total += active(slots[k]).n;
   int64_t item_size = (n_total + eval_slots - 1) / std::max(eval_slots, 1);
   item_size = std::max<int64_t>(GLIO_ITEM_MAX, ((item_size + 255) / 256) * 256);
   ItemPlan<EvalItem> plan(W);
   for (int k = 0; k < W; ++k) {
-    const Slot* sl = slots[k];
-    const int64_t n = active(sl);
-    const int64_t parts = std::max<int64_t>(1, (n + item_size - 1) / item_size);
-    const int64_t per = ((n + parts - 1) / parts + 255) / 256 * 256;      // equal, 256-aligned parts
-    plan.cut(k, n, per, [&](int64_t f, int32_t count) {
-      const bool sel = sl->n_sel >= 0;
-      return EvalItem{(sel ? sl->s_cpw.p : sl->m_cpw.p) + f, (sel ? sl->s_nsd.p : sl->m_nsd.p) + f, count, k};
-    });
+    const CorrView v = active(slots[k]);
+    const int64_t parts = std::max<int64_t>(1, (v.n + item_size - 1) / item_size);
+    const int64_t per = ((v.n + parts - 1) / parts + 255) / 256 * 256;      // equal, 256-aligned parts
+    plan.cut(k, v.n, per, [&](int64_t f, int32_t count) { return EvalItem{v.cpw + f, v.nsd + f, count, k}; });
   }
   return plan;
 }
@@ -585,8 +672,8 @@ void wait_marg_copied(glio_ctx* c) {
 ItemPlan<EdgeItem> plan_edge_items(const glio_ctx* c, int W) {
   ItemPlan<EdgeItem> plan(W);
   for (int k = 0; k < W; ++k) {
-    const EdgeView e = (size_t)k < c->slots.size() && c->slots[k] ? c->slots[k]->edges.active() : EdgeView{nullptr, nullptr, nullptr, 0};
-    plan.cut(k, e.n, GLIO_ITEM_MAX, [&](int64_t f, int32_t count) { return EdgeItem{e.cps + f, e.pa + f, e.pb + f, count, k}; });
+    const CorrView e = (size_t)k < c->slots.size() && c->slots[k] ? c->slots[k]->edges.active() : CorrView{};
+    plan.cut(k, e.n, GLIO_ITEM_MAX, [&](int64_t f, int32_t count) { return EdgeItem{e.cpw + f, e.pa + f, e.pb + f, count, k}; });
   }
   return plan;
 }
@@ -890,21 +977,11 @@ int glio_get_params(const glio_ctx* c, glio_params* out) {
 int glio_set_matches(glio_ctx* c, int slot, const float* cp, const float* nsd, const float* weight, int64_t n) {
   if (!c) return GLIO_ERR_ARG;
   return guarded(c, [&] {
-    Slot& sl = c->slot(slot);
-    sl.n_match = 0; sl.n_sel = -1; c->items_dirty = true;
+    CorrList& l = c->slot(slot).planes;
+    l.clear();
     if (n <= 0) return;
     GLIO_REQUIRE(cp && nsd && weight, GLIO_ERR_ARG, "null match arrays");
-    std::vector<float4> h0(n), h1(n);
-    for (int64_t i = 0; i < n; ++i) {
-      h0[i] = make_float4(cp[3 * i], cp[3 * i + 1], cp[3 * i + 2], weight[i]);
-      h1[i] = make_float4(nsd[4 * i], nsd[4 * i + 1], nsd[4 * i + 2], nsd[4 * i + 3]);
-    }
-    sl.m_cpw.reserve(n); sl.m_nsd.reserve(n); sl.m_src.reserve(n);
-    GLIO_CUDA_TRY(cudaMemcpyAsync(sl.m_cpw.p, h0.data(), n * sizeof(float4), cudaMemcpyHostToDevice, c->st));
-    GLIO_CUDA_TRY(cudaMemcpyAsync(sl.m_nsd.p, h1.data(), n * sizeof(float4), cudaMemcpyHostToDevice, c->st));
-    GLIO_CUDA_TRY(cudaMemsetAsync(sl.m_src.p, 0, n * sizeof(int32_t), c->st));
-    GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
-    sl.n_match = n;
+    upload_matches(c, l, n, cp, weight, nsd, nullptr);
   });
 }
 
@@ -912,9 +989,9 @@ int glio_get_match_counts(glio_ctx* c, int W, int64_t* n_match, int64_t* n_activ
   if (!c) return GLIO_ERR_ARG;
   return guarded(c, [&] {
     for (int k = 0; k < W; ++k) {
-      Slot& sl = c->slot(k);
-      if (n_match) n_match[k] = sl.n_match;
-      if (n_active) n_active[k] = sl.n_sel >= 0 ? sl.n_sel : sl.n_match;
+      const CorrList& l = c->slot(k).planes;
+      if (n_match) n_match[k] = l.n;
+      if (n_active) n_active[k] = l.n_active();
     }
   });
 }
@@ -1102,11 +1179,11 @@ int glio_window_slide(glio_ctx* c, int W) {
     c->slots[W - 1] = std::move(first);                       // its buffers are reused by the next upload
     if (c->slots[W - 1]) {
       Slot& s = *c->slots[W - 1];
-      s.scan.clear(); s.n_match = 0; s.n_sel = -1;
+      s.scan.clear(); s.planes.clear();
       s.corners.clear(); s.edges.clear();                 // the dropped keyframe's corners and edges leave with it
       s.dbg.Q = 0; s.edge_dbg.Q = 0;                      // and its debug views
     }
-    c->items_dirty = true; c->edge_items_dirty = true;
+    c->items_dirty = true; c->edge_items_dirty = true;    // the plans follow the slots' order, which changed
   });
 }
 
@@ -1216,18 +1293,17 @@ int glio_window_associate_edges(glio_ctx* c, int W, const double* poses_body, co
     GLIO_REQUIRE(Qt < ((int64_t)1 << 31), GLIO_ERR_ARG, "glio_window_associate_edges: too many corner points in one window");
     // the slots' edge lists are replaced from here on: they count as empty until the counts arrive (an error below leaves them
     // empty, never pointing at memory that does not hold them)
-    c->edge_items_dirty = true;
     std::vector<EdgeDst> dst(W);
     std::vector<AssocDebug*> dbg(W);
     for (int k = 0; k < W; ++k) {
       Slot& sl = *c->slots[k];
       sl.edges.clear();
-      dst[k] = sl.edges.reserve(sl.corners.n);
+      dst[k] = sl.edges.edge_dst(sl.corners.n);
       dbg[k] = &sl.edge_dbg;
     }
     edge_assoc_launch(c, c->edge_map.grid, segs, dst, Qt, o, nullptr, 0, c->prm.keep_debug ? &dbg : nullptr);
     for (int k = 0; k < W; ++k) {
-      EdgeList& e = c->slots[k]->edges;
+      CorrList& e = c->slots[k]->edges;
       e.n = c->h_counts.p[k]; e.has_src = true;
       if (n_edge) n_edge[k] = e.n;
     }
@@ -1239,16 +1315,16 @@ int glio_window_associate_edges(glio_ctx* c, int W, const double* poses_body, co
 namespace {
 
 // copy-out of an edge list (glio_get_edges / glio_batch_get_edges): all arrays NULL only counts
-void copy_edges_out(glio_ctx* c, const EdgeList& e, int64_t capacity, float* cp, float* pa, float* pb, double* s, int32_t* src, int64_t* n_out) {
+void copy_edges_out(glio_ctx* c, const CorrList& e, int64_t capacity, float* cp, float* pa, float* pb, double* s, int32_t* src, int64_t* n_out) {
   const int64_t n = e.n;
   if (n_out) *n_out = n;
   if (!cp && !pa && !pb && !s && !src) return;             // a count query
   GLIO_REQUIRE(capacity >= n, GLIO_ERR_ARG, "capacity smaller than the edge count");
   if (n == 0) return;
   std::vector<float4> h0(n), h1(n), h2(n);
-  GLIO_CUDA_TRY(cudaMemcpyAsync(h0.data(), e.cps.p, n * sizeof(float4), cudaMemcpyDeviceToHost, c->st));
-  GLIO_CUDA_TRY(cudaMemcpyAsync(h1.data(), e.pa.p, n * sizeof(float4), cudaMemcpyDeviceToHost, c->st));
-  GLIO_CUDA_TRY(cudaMemcpyAsync(h2.data(), e.pb.p, n * sizeof(float4), cudaMemcpyDeviceToHost, c->st));
+  GLIO_CUDA_TRY(cudaMemcpyAsync(h0.data(), e.rec.cpw.p, n * sizeof(float4), cudaMemcpyDeviceToHost, c->st));
+  GLIO_CUDA_TRY(cudaMemcpyAsync(h1.data(), e.rec.pa.p, n * sizeof(float4), cudaMemcpyDeviceToHost, c->st));
+  GLIO_CUDA_TRY(cudaMemcpyAsync(h2.data(), e.rec.pb.p, n * sizeof(float4), cudaMemcpyDeviceToHost, c->st));
   if (src && e.has_src) GLIO_CUDA_TRY(cudaMemcpyAsync(src, e.src.p, n * sizeof(int32_t), cudaMemcpyDeviceToHost, c->st));
   GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
   unpack_float4(h0.data(), n, cp);
@@ -1261,7 +1337,7 @@ void copy_edges_out(glio_ctx* c, const EdgeList& e, int64_t capacity, float* cp,
 }
 
 // upload of an edge list (glio_set_edges / glio_batch_set_pair_edges): (cp, s) / pa / pb as float4, n > 0
-void upload_edges(glio_ctx* c, EdgeList& e, int64_t n, const float* cp, const float* pa, const float* pb, const double* s) {
+void upload_edges(glio_ctx* c, CorrList& e, int64_t n, const float* cp, const float* pa, const float* pb, const double* s) {
   GLIO_REQUIRE(cp && pa && pb && s, GLIO_ERR_ARG, "null edge arrays");
   std::vector<float4> h0(n), h1(n), h2(n);
   for (int64_t i = 0; i < n; ++i) {
@@ -1269,11 +1345,12 @@ void upload_edges(glio_ctx* c, EdgeList& e, int64_t n, const float* cp, const fl
     h1[i] = make_float4(pa[3 * i], pa[3 * i + 1], pa[3 * i + 2], 0.f);
     h2[i] = make_float4(pb[3 * i], pb[3 * i + 1], pb[3 * i + 2], 0.f);
   }
-  e.cps.reserve(n); e.pa.reserve(n); e.pb.reserve(n);
-  GLIO_CUDA_TRY(cudaMemcpyAsync(e.cps.p, h0.data(), n * sizeof(float4), cudaMemcpyHostToDevice, c->st));
-  GLIO_CUDA_TRY(cudaMemcpyAsync(e.pa.p, h1.data(), n * sizeof(float4), cudaMemcpyHostToDevice, c->st));
-  GLIO_CUDA_TRY(cudaMemcpyAsync(e.pb.p, h2.data(), n * sizeof(float4), cudaMemcpyHostToDevice, c->st));
+  e.rec.reserve(e.kind, n);
+  GLIO_CUDA_TRY(cudaMemcpyAsync(e.rec.cpw.p, h0.data(), n * sizeof(float4), cudaMemcpyHostToDevice, c->st));
+  GLIO_CUDA_TRY(cudaMemcpyAsync(e.rec.pa.p, h1.data(), n * sizeof(float4), cudaMemcpyHostToDevice, c->st));
+  GLIO_CUDA_TRY(cudaMemcpyAsync(e.rec.pb.p, h2.data(), n * sizeof(float4), cudaMemcpyHostToDevice, c->st));
   GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
+  e.n = n;
 }
 
 // glio_get_assoc_debug / glio_get_edge_debug: a slot's views of its last plane (nfit = 4) or edge (nfit = 3) association
@@ -1326,27 +1403,7 @@ int glio_window_associate(glio_ctx* c, int W, const double* poses_body, int64_t*
 
 int glio_get_matches(glio_ctx* c, int slot, int64_t capacity, float* cp, float* nsd, float* weight, int32_t* src, int64_t* n_out) {
   if (!c) return GLIO_ERR_ARG;
-  return guarded(c, [&] {
-    Slot& sl = c->slot(slot);
-    const int64_t n = sl.n_match;
-    if (n_out) *n_out = n;
-    GLIO_REQUIRE(capacity >= n, GLIO_ERR_ARG, "capacity smaller than the match count");
-    if (n == 0) return;
-    std::vector<float4> h(n);
-    if (cp || weight) {
-      GLIO_CUDA_TRY(cudaMemcpyAsync(h.data(), sl.m_cpw.p, n * sizeof(float4), cudaMemcpyDeviceToHost, c->st));
-      GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
-      unpack_float4(h.data(), n, cp, weight);
-    }
-    if (nsd) {
-      GLIO_CUDA_TRY(cudaMemcpyAsync(nsd, sl.m_nsd.p, n * sizeof(float4), cudaMemcpyDeviceToHost, c->st));
-      GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
-    }
-    if (src) {
-      GLIO_CUDA_TRY(cudaMemcpyAsync(src, sl.m_src.p, n * sizeof(int32_t), cudaMemcpyDeviceToHost, c->st));
-      GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
-    }
-  });
+  return guarded(c, [&] { copy_matches_out(c, c->slot(slot).planes, capacity, cp, weight, nsd, nullptr, src, n_out); });
 }
 
 int glio_get_assoc_debug(glio_ctx* c, int slot, int64_t Q, uint8_t* status, int32_t* idx5, float* sqd5, float* pm, double* plane) {
@@ -1355,23 +1412,7 @@ int glio_get_assoc_debug(glio_ctx* c, int slot, int64_t Q, uint8_t* status, int3
 
 int glio_select(glio_ctx* c, int slot, const int32_t* keep, int64_t n) {
   if (!c) return GLIO_ERR_ARG;
-  return guarded(c, [&] {
-    Slot& sl = c->slot(slot);
-    c->items_dirty = true;
-    if (n < 0) { sl.n_sel = -1; return; }
-    GLIO_REQUIRE(n == 0 || keep, GLIO_ERR_ARG, "null selection list");
-    sl.n_sel = n;
-    if (n == 0) return;
-    sl.s_keep.reserve(n); c->d_bad.reserve(1);
-    sl.s_cpw.reserve(n); sl.s_nsd.reserve(n);
-    GLIO_CUDA_TRY(cudaMemcpyAsync(sl.s_keep.p, keep, n * sizeof(int32_t), cudaMemcpyHostToDevice, c->st));
-    GLIO_CUDA_TRY(cudaMemsetAsync(c->d_bad.p, 0, sizeof(int), c->st));
-    gather_selection(sl.s_keep.p, n, sl.n_match, sl.m_cpw.p, sl.m_nsd.p, nullptr, sl.s_cpw.p, sl.s_nsd.p, nullptr, c->d_bad.p, c->st, c->lc);
-    int bad = 0;
-    GLIO_CUDA_TRY(cudaMemcpyAsync(&bad, c->d_bad.p, sizeof(int), cudaMemcpyDeviceToHost, c->st));
-    GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
-    if (bad) { sl.n_sel = -1; throw Error{GLIO_ERR_ARG, "selection index out of range"}; }
-  });
+  return guarded(c, [&] { select_keep(c, c->slot(slot).planes, keep, n); });
 }
 
 int glio_eval_unary(glio_ctx* c, int W, const double* poses_body, int jac_kind, double* H, double* g, double* cost) {
@@ -1837,9 +1878,8 @@ int glio_window_solve_band(glio_ctx* c, int W, double* poses, double* speed_bias
 int glio_eval_unary_residuals(glio_ctx* c, int slot, const double pose_body[7], int jac_kind, int64_t capacity, double* r, double* J, int64_t* n_out) {
   if (!c) return GLIO_ERR_ARG;
   return guarded(c, [&] {
-    Slot& sl = c->slot(slot);
-    const bool sel = sl.n_sel >= 0;
-    const int64_t n = sel ? sl.n_sel : sl.n_match;
+    const CorrView v = c->slot(slot).planes.active();
+    const int64_t n = v.n;
     if (n_out) *n_out = n;
     GLIO_REQUIRE(capacity >= n, GLIO_ERR_ARG, "capacity smaller than the residual count");
     if (n == 0) return;
@@ -1847,8 +1887,7 @@ int glio_eval_unary_residuals(glio_ctx* c, int slot, const double pose_body[7], 
     c->d_r.reserve(n); c->d_J.reserve(6 * n); c->d_poses.reserve(7); c->h_poses.reserve(7);
     memcpy(c->h_poses.p, pose_body, 7 * sizeof(double));
     GLIO_CUDA_TRY(cudaMemcpyAsync(c->d_poses.p, c->h_poses.p, 7 * sizeof(double), cudaMemcpyHostToDevice, c->st));
-    eval_unary_residuals_run(sel ? sl.s_cpw.p : sl.m_cpw.p, sel ? sl.s_nsd.p : sl.m_nsd.p, n, c->d_poses.p, eval_params(c), jac_kind,
-                             c->d_r.p, c->d_J.p, c->st, c->lc);
+    eval_unary_residuals_run(v.cpw, v.nsd, n, c->d_poses.p, eval_params(c), jac_kind, c->d_r.p, c->d_J.p, c->st, c->lc);
     if (r) GLIO_CUDA_TRY(cudaMemcpyAsync(r, c->d_r.p, n * sizeof(double), cudaMemcpyDeviceToHost, c->st));
     if (J) GLIO_CUDA_TRY(cudaMemcpyAsync(J, c->d_J.p, 6 * n * sizeof(double), cudaMemcpyDeviceToHost, c->st));
     GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
@@ -1920,8 +1959,7 @@ glio_ctx::Pair& pair_entry(glio_ctx* c, int cur, int oth) {
   auto it = c->pair_index.find(key);
   if (it != c->pair_index.end()) return *c->pairs[it->second];
   c->pair_index[key] = (int)c->pairs.size();
-  c->pairs.emplace_back(new glio_ctx::Pair());
-  c->pairs.back()->cur = cur; c->pairs.back()->oth = oth;
+  c->pairs.emplace_back(new glio_ctx::Pair(cur, oth, &c->bin_dirty, &c->bedge_dirty));
   c->bin_dirty = true;
   return *c->pairs.back();
 }
@@ -1982,18 +2020,15 @@ int glio_batch_associate_pairs(glio_ctx* c, const int32_t* pairs_cur, const int3
       std::vector<CompactDst> dst(nseg);
       for (int s = 0; s < nseg; ++s) {
         const int64_t i = grp.second[s];
-        glio_ctx::Pair& pr = pair_entry(c, pairs_cur[i], pairs_oth[i]);
-        pr.n_match = c->h_counts.p[s]; pr.n_sel = -1;
-        const size_t nm = (size_t)std::max<int64_t>(pr.n_match, 1);
-        pr.m_cpw.reserve(nm); pr.m_nc.reserve(6 * nm); pr.m_src.reserve(nm);
-        dst[s].cpw = pr.m_cpw.p; dst[s].nsd = nullptr; dst[s].nc = pr.m_nc.p; dst[s].src = pr.m_src.p;
-        if (n_match) n_match[i] = pr.n_match;
+        CorrList& l = pair_entry(c, pairs_cur[i], pairs_oth[i]).planes;
+        l.n = c->h_counts.p[s];
+        dst[s] = l.plane_dst(std::max<int64_t>(l.n, 1));
+        if (n_match) n_match[i] = l.n;
       }
       GLIO_CUDA_TRY(cudaMemcpyAsync(c->d_dst.p, dst.data(), nseg * sizeof(CompactDst), cudaMemcpyHostToDevice, c->st));
       compact_scatter(w, c->d_segs.p, nseg, c->w_pos.p, c->d_dst.p, c->st, c->lc);
       GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));   // dst/segs are stack vectors
     }
-    c->bin_dirty = true;
   });
 }
 
@@ -2010,39 +2045,12 @@ int glio_batch_pair_list(glio_ctx* c, int64_t capacity, int32_t* cur, int32_t* o
 
 int glio_batch_get_matches(glio_ctx* c, int cur, int oth, int64_t capacity, float* cp, float* weight, double* normal_cent, int32_t* src, int64_t* n_out) {
   if (!c) return GLIO_ERR_ARG;
-  return guarded(c, [&] {
-    glio_ctx::Pair& pr = find_pair(c, cur, oth);
-    const int64_t n = pr.n_match;
-    if (n_out) *n_out = n;
-    GLIO_REQUIRE(capacity >= n, GLIO_ERR_ARG, "capacity smaller than the match count");
-    if (n == 0) return;
-    std::vector<float4> h;
-    if (cp || weight) { h.resize(n); GLIO_CUDA_TRY(cudaMemcpyAsync(h.data(), pr.m_cpw.p, n * sizeof(float4), cudaMemcpyDeviceToHost, c->st)); }
-    if (normal_cent) GLIO_CUDA_TRY(cudaMemcpyAsync(normal_cent, pr.m_nc.p, 6 * n * sizeof(double), cudaMemcpyDeviceToHost, c->st));
-    if (src) GLIO_CUDA_TRY(cudaMemcpyAsync(src, pr.m_src.p, n * sizeof(int32_t), cudaMemcpyDeviceToHost, c->st));
-    GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
-    if (!h.empty()) unpack_float4(h.data(), n, cp, weight);
-  });
+  return guarded(c, [&] { copy_matches_out(c, find_pair(c, cur, oth).planes, capacity, cp, weight, nullptr, normal_cent, src, n_out); });
 }
 
 int glio_batch_select(glio_ctx* c, int cur, int oth, const int32_t* keep, int64_t n) {
   if (!c) return GLIO_ERR_ARG;
-  return guarded(c, [&] {
-    glio_ctx::Pair& pr = find_pair(c, cur, oth);
-    c->bin_dirty = true;
-    if (n < 0) { pr.n_sel = -1; return; }
-    GLIO_REQUIRE(n == 0 || keep, GLIO_ERR_ARG, "null selection list");
-    pr.n_sel = n;
-    if (n == 0) return;
-    pr.s_keep.reserve(n); c->d_bad.reserve(1); pr.s_cpw.reserve(n); pr.s_nc.reserve(6 * n);
-    GLIO_CUDA_TRY(cudaMemcpyAsync(pr.s_keep.p, keep, n * sizeof(int32_t), cudaMemcpyHostToDevice, c->st));
-    GLIO_CUDA_TRY(cudaMemsetAsync(c->d_bad.p, 0, sizeof(int), c->st));
-    gather_selection(pr.s_keep.p, n, pr.n_match, pr.m_cpw.p, nullptr, pr.m_nc.p, pr.s_cpw.p, nullptr, pr.s_nc.p, c->d_bad.p, c->st, c->lc);
-    int bad = 0;
-    GLIO_CUDA_TRY(cudaMemcpyAsync(&bad, c->d_bad.p, sizeof(int), cudaMemcpyDeviceToHost, c->st));
-    GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
-    if (bad) { pr.n_sel = -1; throw Error{GLIO_ERR_ARG, "selection index out of range"}; }
-  });
+  return guarded(c, [&] { select_keep(c, find_pair(c, cur, oth).planes, keep, n); });
 }
 
 // ---- K1be / K2be: scan-to-multiscan edge association and binary point-to-edge factors
@@ -2073,7 +2081,6 @@ int glio_batch_associate_edges_pairs(glio_ctx* c, const int32_t* pairs_cur, cons
     for (int64_t i = 0; i < n_pairs; ++i)
       GLIO_REQUIRE(c->frames[pairs_cur[i]]->has_edge && c->frames[pairs_oth[i]]->has_edge, GLIO_ERR_STATE,
                    "pair frame has no corner scan (glio_batch_set_edge_frame)");
-    c->bedge_dirty = true;
     for (auto& grp : by_oth) {
       glio_ctx::Frame& fo = *c->frames[grp.first];
       // the group's pairs; their edge lists count as empty until the counts arrive
@@ -2093,7 +2100,7 @@ int glio_batch_associate_edges_pairs(glio_ctx* c, const int32_t* pairs_cur, cons
         const glio_ctx::Frame& fc = *c->frames[pairs_cur[grp.second[s]]];
         if (fc.corners.pts.n == 0) continue;
         segs.push_back(make_seg(fc.corners.pts, Qt, fc.pose));     // body pose applied directly to the stored points (quirk Q7)
-        dst.push_back(prs[s]->edges.reserve(fc.corners.pts.n));
+        dst.push_back(prs[s]->edges.edge_dst(fc.corners.pts.n));
         seg_item.push_back((int64_t)s);
         Qt += fc.corners.pts.n;
       }
@@ -2102,7 +2109,7 @@ int glio_batch_associate_edges_pairs(glio_ctx* c, const int32_t* pairs_cur, cons
       const GridBuild& grid = searched_grid(c, fo, fo.corners);
       edge_assoc_launch(c, grid, segs, dst, Qt, o, fo.corners.pts.ptr, fo.corners.pts.stride, nullptr);
       for (size_t s = 0; s < segs.size(); ++s) {
-        EdgeList& e = prs[seg_item[s]]->edges;
+        CorrList& e = prs[seg_item[s]]->edges;
         e.n = c->h_counts.p[s]; e.has_src = true;
         if (n_edge) n_edge[grp.second[seg_item[s]]] = e.n;
       }
@@ -2122,10 +2129,9 @@ int glio_batch_set_pair_edges(glio_ctx* c, int cur, int oth, const float* cp, co
   return guarded(c, [&] {
     GLIO_REQUIRE(cur >= 0 && oth >= 0 && cur != oth, GLIO_ERR_ARG, "bad pair");
     GLIO_REQUIRE(n >= 0 && (n == 0 || (cp && pa && pb && s)), GLIO_ERR_ARG, "null edge arrays");
-    EdgeList& e = pair_entry(c, cur, oth).edges;
-    e.clear(); c->bedge_dirty = true;
+    CorrList& e = pair_entry(c, cur, oth).edges;
+    e.clear();
     if (n > 0) upload_edges(c, e, n, cp, pa, pb, s);
-    e.n = n;
   });
 }
 
@@ -2205,16 +2211,56 @@ std::vector<int64_t> batch_select_counts(const int32_t* cur, const std::vector<i
   return n_sel;
 }
 
-// a k_sel_sample segment that draws k of the edges of e into its selection buffers
-SelSeg edge_select_seg(EdgeList& e, int k, uint64_t stream) {
-  e.s_cps.reserve(k); e.s_pa.reserve(k); e.s_pb.reserve(k); e.s_keep.reserve(k);
-  SelSeg g{};
-  g.cpw = e.cps.p; g.pa = e.pa.p; g.pb = e.pb.p; g.o_cpw = e.s_cps.p; g.o_pa = e.s_pa.p; g.o_pb = e.s_pb.p;
-  g.keep = e.s_keep.p; g.n = e.n; g.stream = stream; g.k = k;
-  return g;
+uint64_t pair_stream(int32_t cur, int32_t oth) { return ((uint64_t)(uint32_t)cur << 32) | (uint32_t)oth; }
+
+// The seeded selection of lists[i] with the outcomes n_sel[i] (-1 keeps every record, 0 none, k > 0 draws k records with
+// stream[i]): one k_sel_sample launch in the given Philox domain; n_active[i] (nullable) receives each list's active count
+void sample_lists(glio_ctx* c, const std::vector<CorrList*>& lists, const std::vector<int64_t>& n_sel, const std::vector<uint64_t>& stream,
+                  int k, uint64_t domain, const glio_select_options* opt, int64_t* n_active) {
+  std::vector<SelSeg> segs;
+  for (size_t i = 0; i < lists.size(); ++i)
+    if (n_sel[i] > 0) segs.push_back(lists[i]->sample_seg(k, stream[i]));
+  select_launch(c, segs, k, domain, opt->seed, opt->nonce);
+  for (size_t i = 0; i < lists.size(); ++i) {
+    lists[i]->set_selection(n_sel[i]);
+    if (n_active) n_active[i] = lists[i]->n_active();
+  }
 }
 
-uint64_t pair_stream(int32_t cur, int32_t oth) { return ((uint64_t)(uint32_t)cur << 32) | (uint32_t)oth; }
+// featureSelection (Estimator.cpp:3894-3992) on one list of slots 0..W-1 (glio_select_random: the plane matches,
+// glio_select_random_edges: the edges).  The outcome of every slot follows from its record count alone, so the host decides it
+// here and only the sampled slots go to the device.
+void select_random_slots(glio_ctx* c, CorrList Slot::*list, const char* fn, uint64_t domain, int W, const int64_t* stream_ids,
+                         const glio_select_options* opt, int64_t* n_active) {
+  GLIO_REQUIRE(W > 0 && W <= 4096 && stream_ids, GLIO_ERR_ARG, std::string(fn) + ": bad window arguments");
+  check_select_options(opt);
+  std::vector<CorrList*> lists(W);
+  std::vector<int64_t> n_sel(W);
+  std::vector<uint64_t> stream(W);
+  for (int k = 0; k < W; ++k) {
+    lists[k] = &(c->slot(k).*list);
+    n_sel[k] = window_select_count(lists[k]->n, opt);
+    stream[k] = (uint64_t)stream_ids[k];
+  }
+  sample_lists(c, lists, n_sel, stream, opt->feature_res_num, domain, opt, n_active);
+}
+
+// globalFeatureSelection_Batch (mode 0) / globalFeatureSelectionAdd_Batch (mode 1) on one list of the listed pairs
+// (glio_batch_select_random: the plane matches, glio_batch_select_random_edges: the edges)
+void select_random_pairs(glio_ctx* c, CorrList glio_ctx::Pair::*list, const char* fn, uint64_t domain, const int32_t* cur, const int32_t* oth,
+                         int64_t n_pairs, int mode, const glio_select_options* opt, int64_t* n_active) {
+  const std::vector<glio_ctx::Pair*> prs = batch_select_pairs(c, fn, cur, oth, n_pairs, mode, opt);
+  std::vector<CorrList*> lists((size_t)n_pairs);
+  std::vector<int64_t> n((size_t)n_pairs);
+  std::vector<uint64_t> stream((size_t)n_pairs);
+  for (int64_t i = 0; i < n_pairs; ++i) {
+    lists[i] = &(prs[i]->*list);
+    n[i] = lists[i]->n;
+    stream[i] = pair_stream(cur[i], oth[i]);
+  }
+  const int Bn = opt->batch_feature_res_num;
+  sample_lists(c, lists, batch_select_counts(cur, n, mode, Bn), stream, Bn, domain, opt, n_active);
+}
 
 }  // namespace
 
@@ -2227,160 +2273,54 @@ void glio_select_default_options(glio_select_options* o) {
   o->random_select = 1; o->seed = 0; o->nonce = 0;
 }
 
-// featureSelection (Estimator.cpp:3894-3992) for slots 0..W-1.  The outcome of every slot follows from its match count alone, so
-// the host decides it here and only the sampled slots go to the device.
 int glio_select_random(glio_ctx* c, int W, const int64_t* stream_ids, const glio_select_options* opt, int64_t* n_active) {
   if (!c) return GLIO_ERR_ARG;
-  return guarded(c, [&] {
-    GLIO_REQUIRE(W > 0 && W <= 4096 && stream_ids, GLIO_ERR_ARG, "glio_select_random: bad window arguments");
-    check_select_options(opt);
-    const int F = opt->feature_res_num;
-    std::vector<int64_t> n_sel(W);
-    for (int k = 0; k < W; ++k) n_sel[k] = window_select_count((size_t)k < c->slots.size() && c->slots[k] ? c->slots[k]->n_match : 0, opt);
-    std::vector<SelSeg> segs;
-    for (int k = 0; k < W; ++k) {
-      Slot& sl = c->slot(k);
-      if (n_sel[k] > 0) {
-        sl.s_cpw.reserve(F); sl.s_nsd.reserve(F); sl.s_keep.reserve(F);
-        SelSeg g{};
-        g.cpw = sl.m_cpw.p; g.nsd = sl.m_nsd.p; g.nc = nullptr; g.o_cpw = sl.s_cpw.p; g.o_nsd = sl.s_nsd.p; g.o_nc = nullptr;
-        g.keep = sl.s_keep.p; g.n = sl.n_match; g.stream = (uint64_t)stream_ids[k]; g.k = F;
-        segs.push_back(g);
-      }
-    }
-    select_launch(c, segs, F, SEL_DOMAIN_WINDOW, opt->seed, opt->nonce);
-    for (int k = 0; k < W; ++k) {
-      Slot& sl = c->slot(k);
-      sl.n_sel = n_sel[k];
-      if (n_active) n_active[k] = n_sel[k] >= 0 ? n_sel[k] : sl.n_match;
-    }
-    c->items_dirty = true;
-  });
+  return guarded(c, [&] { select_random_slots(c, &Slot::planes, "glio_select_random", SEL_DOMAIN_WINDOW, W, stream_ids, opt, n_active); });
 }
 
-// featureSelection's rule and sampler on the edge lists of slots 0..W-1 (domain 3)
 int glio_select_random_edges(glio_ctx* c, int W, const int64_t* stream_ids, const glio_select_options* opt, int64_t* n_active) {
   if (!c) return GLIO_ERR_ARG;
   return guarded(c, [&] {
-    GLIO_REQUIRE(W > 0 && W <= 4096 && stream_ids, GLIO_ERR_ARG, "glio_select_random_edges: bad window arguments");
-    check_select_options(opt);
-    const int F = opt->feature_res_num;
-    std::vector<int64_t> n_sel(W);
-    std::vector<SelSeg> segs;
-    for (int k = 0; k < W; ++k) {
-      EdgeList& e = c->slot(k).edges;
-      n_sel[k] = window_select_count(e.n, opt);
-      if (n_sel[k] > 0) segs.push_back(edge_select_seg(e, F, (uint64_t)stream_ids[k]));
-    }
-    select_launch(c, segs, F, SEL_DOMAIN_WINDOW_EDGES, opt->seed, opt->nonce);
-    for (int k = 0; k < W; ++k) {
-      EdgeList& e = c->slot(k).edges;
-      e.n_sel = n_sel[k];
-      if (n_active) n_active[k] = n_sel[k] >= 0 ? n_sel[k] : e.n;
-    }
-    c->edge_items_dirty = true;
+    select_random_slots(c, &Slot::edges, "glio_select_random_edges", SEL_DOMAIN_WINDOW_EDGES, W, stream_ids, opt, n_active);
   });
 }
 
-// globalFeatureSelection_Batch (mode 0) / globalFeatureSelectionAdd_Batch (mode 1) for the listed pairs' plane matches
 int glio_batch_select_random(glio_ctx* c, const int32_t* cur, const int32_t* oth, int64_t n_pairs, int mode, const glio_select_options* opt,
                              int64_t* n_active) {
   if (!c) return GLIO_ERR_ARG;
   return guarded(c, [&] {
-    const std::vector<glio_ctx::Pair*> prs = batch_select_pairs(c, "glio_batch_select_random", cur, oth, n_pairs, mode, opt);
-    const int Bn = opt->batch_feature_res_num;
-    std::vector<int64_t> n((size_t)n_pairs);
-    for (int64_t i = 0; i < n_pairs; ++i) n[i] = prs[i]->n_match;
-    const std::vector<int64_t> n_sel = batch_select_counts(cur, n, mode, Bn);
-    std::vector<SelSeg> segs;
-    for (int64_t i = 0; i < n_pairs; ++i) {
-      if (n_sel[i] <= 0) continue;
-      glio_ctx::Pair& pr = *prs[i];
-      pr.s_cpw.reserve(Bn); pr.s_nc.reserve(6 * (size_t)Bn); pr.s_keep.reserve(Bn);
-      SelSeg g{};
-      g.cpw = pr.m_cpw.p; g.nsd = nullptr; g.nc = pr.m_nc.p; g.o_cpw = pr.s_cpw.p; g.o_nsd = nullptr; g.o_nc = pr.s_nc.p;
-      g.keep = pr.s_keep.p; g.n = pr.n_match; g.stream = pair_stream(cur[i], oth[i]); g.k = Bn;
-      segs.push_back(g);
-    }
-    select_launch(c, segs, Bn, mode == 0 ? SEL_DOMAIN_STARTEND : SEL_DOMAIN_ADD, opt->seed, opt->nonce);
-    for (int64_t i = 0; i < n_pairs; ++i) {
-      glio_ctx::Pair& pr = *prs[i];
-      pr.n_sel = n_sel[i];
-      if (n_active) n_active[i] = n_sel[i] >= 0 ? n_sel[i] : pr.n_match;
-    }
-    c->bin_dirty = true;
+    select_random_pairs(c, &glio_ctx::Pair::planes, "glio_batch_select_random", mode == 0 ? SEL_DOMAIN_STARTEND : SEL_DOMAIN_ADD, cur, oth,
+                        n_pairs, mode, opt, n_active);
   });
 }
 
-// the same rules and sampler for the listed pairs' edge lists (domains 4 and 5)
 int glio_batch_select_random_edges(glio_ctx* c, const int32_t* cur, const int32_t* oth, int64_t n_pairs, int mode, const glio_select_options* opt,
                                    int64_t* n_active) {
   if (!c) return GLIO_ERR_ARG;
   return guarded(c, [&] {
-    const std::vector<glio_ctx::Pair*> prs = batch_select_pairs(c, "glio_batch_select_random_edges", cur, oth, n_pairs, mode, opt);
-    const int Bn = opt->batch_feature_res_num;
-    std::vector<int64_t> n((size_t)n_pairs);
-    for (int64_t i = 0; i < n_pairs; ++i) n[i] = prs[i]->edges.n;
-    const std::vector<int64_t> n_sel = batch_select_counts(cur, n, mode, Bn);
-    std::vector<SelSeg> segs;
-    for (int64_t i = 0; i < n_pairs; ++i)
-      if (n_sel[i] > 0) segs.push_back(edge_select_seg(prs[i]->edges, Bn, pair_stream(cur[i], oth[i])));
-    select_launch(c, segs, Bn, mode == 0 ? SEL_DOMAIN_STARTEND_EDGES : SEL_DOMAIN_ADD_EDGES, opt->seed, opt->nonce);
-    for (int64_t i = 0; i < n_pairs; ++i) {
-      EdgeList& e = prs[i]->edges;
-      e.n_sel = n_sel[i];
-      if (n_active) n_active[i] = n_sel[i] >= 0 ? n_sel[i] : e.n;
-    }
-    c->bedge_dirty = true;
+    select_random_pairs(c, &glio_ctx::Pair::edges, "glio_batch_select_random_edges",
+                        mode == 0 ? SEL_DOMAIN_STARTEND_EDGES : SEL_DOMAIN_ADD_EDGES, cur, oth, n_pairs, mode, opt, n_active);
   });
 }
-
-}  // extern "C"
-
-namespace {
-
-void copy_selection(glio_ctx* c, int64_t n_sel, const DevBuf<int32_t>& keep, int64_t cap, int32_t* out, int64_t* n) {
-  if (n) *n = n_sel;
-  if (n_sel <= 0 || !out) return;
-  GLIO_REQUIRE(cap >= n_sel, GLIO_ERR_ARG, "capacity smaller than the selection");
-  GLIO_CUDA_TRY(cudaMemcpyAsync(out, keep.p, n_sel * sizeof(int32_t), cudaMemcpyDeviceToHost, c->st));
-  GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
-}
-
-}  // namespace
-
-extern "C" {
 
 int glio_get_selection(glio_ctx* c, int slot, int64_t capacity, int32_t* keep, int64_t* n) {
   if (!c) return GLIO_ERR_ARG;
-  return guarded(c, [&] {
-    Slot& sl = c->slot(slot);
-    copy_selection(c, sl.n_sel, sl.s_keep, capacity, keep, n);
-  });
+  return guarded(c, [&] { copy_selection(c, c->slot(slot).planes, capacity, keep, n); });
 }
 
 int glio_batch_get_selection(glio_ctx* c, int cur, int oth, int64_t capacity, int32_t* keep, int64_t* n) {
   if (!c) return GLIO_ERR_ARG;
-  return guarded(c, [&] {
-    glio_ctx::Pair& pr = find_pair(c, cur, oth);
-    copy_selection(c, pr.n_sel, pr.s_keep, capacity, keep, n);
-  });
+  return guarded(c, [&] { copy_selection(c, find_pair(c, cur, oth).planes, capacity, keep, n); });
 }
 
 int glio_get_edge_selection(glio_ctx* c, int slot, int64_t capacity, int32_t* keep, int64_t* n) {
   if (!c) return GLIO_ERR_ARG;
-  return guarded(c, [&] {
-    const EdgeList& e = c->slot(slot).edges;
-    copy_selection(c, e.n_sel, e.s_keep, capacity, keep, n);
-  });
+  return guarded(c, [&] { copy_selection(c, c->slot(slot).edges, capacity, keep, n); });
 }
 
 int glio_batch_get_edge_selection(glio_ctx* c, int cur, int oth, int64_t capacity, int32_t* keep, int64_t* n) {
   if (!c) return GLIO_ERR_ARG;
-  return guarded(c, [&] {
-    const EdgeList& e = find_pair(c, cur, oth).edges;
-    copy_selection(c, e.n_sel, e.s_keep, capacity, keep, n);
-  });
+  return guarded(c, [&] { copy_selection(c, find_pair(c, cur, oth).edges, capacity, keep, n); });
 }
 
 }  // extern "C"
@@ -2396,10 +2336,8 @@ void build_bin_items(glio_ctx* c, int K) {
   for (int p = 0; p < P; ++p) {
     const glio_ctx::Pair& pr = *c->pairs[p];
     GLIO_REQUIRE(pr.cur >= 0 && pr.oth >= 0 && pr.cur < K && pr.oth < K, GLIO_ERR_ARG, "pair references a keyframe outside [0, K)");
-    const bool sel = pr.n_sel >= 0;
-    const float4* cpw = sel ? pr.s_cpw.p : pr.m_cpw.p;
-    const double* nc = sel ? pr.s_nc.p : pr.m_nc.p;
-    plan.cut(p, sel ? pr.n_sel : pr.n_match, GLIO_ITEM_MAX, [&](int64_t f, int32_t count) { return BinItem{cpw + f, nc + 6 * f, count, pr.cur, pr.oth}; });
+    const CorrView v = pr.planes.active();
+    plan.cut(p, v.n, GLIO_ITEM_MAX, [&](int64_t f, int32_t count) { return BinItem{v.cpw + f, v.nc + 6 * f, count, pr.cur, pr.oth}; });
     inc[pr.cur].push_back(BinIncidence{p, 0});
     inc[pr.oth].push_back(BinIncidence{p, 1});
   }
@@ -2426,8 +2364,8 @@ void build_bedge_items(glio_ctx* c, int K) {
   ItemPlan<BinEdgeItem> plan(P);
   for (int p = 0; p < P; ++p) {
     const glio_ctx::Pair& pr = *c->pairs[p];
-    const EdgeView e = pr.edges.active();
-    plan.cut(p, e.n, GLIO_ITEM_MAX, [&](int64_t f, int32_t count) { return BinEdgeItem{e.cps + f, e.pa + f, e.pb + f, count, pr.cur, pr.oth}; });
+    const CorrView e = pr.edges.active();
+    plan.cut(p, e.n, GLIO_ITEM_MAX, [&](int64_t f, int32_t count) { return BinEdgeItem{e.cpw + f, e.pa + f, e.pb + f, count, pr.cur, pr.oth}; });
   }
   c->n_bedge_items = (int)plan.items.size();
   c->d_bedge_sums.reserve((size_t)(P + 1) * GLIO_NACC_BIN);
@@ -2803,19 +2741,9 @@ int glio_batch_set_pair_matches(glio_ctx* c, int cur, int oth, const float* cp, 
   return guarded(c, [&] {
     GLIO_REQUIRE(cur >= 0 && oth >= 0 && cur != oth, GLIO_ERR_ARG, "bad pair");
     GLIO_REQUIRE(n >= 0 && (n == 0 || (cp && normal_cent && weight)), GLIO_ERR_ARG, "null match arrays");
-    glio_ctx::Pair& pr = pair_entry(c, cur, oth);
-    pr.n_match = n; pr.n_sel = -1;
-    if (n > 0) {
-      std::vector<float> cpw((size_t)n * 4);
-      std::vector<int32_t> src((size_t)n);
-      for (int64_t i = 0; i < n; ++i) { cpw[4 * i] = cp[3 * i]; cpw[4 * i + 1] = cp[3 * i + 1]; cpw[4 * i + 2] = cp[3 * i + 2]; cpw[4 * i + 3] = weight[i]; src[i] = (int32_t)i; }
-      pr.m_cpw.reserve((size_t)n); pr.m_nc.reserve((size_t)n * 6); pr.m_src.reserve((size_t)n);
-      GLIO_CUDA_TRY(cudaMemcpyAsync(pr.m_cpw.p, cpw.data(), (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, c->st));
-      GLIO_CUDA_TRY(cudaMemcpyAsync(pr.m_nc.p, normal_cent, (size_t)n * 6 * sizeof(double), cudaMemcpyHostToDevice, c->st));
-      GLIO_CUDA_TRY(cudaMemcpyAsync(pr.m_src.p, src.data(), (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice, c->st));
-      GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
-    }
-    c->bin_dirty = true;
+    CorrList& l = pair_entry(c, cur, oth).planes;
+    l.clear();
+    if (n > 0) upload_matches(c, l, n, cp, weight, nullptr, normal_cent);
   });
 }
 
@@ -3101,11 +3029,9 @@ int glio_band_ops(glio_ctx* c, int n, int hb, const double* H, const double* s, 
 int glio_set_edges(glio_ctx* c, int slot, const float* cp, const float* pa, const float* pb, const double* s, int64_t n) {
   if (!c) return GLIO_ERR_ARG;
   return guarded(c, [&] {
-    EdgeList& e = c->slot(slot).edges;
-    e.clear(); c->edge_items_dirty = true;
-    if (n <= 0) return;
-    upload_edges(c, e, n, cp, pa, pb, s);
-    e.n = n;
+    CorrList& e = c->slot(slot).edges;
+    e.clear();
+    if (n > 0) upload_edges(c, e, n, cp, pa, pb, s);
   });
 }
 
