@@ -9,12 +9,14 @@ torch is used only for device buffers/streams by callers (bench.py); this module
 """
 import ctypes as C
 import os
+import threading
 
 import numpy as np
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB_PATH = os.path.join(_HERE, "libglio_b200.so")
 _LIB = None
+_LIB_LOCK = threading.Lock()
 
 HOST, DEVICE = 0, 1
 MATCH_VALID, MATCH_FAIL_RADIUS, MATCH_FAIL_PLANE, MATCH_FAIL_WEIGHT = 0, 1, 2, 3
@@ -32,9 +34,14 @@ class Params(C.Structure):
 
 
 def lib():
-    """Load the CUDA library; raise loudly when it is not built (no fallback path exists)."""
+    """Load the CUDA library; raise loudly when it is not built (no fallback path exists).  Threads that ask first at the same
+    time get the one handle, with its prototypes set before anyone sees it."""
     global _LIB
-    if _LIB is None:
+    if _LIB is not None:
+        return _LIB
+    with _LIB_LOCK:
+        if _LIB is not None:
+            return _LIB
         if not os.path.exists(_LIB_PATH):
             raise GlioError(f"{_LIB_PATH} not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
                             "(glio_b200 has no CPU fallback)")

@@ -314,21 +314,35 @@ struct Trace {
   void mark(const char* label) { if (!on) return; cudaStreamSynchronize(st); fprintf(stderr, "[glio trace] %s %-18s %8.1f us\n", what, label, std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - t0).count()); }
 };
 
+// the last error of the calling thread: glio_last_error(NULL)
 thread_local std::string tl_err;
+
+// An entry point runs on its context's GPU and hands the calling thread back on the device it came with, so a caller that
+// drives contexts on several GPUs (or allocates with torch's current device) keeps its own choice of device.
+struct DeviceGuard {
+  int prev = -1;
+  DeviceGuard() { if (cudaGetDevice(&prev) != cudaSuccess) { cudaGetLastError(); prev = -1; } }
+  cudaError_t use(int device) const { return device == prev ? cudaSuccess : cudaSetDevice(device); }
+  ~DeviceGuard() {
+    int now = -1;
+    if (prev >= 0 && cudaGetDevice(&now) == cudaSuccess && now != prev) cudaSetDevice(prev);
+  }
+};
 
 template <class F>
 int guarded(glio_ctx* ctx, F&& f) {
+  DeviceGuard dev;
   try {
-    if (ctx) GLIO_CUDA_TRY(cudaSetDevice(ctx->device));
+    if (ctx) GLIO_CUDA_TRY(dev.use(ctx->device));
     f();
     return GLIO_OK;
   } catch (const Error& e) {
     if (ctx) ctx->err = e.msg;
-    tl_err = e.msg; set_global_error(e.msg);
+    tl_err = e.msg;
     return e.code;
   } catch (const std::exception& e) {
     if (ctx) ctx->err = e.what();
-    tl_err = e.what(); set_global_error(e.what());
+    tl_err = e.what();
     return GLIO_ERR_STATE;
   }
 }
@@ -900,7 +914,7 @@ int glio_create(int device, const glio_params* params, glio_ctx** out) {
 
 void glio_destroy(glio_ctx* c) {
   if (!c) return;
-  cudaSetDevice(c->device);
+  DeviceGuard dev; dev.use(c->device);
   while (!c->odoms.empty()) glio_odom_destroy(c->odoms.back());   // an odometry still attached (it detaches itself)
   while (!c->loops.empty()) glio_loop_destroy(c->loops.back());   // likewise a loop object
   if (c->marg_thread.joinable()) {
@@ -924,7 +938,7 @@ void glio_destroy(glio_ctx* c) {
   delete c;
 }
 
-const char* glio_last_error(const glio_ctx* c) { return c ? c->err.c_str() : global_error(); }
+const char* glio_last_error(const glio_ctx* c) { return c ? c->err.c_str() : tl_err.c_str(); }
 
 int glio_synchronize(glio_ctx* c) {
   if (!c) return GLIO_ERR_ARG;
@@ -3278,7 +3292,7 @@ int glio_odom_create(glio_ctx* c, const glio_odom_options* options, glio_odom** 
 void glio_odom_destroy(glio_odom* o) {
   if (!o) return;
   glio_ctx* c = o->ctx;
-  cudaSetDevice(c->device);
+  DeviceGuard dev; dev.use(c->device);
   cudaStreamSynchronize(c->st);          // nothing queued may still use the buffers `delete o` frees
   c->odoms.erase(std::remove(c->odoms.begin(), c->odoms.end(), o), c->odoms.end());
   delete o;
@@ -3538,7 +3552,7 @@ int glio_loop_create(glio_ctx* c, const glio_loop_options* options, glio_loop** 
 void glio_loop_destroy(glio_loop* L) {
   if (!L) return;
   glio_ctx* c = L->ctx;
-  cudaSetDevice(c->device);
+  DeviceGuard dev; dev.use(c->device);
   cudaStreamSynchronize(c->st);          // nothing queued may still use the buffers `delete L` frees
   c->loops.erase(std::remove(c->loops.begin(), c->loops.end(), L), c->loops.end());
   delete L;

@@ -26,8 +26,6 @@ struct Error {
   int code;
   std::string msg;
 };
-void set_global_error(const std::string& m);
-const char* global_error();
 
 #define GLIO_CUDA_TRY(expr)                                                                   \
   do {                                                                                        \

@@ -247,8 +247,8 @@ __global__ void __launch_bounds__(256) k_feat_gather(FeatArgs a) {
 }
 
 void features_run(FeatArgs& a, cudaStream_t st, LaunchCounter& lc) {
-  static bool attr_done = false;
-  if (!attr_done) { GLIO_CUDA_TRY(cudaFuncSetAttribute(k_feat_voxel, cudaFuncAttributeMaxDynamicSharedMemorySize, FEAT_RING_CAP * 8)); attr_done = true; }
+  // a function attribute belongs to one device's context: set it on every call, so whichever GPU runs this launch has it
+  GLIO_CUDA_TRY(cudaFuncSetAttribute(k_feat_voxel, cudaFuncAttributeMaxDynamicSharedMemorySize, FEAT_RING_CAP * 8));
   GLIO_CUDA_TRY(cudaMemsetAsync(a.label, 0, (size_t)a.n, st));
   GLIO_CUDA_TRY(cudaMemsetAsync(a.picked, 0, (size_t)a.n, st));
   GLIO_CUDA_TRY(cudaMemsetAsync(a.err, 0, sizeof(int32_t), st));

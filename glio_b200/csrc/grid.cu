@@ -8,10 +8,6 @@
 
 namespace glio {
 
-static std::string g_err;
-void set_global_error(const std::string& m) { g_err = m; }
-const char* global_error() { return g_err.c_str(); }
-
 // ------------------------------------------------------------------------------------------------
 // exclusive scan (int32), 3-phase: per-block scan of 4096 items + scan of block sums (recursive) + add.
 // ------------------------------------------------------------------------------------------------

@@ -17,6 +17,10 @@
  *     device addresses on the context's GPU (used by bench "value" runs with inputs resident in HBM).
  *   - a glio_ctx is single-threaded; create one per concurrent caller (window solve / batch solve run on
  *     different threads in the reference, Estimator.cpp:5352-5368).  Each context owns one CUDA stream.
+ *     Distinct contexts may run at the same time on any threads and on any GPUs of the process; one context
+ *     is never called from two threads at once.
+ *   - a call runs on its context's GPU and returns with the calling thread's current CUDA device as it found
+ *     it, so contexts on several GPUs can be driven from one thread.
  *   - there is NO CPU fallback: without a CUDA device glio_create fails with GLIO_ERR_NO_DEVICE.
  */
 #ifndef GLIO_B200_H
@@ -71,7 +75,7 @@ void glio_default_params(glio_params* p);
 /* lifecycle */
 int glio_create(int device, const glio_params* params, glio_ctx** out);
 void glio_destroy(glio_ctx* ctx);
-const char* glio_last_error(const glio_ctx* ctx);   /* ctx may be NULL: last global error */
+const char* glio_last_error(const glio_ctx* ctx);   /* ctx may be NULL: the last error of the calling thread */
 int glio_synchronize(glio_ctx* ctx);
 /* the context's CUDA stream (cudaStream_t as void*) so callers can time with events on it */
 void* glio_stream(glio_ctx* ctx);
