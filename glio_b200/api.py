@@ -157,7 +157,8 @@ class Context:
                "k_pose_pair_sums", "k_pose_pair_sums_cost", "k_pose_assemble",
                "k_psr_pair_sums", "k_psr_pair_sums_cost", "k_psr_assemble",
                "k_imu_pair_sums", "k_imu_pair_sums_cost", "k_imu_pair_sums_ambient", "k_imu_assemble",
-               "k_band_chol_solve", "k_band_assemble", "k_band_assemble_g", "k_band_scale", "k_band_shift", "k_band_symv"]
+               "k_band_chol_solve", "k_band_assemble", "k_band_assemble_g", "k_band_scale", "k_band_shift", "k_band_symv",
+               "k_bcr_gather", "k_bcr_potrf", "k_bcr_trsm", "k_bcr_update", "k_bcr_back", "k_bcr_finish"]
 
     def lib_profile(self, on):
         self._chk(self._lib.glio_profile_enable(self._h, C.c_int(1 if on else 0)))
@@ -1204,6 +1205,33 @@ def _band_ops(self, H, s, v, x):
 
 
 Context.band_ops = _band_ops
+
+
+# the band solve by block cyclic reduction on the device
+BAND_BCR_MAX_HB = 256                     # GLIO_BAND_BCR_MAX_HB: the largest half bandwidth glio_band_solve_bcr takes
+FACTOR_SEQUENTIAL = 0                     # GLIO_FACTOR_SEQUENTIAL: the device minimizer factors with K4 (the default)
+FACTOR_BCR = 1                            # GLIO_FACTOR_BCR: the device minimizer solves by block cyclic reduction
+
+
+def _band_solve_bcr(self, band, b):
+    """glio_band_solve_bcr: solve A x = b for the symmetric band (n, hb+1) (lower band, glio_batch_solve's layout) by block cyclic
+    reduction on the device; the band is not changed.  Returns (x, ok): ok False when a block pivot was not positive and finite
+    or x is not finite (then x is unspecified)."""
+    A = np.ascontiguousarray(band, np.float64)
+    n, w = A.shape
+    rhs = np.ascontiguousarray(b, np.float64).reshape(n)
+    x = np.zeros(n); ok = C.c_int(0)
+    self._chk(self._lib.glio_band_solve_bcr(self._h, C.c_int(n), C.c_int(w - 1), _ptr(A), _ptr(rhs), _ptr(x), C.byref(ok)))
+    return x, bool(ok.value)
+
+
+def _batch_device_factorization(self, kind):
+    """glio_batch_device_factorization: FACTOR_SEQUENTIAL (K4, the default) or FACTOR_BCR for the device minimizer's solves."""
+    self._chk(self._lib.glio_batch_device_factorization(self._h, C.c_int(kind)))
+
+
+Context.band_solve_bcr = _band_solve_bcr
+Context.batch_device_factorization = _batch_device_factorization
 
 
 def _batch_use_device_solver(self, on):

@@ -296,6 +296,9 @@ struct glio_ctx {
   bool batch_device_solver = false;
   DevBuf<double> dm_H[2], dm_g, dm_Hs, dm_A, dm_v1, dm_v2, dm_v3; DevBuf<int> dm_flag;
   DevBuf<BandBlock> dm_blocks; DevBuf<BandContrib> dm_contrib; PinnedBuf<double> dm_h1, dm_h2;
+  // glio_batch_device_factorization's kind, and the block cyclic reduction's workspace (glio_band_solve_bcr and the minimizer)
+  int batch_factorization = GLIO_FACTOR_SEQUENTIAL;
+  BcrWork bcr;
 
   Slot& slot(int k) {
     GLIO_REQUIRE(k >= 0 && k < 4096, GLIO_ERR_ARG, "slot index out of range");
@@ -2879,11 +2882,18 @@ struct BatchProblem {
 
 // The minimizer's band operations on the device: H and Hc in c->dm_H, Hs, A; n-vectors through pinned staging
 struct DeviceBandOps : BandOps {
-  BatchProblem& P; glio_ctx* c; int n, hb; int cur = 0;
-  explicit DeviceBandOps(BatchProblem& p) : P(p), c(p.c), n(p.n), hb(p.hb) {
+  BatchProblem& P; glio_ctx* c; int n, hb; int cur = 0; bool bcr;
+  explicit DeviceBandOps(BatchProblem& p) : P(p), c(p.c), n(p.n), hb(p.hb), bcr(p.c->batch_factorization == GLIO_FACTOR_BCR) {
     const size_t nb = (size_t)n * (hb + 1);
-    GLIO_REQUIRE(hb <= GLIO_BAND_MAX_HB, GLIO_ERR_ARG, "glio_batch_solve: the device solver needs a half bandwidth <= GLIO_BAND_MAX_HB (160)");
-    c->dm_H[0].reserve(nb); c->dm_H[1].reserve(nb); c->dm_Hs.reserve(nb); c->dm_A.reserve(nb);
+    if (bcr) {
+      GLIO_REQUIRE(hb <= GLIO_BAND_BCR_MAX_HB, GLIO_ERR_ARG,
+                   "glio_batch_solve: the device solver's BCR factorisation needs a half bandwidth <= GLIO_BAND_BCR_MAX_HB (256)");
+      c->bcr.reserve(n, hb);
+    } else {
+      GLIO_REQUIRE(hb <= GLIO_BAND_MAX_HB, GLIO_ERR_ARG, "glio_batch_solve: the device solver needs a half bandwidth <= GLIO_BAND_MAX_HB (160)");
+      c->dm_A.reserve(nb);
+    }
+    c->dm_H[0].reserve(nb); c->dm_H[1].reserve(nb); c->dm_Hs.reserve(nb);
     c->dm_g.reserve(n); c->dm_v1.reserve(n); c->dm_v2.reserve(n); c->dm_v3.reserve(n); c->dm_flag.reserve(1);
     c->dm_h1.reserve(n); c->dm_h2.reserve(n);
     P.hcb.reset(n, hb);
@@ -2916,9 +2926,16 @@ struct DeviceBandOps : BandOps {
     up(v, c->dm_v1.p);
     GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));   // the staging buffer is reused for rhs
     up(rhs, c->dm_v2.p);
+    int ok = 0;
+    if (bcr) {                                     // gathers Hs + diag(v * v) itself: no k_band_shift
+      bcr_solve_run(c->bcr, c->dm_Hs.p, c->dm_v1.p, c->dm_v2.p, c->dm_v3.p, n, hb, c->st, c->lc);
+      int bad = 1;
+      GLIO_CUDA_TRY(cudaMemcpyAsync(&bad, c->bcr.flag.p, sizeof(int), cudaMemcpyDeviceToHost, c->st));
+      down(c->dm_v3.p, y);
+      return bad == 0;
+    }
     band_shift_run(c->dm_Hs.p, c->dm_A.p, c->dm_v1.p, n, hb, c->st, c->lc);
     band_chol_solve_run(c->dm_A.p, c->dm_v2.p, c->dm_v3.p, n, hb, c->dm_flag.p, c->st, c->lc);
-    int ok = 0;
     GLIO_CUDA_TRY(cudaMemcpyAsync(&ok, c->dm_flag.p, sizeof(int), cudaMemcpyDeviceToHost, c->st));
     down(c->dm_v3.p, y);
     return ok == 1;
@@ -2936,6 +2953,12 @@ struct DeviceBandOps : BandOps {
 int glio_batch_use_device_solver(glio_ctx* c, int on) {
   if (!c) return GLIO_ERR_ARG;
   c->batch_device_solver = on != 0;
+  return GLIO_OK;
+}
+
+int glio_batch_device_factorization(glio_ctx* c, int kind) {
+  if (!c || (kind != GLIO_FACTOR_SEQUENTIAL && kind != GLIO_FACTOR_BCR)) return GLIO_ERR_ARG;
+  c->batch_factorization = kind;
   return GLIO_OK;
 }
 
@@ -3009,6 +3032,24 @@ int glio_band_solve(glio_ctx* c, int n, int hb, double* band, const double* b, d
     GLIO_CUDA_TRY(cudaMemcpyAsync(x, c->band_x.p, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, c->st));
     GLIO_CUDA_TRY(cudaMemcpyAsync(ok, c->band_flag.p, sizeof(int), cudaMemcpyDeviceToHost, c->st));
     GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
+  });
+}
+
+int glio_band_solve_bcr(glio_ctx* c, int n, int hb, const double* band, const double* b, double* x, int* ok) {
+  if (!c) return GLIO_ERR_ARG;
+  return guarded(c, [&] {
+    GLIO_REQUIRE(n > 0 && band && b && x && ok, GLIO_ERR_ARG, "glio_band_solve_bcr: need n > 0 and band, b, x, ok");
+    GLIO_REQUIRE(hb >= 0 && hb <= GLIO_BAND_BCR_MAX_HB, GLIO_ERR_ARG, "glio_band_solve_bcr: need 0 <= hb <= GLIO_BAND_BCR_MAX_HB (256)");
+    const size_t nb = (size_t)n * (hb + 1);
+    c->band_a.reserve(nb); c->band_b.reserve((size_t)n); c->band_x.reserve((size_t)n);
+    GLIO_CUDA_TRY(cudaMemcpyAsync(c->band_a.p, band, nb * sizeof(double), cudaMemcpyHostToDevice, c->st));
+    GLIO_CUDA_TRY(cudaMemcpyAsync(c->band_b.p, b, (size_t)n * sizeof(double), cudaMemcpyHostToDevice, c->st));
+    bcr_solve_run(c->bcr, c->band_a.p, nullptr, c->band_b.p, c->band_x.p, n, hb, c->st, c->lc);
+    int bad = 1;
+    GLIO_CUDA_TRY(cudaMemcpyAsync(x, c->band_x.p, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, c->st));
+    GLIO_CUDA_TRY(cudaMemcpyAsync(&bad, c->bcr.flag.p, sizeof(int), cudaMemcpyDeviceToHost, c->st));
+    GLIO_CUDA_TRY(cudaStreamSynchronize(c->st));
+    *ok = bad == 0 ? 1 : 0;
   });
 }
 

@@ -523,4 +523,17 @@ void band_scale_run(const double* d_H, double* d_Hs, const double* d_s, int n, i
 void band_shift_run(const double* d_Hs, double* d_A, const double* d_v, int n, int hb, cudaStream_t st, LaunchCounter& lc);
 void band_symv_run(const double* d_Hs, const double* d_x, double* d_y, int n, int hb, cudaStream_t st, LaunchCounter& lc);
 
+// ---- the band solve by block cyclic reduction (bcr.cu; glio_band_solve_bcr, GLIO_FACTOR_BCR).  Blocks of bcr_block_size(hb) rows;
+// the workspace keeps L, U^T, V^T and w of every level for the back-substitution, grown to the largest shape solved.
+int bcr_block_size(int hb);
+struct BcrWork {
+  DevBuf<double> D, E, U, R, X;   // m blocks each: b x b (D, E, U), b (R, X)
+  DevBuf<int> flag;               // 1 after a pivot that is not positive and finite, or a non-finite x
+  void reserve(int n, int hb);
+};
+// solves A x = b for the band d_band (n x (hb+1), glio_band_solve's layout; the band is only read), with d_v != nullptr the shifted
+// A = band + diag(v * v); d_x[n] out, w.flag[0] = 0 on success.  hb <= GLIO_BAND_BCR_MAX_HB.
+void bcr_solve_run(BcrWork& w, const double* d_band, const double* d_v, const double* d_b, double* d_x, int n, int hb, cudaStream_t st,
+                   LaunchCounter& lc);
+
 }  // namespace glio

@@ -980,7 +980,8 @@ int glio_batch_solve(glio_ctx* ctx, int K, double* poses, double* speed_bias, gl
  * blocks onto it (k_band_assemble, each entry in the host path's order, so the band is the host path's bit for bit); the Jacobi
  * scaling, the shifted factor-and-solve (K4, below) and the band products run on the device, and only n-vectors cross PCIe.
  * The back-substitution and the band product sum in another order than the host's, so results differ from the host path by
- * rounding.  Needs a half bandwidth <= GLIO_BAND_MAX_HB (GLIO_ERR_ARG otherwise).  Default off: glio_batch_solve then runs exactly
+ * rounding.  Needs a half bandwidth <= GLIO_BAND_MAX_HB (GLIO_ERR_ARG otherwise; <= GLIO_BAND_BCR_MAX_HB with the block cyclic
+ * reduction of glio_batch_device_factorization, below).  Default off: glio_batch_solve then runs exactly
  * the host path.  Kernel names for glio_profile_get: k_band_assemble, k_band_assemble_g, k_band_scale, k_band_shift, k_band_symv. */
 int glio_batch_use_device_solver(glio_ctx* ctx, int on);
 /* The batch normal equations at one state: the band (n x (hb+1), n = K * (speed_bias ? 15 : 6), capacity >= n * (hb+1) doubles),
@@ -1008,6 +1009,26 @@ int glio_band_solve(glio_ctx* ctx, int n, int hb, double* band, const double* b,
  * k_band_scale, k_band_shift, k_band_symv. */
 int glio_band_ops(glio_ctx* ctx, int n, int hb, const double* H, const double* s, const double* v, const double* x, double* Hs,
                   double* hs_diag, double* A, double* y);
+
+/* ---- the band solve by block cyclic reduction (BCR) on the device, for half bandwidths up to GLIO_BAND_BCR_MAX_HB.  With blocks of
+ * b = 32 * ceil(max(hb, 1) / 32) rows the band is block tridiagonal; each level eliminates every other block at once (a dense
+ * tiled Cholesky of the block, its couplings and right-hand side through L^-1, then the updates of its even neighbours, left
+ * neighbour first), until one block is left; x follows by back-substitution level by level.  That is a Cholesky factorisation in
+ * a nested-dissection order: its x differs from K4's by rounding, within a normwise backward error
+ * ||A x - b||_inf / (||A||_inf ||x||_inf + ||b||_inf) of about 1e-14 on diagonally dominant bands, and it is the same bit for bit
+ * from run to run and on every context (no floating-point atomics).  band[n*(hb+1)] and b[n] are host buffers in
+ * glio_band_solve's layout and are only read (slots with j < 0 never); x[n] out.  *ok = 0 when a pivot of a block Cholesky is not
+ * positive and finite or x is not finite, and x is then unspecified.  n <= 0, 0 > hb or hb > GLIO_BAND_BCR_MAX_HB, or a null
+ * pointer is GLIO_ERR_ARG.  The call returns when x and *ok have arrived.  Kernel names for glio_profile_get: k_bcr_gather,
+ * k_bcr_potrf, k_bcr_trsm, k_bcr_update, k_bcr_back, k_bcr_finish. */
+enum { GLIO_BAND_BCR_MAX_HB = 256 };
+int glio_band_solve_bcr(glio_ctx* ctx, int n, int hb, const double* band, const double* b, double* x, int* ok);
+/* The factorisation glio_batch_solve's device minimizer runs when glio_batch_use_device_solver is on: GLIO_FACTOR_SEQUENTIAL (K4,
+ * the default; half bandwidth <= GLIO_BAND_MAX_HB) or GLIO_FACTOR_BCR (glio_band_solve_bcr's algorithm on the shifted band, gathered
+ * straight from the scaled band, so k_band_shift does not run; half bandwidth <= GLIO_BAND_BCR_MAX_HB).  Any other kind is
+ * GLIO_ERR_ARG.  With the device solver off the kind changes nothing. */
+enum { GLIO_FACTOR_SEQUENTIAL = 0, GLIO_FACTOR_BCR = 1 };
+int glio_batch_device_factorization(glio_ctx* ctx, int kind);
 
 /* ---- multi-GPU (batch path only; the window path is "replicas only", SURVEY 8e).
  * Keyframe-sharded ranks sum their pose-block buffers once per evaluation.  The library does not link NCCL: the
