@@ -1194,7 +1194,7 @@ Context.band_solve = _band_solve
 def _band_ops(self, H, s, v, x):
     """glio_band_ops: the device minimizer's scale, shift and product on the band H (n, hb+1) and the n-vectors s, v and x.
     Returns (Hs, hs_diag, A, y): Hs = S H S, hs_diag its diagonal, A = Hs + diag(v*v) and y = Hs x.  The slots of Hs and A with
-    j < 0 are unspecified."""
+    j < 0 are unspecified.  Takes hb up to BAND_BCR_MAX_HB, the widest band the device minimizer takes."""
     Hb = np.ascontiguousarray(H, np.float64)
     n, w = Hb.shape
     s, v, x = (np.ascontiguousarray(a, np.float64).reshape(n) for a in (s, v, x))
@@ -1240,7 +1240,8 @@ def _batch_use_device_solver(self, on):
 
 
 def _batch_normal_equations(self, poses, speed_bias=None, host_factors=None, on_device=False):
-    """glio_batch_normal_equations: (band (n, hb+1), g (n), cost) at one state, by the host path or on the device."""
+    """glio_batch_normal_equations: (band (n, hb+1), g (n), cost) at one state, by the host path or on the device (hb up to
+    BAND_BCR_MAX_HB)."""
     pb = np.ascontiguousarray(poses, np.float64).reshape(-1, 7); K = len(pb)
     sb = None if speed_bias is None else np.ascontiguousarray(speed_bias, np.float64).reshape(K, 9)
     n = K * (15 if sb is not None else 6)

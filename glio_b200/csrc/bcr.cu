@@ -120,12 +120,12 @@ __global__ void __launch_bounds__(kThreads) k_bcr_potrf(double* __restrict__ D, 
   }
 }
 
-// The row solves y L^T = a of the blocks k = first + blockIdx.y * step.  Rows [0, b): Ut from E[k-s] transposed (when k >= s),
+// The row solves y L^T = a of the blocks k = first + (y0 + blockIdx.y) * step.  Rows [0, b): Ut from E[k-s] transposed (when k >= s),
 // into U[k]; rows [b, 2b): Vt from E[k] (when k+s < m), in place; row 2b: w from r[k], in place.  blockIdx.x picks 32 rows.
 __global__ void __launch_bounds__(kThreads) k_bcr_trsm(const double* __restrict__ D, double* __restrict__ E, double* __restrict__ U,
-                                                       double* __restrict__ R, int m, int b, int s, int first, int step) {
+                                                       double* __restrict__ R, int m, int b, int s, int first, int step, int y0) {
   extern __shared__ double sm[];
-  const int k = first + blockIdx.y * step, tid = threadIdx.x, nb = b / kT, c0 = kT * blockIdx.x;
+  const int k = first + (y0 + (int)blockIdx.y) * step, tid = threadIdx.x, nb = b / kT, c0 = kT * blockIdx.x;
   const int kind = c0 < b ? 0 : c0 < 2 * b ? 1 : 2;
   if ((kind == 0 && k < s) || (kind == 1 && k + s >= m)) return;
   const int YW = b + 1;                             // odd row stride: conflict-free
@@ -198,12 +198,12 @@ __device__ __forceinline__ void tile_xyt(const double* __restrict__ X, const dou
   }
 }
 
-// The even blocks j = blockIdx.y * 2s of one level.  blockIdx.x: the lower tiles of D_j, then the tiles of the new E_j, then the
+// The even blocks j = (y0 + blockIdx.y) * 2s of one level.  blockIdx.x: the lower tiles of D_j, then the tiles of the new E_j, then the
 // 32-row tiles of r_j.
 __global__ void __launch_bounds__(kThreads) k_bcr_update(double* __restrict__ D, double* __restrict__ E, const double* __restrict__ U,
-                                                         double* __restrict__ R, int m, int b, int s) {
+                                                         double* __restrict__ R, int m, int b, int s, int y0) {
   __shared__ double sX[kT * kP], sY[kT * kP];
-  const int j = blockIdx.y * 2 * s, nb = b / kT, nd = nb * (nb + 1) / 2, tid = threadIdx.x, ty = tid >> 5, tx = tid & 31;
+  const int j = (y0 + (int)blockIdx.y) * 2 * s, nb = b / kT, nd = nb * (nb + 1) / 2, tid = threadIdx.x, ty = tid >> 5, tx = tid & 31;
   const int lft = j >= s ? j - s : -1, rgt = j + s < m ? j + s : -1;
   const size_t bb = (size_t)b * b;
   int t = blockIdx.x;
@@ -312,6 +312,9 @@ __global__ void k_bcr_finish(const double* __restrict__ X, double* __restrict__ 
   if (!isfinite(v)) flag[0] = 1;
 }
 
+// gridDim.y is at most 65 535: launches over more blocks than that go in chunks, each told its first y (one launch below the limit)
+constexpr int kMaxGridY = 65535;
+
 size_t potrf_smem(int b) { return (size_t)b * kP * sizeof(double); }
 size_t trsm_smem(int b) { return ((size_t)kT * (b + 1) + kT * kP) * sizeof(double); }
 
@@ -339,17 +342,24 @@ void bcr_solve_run(BcrWork& w, const double* d_band, const double* d_v, const do
     lc.begin("k_bcr_potrf", st);
     k_bcr_potrf<<<count, kThreads, potrf_smem(b), st>>>(w.D.p, b, first, step, w.flag.p);
     lc.end(st);
-    lc.begin("k_bcr_trsm", st);
-    k_bcr_trsm<<<dim3(2 * nb + 1, count), kThreads, trsm_smem(b), st>>>(w.D.p, w.E.p, w.U.p, w.R.p, m, b, s, first, step);
-    lc.end(st);
+    for (int y0 = 0; y0 < count; y0 += kMaxGridY) {
+      lc.begin("k_bcr_trsm", st);
+      k_bcr_trsm<<<dim3(2 * nb + 1, std::min(count - y0, kMaxGridY)), kThreads, trsm_smem(b), st>>>(w.D.p, w.E.p, w.U.p, w.R.p, m, b, s,
+                                                                                                   first, step, y0);
+      lc.end(st);
+    }
   };
   int s = 1;
   for (; s < m; s *= 2) {                           // level with blocks 0, s, 2s, ... < m: at least two
     const int ml = (m + s - 1) / s;
     eliminate(s, s, 2 * s, ml / 2);
-    lc.begin("k_bcr_update", st);
-    k_bcr_update<<<dim3(nb * (nb + 1) / 2 + nb * nb + nb, (ml + 1) / 2), kThreads, 0, st>>>(w.D.p, w.E.p, w.U.p, w.R.p, m, b, s);
-    lc.end(st);
+    const int even = (ml + 1) / 2;
+    for (int y0 = 0; y0 < even; y0 += kMaxGridY) {
+      lc.begin("k_bcr_update", st);
+      k_bcr_update<<<dim3(nb * (nb + 1) / 2 + nb * nb + nb, std::min(even - y0, kMaxGridY)), kThreads, 0, st>>>(w.D.p, w.E.p, w.U.p, w.R.p,
+                                                                                                             m, b, s, y0);
+      lc.end(st);
+    }
   }
   eliminate(s, 0, 1, 1);                            // the one block left: k = 0, s >= m, no neighbours
   for (; s >= 1; s /= 2) {

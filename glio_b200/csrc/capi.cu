@@ -3001,7 +3001,8 @@ int glio_batch_normal_equations(glio_ctx* c, int K, const double* poses, const d
     P.L.pack(poses, speed_bias, x.data());
     bool ok;
     if (on_device) {
-      GLIO_REQUIRE(P.hb <= GLIO_BAND_MAX_HB, GLIO_ERR_ARG, "glio_batch_normal_equations: the device path needs hb <= GLIO_BAND_MAX_HB (160)");
+      GLIO_REQUIRE(P.hb <= GLIO_BAND_BCR_MAX_HB, GLIO_ERR_ARG,
+                   "glio_batch_normal_equations: the device path needs hb <= GLIO_BAND_BCR_MAX_HB (256)");
       c->dm_H[0].reserve(nb); c->dm_g.reserve(P.n); P.hcb.reset(P.n, P.hb);
       ok = P.device_eval(x.data(), true, cost, c->dm_H[0].p, g);
       if (ok) {
@@ -3061,7 +3062,7 @@ int glio_band_ops(glio_ctx* c, int n, int hb, const double* H, const double* s, 
   return guarded(c, [&] {
     GLIO_REQUIRE(n > 0 && H && s && v && x && Hs && hs_diag && A && y, GLIO_ERR_ARG,
                  "glio_band_ops: need n > 0 and H, s, v, x, Hs, hs_diag, A, y");
-    GLIO_REQUIRE(hb >= 0 && hb <= GLIO_BAND_MAX_HB, GLIO_ERR_ARG, "glio_band_ops: need 0 <= hb <= GLIO_BAND_MAX_HB (160)");
+    GLIO_REQUIRE(hb >= 0 && hb <= GLIO_BAND_BCR_MAX_HB, GLIO_ERR_ARG, "glio_band_ops: need 0 <= hb <= GLIO_BAND_BCR_MAX_HB (256)");
     const size_t nb = (size_t)n * (hb + 1), bb = nb * sizeof(double), vb = (size_t)n * sizeof(double);
     c->dm_H[0].reserve(nb); c->dm_Hs.reserve(nb); c->dm_A.reserve(nb); c->dm_v1.reserve(n); c->dm_v2.reserve(n);
     GLIO_CUDA_TRY(cudaMemcpyAsync(c->dm_H[0].p, H, bb, cudaMemcpyHostToDevice, c->st));

@@ -986,7 +986,8 @@ int glio_batch_solve(glio_ctx* ctx, int K, double* poses, double* speed_bias, gl
 int glio_batch_use_device_solver(glio_ctx* ctx, int on);
 /* The batch normal equations at one state: the band (n x (hb+1), n = K * (speed_bias ? 15 : 6), capacity >= n * (hb+1) doubles),
  * *hb, g (n) and the cost, assembled by the host path (on_device = 0) or by k_band_assemble (on_device != 0), with the switches and
- * lists glio_batch_solve would use.  A failing callback or a non-finite cost is GLIO_ERR_NUMERIC. */
+ * lists glio_batch_solve would use.  The device path takes a half bandwidth up to GLIO_BAND_BCR_MAX_HB, the widest band the device
+ * minimizer factors (GLIO_ERR_ARG above it).  A failing callback or a non-finite cost is GLIO_ERR_NUMERIC. */
 int glio_batch_normal_equations(glio_ctx* ctx, int K, const double* poses, const double* speed_bias, glio_host_factors_band_fn host_factors,
                                 void* user, int on_device, int64_t capacity, double* Hband, int* hb, double* g, double* cost);
 
@@ -1005,7 +1006,8 @@ int glio_band_solve(glio_ctx* ctx, int n, int hb, double* band, const double* b,
  * (H_ij * s_i) * s_j) and hs_diag = diag(Hs); A = Hs + diag(v * v); y = Hs x, per row the columns max(0, i-hb) .. i from row i and
  * then i+1 .. min(n-1, i+hb) from the rows below, each term one rounded product and one rounded sum, starting from 0.0.  H, Hs
  * and A are n x (hb+1) in glio_band_solve's layout; s, v, x, hs_diag and y have n entries.  H's slots with j < 0 are never read,
- * and those of Hs and A are left unspecified.  Same argument checks as glio_band_solve.  Kernel names for glio_profile_get:
+ * and those of Hs and A are left unspecified.  Bad arguments, and 0 > hb or hb > GLIO_BAND_BCR_MAX_HB (below: the widest band the
+ * device minimizer takes; none of these kernels keeps storage that depends on hb), are GLIO_ERR_ARG.  Kernel names for glio_profile_get:
  * k_band_scale, k_band_shift, k_band_symv. */
 int glio_band_ops(glio_ctx* ctx, int n, int hb, const double* H, const double* s, const double* v, const double* x, double* Hs,
                   double* hs_diag, double* A, double* y);
@@ -1014,9 +1016,12 @@ int glio_band_ops(glio_ctx* ctx, int n, int hb, const double* H, const double* s
  * b = 32 * ceil(max(hb, 1) / 32) rows the band is block tridiagonal; each level eliminates every other block at once (a dense
  * tiled Cholesky of the block, its couplings and right-hand side through L^-1, then the updates of its even neighbours, left
  * neighbour first), until one block is left; x follows by back-substitution level by level.  That is a Cholesky factorisation in
- * a nested-dissection order: its x differs from K4's by rounding, within a normwise backward error
- * ||A x - b||_inf / (||A||_inf ||x||_inf + ||b||_inf) of about 1e-14 on diagonally dominant bands, and it is the same bit for bit
- * from run to run and on every context (no floating-point atomics).  band[n*(hb+1)] and b[n] are host buffers in
+ * a nested-dissection order: its x differs from K4's by rounding.  With eps = 2^-53 its normwise backward error
+ * ||A x - b||_inf / (||A||_inf ||x||_inf + ||b||_inf) stays within 4 (b + 2) eps, and ||x - x_ref||_inf / ||x_ref||_inf within
+ * 4 (b + 2) eps kappa(A), on ill-conditioned bands up to kappa 1e12 and on the device minimizer's own Jacobi-scaled, shifted
+ * normal equations (measured on an H100 80GB HBM3 at a 700 W power limit: under 1 % of either bar on the minimizer's systems,
+ * under 5 % on the others).  x is the same bit for bit from run to run and on every context (no floating-point atomics).
+ * band[n*(hb+1)] and b[n] are host buffers in
  * glio_band_solve's layout and are only read (slots with j < 0 never); x[n] out.  *ok = 0 when a pivot of a block Cholesky is not
  * positive and finite or x is not finite, and x is then unspecified.  n <= 0, 0 > hb or hb > GLIO_BAND_BCR_MAX_HB, or a null
  * pointer is GLIO_ERR_ARG.  The call returns when x and *ok have arrived.  Kernel names for glio_profile_get: k_bcr_gather,

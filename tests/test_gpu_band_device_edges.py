@@ -1,6 +1,6 @@
 """Edges of the device minimizer (glio_batch_use_device_solver, band.cu):
 - glio_band_ops, the scale, shift and product kernels alone, bit-identical to tests/band_solve_reference.py over sizes around the
-  launch blocks and up to the level-1 problem, half bandwidths up to GLIO_BAND_MAX_HB, and scales and vectors spanning 1e+-150;
+  launch blocks and up to the level-1 problem, half bandwidths up to GLIO_BAND_BCR_MAX_HB, and scales and vectors spanning 1e+-150;
 - K4 at the edges of its shared-memory ring (n from hb+1 to hb+18 and around 2R), with pivot failures in the prologue's rows and
   the last rows, and on the Jacobi-scaled, shifted normal equations the minimizer hands it;
 - device solves against host solves (tests/test_gpu_imu_factors.py's _compare) at the shipped options, without Jacobi scaling,
@@ -13,6 +13,7 @@ import pytest
 
 from glio_b200 import synth
 from tests import band_solve_reference as br
+from tests.band_refined_reference import backward_error
 from tests import eval_reference as er
 from tests import test_gpu_device_solve as ds
 from tests import test_gpu_imu_factors as ti
@@ -44,7 +45,7 @@ def _differs(a, b):
 # ---------------------------------------------------------------------------------------------------------------------------
 # glio_band_ops: k_band_scale, k_band_shift, k_band_symv
 # ---------------------------------------------------------------------------------------------------------------------------
-HBS = [0, 1, 5, 104, 160]
+HBS = [0, 1, 5, 104, 160, 161, 193, 224, 255, 256]
 
 
 def _ops_cases():
@@ -90,10 +91,10 @@ def test_band_ops_launches_and_is_profiled(api, ctx):
         assert prof[k][1] == 1 and prof[k][0] > 0.0, k
 
 
-def test_band_ops_arguments(api, ctx):
+def test_band_ops_arguments_up_to_bcr_max_hb(api, ctx):
     rng = np.random.default_rng(5)
-    with pytest.raises(api.GlioError, match="GLIO_BAND_MAX_HB"):
-        ctx.band_ops(br.random_spd_band(400, api.BAND_MAX_HB + 1, rng), np.ones(400), np.ones(400), np.ones(400))
+    with pytest.raises(api.GlioError, match="GLIO_BAND_BCR_MAX_HB"):
+        ctx.band_ops(br.random_spd_band(400, api.BAND_BCR_MAX_HB + 1, rng), np.ones(400), np.ones(400), np.ones(400))
     with pytest.raises(api.GlioError, match="n > 0"):
         ctx.band_ops(np.zeros((0, 5)), np.zeros(0), np.zeros(0), np.zeros(0))
     d = np.zeros(40 * 6); p = api._ptr(d)
@@ -149,32 +150,14 @@ def test_band_solve_pivot_failure_then_recovery(ctx, hb, where):
 MIN_LM_DIAGONAL, MAX_LM_DIAGONAL, RADIUS = 1e-6, 1e32, 1e4      # glio_default_solver_options, initial_trust_region_radius
 
 
-def _normwise_backward_error(band, b, x):
-    """||b - A x||_inf / (||A||_inf ||x||_inf + ||b||_inf) in longdouble, A the symmetric band"""
-    n, w = band.shape
-    hb = w - 1
-    A = np.nan_to_num(band).astype(np.longdouble)
-    xl = x.astype(np.longdouble)
-    r = b.astype(np.longdouble).copy()
-    rowabs = np.zeros(n, np.longdouble)
-    rows = np.arange(n)
-    for d in range(-hb, hb + 1):
-        j = rows + d
-        valid = (j >= 0) & (j < n)
-        jc = np.clip(j, 0, n - 1)
-        h = np.where(valid, A[rows, hb + d] if d <= 0 else A[jc, hb - d], 0)
-        r -= h * xl[jc]
-        rowabs += np.abs(h)
-    return float(np.max(np.abs(r)) / (np.max(rowabs) * np.max(np.abs(xl)) + np.max(np.abs(b))))
-
-
 def _minimizer_systems(band, g):
-    """(name, A, rhs): the band scaled as solve() scales it and shifted as the dogleg (three mu) and LM shift it"""
+    """(name, A, rhs): the band scaled as solve() scales it and shifted as the dogleg (mu from its first 1e-8 to its last 1) and
+    LM shift it"""
     s = 1.0 / (1.0 + np.sqrt(band[:, -1]))
     Hs, hd = br.band_scale(band, s)
     gs = g * s
     clamped = np.minimum(np.maximum(hd, MIN_LM_DIAGONAL), MAX_LM_DIAGONAL)
-    out = [(f"dogleg mu={mu:g}", br.band_shift(Hs, np.sqrt(clamped) * np.sqrt(mu)), gs) for mu in (1e-8, 1e-4, 1e-1)]
+    out = [(f"dogleg mu={mu:g}", br.band_shift(Hs, np.sqrt(clamped) * np.sqrt(mu)), gs) for mu in (1e-8, 1e-4, 1e-1, 1.0)]
     out.append(("lm", br.band_shift(Hs, np.sqrt(clamped / RADIUS)), gs))
     return out
 
@@ -199,7 +182,7 @@ def test_band_solve_on_the_minimizers_systems(api, ctx, level, K, prior):
         n_ok += 1
         assert np.array_equal(_bits(L), _bits(L_ref)), f"{name}: L differs at {_differs(L, L_ref)}"
         assert np.array_equal(_bits(x), _bits(x_ref)), f"{name}: x differs at {_differs(x, x_ref)}"
-        assert _normwise_backward_error(A, rhs, x_ref) <= 4 * (hb + 2) * np.finfo(float).eps, name
+        assert backward_error(A, x_ref, rhs) <= 4 * (hb + 2) * np.finfo(float).eps, name
     assert n_ok >= (3 if prior else 1)
 
 

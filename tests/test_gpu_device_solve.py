@@ -49,8 +49,24 @@ def _level1(api, K, pairs=True, edges=False):
     return c, P, P["sb_init"], ti._host_factor_set(api, P)
 
 
+def with_pose_factor(api, made, i, j):
+    """made = (c, P, sb, hf) with one more pose factor, a copy of the first, between keyframes i and j: it sets the half bandwidth
+    to (j - i + 1) nt - 1"""
+    c, P, sb, hf = made
+    pf = api.pose_factor_records(P["i"], P["j"], P["kind"], P["dq"], P["dp"])
+    wide = np.concatenate([pf, pf[:1]])
+    wide["i"][-1], wide["j"][-1] = i, j
+    c.batch_set_pose_factors(wide)
+    return c, P, sb, hf
+
+
 CASES = {"level0": lambda api: _level0(api, 40), "level1": lambda api: _level1(api, 40),
-         "level1_edges": lambda api: _level1(api, 40, edges=True), "level1_no_pairs": lambda api: _level1(api, 40, pairs=False)}
+         "level1_edges": lambda api: _level1(api, 40, edges=True), "level1_no_pairs": lambda api: _level1(api, 40, pairs=False),
+         # half bandwidths the device minimizer takes only with GLIO_FACTOR_BCR: 251 at level 0 (a pose factor 41 keyframes apart),
+         # 194 and 254 at level 1 (12 and 16 apart)
+         "level0_hb251": lambda api: with_pose_factor(api, _level0(api, 200), 3, 44),
+         "level1_hb194": lambda api: with_pose_factor(api, _level1(api, 40), 3, 15),
+         "level1_hb254": lambda api: with_pose_factor(api, _level1(api, 40), 3, 19)}
 
 
 @pytest.mark.parametrize("callback", [True, False])
