@@ -774,6 +774,17 @@ void eval_unary_blocks(glio_ctx* c, int W, const double* poses_body, int jac_kin
   eval_unary_wait(c, eval_unary_launch(c, W, poses_body, jac_kind, want_jac));
 }
 
+// Queues the read-out of an evaluation's n_diag diagonal and n_off off-diagonal block values: with reduce and a sharded run's hook,
+// their sums over the ranks (the off values only with want_jac and n_off > 0), then their copies into pinned memory
+void reduce_and_fetch(glio_ctx* c, bool reduce, bool want_jac, double* d_diag, double* h_diag, int64_t n_diag, double* d_off, double* h_off,
+                      int64_t n_off, const char* diag_err, const char* off_err) {
+  const bool hook = reduce && c->allreduce, off = want_jac && n_off > 0;
+  GLIO_REQUIRE(!hook || c->allreduce(c->allreduce_user, d_diag, n_diag, (void*)c->st) == 0, GLIO_ERR_NCCL, diag_err);
+  GLIO_REQUIRE(!hook || !off || c->allreduce(c->allreduce_user, d_off, n_off, (void*)c->st) == 0, GLIO_ERR_NCCL, off_err);
+  GLIO_CUDA_TRY(cudaMemcpyAsync(h_diag, d_diag, (size_t)n_diag * sizeof(double), cudaMemcpyDeviceToHost, c->st));
+  if (off) GLIO_CUDA_TRY(cudaMemcpyAsync(h_off, d_off, (size_t)n_off * sizeof(double), cudaMemcpyDeviceToHost, c->st));
+}
+
 // Device evaluation of the IMU blocks of list L -> L.h_diag (K x 241), L.h_off (n_pairs x 225), at the poses d_poses (already queued)
 // and speed_bias, which is queued here; jac_kind 1 gives the ambient x, y, z quaternion columns.  With reduce (the batch list) the
 // IMU buffers are summed over the ranks of a sharded run after whatever the caller queued before, one call per buffer.  Queued only;
@@ -789,15 +800,8 @@ int imu_blocks_launch(glio_ctx* c, ImuFactorList& L, int K, const double* d_pose
   GLIO_CUDA_TRY(cudaMemcpyAsync(L.d_sb.p, L.h_sb.p, (size_t)K * 9 * sizeof(double), cudaMemcpyHostToDevice, c->st));
   eval_imu_run(L.d_f.p, L.d_fstart.p, Pi, K, L.max_kf + 1, L.d_inc_start.p, L.d_inc.p, d_poses, L.d_sb.p, jac_kind, want_jac, L.d_sums.p,
                L.d_diag.p, L.d_off.p, c->st, c->lc);
-  if (reduce && c->allreduce) {
-    GLIO_REQUIRE(c->allreduce(c->allreduce_user, L.d_diag.p, (int64_t)K * GLIO_NACC_IMU_KF, (void*)c->st) == 0, GLIO_ERR_NCCL,
-                 "allreduce hook failed (IMU diag)");
-    if (want_jac && Pi > 0)
-      GLIO_REQUIRE(c->allreduce(c->allreduce_user, L.d_off.p, (int64_t)Pi * 225, (void*)c->st) == 0, GLIO_ERR_NCCL,
-                   "allreduce hook failed (IMU off)");
-  }
-  GLIO_CUDA_TRY(cudaMemcpyAsync(L.h_diag.p, L.d_diag.p, (size_t)K * GLIO_NACC_IMU_KF * sizeof(double), cudaMemcpyDeviceToHost, c->st));
-  if (want_jac && Pi > 0) GLIO_CUDA_TRY(cudaMemcpyAsync(L.h_off.p, L.d_off.p, (size_t)Pi * 225 * sizeof(double), cudaMemcpyDeviceToHost, c->st));
+  reduce_and_fetch(c, reduce, want_jac, L.d_diag.p, L.h_diag.p, (int64_t)K * GLIO_NACC_IMU_KF, L.d_off.p, L.h_off.p, (int64_t)Pi * 225,
+                   "allreduce hook failed (IMU diag)", "allreduce hook failed (IMU off)");
   return Pi;
 }
 
@@ -2344,31 +2348,39 @@ int glio_batch_get_edge_selection(glio_ctx* c, int cur, int oth, int64_t capacit
 
 namespace {
 
+// The incidence lists of a pair table for the block assembly, queued into d_kstart / d_inc: per keyframe k < n_kf, by a counting
+// sort, its pairs in table order at inc[kstart[k] .. kstart[k+1]), role 0 where k is the pair's first keyframe, 1 where its second
+void upload_incidence(glio_ctx* c, const std::vector<std::pair<int, int>>& pairs, int n_kf, DevBuf<int>& d_kstart, DevBuf<BinIncidence>& d_inc) {
+  std::vector<int> kstart((size_t)n_kf + 1, 0);
+  for (const auto& pr : pairs) { ++kstart[(size_t)pr.first + 1]; ++kstart[(size_t)pr.second + 1]; }
+  for (size_t k = 1; k < kstart.size(); ++k) kstart[k] += kstart[k - 1];
+  std::vector<BinIncidence> inc(2 * pairs.size());
+  std::vector<int> fill(kstart.begin(), kstart.end() - 1);
+  for (int p = 0; p < (int)pairs.size(); ++p) { inc[fill[pairs[p].first]++] = BinIncidence{p, 0}; inc[fill[pairs[p].second]++] = BinIncidence{p, 1}; }
+  d_kstart.reserve(kstart.size()); d_inc.reserve(inc.size() + 1);
+  GLIO_CUDA_TRY(cudaMemcpyAsync(d_kstart.p, kstart.data(), kstart.size() * sizeof(int), cudaMemcpyHostToDevice, c->st));
+  if (!inc.empty()) GLIO_CUDA_TRY(cudaMemcpyAsync(d_inc.p, inc.data(), inc.size() * sizeof(BinIncidence), cudaMemcpyHostToDevice, c->st));
+}
+
 // work items + incidence lists of the binary evaluation (rebuilt when associations / selections change)
 void build_bin_items(glio_ctx* c, int K) {
   if (!c->bin_dirty && c->bin_K == K) return;
   const int P = (int)c->pairs.size();
   ItemPlan<BinItem> plan(P);
-  std::vector<std::vector<BinIncidence>> inc(K);
+  std::vector<std::pair<int, int>> kf_pairs(P);
   for (int p = 0; p < P; ++p) {
     const glio_ctx::Pair& pr = *c->pairs[p];
     GLIO_REQUIRE(pr.cur >= 0 && pr.oth >= 0 && pr.cur < K && pr.oth < K, GLIO_ERR_ARG, "pair references a keyframe outside [0, K)");
     const CorrView v = pr.planes.active();
     plan.cut(p, v.n, GLIO_ITEM_MAX, [&](int64_t f, int32_t count) { return BinItem{v.cpw + f, v.nc + 6 * f, count, pr.cur, pr.oth}; });
-    inc[pr.cur].push_back(BinIncidence{p, 0});
-    inc[pr.oth].push_back(BinIncidence{p, 1});
+    kf_pairs[p] = {pr.cur, pr.oth};
   }
-  std::vector<int> kstart(K + 1, 0);
-  std::vector<BinIncidence> flat;
-  for (int k = 0; k < K; ++k) { kstart[k] = (int)flat.size(); flat.insert(flat.end(), inc[k].begin(), inc[k].end()); }
-  kstart[K] = (int)flat.size();
   c->n_bin_items = (int)plan.items.size();
-  c->d_kf_inc_start.reserve(K + 1); c->d_inc.reserve(flat.size() + 1); c->d_pair_sums.reserve((size_t)(P + 1) * GLIO_NACC_BIN);
+  c->d_pair_sums.reserve((size_t)(P + 1) * GLIO_NACC_BIN);
   c->d_bin_diag.reserve((size_t)K * GLIO_NACC); c->d_bin_off.reserve((size_t)(P + 1) * 36); c->d_bin_poses.reserve((size_t)K * 7);
   c->h_bin_diag.reserve((size_t)K * GLIO_NACC); c->h_bin_off.reserve((size_t)(P + 1) * 36); c->h_bin_poses.reserve((size_t)K * 7);
-  GLIO_CUDA_TRY(cudaMemcpyAsync(c->d_kf_inc_start.p, kstart.data(), (K + 1) * sizeof(int), cudaMemcpyHostToDevice, c->st));
-  if (!flat.empty()) GLIO_CUDA_TRY(cudaMemcpyAsync(c->d_inc.p, flat.data(), flat.size() * sizeof(BinIncidence), cudaMemcpyHostToDevice, c->st));
-  plan.upload(c, c->d_bin_items, c->d_pair_item_start, c->d_bin_partials, GLIO_NACC_BIN);   // its synchronisation covers kstart / flat
+  upload_incidence(c, kf_pairs, K, c->d_kf_inc_start, c->d_inc);
+  plan.upload(c, c->d_bin_items, c->d_pair_item_start, c->d_bin_partials, GLIO_NACC_BIN);
   c->bin_dirty = false; c->bin_K = K;
 }
 
@@ -2414,9 +2426,11 @@ int eval_blocks_launch(glio_ctx* c, int K, const double* poses, bool want_jac, B
   if (lidar == BIN_EDGES || add_edges)
     eval_binary_edge_run(c->d_bedge_items.p, c->n_bedge_items, c->d_bedge_pstart.p, P, c->d_bin_poses.p, want_jac, c->d_bedge_partials.p,
                          c->d_bedge_sums.p, c->st, c->lc);
-  if (lidar == BIN_EDGES)
-    bin_assemble_run(c->d_bedge_sums.p, K, P, c->d_kf_inc_start.p, c->d_inc.p, want_jac, c->d_bin_diag.p, c->d_bin_off.p, c->st, c->lc);
-  else if (lidar != BIN_NONE)
+  if (lidar == BIN_EDGES) {
+    c->lc.begin("k_bin_assemble", c->st);
+    pair_assemble_run<BinLayout>(c->d_bedge_sums.p, K, P, K, c->d_kf_inc_start.p, c->d_inc.p, want_jac, false, c->d_bin_diag.p, c->d_bin_off.p, c->st);
+    c->lc.end(c->st);
+  } else if (lidar != BIN_NONE)
     eval_binary_run(c->d_bin_items.p, c->n_bin_items, c->d_pair_item_start.p, P, K, c->d_bin_poses.p, c->prm.batch_score,
                     /*no loss on batch LiDAR factors, Estimator.cpp:2768*/ 0.0, want_jac, c->d_bin_partials.p, c->d_pair_sums.p,
                     c->d_kf_inc_start.p, c->d_inc.p, c->d_bin_diag.p, c->d_bin_off.p, c->st, c->lc, add_edges ? c->d_bedge_sums.p : nullptr);
@@ -2427,15 +2441,9 @@ int eval_blocks_launch(glio_ctx* c, int K, const double* poses, bool want_jac, B
     eval_dd_psr_run(c->d_dd_f.p, c->dd.d_fstart.p, c->d_dd_sats.p, c->d_dd_w.p, c->dd_frame, Pd, K, c->dd.max_kf + 1,
                     c->dd.d_inc_start.p, c->dd.d_inc.p, c->d_bin_poses.p, want_jac, /*add*/ lidar != BIN_NONE || add_pose, c->dd.d_sums.p,
                     c->d_bin_diag.p, c->d_bin_off.p + (size_t)(P + Pp) * 36, c->st, c->lc);
-  if (c->allreduce) {
-    // keyframe-sharded evaluation: every rank holds the same pair lists but only its own pairs and factors carry residuals;
-    // one sum over ranks of the pose-block buffers per evaluation (SURVEY 8e "pose-block allreduce")
-    GLIO_REQUIRE(c->allreduce(c->allreduce_user, c->d_bin_diag.p, (int64_t)K * GLIO_NACC, (void*)c->st) == 0, GLIO_ERR_NCCL, "allreduce hook failed (diag)");
-    if (want_jac && Pt > 0)
-      GLIO_REQUIRE(c->allreduce(c->allreduce_user, c->d_bin_off.p, (int64_t)Pt * 36, (void*)c->st) == 0, GLIO_ERR_NCCL, "allreduce hook failed (off)");
-  }
-  GLIO_CUDA_TRY(cudaMemcpyAsync(c->h_bin_diag.p, c->d_bin_diag.p, (size_t)K * GLIO_NACC * sizeof(double), cudaMemcpyDeviceToHost, c->st));
-  if (want_jac && Pt > 0) GLIO_CUDA_TRY(cudaMemcpyAsync(c->h_bin_off.p, c->d_bin_off.p, (size_t)Pt * 36 * sizeof(double), cudaMemcpyDeviceToHost, c->st));
+  // keyframe-sharded: every rank holds the same pair lists, only its own pairs and factors carry residuals (SURVEY 8e "pose-block allreduce")
+  reduce_and_fetch(c, true, want_jac, c->d_bin_diag.p, c->h_bin_diag.p, (int64_t)K * GLIO_NACC, c->d_bin_off.p, c->h_bin_off.p,
+                   (int64_t)Pt * 36, "allreduce hook failed (diag)", "allreduce hook failed (off)");
   return Pt;
 }
 
@@ -2465,11 +2473,10 @@ int eval_blocks_out(glio_ctx* c, const char* who, int K, const double* poses, Bi
 
 // The pair plan of a factor list with keyframes i, j and an active flag (pose and DD factors): the distinct unordered pairs
 // (a, b), a < b, in order of first appearance; the active factors' list positions grouped by pair, list order inside a pair
-// (order[fstart[p] .. fstart[p+1])); per keyframe 0 .. max_kf its pairs in table order (role 0 = a, 1 = b), by a counting sort.
+// (order[fstart[p] .. fstart[p+1])).
 struct PairPlan {
   std::vector<std::pair<int, int>> pairs;
-  std::vector<int> fstart, order, kstart;
-  std::vector<BinIncidence> inc;
+  std::vector<int> fstart, order;
   int max_kf = -1;
 };
 template <class F>
@@ -2492,18 +2499,12 @@ PairPlan plan_factor_pairs(const F* f, int64_t n) {
   std::vector<int> pos(pl.fstart.begin(), pl.fstart.end() - 1);
   for (int64_t k = 0; k < n; ++k)
     if (f[k].active) pl.order[pos[fpair[k]]++] = (int)k;
-  pl.kstart.assign((size_t)pl.max_kf + 2, 0);
-  for (const auto& pr : pl.pairs) { ++pl.kstart[(size_t)pr.first + 1]; ++pl.kstart[(size_t)pr.second + 1]; }
-  for (size_t k = 1; k < pl.kstart.size(); ++k) pl.kstart[k] += pl.kstart[k - 1];
-  pl.inc.resize((size_t)2 * Pn);
-  std::vector<int> fill(pl.kstart.begin(), pl.kstart.end() - 1);
-  for (int p = 0; p < Pn; ++p) { pl.inc[fill[pl.pairs[p].first]++] = BinIncidence{p, 0}; pl.inc[fill[pl.pairs[p].second]++] = BinIncidence{p, 1}; }
   return pl;
 }
 
 // A new pair-factor list from n records (glio_batch_set_pose_factors, glio_batch_set_dd_psr_factors), after the checks every
-// record shares (i != j, both in [0, max_kf); ij_err otherwise): its pair plan, and its active records grouped by pair into d_f,
-// queued on the stream into buffers of their own.  The caller queues its own payload, synchronises, and only then hands the
+// record shares (i != j, both in [0, max_kf); ij_err otherwise): its pair plan, the incidence lists of keyframes 0 .. max_kf of the
+// list, and its active records grouped by pair into d_f, queued on the stream into buffers of their own.  The caller queues its own payload, synchronises, and only then hands the
 // buffers to the context, so a failed call leaves the previous list and its buffers as they were.
 template <class F, class Rec>
 PairFactorList upload_pair_factors(glio_ctx* c, const Rec* f, int64_t n, int max_kf, int nacc, const char* ij_err, DevBuf<F>& d_f) {
@@ -2513,12 +2514,10 @@ PairFactorList upload_pair_factors(glio_ctx* c, const Rec* f, int64_t n, int max
   std::vector<F> grouped(pl.order.size());
   for (size_t q = 0; q < grouped.size(); ++q) memcpy(&grouped[q], &f[pl.order[q]], sizeof(F));
   PairFactorList l;
-  d_f.reserve(grouped.size() + 1); l.d_fstart.reserve(pl.fstart.size()); l.d_inc_start.reserve(pl.kstart.size());
-  l.d_inc.reserve(pl.inc.size() + 1); l.d_sums.reserve((pl.pairs.size() + 1) * nacc);
+  d_f.reserve(grouped.size() + 1); l.d_fstart.reserve(pl.fstart.size()); l.d_sums.reserve((pl.pairs.size() + 1) * nacc);
   if (!grouped.empty()) GLIO_CUDA_TRY(cudaMemcpyAsync(d_f.p, grouped.data(), grouped.size() * sizeof(F), cudaMemcpyHostToDevice, c->st));
   GLIO_CUDA_TRY(cudaMemcpyAsync(l.d_fstart.p, pl.fstart.data(), pl.fstart.size() * sizeof(int), cudaMemcpyHostToDevice, c->st));
-  GLIO_CUDA_TRY(cudaMemcpyAsync(l.d_inc_start.p, pl.kstart.data(), pl.kstart.size() * sizeof(int), cudaMemcpyHostToDevice, c->st));
-  if (!pl.inc.empty()) GLIO_CUDA_TRY(cudaMemcpyAsync(l.d_inc.p, pl.inc.data(), pl.inc.size() * sizeof(BinIncidence), cudaMemcpyHostToDevice, c->st));
+  upload_incidence(c, pl.pairs, pl.max_kf + 1, l.d_inc_start, l.d_inc);
   l.pairs.swap(pl.pairs); l.max_kf = pl.max_kf;
   return l;
 }

@@ -326,18 +326,23 @@ struct BinItem {
 };
 // Per-pair sums of the binary factors, whose Jacobians are J_c = [u | v], J_o = [-u | z] (u, v, z: 3-vectors): J^T J needs only
 // the distinct products uu(6) uv(9) vv(6) uz(9) vz(9) zz(6) (uu, vv, zz upper-triangular, uv / uz / vz row-major), then J^T r as
-// r*u(3) r*v(3) r*z(3), then the cost.  eval.cu's pair_accumulate writes it, k_bin_assemble reads it.
+// r*u(3) r*v(3) r*z(3), then the cost.  eval.cu's pair_accumulate writes it, its BinLayout reads it.
 constexpr int GLIO_NACC_BIN = 55;
-// incidence list of a keyframe for the deterministic block assembly: (pair index, role 0 = cur / 1 = oth)
+// incidence list of a keyframe for the deterministic block assembly: (pair index, role 0 = the pair's first keyframe (cur, a) /
+// 1 = its second (oth, b))
 struct BinIncidence { int32_t pair; int32_t role; };
+// k_pair_assemble (eval.cu) over pair sums in layout L (BinLayout: K2b / K2be, n_pairs x 55): per keyframe k < n_inc_kf the pairs of
+// its incidence list, in order, summed into d_diag (K x L::ND; added to its contents when add, else written) and, with want_jac,
+// the off-diagonal blocks -> d_off (n_pairs x L::NO).  One launch queued on st and checked; the caller names it to its counter.
+struct BinLayout;
+template <class L>
+void pair_assemble_run(const double* d_sums, int K, int n_pairs, int n_inc_kf, const int* d_kf_inc_start, const BinIncidence* d_inc,
+                       bool want_jac, bool add, double* d_diag, double* d_off, cudaStream_t st);
 // d_pair_sums_edge (nullable): per-pair K2be sums added to the plane sums (S = S_plane + S_edge) before the block assembly
 void eval_binary_run(const BinItem* d_items, int nitems, const int* d_pair_item_start, int n_pairs, int K, const double* d_poses,
                      double score_scale, double huber_delta, bool want_jac, double* d_partials, double* d_pair_sums,
                      const int* d_kf_inc_start, const BinIncidence* d_inc, double* d_diag /*K*28*/, double* d_off /*n_pairs*36*/,
                      cudaStream_t st, LaunchCounter& lc, const double* d_pair_sums_edge = nullptr);
-// k_bin_assemble alone: per-pair sums S -> d_diag (K x 28) and, with want_jac, d_off (n_pairs x 36)
-void bin_assemble_run(const double* d_pair_sums, int K, int n_pairs, const int* d_kf_inc_start, const BinIncidence* d_inc, bool want_jac,
-                      double* d_diag, double* d_off, cudaStream_t st, LaunchCounter& lc);
 
 // ---- K2be (eval.cu): binary point-to-edge factors, the edge counterpart of BinaryLidarPlaneNormFactor
 struct BinEdgeItem {

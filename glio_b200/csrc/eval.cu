@@ -461,7 +461,7 @@ __global__ void __launch_bounds__(BIN_T) k_eval_binary(const BinItem* __restrict
 // BinaryLidarPlaneNormFactor (no extrinsic, the line moves with oth, no loss):
 //   p_w = R(q_c) cp + t_c ;  A = R(q_o) a_l + t_o ;  B = R(q_o) b_l + t_o ;  e = (p_w - A) x (p_w - B) ;  r = s |e| / |A - B|
 // tangent Jacobians:  J_c = [g | 2 (R(q_c)cp x g)],  J_o = [-g | 2 (g x (p_w - t_o))]  with  g = s/|A-B| ((A-B) x e/|e|),
-// i.e. K2b's u, v, z with g in place of s N: the same 55 sums, so k_bin_pair_sums and k_bin_assemble take them unchanged.
+// i.e. K2b's u, v, z with g in place of s N: the same 55 sums, so k_bin_pair_sums and the block assembly take them unchanged.
 // Differences are formed relative to t_o (p_w - t_o and R(q_o) a_l), so kilometre offsets cancel before the cross product.
 // A point exactly on its line (|e| = 0) behaves as in K2e: r = 0 and a non-finite g.
 // HBM traffic per residual: 3 x 16 B (cp with s in .w, a_l, b_l).
@@ -521,46 +521,78 @@ __global__ void __launch_bounds__(64) k_bin_pair_sums(const double* __restrict__
   pair_sums[(size_t)p * NB + k] = v;
 }
 
-__device__ __forceinline__ int sym3(int a, int b) { return a <= b ? (a * 3 - a * (a - 1) / 2 + (b - a)) : (b * 3 - b * (b - 1) / 2 + (a - b)); }
-
-// block assembly: blocks [0,K) -> diagonal 6x6 (21 upper-tri) + g (6) + per-KF cost share (cost is attributed to cur);
-// blocks [K, K+n_pairs) -> off-diagonal 6x6 (row = cur tangent, col = oth tangent)
-__global__ void __launch_bounds__(64) k_bin_assemble(const double* __restrict__ S, int K, int n_pairs, const int* __restrict__ kf_inc_start,
-                                                     const BinIncidence* __restrict__ inc, double* __restrict__ diag, double* __restrict__ off) {
-  const int b = blockIdx.x, e = threadIdx.x;
-  if (b < K) {
-    if (e >= GLIO_NACC) return;
+// ---------------------------------------------------------------------------------------------------------------
+// Block assembly of the pair kinds (K2b / K2be, K2p, K2g, K2i): per-pair sums S (n_pairs x L::NS) -> per keyframe the L::ND
+// entries of its diagonal block, g and cost, each summed over the keyframe's incidence list in order (deterministic, no atomics),
+// and with WANT_JAC per pair its L::NO off-diagonal entries.  A layout L says where the entries come from: L::diag(s, role, e) is
+// the term one incidence with pair sums s adds to entry e, +0.0 for none (the sum starts at +0.0, so it is never -0.0, and adding
+// +0.0 leaves its bits as they are); L::off(s, e) is off-diagonal entry e.  Without WANT_JAC only the cost entry L::COST is summed,
+// the others are written as 0.
+// Thread t < K * ND: diag entry (kf, e), with no terms for kf >= n_inc_kf, added to diag's contents when add, else written; then,
+// with WANT_JAC, one thread per entry of the n_pairs off-diagonal blocks.
+// ---------------------------------------------------------------------------------------------------------------
+template <class L, bool WANT_JAC>
+__global__ void __launch_bounds__(256) k_pair_assemble(const double* __restrict__ S, int K, int n_pairs, int n_inc_kf,
+                                                       const int* __restrict__ kf_inc_start, const BinIncidence* __restrict__ inc, bool add,
+                                                       double* __restrict__ diag, double* __restrict__ off) {
+  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const int64_t nd = (int64_t)K * L::ND;
+  if (t < nd) {
+    const int kf = (int)(t / L::ND), e = (int)(t - (int64_t)kf * L::ND);
     double v = 0.0;
-    // decode entry e: [0,21) upper-tri (p<=q) of the 6x6, [21,27) g, 27 cost
-    int p = 0, q = 0;
-    if (e < 21) { int k = e; for (p = 0; p < 6; ++p) { if (k < 6 - p) { q = p + k; break; } k -= 6 - p; } }
-    for (int i = kf_inc_start[b]; i < kf_inc_start[b + 1]; ++i) {
-      const double* s = S + (size_t)inc[i].pair * NB;
-      const int role = inc[i].role;
-      if (e < 21) {
-        if (p < 3 && q < 3) v += s[sym3(p, q)];                                         // uu (both roles)
-        else if (p < 3) v += role == 0 ? s[6 + 3 * p + (q - 3)] : -s[21 + 3 * p + (q - 3)];   // uv | -uz
-        else v += role == 0 ? s[15 + sym3(p - 3, q - 3)] : s[39 + sym3(p - 3, q - 3)];  // vv | zz
-      } else if (e < 27) {
-        const int c = e - 21;
-        if (c < 3) v += role == 0 ? s[45 + c] : -s[45 + c];                              // r u | -r u
-        else v += role == 0 ? s[48 + (c - 3)] : s[51 + (c - 3)];                         // r v | r z
-      } else if (role == 0) v += s[54];
+    if (kf < n_inc_kf && (WANT_JAC || e == L::COST)) {
+      for (int i = kf_inc_start[kf]; i < kf_inc_start[kf + 1]; ++i) v += L::diag(S + (size_t)inc[i].pair * L::NS, inc[i].role, e);
     }
-    diag[(size_t)b * GLIO_NACC + e] = v;
-  } else {
-    const int pr = b - K;
-    if (pr >= n_pairs || e >= 36) return;
-    const double* s = S + (size_t)pr * NB;
-    const int p = e / 6, q = e % 6;
-    double v;
-    if (p < 3 && q < 3) v = -s[sym3(p, q)];                 // -u u^T
-    else if (p < 3) v = s[21 + 3 * p + (q - 3)];            //  u z^T
-    else if (q < 3) v = -s[6 + 3 * q + (p - 3)];            // -v u^T
-    else v = s[30 + 3 * (p - 3) + (q - 3)];                 //  v z^T
-    off[(size_t)pr * 36 + e] = v;
+    diag[t] = add ? diag[t] + v : v;
+  } else if (WANT_JAC) {
+    const int64_t o = t - nd;
+    if (o < (int64_t)n_pairs * L::NO) {
+      const int64_t pr = o / L::NO;
+      off[o] = L::off(S + pr * L::NS, (int)(o - pr * L::NO));
+    }
   }
 }
+
+template <class L>
+void pair_assemble_run(const double* d_sums, int K, int n_pairs, int n_inc_kf, const int* d_kf_inc_start, const BinIncidence* d_inc,
+                       bool want_jac, bool add, double* d_diag, double* d_off, cudaStream_t st) {
+  const int64_t n = (int64_t)K * L::ND + (want_jac ? (int64_t)n_pairs * L::NO : 0);
+  (want_jac ? k_pair_assemble<L, true> : k_pair_assemble<L, false>)<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(
+      d_sums, K, n_pairs, n_inc_kf, d_kf_inc_start, d_inc, add, d_diag, d_off);
+  GLIO_CUDA_TRY(cudaGetLastError());
+}
+
+// K2b / K2be: diagonal 6x6 (21 upper-tri) + g (6) + per-KF cost share (cost is attributed to cur); off-diagonal 6x6 (row = cur
+// tangent, col = oth tangent)
+struct BinLayout {
+  static constexpr int NS = NB, ND = GLIO_NACC, NO = 36, COST = 27;
+  __device__ static __forceinline__ int sym3(int a, int b) { return a <= b ? (a * 3 - a * (a - 1) / 2 + (b - a)) : (b * 3 - b * (b - 1) / 2 + (a - b)); }
+  __device__ static __forceinline__ double diag(const double* s, int role, int e) {
+    if (e < 21) {
+      // decode entry e: [0,21) upper-tri (p<=q) of the 6x6, [21,27) g, 27 cost
+      int p = 0, q = 0, k = e;
+      for (p = 0; p < 6; ++p) { if (k < 6 - p) { q = p + k; break; } k -= 6 - p; }
+      if (p < 3 && q < 3) return s[sym3(p, q)];                                            // uu (both roles)
+      if (p < 3) return role == 0 ? s[6 + 3 * p + (q - 3)] : -s[21 + 3 * p + (q - 3)];    // uv | -uz
+      return role == 0 ? s[15 + sym3(p - 3, q - 3)] : s[39 + sym3(p - 3, q - 3)];          // vv | zz
+    }
+    if (e < 27) {
+      const int c = e - 21;
+      if (c < 3) return role == 0 ? s[45 + c] : -s[45 + c];                                // r u | -r u
+      return role == 0 ? s[48 + (c - 3)] : s[51 + (c - 3)];                                // r v | r z
+    }
+    return role == 0 ? s[54] : 0.0;
+  }
+  __device__ static __forceinline__ double off(const double* s, int e) {
+    const int p = e / 6, q = e % 6;
+    if (p < 3 && q < 3) return -s[sym3(p, q)];                 // -u u^T
+    if (p < 3) return s[21 + 3 * p + (q - 3)];                 //  u z^T
+    if (q < 3) return -s[6 + 3 * q + (p - 3)];                 // -v u^T
+    return s[30 + 3 * (p - 3) + (q - 3)];                      //  v z^T
+  }
+};
+template void pair_assemble_run<BinLayout>(const double*, int, int, int, const int*, const BinIncidence*, bool, bool, double*, double*,
+                                           cudaStream_t);
 
 void eval_binary_run(const BinItem* d_items, int nitems, const int* d_pair_item_start, int n_pairs, int K, const double* d_poses,
                      double score_scale, double huber_delta, bool want_jac, double* d_partials, double* d_pair_sums,
@@ -578,15 +610,9 @@ void eval_binary_run(const BinItem* d_items, int nitems, const int* d_pair_item_
       lc.begin("k_bin_pair_add", st); k_bin_pair_add<<<(n + 255) / 256, 256, 0, st>>>(d_pair_sums, d_pair_sums_edge, n); lc.end(st);
     }
   }
-  bin_assemble_run(d_pair_sums, K, n_pairs, d_kf_inc_start, d_inc, want_jac, d_diag, d_off, st, lc);
-}
-
-void bin_assemble_run(const double* d_pair_sums, int K, int n_pairs, const int* d_kf_inc_start, const BinIncidence* d_inc, bool want_jac,
-                      double* d_diag, double* d_off, cudaStream_t st, LaunchCounter& lc) {
   lc.begin("k_bin_assemble", st);
-  k_bin_assemble<<<K + (want_jac ? n_pairs : 0), 64, 0, st>>>(d_pair_sums, K, n_pairs, d_kf_inc_start, d_inc, d_diag, d_off);
+  pair_assemble_run<BinLayout>(d_pair_sums, K, n_pairs, K, d_kf_inc_start, d_inc, want_jac, false, d_diag, d_off, st);
   lc.end(st);
-  GLIO_CUDA_TRY(cudaGetLastError());
 }
 
 void eval_binary_edge_run(const BinEdgeItem* d_items, int nitems, const int* d_pair_item_start, int n_pairs, const double* d_poses,
@@ -612,7 +638,7 @@ void eval_binary_edge_run(const BinEdgeItem* d_items, int nitems, const int* d_p
 // ambient Jacobian times the 4 x 3 local Jacobian, exact at non-unit quaternions too.
 // Layout: one half-warp per distinct pair (a, b); lane l < 12 owns tangent column l of (t_a, d_a, t_b, d_b), walks the pair's
 // factors in list order and keeps row l of the pair's 12 x 12 J^T J and entry l of J^T r in registers (12 + 1 doubles); the other
-// columns come by shuffle.  k_pose_assemble then sums each keyframe's pairs in incidence order.  No floating-point atomics.
+// columns come by shuffle.  k_pair_assemble (PoseLayout) then sums each keyframe's pairs in incidence order.  No floating-point atomics.
 // ---------------------------------------------------------------------------------------------------------------
 constexpr int NP = GLIO_NACC_POSE;
 constexpr int POSE_T = 128;   // 8 pairs per block
@@ -733,35 +759,16 @@ __global__ void __launch_bounds__(POSE_T) k_pose_pair_sums(const PoseFactor* __r
   if (l == 0) S[90] = cost;
 }
 
-// thread t < K*28: diag entry (kf, e) (the GLIO_NACC layout) from the kf's pairs in incidence order; then, with WANT_JAC, one
-// thread per entry of the n_pairs ab blocks
-template <bool WANT_JAC>
-__global__ void __launch_bounds__(256) k_pose_assemble(const double* __restrict__ S, int K, int n_pairs, int n_inc_kf,
-                                                       const int* __restrict__ kf_inc_start, const BinIncidence* __restrict__ inc, bool add,
-                                                       double* __restrict__ diag, double* __restrict__ off) {
-  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const int64_t nd = (int64_t)K * GLIO_NACC;
-  if (t < nd) {
-    const int kf = (int)(t / GLIO_NACC), e = (int)(t - (int64_t)kf * GLIO_NACC);
-    double v = 0.0;
-    if (kf < n_inc_kf && (WANT_JAC || e == 27)) {
-      for (int i = kf_inc_start[kf]; i < kf_inc_start[kf + 1]; ++i) {
-        const double* s = S + (size_t)inc[i].pair * NP;
-        const int role = inc[i].role;
-        if (e < 21) v += s[21 * role + e];                       // aa | bb
-        else if (e < 27) v += s[78 + 6 * role + (e - 21)];      // g_a | g_b
-        else if (role == 0) v += s[90];                         // the cost goes to a
-      }
-    }
-    diag[t] = add ? diag[t] + v : v;
-  } else if (WANT_JAC) {
-    const int64_t o = t - nd;
-    if (o < (int64_t)n_pairs * 36) {
-      const int64_t pr = o / 36;
-      off[o] = S[pr * NP + 42 + (o - pr * 36)];
-    }
+// K2p: the GLIO_NACC layout per keyframe, the ab blocks per pair
+struct PoseLayout {
+  static constexpr int NS = NP, ND = GLIO_NACC, NO = 36, COST = 27;
+  __device__ static __forceinline__ double diag(const double* s, int role, int e) {
+    if (e < 21) return s[21 * role + e];                       // aa | bb
+    if (e < 27) return s[78 + 6 * role + (e - 21)];            // g_a | g_b
+    return role == 0 ? s[90] : 0.0;                            // the cost goes to a
   }
-}
+  __device__ static __forceinline__ double off(const double* s, int e) { return s[42 + e]; }
+};
 
 void eval_pose_run(const PoseFactor* d_f, const int* d_fstart, int n_pairs, int K, int n_inc_kf, const int* d_kf_inc_start,
                    const BinIncidence* d_inc, const double* d_poses, bool want_jac, bool add, double* d_sums, double* d_diag, double* d_off,
@@ -772,12 +779,9 @@ void eval_pose_run(const PoseFactor* d_f, const int* d_fstart, int n_pairs, int 
     (want_jac ? k_pose_pair_sums<true> : k_pose_pair_sums<false>)<<<nb, POSE_T, 0, st>>>(d_f, d_fstart, n_pairs, d_poses, d_sums);
     lc.end(st);
   }
-  const int64_t n = (int64_t)K * GLIO_NACC + (want_jac ? (int64_t)n_pairs * 36 : 0);
   lc.begin("k_pose_assemble", st);
-  (want_jac ? k_pose_assemble<true> : k_pose_assemble<false>)<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(
-      d_sums, K, n_pairs, n_inc_kf, d_kf_inc_start, d_inc, add, d_diag, d_off);
+  pair_assemble_run<PoseLayout>(d_sums, K, n_pairs, n_inc_kf, d_kf_inc_start, d_inc, want_jac, add, d_diag, d_off, st);
   lc.end(st);
-  GLIO_CUDA_TRY(cudaGetLastError());
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -789,8 +793,8 @@ void eval_pose_run(const PoseFactor* d_f, const int* d_fstart, int n_pairs, int 
 //   then r = W r, J = W J when the factor has a weight matrix.  normalized() is Eigen 3.3's: d / |d| if |d|^2 > 0, else d.
 // Layout: one warp per distinct pair (a, b); lane k owns row k, walks the pair's factors in list order and accumulates its row's
 // contributions to the 28 pair sums (aa, bb upper-triangular over t, ab, g, cost) in registers; W is applied by broadcasting the
-// raw rows with __shfl_sync in index order; one butterfly reduction over the lanes at the end.  k_psr_assemble then sums each
-// keyframe's pairs in incidence order into the t columns of the K x 28 layout.  No floating-point atomics.
+// raw rows with __shfl_sync in index order; one butterfly reduction over the lanes at the end.  k_pair_assemble (DdLayout) then
+// sums each keyframe's pairs in incidence order into the t columns of the K x 28 layout.  No floating-point atomics.
 // ---------------------------------------------------------------------------------------------------------------
 constexpr int ND = GLIO_NACC_DD;
 constexpr int PSR_T = 128;   // 4 pairs per block
@@ -896,38 +900,22 @@ __global__ void __launch_bounds__(PSR_T) k_psr_pair_sums(const DdPsrFactor* __re
     if (k == e) Sp[e] = acc[e];
 }
 
-// thread t < K*28: diag entry (kf, e) (the GLIO_NACC layout) from the kf's pairs in incidence order, the t rows and columns only;
-// then, with WANT_JAC, one thread per entry of the n_pairs 6 x 6 ab blocks
-template <bool WANT_JAC>
-__global__ void __launch_bounds__(256) k_psr_assemble(const double* __restrict__ S, int K, int n_pairs, int n_inc_kf,
-                                                      const int* __restrict__ kf_inc_start, const BinIncidence* __restrict__ inc, bool add,
-                                                      double* __restrict__ diag, double* __restrict__ off) {
-  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const int64_t nd = (int64_t)K * GLIO_NACC;
-  if (t < nd) {
-    const int kf = (int)(t / GLIO_NACC), e = (int)(t - (int64_t)kf * GLIO_NACC);
+// K2g: the GLIO_NACC layout per keyframe, the t rows and columns only; the 6 x 6 ab blocks per pair, zero outside t x t
+struct DdLayout {
+  static constexpr int NS = GLIO_NACC_DD, ND = GLIO_NACC, NO = 36, COST = 27;
+  __device__ static __forceinline__ double diag(const double* s, int role, int e) {
     // 6 x 6 upper triangle -> the 3 x 3 t block: (0,0..2) = 0..2, (1,1..2) = 6..7, (2,2) = 11; g_t = 21..23; cost = 27
     const int src = e <= 2 ? e : e == 6 || e == 7 ? e - 3 : e == 11 ? 5 : -1;
-    double v = 0.0;
-    if (kf < n_inc_kf && ((WANT_JAC && (src >= 0 || (e >= 21 && e < 24))) || e == 27)) {
-      for (int i = kf_inc_start[kf]; i < kf_inc_start[kf + 1]; ++i) {
-        const double* s = S + (size_t)inc[i].pair * ND;
-        const int role = inc[i].role;
-        if (e < 21) v += s[6 * role + src];                     // aa | bb
-        else if (e < 27) v += s[21 + 3 * role + (e - 21)];     // g_a | g_b
-        else if (role == 0) v += s[27];                         // the cost goes to a
-      }
-    }
-    diag[t] = add ? diag[t] + v : v;
-  } else if (WANT_JAC) {
-    const int64_t o = t - nd;
-    if (o < (int64_t)n_pairs * 36) {
-      const int64_t pr = o / 36;
-      const int q = (int)(o - pr * 36), row = q / 6, col = q - 6 * row;
-      off[o] = row < 3 && col < 3 ? S[pr * ND + 12 + 3 * row + col] : 0.0;
-    }
+    if (e < 21) return src >= 0 ? s[6 * role + src] : 0.0;    // aa | bb
+    if (e < 24) return s[21 + 3 * role + (e - 21)];            // g_a | g_b
+    if (e < 27) return 0.0;
+    return role == 0 ? s[27] : 0.0;                            // the cost goes to a
   }
-}
+  __device__ static __forceinline__ double off(const double* s, int e) {
+    const int row = e / 6, col = e - 6 * row;
+    return row < 3 && col < 3 ? s[12 + 3 * row + col] : 0.0;
+  }
+};
 
 void eval_dd_psr_run(const DdPsrFactor* d_f, const int* d_fstart, const DdPsrSat* d_sats, const double* d_w, const DdPsrFrame& frame,
                      int n_pairs, int K, int n_inc_kf, const int* d_kf_inc_start, const BinIncidence* d_inc, const double* d_poses,
@@ -939,12 +927,9 @@ void eval_dd_psr_run(const DdPsrFactor* d_f, const int* d_fstart, const DdPsrSat
                                                                                      d_poses, d_sums);
     lc.end(st);
   }
-  const int64_t n = (int64_t)K * GLIO_NACC + (want_jac ? (int64_t)n_pairs * 36 : 0);
   lc.begin("k_psr_assemble", st);
-  (want_jac ? k_psr_assemble<true> : k_psr_assemble<false>)<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(
-      d_sums, K, n_pairs, n_inc_kf, d_kf_inc_start, d_inc, add, d_diag, d_off);
+  pair_assemble_run<DdLayout>(d_sums, K, n_pairs, n_inc_kf, d_kf_inc_start, d_inc, want_jac, add, d_diag, d_off, st);
   lc.end(st);
-  GLIO_CUDA_TRY(cudaGetLastError());
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -958,7 +943,7 @@ void eval_dd_psr_run(const DdPsrFactor* d_f, const int* d_fstart, const DdPsrSat
 // QuaternionParameterization local Jacobian at the unnormalised parameter, [0, e_k] (x) q, then sqrt_info times every column.
 // Layout: one warp per distinct pair (a, b); lane l < 30 owns tangent column l of (x_a, x_b), x = [t, delta, v, ba, bg], walks the
 // pair's factors in list order and keeps row l of the pair's 30 x 30 J^T J and entry l of J^T r in registers; the other columns,
-// and row a of r from lane a, come by shuffle; the lanes' cost shares are summed by one butterfly at the end.  k_imu_assemble then sums each keyframe's pairs in incidence order.  No floating-point atomics.
+// and row a of r from lane a, come by shuffle; the lanes' cost shares are summed by one butterfly at the end.  k_pair_assemble (ImuLayout) then sums each keyframe's pairs in incidence order.  No floating-point atomics.
 // ---------------------------------------------------------------------------------------------------------------
 constexpr int NI = GLIO_NACC_IMU, NIK = GLIO_NACC_IMU_KF;
 constexpr int IMU_T = 128;   // 4 pairs per block
@@ -1154,35 +1139,16 @@ __global__ void __launch_bounds__(IMU_T) k_imu_pair_sums(const ImuFactor* __rest
   if (l == 0) S[705] = cost;
 }
 
-// thread t < K*241: diag entry (kf, e) from the kf's pairs in incidence order; then, with WANT_JAC, one thread per entry of the
-// n_pairs ab blocks
-template <bool WANT_JAC>
-__global__ void __launch_bounds__(256) k_imu_assemble(const double* __restrict__ S, int K, int n_pairs, int n_inc_kf,
-                                                      const int* __restrict__ kf_inc_start, const BinIncidence* __restrict__ inc,
-                                                      double* __restrict__ diag, double* __restrict__ off) {
-  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const int64_t nd = (int64_t)K * NIK;
-  if (t < nd) {
-    const int kf = (int)(t / NIK), e = (int)(t - (int64_t)kf * NIK);
-    double v = 0.0;
-    if (kf < n_inc_kf && (WANT_JAC || e == 240)) {
-      for (int i = kf_inc_start[kf]; i < kf_inc_start[kf + 1]; ++i) {
-        const double* s = S + (size_t)inc[i].pair * NI;
-        const int role = inc[i].role;
-        if (e < 225) v += s[225 * role + e];                     // aa | bb
-        else if (e < 240) v += s[675 + 15 * role + (e - 225)];  // g_a | g_b
-        else if (role == 0) v += s[705];                        // the cost goes to a
-      }
-    }
-    diag[t] = v;
-  } else if (WANT_JAC) {
-    const int64_t o = t - nd;
-    if (o < (int64_t)n_pairs * 225) {
-      const int64_t pr = o / 225;
-      off[o] = S[pr * NI + 450 + (o - pr * 225)];
-    }
+// K2i: per keyframe its 15 x 15 block, g and cost (GLIO_NACC_IMU_KF), the ab blocks per pair
+struct ImuLayout {
+  static constexpr int NS = NI, ND = NIK, NO = 225, COST = 240;
+  __device__ static __forceinline__ double diag(const double* s, int role, int e) {
+    if (e < 225) return s[225 * role + e];                     // aa | bb
+    if (e < 240) return s[675 + 15 * role + (e - 225)];        // g_a | g_b
+    return role == 0 ? s[705] : 0.0;                           // the cost goes to a
   }
-}
+  __device__ static __forceinline__ double off(const double* s, int e) { return s[450 + e]; }
+};
 
 // the pair sums alone: n_pairs pairs from d_fstart, JAC_KIND jac_kind with want_jac, the cost otherwise
 void eval_imu_pair_sums_run(const ImuFactor* d_f, const int* d_fstart, int n_pairs, const double* d_poses, const double* d_sb, int jac_kind,
@@ -1200,12 +1166,9 @@ void eval_imu_run(const ImuFactor* d_f, const int* d_fstart, int n_pairs, int K,
                   const BinIncidence* d_inc, const double* d_poses, const double* d_sb, int jac_kind, bool want_jac, double* d_sums,
                   double* d_diag, double* d_off, cudaStream_t st, LaunchCounter& lc) {
   eval_imu_pair_sums_run(d_f, d_fstart, n_pairs, d_poses, d_sb, jac_kind, want_jac, d_sums, st, lc);
-  const int64_t n = (int64_t)K * NIK + (want_jac ? (int64_t)n_pairs * 225 : 0);
   lc.begin("k_imu_assemble", st);
-  (want_jac ? k_imu_assemble<true> : k_imu_assemble<false>)<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(
-      d_sums, K, n_pairs, n_inc_kf, d_kf_inc_start, d_inc, d_diag, d_off);
+  pair_assemble_run<ImuLayout>(d_sums, K, n_pairs, n_inc_kf, d_kf_inc_start, d_inc, want_jac, false, d_diag, d_off, st);
   lc.end(st);
-  GLIO_CUDA_TRY(cudaGetLastError());
 }
 
 }  // namespace glio
